@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native Caffe-MPI training hot path.
+"""bench.py -- headline benchmark of the H100-native Caffe-MPI training hot path.
 
 Metric (BASELINE.json): images/sec, ResNet-50 fp32 training, batch 64 per GPU, synthetic ImageNet-shaped input.
 One "step" = one Solver::Step iteration of the WHOLE prototxt graph (models/resnet50/train_val.prototxt semantics, generated
-by caffe_mpi_b200/models.py because the reference tree does not exist on the GPU box): every layer forward and backward
+by caffe_mpi_b200/models.py, so the benchmark needs no reference tree): every layer forward and backward
 through the C++ host layer (caffe::TrainNet), the bucketed gradient allreduce over the contiguous diff arena through
 P2PSync / ReduceScheduler (N > 1, overlapped with the rest of backward) and the fused SGD-momentum update.  Nothing is
 left out of the timed region.
@@ -11,12 +11,11 @@ left out of the timed region.
   python bench.py --gpus N --steps K --warmup W [--model resnet50|alexnet|vgg16|googlenet|lenet] [--batch B]
                                                             (N>1: launched by torch.distributed.run, one rank per GPU)
   python bench.py --impl reference ...                      (the reference's CPU conv path + host SGD on the host cores)
+  python bench.py ... --dump-outputs DIR                    (after the timed steps: what the last one computed, as DIR/*.npy)
 
 Prints ONE JSON line on rank 0 (key list in DESIGN.md "Measurement").
 """
 import argparse
-import csv
-import glob
 import json
 import os
 import subprocess
@@ -40,7 +39,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained"),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=None, source="NVIDIA H100 SXM data sheet (dense, 700 W)")
 
 
 # ------------------------------------------------------------------------------------------- reference arm
@@ -195,32 +194,23 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def ncu_traffic(kernel_substr):
-    """DRAM bytes per launch of the kernels whose name contains `kernel_substr`, from the newest committed ncu launch list of
-    this round (profiles/r02_*launches*.csv: gpu__time_duration.sum, dram__bytes_read.sum, dram__bytes_write.sum per launch).
-    Returns (read_bytes, write_bytes, launches, file) or None."""
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r02_*launches*.csv")))      # r02_final_* sorts after the per-call r02_cN_* lists
-    for path in reversed(files):
-        try:
-            rows = list(csv.reader(l for l in open(path) if l.startswith('"')))
-            hdr = rows[0]
-            iname, imet, ival, iunit = hdr.index("Kernel Name"), hdr.index("Metric Name"), hdr.index("Metric Value"), hdr.index("Metric Unit")
-            iid = hdr.index("ID")
-            rd, wr, ids = 0.0, 0.0, set()
-            scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "B": 1.0, "KB": 1e3, "MB": 1e6, "GB": 1e9}
-            for r in rows[1:]:
-                if kernel_substr not in r[iname]:
-                    continue
-                v = float(r[ival].replace(",", "")) * scale.get(r[iunit], 1.0)
-                if r[imet] == "dram__bytes_read.sum":
-                    rd += v; ids.add(r[iid])
-                elif r[imet] == "dram__bytes_write.sum":
-                    wr += v
-            if ids:
-                return rd / len(ids), wr / len(ids), len(ids), os.path.relpath(path, ROOT)
-        except Exception:
-            continue
-    return None
+# what --dump-outputs writes of a vector longer than this: the elements at np.sort(default_rng(1701).choice(size, DUMP_MAX_FLOATS,
+# replace=False)), the same for every build (2 x 16 MB of float32 at most)
+DUMP_MAX_FLOATS = 4 << 20
+
+
+def dump_outputs(t, out_dir):
+    """The arrays a caller of the timed step receives, as float32 .npy files: the loss of the last step, every learnable blob
+    after its update (data) and its momentum history, which is the step the update subtracted from it (the diffs themselves
+    are cleared by the update), each flattened and concatenated in learnable-blob order."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([t.loss()], np.float32))
+    for name, what in (("params", 0), ("param_history", 2)):
+        v = np.concatenate([t.get_param(i, what) for i in range(t.num_params())]).astype(np.float32)
+        if v.size > DUMP_MAX_FLOATS:
+            v = v[np.sort(np.random.default_rng(1701).choice(v.size, DUMP_MAX_FLOATS, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), v)
 
 
 def run_ours(args):
@@ -274,6 +264,8 @@ def run_ours(args):
     launches = L.b2c_launch_count() - l0
     clocks = sampler.stop() if sampler else None
     loss = t.loss()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(t, args.dump_outputs)
     # ---- end to end: every step copies the batch from pinned host memory and reads the loss back ---------------------------
     t.step(1, copy_input=True)
     barrier()
@@ -334,7 +326,6 @@ def run_ours(args):
         }
         dom = max(fam, key=lambda k: fam[k][1])
         ach = fam[dom][0] / (fam[dom][1] / 1e3) / 1e12 if fam[dom][1] > 0 else 0.0
-        tr = ncu_traffic("igemm_stg" if fam[dom][2] == "igemm" else "wgrad")
         step_ms = ms / args.steps
         out = {
             "metric": metric_name(model), "value": value, "unit": "images/sec", "n_gpus": world, "steps": args.steps,
@@ -347,7 +338,7 @@ def run_ours(args):
                        "reduce_buckets": args.buckets if args.buckets > 0 else 6,
                        "math": {"fp32": "fp32-equivalent: bf16x3 split (staged fwd/dgrad kernel) and 3xTF32 split (all other conv kernels), fp32 accumulate",
                                 "tf32": "tf32 single pass (informational)", "3xtf32": "fp32-equivalent: 3xTF32 split everywhere"}[args.math],
-                       "l2_policy": f"per-step activation working set {t.activation_floats() * 4 / 1e9:.2f} GB exceeds the 126 MB L2; every layer has its own blobs"},
+                       "l2_policy": f"per-step activation working set {t.activation_floats() * 4 / 1e9:.2f} GB exceeds the 50 MB L2; every layer has its own blobs"},
             "gpu_launches": launches,
             "loss": loss,
             "e2e": {"value": e2e_v, "unit": "images/sec", "h2d_bytes_per_step": t.input_bytes() * world,
@@ -357,8 +348,6 @@ def run_ours(args):
             "roofline": {"bound": "tensor", "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s", "frac": ach / tf32_peak if tf32_peak else None,
                          "kernel": dom,
                          "share_of_step": fam[dom][1] / step_ms if step_ms else None,
-                         "traffic": (tr[0] + tr[1]) if tr else None,
-                         "traffic_read_write": {"read": tr[0], "write": tr[1], "launches": tr[2], "file": tr[3], "unit": "bytes per launch (mean)"} if tr else None,
                          "peak_source": pk["source"] + ": bf16_tflops/2 (TF32 dense); fp32-equivalent ceilings: 2/3 of this peak for the "
                                         "bf16x3 kernel (three bf16 MMAs = 1.5 TF32 MMAs per MAC), 1/3 for the 3xTF32 kernels",
                          "families": {k: {"tflops": (v[0] / (v[1] / 1e3) / 1e12 if v[1] > 0 else None), "ms_per_step": round(v[1], 3),
@@ -429,7 +418,8 @@ def time_allreduce(t, world, dev, reps=5):
     if buf is None:
         L.b2c_comm_mem_free(ptr)
     algbw = n * 4 / (ms_ / 1e3) / 1e9
-    return {"bytes": n * 4, "ms": ms_, "algbw_gbs": algbw, "busbw_gbs": algbw * 2 * (world - 1) / world, "nvlink_ref_gbs": 900.0,
+    # nvlink_ref_gbs: H100 SXM NVLink 4 per direction, what busbw (nccl-tests convention) is compared with
+    return {"bytes": n * 4, "ms": ms_, "algbw_gbs": algbw, "busbw_gbs": algbw * 2 * (world - 1) / world, "nvlink_ref_gbs": 450.0,
             "buffer": "ncclMemAlloc + ncclCommRegister" if registered else "cudaMalloc"}
 
 
@@ -448,6 +438,8 @@ def main():
     ap.add_argument("--lmdb", default="", help="train from this LMDB of raw uint8 Datums (tools/make_lmdb.py writes one) instead of the "
                                                "synthetic in-memory source; e2e then includes the parser threads and the database read")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the cpu_baseline leg (N = 1 only)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the loss, learnable blobs and momentum history of the last step to DIR/*.npy")
     args = ap.parse_args()
     if not args.batch:
         from caffe_mpi_b200 import models

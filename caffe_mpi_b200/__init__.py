@@ -1,4 +1,4 @@
-"""caffe_mpi_b200 -- B200-native (sm_100a) data-parallel hot path of Caffe-MPI.
+"""caffe_mpi_b200 -- H100-native (sm_90a) data-parallel hot path of Caffe-MPI.
 
 The product is ``libb2c.so`` (CUDA kernels + the C ABI declared in ``include/b2c.h``) and the C++
 host layer in ``host/`` that mirrors the reference's ``caffe::Blob / Layer / Net / Solver`` surface

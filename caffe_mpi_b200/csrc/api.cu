@@ -3,7 +3,7 @@
 // The dispatch mirrors GetConvolutionLayer (reference src/caffe/layer_factory.cpp:53-88):
 //   engine CAFFE          -> explicit per-image im2col + GEMM + bias, the literal structure of
 //                            ConvolutionLayer::Forward_gpu/Backward_gpu (conv_layer.cu:7-57).
-//   engine DEFAULT/CUDNN  -> whole-batch implicit GEMM (the cuDNN role): tcgen05 kernels
+//   engine DEFAULT/CUDNN  -> whole-batch implicit GEMM (the cuDNN role): wgmma tensor-core kernels
 //                            (conv_tc.cu) when the shape qualifies, else the SIMT direct kernels.
 #include <stdarg.h>
 #include <stdio.h>
@@ -35,10 +35,10 @@ int sm_count() {
   // cached per device (a process may drive several GPUs, like the reference's solver threads)
   static int cache[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (!cache[dev]) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cache[dev] = n;
   }
   return cache[dev];
@@ -57,7 +57,7 @@ int launch_conv_dgrad_simt(const ConvShape&, const float*, const float*, float*,
 int launch_conv_wgrad_simt(const ConvShape&, const float*, const float*, float*, cudaStream_t);
 int launch_bias_add(int, int, int, const float*, float*, cudaStream_t);
 int launch_bias_grad(int, int, int, const float*, float*, cudaStream_t);
-// tcgen05 family (conv_tc.cu / gemm_tc.cu)
+// tensor-core family (conv_tc*.cu)
 bool tc_conv_supported(const ConvShape&, int op);
 size_t tc_conv_workspace(const ConvShape&, int op, int math);
 int launch_conv_tc(const ConvShape&, int op, int math, const float* a, const float* b, const float* bias, float* out,
@@ -138,7 +138,7 @@ static int resolve_algo(const b2c_conv_desc* d, int op) {
 using namespace b2c;
 
 extern "C" const char* b2c_last_error(void) { return last_error().c_str(); }
-extern "C" const char* b2c_version(void) { return "b2c 0.1 (sm_100a)"; }
+extern "C" const char* b2c_version(void) { return "b2c 0.1 (sm_90a)"; }
 extern "C" uint64_t b2c_launch_count(void) { return g_launches.load(); }
 extern "C" int b2c_set_default_math(int m) {
   if (m < B2C_MATH_FP32 || m > B2C_MATH_FP32_3XTF32) return fail(B2C_ERR_INVALID, "bad math mode %d", m);

@@ -1,4 +1,4 @@
-// b2c_common.cuh -- shared helpers for the sm_100a kernels behind include/b2c.h.
+// b2c_common.cuh -- shared helpers for the sm_90a kernels behind include/b2c.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

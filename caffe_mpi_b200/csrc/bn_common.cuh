@@ -147,10 +147,9 @@ static inline unsigned bn_max_cluster() {
   return (unsigned)v;
 }
 // cluster size for the per-channel kernels: ~16K values or more per CTA, at least one CTA per SM, at most bn_max_cluster().
-// Measured (profiles/r02_c11_bn_sweep.log, r02_c11_bench*.json): FEWER, FATTER CTAs win -- halving the slices (so that both
-// backward streams fit shared memory) cost 25 % on the 28x28 layers, 16-CTA clusters another 40 % on the 56x56 ones (co-scheduling
-// sixteen 512-thread CTAs in one GPC), and a floor of two CTAs per SM put the 14x14 layers on 512 three-iteration CTAs in two
-// waves (~20 us per launch whatever the tensor size, r02_c8_bn_sweep.log).
+// FEWER, FATTER CTAs win: halving the slices (so that both backward streams fit shared memory) slows the 28x28 layers down,
+// 16-CTA clusters slow the 56x56 ones (co-scheduling sixteen 512-thread CTAs in one GPC), and a floor of two CTAs per SM puts
+// the 14x14 layers on many short CTAs in two waves (a fixed cost per launch whatever the tensor size).
 static inline unsigned bn_cluster_size(int N, int C, int S) {
   const size_t E = (size_t)N * S;
   const unsigned maxc = bn_max_cluster();
@@ -161,10 +160,10 @@ static inline unsigned bn_cluster_size(int N, int C, int S) {
 }
 // one cluster of `cs` CTAs per channel; `smem_pad` bytes of (unused) dynamic shared memory bound the CTAs per SM
 // threads per CTA: 512, or 128 for channels of at most 4 096 values (ResNet-50's 7x7 layers: 2 048 channels x 3 136 values --
-// one 512-thread CTA per channel was seven waves of CTAs that are all set-up and barriers, ~85 us for a 26 MB tensor)
+// one 512-thread CTA per channel is several waves of CTAs that are all set-up and barriers)
 static inline unsigned bn_threads(int N, int S, bool forward) {
-  // 4 097 .. 16 384 values per channel (the 14x14 layers): 256 threads forward (C1024: 55 -> 43 us), 512 backward (256 is 6 % slower
-  // there: the parked streams leave room for two CTAs per SM either way) -- profiles/r02_c15_bn_threads.log
+  // 4 097 .. 16 384 values per channel (the 14x14 layers): 256 threads forward, 512 backward (the parked streams leave room for
+  // two CTAs per SM either way)
   const size_t E = (size_t)N * S;
   return E <= 4096 ? 128u : (E <= 16384 && forward) ? 256u : (unsigned)BN_THREADS;
 }

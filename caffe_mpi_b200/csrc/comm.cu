@@ -1,4 +1,4 @@
-// comm.cu -- gradient exchange over NCCL (NVLink 5 / NVSwitch), one communicator per process.
+// comm.cu -- gradient exchange over NCCL (NVLink 4 / NVSwitch), one communicator per process.
 //
 // Replaces the NCCL use of P2PManager / P2PSync (reference src/caffe/parallel.cpp:36-87,
 // 145-253: ncclGetUniqueId + MPI_Bcast, ncclCommInitRank between MPI_Barriers, ncclBcast of the
@@ -42,7 +42,7 @@ extern "C" int b2c_comm_init(int nranks, int rank, const void* id, b2c_comm** ou
   ncclUniqueId uid;
   memcpy(&uid, id, sizeof(uid));
   b2c_comm* c = new b2c_comm{nullptr, nranks, rank, {}};
-  // B2C_NCCL_MAX_CTAS: cap the CTAs NCCL may use per collective.  The tcgen05 conv kernels are persistent with one CTA per
+  // B2C_NCCL_MAX_CTAS: cap the CTAs NCCL may use per collective.  The tensor-core conv kernels are persistent with one CTA per
   // SM, so an allreduce overlapped with backward only gets SMs at kernel tails; fewer, NVLS-fed CTAs disturb them less.
   ncclConfig_t cfg = NCCL_CONFIG_INITIALIZER;
   if (const char* e = getenv("B2C_NCCL_MAX_CTAS")) { const int v = atoi(e); if (v > 0) cfg.maxCTAs = v; }

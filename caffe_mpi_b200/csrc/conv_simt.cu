@@ -1,7 +1,7 @@
 // conv_simt.cu -- fp32 SIMT direct-convolution kernels (B2C_ALGO_SIMT) and the bias kernels.
 //
 // Exact-fp32 (FFMA) implicit-GEMM family behind b2c_conv_forward / backward_data /
-// backward_filter for shapes the tcgen05 kernels do not take, and the on-device second
+// backward_filter for shapes the tensor-core kernels do not take, and the on-device second
 // opinion for them.  Same contract as the cuDNN calls they stand in for (reference
 // src/caffe/layers/cudnn_conv_layer.cu:25-29,95-99,118-123): whole batch per launch,
 // y / dx overwritten, dw accumulated.  Bias forward / backward replace cudnnAddTensor and

@@ -1,4 +1,4 @@
-// conv_tc.cu -- tcgen05 (5th-gen tensor core) implicit-GEMM convolution, forward and data-gradient (sm_100a).
+// conv_tc.cu -- wgmma (Hopper tensor core) implicit-GEMM convolution, forward and data-gradient (sm_90a).
 //
 // Replaces cudnnConvolutionForward / cudnnConvolutionBackwardData as called by the reference's
 // CuDNNConvolutionLayer (src/caffe/layers/cudnn_conv_layer.cu:25-29,118-123) and, semantically, the
@@ -10,21 +10,19 @@
 //   dgrad   : the same kernel run on dY with the transposed (+ flipped) filter for stride-1 layers, or
 //             on the top grid with a strided scatter epilogue for 1x1 / stride>1 / pad 0 layers.
 //
-// Kernel anatomy -- persistent, one CTA per SM, 128 x N_TILE output tiles, 704 threads:
-//   warps 0-15 A producers.  Four threads per GEMM row (pixel), each owning two of the eight 16-byte K
+// Kernel anatomy -- persistent, one CTA per SM, 128 x N_TILE output tiles, 544 threads:
+//   warps 0-7  two consumer warpgroups: wgmma.mma_async.m64nNk8.tf32 from shared-memory descriptors, the fp32
+//              accumulators of rows [64 cw, 64 cw + 64) in registers; then the epilogue: accumulators -> shared
+//              memory [channel][pixel] -> bias -> coalesced NCHW stores.
+//   warps 8-15 A producers.  Two threads per GEMM row (pixel), each owning four of the eight 16-byte K
 //              chunks of a K block; the im2col gather reads NCHW global memory directly (coalesced along
 //              W) from a per-kernel smem table of chunk offsets (the (c,i,j) decode is the same for every
 //              tile), keeps two K blocks of loads in flight in registers across tile boundaries, splits
-//              to TF32 hi (+ lo) on the ALU pipe and writes its row of the A tile straight into tensor
-//              memory (tcgen05.st, lane = GEMM row).  K is ordered (channel/4, tap, channel%4) when C/g % 4 == 0.
+//              to TF32 hi (+ lo) on the ALU pipe and writes its row of the A tile into shared memory (K-major,
+//              no swizzle).  K is ordered (channel/4, tap, channel%4) when C/g % 4 == 0.
 //   warp  16   TMA producer for the filter operand: a prepass kernel writes the filter in GEMM-K order,
 //              already split into TF32 hi / lo and zero padded to a multiple of 32; cp.async.bulk.tensor
 //              (SWIZZLE_128B) drops [N_TILE x 32] boxes into smem, completion on the stage mbarrier.
-//   warp  17   allocates TMEM and issues tcgen05.mma.kind::tf32 (M=128, N=N_TILE, K=8) with the A operand in
-//              TENSOR MEMORY (written there by the producers with tcgen05.st) and B from smem: the 3xTF32 mode
-//              is otherwise shared-memory-bandwidth bound (each K step reads A and B three times); tcgen05.commit releases smem stages and publishes finished accumulators.
-//   warps 18-21 epilogue: tcgen05.ld TMEM -> registers -> bias -> coalesced NCHW stores, overlapped with
-//              the next tile's main loop through the double-buffered accumulator.
 // The activation operand is not TMA-staged: with NCHW the GEMM-K axis (c,i,j) is not unit-stride and
 // 7x7 maps have 196-byte channel pitches (TMA needs 16-byte multiples); see DESIGN.md.
 // fp32 math mode = 3 TF32 MMAs per K step (lo*hi, hi*lo, hi*hi); TF32 mode = 1.
@@ -39,8 +37,11 @@
 namespace b2c {
 using namespace tc;
 
-constexpr int NPW = 16;                     // A-producer warps
-constexpr int FW_THREADS = (NPW + 6) * 32;  // + TMA warp, MMA warp, 4 epilogue warps = 704
+constexpr int NCONS = 8;                    // consumer warps: two warpgroups, tile rows [0, 64) and [64, 128)
+constexpr int NPW = 8;                      // A-producer warps
+constexpr int W_PROD0 = NCONS;              // first A-producer warp
+constexpr int W_TMA = NCONS + NPW;          // filter TMA warp
+constexpr int FW_THREADS = (NCONS + NPW + 1) * 32;  // 544
 constexpr int TAB_ENTRIES = 1152;   // gather table: one entry per K chunk (KMODE 1) or per K element (KMODE 0)
 
 struct FwdParams {
@@ -62,39 +63,26 @@ struct FwdParams {
   int dbg;            // B2C_DBG experiments: 1 = skip the global gather (producer-side ceiling), 2 = skip the MMAs
 };
 
-// Resources of one CTA.  Shared memory holds only the filter (B) stages; the activation (A) operand
-// lives in tensor memory next to the accumulators:
-//   TMEM columns [0, ACC_BUFS*N_TILE)            fp32 accumulators (double buffered unless N_TILE = 256)
-//                [A_COL0 + s*A_COLS, +A_COLS)     A stage s: 32 columns TF32 hi (+ 32 columns lo)
+// One pipeline stage: [B hi | B lo | A hi | A lo].  B (filter) is a TMA box in the SWIZZLE_128B K-major layout (1024-byte
+// aligned); A (activations) is written by the producers in the padded K-major no-swizzle layout of tc_common.cuh.
 template <int N_TILE, bool SPLIT>
 struct FwdSmem {
   static constexpr uint32_t B_BYTES = N_TILE * 128u;                       // [N_TILE rows][32 fp32], SW128
+  static constexpr uint32_t A_BYTES = tile_bytes(128);                     // [128 rows][32 fp32]
   static constexpr uint32_t NP = SPLIT ? 2u : 1u;
-  static constexpr uint32_t STAGE = NP * B_BYTES;                          // multiple of 1024
-  static constexpr int ACC_BUFS = N_TILE == 256 ? 1 : 2;
-  static constexpr uint32_t A_COL0 = ACC_BUFS * N_TILE;
-  static constexpr uint32_t A_COLS = SPLIT ? 64u : 32u;
-  static constexpr int TMEM_STAGES = (int)((512u - A_COL0) / A_COLS);
-  static constexpr int SMEM_STAGES = (int)((164u * 1024u) / STAGE);         // leaves room for the epilogue staging below
-  static constexpr int STAGES_ = TMEM_STAGES < SMEM_STAGES ? TMEM_STAGES : SMEM_STAGES;
+  static constexpr uint32_t B_STAGE = NP * B_BYTES;
+  static constexpr uint32_t STAGE = B_STAGE + ((NP * A_BYTES + 1023u) & ~1023u);
+  static constexpr uint32_t EPI_BYTES = 32u * 128u * 4u;                   // [32 channels][128 pixels] fp32 (epilogue transpose)
+  static constexpr uint32_t FIXED = 256u + TAB_ENTRIES * 8u + EPI_BYTES + 1024u;   // + alignment slack
+  static constexpr int STAGES_ = (int)((227u * 1024u - FIXED) / STAGE);
   static constexpr int STAGES = STAGES_ > 6 ? 6 : STAGES_;
   static constexpr uint32_t BAR_OFF = STAGES * STAGE;
   static constexpr uint32_t TAB_OFF = BAR_OFF + 256;
-  static constexpr uint32_t EPI_OFF = TAB_OFF + TAB_ENTRIES * 8;           // 2 x [32 channels][128 pixels] fp32 (epilogue transpose)
-  static constexpr uint32_t EPI_BYTES = 2u * 32u * 128u * 4u;
-  static constexpr uint32_t TOTAL = EPI_OFF + EPI_BYTES + 1024;             // + alignment slack
-  static constexpr uint32_t TX_BYTES = NP * B_BYTES;
+  static constexpr uint32_t EPI_OFF = TAB_OFF + TAB_ENTRIES * 8;
+  static constexpr uint32_t TOTAL = EPI_OFF + EPI_BYTES + 1024;
+  static constexpr uint32_t TX_BYTES = B_STAGE;
+  static_assert(STAGES >= 2, "shared memory budget");
 };
-
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;                    // LBO (ignored for swizzled K-major)
-  d |= (uint64_t)(1024u >> 4) << 32;         // SBO: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;                    // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                    // SWIZZLE_128B
-  return d;
-}
 
 __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
@@ -115,15 +103,14 @@ __global__ void __launch_bounds__(FW_THREADS, 1)
 igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CUtensorMap map_hi,
                  const __grid_constant__ CUtensorMap map_lo) {
   using S = FwdSmem<N_TILE, SPLIT>;
+  using MMA = WgmmaTf32<N_TILE>;
   constexpr int STAGES = S::STAGES;
+  constexpr uint32_t LBO_A = tile_lbo(128);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SW128 tiles need 1024-byte alignment
   uint8_t* sptr = smem_raw + (sbase - smem_u32(smem_raw));
   const uint32_t bar_full = sbase + S::BAR_OFF;
   const uint32_t bar_empty = bar_full + 8 * STAGES;
-  const uint32_t bar_tfull = bar_empty + 8 * STAGES;     // 2 x 8 B
-  const uint32_t bar_tempty = bar_tfull + 16;            // 2 x 8 B
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sptr + S::BAR_OFF + 8 * (2 * STAGES + 4));
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nkb = p.Kp / BK;
@@ -131,12 +118,10 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(bar_full + 8 * s, NPW + 1);   // one elected arrive per producer warp + the TMA thread's expect_tx
-      mbar_init(bar_empty + 8 * s, 1);        // one tcgen05.commit
+      mbar_init(bar_empty + 8 * s, NCONS);    // one arrive per consumer warp once its MMAs have read the stage
     }
-    for (int b = 0; b < 2; ++b) { mbar_init(bar_tfull + 8 * b, 1); mbar_init(bar_tempty + 8 * b, 4); }
     fence_barrier_init();
   }
-  if (warp == NPW + 1) tmem_alloc(smem_u32(tmem_slot), 512);
   // gather table (identical for every tile): element offset inside one image's group slab + tap offsets
   {
     int2* tab = reinterpret_cast<int2*>(sptr + S::TAB_OFF);
@@ -156,15 +141,11 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
       tab[e] = t;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // smem stage layout: [B_hi | B_lo], 1024-aligned; A stages are TMEM columns
   auto stage_b_hi = [&](int s) { return sbase + s * S::STAGE; };
   auto stage_b_lo = [&](int s) { return sbase + s * S::STAGE + S::B_BYTES; };
-  auto stage_a_col = [&](int s) { return S::A_COL0 + (uint32_t)s * S::A_COLS; };
+  auto stage_a_hi = [&](int s) { return sbase + s * S::STAGE + S::B_STAGE; };
 
   auto tile_coords = [&](int tile, int& m0, int& n0, int& g) {
     const int nt = tile % p.n_tiles;
@@ -174,17 +155,17 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
     m0 = mt * 128; n0 = nt * N_TILE;
   };
 
-  if (warp < NPW) {
+  if (warp >= W_PROD0 && warp < W_PROD0 + NPW) {
     // ================= A producers =====================================================================
-    // 16 warps: four threads per GEMM row, each owning two of the eight 16-byte K chunks of every K block.
-    // (A warp is one sequential instruction stream: with 4-8 producer warps the ~170 dependent instructions
-    // per K block and warp, not bandwidth, set the K-block period -- measured ~1450 cycles regardless of
-    // MMA count, tile width or staging path.  More, lighter warps cut that chain to ~60 instructions.)
+    // 8 warps: two threads per GEMM row, each owning four of the eight 16-byte K chunks of every K block.  (Twice as
+    // many, lighter warps would shorten each warp's dependent chain per K block, but their registers are what the
+    // consumers' 128 x 128 fp32 accumulators need.)
     const int2* tab = reinterpret_cast<const int2*>(sptr + S::TAB_OFF);
     const long long HW = (long long)p.H * p.W;
     const int P = p.Ho * p.Wo;
-    const int row = tid & 127, cp = tid >> 7;              // chunk pair 0..3 -> chunks 2cp, 2cp+1 (8 K columns)
-    const uint32_t a_lane = (uint32_t)((warp & 3) * 32) << 16;   // TMEM lane quarter of this warp; row == (warp&3)*32 + lane
+    const int ptid = tid - W_PROD0 * 32;
+    const int row = ptid & 127, cp = ptid >> 7;            // chunk quad 0..1 -> chunks 4cp .. 4cp+3 (16 K columns)
+    const uint32_t a_off = (uint32_t)(4 * cp) * LBO_A + (uint32_t)(row >> 3) * 128u + (uint32_t)(row & 7) * 16u;
     const int my_tiles = (p.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     const int total_blocks = my_tiles * nkb;
     const float* xrow = p.x;
@@ -193,7 +174,7 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
     int lt = 0, lkb = 0;       // load cursor: local tile index, K block inside it
 
     long long pw_load = 0;
-    auto load_block_ = [&](float (&v)[8]) {
+    auto load_block_ = [&](float (&v)[16]) {
       if (lkb == 0) {
         int m0, n0, g;
         tile_coords((int)blockIdx.x + lt * (int)gridDim.x, m0, n0, g);
@@ -207,11 +188,11 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
       }
       if (p.dbg & 1) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = 1.0f;
+        for (int e = 0; e < 16; ++e) v[e] = 1.0f;
       } else if (KMODE == 1) {
-        const int2* te = tab + lkb * KCHUNKS + cp * 2;
+        const int2* te = tab + lkb * KCHUNKS + cp * 4;
 #pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
+        for (int ch = 0; ch < 4; ++ch) {
           const int2 tt = te[ch];
           const bool ok = mvalid && tt.x != INT_MIN && (unsigned)(ih0 + (tt.y & 0xffff)) < (unsigned)p.H &&
                           (unsigned)(iw0 + (tt.y >> 16)) < (unsigned)p.W;
@@ -220,9 +201,9 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
           for (int e = 0; e < 4; ++e) v[ch * 4 + e] = ok ? __ldg(src + e * HW) : 0.0f;
         }
       } else {
-        const int2* te = tab + lkb * BK + cp * 8;
+        const int2* te = tab + lkb * BK + cp * 16;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
+        for (int e = 0; e < 16; ++e) {
           const int2 tt = te[e];
           const bool ok = mvalid && tt.x != INT_MIN && (unsigned)(ih0 + (tt.y & 0xffff)) < (unsigned)p.H &&
                           (unsigned)(iw0 + (tt.y >> 16)) < (unsigned)p.W;
@@ -231,31 +212,20 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
       }
       if (++lkb == nkb) { lkb = 0; ++lt; }
     };
-    auto load_block = [&](float (&v)[8]) { const long long a0 = clock64(); load_block_(v); pw_load += clock64() - a0; };
+    auto load_block = [&](float (&v)[16]) { const long long a0 = clock64(); load_block_(v); pw_load += clock64() - a0; };
     int kbg = 0;   // pipeline position of the store cursor
     long long pw_empty = 0, pw_store = 0;
     const long long pt0 = clock64();
-    auto store_block = [&](const float (&v)[8]) {
+    auto store_block = [&](const float (&v)[16]) {
       const int s = kbg % STAGES, it = kbg / STAGES;
       const long long t0 = clock64();
       mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 40);
       const long long t1 = clock64();
-      tc_fence_after();
-      const uint32_t a_hi = tmem_base + a_lane + stage_a_col(s) + (uint32_t)(cp * 8);
-      if (SPLIT) {
-        float hi[8], lo[8];
+      const uint32_t a_hi = stage_a_hi(s) + a_off;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) split_tf32(v[e], hi[e], lo[e]);
-        tmem_st8(a_hi, hi);
-        tmem_st8(a_hi + 32, lo);
-      } else {
-        float hi[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) hi[e] = to_tf32(v[e]);
-        tmem_st8(a_hi, hi);
-      }
-      tmem_st_wait();
-      tc_fence_before();
+      for (int ch = 0; ch < 4; ++ch)
+        store_chunk<SPLIT>(a_hi + ch * LBO_A, a_hi + ch * LBO_A + S::A_BYTES, v[4 * ch], v[4 * ch + 1], v[4 * ch + 2], v[4 * ch + 3]);
+      fence_proxy_async();
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_full + 8 * s);
       ++kbg;
@@ -263,7 +233,7 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
     };
 
     // two K blocks of loads in flight ahead of the block being stored, across tile boundaries
-    float v0[8], v1[8], v2[8];
+    float v0[16], v1[16], v2[16];
     int issued = 0;
     if (issued < total_blocks) { load_block(v0); ++issued; }
     if (issued < total_blocks) { load_block(v1); ++issued; }
@@ -277,175 +247,131 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
       if (issued < total_blocks) { load_block(v1); ++issued; }
       store_block(v2);
     }
-    if (p.prof && blockIdx.x == 0 && tid == 0) {
+    if (p.prof && blockIdx.x == 0 && ptid == 0) {
       p.prof[0] = clock64() - pt0; p.prof[1] = pw_empty; p.prof[2] = pw_store; p.prof[3] = pw_load; p.prof[4] = total_blocks;
     }
-  } else if (warp == NPW) {
+  } else if (warp == W_TMA) {
     // ================= TMA producer (filter operand) ===================================================
     // (whole warp runs the loop converged; one elected lane issues)
-    {
-      int kbg = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        int m0, n0, g;
-        tile_coords(tile, m0, n0, g);
-        for (int kb = 0; kb < nkb; ++kb, ++kbg) {
-          const int s = kbg % STAGES, it = kbg / STAGES;
-          mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 40);
-          if (elect_one()) {
-            if (p.dbg & 8) {
-              mbar_arrive(bar_full + 8 * s);
-            } else {
-              mbar_arrive_expect_tx(bar_full + 8 * s, S::TX_BYTES);
-              tma_load_3d(stage_b_hi(s), &map_hi, bar_full + 8 * s, kb * BK, n0, g);
-              if (SPLIT) tma_load_3d(stage_b_lo(s), &map_lo, bar_full + 8 * s, kb * BK, n0, g);
-            }
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == NPW + 1) {
-    // ================= MMA issuer ========================================================================
-    // whole warp converged; the elected lane issues tcgen05.mma / tcgen05.commit
-    {
-      constexpr uint32_t IDESC = idesc_tf32(128, N_TILE);
-      int kbg = 0, ti = 0;
-      long long mw_full = 0, mw_issue = 0, mw_tempty = 0;
-      const long long mt0 = clock64();
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++ti) {
-        const int buf = ti % S::ACC_BUFS, use = ti / S::ACC_BUFS;
-        const long long q0 = clock64();
-        mbar_wait(bar_tempty + 8 * buf, (use & 1) ^ 1);         // epilogue has drained this accumulator
-        mw_tempty += clock64() - q0;
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * N_TILE);
-        uint32_t acc = 0;
-        for (int kb = 0; kb < nkb; ++kb, ++kbg) {
-          const int s = kbg % STAGES, it = kbg / STAGES;
-          const long long f0 = clock64();
-          mbar_wait(bar_full + 8 * s, it & 1);
-          const long long f1 = clock64();
-          mw_full += f1 - f0;
-          tc_fence_after();
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < BK / 8; ++kk) {
-              if (p.dbg & 2) break;
-              const uint32_t ah = tmem_base + stage_a_col(s) + (uint32_t)(kk * 8);
-              const uint64_t bh = smem_desc_sw128(stage_b_hi(s) + kk * 32);
-              if (SPLIT) {
-                const uint64_t bl = smem_desc_sw128(stage_b_lo(s) + kk * 32);
-                umma_tf32_ts(d_tmem, ah + 32, bh, IDESC, (kb | kk) != 0);   // lo * hi
-                umma_tf32_ts(d_tmem, ah, bl, IDESC, 1);                      // hi * lo
-                umma_tf32_ts(d_tmem, ah, bh, IDESC, 1);                      // hi * hi
-              } else {
-                umma_tf32_ts(d_tmem, ah, bh, IDESC, (kb | kk) != 0);
-              }
-            }
-            umma_commit(bar_empty + 8 * s);
-            if (kb == nkb - 1) umma_commit(bar_tfull + 8 * buf);
-          }
-          __syncwarp();
-          mw_issue += clock64() - f1;
-        }
-        (void)acc;
-      }
-      if (p.prof && blockIdx.x == 0 && lane == 0) { p.prof[8] = clock64() - mt0; p.prof[9] = mw_full; p.prof[10] = mw_issue; p.prof[11] = mw_tempty; }
-    }
-  } else {
-    // ================= epilogue warps NPW+2 .. NPW+5 ============================================================
-    const int lg = warp & 3;                 // TMEM lane group this warp may access
-    const int r = lg * 32 + lane;            // GEMM row inside the tile
-    const int P = p.Ho * p.Wo;
-    int ti = 0;
-    long long ep_wait = 0, ep_work = 0;
-    float* epi = reinterpret_cast<float*>(sptr + S::EPI_OFF);
-    int epi_chunk = 0;
-    const bool vec_epi = p.out_ws == 1 && p.out_hs == p.Wo && (P & 3) == 0 && (p.out_plane & 3) == 0 &&
-                         (reinterpret_cast<uintptr_t>(p.out) & 15u) == 0 && !(p.dbg & 16);
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++ti) {
+    int kbg = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       int m0, n0, g;
       tile_coords(tile, m0, n0, g);
-      const int buf = ti % S::ACC_BUFS, use = ti / S::ACC_BUFS;
+      for (int kb = 0; kb < nkb; ++kb, ++kbg) {
+        const int s = kbg % STAGES, it = kbg / STAGES;
+        mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 40);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(bar_full + 8 * s, S::TX_BYTES);
+          tma_load_3d(stage_b_hi(s), &map_hi, bar_full + 8 * s, kb * BK, n0, g);
+          if (SPLIT) tma_load_3d(stage_b_lo(s), &map_lo, bar_full + 8 * s, kb * BK, n0, g);
+        }
+        __syncwarp();
+      }
+    }
+  } else if (warp < NCONS) {
+    // ================= consumers: wgmma (accumulators in registers) + epilogue ==============================
+    // warpgroup cw owns tile rows [64 cw, 64 cw + 64); a stage is released once the MMAs of the NEXT stage are
+    // issued (wgmma.wait_group 1), so the tensor core always has the following K block queued.
+    const int cw = warp >> 2, t = tid & 127;
+    const int P = p.Ho * p.Wo;
+    float* epi = reinterpret_cast<float*>(sptr + S::EPI_OFF);
+    const bool vec_epi = p.out_ws == 1 && p.out_hs == p.Wo && (P & 3) == 0 && (p.out_plane & 3) == 0 &&
+                         (reinterpret_cast<uintptr_t>(p.out) & 15u) == 0 && !(p.dbg & 16);
+    float acc[N_TILE / 2];
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
+    int kbg = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      int m0, n0, g;
+      tile_coords(tile, m0, n0, g);
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb, ++kbg) {
+        const int s = kbg % STAGES, it = kbg / STAGES;
+        mbar_wait(bar_full + 8 * s, it & 1);
+        wgmma_fence();
+        if (!(p.dbg & 2)) {
+#pragma unroll
+          for (int kk = 0; kk < BK / 8; ++kk) {
+            const uint32_t a = stage_a_hi(s) + 2u * kk * LBO_A + (uint32_t)cw * 1024u;
+            const uint64_t ah = smem_desc(a, LBO_A, 128);
+            const uint64_t bh = smem_desc_sw128(stage_b_hi(s) + kk * 32);
+            if (SPLIT) {
+              const uint64_t al = smem_desc(a + S::A_BYTES, LBO_A, 128);
+              const uint64_t bl = smem_desc_sw128(stage_b_lo(s) + kk * 32);
+              MMA::mma(acc, al, bh, (kb | kk) != 0);   // lo * hi
+              MMA::mma(acc, ah, bl, 1);                // hi * lo
+              MMA::mma(acc, ah, bh, 1);                // hi * hi
+            } else {
+              MMA::mma(acc, ah, bh, (kb | kk) != 0);
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
+        prev = s;
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+
+      // ---- epilogue: 32-channel chunks transposed through shared memory [channel][128 pixels], then stored
+      const float* brow = p.bias ? p.bias + (long long)g * p.Ntot + n0 : nullptr;
+      const int r = tid & 127, half = tid >> 7;            // row-per-thread store path: channels [16 half, 16 half + 16)
       const int m = m0 + r;
       const bool mvalid = m < p.Mtot;
-      const int mm = mvalid ? m : 0;
-      const int n = mm / P, pix = mm - n * P;
-      const int ho = pix / p.Wo, wo = pix - ho * p.Wo;
-      float* orow = p.out + ((long long)n * p.Cout_tot + (long long)g * p.Ntot + n0) * p.out_plane +
-                    (long long)ho * p.out_hs + (long long)wo * p.out_ws;
-      const float* brow = p.bias ? p.bias + (long long)g * p.Ntot + n0 : nullptr;
-      const long long e0 = clock64();
-      mbar_wait_backoff(bar_tfull + 8 * buf, use & 1, 200);
-      const long long e1 = clock64();
-      ep_wait += e1 - e0;
-      tc_fence_after();
-      if (vec_epi) {
-        // Contiguous output planes: 4-byte stores (128 B per warp instruction, one per channel) left this kernel
-        // bound by the number of store requests in flight on the short-K 1x1 layers (8 000 cycles of stores per
-        // tile against 1 500 of MMA).  Transpose each 32-channel chunk through shared memory so that one warp
-        // instruction writes 128 consecutive pixels of a channel: 512 B per request, a quarter of the requests.
-        const int mv = m0 + lane * 4;                      // this lane's 4 pixels in the store phase
-        const bool mv_ok = mv < p.Mtot;                    // P % 4 == 0: the group is valid or not as a whole
-        const int nv = (mv_ok ? mv : 0) / P, pv = (mv_ok ? mv : 0) - nv * P;
-        float* vbase = p.out + ((long long)nv * p.Cout_tot + (long long)g * p.Ntot + n0) * p.out_plane + pv;
-#pragma unroll 1
-        for (int c0 = 0; c0 < N_TILE; c0 += 32, ++epi_chunk) {
-          if (n0 + c0 >= p.Ntot) break;   // uniform over the four epilogue warps
-          float v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(buf * N_TILE + c0), v);
-          if (c0 + 32 >= N_TILE || n0 + c0 + 32 >= p.Ntot) {   // accumulator fully read: hand it back before storing
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_tempty + 8 * buf);
-          }
-          float* E = epi + (epi_chunk & 1) * (32 * 128);
+      float* orow;
+      {
+        const int mm = mvalid ? m : 0;
+        const int n = mm / P, pix = mm - n * P;
+        const int ho = pix / p.Wo, wo = pix - ho * p.Wo;
+        orow = p.out + ((long long)n * p.Cout_tot + (long long)g * p.Ntot + n0) * p.out_plane +
+               (long long)ho * p.out_hs + (long long)wo * p.out_ws;
+      }
+      const int mv = m0 + lane * 4;                        // vector path: this lane's 4 pixels
+      const bool mv_ok = mv < p.Mtot;                      // P % 4 == 0: the group is valid or not as a whole
+      float* vbase;
+      {
+        const int nv = (mv_ok ? mv : 0) / P, pv = (mv_ok ? mv : 0) - ((mv_ok ? mv : 0) / P) * P;
+        vbase = p.out + ((long long)nv * p.Cout_tot + (long long)g * p.Ntot + n0) * p.out_plane + pv;
+      }
 #pragma unroll
-          for (int j = 0; j < 32; ++j) E[j * 128 + r] = v[j];           // lanes = consecutive pixels: conflict-free
-          asm volatile("bar.sync 1, 128;" ::: "memory");                // the four epilogue warps
-          if (!(p.dbg & 4)) {
+      for (int c = 0; c < N_TILE / 32; ++c) {
+        const int c0 = c * 32;
+        if (n0 + c0 >= p.Ntot) break;                      // uniform over the consumers
+        named_bar(1, NCONS * 32);                          // the previous chunk's stores have read the staging buffer
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const int ch = lg * 8 + q;
-              if (mv_ok && n0 + c0 + ch < p.Ntot) {
-                float4 t = *reinterpret_cast<const float4*>(E + ch * 128 + lane * 4);
-                if (brow) { const float b = __ldg(brow + c0 + ch); t.x += b; t.y += b; t.z += b; t.w += b; }
-                *reinterpret_cast<float4*>(vbase + (long long)(c0 + ch) * p.out_plane) = t;
-              }
+        for (int i = 0; i < N_TILE / 2; ++i)
+          if ((i >> 4) == c) epi[(frag_col(t, i) - c0) * 128 + cw * 64 + frag_row(t, i)] = acc[i];
+        named_bar(1, NCONS * 32);
+        if (p.dbg & 4) continue;
+        if (vec_epi) {
+          // contiguous output planes: one warp instruction writes 128 consecutive pixels of a channel (512 B per request)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int ch = warp * 4 + q;
+            if (mv_ok && n0 + c0 + ch < p.Ntot) {
+              float4 v = *reinterpret_cast<const float4*>(epi + ch * 128 + lane * 4);
+              if (brow) { const float b = __ldg(brow + c0 + ch); v.x += b; v.y += b; v.z += b; v.w += b; }
+              *reinterpret_cast<float4*>(vbase + (long long)(c0 + ch) * p.out_plane) = v;
             }
           }
-        }
-        ep_work += clock64() - e1;
-        continue;
-      }
-#pragma unroll 1
-      for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-        if (n0 + c0 >= p.Ntot) break;   // warp-uniform
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(buf * N_TILE + c0), v);
-        if (mvalid && !(p.dbg & 4)) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (n0 + c0 + j < p.Ntot) {
-              float t = v[j];
-              if (brow) t += __ldg(brow + c0 + j);
-              orow[(long long)(c0 + j) * p.out_plane] = t;
+        } else if (mvalid) {
+#pragma unroll 4
+          for (int j = 0; j < 16; ++j) {
+            const int ch = half * 16 + j;
+            if (n0 + c0 + ch < p.Ntot) {
+              float v = epi[ch * 128 + r];
+              if (brow) v += __ldg(brow + c0 + ch);
+              orow[(long long)(c0 + ch) * p.out_plane] = v;
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * buf);
-      ep_work += clock64() - e1;
     }
-    if (p.prof && blockIdx.x == 0 && r == 0) { p.prof[16] = ep_wait; p.prof[17] = ep_work; p.prof[18] = ti; }
   }
   __syncthreads();
-  if (warp == NPW + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
@@ -499,12 +425,10 @@ static int launch_fwd_n(const FwdParams& p, const CUtensorMap& mh, const CUtenso
   return kmode ? launch_fwd_inst<N_TILE, false, 1>(p, mh, ml, st) : launch_fwd_inst<N_TILE, false, 0>(p, mh, ml, st);
 }
 
-// N tile choice, from the per-layer sweeps in profiles/: the producers stage 32 KB of TF32 hi/lo per K block
-// into tensor memory regardless of N, so narrow tiles are staging-bound (N = 64: ~2x slower per FLOP than
-// N = 128) and N = 256 loses the second accumulator buffer (exposed epilogue).  128 whenever the layer has
-// more than 64 output columns, else the smallest tile that covers them.
-static int pick_n_tile(int Mtot, int Ntot, int G, int Kp, int math) {
-  (void)Mtot; (void)G; (void)Kp; (void)math;
+// N tile choice: the producers stage 16 KB of TF32 hi/lo per K block regardless of N, so narrow tiles are
+// staging-bound; 128 (64 accumulator registers per consumer thread) whenever the layer has more than 64 output
+// columns, else the smallest tile that covers them.
+static int pick_n_tile(int Ntot) {
   if (Ntot > 64) return 128;
   if (Ntot > 32) return 64;
   return 32;
@@ -558,7 +482,7 @@ void tc_conv_prep_entry(const ConvShape& s, int op, int math, const float* w, vo
 int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const float* b, const float* bias, float* out,
                    void* ws, size_t ws_bytes, const void* prepared, cudaStream_t st) {
   if (op == B2C_OP_BACKWARD_FILTER) return launch_conv_tc_wgrad(s, math, a, b, out, ws, ws_bytes, st);
-  if (!prepared && (ws_bytes < tc_conv_workspace(s, op, math) || !ws)) return fail(B2C_ERR_WORKSPACE, "tcgen05 conv: workspace too small");
+  if (!prepared && (ws_bytes < tc_conv_workspace(s, op, math) || !ws)) return fail(B2C_ERR_WORKSPACE, "tensor-core conv: workspace too small");
   FwdParams p;
   PrepEntry q;
   tc_conv_prep_entry(s, op, math, b, prepared ? const_cast<void*>(prepared) : ws, &q);
@@ -600,9 +524,9 @@ int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const f
   if (!prepared)
     if (int rc = launch_filter_prep(&q, 1, st)) return rc;
 
-  int n_tile = pick_n_tile(p.Mtot, p.Ntot, s.G, p.Kp, math);
+  int n_tile = pick_n_tile(p.Ntot);
   { static int force = -1; if (force < 0) { const char* e = getenv("B2C_NTILE"); force = e ? atoi(e) : 0; }
-    if (force && force / 2 < p.Ntot) n_tile = force; }
+    if ((force == 32 || force == 64 || force == 128) && force / 2 < p.Ntot) n_tile = force; }
   p.m_tiles = (p.Mtot + 127) / 128; p.n_tiles = (p.Ntot + n_tile - 1) / n_tile; p.G = s.G;
   p.total_tiles = p.m_tiles * p.n_tiles * p.G;
   alignas(64) CUtensorMap mh, ml;
@@ -613,12 +537,11 @@ int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const f
     int rc = n_tile == 128 ? launch_fwd_n<128>(p, mh, ml, math, kmode, st) : n_tile == 64 ? launch_fwd_n<64>(p, mh, ml, math, kmode, st) : launch_fwd_n<32>(p, mh, ml, math, kmode, st);
     long long h[32];
     cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[prof] N_TILE=%d nkb=%d tiles=%d | producer(t0): total=%lld wait_empty=%lld store=%lld load=%lld blocks=%lld | mma: total=%lld wait_full=%lld issue=%lld wait_tempty=%lld | epi: wait=%lld work=%lld tiles=%lld\n",
-            n_tile, p.Kp / 32, p.total_tiles, h[0], h[1], h[2], h[3], h[4], h[8], h[9], h[10], h[11], h[16], h[17], h[18]);
+    fprintf(stderr, "[prof] N_TILE=%d nkb=%d tiles=%d | producer(t0): total=%lld wait_empty=%lld store=%lld load=%lld blocks=%lld\n",
+            n_tile, p.Kp / 32, p.total_tiles, h[0], h[1], h[2], h[3], h[4]);
     return rc;
   }
   switch (n_tile) {
-    case 256: return launch_fwd_n<256>(p, mh, ml, math, kmode, st);
     case 128: return launch_fwd_n<128>(p, mh, ml, math, kmode, st);
     case 64: return launch_fwd_n<64>(p, mh, ml, math, kmode, st);
     default: return launch_fwd_n<32>(p, mh, ml, math, kmode, st);

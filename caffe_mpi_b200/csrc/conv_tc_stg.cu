@@ -1,4 +1,4 @@
-// conv_tc_stg.cu -- tcgen05 implicit-GEMM convolution with BULK-COPY-STAGED activations and bf16x3 math (sm_100a):
+// conv_tc_stg.cu -- wgmma implicit-GEMM convolution with BULK-COPY-STAGED activations and bf16x3 math (sm_90a):
 // forward and data-gradient of stride-1 "same" convolutions (1x1 / pad 0, 3x3 / pad 1, 5x5 / pad 2 ...), which are
 // 43 of ResNet-50's 53 layers and every VGG-16 / GoogLeNet inception convolution with C % 32 == 0.
 //
@@ -6,33 +6,30 @@
 // (src/caffe/layers/cudnn_conv_layer.cu:25-29,118-123); same contract as conv_tc.cu: NCHW fp32 in and out, whole
 // batch per launch, y / dx overwritten, bias fused.
 //
-// Why a second kernel.  conv_tc.cu gathers the im2col rows with per-thread __ldg: ~1 400 cycles per 128x32 K block
-// against 768 cycles of MMA (profiles/README.md), and it re-reads every input pixel kh*kw times through L1/L2.  Here
-// no thread touches global memory for the activation operand:
+// Why a second kernel.  conv_tc.cu gathers the im2col rows with per-thread __ldg and re-reads every input pixel kh*kw
+// times through L1/L2.  Here no thread touches global memory for the activation operand:
 //   * GEMM rows are 128 CONSECUTIVE flattened pixels q = n*H*W + p.  For 32 input channels the pixels a tile needs --
 //     its own 128 plus a halo of pad*W + pad on either side -- are ONE TMA box per image the tile touches (at most two):
 //     a 3-D tensor map {H*W, C, N} over the NCHW blob, box {BWT pixels, 32 channels, 1 image}, start column
-//     p0 - halo; columns outside the image read as zero.  (A first version used one 1-D bulk copy per channel: the TMA
-//     unit retires ~1 small bulk operation per 90 cycles, 3 000 cycles per 32-channel group -- 1x1 layers ran 2-3x
-//     SLOWER than the gather kernel, profiles/r02_c2_*.)
+//     p0 - halo; columns outside the image read as zero.  (One 1-D bulk copy per channel instead would cost one small
+//     bulk operation per channel, which the TMA unit retires far more slowly than one box.)
 //   * All kh*kw taps of those 32 channels are then served from that ONE staged copy: tap (i,j) of row r is the staged
 //     value at column r + halo + (i-pad)*W + (j-pad); rows whose tap falls outside the image (zero padding, image
 //     borders, row wrap) are masked with a per-row bit computed once per tile.  Global->smem traffic per tile is
 //     (128 + 2*halo)/128 of the input instead of kh*kw times it.
-//   * 16 converter warps read the staged fp32 values (lanes = consecutive pixels: conflict-free; the row pitch BWT is a
-//     template parameter so the eight channel loads of a thread are one base register + immediates), split each into
-//     bf16 hi + bf16 lo (hi = rn(a), lo = rn(a - hi)), pack pairs along K and write the A operand straight into TENSOR
-//     MEMORY with tcgen05.st (lane = GEMM row), 64 K-elements per stage.
+//   * 8 converter warps read the staged fp32 values (lanes = consecutive pixels: conflict-free; the row pitch BWT is a
+//     template parameter so the sixteen channel loads of a thread are one base register + immediates), split each into
+//     bf16 hi + bf16 lo (hi = rn(a), lo = rn(a - hi)), pack pairs along K and write the A operand into shared memory
+//     (K-major, no swizzle, tc_common.cuh), 64 K-elements per stage.
 //   * The filter is pre-split into bf16 hi / lo in GEMM-K order (channel group, tap, channel) by a prepass and streamed
-//     by TMA (SWIZZLE_128B, [N_TILE x 64] boxes); one converged warp issues tcgen05.mma.kind::f16 (bf16 x bf16 -> fp32):
-//     lo*hi + hi*lo + hi*hi per K step -- three bf16 MMAs cost 1.5 TF32-MMA equivalents (3xTF32 costs 3), and the
-//     operand bytes in shared / tensor memory halve.  Dropped terms (lo*lo and the bf16 rounding of lo) are ~2^-17 per
-//     product: measured 5e-6..1.3e-5 blob-level against the 3xTF32 kernel (profiles/r02_c2_diag.log), 100x inside 1e-3.
-//   * Epilogue: double-buffered TMEM accumulators, tcgen05.ld, (+ bias), 32-channel chunks transposed through shared
+//     by TMA (SWIZZLE_128B, [N_TILE x 64] boxes).  Two consumer warpgroups issue wgmma.mma_async.m64nNk16.bf16 (fp32
+//     accumulators in registers, rows [64 cw, 64 cw + 64) each): lo*hi + hi*lo + hi*hi per K step -- three bf16 MMAs
+//     cost 1.5 TF32-MMA equivalents (3xTF32 costs 3), and the operand bytes in shared memory halve.  Dropped terms
+//     (lo*lo and the bf16 rounding of lo) are ~2^-17 per product, far inside the 1e-3 blob tolerance.
+//   * Epilogue (the consumers, after the tile's last K block): (+ bias), 32-channel chunks transposed through shared
 //     memory [channel][128 pixels] and written by the TMA unit when the tile lies inside one image: one tensor store per
 //     chunk (box {128, 32, 1} of the output blob, clipped by the hardware at the image end and the channel count; the start
-//     column is never negative -- a negative store coordinate is an illegal-instruction fault, measured).  Tiles that span
-//     two images write the staged chunk with 16-byte st.global.
+//     column is never negative).  Tiles that span two images write the staged chunk with 16-byte st.global.
 //   * Plane mode (BWT < 128): 7x7 maps, whole image planes staged -- see Smem below.
 // dgrad of a stride-1 same convolution is the same kernel on dY with the transposed + flipped filter.
 #include <cuda.h>
@@ -50,16 +47,15 @@ using namespace tc;
 
 namespace stg {
 
-constexpr int NCW = 16;                       // converter warps
-constexpr int W_BTMA = NCW;                   // filter TMA warp
-constexpr int W_MMA = NCW + 1;                // MMA issuer (also owns the TMEM allocation)
-constexpr int W_STG = NCW + 2;                // activation TMA warp
-constexpr int W_EPI0 = NCW + 3;               // first of 4 epilogue warps
-constexpr int THREADS = (NCW + 7) * 32;       // 736
+constexpr int NCONS = 8;                      // consumer warps: two warpgroups (wgmma + epilogue), tile rows [64 cw, 64 cw + 64)
+constexpr int NCW = 8;                        // converter warps
+constexpr int W_CONV0 = NCONS;                // first converter warp
+constexpr int W_BTMA = NCONS + NCW;           // filter TMA warp
+constexpr int W_STG = NCONS + NCW + 1;        // activation TMA warp
+constexpr int THREADS = (NCONS + NCW + 2) * 32;   // 576
 constexpr int CB = 32;                        // channels per staged group
 constexpr int BKE = 64;                       // bf16 K elements per pipeline stage (two (group, tap) half blocks)
-constexpr int STAGES = 3;                     // operand pipeline depth (B in smem, A in TMEM)
-constexpr uint32_t STG_POOL = 96u * 1024u;    // activation staging pool, carved into slots of one TMA box each
+constexpr uint32_t STG_POOL = 64u * 1024u;    // activation staging pool, carved into slots of one TMA box each
 constexpr int MAX_SLOTS = 6;
 constexpr int MAX_TAPS = 32;                  // per-row validity mask is one 32-bit word
 constexpr int PLANE_IMGS = 4;                 // plane mode: images per staging slot (a 128-row tile of 7x7 maps touches <= 4)
@@ -83,8 +79,8 @@ struct Params {
 template <int N_TILE, int BWT>
 struct Smem {
   static constexpr uint32_t B_BYTES = (uint32_t)N_TILE * 128u;              // [N_TILE rows][64 bf16], SW128
-  static constexpr uint32_t STAGE = 2u * B_BYTES;                           // hi + lo
-  static constexpr uint32_t STG_OFF = STAGES * STAGE;
+  static constexpr uint32_t A_BYTES = tile_bytes(128);                      // [128 rows][64 bf16], K-major no swizzle
+  static constexpr uint32_t STAGE = 2u * B_BYTES + ((2u * A_BYTES + 1023u) & ~1023u);   // B hi, B lo, A hi, A lo
   // BWT >= 128: one box = [32 channels][BWT pixels] fp32.  BWT < 128 ("plane mode", maps of BWT = H*W pixels whose
   // channel pitch TMA cannot address, 7x7 = 196 bytes): one slot = up to PLANE_IMGS whole images x [32 channels][H*W]
   static constexpr bool PLANE = BWT < 128;
@@ -95,39 +91,20 @@ struct Smem {
   static_assert(!PLANE || 127 / BWT + 2 <= PLANE_IMGS, "a 128-row tile touches at most PLANE_IMGS images");
   static constexpr int NSLOT_ = (int)(STG_POOL / SLOT_BYTES);
   static constexpr int NSLOT = NSLOT_ > MAX_SLOTS ? MAX_SLOTS : NSLOT_;
-  static constexpr uint32_t EPI_OFF = STG_OFF + STG_POOL;                   // 2 x [32 channels][128 pixels] fp32
-  static constexpr uint32_t EPI_BYTES = 2u * 32u * 128u * 4u;
+  static constexpr uint32_t EPI_BYTES = 32u * 128u * 4u;                    // [32 channels][128 pixels] fp32
+  static constexpr uint32_t FIXED = STG_POOL + EPI_BYTES + 256u + MAX_TAPS * 4u + 1024u;
+  static constexpr int STAGES_ = (int)((227u * 1024u - FIXED) / STAGE);
+  static constexpr int STAGES = STAGES_ > 3 ? 3 : STAGES_;                  // operand pipeline depth
+  static constexpr uint32_t STG_OFF = STAGES * STAGE;
+  static constexpr uint32_t EPI_OFF = STG_OFF + STG_POOL;
   static constexpr uint32_t BAR_OFF = EPI_OFF + EPI_BYTES;
   static constexpr uint32_t TAP_OFF = BAR_OFF + 256;                        // int tap offsets [MAX_TAPS]
   static constexpr uint32_t TOTAL = TAP_OFF + MAX_TAPS * 4 + 1024;          // + alignment slack
-  static constexpr uint32_t TX_BYTES = STAGE;
-  static constexpr uint32_t A_COL0 = 2u * N_TILE;                           // after the two accumulators
-  static constexpr uint32_t A_COLS = 64u;                                   // 32 packed hi columns + 32 packed lo columns
-  static_assert(A_COL0 + STAGES * A_COLS <= 512u, "TMEM budget");
+  static constexpr uint32_t TX_BYTES = 2u * B_BYTES;
+  static_assert(STAGES >= 2, "shared memory budget");
   static_assert(NSLOT >= 2, "a tile that spans two images needs two boxes per channel group");
 };
 
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// D=F32, A=B=BF16, both K-major
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -152,11 +129,11 @@ __device__ __forceinline__ float lds32(uint32_t addr) {
   asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(addr), "n"(OFF));
   return v;
 }
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+__device__ __forceinline__ void sts128u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 // fp32 pair (k even, k odd) -> packed bf16 hi word and packed bf16 lo word; element k sits in the LOW half
-// (tensor-memory A operand of kind::f16: two consecutive K elements per 32-bit column, little endian)
+// (two consecutive K elements per 32-bit word of the K-major operand tile, little endian)
 __device__ __forceinline__ void split_pack_bf16(float e, float o, uint32_t& hi, uint32_t& lo) {
   const __nv_bfloat162 h = __floats2bfloat162_rn(e, o);            // .x = e (low half), .y = o
   const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h);
@@ -171,41 +148,36 @@ __global__ void __launch_bounds__(THREADS, 1)
 igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                  const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y) {
   using S = Smem<N_TILE, BWT>;
+  using MMA = WgmmaBf16<N_TILE>;
+  constexpr int STAGES = S::STAGES;
   constexpr int NSLOT = S::NSLOT;
   constexpr bool PLANE = S::PLANE;
+  constexpr uint32_t LBO_A = tile_lbo(128);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* sptr = smem_raw + (sbase - smem_u32(smem_raw));
-  const uint32_t bar_full = sbase + S::BAR_OFF;                 // STAGES: 16 converter warps + the filter TMA's expect_tx
-  const uint32_t bar_empty = bar_full + 8 * STAGES;             // STAGES: tcgen05.commit
-  const uint32_t bar_tfull = bar_empty + 8 * STAGES;            // 2
-  const uint32_t bar_tempty = bar_tfull + 16;                   // 2
-  const uint32_t bar_sfull = bar_tempty + 16;                   // MAX_SLOTS: staged box landed
+  const uint32_t bar_full = sbase + S::BAR_OFF;                 // STAGES: 8 converter warps + the filter TMA's expect_tx
+  const uint32_t bar_empty = bar_full + 8 * STAGES;             // STAGES: the 8 consumer warps are done with the stage
+  const uint32_t bar_sfull = bar_empty + 8 * STAGES;            // MAX_SLOTS: staged box landed
   const uint32_t bar_sempty = bar_sfull + 8 * MAX_SLOTS;        // MAX_SLOTS: the converters are done with the box
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sptr + S::BAR_OFF + 8 * (2 * STAGES + 4 + 2 * MAX_SLOTS));
   int* tapoff = reinterpret_cast<int*>(sptr + S::TAP_OFF);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, NCW + 1); mbar_init(bar_empty + 8 * s, 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(bar_tfull + 8 * b, 1); mbar_init(bar_tempty + 8 * b, 4); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, NCW + 1); mbar_init(bar_empty + 8 * s, NCONS); }
     for (int b = 0; b < MAX_SLOTS; ++b) { mbar_init(bar_sfull + 8 * b, 1); mbar_init(bar_sempty + 8 * b, NCW); }
     fence_barrier_init();
   }
-  if (warp == W_MMA) tmem_alloc(smem_u32(tmem_slot), 512);
   if (tid < p.taps) {
     const int i = tid / p.kw, j = tid - i * p.kw;
     tapoff[tid] = ((i - p.ph) * p.W + (j - p.pw)) * 4;          // byte offset inside a staged channel row
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto stage_b_hi = [&](int s) { return sbase + (uint32_t)s * S::STAGE; };
   auto stage_b_lo = [&](int s) { return sbase + (uint32_t)s * S::STAGE + S::B_BYTES; };
-  auto stage_a_col = [&](int s) { return S::A_COL0 + (uint32_t)s * S::A_COLS; };
+  auto stage_a_hi = [&](int s) { return sbase + (uint32_t)s * S::STAGE + 2u * S::B_BYTES; };
   auto slot_addr = [&](int slot) { return sbase + S::STG_OFF + (uint32_t)slot * S::SLOT_BYTES; };
   auto tile_coords = [&](int tile, int& m0, int& n0) {
     const int nt = tile % p.n_tiles;
@@ -222,11 +194,13 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   };
   const bool prof = p.prof != nullptr && blockIdx.x == 0;
 
-  if (warp < NCW) {
-    // ================= converters: staged fp32 -> bf16 hi/lo -> tensor memory ===============================
-    const int rq = warp & 3, sub = warp >> 2;                 // TMEM lane quarter, channel octet [sub*8, sub*8+8) of every half block
+  if (warp >= W_CONV0 && warp < W_CONV0 + NCW) {
+    // ================= converters: staged fp32 -> bf16 hi/lo -> A tile in shared memory ========================
+    // thread = (GEMM row, channel octets sub and sub + 2 of every 32-channel half block)
+    const int cw = warp - W_CONV0;
+    const int rq = cw & 3, sub = cw >> 2;
     const int row = rq * 32 + lane;
-    const uint32_t a_lane = (uint32_t)(rq * 32) << 16;
+    const uint32_t a_row = (uint32_t)(row >> 3) * 128u + (uint32_t)(row & 7) * 16u;
     long long c_t0 = 0;
     if (prof) c_t0 = clock64();
     int kbg = 0;                                               // K blocks processed by this CTA (stage ring position)
@@ -258,9 +232,8 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       }
       // byte offset of this row at tap offset 0 inside its image's box, plus the channel octet of this warp.  Box column 0
       // is pixel max(first pixel of the segment - halo, 0) of the image rounded DOWN to a multiple of 4: the innermost TMA
-      // coordinate has to be 16-byte aligned (an odd start column is an illegal-instruction fault, measured) and never
-      // negative; the TMA unit zero-fills past the image END; taps that reach before pixel 0 belong to masked rows, whatever
-      // they read is discarded
+      // coordinate has to be 16-byte aligned and never negative; the TMA unit zero-fills past the image END; taps that reach
+      // before pixel 0 belong to masked rows, whatever they read is discarded
       // plane mode: whole images are staged, [image][32 channels][H*W]
       const int pp_r = m0 + row - (n_first + img_r) * p.HW;                       // this row's pixel inside its image
       const int start_r = (PLANE || seg_r) ? 0 : max((m0 - n_first * p.HW - p.halo) & ~3, 0);
@@ -268,7 +241,7 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       int g = 0, tap = 0;
       uint32_t src_base = 0;
       for (int kb = 0; kb < p.nkb; ++kb, ++kbg) {
-        uint32_t hi[8], lo[8];
+        uint32_t hi[16], lo[16];                               // [octet o][half block h][4 words]
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (2 * kb + h < p.nhb) {
@@ -280,17 +253,21 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
             }
             const bool ok = (mask >> tap) & 1u;
             const uint32_t src = src_base + (uint32_t)tapoff[tap];
-            float v[8];
             constexpr int CP = (int)S::PITCH;
+            float v[16];
             v[0] = lds32<0>(src); v[1] = lds32<CP>(src); v[2] = lds32<2 * CP>(src); v[3] = lds32<3 * CP>(src);
             v[4] = lds32<4 * CP>(src); v[5] = lds32<5 * CP>(src); v[6] = lds32<6 * CP>(src); v[7] = lds32<7 * CP>(src);
+            v[8] = lds32<16 * CP>(src); v[9] = lds32<17 * CP>(src); v[10] = lds32<18 * CP>(src); v[11] = lds32<19 * CP>(src);
+            v[12] = lds32<20 * CP>(src); v[13] = lds32<21 * CP>(src); v[14] = lds32<22 * CP>(src); v[15] = lds32<23 * CP>(src);
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              uint32_t hw, lw;
-              split_pack_bf16(v[2 * e], v[2 * e + 1], hw, lw);
-              hi[h * 4 + e] = ok ? hw : 0u;                    // masked taps contribute exact zeros (never NaN from stale smem)
-              lo[h * 4 + e] = ok ? lw : 0u;
-            }
+            for (int o = 0; o < 2; ++o)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                uint32_t hw, lw;
+                split_pack_bf16(v[o * 8 + 2 * e], v[o * 8 + 2 * e + 1], hw, lw);
+                hi[(o * 2 + h) * 4 + e] = ok ? hw : 0u;        // masked taps contribute exact zeros (never NaN from stale smem)
+                lo[(o * 2 + h) * 4 + e] = ok ? lw : 0u;
+              }
             if (++tap == p.taps) {                             // group fully consumed by this warp: hand its box(es) back
               tap = 0;
               __syncwarp();
@@ -302,25 +279,30 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
             }
           } else {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) { hi[h * 4 + e] = 0u; lo[h * 4 + e] = 0u; }   // K padding: finite zeros
+            for (int o = 0; o < 2; ++o)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) { hi[(o * 2 + h) * 4 + e] = 0u; lo[(o * 2 + h) * 4 + e] = 0u; }   // K padding: finite zeros
           }
         }
         const int s = kbg % STAGES, it = kbg / STAGES;
         mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 32);
-        tc_fence_after();
-        const uint32_t a0 = tmem_base + a_lane + stage_a_col(s) + (uint32_t)(sub * 4);
-        tmem_st4(a0, hi[0], hi[1], hi[2], hi[3]);
-        tmem_st4(a0 + 16, hi[4], hi[5], hi[6], hi[7]);
-        tmem_st4(a0 + 32, lo[0], lo[1], lo[2], lo[3]);
-        tmem_st4(a0 + 48, lo[4], lo[5], lo[6], lo[7]);
-        tmem_st_wait();
-        tc_fence_before();
+        const uint32_t a0 = stage_a_hi(s) + a_row;
+#pragma unroll
+        for (int o = 0; o < 2; ++o)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t a = a0 + (uint32_t)(h * 4 + sub + 2 * o) * LBO_A;      // 16-byte K chunk = 8 channels
+            const int b = (o * 2 + h) * 4;
+            sts128u(a, hi[b], hi[b + 1], hi[b + 2], hi[b + 3]);
+            sts128u(a + S::A_BYTES, lo[b], lo[b + 1], lo[b + 2], lo[b + 3]);
+          }
+        fence_proxy_async();
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_full + 8 * s);
       }
       u_base += p.groups * nseg;
     }
-    if (prof && tid == 0) { p.prof[0] = clock64() - c_t0; p.prof[3] = kbg; }
+    if (prof && cw == 0 && lane == 0) { p.prof[0] = clock64() - c_t0; p.prof[3] = kbg; }
   } else if (warp == W_BTMA) {
     // ================= filter TMA producer ====================================================================
     int kbg = 0;
@@ -369,140 +351,115 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       }
     }
     if (prof && lane == 0) { p.prof[4] = s_wait; p.prof[5] = u; }
-  } else if (warp == W_MMA) {
-    // ================= MMA issuer ==============================================================================
-    constexpr uint32_t IDESC = idesc_bf16(128, N_TILE);
-    int kbg = 0, ti = 0;
+  } else if (warp < NCONS) {
+    // ================= consumers: wgmma + epilogue ===============================================================
+    const int cwg = warp >> 2, t = tid & 127;
+    float* epi = reinterpret_cast<float*>(sptr + S::EPI_OFF);
+    const bool issuer = warp == 0;
+    float acc[N_TILE / 2];
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
+    int kbg = 0;
     long long m_full = 0, m_t0 = 0;
     if (prof) m_t0 = clock64();
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++ti) {
-      const int buf = ti & 1, use = ti >> 1;
-      mbar_wait(bar_tempty + 8 * buf, (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(buf * N_TILE);
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      int m0, n0, n_first, nseg, split, nimg;
+      tile_coords(tile, m0, n0);
+      tile_images(m0, n_first, nseg, split, nimg);
+      int prev = -1;
       for (int kb = 0; kb < p.nkb; ++kb, ++kbg) {
         const int s = kbg % STAGES, it = kbg / STAGES;
         if (prof) { const long long t0 = clock64(); mbar_wait(bar_full + 8 * s, it & 1); m_full += clock64() - t0; }
         else mbar_wait(bar_full + 8 * s, it & 1);
-        tc_fence_after();
-        if (elect_one()) {
+        wgmma_fence();
 #pragma unroll
-          for (int kk = 0; kk < BKE / 16; ++kk) {
-            const uint32_t ah = tmem_base + stage_a_col(s) + (uint32_t)(kk * 8);
-            const uint64_t bh = desc_sw128(stage_b_hi(s) + kk * 32);
-            const uint64_t bl = desc_sw128(stage_b_lo(s) + kk * 32);
-            umma_bf16_ts(d_tmem, ah + 32, bh, IDESC, (kb | kk) != 0);   // lo * hi
-            umma_bf16_ts(d_tmem, ah, bl, IDESC, 1);                      // hi * lo
-            umma_bf16_ts(d_tmem, ah, bh, IDESC, 1);                      // hi * hi
-          }
-          umma_commit(bar_empty + 8 * s);
-          if (kb == p.nkb - 1) umma_commit(bar_tfull + 8 * buf);
+        for (int kk = 0; kk < BKE / 16; ++kk) {
+          const uint32_t a = stage_a_hi(s) + 2u * kk * LBO_A + (uint32_t)cwg * 1024u;
+          const uint64_t ah = smem_desc(a, LBO_A, 128), al = smem_desc(a + S::A_BYTES, LBO_A, 128);
+          const uint64_t bh = smem_desc_sw128(stage_b_hi(s) + kk * 32), bl = smem_desc_sw128(stage_b_lo(s) + kk * 32);
+          MMA::mma(acc, al, bh, (kb | kk) != 0);   // lo * hi
+          MMA::mma(acc, ah, bl, 1);                // hi * lo
+          MMA::mma(acc, ah, bh, 1);                // hi * hi
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
+        prev = s;
       }
-    }
-    if (prof && lane == 0) { p.prof[8] = clock64() - m_t0; p.prof[9] = m_full; p.prof[10] = kbg; }
-  } else {
-    // ================= epilogue warps ============================================================================
-    // tcgen05.ld -> (+ bias) -> 32-channel chunk transposed into shared memory [channel][128 pixels] -> one TMA tensor
-    // store per image the tile touches.  (The warps' own st.global path cost ~3 100 cycles per 128x128 tile on the
-    // short-K 1x1 layers, profiles/r01_prof_1x1_fwd_store_ablation.txt; 32 one-channel bulk stores per chunk cost ~2 900.)
-    const int lg = warp & 3;                  // TMEM lane quarter this warp may read (warp id % 4)
-    const int r = lg * 32 + lane;
-    const bool issuer = warp == W_EPI0;
-    float* epi = reinterpret_cast<float*>(sptr + S::EPI_OFF);
-    int epi_chunk = 0, ti = 0;
-    long long e_wait = 0, e_work = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++ti) {
-      int m0, n0, n_first, nseg, split, nimg;
-      tile_coords(tile, m0, n0);
-      tile_images(m0, n_first, nseg, split, nimg);
-      const int buf = ti & 1, use = ti >> 1;
-      const float* brow = p.bias ? p.bias + n0 : nullptr;
-      long long e0 = 0;
-      if (prof) e0 = clock64();
-      mbar_wait_backoff(bar_tfull + 8 * buf, use & 1, 128);
-      long long e1 = 0;
-      if (prof) { e1 = clock64(); e_wait += e1 - e0; }
-      tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < N_TILE; c0 += 32, ++epi_chunk) {
-        if (n0 + c0 >= p.Ntot) break;                     // uniform over the four epilogue warps
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(buf * N_TILE + c0), v);
-        if (c0 + 32 >= N_TILE || n0 + c0 + 32 >= p.Ntot) {   // accumulator fully read: hand it back before storing
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_tempty + 8 * buf);
-        }
-        if (brow) {
-          const int nb = min(32, p.Ntot - n0 - c0);
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+
+      // ---- epilogue: (+ bias) -> 32-channel chunks transposed into shared memory [channel][128 pixels] -> one TMA tensor
+      // store per chunk when the tile lies inside one image, else 16-byte st.global; plane mode: per-pixel stores
 #pragma unroll
-          for (int j = 0; j < 32; ++j) if (j < nb) v[j] += __ldg(brow + c0 + j);    // warp-uniform address: broadcast
-        }
+      for (int c = 0; c < N_TILE / 32; ++c) {
+        const int c0 = c * 32;
+        if (n0 + c0 >= p.Ntot) break;                     // uniform over the consumers
+        // the TMA store of the previous chunk has finished reading the staging buffer (elect.sync on a converged warp always
+        // elects the same lane, which owns the bulk-async groups)
+        if (issuer && elect_one()) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        named_bar(1, NCONS * 32);
+#pragma unroll
+        for (int i = 0; i < N_TILE / 2; ++i)
+          if ((i >> 4) == c) {
+            const int col = frag_col(t, i);
+            float v = acc[i];
+            if (p.bias && n0 + col < p.Ntot) v += __ldg(p.bias + n0 + col);
+            epi[(col - c0) * 128 + cwg * 64 + frag_row(t, i)] = v;
+          }
+        fence_proxy_async();                               // generic-proxy writes -> visible to the TMA store
+        named_bar(1, NCONS * 32);
         if constexpr (PLANE) {
-          // lanes = consecutive pixels of an image plane: every channel's store is one (unaligned) 128-byte run per warp,
-          // straight from the registers
+          // thread = (pixel r, 16 channels): every channel's store is one (unaligned) 128-byte run per warp
+          const int r = tid & 127, hc = tid >> 7;
           const int q = m0 + r;
           if (q < p.Mtot) {
             const int nq = q / p.HW;
             float* ob = p.out + ((size_t)nq * p.Ntot + n0 + c0) * p.HW + (q - nq * p.HW);
-            const int nb = min(32, p.Ntot - n0 - c0);
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (j < nb) { float* d = ob + (size_t)j * p.HW; *d = p.accumulate ? *d + v[j] : v[j]; }
+#pragma unroll 4
+            for (int j = 0; j < 16; ++j) {
+              const int ch = hc * 16 + j;
+              if (n0 + c0 + ch < p.Ntot) { float* d = ob + (size_t)ch * p.HW; const float v = epi[ch * 128 + r]; *d = p.accumulate ? *d + v : v; }
+            }
           }
-          continue;
-        }
-        // the store issued two chunks ago from this staging buffer has finished reading it (elect.sync on a converged
-        // warp always elects the same lane, which owns the bulk-async groups)
-        if (issuer && elect_one()) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        float* E = epi + (epi_chunk & 1) * (32 * 128);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) E[j * 128 + r] = v[j];           // lanes = consecutive pixels: conflict-free
-        fence_proxy_async();                                           // generic-proxy writes -> visible to the TMA store
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (nseg == 1 && !(p.dbg & 1)) {
+        } else if (nseg == 1 && !(p.dbg & 1)) {
           // the tile lies inside one image: box column 0 = tile row 0 = pixel m0 - n*HW >= 0; columns past the image end
           // (last tile of an image, rows past the batch) and channels past Ntot are clipped by the TMA unit
           if (issuer && elect_one()) {
-            if (p.accumulate) tma_reduce_add_3d(&map_y, smem_u32(E), m0 - n_first * p.HW, n0 + c0, n_first);
-            else tma_store_3d(&map_y, smem_u32(E), m0 - n_first * p.HW, n0 + c0, n_first);
+            if (p.accumulate) tma_reduce_add_3d(&map_y, smem_u32(epi), m0 - n_first * p.HW, n0 + c0, n_first);
+            else tma_store_3d(&map_y, smem_u32(epi), m0 - n_first * p.HW, n0 + c0, n_first);
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
           }
         } else {
-          // the tile spans two images (1 in 24 tiles at 56x56, 2 in 3 at 14x14): 16-byte st.global from the staged chunk
-          const int mv = m0 + lane * 4;                    // this lane's 4 pixels (H*W % 4 == 0: never across an image end)
+          // the tile spans two images: 16-byte st.global from the staged chunk, warp = 4 channels, lane = 4 pixels
+          const int mv = m0 + lane * 4;                    // H*W % 4 == 0: never across an image end
           if (mv < p.Mtot) {
             const int nv = mv / p.HW, pv = mv - nv * p.HW;
             float* vbase = p.out + ((size_t)nv * p.Ntot + n0 + c0) * p.HW + pv;
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const int ch = lg * 8 + q;
+            for (int q = 0; q < 4; ++q) {
+              const int ch = warp * 4 + q;
               if (n0 + c0 + ch < p.Ntot) {
-                float4 t = *reinterpret_cast<const float4*>(E + ch * 128 + lane * 4);
+                float4 v = *reinterpret_cast<const float4*>(epi + ch * 128 + lane * 4);
                 float4* dst = reinterpret_cast<float4*>(vbase + (size_t)ch * p.HW);
-                if (p.accumulate) { const float4 o = *dst; t.x += o.x; t.y += o.y; t.z += o.z; t.w += o.w; }
-                *dst = t;
+                if (p.accumulate) { const float4 o = *dst; v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w; }
+                *dst = v;
               }
             }
           }
         }
-        if (issuer && elect_one()) asm volatile("cp.async.bulk.commit_group;" ::: "memory");   // one (possibly empty) group per chunk
       }
-      if (prof) e_work += clock64() - e1;
     }
     if (issuer && elect_one()) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    if (prof && r == 0) { p.prof[16] = e_wait; p.prof[17] = e_work; p.prof[18] = ti; }
+    if (prof && tid == 0) { p.prof[8] = clock64() - m_t0; p.prof[9] = m_full; p.prof[10] = kbg; }
   }
   __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 }  // namespace stg
+
 
 // ---- host side ------------------------------------------------------------------------------------------------------
 typedef CUresult (*StgEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -651,10 +608,10 @@ bool tc_stg_prep_entry(const ConvShape& s, int op, const float* w, void* dst, Pr
 int launch_conv_tc_stg(const ConvShape& s, int op, const float* a, const float* w, const float* bias, float* out, void* ws,
                        size_t ws_bytes, const void* prepared, bool accumulate, cudaStream_t st) {
   StgGeom g;
-  if (!stg_geom(s, op, &g)) return fail(B2C_ERR_INVALID, "staged tcgen05 conv: shape not eligible");
-  if (!prepared && (!ws || ws_bytes < tc_stg_workspace(s, op))) return fail(B2C_ERR_WORKSPACE, "staged tcgen05 conv: workspace too small");
+  if (!stg_geom(s, op, &g)) return fail(B2C_ERR_INVALID, "staged tensor-core conv: shape not eligible");
+  if (!prepared && (!ws || ws_bytes < tc_stg_workspace(s, op))) return fail(B2C_ERR_WORKSPACE, "staged tensor-core conv: workspace too small");
   if ((reinterpret_cast<uintptr_t>(a) & 15u) || (reinterpret_cast<uintptr_t>(out) & 15u))
-    return fail(B2C_ERR_INVALID, "staged tcgen05 conv: activations must be 16-byte aligned");
+    return fail(B2C_ERR_INVALID, "staged tensor-core conv: activations must be 16-byte aligned");
   PrepEntry q;
   tc_stg_prep_entry(s, op, w, prepared ? const_cast<void*>(prepared) : ws, &q);
   if (!prepared)
@@ -696,8 +653,8 @@ int launch_conv_tc_stg(const ConvShape& s, int op, const float* a, const float* 
   if (rc == B2C_OK && prof_on) {
     long long h[32];
     cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[stg-prof] N_TILE=%d BWT=%d nkb=%d groups=%d taps=%d tiles=%d | conv(t0): total=%lld kblocks=%lld | act-tma: wait_empty=%lld boxes=%lld | mma: total=%lld wait_full=%lld | epi: wait=%lld work=%lld tiles=%lld\n",
-            n_tile, g.bwt, g.nkb, g.groups, g.taps, p.total_tiles, h[0], h[3], h[4], h[5], h[8], h[9], h[16], h[17], h[18]);
+    fprintf(stderr, "[stg-prof] N_TILE=%d BWT=%d nkb=%d groups=%d taps=%d tiles=%d | conv(t0): total=%lld kblocks=%lld | act-tma: wait_empty=%lld boxes=%lld | consumer: total=%lld wait_full=%lld kblocks=%lld\n",
+            n_tile, g.bwt, g.nkb, g.groups, g.taps, p.total_tiles, h[0], h[3], h[4], h[5], h[8], h[9], h[10]);
   }
   return rc;
 }

@@ -1,11 +1,12 @@
-// conv_tc_wgrad.cu -- tcgen05 implicit-GEMM weight-gradient kernel (sm_100a).
+// conv_tc_wgrad.cu -- wgmma implicit-GEMM weight-gradient kernels (sm_90a).
 //
 // Replaces cudnnConvolutionBackwardFilter beta=1 (reference src/caffe/layers/cudnn_conv_layer.cu:95-99)
 // and, semantically, the per-image weight_gpu_gemm loop (base_conv_layer.hpp:148-162):
 //     dW[o][k'=(c,i,j)] += sum_{q=(n,ho,wo)} dY[n,o,ho,wo] * X[n,c,ho*s-p+i*d,wo*s-p+j*d]
 // GEMM view: M = output channels of one group (tile 128), N = K_dim = (C/g)*kh*kw (tile N_TILE), the
 // reduction runs over q = N*Ho*Wo, which is the CONTIGUOUS axis of both operands in NCHW memory, so both
-// smem tiles are filled "lanes along K": dY with 128-bit loads, X through the im2col gather.  The
+// smem tiles are filled "lanes along K": dY with 128-bit loads, X through the im2col gather.  Two consumer
+// warpgroups (warps 0-7) issue wgmma from the two tiles and keep the fp32 accumulators in registers.  The
 // reduction is split across CTAs (grid.x); partial tiles go to a workspace and the tile's CTAs then add them
 // to dW in split order (splitk_fused_reduce; the reference accumulates image by image, also a fixed order).
 #include <cuda.h>
@@ -16,9 +17,10 @@
 namespace b2c {
 using namespace tc;
 
-constexpr int WG_YW = 8;                        // dY producer warps (warps 0-3 of them run the epilogue afterwards)
-constexpr int WG_GW = 16;                       // X-gather producer warps
-constexpr int WG_THREADS = (WG_YW + WG_GW + 1) * 32;   // + the MMA warp
+constexpr int NCONS = 8;                        // consumer warps: two warpgroups (wgmma + epilogue), tile rows [64 cw, 64 cw + 64)
+constexpr int WG_YW = 8;                        // dY producer warps
+constexpr int WG_GW = 8;                        // X-gather producer warps
+constexpr int WG_THREADS = (NCONS + WG_YW + WG_GW) * 32;   // 768
 
 struct WgradParams {
   const float* dy;   // [N, O, Ho, Wo]
@@ -40,10 +42,13 @@ struct WgradSmem {
   static constexpr uint32_t B_BYTES = tile_bytes(N_TILE);
   static constexpr uint32_t STAGE = (SPLIT ? 2u : 1u) * (A_BYTES + B_BYTES);
   static constexpr uint32_t TABLE = N_TILE * 8u;
-  static constexpr int STAGES = (int)((216u * 1024u) / STAGE) > 6 ? 6 : (int)((216u * 1024u) / STAGE);
+  static constexpr uint32_t PROM_BYTES = NCONS * 32u * (N_TILE / 2) * 4u;   // the consumers' promoted accumulators
+  static constexpr int STAGES_ = (int)((216u * 1024u - PROM_BYTES) / STAGE);
+  static constexpr int STAGES = STAGES_ > 6 ? 6 : STAGES_;
   static constexpr uint32_t BAR_OFF = STAGES * STAGE;
   static constexpr uint32_t TAB_OFF = BAR_OFF + 256;
-  static constexpr uint32_t TOTAL = TAB_OFF + TABLE;
+  static constexpr uint32_t PROM_OFF = TAB_OFF + TABLE;
+  static constexpr uint32_t TOTAL = PROM_OFF + PROM_BYTES;
 };
 
 // ---- split-K reduction fused into the tile's own CTAs ---------------------------------------------------------------------
@@ -94,13 +99,12 @@ template <int N_TILE, bool SPLIT, bool X1X1>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
   using S = WgradSmem<N_TILE, SPLIT>;
+  using MMA = WgmmaTf32<N_TILE>;
   constexpr int STAGES = S::STAGES;
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar_full = sbase + S::BAR_OFF;
   const uint32_t bar_empty = bar_full + 8 * STAGES;
-  const uint32_t bar_tmem = bar_empty + 8 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + S::BAR_OFF + 8 * (2 * STAGES + 1));
   int2* rowtab = reinterpret_cast<int2*>(smem + S::TAB_OFF);   // per B row: {channel offset, hoff | woff<<16}
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -117,11 +121,9 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
   const int nkb = (int)(kb_end - kb_begin);           // >= 1 by construction
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, WG_YW + WG_GW); mbar_init(bar_empty + 8 * s, 1); }   // one elected arrive per producer warp
-    mbar_init(bar_tmem, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, WG_YW + WG_GW); mbar_init(bar_empty + 8 * s, NCONS); }   // one elected arrive per producer / consumer warp
     fence_barrier_init();
   }
-  if (warp == WG_YW + WG_GW) tmem_alloc(smem_u32(tmem_slot), N_TILE);
   // row table for the X gather: k' = (c,i,j)
   for (int r = tid; r < N_TILE; r += WG_THREADS) {
     const int kp = n0 + r;
@@ -133,10 +135,7 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
     }
     rowtab[r] = e;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   constexpr uint32_t LBO_A = tile_lbo(128), LBO_B = tile_lbo(N_TILE);
   auto stage_a_hi = [&](int s) { return sbase + s * S::STAGE; };
@@ -144,9 +143,10 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
   auto stage_b_hi = [&](int s) { return sbase + s * S::STAGE + (SPLIT ? 2u : 1u) * S::A_BYTES; };
   auto stage_b_lo = [&](int s) { return stage_b_hi(s) + S::B_BYTES; };
 
-  if (warp < WG_YW) {
+  if (warp >= NCONS && warp < NCONS + WG_YW) {
     // ================= A producer: dY rows (output channels), lanes along q ==========================
-    const int kc = tid & 7, rb = tid >> 3;              // rb in [0, 32): rows r*32 + rb, r < 4
+    const int ytid = tid - NCONS * 32;
+    const int kc = ytid & 7, rb = ytid >> 3;            // rb in [0, 32): rows r*32 + rb, r < 4
     const bool vec_ok = (P % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.dy) & 15u) == 0);
     // loads of k-block kb+1 are issued before the stores of k-block kb (register double buffer)
     // q = n*P + p of this thread's first element; advanced by BK per K block with 32-bit arithmetic only
@@ -219,48 +219,16 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
       }
       if (kb < nkb) store_block(kb, va);
     }
-    const long long pa_t1 = clock64();
-    if (warp < 4) {
-    // ================= epilogue: TMEM -> registers -> smem transpose -> coalesced row stores ===========
-    mbar_wait_backoff(bar_tmem, 0, 100);
-    const long long pa_t2 = clock64();
-    tc_fence_after();
-    // all MMAs have completed, so the pipeline stages are free: each warp uses a private 32 x 33 fp32 pad
-    float* tpad = reinterpret_cast<float*>(smem) + warp * (32 * 33);
-    float* obase = p.out + (p.splits > 1 ? (long long)split * p.O * p.Kd : 0LL) + ((long long)g * p.Og + m0 + warp * 32) * p.Kd + n0;
-    const int rows_valid = p.Og - (m0 + warp * 32);       // rows of this warp's 32 that exist
-    const bool accumulate = p.splits == 1;
-#pragma unroll 1
-    for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-      if (n0 + c0 >= p.Kd) break;
-      float v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) tpad[lane * 33 + j] = v[j];     // row = lane, conflict-free (stride 33)
-      __syncwarp();
-      const bool colok = n0 + c0 + lane < p.Kd;
-#pragma unroll 4
-      for (int r = 0; r < 32; ++r) {
-        if (r < rows_valid && colok) {
-          float* dst = obase + (long long)r * p.Kd + c0 + lane;     // 32 lanes -> 128 contiguous bytes
-          const float t = tpad[r * 33 + lane];
-          *dst = accumulate ? *dst + t : t;
-        }
-      }
-      __syncwarp();
+    if (p.prof && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && ytid == 0) {
+      p.prof[0] = clock64() - pa_t0; p.prof[1] = pa_wait; p.prof[2] = pa_store; p.prof[5] = nkb;
     }
-    tc_fence_before();
-    if (p.prof && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && tid == 0) {
-      p.prof[0] = pa_t1 - pa_t0; p.prof[1] = pa_wait; p.prof[2] = pa_store; p.prof[3] = pa_t2 - pa_t1; p.prof[4] = clock64() - pa_t2; p.prof[5] = nkb;
-    }
-    }
-  } else if (warp < WG_YW + WG_GW) {
+  } else if (warp >= NCONS + WG_YW) {
     // ================= B producer: im2col gather of X, rows k'=(c,i,j), lanes along q ==================
-    const int t = tid - WG_YW * 32;
-    const int kc = t & 7, rb = t >> 3;                 // rb in [0, 64)
+    const int t = tid - (NCONS + WG_YW) * 32;
+    const int kc = t & 7, rb = t >> 3;                 // rb in [0, 32): rows r*32 + rb, r < N_TILE / 32
     const bool vec_ok = X1X1 && (P % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.x) & 15u) == 0);
-    constexpr int RB = N_TILE >= 64 ? N_TILE / 64 : 1;
-    const bool row_active = rb < N_TILE;               // N_TILE = 32: upper half of the threads only arrive
+    constexpr int RB = N_TILE / 32;
+    const bool row_active = true;
     int cur_n, cur_ho, cur_wo;
     {
       const long long q0 = kb_begin * BK + kc * 4;
@@ -296,7 +264,7 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
         float* vv = v + r * 4;
         vv[0] = vv[1] = vv[2] = vv[3] = 0.f;
         if (!row_active) continue;
-        const int2 rt = rowtab[r * 64 + rb];
+        const int2 rt = rowtab[r * 32 + rb];
         if (rt.x >= 0) {
           if (X1X1) {
             // k=1, s=1, p=0: X rows are contiguous in q exactly like dY
@@ -332,7 +300,7 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
       if (row_active) {
 #pragma unroll
         for (int r = 0; r < RB; ++r) {
-          const int row = r * 64 + rb;
+          const int row = r * 32 + rb;
           store_chunk<SPLIT>(b_hi + row * 16, b_lo + row * 16, v[r * 4], v[r * 4 + 1], v[r * 4 + 2], v[r * 4 + 3]);
         }
       }
@@ -353,53 +321,73 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
       }
       if (kb < nkb) store_block(kb, va);
     }
-    if (p.prof && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && tid == WG_YW * 32) {  // first X-gather thread
+    if (p.prof && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && t == 0) {  // first X-gather thread
       p.prof[8] = clock64() - pb_t0; p.prof[9] = pb_wait; p.prof[10] = pb_store;
     }
-  } else {
-    // MMA issuer: whole warp converged, the elected lane issues (see elect_one() in tc_common.cuh)
-    constexpr uint32_t IDESC = idesc_tf32(128, N_TILE);
-    long long mw = 0, mi = 0;
-    const long long m_t0 = clock64();
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % STAGES, it = kb / STAGES;
-      const long long f0 = clock64();
-      mbar_wait(bar_full + 8 * s, it & 1);
-      const long long f1 = clock64();
-      mw += f1 - f0;
-      tc_fence_after();
-      if (elect_one()) {
+  } else if (warp < NCONS) {
+    // ================= consumers: wgmma over the CTA's K range, then the partial tile from registers =================
+    // Every PROMOTE K blocks (512 pixels) the wgmma accumulator is added into a promoted sum on the CUDA cores and restarted.
+    // Accumulating a whole split in the wgmma accumulator measured outside the 3e-4 dW bar of test_full_size_vs_reference_loop
+    // on an H100 where the one-wave split plan leaves each CTA a long reduction: AlexNet conv2 (g = 2, N = 256) 4.3e-4, conv3
+    // 3.1e-4 (43k pixels per CTA); with the promotion both pass.
+    // The promoted sum lives in shared memory, element i of consumer thread tid at prom[i * 256 + tid] (conflict-free): the
+    // 80 registers a thread of this 768-thread kernel has hold the wgmma accumulators, not a second copy of them.
+    constexpr int PROMOTE = 16;
+    const int cw = warp >> 2, t = tid & 127;
+    float acc[N_TILE / 2];
+    float* prom = reinterpret_cast<float*>(smem + S::PROM_OFF) + tid;
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) prom[i * NCONS * 32] = 0.f;
+    int prev = -1;
+    // chunks of PROMOTE K blocks: the wait for the whole chunk's MMAs is unconditional (a wgmma wait under a data-dependent
+    // branch makes ptxas serialize every wgmma of the kernel)
+    for (int kb0 = 0; kb0 < nkb; kb0 += PROMOTE) {
+      const int kend = min(nkb, kb0 + PROMOTE);
+      for (int kb = kb0; kb < kend; ++kb) {
+        const int s = kb % STAGES, it = kb / STAGES;
+        mbar_wait(bar_full + 8 * s, it & 1);
+        wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < BK / 8; ++kk) {
-          const uint64_t ah = smem_desc(stage_a_hi(s) + 2 * kk * LBO_A, LBO_A, 128);
+          const uint32_t a = stage_a_hi(s) + 2u * kk * LBO_A + (uint32_t)cw * 1024u;
+          const uint64_t ah = smem_desc(a, LBO_A, 128);
           const uint64_t bh = smem_desc(stage_b_hi(s) + 2 * kk * LBO_B, LBO_B, 128);
           if (SPLIT) {
-            const uint64_t al = smem_desc(stage_a_lo(s) + 2 * kk * LBO_A, LBO_A, 128);
+            const uint64_t al = smem_desc(stage_a_lo(s) + 2u * kk * LBO_A + (uint32_t)cw * 1024u, LBO_A, 128);
             const uint64_t bl = smem_desc(stage_b_lo(s) + 2 * kk * LBO_B, LBO_B, 128);
-            umma_tf32(tmem_base, al, bh, IDESC, (kb | kk) != 0);
-            umma_tf32(tmem_base, ah, bl, IDESC, 1);
-            umma_tf32(tmem_base, ah, bh, IDESC, 1);
+            MMA::mma(acc, al, bh, kb != kb0 || kk != 0);
+            MMA::mma(acc, ah, bl, 1);
+            MMA::mma(acc, ah, bh, 1);
           } else {
-            umma_tf32(tmem_base, ah, bh, IDESC, (kb | kk) != 0);
+            MMA::mma(acc, ah, bh, kb != kb0 || kk != 0);
           }
         }
-        umma_commit(bar_empty + 8 * s);
-        if (kb == nkb - 1) umma_commit(bar_tmem);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
+        prev = s;
       }
-      __syncwarp();
-      mi += clock64() - f1;
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+#pragma unroll
+      for (int i = 0; i < N_TILE / 2; ++i) prom[i * NCONS * 32] += acc[i];
     }
-    if (p.prof && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && lane == 0) { p.prof[16] = clock64() - m_t0; p.prof[17] = mw; p.prof[18] = mi; }
+    // row = output channel, column = k'; lanes of a quad write 8 consecutive columns of a row
+    const bool accumulate = p.splits == 1;
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) {
+      const int r = m0 + cw * 64 + frag_row(t, i), c = n0 + frag_col(t, i);
+      if (r < p.Og && c < p.Kd) {
+        float* dst = p.out + (p.splits > 1 ? (long long)split * p.O * p.Kd : 0LL) + ((long long)g * p.Og + r) * p.Kd + c;
+        const float v = prom[i * NCONS * 32];
+        *dst = accumulate ? *dst + v : v;
+      }
+    }
   }
   if (p.splits > 1) {
     const int tile_id = blockIdx.z * gridDim.y + blockIdx.y;
     splitk_fused_reduce(p.out, p.grad, p.counters + tile_id, split, p.splits, (long long)p.O * p.Kd,
                         ((long long)g * p.Og + m0) * p.Kd + n0, p.Kd, min(128, p.Og - m0), min(N_TILE, p.Kd - n0));
-  }
-  __syncthreads();
-  if (warp == WG_YW + WG_GW) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, N_TILE);
   }
 }
 
@@ -407,17 +395,17 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
 // 1x1 / stride 1 / pad 0 layers (24 of ResNet-50's 53): per image both operands are plain row-major matrices with the
 // reduction axis q = (ho,wo) contiguous -- dY[n] is [O x P], X[n] is [C x P] -- so neither needs a gather:
 //   * one elected thread drops [128 x 32] (dY) and [N_TILE x 32] (X) fp32 boxes into shared memory with TMA
-//     (3-D tensor maps {P, rows, N}, SWIZZLE_128B = the canonical K-major UMMA layout; rows past O / C and columns
+//     (3-D tensor maps {P, rows, N}, SWIZZLE_128B = a canonical K-major wgmma layout; rows past O / C and columns
 //     past P are zero-filled by the TMA unit, which is exactly the padding the GEMM needs);
-//   * the RAW tile is the TF32 "hi" operand as it stands: kind::tf32 reads the top 19 bits of each fp32 word, i.e.
+//   * the RAW tile is the TF32 "hi" operand as it stands: the tf32 MMA reads the top 19 bits of each fp32 word, i.e.
 //     a & 0xffffe000 -- the same truncation split_tf32() applies in software;
 //   * 8 converter warps produce the "lo" tiles, lo = a - (a & 0xffffe000), position by position (the copy is
 //     layout-agnostic: same swizzled offset in a second buffer), 12 x (LDS.128 + 8 ALU + STS.128) per thread and K block;
-//   * the MMA warp issues lo*hi + hi*lo + hi*hi from shared-memory descriptors as in the gather kernel.
+//   * two consumer warpgroups issue lo*hi + hi*lo + hi*hi from shared-memory descriptors as in the gather kernel.
 // K blocks are enumerated per image (ceil(P/32) chunks, the last one zero padded) and split across CTAs in one wave.
 // fp32-equivalent math only: single-pass TF32 mode needs round-to-nearest operands and keeps the gather kernel.
-constexpr int WT_CW = 8;                               // converter warps (warps 0-3 also run the epilogue)
-constexpr int WT_THREADS = (WT_CW + 2) * 32;           // + TMA warp + MMA warp
+constexpr int WT_CW = 8;                               // converter warps
+constexpr int WT_THREADS = (NCONS + WT_CW + 1) * 32;   // consumers + converters + TMA warp = 544
 
 struct WgradTmaParams {
   int O, C;              // rows of dY / X per image (G = 1)
@@ -441,15 +429,6 @@ struct WgradTmaSmem {
   static constexpr uint32_t TOTAL = BAR_OFF + 256 + 1024;              // + 1024-byte alignment slack
 };
 
-__device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t addr) {    // K-major, SWIZZLE_128B, 8-row groups 1024 B apart
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
 __device__ __forceinline__ void wg_tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -470,6 +449,7 @@ __global__ void __launch_bounds__(WT_THREADS, 1)
 wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_constant__ CUtensorMap map_dy,
                     const __grid_constant__ CUtensorMap map_x) {
   using S = WgradTmaSmem<N_TILE>;
+  using MMA = WgmmaTf32<N_TILE>;
   constexpr int STAGES = S::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;        // SW128 tiles need 1024-byte alignment
@@ -477,8 +457,6 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
   const uint32_t bar_raw = sbase + S::BAR_OFF;                         // TMA bytes have landed
   const uint32_t bar_full = bar_raw + 8 * STAGES;                      // lo tiles written
   const uint32_t bar_empty = bar_full + 8 * STAGES;                    // MMAs of the stage have completed
-  const uint32_t bar_tmem = bar_empty + 8 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sptr + S::BAR_OFF + 8 * (3 * STAGES + 1));
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int split = blockIdx.x;
@@ -493,21 +471,16 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(bar_raw + 8 * s, 1);
       mbar_init(bar_full + 8 * s, WT_CW);
-      mbar_init(bar_empty + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, NCONS);
     }
-    mbar_init(bar_tmem, 1);
     fence_barrier_init();
   }
-  if (warp == WT_CW + 1) tmem_alloc(smem_u32(tmem_slot), N_TILE);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto stage_a = [&](int s) { return sbase + (uint32_t)s * S::STAGE; };            // raw dY tile (hi operand)
   auto stage_b = [&](int s) { return sbase + (uint32_t)s * S::STAGE + S::A_BYTES; };  // raw X tile
 
-  if (warp < WT_CW) {
+  if (warp >= NCONS && warp < NCONS + WT_CW) {
     // ================= converters: lo = a - trunc_tf32(a), same offset in the lo half of the stage =============
     constexpr int UNITS = (int)(S::RAW_BYTES / 16u);                   // 16-byte units per stage, multiple of 256
     for (int kb = 0; kb < nkb; ++kb) {
@@ -515,7 +488,7 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
       mbar_wait_backoff(bar_raw + 8 * s, it & 1, 20);
       const uint32_t src = stage_a(s);
 #pragma unroll 4
-      for (int u = tid; u < UNITS; u += WT_CW * 32) {
+      for (int u = tid - NCONS * 32; u < UNITS; u += WT_CW * 32) {
         const float4 v = wg_lds128(src + (uint32_t)u * 16u);
         float h, l0, l1, l2, l3;
         split_tf32(v.x, h, l0); split_tf32(v.y, h, l1); split_tf32(v.z, h, l2); split_tf32(v.w, h, l3);
@@ -525,36 +498,7 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_full + 8 * s);
     }
-    if (warp < 4) {
-      // ================= epilogue: TMEM -> registers -> smem transpose -> coalesced row stores ==================
-      mbar_wait_backoff(bar_tmem, 0, 100);
-      tc_fence_after();
-      float* tpad = reinterpret_cast<float*>(sptr) + warp * (32 * 33);   // all MMAs done: the stages are free
-      float* obase = p.out + (p.splits > 1 ? (long long)split * p.O * p.C : 0LL) + (long long)(m0 + warp * 32) * p.C + n0;
-      const int rows_valid = p.O - (m0 + warp * 32);
-      const bool accumulate = p.splits == 1;
-#pragma unroll 1
-      for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-        if (n0 + c0 >= p.C) break;
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) tpad[lane * 33 + j] = v[j];
-        __syncwarp();
-        const bool colok = n0 + c0 + lane < p.C;
-#pragma unroll 4
-        for (int r = 0; r < 32; ++r) {
-          if (r < rows_valid && colok) {
-            float* dst = obase + (long long)r * p.C + c0 + lane;
-            const float t = tpad[r * 33 + lane];
-            *dst = accumulate ? *dst + t : t;
-          }
-        }
-        __syncwarp();
-      }
-      tc_fence_before();
-    }
-  } else if (warp == WT_CW) {
+  } else if (warp == NCONS + WT_CW) {
     // ================= TMA producer (whole warp converged, one elected lane issues) ============================
     int n = (int)(kb_begin / p.cpi), j = (int)(kb_begin - (long long)n * p.cpi);
     for (int kb = 0; kb < nkb; ++kb) {
@@ -568,28 +512,40 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
       __syncwarp();
       if (++j == p.cpi) { j = 0; ++n; }
     }
-  } else {
-    // ================= MMA issuer (whole warp converged, elect.sync) ============================================
-    constexpr uint32_t IDESC = idesc_tf32(128, N_TILE);
+  } else if (warp < NCONS) {
+    // ================= consumers: wgmma over the CTA's K range, then the partial tile from registers =================
+    const int cw = warp >> 2, t = tid & 127;
+    float acc[N_TILE / 2];
+    int prev = -1;
     for (int kb = 0; kb < nkb; ++kb) {
       const int s = kb % STAGES, it = kb / STAGES;
       mbar_wait(bar_full + 8 * s, it & 1);
-      tc_fence_after();
-      if (elect_one()) {
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < BK / 8; ++kk) {
-          const uint64_t ah = wg_desc_sw128(stage_a(s) + kk * 32);
-          const uint64_t bh = wg_desc_sw128(stage_b(s) + kk * 32);
-          const uint64_t al = wg_desc_sw128(stage_a(s) + S::RAW_BYTES + kk * 32);
-          const uint64_t bl = wg_desc_sw128(stage_b(s) + S::RAW_BYTES + kk * 32);
-          umma_tf32(tmem_base, al, bh, IDESC, (kb | kk) != 0);
-          umma_tf32(tmem_base, ah, bl, IDESC, 1);
-          umma_tf32(tmem_base, ah, bh, IDESC, 1);
-        }
-        umma_commit(bar_empty + 8 * s);
-        if (kb == nkb - 1) umma_commit(bar_tmem);
+      for (int kk = 0; kk < BK / 8; ++kk) {
+        const uint32_t a = stage_a(s) + (uint32_t)cw * 8192u + kk * 32;     // rows [64 cw, 64 cw + 64): 8 groups of 8 rows x 128 B
+        const uint64_t ah = smem_desc_sw128(a), al = smem_desc_sw128(a + S::RAW_BYTES);
+        const uint64_t bh = smem_desc_sw128(stage_b(s) + kk * 32), bl = smem_desc_sw128(stage_b(s) + S::RAW_BYTES + kk * 32);
+        MMA::mma(acc, al, bh, (kb | kk) != 0);
+        MMA::mma(acc, ah, bl, 1);
+        MMA::mma(acc, ah, bh, 1);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence(acc);
+    // row = output channel, column = k'; lanes of a quad write 8 consecutive columns of a row
+    const bool accumulate = p.splits == 1;
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) {
+      const int r = m0 + cw * 64 + frag_row(t, i), c = n0 + frag_col(t, i);
+      if (r < p.O && c < p.C) {
+        float* dst = p.out + (p.splits > 1 ? (long long)split * p.O * p.C : 0LL) + (long long)r * p.C + c;
+        *dst = accumulate ? *dst + acc[i] : acc[i];
+      }
     }
   }
   if (p.splits > 1) {
@@ -597,18 +553,13 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
     splitk_fused_reduce(p.out, p.grad, p.counters + tile_id, split, p.splits, (long long)p.O * p.C, (long long)m0 * p.C + n0, p.C,
                         min(128, p.O - m0), min(N_TILE, p.C - n0));
   }
-  __syncthreads();
-  if (warp == WT_CW + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, N_TILE);
-  }
 }
 
 struct WgradPlan { int n_tile, splits, kb_per_split; };
 
 static WgradPlan wgrad_plan(const ConvShape& s) {
   WgradPlan pl;
-  pl.n_tile = s.Kd > 128 ? 256 : s.Kd > 64 ? 128 : s.Kd > 32 ? 64 : 32;
+  pl.n_tile = s.Kd > 32 ? 64 : 32;                  // 768 threads leave 80 registers: 32 accumulators per consumer thread
   const long long Q = (long long)s.N * s.Ho * s.Wo;
   const long long nkb = (Q + BK - 1) / BK;
   const long long mn = (long long)((s.Og + 127) / 128) * ((s.Kd + pl.n_tile - 1) / pl.n_tile) * s.G;
@@ -672,7 +623,7 @@ static bool wgrad_tma_shape_ok(const ConvShape& s) {
 }
 static WgradPlan wgrad_tma_plan(const ConvShape& s, int* cpi_out) {
   WgradPlan pl;
-  pl.n_tile = s.C > 128 ? 256 : s.C > 64 ? 128 : s.C > 32 ? 64 : 32;
+  pl.n_tile = s.C > 64 ? 128 : s.C > 32 ? 64 : 32;  // 128 x 128 fp32 accumulators = 64 registers per consumer thread
   const int cpi = (s.Ho * s.Wo + BK - 1) / BK;
   const long long nkb = (long long)s.N * cpi;
   const long long mn = (long long)((s.O + 127) / 128) * ((s.C + pl.n_tile - 1) / pl.n_tile);
@@ -743,7 +694,6 @@ static int launch_conv_tc_wgrad_tma(const ConvShape& s, const float* x, const fl
   rc = wg_make_map(&mx, x, P, s.C, s.N, pl.n_tile);
   if (rc) return rc;
   switch (pl.n_tile) {
-    case 256: rc = launch_wgrad_tma_inst<256>(p, mdy, mx, st); break;
     case 128: rc = launch_wgrad_tma_inst<128>(p, mdy, mx, st); break;
     case 64: rc = launch_wgrad_tma_inst<64>(p, mdy, mx, st); break;
     default: rc = launch_wgrad_tma_inst<32>(p, mdy, mx, st); break;
@@ -754,10 +704,9 @@ static int launch_conv_tc_wgrad_tma(const ConvShape& s, const float* x, const fl
 
 // ---- strided 1x1 layers (pad 0, stride > 1): subsample, then the TMA path ------------------------------------------
 // On by default for layers with more than 128 output channels (B2C_WGRAD_COMPACT=0 switches it off, =2 forces it for every
-// eligible layer).  Measured on ResNet-50's strided projections at N = 64 (profiles/r02_c1_sweep_compact.txt): C256->O512@56
-// 183 -> 136 us, C512->O1024@28 196 -> 124 us, C512->O256@28 89 -> 72 us, but C256->O128@56 89 -> 97 us (the extra pass over X
-// costs more than the gather it replaces when the GEMM is that small).  dW[o][c] = sum_q dY[o][q] * X[c][ho*sh][wo*sw]: the gather kernel reads X with 8-byte-strided
-// 4-byte loads (36 TFLOP/s on ResNet-50's six such layers, 0.92 ms per step against 0.17 ms of MMA).  Copying the
+// eligible layer).  On ResNet-50's strided projections the wide layers gain, while for C256->O128@56 the extra pass over X
+// costs more than the gather it replaces (the GEMM is that small).  dW[o][c] = sum_q dY[o][q] * X[c][ho*sh][wo*sw]: the gather
+// kernel reads X with 8-byte-strided 4-byte loads, far slower than its MMAs.  Copying the
 // sampled pixels into a dense [N][C][Ho*Wo] buffer first is one HBM-bound pass over half of X's rows, after which the
 // layer is an ordinary 1x1 / stride 1 weight gradient for the TMA-fed kernel.
 static int wgrad_compact_mode() {
@@ -856,8 +805,6 @@ int launch_conv_tc_wgrad(const ConvShape& s, int math, const float* x, const flo
   if (pl.splits > 1) B2C_CUDA_OK(cudaMemsetAsync(ws, 0, WG_COUNTER_BYTES, st));
   int rc;
   switch (pl.n_tile) {
-    case 256: rc = launch_wgrad_n<256>(p, s.G, math, s.is_1x1, st); break;
-    case 128: rc = launch_wgrad_n<128>(p, s.G, math, s.is_1x1, st); break;
     case 64: rc = launch_wgrad_n<64>(p, s.G, math, s.is_1x1, st); break;
     default: rc = launch_wgrad_n<32>(p, s.G, math, s.is_1x1, st); break;
   }
@@ -865,8 +812,8 @@ int launch_conv_tc_wgrad(const ConvShape& s, int math, const float* x, const flo
   if (prof_on) {
     long long h[32];
     cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[wprof] N_TILE=%d splits=%d nkb=%lld | dY-prod: loop=%lld wait_empty=%lld store=%lld wait_tmem=%lld epilogue=%lld | X-prod: loop=%lld wait_empty=%lld store=%lld | mma: total=%lld wait_full=%lld issue=%lld\n",
-            pl.n_tile, pl.splits, h[5], h[0], h[1], h[2], h[3], h[4], h[8], h[9], h[10], h[16], h[17], h[18]);
+    fprintf(stderr, "[wprof] N_TILE=%d splits=%d nkb=%lld | dY-prod: loop=%lld wait_empty=%lld store=%lld | X-prod: loop=%lld wait_empty=%lld store=%lld\n",
+            pl.n_tile, pl.splits, h[5], h[0], h[1], h[2], h[8], h[9], h[10]);
   }
   return B2C_OK;
 }

@@ -1,4 +1,4 @@
-// conv_tc_wgrad_stg.cu -- tcgen05 weight gradient with TMA-STAGED operands and bf16x3 math (sm_100a), for the stride-1
+// conv_tc_wgrad_stg.cu -- wgmma weight gradient with TMA-STAGED operands and bf16x3 math (sm_90a), for the stride-1
 // "same" convolutions with 1 or 9 taps (1x1 / pad 0 and 3x3 / pad 1: 40 of ResNet-50's 53 layers, all of VGG-16's).
 //
 // Replaces cudnnConvolutionBackwardFilter beta=1 (reference src/caffe/layers/cudnn_conv_layer.cu:95-99) and, semantically,
@@ -6,17 +6,17 @@
 //     dW[o][c][tap] += sum_{n,p} dY[n][o][p] * X[n][c][p + off(tap)]        (X read as zero outside the image)
 // GEMM view: M = 128 output channels, N = CN input channels x T taps (columns ordered (c, tap) = dW's own memory order, so
 // a tile row is one contiguous run of dW), K = pixels.  The gather kernel (conv_tc_wgrad.cu) builds the X operand with
-// per-thread predicated 4-byte loads: ~2 900 cycles per 32-pixel K block against 1 536 of MMA (profiles/README.md), 50-110
-// TFLOP/s on the 3x3 layers.  Here, per K block of 64 pixels of one image:
+// per-thread predicated 4-byte loads.  Here, per K block of 64 pixels of one image:
 //   * TMA brings in dY as two [128 o][32 px] fp32 boxes (SWIZZLE_128B) and X as ONE [CN c][64 + 2*halo px] fp32 box; pixels
 //     past the image end and channels past O / C read as zero, which is the padding both the K tail and the M / N tails need;
-//   * 16 converter warps split dY into bf16 hi / lo and write it into TENSOR MEMORY as the A operand (tcgen05.st, lane =
-//     output channel; the swizzled 16-byte chunks make the row-wise ld.shared.v4 conflict-free), and build the B operand in
-//     shared memory: row (c, tap) of the K-major SWIZZLE_128B tile is the staged row of channel c shifted by the tap offset,
-//     masked where the tap leaves the image (zero padding / row wrap; one bit per pixel and tap, computed once per K block),
-//     split into bf16 hi / lo; lanes run along the pixels, so both the reads and the 4-byte writes are conflict-free;
-//   * one converged warp issues tcgen05.mma.kind::f16: lo*hi + hi*lo + hi*hi per 16-pixel K step, N = 256 (+ 32 for the 288
-//     columns of a 3x3 tile), accumulators in TMEM for the whole K range of the CTA;
+//   * 8 converter warps split dY into bf16 hi / lo and write it into shared memory as the A operand (K-major, no swizzle;
+//     the swizzled 16-byte chunks make the row-wise ld.shared.v4 conflict-free), and build the B operand in shared memory:
+//     row (c, tap) of the K-major SWIZZLE_128B tile is the staged row of channel c shifted by the tap offset, masked where
+//     the tap leaves the image (zero padding / row wrap; one bit per pixel and tap, computed once per K block), split into
+//     bf16 hi / lo; lanes run along the pixels, so both the reads and the 4-byte writes are conflict-free;
+//   * two consumer warpgroups issue wgmma.mma_async.m64nNk16.bf16: lo*hi + hi*lo + hi*hi per 16-pixel K step, N = 128 / 64
+//     (1x1) or 72 (8 channels x 9 taps), fp32 accumulators in registers for the whole K range of the CTA (pixels past the
+//     image end are zeros in both tiles, so every K block runs all four K steps);
 //   * the reduction over pixels is split across CTAs in one wave; partial tiles meet through the fused, deterministic
 //     split-K reduction of conv_tc_wgrad.cu (arrival counter + per-CTA slice, fixed split order).
 // Three bf16 MMAs per MAC cost 1.5 TF32 MMAs (3xTF32: 3); dropped terms ~2^-17 per product.
@@ -33,10 +33,11 @@ using namespace tc;
 
 namespace wstg {
 
-constexpr int NCW = 16;                       // converter warps (warps 0-3 also run the epilogue)
-constexpr int W_TMA = NCW;
-constexpr int W_MMA = NCW + 1;
-constexpr int THREADS = (NCW + 2) * 32;       // 576
+constexpr int NCONS = 8;                      // consumer warps: two warpgroups (wgmma + epilogue), rows [64 cw, 64 cw + 64)
+constexpr int NCW = 8;                        // converter warps
+constexpr int W_CONV0 = NCONS;
+constexpr int W_TMA = NCONS + NCW;
+constexpr int THREADS = (NCONS + NCW + 1) * 32;   // 544
 constexpr int KPX = 64;                       // pixels per K block
 constexpr uint32_t DY_BYTES = 2u * 128u * 128u;   // two [128 rows][32 px] fp32 boxes
 
@@ -55,52 +56,29 @@ struct Params {
 
 template <int T, int CN>
 struct Cfg {
-  static constexpr int NROWS = T * CN;                                  // B rows = GEMM N
-  static constexpr int N0 = NROWS > 256 ? 256 : NROWS;                  // first MMA
-  static constexpr int N1 = NROWS - N0;                                 // second MMA (0 or 32)
-  static constexpr uint32_t B_PLANE = (uint32_t)NROWS * 128u;           // [NROWS][64 bf16]
+  static constexpr int NROWS = T * CN;                                  // B rows = GEMM N (one wgmma)
+  static constexpr uint32_t B_PLANE = (uint32_t)NROWS * 128u;           // [NROWS][64 bf16], SW128
   static constexpr uint32_t B_STAGE = 2u * B_PLANE;                     // hi + lo
   static constexpr int BSTAGES = 2;
-  // raw operands as TMA delivers them.  dY and X have their own rings: the converters are done with a dY stage after the
-  // first fifth of a K block (it goes to tensor memory), so ONE dY stage reloads in the shadow of the B-tile build, while X
-  // is read until the end of the block and wants two.  3x3: X pool = 2 x [32 c][184 px] (W <= 56; wider maps, up to the
-  // 256-column TMA box, run with one X stage).
-  static constexpr int NDY = T == 1 ? 2 : 1;
+  static constexpr uint32_t A_BYTES = tile_bytes(128);                  // [128 rows][64 bf16], K-major no swizzle
+  // raw operands as TMA delivers them.  dY and X have their own rings: the converters are done with a dY stage early
+  // (it is converted into the A tile first), while X is read until the end of the block and wants two stages.
+  // 3x3: X pool = 2 x [CN c][184 px] (W <= 56; wider maps, up to the 256-column TMA box, run with one X stage).
+  static constexpr int NDY = 1;
   static constexpr uint32_t XMAX = (uint32_t)CN * (T == 1 ? 64u : 256u) * 4u;   // raw X box upper bound (1x1: no halo; else bwx <= 256)
   static constexpr uint32_t XPOOL = T == 1 ? 2u * XMAX : 2u * (uint32_t)CN * 184u * 4u;
   static_assert(XPOOL >= XMAX, "one X stage always fits");
-  static constexpr uint32_t B_OFF = 0;
-  static constexpr uint32_t DY_OFF = BSTAGES * B_STAGE;
-  static constexpr uint32_t X_OFF = DY_OFF + NDY * DY_BYTES;
+  static constexpr uint32_t B_OFF = 0;                                  // SW128 tiles: 1024-byte aligned
+  static constexpr uint32_t DY_OFF = BSTAGES * B_STAGE;                 // SW128 boxes: 1024-byte aligned
+  static constexpr uint32_t A_OFF = DY_OFF + NDY * DY_BYTES;
+  static constexpr uint32_t X_OFF = A_OFF + BSTAGES * 2u * A_BYTES;    // 128-byte aligned
   static constexpr uint32_t BAR_OFF = X_OFF + XPOOL;
   static constexpr uint32_t TOTAL = BAR_OFF + 256 + 1024;
-  static constexpr uint32_t D_COLS = NROWS;                             // fp32 accumulator columns
-  static constexpr uint32_t A_COL0 = ((NROWS + 31) / 32) * 32;
-  static_assert(A_COL0 + BSTAGES * 64 <= 512, "TMEM budget");
-  static_assert(NROWS % 16 == 0 && N0 % 16 == 0 && (N1 == 0 || N1 % 16 == 0), "UMMA N granularity");
+  static_assert(NROWS % 8 == 0 && NROWS <= 256, "wgmma N");
+  static_assert(X_OFF % 128u == 0, "TMA destinations are 128-byte aligned");
   static_assert(TOTAL <= 227u * 1024u, "shared memory budget");
 };
 
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -134,6 +112,9 @@ __device__ __forceinline__ float2 lds64(uint32_t addr) {
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
+__device__ __forceinline__ void sts128u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
 // fp32 pair (k even, k odd) -> packed bf16 hi word and packed bf16 lo word (element k in the low half)
 __device__ __forceinline__ void split_pack_bf16(float e, float o, uint32_t& hi, uint32_t& lo) {
   const __nv_bfloat162 h = __floats2bfloat162_rn(e, o);
@@ -142,10 +123,6 @@ __device__ __forceinline__ void split_pack_bf16(float e, float o, uint32_t& hi, 
   const __nv_bfloat162 l = __floats2bfloat162_rn(e - he, o - ho);
   hi = hb;
   lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__device__ __forceinline__ void tmem_st8u(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
 }
 
 // the deterministic split-K reduction shared with the other weight-gradient kernels (conv_tc_wgrad.cu has the twin)
@@ -194,18 +171,17 @@ template <int T, int CN, bool PLANE>
 __global__ void __launch_bounds__(THREADS, 1)
 wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x) {
   using S = Cfg<T, CN>;
+  using MMA = WgmmaBf16<S::NROWS>;
   constexpr int NROWS = S::NROWS, NDY = S::NDY, BST = S::BSTAGES;
+  constexpr uint32_t LBO_A = tile_lbo(128);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sptr = smem_raw + (sbase - smem_u32(smem_raw));
   const uint32_t bar_dy_full = sbase + S::BAR_OFF;         // 2: dY boxes landed
   const uint32_t bar_dy_empty = bar_dy_full + 16;          // 2: converters have read the dY stage
   const uint32_t bar_x_full = bar_dy_empty + 16;           // 2: X box landed
   const uint32_t bar_x_empty = bar_x_full + 16;            // 2: converters have read the X stage
-  const uint32_t bar_b_full = bar_x_empty + 16;            // BST: A in TMEM + B tile written
-  const uint32_t bar_b_empty = bar_b_full + 16;            // BST: MMAs of the stage completed
-  const uint32_t bar_done = bar_b_empty + 16;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sptr + S::BAR_OFF + 128);
+  const uint32_t bar_b_full = bar_x_empty + 16;            // BST: A and B tiles written
+  const uint32_t bar_b_empty = bar_b_full + 16;            // BST: the MMAs of the stage have completed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int split = blockIdx.x;
@@ -216,59 +192,56 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   if (kb_end > p.nkb_total) kb_end = p.nkb_total;
   const int nkb = (int)(kb_end - kb_begin);                // >= 1 by construction
   const uint32_t x_bytes = (uint32_t)CN * (uint32_t)p.bwx * 4u;      // plane mode: bwx = H*W (the channel pitch of the box)
+  const uint32_t x_stride = (x_bytes + 127u) & ~127u;      // TMA destinations are 128-byte aligned
   const uint32_t dy_bytes = PLANE ? 128u * (uint32_t)p.HW * 4u : DY_BYTES;
-  const int nx = 2u * x_bytes <= S::XPOOL ? 2 : 1;         // X stages
+  const int nx = 2u * x_stride <= S::XPOOL ? 2 : 1;        // X stages
 
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(bar_dy_full + 8 * s, 1); mbar_init(bar_dy_empty + 8 * s, NCW);
       mbar_init(bar_x_full + 8 * s, 1); mbar_init(bar_x_empty + 8 * s, NCW);
     }
-    for (int s = 0; s < BST; ++s) { mbar_init(bar_b_full + 8 * s, NCW); mbar_init(bar_b_empty + 8 * s, 1); }
-    mbar_init(bar_done, 1);
+    for (int s = 0; s < BST; ++s) { mbar_init(bar_b_full + 8 * s, NCW); mbar_init(bar_b_empty + 8 * s, NCONS); }
     fence_barrier_init();
   }
-  if (warp == W_MMA) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto b_hi = [&](int s) { return sbase + S::B_OFF + (uint32_t)s * S::B_STAGE; };
   auto b_lo = [&](int s) { return sbase + S::B_OFF + (uint32_t)s * S::B_STAGE + S::B_PLANE; };
+  auto a_hi = [&](int s) { return sbase + S::A_OFF + (uint32_t)s * 2u * S::A_BYTES; };
   auto raw_dy = [&](int r) { return sbase + S::DY_OFF + (uint32_t)r * DY_BYTES; };
-  auto raw_x = [&](int r) { return sbase + S::X_OFF + (uint32_t)r * x_bytes; };
-  auto a_col = [&](int s) { return S::A_COL0 + (uint32_t)s * 64u; };
+  auto raw_x = [&](int r) { return sbase + S::X_OFF + (uint32_t)r * x_stride; };
   // first pixel of the staged X row for K block j of an image: 16-byte aligned, never negative
   auto x_start = [&](int j) { return max((j * KPX - p.halo) & ~3, 0); };
 
-  if (warp < NCW) {
+  if (warp >= W_CONV0 && warp < W_CONV0 + NCW) {
     // ================= converters ===============================================================================
-    const int rq = warp & 3, cg = warp >> 2;               // dY: TMEM lane quarter / 16-pixel column group
+    const int cw = warp - W_CONV0;
+    const int rq = cw & 3, ch2 = cw >> 2;                  // dY: row quarter / 32-pixel half of the K block
     const int row = rq * 32 + lane;
-    const uint32_t a_lane = (uint32_t)(rq * 32) << 16;
+    const uint32_t a_row = (uint32_t)(row >> 3) * 128u + (uint32_t)(row & 7) * 16u;
     int n_img = (int)(kb_begin / p.bpi), j = (int)(kb_begin - (long long)n_img * p.bpi);
     const uint32_t lq = (uint32_t)lane >> 2, wr_off = (uint32_t)(lane & 3) * 4u;   // 16-byte chunk / byte inside it of this lane's pixel pair
     for (int i = 0; i < nkb; ++i) {
       const int rd = i % NDY, rx = i % nx, s = i % BST;
       mbar_wait(bar_dy_full + 8 * rd, (i / NDY) & 1);
-      // ---- (a) dY -> bf16 hi / lo -> tensor memory: this thread's row (output channel), pixels [cg*16, cg*16 + 16)
-      uint32_t hi[8], lo[8];
+      // ---- (a) dY -> bf16 hi / lo: this thread's row (output channel), pixels [ch2*32, ch2*32 + 32)
+      uint32_t hi[16], lo[16];
       if constexpr (PLANE) {
-        const uint32_t rowb = raw_dy(rd) + (uint32_t)row * (uint32_t)(p.HW * 4) + (uint32_t)(cg * 64);
+        const uint32_t rowb = raw_dy(rd) + (uint32_t)row * (uint32_t)(p.HW * 4) + (uint32_t)(ch2 * 128);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
+        for (int q = 0; q < 8; ++q) {
           float v[4];
 #pragma unroll
-          for (int e = 0; e < 4; ++e) v[e] = cg * 16 + q * 4 + e < p.HW ? lds32(rowb + (uint32_t)((q * 4 + e) * 4)) : 0.f;
+          for (int e = 0; e < 4; ++e) v[e] = ch2 * 32 + q * 4 + e < p.HW ? lds32(rowb + (uint32_t)((q * 4 + e) * 4)) : 0.f;
           split_pack_bf16(v[0], v[1], hi[2 * q], lo[2 * q]);
           split_pack_bf16(v[2], v[3], hi[2 * q + 1], lo[2 * q + 1]);
         }
       } else {
-        const uint32_t box = raw_dy(rd) + (uint32_t)(cg >> 1) * (128u * 128u) + (uint32_t)row * 128u;
+        const uint32_t box = raw_dy(rd) + (uint32_t)ch2 * (128u * 128u) + (uint32_t)row * 128u;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint32_t chunk = (uint32_t)((cg & 1) * 4 + q) ^ (uint32_t)(row & 7);
+        for (int q = 0; q < 8; ++q) {
+          const uint32_t chunk = (uint32_t)q ^ (uint32_t)(row & 7);
           const float4 v = lds128(box + chunk * 16u);
           split_pack_bf16(v.x, v.y, hi[2 * q], lo[2 * q]);
           split_pack_bf16(v.z, v.w, hi[2 * q + 1], lo[2 * q + 1]);
@@ -277,11 +250,11 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_dy_empty + 8 * rd);      // the dY stage reloads while the B tile is built
       mbar_wait_backoff(bar_b_empty + 8 * s, ((i / BST) & 1) ^ 1, 32);
-      tc_fence_after();
-      {
-        const uint32_t a0 = tmem_base + a_lane + a_col(s) + (uint32_t)(cg * 8);
-        tmem_st8u(a0, hi);
-        tmem_st8u(a0 + 32, lo);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {                            // 16-byte K chunk = 8 pixels
+        const uint32_t a = a_hi(s) + (uint32_t)(ch2 * 4 + q) * LBO_A + a_row;
+        sts128u(a, hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]);
+        sts128u(a + S::A_BYTES, lo[4 * q], lo[4 * q + 1], lo[4 * q + 2], lo[4 * q + 3]);
       }
       // ---- (b) X -> B tile rows (c, tap): lanes run along the pixels, two adjacent pixels per lane
       const int col0 = j * KPX - x_start(j) + 2 * lane;       // staged column of this lane's first pixel at tap offset 0
@@ -309,7 +282,7 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
         const int w4 = p.W * 4;
 #pragma unroll
         for (int c = 0; c < CPW; ++c) {
-          const int cl = warp * CPW + c;
+          const int cl = cw * CPW + c;
           const uint32_t srcc = raw_x(rx) + (uint32_t)((cl * p.bwx + col0) * 4);
           const uint32_t n0 = (uint32_t)cl * 9u;
 #pragma unroll
@@ -335,13 +308,13 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
         mbar_wait(bar_x_full + 8 * rx, (i / nx) & 1);
         constexpr int RPW = CN / NCW;                           // channels (= B rows) per warp
         // 1x1: no halo, the box starts at the K block's first pixel: the pair is 8-byte aligned
-        const uint32_t srcw = raw_x(rx) + (uint32_t)((warp * RPW * KPX + 2 * lane) * 4);
+        const uint32_t srcw = raw_x(rx) + (uint32_t)((cw * RPW * KPX + 2 * lane) * 4);
 #pragma unroll
         for (int k = 0; k < RPW; ++k) {
           float2 v;
           if constexpr (PLANE) {
             // channel pitch H*W*4 bytes (4-byte aligned only); pixels past the image are the next channel's: zeros instead
-            const uint32_t a = raw_x(rx) + (uint32_t)(((warp * RPW + k) * p.HW + 2 * lane) * 4);
+            const uint32_t a = raw_x(rx) + (uint32_t)(((cw * RPW + k) * p.HW + 2 * lane) * 4);
             v.x = 2 * lane < p.HW ? lds32(a) : 0.f;
             v.y = 2 * lane + 1 < p.HW ? lds32(a + 4u) : 0.f;
           } else {
@@ -349,7 +322,7 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
           }
           uint32_t hw, lw;
           split_pack_bf16(v.x, v.y, hw, lw);
-          const uint32_t n = (uint32_t)(warp * RPW + k);
+          const uint32_t n = (uint32_t)(cw * RPW + k);
           const uint32_t dst = bh + n * 128u + ((lq ^ (n & 7u)) << 4) + wr_off;
           sts32(dst, hw);
           sts32(dst + S::B_PLANE, lw);
@@ -358,42 +331,10 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       // X stage fully read by this warp: hand it back to the TMA warp
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_x_empty + 8 * rx);
-      fence_proxy_async();                                  // st.shared B tile -> visible to the MMA's async-proxy reads
-      tmem_st_wait();
-      tc_fence_before();
+      fence_proxy_async();                                  // st.shared A / B tiles -> visible to the MMA's async-proxy reads
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_b_full + 8 * s);
       if (++j == p.bpi) { j = 0; ++n_img; }
-    }
-    if (warp < 4) {
-      // ================= epilogue: TMEM -> registers -> smem transpose -> coalesced row stores of the partial tile ===
-      mbar_wait_backoff(bar_done, 0, 128);
-      tc_fence_after();
-      float* tpad = reinterpret_cast<float*>(sptr) + warp * (32 * 33);     // all MMAs done: the B stages are free
-      float* obase = p.out + (p.splits > 1 ? (long long)split * p.O * p.Kd : 0LL) + (long long)(m0 + warp * 32) * p.Kd + (long long)c0 * T;
-      const int rows_valid = p.O - (m0 + warp * 32);
-      const int cols_valid = min(NROWS, (p.C - c0) * T);
-      const bool accumulate = p.splits == 1;
-#pragma unroll 1
-      for (int q0 = 0; q0 < NROWS; q0 += 32) {
-        if (q0 >= cols_valid) break;
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)q0, v);
-#pragma unroll
-        for (int jj = 0; jj < 32; ++jj) tpad[lane * 33 + jj] = v[jj];
-        __syncwarp();
-        const bool colok = q0 + lane < cols_valid;
-#pragma unroll 4
-        for (int rr = 0; rr < 32; ++rr) {
-          if (rr < rows_valid && colok) {
-            float* dst = obase + (long long)rr * p.Kd + q0 + lane;
-            const float t = tpad[rr * 33 + lane];
-            *dst = accumulate ? *dst + t : t;
-          }
-        }
-        __syncwarp();
-      }
-      tc_fence_before();
     }
   } else if (warp == W_TMA) {
     // ================= TMA producer ================================================================================
@@ -420,37 +361,62 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       __syncwarp();
       if (++j == p.bpi) { j = 0; ++n_img; }
     }
-  } else {
-    // ================= MMA issuer ===================================================================================
-    constexpr uint32_t IDESC0 = idesc_bf16(128, S::N0);
-    constexpr uint32_t IDESC1 = idesc_bf16(128, S::N1 > 0 ? S::N1 : 16);
-    int j = (int)(kb_begin % p.bpi);
+  } else if (warp < NCONS) {
+    // ================= consumers: wgmma over the CTA's K range, then the partial tile from registers ==============
+    // For T = 9 the wgmma accumulator is added into `tot` on the CUDA cores every PROMOTE K blocks (512 pixels) and restarted.
+    // Accumulating a whole split in the wgmma accumulator measured 7.5e-4 against the 3e-4 dW bar of
+    // test_full_size_vs_reference_loop on an H100 for VGG-16 conv1_2 (N = 32, ~10^5 pixels per CTA); with the promotion it passes.
+    // (The 1x1 tiles are wider -- no registers for a second copy -- and have enough tiles to keep their chains short.)
+    constexpr int PROMOTE = T == 9 ? 8 : 1 << 30;
+    constexpr int NT = T == 9 ? NROWS / 2 : 1;
+    const int cwg = warp >> 2, t = tid & 127;
+    float acc[NROWS / 2], tot[NT];
+#pragma unroll
+    for (int q = 0; q < NROWS / 2; ++q) acc[q] = 0.f;
+#pragma unroll
+    for (int q = 0; q < NT; ++q) tot[q] = 0.f;
+    int prev = -1;
     for (int i = 0; i < nkb; ++i) {
       const int s = i % BST;
+      const int fresh = i % PROMOTE == 0;
       mbar_wait(bar_b_full + 8 * s, (i / BST) & 1);
-      tc_fence_after();
-      const int valid = min(KPX, p.HW - j * KPX);
-      const int ks = (valid + 15) >> 4;                      // K steps with any in-image pixel (the rest is all zero)
-      if (elect_one()) {
-        for (int kk = 0; kk < ks; ++kk) {
-          const uint32_t ah = tmem_base + a_col(s) + (uint32_t)(kk * 8);
-          const uint64_t bh = desc_sw128(b_hi(s) + kk * 32), bl = desc_sw128(b_lo(s) + kk * 32);
-          const uint32_t acc = (i | kk) != 0;
-          umma_bf16_ts(tmem_base, ah + 32, bh, IDESC0, acc);      // lo * hi
-          umma_bf16_ts(tmem_base, ah, bl, IDESC0, 1);              // hi * lo
-          umma_bf16_ts(tmem_base, ah, bh, IDESC0, 1);              // hi * hi
-          if (S::N1 > 0) {
-            const uint64_t bh1 = desc_sw128(b_hi(s) + 256u * 128u + kk * 32), bl1 = desc_sw128(b_lo(s) + 256u * 128u + kk * 32);
-            umma_bf16_ts(tmem_base + 256, ah + 32, bh1, IDESC1, acc);
-            umma_bf16_ts(tmem_base + 256, ah, bl1, IDESC1, 1);
-            umma_bf16_ts(tmem_base + 256, ah, bh1, IDESC1, 1);
-          }
-        }
-        umma_commit(bar_b_empty + 8 * s);
-        if (i == nkb - 1) umma_commit(bar_done);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < KPX / 16; ++kk) {
+        const uint32_t a = a_hi(s) + 2u * kk * LBO_A + (uint32_t)cwg * 1024u;
+        const uint64_t ah = smem_desc(a, LBO_A, 128), al = smem_desc(a + S::A_BYTES, LBO_A, 128);
+        const uint64_t bh = smem_desc_sw128(b_hi(s) + kk * 32), bl = smem_desc_sw128(b_lo(s) + kk * 32);
+        MMA::mma(acc, al, bh, !fresh || kk != 0);  // lo * hi
+        MMA::mma(acc, ah, bl, 1);                 // hi * lo
+        MMA::mma(acc, ah, bh, 1);                 // hi * hi
       }
-      __syncwarp();
-      if (++j == p.bpi) j = 0;
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_b_empty + 8 * prev); }
+      prev = s;
+      if constexpr (T == 9) {
+        if (i % PROMOTE == PROMOTE - 1 || i == nkb - 1) {
+          wgmma_wait<0>();
+          wgmma_reg_fence(acc);
+#pragma unroll
+          for (int q = 0; q < NT; ++q) tot[q] += acc[q];
+        }
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence(acc);
+    // row = output channel, column = (c, tap) = dW's own order; lanes of a quad write 8 consecutive columns of a row
+    float* obase = p.out + (p.splits > 1 ? (long long)split * p.O * p.Kd : 0LL) + (long long)c0 * T;
+    const int cols_valid = min(NROWS, (p.C - c0) * T);
+    const bool accumulate = p.splits == 1;
+#pragma unroll
+    for (int q = 0; q < NROWS / 2; ++q) {
+      const int r = m0 + cwg * 64 + frag_row(t, q), c = frag_col(t, q);
+      if (r < p.O && c < cols_valid) {
+        float* dst = obase + (long long)r * p.Kd + c;
+        const float v = T == 9 ? tot[q < NT ? q : 0] : acc[q];
+        *dst = accumulate ? *dst + v : v;
+      }
     }
   }
   if (p.splits > 1) {
@@ -458,14 +424,10 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
     splitk_fused_reduce(p.out, p.grad, p.counters + tile_id, split, p.splits, (long long)p.O * p.Kd, (long long)m0 * p.Kd + (long long)c0 * T, p.Kd,
                         min(128, p.O - m0), min(NROWS, (p.C - c0) * T));
   }
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 }  // namespace wstg
+
 
 // ---- host side ------------------------------------------------------------------------------------------------------
 typedef CUresult (*WsEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -525,7 +487,7 @@ static bool wstg_plan(const ConvShape& s, WstgPlan* pl) {
   if (!pl) return true;
   pl->T = T;
   pl->plane = plane;
-  pl->cn = k1 ? (s.C > 64 ? 128 : 64) : 32;
+  pl->cn = k1 ? (s.C > 64 ? 128 : 64) : 8;           // N = 128 / 64 / 72 columns: <= 64 accumulator registers per consumer thread
   pl->bwx = plane ? (int)HW : (need + 3) & ~3;
   pl->bpi = (int)((HW + wstg::KPX - 1) / wstg::KPX);
   pl->nkb = (long long)s.N * pl->bpi;
@@ -595,7 +557,7 @@ int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const fl
   (void)math;
   if (!tc_gemm_supported(tA, tB, M, N, K) || alpha != 1.0f || (beta != 0.0f && beta != 1.0f) ||
       ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 15u))
-    return fail(B2C_ERR_INVALID, "tcgen05 GEMM: only C (+)= A * B^T with alpha = 1, beta in {0, 1}, K %% 4 == 0 and 16-byte aligned operands");
+    return fail(B2C_ERR_INVALID, "tensor-core GEMM: only C (+)= A * B^T with alpha = 1, beta in {0, 1}, K %% 4 == 0 and 16-byte aligned operands");
   if (beta == 0.0f) B2C_CUDA_OK(cudaMemsetAsync(Cm, 0, sizeof(float) * (size_t)M * N, st));
   ConvShape s{};
   s.N = 1; s.C = N; s.H = 1; s.W = K; s.O = M; s.G = 1; s.kh = s.kw = 1; s.sh = s.sw = 1; s.ph = s.pw = 0; s.dh = s.dw = 1; s.has_bias = 0;
@@ -625,13 +587,13 @@ static int launch_wstg_planned(const ConvShape& s, const WstgPlan& pl, const flo
     // {4*HW, channels/4, N}: four channels per tensor row (a 16-byte-multiple pitch); box rows = tile channels / 4
     if (int rc = ws_make_map(&mdy, dy, p.HW * 4, s.O / 4, s.N, p.HW * 4, 32, false)) return rc;
     if (int rc = ws_make_map(&mx, x, p.HW * 4, s.C / 4, s.N, p.HW * 4, pl.cn / 4, false)) return rc;
-    if (pl.T == 9) return wstg_launch<9, 32, true>(p, mdy, mx, c_tiles, o_tiles, st);
+    if (pl.T == 9) return wstg_launch<9, 8, true>(p, mdy, mx, c_tiles, o_tiles, st);
     if (pl.cn == 128) return wstg_launch<1, 128, true>(p, mdy, mx, c_tiles, o_tiles, st);
     return wstg_launch<1, 64, true>(p, mdy, mx, c_tiles, o_tiles, st);
   }
   if (int rc = ws_make_map(&mdy, dy, p.HW, s.O, s.N, 32, 128, true)) return rc;
   if (int rc = ws_make_map(&mx, x, p.HW, s.C, s.N, pl.bwx, pl.cn, false)) return rc;
-  if (pl.T == 9) return wstg_launch<9, 32, false>(p, mdy, mx, c_tiles, o_tiles, st);
+  if (pl.T == 9) return wstg_launch<9, 8, false>(p, mdy, mx, c_tiles, o_tiles, st);
   if (pl.cn == 128) return wstg_launch<1, 128, false>(p, mdy, mx, c_tiles, o_tiles, st);
   return wstg_launch<1, 64, false>(p, mdy, mx, c_tiles, o_tiles, st);
 }

@@ -1,4 +1,4 @@
-// filter_prep.cuh -- the filter operand of the tcgen05 forward / dgrad kernels in its GEMM layout, as ONE multi-tensor launch.
+// filter_prep.cuh -- the filter operand of the tensor-core forward / dgrad kernels in its GEMM layout, as ONE multi-tensor launch.
 //
 // Both kernels read the filter through TMA as a [rows][Kp] matrix in GEMM-K order, pre-split into hi / lo parts:
 //   kind GATHER (conv_tc.cu)     fp32 TF32-hi / lo planes [G][rows][Kp], K = (c,i,j) natural or (c/4, tap, c%4) "tap major"

@@ -1,4 +1,4 @@
-// im2col.cu -- im2col / col2im (2-D and N-D) for sm_100a.
+// im2col.cu -- im2col / col2im (2-D and N-D) for sm_90a.
 //
 // Replaces im2col_gpu / col2im_gpu / im2col_nd_gpu / col2im_nd_gpu
 // (reference src/caffe/util/im2col.cu:42-62,298-317,165-253,443-530).  These are pure

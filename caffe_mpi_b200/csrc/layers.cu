@@ -309,9 +309,8 @@ pool_max_fwd_q_kernel(long long groups, int H, int W, int Ho, int Wo, int ph, in
     }
   }
 }
-// One block per input row (plane nc, row h): the row's window range in h is computed once, threads walk w.  (The first version
-// decoded a flat 64-bit element index with three runtime divisions per element and ran at 380 GB/s -- 0.67 ms per ResNet-50 step for
-// its one 3x3 / stride 2 pool, profiles/r02_c6_fullnet_launches.csv.)  Same ascending (a, b) summation order as before.
+// One block per input row (plane nc, row h): the row's window range in h is computed once, threads walk w, instead of decoding a
+// flat 64-bit element index with three runtime divisions per element.  Ascending (a, b) summation order.
 __global__ void __launch_bounds__(128)
 pool_max_bwd_kernel(int rows, int H, int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw,
                     const float* __restrict__ dy, const int* __restrict__ mask, float* __restrict__ dx) {

@@ -1,5 +1,5 @@
 // layers_fused.cu -- fused forms of the BatchNorm / ReLU / Eltwise chain of a residual block (HBM-bound passes; fusion is the
-// only lever left once each pass runs at 60-95% of the HBM roofline, profiles/r01_fullnet_launches.csv):
+// only lever left once each pass runs close to the HBM roofline):
 //
 //   b2c_bn_forward_train_fused : batch statistics + y = [max(0, .)] (gamma * x_norm + beta).  x_norm is NOT written: the
 //                                backward pass recomputes it from the layer's input x and the saved mean / inverse std
@@ -11,8 +11,8 @@
 //     Both are ONE launch: a thread-block cluster per channel reduces its slice of the channel (phase 1), the partial sums
 //     meet in rank 0 through distributed shared memory, the result is broadcast back the same way, and every CTA walks ITS
 //     OWN slice again for the elementwise pass (phase 2).  The slice is ~100 KB per CTA and at most two CTAs run per SM
-//     (bounded by a dynamic-shared-memory pad), so the 30-90 MB in flight sit in the 126 MB L2 and the second walk does not
-//     go to HBM: 8 B/element forward (read x, write y) and 12 B/element backward (read dy, x, write dx) instead of 12 / 20
+//     (bounded by a dynamic-shared-memory pad), so what is in flight (~26 MB on 132 SMs) sits in the 50 MB L2 and the second
+//     walk does not go to HBM: 8 B/element forward (read x, write y) and 12 B/element backward (read dy, x, write dx) instead of 12 / 20
 //     for the two-launch form (B2C_BN_ONEPASS=0), 12 / 32 for the unfused layers.
 //   b2c_add_relu               : y = max(0, a + b)                      (Eltwise SUM + in-place ReLU, one pass instead of two)
 //   b2c_relu_backward2         : dx_a = dx_b = dy * (y > 0)             (ReLU backward + Eltwise SUM backward's two copies)

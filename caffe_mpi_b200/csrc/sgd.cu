@@ -1,4 +1,4 @@
-// sgd.cu -- fused SGD-momentum update (regularise + history + apply + clear), sm_100a.
+// sgd.cu -- fused SGD-momentum update (regularise + history + apply + clear), sm_90a.
 //
 // Replaces SGDRegUpdateAllAndClear<float,float> and its launcher (reference
 // src/caffe/solvers/sgd_solver.cu:9-20,57-72): there it is one unvectorised launch plus a

@@ -2,7 +2,7 @@
 //
 // Replaces caffe_gpu_gemm<float> / caffe_gpu_gemv<float> (reference
 // src/caffe/util/math_functions.cu:11-26,73-82 -> cublasSgemm / cublasSgemv).  This is the
-// exact-fp32 (FFMA) kernel family: it serves b2c_sgemm for shapes the tcgen05 GEMM does not
+// exact-fp32 (FFMA) kernel family: it serves b2c_sgemm for shapes the tensor-core GEMM does not
 // take (tiny / unaligned problems such as the rank-1 bias GEMM and the integer known-answer
 // vectors of test_util_blas.cpp) and is the on-device second opinion for the tensor-core
 // kernels.  64x64 output tile, BK=16, 256 threads x (4x4) micro-tile, smem double buffered.

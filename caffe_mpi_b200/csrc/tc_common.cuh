@@ -1,5 +1,5 @@
-// tc_common.cuh -- Blackwell (sm_100a) building blocks for the tcgen05 kernels: mbarrier, proxy fences,
-// TMEM allocation, UMMA shared-memory / instruction descriptors, tcgen05.mma / commit / ld wrappers,
+// tc_common.cuh -- Hopper (sm_90a) building blocks for the tensor-core kernels: mbarrier, proxy fences,
+// wgmma shared-memory matrix descriptors, wgmma fence / commit / wait and the accumulator fragment map,
 // and the TF32 hi/lo split used by the fp32-equivalent (3xTF32) math mode.
 //
 // Shared-memory operand layout used by every kernel here: K-major, no swizzle ("interleave"),
@@ -11,6 +11,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "wgmma_ops.cuh"
 
 namespace b2c {
 namespace tc {
@@ -103,13 +104,12 @@ __device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity,
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// generic-proxy st.shared -> visible to the async proxy (tcgen05.mma operand reads)
+// generic-proxy st.shared -> visible to the async proxy (wgmma operand reads, TMA stores)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// One lane of a CONVERGED warp.  tcgen05.mma / tcgen05.commit / TMA are uniform-datapath instructions: issued
-// under `if (lane == 0)` the compiler wraps every one of them in an ELECT/branch loop over the active lanes
-// (~80 cycles per MMA measured: the single issuing thread, not the tensor pipe, bounded the kernel).  With
-// elect.sync on a converged warp they become straight-line uniform instructions.
+// One lane of a CONVERGED warp.  TMA issue is a uniform-datapath instruction: issued under `if (lane == 0)` the
+// compiler wraps it in an ELECT/branch loop over the active lanes; with elect.sync on a converged warp it is
+// straight-line code.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -121,91 +121,37 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// ---- tcgen05 ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// whole warp; writes the TMEM base address to *smem_dst
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// 64-bit shared-memory matrix descriptor, K-major, SWIZZLE_NONE, Blackwell version field = 1.
+// ---- wgmma ------------------------------------------------------------------------------------------
+// 64-bit shared-memory matrix descriptor (sm_90a layout): start address, LBO (K-direction core-matrix stride for
+// K-major SWIZZLE_NONE; ignored for swizzled K-major), SBO (stride between 8-row groups), layout type in bits 62-63.
 __device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-
-// 32-bit instruction descriptor: D=F32, A=B=TF32, both K-major, M x N.
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// K-major SWIZZLE_128B tile (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): 128-byte rows, 8-row groups 1024 B apart,
+// tile base 1024-byte aligned; a K step inside the 128-byte row advances the start address.
+__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t addr) {
+  return smem_desc(addr, 16u, 1024u) | ((uint64_t)1 << 62);
 }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, 128 x N x 8 (tf32).  One thread issues.
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread t gets lane base+t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// registers -> TMEM: this warp's 32 lanes x 16 consecutive 32-bit columns (thread t writes lane base+t)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-// registers -> TMEM, 8 columns
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float (&v)[8]) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[tmem] * B[smem]^T: A operand read from tensor memory (rows = lanes, K along columns)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
+// Accumulator fragment of m64nN (fp32): element i of thread t of the warpgroup is row frag_row(t, i) (0..63), column
+// frag_col(t, i) (0..N-1).
+__device__ __forceinline__ int frag_row(int t, int i) { return ((t >> 5) << 4) + ((t & 31) >> 2) + ((i & 2) ? 8 : 0); }
+__device__ __forceinline__ int frag_col(int t, int i) { return ((i >> 2) << 3) + ((t & 3) << 1) + (i & 1); }
+// named barrier over `n` threads (the consumer warpgroups of a kernel)
+__device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // ---- TF32 split ------------------------------------------------------------------------------------
 // fp32-equivalent mode: hi = a with the 13 low mantissa bits cleared (exactly a TF32 value), lo = a - hi

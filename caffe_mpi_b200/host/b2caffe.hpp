@@ -1,4 +1,4 @@
-// b2caffe.hpp -- C++ host layer of the B200-native Caffe-MPI hot path.
+// b2caffe.hpp -- C++ host layer of the H100-native Caffe-MPI hot path.
 //
 // Mirrors, for this path only, the reference's operator / plugin surface so that code written against
 // caffe::Blob / caffe::Layer / caffe::LayerRegistry / caffe::SGDSolver / caffe::P2PSync reads the same:

@@ -7,7 +7,7 @@
 // src/caffe/data_transformer.{cpp,cu} (crop / mirror / mean_file | mean_value / scale; "Cannot specify mean_file and mean_value at
 // the same time").
 //
-// B200-first shape of the same pipeline:
+// GPU-first shape of the same pipeline:
 //   parser threads (DataReader)  --memcpy from the file mapping-->  pinned slot k  --cudaMemcpyAsync, copy stream-->  device slot k
 //   --b2c_transform_u8 on the compute stream, first thing of the step-->  top[0];   labels ride along and are copied into top[1].
 // K = max(2, parser_threads + 1) slots circulate: while step i computes, batch i+1 is crossing PCIe and batches i+2.. are being
@@ -61,7 +61,7 @@ class DataLayer : public LayerBase {
   bool host_crop_ = false;
   // DataParameter.parser_threads; 0 ("Caffe optimizes it automatically", caffe.proto:841-844; the reference's auto mode ends between 1
   // and 4, data_layer.cpp:85-95) becomes 1 for raw datums -- one thread's memcpy outruns the GPU -- and 6 for encoded ones: at
-  // ~0.8 k decoded 256x256 JPEGs per second and thread that is what a B200 training ResNet-50 at ~4 k img/s asks for
+  // ~0.8 k decoded 256x256 JPEGs per second and thread that is what a GPU training ResNet-50 at a few thousand img/s asks for
   int parsers_ = 1;
   NetLayer L_;
   uint64_t seed_;

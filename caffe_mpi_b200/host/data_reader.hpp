@@ -12,7 +12,7 @@
 //   * wrap-around by cursor stepping: Next(), and SeekToFirst() when the cursor runs off the end (data_reader.cpp:246-258,
 //     300-305), i.e. positions are record ids modulo the number of entries;
 //   * Datum::record_id numbering (data_reader.cpp:239).
-// B200-first differences: the unit handed between threads is a BATCH, not a Datum -- a parser thread owns the B records of its
+// GPU-first differences: the unit handed between threads is a BATCH, not a Datum -- a parser thread owns the B records of its
 // batch anyway -- and it is assembled in place in a buffer the consumer provides (the data layer passes pinned host memory), the
 // datum's pixel bytes being copied once, from the file mapping.  The reference moves every datum three times (LMDB value ->
 // Datum string -> batch blob -> device).  DataParameter.cache / shuffle are accepted and ignored with a note: the mapping is the

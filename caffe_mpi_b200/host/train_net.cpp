@@ -161,9 +161,9 @@ void InnerProductLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) 
   // backward: dW = dy^T[N x M] * (x^T[K x M])^T (reduction over the batch), dx = dy[M x N] * (W^T[K x N])^T (reduction over the outputs)
   const char* e = getenv("B2C_IP_BWD_TC");
   const bool on = !e || atoi(e) != 0;
-  // dW: the reduction runs over the batch -- only a few K blocks per 128 x 128 output tile unless the batch is large; measured on
-  // AlexNet (batch 256, 4096 x 9216 outputs) the tile set-up and the read-modify-write epilogue cost more than the FFMA kernel
-  // (InnerProduct backward 2.95 -> 3.11 ms, profiles/r02_c12_bench_alexnet.json), so the batch has to be at least 512
+  // dW: the reduction runs over the batch -- only a few K blocks per 128 x 128 output tile unless the batch is large; on AlexNet
+  // (batch 256, 4096 x 9216 outputs) the tile set-up and the read-modify-write epilogue cost more than the FFMA kernel saves,
+  // so the batch has to be at least 512
   bwd_w_tc_ = on && M_ >= 512 && b2c_sgemm_tc_supported(0, 1, num_output_, K_, M_) != 0;
   bwd_x_tc_ = on && b2c_sgemm_tc_supported(0, 1, M_, K_, num_output_) != 0;
   size_t bws = 0;

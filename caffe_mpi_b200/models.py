@@ -1,6 +1,6 @@
-"""Prototxt text generators for the BASELINE nets (the reference's models/*.prototxt are not available on the GPU box,
-so bench.py builds the same architectures from here; tests/test_prototxt.py checks that the generated net has exactly
-the inventory of the reference file when the reference tree is mounted).  Layer and blob names follow
+"""Prototxt text generators for the BASELINE nets (bench.py builds the architectures of the reference's models/*.prototxt
+from here; tests/test_prototxt.py checks that the generated net has exactly the inventory of the reference file, stored
+under tests/golden/reference_models).  Layer and blob names follow
 models/resnet50/train_val.prototxt (res<stage>.<block>.conv<k>, .../bn, .skipConv, .sum, .relu, pool1/pool2, fc, loss)."""
 
 

@@ -1,5 +1,5 @@
 /*
- * b2c.h -- C ABI of the B200-native Caffe-MPI data-parallel hot path
+ * b2c.h -- C ABI of the H100-native Caffe-MPI data-parallel hot path
  *          (ConvolutionLayer forward/backward, im2col/col2im, SGEMM/SGEMV, fused
  *          SGD-momentum update, NCCL gradient exchange).
  *
@@ -44,14 +44,15 @@ typedef enum { B2C_ENGINE_DEFAULT = 0, B2C_ENGINE_CAFFE = 1, B2C_ENGINE_CUDNN = 
 
 /* Math mode of the tensor-core kernels (NetParameter default_forward_math /
  * default_backward_math, caffe.proto:124-127, is the reference's analogous knob).
- * FP32        : split-precision tcgen05 MMA, fp32-equivalent results (default): bf16 hi/lo split, three
- *               kind::f16 MMAs per K step, on the layers the bulk-copy-staged kernel takes (stride-1 "same"
+ * FP32        : split-precision wgmma, fp32-equivalent results (default): bf16 hi/lo split, three
+ *               bf16 MMAs per K step, on the layers the bulk-copy-staged kernel takes (stride-1 "same"
  *               convolutions, forward and dgrad); 3xTF32 split everywhere else.  Blob error ~1e-6..1e-5.
  * TF32        : single-pass TF32 (round-to-nearest operands), ~1e-3 relative.
  * FP32_3XTF32 : the 3xTF32 split on every layer (the round-1 default; ~1e-7..4e-5).          */
 typedef enum { B2C_MATH_FP32 = 0, B2C_MATH_TF32 = 1, B2C_MATH_FP32_3XTF32 = 2 } b2c_math;
 
-/* Kernel family used by the implicit-GEMM engine (diagnostics / tests). */
+/* Kernel family used by the implicit-GEMM engine (diagnostics / tests); B2C_ALGO_TCGEN05 names the tensor-core
+ * kernels (wgmma on sm_90a). */
 typedef enum { B2C_ALGO_AUTO = 0, B2C_ALGO_SIMT = 1, B2C_ALGO_TCGEN05 = 2 } b2c_algo;
 
 typedef enum { B2C_OP_FORWARD = 0, B2C_OP_BACKWARD_DATA = 1, B2C_OP_BACKWARD_FILTER = 2 } b2c_conv_op;
@@ -92,10 +93,10 @@ int b2c_conv_out_shape(const b2c_conv_desc* d, int* Ho, int* Wo);
 /* scratch bytes the given op needs (col buffer for CAFFE engine: base_conv_layer.cpp:225-233;
  * split-K partials / transformed weights for the implicit engine).                   */
 size_t b2c_conv_workspace_bytes(const b2c_conv_desc* d, int op);
-/* which kernel family the op will run (b2c_algo) -- lets tests assert "tcgen05 ran". */
+/* which kernel family the op will run (b2c_algo) -- lets tests assert "the tensor cores ran". */
 int b2c_conv_algo_used(const b2c_conv_desc* d, int op);
 
-/* Prepared filters.  The tcgen05 forward / dgrad kernels read the filter through TMA in a GEMM-ordered, hi/lo-split copy
+/* Prepared filters.  The tensor-core forward / dgrad kernels read the filter through TMA in a GEMM-ordered, hi/lo-split copy
  * that b2c_conv_forward / b2c_conv_backward_data otherwise rebuild on every call.  Weights change once per iteration
  * (SGDSolver::ApplyUpdate, sgd_solver.cpp:143-149), so a caller that owns the iteration can build the copies ONCE:
  *   bytes = b2c_conv_filter_cache_bytes(d);            cudaMalloc(&cache, bytes)  (256-byte aligned; 0 = nothing to cache)

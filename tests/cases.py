@@ -91,6 +91,13 @@ def tensors(rng, prm, scale_w=None):
     return x, w, b, dy
 
 
+def sample_index(name, k, size, samples=2048):
+    """The fixed sample of blob `k` of full-size case `name` that golden/full_size_ref_golden.npz stores."""
+    import numpy as np
+    seed = sum(ord(ch) for ch in name + "/" + k)
+    return np.sort(np.random.default_rng(seed).choice(size, min(samples, size), replace=False))
+
+
 def rel_err(a, ref):
     """max|a-ref| / max|ref| -- the blob-level relative error the 1e-3 bar is stated in (DESIGN.md)."""
     import numpy as np

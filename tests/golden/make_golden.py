@@ -1,9 +1,15 @@
-"""Generate tests/golden/conv_ref_golden.npz from oracle/_ref, i.e. from the reference's own
-src/caffe/util/im2col.cpp compiled verbatim, driven through the per-image / per-group
-ConvolutionLayer CPU loop with OpenBLAS cblas_sgemm/sgemv (the reference's BLAS := open).
+"""Generate the convolution fixtures from oracle/_ref, i.e. from the reference's own src/caffe/util/im2col.cpp compiled
+verbatim, driven through the per-image / per-group ConvolutionLayer CPU loop with OpenBLAS cblas_sgemm/sgemv (the
+reference's BLAS := open):
 
-Run in the build container (needs /root/reference):   python tests/golden/make_golden.py
-The fixture travels to the GPU box; /root/reference does not."""
+  conv_ref_golden.npz        small cases, every blob in full
+  im2col_ref_sha256.json     SHA-256 of the reference's im2col / col2im (2-D and N-D) outputs on test_oracle.py's
+                             IM2COL_SHAPES, inputs from the test's own seed (the test asserts bit-exact equality)
+  full_size_ref_golden.npz   the FULL_SIZE_CASES of tests/cases.py (the benchmark's layer shapes and batch sizes): inputs
+                             from the test's own seed, outputs stored as a fixed sample of elements per blob (cases.sample_index) (with
+                             max|blob|, the denominator of rel_err), bias gradients in full
+
+Needs oracle/_ref, which build() makes only where the reference tree is present:   python tests/golden/make_golden.py"""
 import os
 import sys
 
@@ -13,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import oracle as o  # noqa: E402
-from cases import make  # noqa: E402
+from cases import FULL_SIZE_CASES, make, sample_index  # noqa: E402
 
 CASES = [
     ("simple", dict(N=2, Cin=3, H=6, W=4, O=4, k=3, s=2, p=0, d=1, G=1, bias=True)),
@@ -59,5 +65,66 @@ def main():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def full_size():
+    assert o.ref() is not None and o.ref_blas_open(os.cpu_count() or 1), "oracle/_ref or OpenBLAS unavailable"
+    out = {}
+    for name, c in FULL_SIZE_CASES:
+        rng = np.random.default_rng(1701)              # the tests' rng fixture; the draws below are test_full_size_vs_reference_loop's
+        po = make(o, c)
+        x = rng.standard_normal(po.x_shape(), dtype=np.float32)
+        w = rng.standard_normal(po.w_shape(), dtype=np.float32) * np.float32((2.0 / po.Kd) ** 0.5)
+        b = (rng.standard_normal(po.O, dtype=np.float32) * np.float32(0.1)) if po.has_bias else None
+        dy = rng.standard_normal(po.y_shape(), dtype=np.float32)
+        dw0 = rng.standard_normal(po.w_shape(), dtype=np.float32) * np.float32(0.1)
+        y = np.empty(po.y_shape(), np.float32)
+        dw = dw0.copy()
+        db = np.zeros(po.O, np.float32) if po.has_bias else None
+        dx = np.empty(po.x_shape(), np.float32)
+        assert o.ref_conv_fwd_bwd(po, x, w, b, y=y, dy=dy, dw=dw, db=db, dx=dx) == 0
+        for k, v in (("y", y), ("dx", dx), ("dw", dw)):
+            v = v.reshape(-1)
+            out[f"{name}/{k}"] = v[sample_index(name, k, v.size)]
+            out[f"{name}/{k}_absmax"] = np.array(np.abs(v).max(), np.float32)
+        if db is not None:
+            out[name + "/db"] = db
+        print(name, flush=True)
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "full_size_ref_golden.npz")
+    np.savez_compressed(path, **out)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
+def im2col_digests():
+    import hashlib
+    import json
+    from test_oracle import IM2COL_SHAPES
+    R = o.ref()
+    assert R is not None, "oracle/_ref unavailable"
+    sha = lambda a: hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+    out = {}
+    for shape in IM2COL_SHAPES:
+        Cc, H, W, k, st, p, d = shape
+        rng = np.random.default_rng(1701)          # the tests' rng fixture; the draws below are the test's
+        im = rng.standard_normal((Cc, H, W)).astype(np.float32)
+        col = np.empty_like(o.im2col(im, k, st, p, d))
+        R.ref_im2col_cpu(im, Cc, H, W, k[0], k[1], p[0], p[1], st[0], st[1], d[0], d[1], col)
+        colr = rng.standard_normal(col.shape).astype(np.float32)
+        back = np.empty((Cc, H, W), np.float32)
+        R.ref_col2im_cpu(colr, Cc, H, W, k[0], k[1], p[0], p[1], st[0], st[1], d[0], d[1], back)
+        ims, cols = np.asarray(im.shape, np.int32), np.asarray(col.shape, np.int32)
+        nd = [np.asarray(v, np.int32) for v in (k, p, st, d)]
+        coln = np.empty_like(col)
+        R.ref_im2col_nd_cpu(im, 2, ims, cols, *nd, coln)
+        backn = np.empty_like(back)
+        R.ref_col2im_nd_cpu(colr, 2, ims, cols, *nd, backn)
+        out[str(shape)] = {"col": sha(col), "back": sha(back), "col_nd": sha(coln), "back_nd": sha(backn)}
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "im2col_ref_sha256.json")
+    with open(path, "w") as f:
+        json.dump(out, f, indent=1)
+        f.write("\n")
+    print("wrote", path)
+
+
 if __name__ == "__main__":
     main()
+    im2col_digests()
+    full_size()

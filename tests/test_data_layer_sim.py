@@ -7,7 +7,7 @@ parser threads' pinned buffers, the host -> device copies and the transform show
 
 What this does NOT cover: the transform kernel itself (a host closure stands in for it here; the real one is checked bit-exactly
 on hardware by tests/test_layers_extra_gpu.py) and real PCIe / driver behaviour -- tests/test_zz_data_layer_gpu.py is the same
-comparison on a B200."""
+comparison on an H100."""
 import ctypes as C
 import os
 import subprocess

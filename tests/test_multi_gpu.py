@@ -1,4 +1,4 @@
-"""Multi-GPU correctness on hardware (needs >= 2 GPUs; run with `gpurun --gpus 2`): N data-parallel solvers over the C++
+"""Multi-GPU correctness on hardware (needs >= 2 GPUs): N data-parallel solvers over the C++
 P2PSync / ReduceScheduler are equivalent to one solver on the concatenated batch -- the reference's own check
 (src/caffe/test/test_gradient_based_solver.cpp:471-509 runs every solver test with several devices and compares against the
 single-device update; parallel.cpp:208-253 and net.cpp:880-912 are the paths exercised)."""

@@ -1,7 +1,7 @@
 """CPU tests of the text-format prototxt reader and the Net graph builder (host/prototxt.cpp, SURVEY 8(f) rank 1).
-Part 1 uses small nets written here; part 2 reads the reference's own models/*.prototxt UNMODIFIED (skipped when the
-reference tree is not mounted, e.g. on the GPU box) and checks the derived inventories against SURVEY Appendix A and
-against caffe_mpi_b200/shapes.py, which bench.py uses where the prototxts are not available."""
+Part 1 uses small nets written here; part 2 reads the reference's own models/*.prototxt UNMODIFIED (stored under
+tests/golden/reference_models) and checks the derived inventories against SURVEY Appendix A, against
+caffe_mpi_b200/shapes.py and against the generated prototxts of caffe_mpi_b200/models.py, which bench.py trains."""
 import os
 
 import pytest
@@ -9,8 +9,8 @@ import pytest
 from caffe_mpi_b200 import host_api as h
 from caffe_mpi_b200.shapes import MODELS, EXTRA_PARAMS
 
-REF = "/root/reference"
-needs_ref = pytest.mark.skipif(not os.path.isdir(REF + "/models"), reason="reference tree not mounted")
+# the reference's model and solver files the tests below parse, stored unmodified as fixtures
+REF = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_models")
 
 TINY = """
 name: "tiny"   # comment
@@ -103,7 +103,6 @@ REF_MODELS = [
 ]
 
 
-@needs_ref
 @pytest.mark.parametrize("name,path,kw,nconv,gf,nblobs,nfloats", REF_MODELS, ids=[m[0] for m in REF_MODELS])
 def test_reference_prototxts_parse_unmodified(name, path, kw, nconv, gf, nblobs, nfloats):
     n = h.Net(os.path.join(REF, path), "TRAIN", batch_override=1, **kw)
@@ -123,7 +122,6 @@ def test_reference_prototxts_parse_unmodified(name, path, kw, nconv, gf, nblobs,
         assert nfloats - conv_floats == EXTRA_PARAMS[name]
 
 
-@needs_ref
 def test_reference_solver_prototxts():
     for path, policy, lr in (("models/resnet50/solver.prototxt", "poly", 0.001), ("models/bvlc_alexnet/solver.prototxt", None, None),
                              ("models/vgg16/solver.prototxt", None, None), ("examples/mnist/lenet_solver.prototxt", "inv", 0.01)):
@@ -135,21 +133,19 @@ def test_reference_solver_prototxts():
 
 
 def test_generated_resnet50_has_the_reference_inventory():
-    """caffe_mpi_b200.models.resnet50_prototxt (used on the GPU box, where the reference tree is absent) against the
-    inventory of models/resnet50/train_val.prototxt: SURVEY Appendix A numbers, and layer by layer when the file is here."""
+    """caffe_mpi_b200.models.resnet50_prototxt (what bench.py trains) against the
+    inventory of models/resnet50/train_val.prototxt: SURVEY Appendix A numbers, and layer by layer."""
     import os
     from caffe_mpi_b200 import host_api, models
     net = host_api.Net(models.resnet50_prototxt(2), "TRAIN", is_text=True)
     params = net.learnable_params()
     assert len(net.conv_layers()) == 53 and len(params) == 161
     assert sum(p[1] for p in params) == 25557032
-    ref = "/root/reference/models/resnet50/train_val.prototxt"
-    if os.path.exists(ref):
-        rnet = host_api.Net(ref, "TRAIN", batch_override=2)
-        assert net.layers() == [l for l in rnet.layers() if l[1] != "Accuracy"]
-        assert params == rnet.learnable_params()
-        a, b = net.conv_layers(), rnet.conv_layers()
-        assert [(n, bytes(p), pd) for n, p, pd in a] == [(n, bytes(p), pd) for n, p, pd in b]
+    rnet = host_api.Net(os.path.join(REF, "models/resnet50/train_val.prototxt"), "TRAIN", batch_override=2)
+    assert net.layers() == [l for l in rnet.layers() if l[1] != "Accuracy"]
+    assert params == rnet.learnable_params()
+    a, b = net.conv_layers(), rnet.conv_layers()
+    assert [(n, bytes(p), pd) for n, p, pd in a] == [(n, bytes(p), pd) for n, p, pd in b]
 
 
 GENERATED = [("alexnet", "models/bvlc_alexnet/train_val.prototxt", {}), ("vgg16", "models/vgg16/train_val.prototxt", {}),
@@ -159,12 +155,10 @@ GENERATED = [("alexnet", "models/bvlc_alexnet/train_val.prototxt", {}), ("vgg16"
 
 @pytest.mark.parametrize("name,ref,kw", GENERATED, ids=[g[0] for g in GENERATED])
 def test_generated_prototxt_has_the_reference_inventory(name, ref, kw):
-    """caffe_mpi_b200/models.py generators (what bench.py and the GPU box use, where /root/reference does not exist) against
+    """caffe_mpi_b200/models.py generators (what bench.py uses) against
     the reference's own model files: same TRAIN-phase layer list (name, type), conv shapes and learnable-parameter list."""
     from caffe_mpi_b200 import host_api, models
-    path = os.path.join("/root/reference", ref)
-    if not os.path.exists(path):
-        pytest.skip("reference tree not mounted")
+    path = os.path.join(REF, ref)
     r = host_api.Net(path, batch_override=8, **kw)
     g = host_api.Net(models.PROTOTXT[name](8), is_text=True, **kw)
     fields = lambda p: tuple(getattr(p, f) for f, _ in p._fields_)

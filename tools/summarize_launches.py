@@ -1,5 +1,5 @@
 """Per-kernel summary of an ncu launch list (csv with gpu__time_duration.sum and, optionally, dram__bytes_read/write.sum):
-launches, total ms, share, mean us, DRAM GB/s.   python tools/summarize_launches.py profiles/r02_xxx_launches.csv [skip_first_n]"""
+launches, total ms, share, mean us, DRAM GB/s.   python tools/summarize_launches.py <ncu launch list .csv> [skip_first_n]"""
 import csv, re, sys
 path = sys.argv[1]
 skip = int(sys.argv[2]) if len(sys.argv) > 2 else 0

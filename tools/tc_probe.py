@@ -1,4 +1,4 @@
-"""Diagnostic sweep of the tcgen05 conv kernels vs the oracle (prints errors, never asserts)."""
+"""Diagnostic sweep of the tensor-core conv kernels vs the oracle (prints errors, never asserts)."""
 import os, sys, time
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
