@@ -22,14 +22,16 @@
 //     bf16 hi + bf16 lo (hi = rn(a), lo = rn(a - hi)), pack pairs along K and write the A operand into shared memory
 //     (K-major, no swizzle, tc_common.cuh), 64 K-elements per stage.
 //   * The filter is pre-split into bf16 hi / lo in GEMM-K order (channel group, tap, channel) by a prepass and streamed
-//     by TMA (SWIZZLE_128B, [N_TILE x 64] boxes).  Two consumer warpgroups issue wgmma.mma_async.m64nNk16.bf16 (fp32
-//     accumulators in registers, rows [64 cw, 64 cw + 64) each): lo*hi + hi*lo + hi*hi per K step -- three bf16 MMAs
-//     cost 1.5 TF32-MMA equivalents (3xTF32 costs 3), and the operand bytes in shared memory halve.  Dropped terms
-//     (lo*lo and the bf16 rounding of lo) are ~2^-17 per product, far inside the 1e-3 blob tolerance.
-//   * Epilogue (the consumers, after the tile's last K block): (+ bias), 32-channel chunks transposed through shared
-//     memory [channel][128 pixels] and written by the TMA unit when the tile lies inside one image: one tensor store per
-//     chunk (box {128, 32, 1} of the output blob, clipped by the hardware at the image end and the channel count; the start
-//     column is never negative).  Tiles that span two images write the staged chunk with 16-byte st.global.
+//     by TMA (SWIZZLE_128B, [N_TILE x 64] boxes).  Two consumer warpgroups take turns over the CTA's tiles (ping-pong):
+//     each issues wgmma.mma_async.m64nNk16.bf16 for both 64-row halves of its own tile (fp32 accumulators in registers,
+//     N_TILE per thread): lo*hi + hi*lo + hi*hi per K step -- three bf16 MMAs cost 1.5 TF32-MMA equivalents (3xTF32
+//     costs 3), and the operand bytes in shared memory halve.  Dropped terms (lo*lo and the bf16 rounding of lo) are
+//     ~2^-17 per product, far inside the 1e-3 blob tolerance.
+//   * Epilogue (the tile's warpgroup, after its last K block, while the other warpgroup runs the next tile's MMAs):
+//     (+ bias), 32-channel chunks transposed through the warpgroup's own shared-memory buffer [channel][128 pixels] and
+//     written by the TMA unit when the tile lies inside one image: one tensor store per chunk (box {128, 32, 1} of the
+//     output blob, clipped by the hardware at the image end and the channel count; the start column is never negative).
+//     Tiles that span two images write the staged chunk with 16-byte st.global.
 //   * Plane mode (BWT < 128): 7x7 maps, whole image planes staged -- see Smem below.
 // dgrad of a stride-1 same convolution is the same kernel on dY with the transposed + flipped filter.
 #include <cuda.h>
@@ -47,12 +49,21 @@ using namespace tc;
 
 namespace stg {
 
-constexpr int NCONS = 8;                      // consumer warps: two warpgroups (wgmma + epilogue), tile rows [64 cw, 64 cw + 64)
+// Five whole warpgroups, so that setmaxnreg can give each role its own register budget:
+//   WG0, WG1  consumers (wgmma + epilogue), ping-pong: each owns whole 128 x N_TILE tiles, the CTA's even / odd ones
+//   WG2, WG3  the 8 converter warps
+//   WG4       filter TMA warp, activation TMA warp, two idle warps
 constexpr int NCW = 8;                        // converter warps
-constexpr int W_CONV0 = NCONS;                // first converter warp
-constexpr int W_BTMA = NCONS + NCW;           // filter TMA warp
-constexpr int W_STG = NCONS + NCW + 1;        // activation TMA warp
-constexpr int THREADS = (NCONS + NCW + 2) * 32;   // 576
+constexpr int W_CONV0 = 8;                    // first converter warp
+constexpr int W_BTMA = 16;                    // filter TMA warp
+constexpr int W_STG = 17;                     // activation TMA warp
+constexpr int THREADS = 5 * 128;              // 640
+// registers per thread after setmaxnreg: the consumers hold two m64 x N_TILE accumulator sets (N_TILE fp32 per thread).
+// All budgets together must fit what the CTA is launched with: 65536 / 640 rounded down to the allocation unit of 8 = 96.
+constexpr int REG_CONS = 176, REG_CONV = 48, REG_TMA = 32;
+static_assert(2 * 128 * REG_CONS + 2 * 128 * REG_CONV + 128 * REG_TMA <= THREADS * ((65536 / THREADS) & ~7), "register budget");
+// named barriers: 1 + w = warpgroup w's epilogue, 3 + w = "warpgroup w may start its next tile's MMAs"
+constexpr int BAR_EPI = 1, BAR_ORDER = 3;
 constexpr int CB = 32;                        // channels per staged group
 constexpr int BKE = 64;                       // bf16 K elements per pipeline stage (two (group, tap) half blocks)
 constexpr uint32_t STG_POOL = 64u * 1024u;    // activation staging pool, carved into slots of one TMA box each
@@ -80,7 +91,7 @@ template <int N_TILE, int BWT>
 struct Smem {
   static constexpr uint32_t B_BYTES = (uint32_t)N_TILE * 128u;              // [N_TILE rows][64 bf16], SW128
   static constexpr uint32_t A_BYTES = tile_bytes(128);                      // [128 rows][64 bf16], K-major no swizzle
-  static constexpr uint32_t STAGE = 2u * B_BYTES + ((2u * A_BYTES + 1023u) & ~1023u);   // B hi, B lo, A hi, A lo
+  static constexpr uint32_t STAGE = 2u * B_BYTES + 2u * A_BYTES;           // B hi, B lo, A hi, A lo
   // BWT >= 128: one box = [32 channels][BWT pixels] fp32.  BWT < 128 ("plane mode", maps of BWT = H*W pixels whose
   // channel pitch TMA cannot address, 7x7 = 196 bytes): one slot = up to PLANE_IMGS whole images x [32 channels][H*W]
   static constexpr bool PLANE = BWT < 128;
@@ -91,13 +102,16 @@ struct Smem {
   static_assert(!PLANE || 127 / BWT + 2 <= PLANE_IMGS, "a 128-row tile touches at most PLANE_IMGS images");
   static constexpr int NSLOT_ = (int)(STG_POOL / SLOT_BYTES);
   static constexpr int NSLOT = NSLOT_ > MAX_SLOTS ? MAX_SLOTS : NSLOT_;
-  static constexpr uint32_t EPI_BYTES = 32u * 128u * 4u;                    // [32 channels][128 pixels] fp32
-  static constexpr uint32_t FIXED = STG_POOL + EPI_BYTES + 256u + MAX_TAPS * 4u + 1024u;
+  static constexpr uint32_t EPI_BYTES = 32u * 128u * 4u;                    // [32 channels][128 pixels] fp32, one per consumer warpgroup
+  static constexpr uint32_t FIXED = STG_POOL + 2u * EPI_BYTES + 256u + MAX_TAPS * 4u + 1024u;
   static constexpr int STAGES_ = (int)((227u * 1024u - FIXED) / STAGE);
   static constexpr int STAGES = STAGES_ > 3 ? 3 : STAGES_;                  // operand pipeline depth
-  static constexpr uint32_t STG_OFF = STAGES * STAGE;
+  // the B tiles of every stage first (SWIZZLE_128B wants 1024-byte alignment), then the A tiles, packed
+  static constexpr uint32_t A_OFF = STAGES * 2u * B_BYTES;
+  static constexpr uint32_t STG_OFF = A_OFF + STAGES * 2u * A_BYTES;
   static constexpr uint32_t EPI_OFF = STG_OFF + STG_POOL;
-  static constexpr uint32_t BAR_OFF = EPI_OFF + EPI_BYTES;
+  static constexpr uint32_t BAR_OFF = EPI_OFF + 2u * EPI_BYTES;
+  static_assert(STG_OFF % 128u == 0, "TMA destinations are 128-byte aligned");
   static constexpr uint32_t TAP_OFF = BAR_OFF + 256;                        // int tap offsets [MAX_TAPS]
   static constexpr uint32_t TOTAL = TAP_OFF + MAX_TAPS * 4 + 1024;          // + alignment slack
   static constexpr uint32_t TX_BYTES = 2u * B_BYTES;
@@ -157,7 +171,7 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* sptr = smem_raw + (sbase - smem_u32(smem_raw));
   const uint32_t bar_full = sbase + S::BAR_OFF;                 // STAGES: 8 converter warps + the filter TMA's expect_tx
-  const uint32_t bar_empty = bar_full + 8 * STAGES;             // STAGES: the 8 consumer warps are done with the stage
+  const uint32_t bar_empty = bar_full + 8 * STAGES;             // STAGES: the 4 warps of the consumer warpgroup that owns the stage's tile are done with it
   const uint32_t bar_sfull = bar_empty + 8 * STAGES;            // MAX_SLOTS: staged box landed
   const uint32_t bar_sempty = bar_sfull + 8 * MAX_SLOTS;        // MAX_SLOTS: the converters are done with the box
   int* tapoff = reinterpret_cast<int*>(sptr + S::TAP_OFF);
@@ -165,7 +179,7 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, NCW + 1); mbar_init(bar_empty + 8 * s, NCONS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, NCW + 1); mbar_init(bar_empty + 8 * s, 4); }
     for (int b = 0; b < MAX_SLOTS; ++b) { mbar_init(bar_sfull + 8 * b, 1); mbar_init(bar_sempty + 8 * b, NCW); }
     fence_barrier_init();
   }
@@ -175,9 +189,9 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   }
   __syncthreads();
 
-  auto stage_b_hi = [&](int s) { return sbase + (uint32_t)s * S::STAGE; };
-  auto stage_b_lo = [&](int s) { return sbase + (uint32_t)s * S::STAGE + S::B_BYTES; };
-  auto stage_a_hi = [&](int s) { return sbase + (uint32_t)s * S::STAGE + 2u * S::B_BYTES; };
+  auto stage_b_hi = [&](int s) { return sbase + (uint32_t)s * 2u * S::B_BYTES; };
+  auto stage_b_lo = [&](int s) { return sbase + (uint32_t)s * 2u * S::B_BYTES + S::B_BYTES; };
+  auto stage_a_hi = [&](int s) { return sbase + S::A_OFF + (uint32_t)s * 2u * S::A_BYTES; };
   auto slot_addr = [&](int slot) { return sbase + S::STG_OFF + (uint32_t)slot * S::SLOT_BYTES; };
   auto tile_coords = [&](int tile, int& m0, int& n0) {
     const int nt = tile % p.n_tiles;
@@ -197,6 +211,7 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   if (warp >= W_CONV0 && warp < W_CONV0 + NCW) {
     // ================= converters: staged fp32 -> bf16 hi/lo -> A tile in shared memory ========================
     // thread = (GEMM row, channel octets sub and sub + 2 of every 32-channel half block)
+    setmaxnreg_dec<REG_CONV>();
     const int cw = warp - W_CONV0;
     const int rq = cw & 3, sub = cw >> 2;
     const int row = rq * 32 + lane;
@@ -241,9 +256,12 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       int g = 0, tap = 0;
       uint32_t src_base = 0;
       for (int kb = 0; kb < p.nkb; ++kb, ++kbg) {
-        uint32_t hi[16], lo[16];                               // [octet o][half block h][4 words]
+        // one half block at a time: 8 + 8 words live, not 16 + 16.  The first one is converted before waiting for the stage.
+        const int s = kbg % STAGES, it = kbg / STAGES;
+        const uint32_t a0 = stage_a_hi(s) + a_row;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
+          uint32_t hi[8], lo[8];                               // [octet o][4 words]
           if (2 * kb + h < p.nhb) {
             const int u0 = u_base + g * nseg;
             if (tap == 0) {                                    // first tap of a channel group: its box(es) must have landed
@@ -265,8 +283,8 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
               for (int e = 0; e < 4; ++e) {
                 uint32_t hw, lw;
                 split_pack_bf16(v[o * 8 + 2 * e], v[o * 8 + 2 * e + 1], hw, lw);
-                hi[(o * 2 + h) * 4 + e] = ok ? hw : 0u;        // masked taps contribute exact zeros (never NaN from stale smem)
-                lo[(o * 2 + h) * 4 + e] = ok ? lw : 0u;
+                hi[o * 4 + e] = ok ? hw : 0u;                  // masked taps contribute exact zeros (never NaN from stale smem)
+                lo[o * 4 + e] = ok ? lw : 0u;
               }
             if (++tap == p.taps) {                             // group fully consumed by this warp: hand its box(es) back
               tap = 0;
@@ -281,21 +299,16 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
 #pragma unroll
             for (int o = 0; o < 2; ++o)
 #pragma unroll
-              for (int e = 0; e < 4; ++e) { hi[(o * 2 + h) * 4 + e] = 0u; lo[(o * 2 + h) * 4 + e] = 0u; }   // K padding: finite zeros
+              for (int e = 0; e < 4; ++e) { hi[o * 4 + e] = 0u; lo[o * 4 + e] = 0u; }   // K padding: finite zeros
+          }
+          if (h == 0) mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 32);
+#pragma unroll
+          for (int o = 0; o < 2; ++o) {
+            const uint32_t a = a0 + (uint32_t)(h * 4 + sub + 2 * o) * LBO_A;      // 16-byte K chunk = 8 channels
+            sts128u(a, hi[o * 4], hi[o * 4 + 1], hi[o * 4 + 2], hi[o * 4 + 3]);
+            sts128u(a + S::A_BYTES, lo[o * 4], lo[o * 4 + 1], lo[o * 4 + 2], lo[o * 4 + 3]);
           }
         }
-        const int s = kbg % STAGES, it = kbg / STAGES;
-        mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 32);
-        const uint32_t a0 = stage_a_hi(s) + a_row;
-#pragma unroll
-        for (int o = 0; o < 2; ++o)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t a = a0 + (uint32_t)(h * 4 + sub + 2 * o) * LBO_A;      // 16-byte K chunk = 8 channels
-            const int b = (o * 2 + h) * 4;
-            sts128u(a, hi[b], hi[b + 1], hi[b + 2], hi[b + 3]);
-            sts128u(a + S::A_BYTES, lo[b], lo[b + 1], lo[b + 2], lo[b + 3]);
-          }
         fence_proxy_async();
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_full + 8 * s);
@@ -303,126 +316,156 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       u_base += p.groups * nseg;
     }
     if (prof && cw == 0 && lane == 0) { p.prof[0] = clock64() - c_t0; p.prof[3] = kbg; }
-  } else if (warp == W_BTMA) {
-    // ================= filter TMA producer ====================================================================
-    int kbg = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      int m0, n0;
-      tile_coords(tile, m0, n0);
-      for (int kb = 0; kb < p.nkb; ++kb, ++kbg) {
-        const int s = kbg % STAGES, it = kbg / STAGES;
-        mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 32);
-        if (elect_one()) {
-          arrive_expect_tx(bar_full + 8 * s, S::TX_BYTES);
-          tma_load_3d(stage_b_hi(s), &map_hi, bar_full + 8 * s, kb * BKE, n0, 0);
-          tma_load_3d(stage_b_lo(s), &map_lo, bar_full + 8 * s, kb * BKE, n0, 0);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == W_STG) {
-    // ================= activation TMA producer: one box per channel group and image ==============================
-    int u = 0;
-    long long s_wait = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      int m0, n0, n_first, nseg, split, nimg;
-      tile_coords(tile, m0, n0);
-      tile_images(m0, n_first, nseg, split, nimg);
-      for (int g = 0; g < p.groups; ++g) {
-        for (int seg = 0; seg < nseg; ++seg, ++u) {
-          const int slot = u % NSLOT;
-          if (prof) { const long long t0 = clock64(); mbar_wait_backoff(bar_sempty + 8 * slot, ((u / NSLOT) & 1) ^ 1, 32); s_wait += clock64() - t0; }
-          else mbar_wait_backoff(bar_sempty + 8 * slot, ((u / NSLOT) & 1) ^ 1, 32);
+  } else if (warp >= W_BTMA) {
+    setmaxnreg_dec<REG_TMA>();
+    if (warp == W_BTMA) {
+      // ================= filter TMA producer ====================================================================
+      int kbg = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        int m0, n0;
+        tile_coords(tile, m0, n0);
+        for (int kb = 0; kb < p.nkb; ++kb, ++kbg) {
+          const int s = kbg % STAGES, it = kbg / STAGES;
+          mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 32);
           if (elect_one()) {
-            if constexpr (PLANE) {
-              // the blob viewed as {4*H*W, C/4, N} (four channels per row: a 16-byte multiple pitch); box {4*H*W, 8, 1} is
-              // 32 channels of one image, contiguous
-              arrive_expect_tx(bar_sfull + 8 * slot, (uint32_t)nimg * S::IMG_BYTES);
-              for (int k = 0; k < nimg; ++k)
-                tma_load_3d(slot_addr(slot) + (uint32_t)k * S::IMG_BYTES, &map_x, bar_sfull + 8 * slot, 0, g * (CB / 4), n_first + k);
-            } else {
-              arrive_expect_tx(bar_sfull + 8 * slot, S::SLOT_BYTES);
-              const int col0 = seg ? 0 : max((m0 - n_first * p.HW - p.halo) & ~3, 0);   // 16-byte aligned; columns past the image end read as zero
-              tma_load_3d(slot_addr(slot), &map_x, bar_sfull + 8 * slot, col0, g * CB, n_first + seg);
-            }
+            arrive_expect_tx(bar_full + 8 * s, S::TX_BYTES);
+            tma_load_3d(stage_b_hi(s), &map_hi, bar_full + 8 * s, kb * BKE, n0, 0);
+            tma_load_3d(stage_b_lo(s), &map_lo, bar_full + 8 * s, kb * BKE, n0, 0);
           }
           __syncwarp();
         }
       }
-    }
-    if (prof && lane == 0) { p.prof[4] = s_wait; p.prof[5] = u; }
-  } else if (warp < NCONS) {
-    // ================= consumers: wgmma + epilogue ===============================================================
-    const int cwg = warp >> 2, t = tid & 127;
-    float* epi = reinterpret_cast<float*>(sptr + S::EPI_OFF);
-    const bool issuer = warp == 0;
-    float acc[N_TILE / 2];
+    } else if (warp == W_STG) {
+      // ================= activation TMA producer: one box per channel group and image ==============================
+      int u = 0;
+      long long s_wait = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        int m0, n0, n_first, nseg, split, nimg;
+        tile_coords(tile, m0, n0);
+        tile_images(m0, n_first, nseg, split, nimg);
+        for (int g = 0; g < p.groups; ++g) {
+          for (int seg = 0; seg < nseg; ++seg, ++u) {
+            const int slot = u % NSLOT;
+            if (prof) { const long long t0 = clock64(); mbar_wait_backoff(bar_sempty + 8 * slot, ((u / NSLOT) & 1) ^ 1, 32); s_wait += clock64() - t0; }
+            else mbar_wait_backoff(bar_sempty + 8 * slot, ((u / NSLOT) & 1) ^ 1, 32);
+            if (elect_one()) {
+              if constexpr (PLANE) {
+                // the blob viewed as {4*H*W, C/4, N} (four channels per row: a 16-byte multiple pitch); box {4*H*W, 8, 1} is
+                // 32 channels of one image, contiguous
+                arrive_expect_tx(bar_sfull + 8 * slot, (uint32_t)nimg * S::IMG_BYTES);
+                for (int k = 0; k < nimg; ++k)
+                  tma_load_3d(slot_addr(slot) + (uint32_t)k * S::IMG_BYTES, &map_x, bar_sfull + 8 * slot, 0, g * (CB / 4), n_first + k);
+              } else {
+                arrive_expect_tx(bar_sfull + 8 * slot, S::SLOT_BYTES);
+                const int col0 = seg ? 0 : max((m0 - n_first * p.HW - p.halo) & ~3, 0);   // 16-byte aligned; columns past the image end read as zero
+                tma_load_3d(slot_addr(slot), &map_x, bar_sfull + 8 * slot, col0, g * CB, n_first + seg);
+              }
+            }
+            __syncwarp();
+          }
+        }
+      }
+      if (prof && lane == 0) { p.prof[4] = s_wait; p.prof[5] = u; }
+    }                                                    // warps 18 and 19: no work
+  } else {
+    // ================= consumers: ping-pong wgmma + epilogue =====================================================
+    // Warpgroup cw owns the CTA's tiles of ordinal j = cw, cw + 2, ... and issues both m64 row halves of each (rows [0, 64)
+    // into acc0, [64, 128) into acc1).  Its epilogue then runs while the other warpgroup issues the next tile's MMAs.
+    setmaxnreg_inc<REG_CONS>();
+    const int cw = warp >> 2, wq = warp & 3, t = tid & 127;
+    float* epi = reinterpret_cast<float*>(sptr + S::EPI_OFF + (uint32_t)cw * S::EPI_BYTES);
+    const bool issuer = wq == 0;
+    float acc0[N_TILE / 2], acc1[N_TILE / 2];
 #pragma unroll
-    for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
-    int kbg = 0;
-    long long m_full = 0, m_t0 = 0;
-    if (prof) m_t0 = clock64();
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    for (int i = 0; i < N_TILE / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    // profile counters of CTA 0 (B2C_PROF), SM cycles added straight into the zeroed buffer: no registers held across the loop
+    long long* const pc = p.prof + 8 + 8 * cw;
+    const bool tally = prof && t == 0;
+    long long m_t0 = 0;
+    if (tally) m_t0 = clock64();
+    for (int j = cw, tile = blockIdx.x + cw * (int)gridDim.x; tile < p.total_tiles; j += 2, tile += 2 * (int)gridDim.x) {
       int m0, n0, n_first, nseg, split, nimg;
       tile_coords(tile, m0, n0);
       tile_images(m0, n_first, nseg, split, nimg);
+      // Start only once the other warpgroup has seen every K block of tile j - 1 land: the producers fill the stage ring in
+      // tile order, so every earlier fill of this tile's stages is then complete and the parity waits below cannot match a
+      // phase two behind.  It also keeps the tensor core working on one tile at a time.
+      if (j > 0) {
+        const long long t0 = tally ? clock64() : 0;
+        named_bar(BAR_ORDER + cw, 256);
+        if (tally) pc[2] += clock64() - t0;
+      }
+      int kbg = j * p.nkb;                                 // this tile's position in the stage ring
       int prev = -1;
       for (int kb = 0; kb < p.nkb; ++kb, ++kbg) {
         const int s = kbg % STAGES, it = kbg / STAGES;
-        if (prof) { const long long t0 = clock64(); mbar_wait(bar_full + 8 * s, it & 1); m_full += clock64() - t0; }
-        else mbar_wait(bar_full + 8 * s, it & 1);
+        const long long t0 = tally ? clock64() : 0;
+        mbar_wait(bar_full + 8 * s, it & 1);
+        if (tally) pc[1] += clock64() - t0;
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < BKE / 16; ++kk) {
-          const uint32_t a = stage_a_hi(s) + 2u * kk * LBO_A + (uint32_t)cwg * 1024u;
-          const uint64_t ah = smem_desc(a, LBO_A, 128), al = smem_desc(a + S::A_BYTES, LBO_A, 128);
+          const uint32_t a = stage_a_hi(s) + 2u * kk * LBO_A;
+          const uint64_t ah0 = smem_desc(a, LBO_A, 128), al0 = smem_desc(a + S::A_BYTES, LBO_A, 128);
+          const uint64_t ah1 = smem_desc(a + 1024u, LBO_A, 128), al1 = smem_desc(a + 1024u + S::A_BYTES, LBO_A, 128);
           const uint64_t bh = smem_desc_sw128(stage_b_hi(s) + kk * 32), bl = smem_desc_sw128(stage_b_lo(s) + kk * 32);
-          MMA::mma(acc, al, bh, (kb | kk) != 0);   // lo * hi
-          MMA::mma(acc, ah, bl, 1);                // hi * lo
-          MMA::mma(acc, ah, bh, 1);                // hi * hi
+          MMA::mma(acc0, al0, bh, (kb | kk) != 0);   // lo * hi
+          MMA::mma(acc0, ah0, bl, 1);                // hi * lo
+          MMA::mma(acc0, ah0, bh, 1);                // hi * hi
+          MMA::mma(acc1, al1, bh, (kb | kk) != 0);
+          MMA::mma(acc1, ah1, bl, 1);
+          MMA::mma(acc1, ah1, bh, 1);
         }
         wgmma_commit();
         wgmma_wait<1>();
         if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
         prev = s;
       }
+      if (tally) pc[5] += p.nkb;
+      if (tile + (int)gridDim.x < p.total_tiles) named_bar_arrive(BAR_ORDER + (cw ^ 1), 256);   // tile j + 1 may start
+      long long e0 = tally ? clock64() : 0;
       wgmma_wait<0>();
-      wgmma_reg_fence(acc);
+      wgmma_reg_fence(acc0);
+      wgmma_reg_fence(acc1);
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+      if (tally) { const long long e1 = clock64(); pc[3] += e1 - e0; e0 = e1; }
 
-      // ---- epilogue: (+ bias) -> 32-channel chunks transposed into shared memory [channel][128 pixels] -> one TMA tensor
-      // store per chunk when the tile lies inside one image, else 16-byte st.global; plane mode: per-pixel stores
+      // ---- epilogue: (+ bias) -> 32-channel chunks transposed into this warpgroup's [channel][128 pixels] buffer -> one
+      // TMA tensor store per chunk when the tile lies inside one image, else 16-byte st.global; plane mode: per-pixel stores
+      // A warp's fragment covers 16 rows and the buffer's row pitch is 128 words, so at best 16 banks take a store: lanes
+      // of odd column pairs write element i ^ 2 (row + 8) where the others write element i (2-way conflicts, not 4-way).
+      const int sw = (lane & 1) << 1;
+      const int nrem = p.Ntot - n0;                        // channels of this tile inside the output
 #pragma unroll
       for (int c = 0; c < N_TILE / 32; ++c) {
         const int c0 = c * 32;
-        if (n0 + c0 >= p.Ntot) break;                     // uniform over the consumers
-        // the TMA store of the previous chunk has finished reading the staging buffer (elect.sync on a converged warp always
-        // elects the same lane, which owns the bulk-async groups)
+        if (c0 >= nrem) break;                             // uniform over the warpgroup
+        // the TMA store of the previous chunk has finished reading the buffer (elect.sync on a converged warp always elects
+        // the same lane, which owns the bulk-async groups)
         if (issuer && elect_one()) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        named_bar(1, NCONS * 32);
+        named_bar(BAR_EPI + cw, 128);
 #pragma unroll
         for (int i = 0; i < N_TILE / 2; ++i)
           if ((i >> 4) == c) {
-            const int col = frag_col(t, i);
-            float v = acc[i];
-            if (p.bias && n0 + col < p.Ntot) v += __ldg(p.bias + n0 + col);
-            epi[(col - c0) * 128 + cwg * 64 + frag_row(t, i)] = v;
+            const int col = frag_col(t, i), row = frag_row(t, i ^ sw);   // frag_col(t, i ^ 2) == frag_col(t, i)
+            float v0 = sw ? acc0[i ^ 2] : acc0[i];
+            float v1 = sw ? acc1[i ^ 2] : acc1[i];
+            if (p.bias && col < nrem) { const float b = __ldg(p.bias + n0 + col); v0 += b; v1 += b; }
+            epi[(col - c0) * 128 + row] = v0;
+            epi[(col - c0) * 128 + 64 + row] = v1;
           }
         fence_proxy_async();                               // generic-proxy writes -> visible to the TMA store
-        named_bar(1, NCONS * 32);
+        named_bar(BAR_EPI + cw, 128);
         if constexpr (PLANE) {
-          // thread = (pixel r, 16 channels): every channel's store is one (unaligned) 128-byte run per warp
-          const int r = tid & 127, hc = tid >> 7;
-          const int q = m0 + r;
+          // thread = pixel: every channel's store is one (unaligned) 128-byte run per warp
+          const int q = m0 + t;
           if (q < p.Mtot) {
             const int nq = q / p.HW;
             float* ob = p.out + ((size_t)nq * p.Ntot + n0 + c0) * p.HW + (q - nq * p.HW);
 #pragma unroll 4
-            for (int j = 0; j < 16; ++j) {
-              const int ch = hc * 16 + j;
-              if (n0 + c0 + ch < p.Ntot) { float* d = ob + (size_t)ch * p.HW; const float v = epi[ch * 128 + r]; *d = p.accumulate ? *d + v : v; }
-            }
+            for (int ch = 0; ch < 32; ++ch)
+              if (c0 + ch < nrem) { float* d = ob + (size_t)ch * p.HW; const float v = epi[ch * 128 + t]; *d = p.accumulate ? *d + v : v; }
           }
         } else if (nseg == 1 && !(p.dbg & 1)) {
           // the tile lies inside one image: box column 0 = tile row 0 = pixel m0 - n*HW >= 0; columns past the image end
@@ -433,15 +476,15 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
           }
         } else {
-          // the tile spans two images: 16-byte st.global from the staged chunk, warp = 4 channels, lane = 4 pixels
+          // the tile spans two images: 16-byte st.global from the staged chunk, warp = 8 channels, lane = 4 pixels
           const int mv = m0 + lane * 4;                    // H*W % 4 == 0: never across an image end
           if (mv < p.Mtot) {
             const int nv = mv / p.HW, pv = mv - nv * p.HW;
             float* vbase = p.out + ((size_t)nv * p.Ntot + n0 + c0) * p.HW + pv;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int ch = warp * 4 + q;
-              if (n0 + c0 + ch < p.Ntot) {
+            for (int q = 0; q < 8; ++q) {
+              const int ch = wq * 8 + q;
+              if (c0 + ch < nrem) {
                 float4 v = *reinterpret_cast<const float4*>(epi + ch * 128 + lane * 4);
                 float4* dst = reinterpret_cast<float4*>(vbase + (size_t)ch * p.HW);
                 if (p.accumulate) { const float4 o = *dst; v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w; }
@@ -451,9 +494,10 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
           }
         }
       }
+      if (tally) pc[4] += clock64() - e0;
     }
     if (issuer && elect_one()) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    if (prof && tid == 0) { p.prof[8] = clock64() - m_t0; p.prof[9] = m_full; p.prof[10] = kbg; }
+    if (tally) pc[0] = clock64() - m_t0;
   }
   __syncthreads();
 }
@@ -653,8 +697,15 @@ int launch_conv_tc_stg(const ConvShape& s, int op, const float* a, const float* 
   if (rc == B2C_OK && prof_on) {
     long long h[32];
     cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[stg-prof] N_TILE=%d BWT=%d nkb=%d groups=%d taps=%d tiles=%d | conv(t0): total=%lld kblocks=%lld | act-tma: wait_empty=%lld boxes=%lld | consumer: total=%lld wait_full=%lld kblocks=%lld\n",
-            n_tile, g.bwt, g.nkb, g.groups, g.taps, p.total_tiles, h[0], h[3], h[4], h[5], h[8], h[9], h[10]);
+    fprintf(stderr, "[stg-prof] N_TILE=%d BWT=%d nkb=%d groups=%d taps=%d tiles=%d | conv(t0): total=%lld kblocks=%lld | act-tma: wait_empty=%lld boxes=%lld\n",
+            n_tile, g.bwt, g.nkb, g.groups, g.taps, p.total_tiles, h[0], h[3], h[4], h[5]);
+    // CTA 0's consumer warpgroups, SM cycles: issue = total - wait_full - wait_order - mma_drain - epilogue (issuing MMAs, and
+    // waiting behind the other warpgroup's MMAs in the tensor core)
+    for (int w = 0; w < 2; ++w) {
+      const long long* c = h + 8 + 8 * w;
+      fprintf(stderr, "[stg-prof]   consumer wg%d: total=%lld wait_full=%lld wait_order=%lld mma_drain=%lld epilogue=%lld issue=%lld kblocks=%lld\n",
+              w, c[0], c[1], c[2], c[3], c[4], c[0] - c[1] - c[2] - c[3] - c[4], c[5]);
+    }
   }
   return rc;
 }

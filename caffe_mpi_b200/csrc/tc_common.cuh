@@ -152,6 +152,14 @@ __device__ __forceinline__ int frag_row(int t, int i) { return ((t >> 5) << 4) +
 __device__ __forceinline__ int frag_col(int t, int i) { return ((i >> 2) << 3) + ((t & 3) << 1) + (i & 1); }
 // named barrier over `n` threads (the consumer warpgroups of a kernel)
 __device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// signal side of a named barrier: counts the calling warp towards `n` without waiting (the waiting side calls named_bar)
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// per-warpgroup register budget (all four warps of the warpgroup execute it): .dec returns registers to the CTA's pool,
+// .inc waits until the pool holds enough.  The budgets of all warpgroups must fit the registers the CTA was launched with.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ---- TF32 split ------------------------------------------------------------------------------------
 // fp32-equivalent mode: hi = a with the 13 low mantissa bits cleared (exactly a TF32 value), lo = a - hi
