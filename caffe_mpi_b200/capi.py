@@ -12,6 +12,9 @@ MATH_FP32, MATH_TF32, MATH_FP32_3XTF32 = 0, 1, 2
 ALGO_AUTO, ALGO_SIMT, ALGO_TCGEN05 = 0, 1, 2
 OP_FORWARD, OP_BACKWARD_DATA, OP_BACKWARD_FILTER = 0, 1, 2
 UNIQUE_ID_BYTES = 128
+# b2c_wgrad_route, in enum order
+WGRAD_ROUTES = ("caffe", "simt", "gather", "staged_3x3", "staged_3x3_plane", "staged_1x1", "staged_1x1_plane", "tma_1x1",
+                "compact_staged", "compact_tma")
 
 
 class B2CError(RuntimeError):
@@ -94,6 +97,7 @@ def lib():
         "b2c_conv_out_shape": (i, [vp, C.POINTER(i), C.POINTER(i)]),
         "b2c_conv_workspace_bytes": (sz, [vp, i]),
         "b2c_conv_algo_used": (i, [vp, i]),
+        "b2c_debug_wgrad_plan": (i, [vp, C.POINTER(i), i]),
         "b2c_conv_forward": (i, [vp, vp, vp, vp, vp, vp, sz, vp]),
         "b2c_conv_backward_data": (i, [vp, vp, vp, vp, vp, sz, vp]),
         "b2c_conv_backward_filter": (i, [vp, vp, vp, vp, vp, sz, vp]),
@@ -187,6 +191,12 @@ class ConvDesc:
 
     def algo_used(self, op):
         return int(lib().b2c_conv_algo_used(self._h, op))
+
+    def wgrad_plan(self):
+        """b2c_debug_wgrad_plan: the weight-gradient route for 16-byte aligned operands and its split-K plan."""
+        out = (C.c_int * 6)()
+        check(lib().b2c_debug_wgrad_plan(self._h, out, 6))
+        return dict(route=WGRAD_ROUTES[out[0]], splits=out[1], per=out[2], nkb=out[3], cols=out[4], bpi=out[5])
 
     def _workspace(self, op, like):
         import torch

@@ -73,6 +73,10 @@ int launch_conv_tc_stg(const ConvShape&, int op, const float* a, const float* w,
 bool tc_wgrad_stg_supported(const ConvShape&);
 size_t tc_wgrad_stg_workspace(const ConvShape&);
 int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t);
+bool tc_wgrad_stg_plan_info(const ConvShape&, WgradPlanInfo*);
+// weight-gradient route among the gather-family kernels (conv_tc_wgrad.cu) and its plan
+int tc_wgrad_route(const ConvShape&, int math, bool x_ok, bool dy_ok, bool ws_ok);
+void tc_wgrad_plan_info(const ConvShape&, int route, WgradPlanInfo*);
 bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K);
 size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K);
 int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const float* A, const float* B, float beta,
@@ -93,6 +97,21 @@ static bool use_staged(const b2c_conv_desc* d, int op) {
 }
 // math mode handed to the gather kernels (conv_tc.cu / conv_tc_wgrad.cu), which know FP32 (= 3xTF32) and TF32
 static int gather_math(const b2c_conv_desc* d) { return d->math == B2C_MATH_TF32 ? B2C_MATH_TF32 : B2C_MATH_FP32; }
+
+// The kernel b2c_conv_backward_filter runs (b2c_wgrad_route), decided in one place for the launch and for b2c_debug_wgrad_plan.
+// x_ok / dy_ok / ws_ok: those pointers are 16-byte aligned (the staged and TMA-fed kernels need it; otherwise the gather kernel).
+static int wgrad_route(const b2c_conv_desc* d, bool x_ok, bool dy_ok, bool ws_ok) {
+  if (d->engine == B2C_ENGINE_CAFFE) return B2C_WGRAD_ROUTE_CAFFE;
+  if (use_staged(d, B2C_OP_BACKWARD_FILTER) && x_ok && dy_ok) {
+    WgradPlanInfo q{};
+    tc_wgrad_stg_plan_info(d->s, &q);
+    if (q.taps == 9) return q.plane ? B2C_WGRAD_ROUTE_STAGED_3X3_PLANE : B2C_WGRAD_ROUTE_STAGED_3X3;
+    return q.plane ? B2C_WGRAD_ROUTE_STAGED_1X1_PLANE : B2C_WGRAD_ROUTE_STAGED_1X1;
+  }
+  if (tc_conv_supported(d->s, B2C_OP_BACKWARD_FILTER) && d->algo != B2C_ALGO_SIMT)
+    return tc_wgrad_route(d->s, gather_math(d), x_ok, dy_ok, ws_ok);
+  return B2C_WGRAD_ROUTE_SIMT;
+}
 
 // ---- prepared-filter cache: [forward layout | dgrad layout], each region 256-byte aligned -------------------------------
 static size_t cache_region_bytes(const b2c_conv_desc* d, int op) {
@@ -309,7 +328,9 @@ extern "C" int b2c_conv_backward_filter(const b2c_conv_desc* d, const float* x, 
   cudaStream_t st = as_stream(stream);
   const size_t need = b2c_conv_workspace_bytes(d, B2C_OP_BACKWARD_FILTER);
   if (ws_bytes < need || (need && !ws)) return fail(B2C_ERR_WORKSPACE, "backward_filter workspace too small");
-  if (d->engine == B2C_ENGINE_CAFFE) {
+  auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+  const int route = wgrad_route(d, aligned(x), aligned(dy), ws && aligned(ws));
+  if (route == B2C_WGRAD_ROUTE_CAFFE) {
     const int P = s.Ho * s.Wo;
     const size_t bdim = (size_t)s.C * s.H * s.W, tdim = (size_t)s.O * P;
     float* col = static_cast<float*>(ws);
@@ -325,12 +346,21 @@ extern "C" int b2c_conv_backward_filter(const b2c_conv_desc* d, const float* x, 
     }
     return B2C_OK;
   }
-  if (use_staged(d, B2C_OP_BACKWARD_FILTER) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy)) & 15u) == 0)
+  if (route >= B2C_WGRAD_ROUTE_STAGED_3X3 && route <= B2C_WGRAD_ROUTE_STAGED_1X1_PLANE)
     return launch_conv_tc_wgrad_stg(s, x, dy, dw, ws, ws_bytes, st);
-  if (tc_conv_supported(s, B2C_OP_BACKWARD_FILTER) && d->algo != B2C_ALGO_SIMT)
+  if (route != B2C_WGRAD_ROUTE_SIMT)   // the gather kernel or the TMA-fed 1x1 kernel, with or without compaction (conv_tc_wgrad.cu)
     return launch_conv_tc(s, B2C_OP_BACKWARD_FILTER, gather_math(d), x, dy, nullptr, dw, ws, ws_bytes, nullptr, st);
   note_simt_fallback(d, B2C_OP_BACKWARD_FILTER);
   return launch_conv_wgrad_simt(s, x, dy, dw, st);
+}
+
+extern "C" int b2c_debug_wgrad_plan(const b2c_conv_desc* d, int* out, int n) {
+  if (!d || !out || n < 6) return fail(B2C_ERR_INVALID, "b2c_debug_wgrad_plan: need a descriptor and 6 ints");
+  const int route = wgrad_route(d, true, true, true);
+  WgradPlanInfo q;
+  tc_wgrad_plan_info(d->s, route, &q);
+  out[0] = route; out[1] = q.splits; out[2] = q.kb_per_split; out[3] = (int)q.nkb; out[4] = q.cols; out[5] = q.bpi;
+  return B2C_OK;
 }
 
 namespace b2c {

@@ -51,6 +51,15 @@ struct ConvShape {
   bool is_1x1;             // k=1, s=1, p=0 on every axis (base_conv_layer.cpp:99-103)
 };
 
+// A weight-gradient kernel's split-K plan as b2c_debug_wgrad_plan reports it: split i walks K blocks
+// [i * kb_per_split, min(nkb, (i + 1) * kb_per_split)); bpi = K blocks per image (0: blocks run over the flattened pixels).
+struct WgradPlanInfo {
+  int splits, kb_per_split;
+  long long nkb;
+  int cols, bpi, taps;
+  bool plane;
+};
+
 }  // namespace b2c
 
 struct b2c_conv_desc {

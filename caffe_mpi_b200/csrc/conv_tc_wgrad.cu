@@ -555,7 +555,7 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
   }
 }
 
-struct WgradPlan { int n_tile, splits, kb_per_split; };
+struct WgradPlan { int n_tile, splits, kb_per_split; long long nkb; };
 
 static WgradPlan wgrad_plan(const ConvShape& s) {
   WgradPlan pl;
@@ -573,6 +573,7 @@ static WgradPlan wgrad_plan(const ConvShape& s) {
   splits = (nkb + per - 1) / per;
   pl.splits = (int)splits;
   pl.kb_per_split = (int)per;
+  pl.nkb = nkb;
   return pl;
 }
 
@@ -634,6 +635,7 @@ static WgradPlan wgrad_tma_plan(const ConvShape& s, int* cpi_out) {
   const long long per = (nkb + splits - 1) / splits;
   pl.splits = (int)((nkb + per - 1) / per);
   pl.kb_per_split = (int)per;
+  pl.nkb = nkb;
   if (cpi_out) *cpi_out = cpi;
   return pl;
 }
@@ -763,26 +765,52 @@ static int launch_wgrad_n(const WgradParams& p, int G, int math, bool x1, cudaSt
   return x1 ? launch_wgrad_inst<N_TILE, false, true>(p, G, st) : launch_wgrad_inst<N_TILE, false, false>(p, G, st);
 }
 
+// The kernel launch_conv_tc_wgrad runs, decided in one place for the launch and for b2c_debug_wgrad_plan.  x_ok / dy_ok: the
+// operands are 16-byte aligned (the TMA maps need it); ws_ok: a 16-byte aligned workspace, which holds the compacted X.
+int tc_wgrad_route(const ConvShape& s, int math, bool x_ok, bool dy_ok, bool ws_ok) {
+  if (math == B2C_MATH_FP32 && wgrad_tma_shape_ok(s) && x_ok && dy_ok) return B2C_WGRAD_ROUTE_TMA_1X1;
+  if (math == B2C_MATH_FP32 && wgrad_compact_shape_ok(s) && dy_ok && ws_ok)
+    return tc_wgrad_stg_supported(wgrad_compact_dense_shape(s)) ? B2C_WGRAD_ROUTE_COMPACT_STAGED : B2C_WGRAD_ROUTE_COMPACT_TMA;
+  return B2C_WGRAD_ROUTE_GATHER;
+}
+
+bool tc_wgrad_stg_plan_info(const ConvShape& s, WgradPlanInfo* q);
+// the plan the planner of `route`'s kernel makes for s (compaction routes: for the dense 1x1 problem)
+void tc_wgrad_plan_info(const ConvShape& s, int route, WgradPlanInfo* q) {
+  *q = WgradPlanInfo{};
+  const bool compact = route == B2C_WGRAD_ROUTE_COMPACT_STAGED || route == B2C_WGRAD_ROUTE_COMPACT_TMA;
+  const ConvShape d = compact ? wgrad_compact_dense_shape(s) : s;
+  if (route == B2C_WGRAD_ROUTE_TMA_1X1 || route == B2C_WGRAD_ROUTE_COMPACT_TMA) {
+    int cpi = 0;
+    const WgradPlan pl = wgrad_tma_plan(d, &cpi);
+    q->splits = pl.splits; q->kb_per_split = pl.kb_per_split; q->nkb = pl.nkb; q->cols = pl.n_tile; q->bpi = cpi; q->taps = 1;
+  } else if (route == B2C_WGRAD_ROUTE_GATHER) {
+    const WgradPlan pl = wgrad_plan(d);
+    q->splits = pl.splits; q->kb_per_split = pl.kb_per_split; q->nkb = pl.nkb; q->cols = pl.n_tile; q->taps = s.kh * s.kw;
+  } else if (route != B2C_WGRAD_ROUTE_CAFFE && route != B2C_WGRAD_ROUTE_SIMT) {
+    tc_wgrad_stg_plan_info(d, q);
+  }
+}
+
 int launch_conv_tc_wgrad(const ConvShape& s, int math, const float* x, const float* dy, float* dw, void* ws,
                          size_t ws_bytes, cudaStream_t st) {
-  if (math == B2C_MATH_FP32 && wgrad_tma_shape_ok(s) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy)) & 15u) == 0)
-    return launch_conv_tc_wgrad_tma(s, x, dy, dw, ws, ws_bytes, st);
-  if (math == B2C_MATH_FP32 && wgrad_compact_shape_ok(s) && (reinterpret_cast<uintptr_t>(dy) & 15u) == 0 && ws) {
+  auto aligned = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; };
+  const int route = tc_wgrad_route(s, math, aligned(x), aligned(dy), ws && aligned(ws));
+  if (route == B2C_WGRAD_ROUTE_TMA_1X1) return launch_conv_tc_wgrad_tma(s, x, dy, dw, ws, ws_bytes, st);
+  if (route == B2C_WGRAD_ROUTE_COMPACT_STAGED || route == B2C_WGRAD_ROUTE_COMPACT_TMA) {
     const ConvShape d = wgrad_compact_dense_shape(s);
     const WgradPlan pt = wgrad_tma_plan(d, nullptr);
-    const bool staged = tc_wgrad_stg_supported(d);
+    const bool staged = route == B2C_WGRAD_ROUTE_COMPACT_STAGED;
     const size_t part = staged ? tc_wgrad_stg_workspace(d) : pt.splits > 1 ? WG_COUNTER_BYTES + sizeof(float) * (size_t)pt.splits * s.O * s.C : 0;
     const size_t xoff = (part + 255) & ~(size_t)255;
     const size_t xbytes = sizeof(float) * (size_t)s.N * s.C * s.Ho * s.Wo;
     if (ws_bytes < xoff + xbytes) return fail(B2C_ERR_WORKSPACE, "wgrad (compact): workspace too small");
-    float* xc = reinterpret_cast<float*>(static_cast<char*>(ws) + xoff);       // cudaMalloc'ed workspace: 256-byte aligned base
-    if ((reinterpret_cast<uintptr_t>(xc) & 15u) == 0) {
-      const long long planes = (long long)s.N * s.C;
-      subsample_kernel<<<grid_for((size_t)(planes * s.Ho * s.Wo), 256), 256, 0, st>>>(x, xc, planes, s.H, s.W, s.Ho, s.Wo, s.sh, s.sw);
-      B2C_POST_LAUNCH();
-      if (staged) return launch_conv_tc_wgrad_stg(d, xc, dy, dw, ws, part, st);
-      return launch_conv_tc_wgrad_tma(d, xc, dy, dw, ws, part, st);
-    }
+    float* xc = reinterpret_cast<float*>(static_cast<char*>(ws) + xoff);       // 16-byte aligned: ws is, xoff is a multiple of 256
+    const long long planes = (long long)s.N * s.C;
+    subsample_kernel<<<grid_for((size_t)(planes * s.Ho * s.Wo), 256), 256, 0, st>>>(x, xc, planes, s.H, s.W, s.Ho, s.Wo, s.sh, s.sw);
+    B2C_POST_LAUNCH();
+    if (staged) return launch_conv_tc_wgrad_stg(d, xc, dy, dw, ws, part, st);
+    return launch_conv_tc_wgrad_tma(d, xc, dy, dw, ws, part, st);
   }
   const WgradPlan pl = wgrad_plan(s);
   WgradParams p;

@@ -503,6 +503,13 @@ static bool wstg_plan(const ConvShape& s, WstgPlan* pl) {
 }
 constexpr size_t WSTG_COUNTER_BYTES = 1024;
 bool tc_wgrad_stg_supported(const ConvShape& s) { return wstg_plan(s, nullptr); }
+bool tc_wgrad_stg_plan_info(const ConvShape& s, WgradPlanInfo* q) {
+  WstgPlan pl;
+  if (!wstg_plan(s, &pl)) return false;
+  q->splits = pl.splits; q->kb_per_split = pl.kb_per_split; q->nkb = pl.nkb;
+  q->cols = pl.cn * pl.T; q->bpi = pl.bpi; q->taps = pl.T; q->plane = pl.plane;
+  return true;
+}
 size_t tc_wgrad_stg_workspace(const ConvShape& s) {
   WstgPlan pl;
   if (!wstg_plan(s, &pl)) return 0;

@@ -285,6 +285,26 @@ int b2c_sgd_update_arena(int nseg, const size_t* offset, const size_t* count,
 int b2c_debug_mbar_timeouts(unsigned int* out, int cap_words);
 int b2c_debug_mbar_set_trap(int on);
 
+/* The kernel b2c_conv_backward_filter runs for a descriptor (b2c_debug_wgrad_plan out[0]). */
+typedef enum {
+  B2C_WGRAD_ROUTE_CAFFE = 0,             /* engine CAFFE: per-image im2col + b2c_sgemm                                   */
+  B2C_WGRAD_ROUTE_SIMT = 1,              /* FFMA direct kernel                                                           */
+  B2C_WGRAD_ROUTE_GATHER = 2,            /* implicit-GEMM gather kernel (3xTF32, or TF32 in that math mode)              */
+  B2C_WGRAD_ROUTE_STAGED_3X3 = 3,        /* TMA-staged bf16x3 kernel, 3x3 / pad 1: 8 channels x 9 taps per tile          */
+  B2C_WGRAD_ROUTE_STAGED_3X3_PLANE = 4,  /* the same on 7x7 maps, one image per K block                                  */
+  B2C_WGRAD_ROUTE_STAGED_1X1 = 5,        /* TMA-staged bf16x3 kernel, 1x1                                                */
+  B2C_WGRAD_ROUTE_STAGED_1X1_PLANE = 6,  /* the same on 7x7 maps                                                         */
+  B2C_WGRAD_ROUTE_TMA_1X1 = 7,           /* TMA-fed 3xTF32 1x1 kernel                                                    */
+  B2C_WGRAD_ROUTE_COMPACT_STAGED = 8,    /* strided 1x1: X subsampled into the workspace, then the staged 1x1 kernel     */
+  B2C_WGRAD_ROUTE_COMPACT_TMA = 9        /* strided 1x1: X subsampled, then the TMA-fed 1x1 kernel                       */
+} b2c_wgrad_route;
+/* Which weight-gradient route b2c_conv_backward_filter takes for this descriptor with 16-byte-aligned x / dy (and workspace),
+ * and its split-K plan: out[0] route (b2c_wgrad_route), [1] splits, [2] K blocks per split, [3] K blocks in total,
+ * [4] tile columns (channels x taps, or N_TILE), [5] K blocks per image (0 where the route has no per-image blocking).
+ * For the compaction routes the plan is that of the dense 1x1 problem; the CAFFE and SIMT routes report zeros.
+ * Needs n >= 6.  Pure host computation: splits follow the current device's SM count (132 without a device). */
+int b2c_debug_wgrad_plan(const b2c_conv_desc* d, int* out, int n);
+
 #define B2C_UNIQUE_ID_BYTES 128
 int b2c_comm_get_unique_id(void* id_out /* B2C_UNIQUE_ID_BYTES */);
 int b2c_comm_init(int nranks, int rank, const void* id, b2c_comm** out);

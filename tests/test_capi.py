@@ -46,6 +46,28 @@ def test_output_shape_and_workspace():
     assert d1.workspace_bytes(capi.OP_FORWARD) == 0
 
 
+def test_wgrad_plan_routes():
+    """b2c_debug_wgrad_plan is host-only: the route choice of b2c_conv_backward_filter, with or without a device"""
+    def plan(N, Cin, H, W, O, k, s=1, p=0, d=1, G=1, engine=capi.ENGINE_DEFAULT, math=None, algo=None):
+        return m.ConvDesc(m.ConvParams.make(N, Cin, H, W, O, k, s, p, d, G, False), engine, math, algo).wgrad_plan()
+    assert plan(8, 16, 16, 16, 32, 3, p=1)["route"] == "staged_3x3"
+    assert plan(8, 16, 7, 7, 32, 3, p=1)["route"] == "staged_3x3_plane"
+    assert plan(8, 16, 7, 7, 32, 1)["route"] == "staged_1x1_plane"
+    assert plan(8, 16, 8, 8, 32, 1)["route"] == "staged_1x1"
+    assert plan(8, 16, 6, 6, 32, 1)["route"] == "tma_1x1"
+    assert plan(8, 16, 16, 16, 32, 1, s=2)["route"] == "compact_staged"
+    assert plan(8, 16, 12, 12, 136, 1, s=2)["route"] == "compact_tma"
+    assert plan(8, 16, 12, 12, 96, 1, s=2)["route"] == "gather"
+    assert plan(8, 18, 7, 7, 32, 3, p=1)["route"] == "gather"                       # plane mode needs C % 4 == 0
+    assert plan(8, 16, 16, 16, 32, 3, p=1, math=capi.MATH_TF32)["route"] == "gather"
+    assert plan(8, 16, 16, 16, 32, 3, p=1, algo=capi.ALGO_SIMT)["route"] == "simt"
+    assert plan(8, 16, 16, 16, 32, 3, p=1, engine=capi.ENGINE_CAFFE)["route"] == "caffe"
+    q = plan(8, 16, 16, 16, 32, 3, p=1)
+    assert (q["cols"], q["bpi"], q["nkb"]) == (72, 4, 32) and q["per"] * (q["splits"] - 1) < q["nkb"] <= q["per"] * q["splits"]
+    d = m.ConvDesc(m.ConvParams.make(1, 3, 8, 8, 4, 3))
+    assert m.lib().b2c_debug_wgrad_plan(d._h, (C.c_int * 5)(), 5) == -1
+
+
 def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():
