@@ -469,4 +469,94 @@ long long b2h_trainer_database_batches(void* hv) {
 }
 long long b2h_trainer_activation_floats(void* hv) { return (long long)static_cast<TrainerHandle*>(hv)->net->activation_floats(); }
 
+// ---- TEST-phase net (TrainNet over a Net filtered for TEST): forward only, scored like tools/caffe.cpp test() -------------------
+struct TesterHandle {
+  std::unique_ptr<Net> desc;
+  std::unique_ptr<TrainNet> net;
+};
+void* b2h_tester_create(const char* net_src, int net_is_text, int batch, int num_classes, unsigned long long seed, int math, int def_channels,
+                        int def_size) {
+  try {
+    auto* h = new TesterHandle;
+    PMessage nm = net_is_text ? ParseTextProto(net_src) : ParseTextProtoFile(net_src);
+    h->desc.reset(new Net(nm, TEST, batch, def_channels, def_size));
+    h->net.reset(new TrainNet(*h->desc, SolverParameter(), num_classes, seed, math));
+    return h;
+  } catch (const std::exception& e) { g_err = e.what(); return nullptr; }
+}
+void b2h_tester_destroy(void* hv) { delete static_cast<TesterHandle*>(hv); }
+int b2h_tester_copy_from(void* hv, const char* model_path, int* copied) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({ *copied = h->net->CopyTrainedLayersFrom(model_path); });
+}
+// the trainer handle must outlive the tester: the tester reads the trainer's parameter blobs
+int b2h_tester_share_from(void* hv, void* trainer) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({ h->net->ShareTrainedLayersWith(*static_cast<TrainerHandle*>(trainer)->net); });
+}
+int b2h_tester_forward(void* hv) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({ h->net->MarkParamsDirty(); h->net->ForwardTest(); CUDA_CHECK(cudaStreamSynchronize(Caffe::thread_stream())); });
+}
+int b2h_tester_num_outputs(void* hv) { return (int)static_cast<TesterHandle*>(hv)->net->outputs().size(); }
+int b2h_tester_output(void* hv, int i, char* name, int cap, float* loss_weight, long long* count) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({
+    const TrainNet::Output& o = h->net->outputs().at(i);
+    snprintf(name, cap, "%s", o.name.c_str());
+    *loss_weight = o.loss_weight;
+    *count = (long long)o.blob->count();
+  });
+}
+// per_batch: iterations x (sum of the output counts), output order; mean: one value per output element
+int b2h_tester_test(void* hv, int iterations, float* per_batch, float* mean, float* loss) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({
+    vector<float> pb;
+    vector<float> m;
+    *loss = h->net->Test(iterations, &pb, &m);
+    memcpy(per_batch, pb.data(), sizeof(float) * pb.size());
+    memcpy(mean, m.data(), sizeof(float) * m.size());
+  });
+}
+long long b2h_tester_blob_count(void* hv, const char* name) {
+  Blob* b = static_cast<TesterHandle*>(hv)->net->blob(name);
+  return b ? (long long)b->count() : -1;
+}
+int b2h_tester_blob(void* hv, const char* name, int set, float* buf) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({
+    Blob* b = h->net->blob(name);
+    B2_CHECK(b != nullptr, std::string("no blob named ") + name);
+    if (set) memcpy(b->mutable_cpu_data(), buf, sizeof(float) * b->count());
+    else memcpy(buf, b->cpu_data(), sizeof(float) * b->count());
+  });
+}
+int b2h_tester_has_solver(void* hv) { return static_cast<TesterHandle*>(hv)->net->has_solver() ? 1 : 0; }
+int b2h_tester_num_layers(void* hv) { return static_cast<TesterHandle*>(hv)->net->num_layers(); }
+int b2h_tester_layer(void* hv, int i, char* name, char* type, int len) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({ snprintf(name, len, "%s", h->net->layer_name(i).c_str()); snprintf(type, len, "%s", h->net->layer_type(i).c_str()); });
+}
+int b2h_tester_timed_forwards(void* hv, int n, float* ms) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({ *ms = h->net->TimedForwards(n); });
+}
+// per layer mean forward ms over n profiled forwards (b2h_trainer_profile's layout, op 0 only)
+int b2h_tester_profile(void* hv, int n, int cap, int* layer, float* ms, int* count) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  B2H_TRY({
+    std::vector<int> l;
+    std::vector<int> o;
+    std::vector<float> m;
+    h->net->ProfileForwards(n, &l, &o, &m);
+    *count = (int)l.size();
+    for (int i = 0; i < *count && i < cap; ++i) { layer[i] = l[i]; ms[i] = m[i]; }
+  });
+}
+long long b2h_tester_database_batches(void* hv) {
+  DataLayer* d = static_cast<TesterHandle*>(hv)->net->database_layer();
+  return d ? (long long)d->batches_loaded() : -1;
+}
+
 }  // extern "C"

@@ -8,7 +8,7 @@
 
 namespace caffe {
 
-DataLayer::DataLayer(const NetLayer& L, uint64_t seed) : LayerBase(L.param), L_(L), seed_(seed) {}
+DataLayer::DataLayer(const NetLayer& L, uint64_t seed, bool train) : LayerBase(L.param), L_(L), seed_(seed), train_(train) {}
 
 DataLayer::~DataLayer() {
   if (copy_stream_) cudaStreamSynchronize(copy_stream_);
@@ -104,12 +104,13 @@ void DataLayer::EnsureStarted() {
   p.parser_threads = (size_t)parsers_;
   p.force_encoded_color = L_.force_encoded_color;
   p.host_crop = host_crop_ ? L_.crop_size : 0;
+  p.train = train_;
   reader_.reset(new DataReader(p));
   B2_CHECK(reader_->channels() == C_ && reader_->height() == Hd_ && reader_->width() == Wd_, "database changed shape between set-up and start");
   // random_seed >= 0: "Use random_seed setting for deterministic transformations" (data_transformer.cpp:733-736); otherwise every
   // solver gets its own stream (the reference: Caffe::next_seed() of a solver seeded with seed + rank, parallel.cpp:179-187)
   const uint64_t s = L_.transform_random_seed >= 0 ? (uint64_t)L_.transform_random_seed : seed_ + 0x9E3779B9ull * (uint64_t)(solver_rank_ + 1);
-  draws_.reset(new TransformDraws(s, L_.mirror, L_.crop_size, /*train=*/true));
+  draws_.reset(new TransformDraws(s, L_.mirror, L_.crop_size, train_));
   for (int s = 0; s < (int)slot_.size(); ++s) HandToReader(s);   // slot k assembles batch k, k + K, k + 2K, ...
 }
 

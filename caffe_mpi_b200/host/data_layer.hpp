@@ -22,8 +22,9 @@ namespace caffe {
 
 class DataLayer : public LayerBase {
  public:
-  // `seed` feeds the crop / mirror stream when transform_param.random_seed is unset (the reference draws Caffe::next_seed())
-  DataLayer(const NetLayer& L, uint64_t seed);
+  // `seed` feeds the crop / mirror stream when transform_param.random_seed is unset (the reference draws Caffe::next_seed());
+  // train = false (TEST phase): the centre crop window
+  DataLayer(const NetLayer& L, uint64_t seed, bool train = true);
   ~DataLayer() override;
   const char* type() const override { return "Data"; }
   void LayerSetUp(const vector<Blob*>& bottom, const vector<Blob*>& top) override;
@@ -65,6 +66,7 @@ class DataLayer : public LayerBase {
   int parsers_ = 1;
   NetLayer L_;
   uint64_t seed_;
+  bool train_;
   int solver_count_ = 1, solver_rank_ = 0;
   int N_ = 0, C_ = 0, Hd_ = 0, Wd_ = 0, crop_h_ = 0, crop_w_ = 0;
   size_t u8_bytes_ = 0;

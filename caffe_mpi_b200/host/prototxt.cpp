@@ -183,6 +183,7 @@ size_t Net::learnable_count() const { size_t c = 0; for (auto& p : params_) c +=
 
 Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channels, int default_size) {
   name_ = np.str("name");
+  phase_ = phase;
   reduce_buckets_ = (int)np.integer("reduce_buckets", 6);          // caffe.proto:140
   global_grad_scale_ = (float)np.num("global_grad_scale", 1.0);    // caffe.proto:130
   if (!np.all("layers").empty()) Fatal(__FILE__, __LINE__, "V1 'layers' prototxt: run upgrade_net_proto_text first (not on this path)");

@@ -88,6 +88,7 @@ class Net {
   Net(const PMessage& net_param, Phase phase, int batch_override = 0, int default_channels = 3, int default_size = 224);
   static Net FromFile(const std::string& path, Phase phase, int batch_override = 0);
   const std::string& name() const { return name_; }
+  Phase phase() const { return phase_; }
   const std::vector<NetLayer>& layers() const { return layers_; }
   const std::map<std::string, std::vector<int>>& blob_shapes() const { return shapes_; }
   const std::vector<int>& top_shape(int layer, int top = 0) const { return layer_top_shapes_[layer][top]; }
@@ -98,6 +99,7 @@ class Net {
   size_t learnable_count() const;
  private:
   std::string name_;
+  Phase phase_ = TRAIN;
   std::vector<NetLayer> layers_;
   std::map<std::string, std::vector<int>> shapes_;
   std::vector<std::vector<std::vector<int>>> layer_top_shapes_;

@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <cstring>
 #include <cstdlib>
+#include <set>
 
 namespace caffe {
 
@@ -40,11 +41,19 @@ void BatchNormLayer::LayerSetUp(const vector<Blob*>& b, const vector<Blob*>&) {
 void BatchNormLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
   if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]);
   const int C = b[0]->shape(1);
-  if (!(recompute_ && t[0] != b[0])) xnorm_.ReshapeLike(*b[0]);
+  if (!test_ && !(recompute_ && t[0] != b[0])) xnorm_.ReshapeLike(*b[0]);
   save_mean_.Reshape({C}); save_invstd_.Reshape({C}); scratch_.Reshape({2 * C});
 }
 void BatchNormLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   const int N = b[0]->shape(0), C = b[0]->shape(1), Sp = (int)(b[0]->count() / ((size_t)N * C));
+  if (test_) {
+    // TEST: normalise with the running statistics (batch_norm_layer.cu:22-34), [+ the residual tail's other operand], [ReLU]
+    B2C_CHECK(b2c_bn_forward_inference(N, C, Sp, b[0]->gpu_data(), scale_bias_ ? blobs_[3]->gpu_data() : nullptr,
+                                       scale_bias_ ? blobs_[4]->gpu_data() : nullptr, eps_, blobs_[0]->gpu_data(), blobs_[1]->gpu_data(),
+                                       res_sum_ ? res_other_->gpu_data() : nullptr,
+                                       res_sum_ ? res_sum_->mutable_gpu_data() : t[0]->mutable_gpu_data(), res_sum_ || fuse_relu_ ? 1 : 0, S()));
+    return;
+  }
   if (res_sum_) {
     // residual tail: sum_top = max(0, BatchNorm(x) + other); this layer's own top blob is not materialised
     B2C_CHECK(b2c_bn_forward_train_fused_res(N, C, Sp, b[0]->gpu_data(), scale_bias_ ? blobs_[3]->gpu_data() : nullptr,
@@ -218,6 +227,11 @@ void LRNLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, cons
                              b[0]->mutable_gpu_diff(), S()));
 }
 void DropoutLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  if (test_) {                               // TEST: the identity (dropout_layer.cu); no mask is drawn and the stream offset stays
+    if (t[0] != b[0])
+      CUDA_CHECK(cudaMemcpyAsync(t[0]->mutable_gpu_data(), b[0]->gpu_data(), sizeof(float) * b[0]->count(), cudaMemcpyDeviceToDevice, S()));
+    return;
+  }
   B2C_CHECK(b2c_dropout_mask(b[0]->count(), ratio_, seed_, offset_, mask_.mutable_gpu_data(), S()));
   offset_ += b[0]->count();
   B2C_CHECK(b2c_mul(b[0]->count(), b[0]->gpu_data(), mask_.gpu_data(), t[0]->mutable_gpu_data(), S()));
@@ -375,8 +389,8 @@ void SyntheticDataLayer::IssueCopy(int s) {
     const unsigned r0 = (unsigned)(splitmix64(seed_ + base) >> 33) + 1, r1 = (unsigned)(splitmix64(seed_ + base + 1) >> 33) + 1,
                    r2 = (unsigned)(splitmix64(seed_ + base + 2) >> 33) + 1;
     mir[i] = (tf_.mirror && (r0 % 2)) ? 1 : 0;
-    sl.host_off[i] = (int)(r1 % (unsigned)(hd_ - tf_.crop + 1));
-    sl.host_off[N + i] = (int)(r2 % (unsigned)(wd_ - tf_.crop + 1));
+    sl.host_off[i] = tf_.train ? (int)(r1 % (unsigned)(hd_ - tf_.crop + 1)) : (hd_ - tf_.crop) / 2;
+    sl.host_off[N + i] = tf_.train ? (int)(r2 % (unsigned)(wd_ - tf_.crop + 1)) : (wd_ - tf_.crop) / 2;
   }
   ++draws_;
   CUDA_CHECK(cudaMemcpyAsync(sl.dev_u8, host_u8_, u8_bytes_, cudaMemcpyHostToDevice, copy_stream_));
@@ -388,6 +402,7 @@ void SyntheticDataLayer::IssueCopy(int s) {
 // ================================================================================================ TrainNet
 TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, uint64_t seed, int math) {
   name_ = net.name();
+  test_ = net.phase() == TEST;
   Caffe::set_random_seed(seed);
   std::map<string, bool> need;
   vector<ParamSpec> specs;
@@ -409,7 +424,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
     if (type == "Data" && L.use_database) {
       // data_param.source opened: the layer reads it (parser threads -> pinned batch -> device transform), data_layer.hpp
       B2_CHECK(db_data_ == nullptr && data_ == nullptr, "TrainNet: one data source per net");
-      auto* d = new DataLayer(L, seed);
+      auto* d = new DataLayer(L, seed, !test_);
       layer.reset(d);
       db_data_ = d;
       db_data_node_ = (int)layers_.size();
@@ -417,7 +432,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       vector<vector<int>> shapes;
       for (size_t t = 0; t < L.param.top.size(); ++t) shapes.push_back(net.top_shape((int)li, (int)t));
       SyntheticDataLayer::Transform tf;
-      tf.on = L.has_transform; tf.mirror = L.mirror; tf.crop = L.crop_size; tf.scale = L.transform_scale; tf.mean_value = L.mean_value;
+      tf.on = L.has_transform; tf.mirror = L.mirror; tf.train = !test_; tf.crop = L.crop_size; tf.scale = L.transform_scale; tf.mean_value = L.mean_value;
       auto* d = new SyntheticDataLayer(L.param, shapes, num_classes, seed, tf);
       layer.reset(d);
       data_ = d;
@@ -427,7 +442,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       layer = LayerRegistry::CreateLayer(lp);
     } else if (type == "ReLU") layer.reset(new ReLULayer(L.param, L.relu_slope));
     else if (type == "BatchNorm") {
-      auto* bn = new BatchNormLayer(L.param, L.bn_scale_bias, L.bn_eps, L.bn_maf);
+      auto* bn = new BatchNormLayer(L.param, L.bn_scale_bias, L.bn_eps, L.bn_maf, test_);
       if (L.bn_has_scale_filler) bn->set_scale_filler(L.bn_scale_filler);      // batch_norm_layer.cpp:52-63
       if (L.bn_has_bias_filler) bn->set_bias_filler(L.bn_bias_filler);
       layer.reset(bn);
@@ -449,7 +464,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       B2_CHECK(L.lrn_region == 0, "TrainNet: LRN WITHIN_CHANNEL is not built (the BASELINE nets use ACROSS_CHANNELS)");
       layer.reset(new LRNLayer(L.param, L.lrn_size, L.lrn_alpha, L.lrn_beta, L.lrn_k));
     }
-    else if (type == "Dropout") layer.reset(new DropoutLayer(L.param, L.dropout_ratio, seed * 0x100000001B3ull + li));
+    else if (type == "Dropout") layer.reset(new DropoutLayer(L.param, L.dropout_ratio, seed * 0x100000001B3ull + li, test_));
     else if (type == "Concat") {
       B2_CHECK(L.concat_axis == 1, "TrainNet: Concat is built for the channel axis only");
       layer.reset(new ConcatLayer(L.param));
@@ -477,7 +492,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       nb |= bneed;
     }
     for (int k = 0; k < node.num_params; ++k) nb |= specs[node.first_param + k].lr_mult != 0.f;
-    if (layer.get() == data_ || type == "Accuracy") nb = false;      // Accuracy: forward-only metric (accuracy_layer.hpp: "cannot backpropagate")
+    if (layer.get() == data_ || type == "Accuracy" || test_) nb = false;      // Accuracy: forward-only metric (accuracy_layer.hpp: "cannot backpropagate")
     node.need_backward = nb;
     for (auto& tn : L.param.top) need[tn] = nb;
     if (type == "SoftmaxWithLoss") loss_blob_ = node.top[0];
@@ -509,7 +524,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
         if (relu && !(nodes_[i + 1].bottom[0] == nodes_[i].top[0] && nodes_[i + 1].top[0] == nodes_[i].top[0] && relu->negative_slope() == 0.f))
           relu = nullptr;
       }
-      if (bn && out_of_place) {
+      if (bn && (out_of_place || test_)) {           // (TEST: the inference kernel also runs in place)
         bn->set_fusion(true, relu != nullptr);
         bn->Reshape(nodes_[i].bottom, nodes_[i].top);
         if (relu) relu->set_fused_away(true);
@@ -544,7 +559,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
   // among the producers of the sum's bottoms takes over the sum and the ReLU in both directions (csrc/layers_fused.cu, *_res): its
   // top is not materialised, four passes over a block-output-sized tensor go away per block and step.  Conditions: the
   // BatchNorm's top has no other consumer, nothing between it and the sum rewrites the other operand, the sum is the first
-  // backward writer of both bottoms (no shadow diffs).
+  // backward writer of both bottoms (no shadow diffs).  A TEST net has no backward: there only the first two conditions apply.
   {
     const char* e = getenv("B2C_FUSE");
     const char* er = getenv("B2C_FUSE_RES");
@@ -552,7 +567,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
     for (size_t i = 0; fuse_res && i < layers_.size(); ++i) {
       auto* el = dynamic_cast<EltwiseLayer*>(layers_[i].get());
       Node& en = nodes_[i];
-      if (!el || !el->fuse_relu() || en.bottom.size() != 2 || !en.need_backward) continue;
+      if (!el || !el->fuse_relu() || en.bottom.size() != 2 || (!test_ && !en.need_backward)) continue;
       if (!en.accumulate_bottom.empty() || en.bottom_diff_tmp[0] || en.bottom_diff_tmp[1]) continue;
       int prod[2] = {-1, -1};
       for (int k = 0; k < 2; ++k)
@@ -561,14 +576,14 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       if (prod[0] < 0 || prod[1] < 0 || prod[0] == prod[1]) continue;
       const int k = prod[0] > prod[1] ? 0 : 1, j = prod[k];
       auto* bn = dynamic_cast<BatchNormLayer*>(layers_[j].get());
-      if (!bn || !bn->recompute() || bn->fuse_relu() || nodes_[j].top[0] == nodes_[j].bottom[0] || !en.propagate_down[k]) continue;
+      if (!bn || !bn->recompute() || bn->fuse_relu() || nodes_[j].top[0] == nodes_[j].bottom[0] || (!test_ && !en.propagate_down[k])) continue;
       int consumers = 0;
       for (size_t l = 0; l < nodes_.size(); ++l)
         for (Blob* bb : nodes_[l].bottom) if (bb == en.bottom[k]) ++consumers;
       bool other_rewritten = false;
       for (size_t l = (size_t)j + 1; l < i; ++l) {       // ... nor reads it (its backward would add into a diff this layer has yet to write)
         for (Blob* tb : nodes_[l].top) if (tb == en.bottom[1 - k]) other_rewritten = true;
-        for (Blob* bb : nodes_[l].bottom) if (bb == en.bottom[1 - k]) other_rewritten = true;
+        if (!test_) for (Blob* bb : nodes_[l].bottom) if (bb == en.bottom[1 - k]) other_rewritten = true;
       }
       if (consumers != 1 || other_rewritten) continue;
       bn->set_residual(en.bottom[1 - k], en.top[0], en.propagate_down[1 - k]);
@@ -595,12 +610,28 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       }
     }
   }
-  solver_.reset(new SGDSolver(sp));
-  solver_->SetParams(learnable_, specs);
+  if (!test_) {
+    solver_.reset(new SGDSolver(sp));
+    solver_->SetParams(learnable_, specs);
+  }
   for (auto& l : layers_)
     if (auto* c = dynamic_cast<ConvolutionLayer*>(l.get()))
       if (c->EnableFilterCache()) cached_convs_.push_back(c);
-  sched_.reset(new ReduceScheduler(solver_.get(), nullptr));
+  if (!test_) sched_.reset(new ReduceScheduler(solver_.get(), nullptr));
+  // output blobs and loss weights (Net::Init, net.cpp: available_blobs; Layer::SetLossWeights, LossLayer::LayerSetUp)
+  {
+    std::set<string> available;
+    std::map<string, float> weight;
+    for (const NetLayer& L : net.layers()) {
+      for (auto& bn : L.param.bottom) available.erase(bn);
+      const bool loss = L.param.type.size() >= 4 && L.param.type.compare(L.param.type.size() - 4, 4, "Loss") == 0;
+      for (size_t t = 0; t < L.param.top.size(); ++t) {
+        available.insert(L.param.top[t]);
+        weight[L.param.top[t]] = t < L.loss_weight.size() ? L.loss_weight[t] : (loss && t == 0 ? 1.f : 0.f);
+      }
+    }
+    for (const string& n : available) outputs_.push_back({n, blobs_[n].get(), weight[n]});
+  }
   CUDA_CHECK(cudaStreamSynchronize(S()));
 }
 TrainNet::~TrainNet() {}
@@ -709,10 +740,13 @@ float TrainNet::TimedSteps(int n, bool copy_input, bool read_loss) {
   return ms;
 }
 void TrainNet::ProfileSteps(int n, vector<int>* layer, vector<int>* op, vector<float>* ms) {
+  Profile(n, [this] { Step(false); }, layer, op, ms);
+}
+void TrainNet::Profile(int n, const std::function<void()>& iteration, vector<int>* layer, vector<int>* op, vector<float>* ms) {
   EventProfiler prof;
   CUDA_CHECK(cudaDeviceSynchronize());
   Caffe::set_profiler(&prof);
-  try { for (int i = 0; i < n; ++i) Step(false); } catch (...) { Caffe::set_profiler(nullptr); throw; }
+  try { for (int i = 0; i < n; ++i) iteration(); } catch (...) { Caffe::set_profiler(nullptr); throw; }
   Caffe::set_profiler(nullptr);
   std::map<std::pair<int, int>, float> acc;
   prof.collect(&acc);
@@ -789,5 +823,74 @@ void TrainNet::Restore(const string& state_path) {
     if (auto* bn = dynamic_cast<BatchNormLayer*>(l.get())) bn->set_iter(st.iter + 1);   // running statistics are warm
 }
 float TrainNet::last_loss() { return loss_blob_ ? loss_blob_->cpu_data()[0] : 0.f; }
+
+// ---- TEST phase --------------------------------------------------------------------------------------------------------
+void TrainNet::ShareTrainedLayersWith(TrainNet& train) {
+  B2_CHECK(test_, "ShareTrainedLayersWith: only a TEST-phase net takes another net's parameters");
+  CUDA_CHECK(cudaStreamSynchronize(S()));
+  for (size_t i = 0; i < layers_.size(); ++i) {
+    size_t k = 0;
+    while (k < train.layer_names_.size() && train.layer_names_[k] != layer_names_[i]) ++k;
+    if (k == train.layer_names_.size() || train.layers_[k]->blobs().empty()) continue;     // "Ignoring source layer" (net.cpp)
+    auto& src = train.layers_[k]->blobs();
+    auto& dst = layers_[i]->blobs();
+    B2_CHECK(src.size() == dst.size(), "Incompatible number of blobs for layer " + layer_names_[i]);
+    for (size_t j = 0; j < src.size(); ++j) {
+      B2_CHECK(src[j]->shape() == dst[j]->shape(), "Cannot share param " + std::to_string(j) + " weights from layer '" + layer_names_[i] +
+                                                       "'; shape mismatch.  Source param shape is " + src[j]->shape_string() +
+                                                       "; target param shape is " + dst[j]->shape_string());
+      dst[j] = src[j];
+      learnable_[nodes_[i].first_param + j] = src[j];
+    }
+  }
+  filters_dirty_ = true;
+}
+void TrainNet::ForwardTest() {
+  B2_CHECK(test_, "ForwardTest: the net was built for the TRAIN phase");
+  if (db_data_) db_data_->LoadBatch(nodes_[db_data_node_].top, S());   // every TEST forward reads the next batch
+  Forward(false);
+}
+float TrainNet::Test(int iterations, vector<float>* per_batch, vector<float>* mean) {
+  B2_CHECK(iterations > 0, "Test: iterations must be positive");
+  filters_dirty_ = true;          // shared weights change under this net between calls: never score on a stale filter cache
+  size_t width = 0;
+  for (const Output& o : outputs_) width += o.blob->count();
+  per_batch->clear();
+  vector<float> sum(width, 0.f);
+  float loss = 0.f;
+  for (int i = 0; i < iterations; ++i) {
+    ForwardTest();
+    float iter_loss = 0.f;
+    size_t idx = 0;
+    for (const Output& o : outputs_) {
+      const float* v = o.blob->cpu_data();
+      for (size_t k = 0; k < o.blob->count(); ++k, ++idx) {
+        per_batch->push_back(v[k]);
+        sum[idx] += v[k];                                   // tools/caffe.cpp:272-289: float sums, then / iterations
+        iter_loss += o.loss_weight * v[k];                  // Layer::Forward's loss: loss_weight . top
+      }
+    }
+    loss += iter_loss;
+  }
+  mean->resize(width);
+  for (size_t k = 0; k < width; ++k) (*mean)[k] = sum[k] / iterations;
+  return loss / iterations;
+}
+float TrainNet::TimedForwards(int n) {
+  cudaEvent_t a, b;
+  CUDA_CHECK(cudaEventCreate(&a)); CUDA_CHECK(cudaEventCreate(&b));
+  CUDA_CHECK(cudaStreamSynchronize(S()));
+  CUDA_CHECK(cudaEventRecord(a, S()));
+  for (int i = 0; i < n; ++i) ForwardTest();
+  CUDA_CHECK(cudaEventRecord(b, S()));
+  CUDA_CHECK(cudaEventSynchronize(b));
+  float ms = 0.f;
+  CUDA_CHECK(cudaEventElapsedTime(&ms, a, b));
+  cudaEventDestroy(a); cudaEventDestroy(b);
+  return ms;
+}
+void TrainNet::ProfileForwards(int n, vector<int>* layer, vector<int>* op, vector<float>* ms) {
+  Profile(n, [this] { ForwardTest(); }, layer, op, ms);
+}
 
 }  // namespace caffe

@@ -28,7 +28,9 @@ class ReLULayer : public LayerBase {
 
 class BatchNormLayer : public LayerBase {      // NVCaffe BatchNorm with scale_bias (batch_norm_layer.cpp)
  public:
-  BatchNormLayer(const LayerParameter& p, bool scale_bias, float eps, float maf) : LayerBase(p), scale_bias_(scale_bias), eps_(eps), maf_(maf) {
+  // test: the TEST phase -- normalise with the running statistics (b2c_bn_forward_inference), never write blobs 0-4
+  BatchNormLayer(const LayerParameter& p, bool scale_bias, float eps, float maf, bool test = false)
+      : LayerBase(p), scale_bias_(scale_bias), eps_(eps), maf_(maf), test_(test) {
     scale_filler_.type = "constant"; scale_filler_.value = 1.f;
   }
   void set_scale_filler(const FillerParameter& f) { scale_filler_ = f; }
@@ -44,6 +46,7 @@ class BatchNormLayer : public LayerBase {      // NVCaffe BatchNorm with scale_b
   FillerParameter scale_filler_, bias_filler_;
   bool fuse_relu_ = false;   // an in-place ReLU on the top blob is folded into this layer's kernels (TrainNet's fusion pass)
   bool recompute_ = false;   // do not store x_norm: backward recomputes it from the bottom blob (needs top != bottom)
+  bool test_;
   int iter_ = 0;
  public:
   void set_iter(int i) { iter_ = i; }
@@ -135,9 +138,9 @@ class LRNLayer : public LayerBase {            // ACROSS_CHANNELS only (the BASE
   Blob scale_;
 };
 
-class DropoutLayer : public LayerBase {        // TRAIN phase: y = x * mask, mask in {0, 1/(1-ratio)}
+class DropoutLayer : public LayerBase {        // TRAIN phase: y = x * mask, mask in {0, 1/(1-ratio)}; TEST phase: y = x
  public:
-  DropoutLayer(const LayerParameter& p, float ratio, uint64_t seed) : LayerBase(p), ratio_(ratio), seed_(seed) {}
+  DropoutLayer(const LayerParameter& p, float ratio, uint64_t seed, bool test = false) : LayerBase(p), ratio_(ratio), seed_(seed), test_(test) {}
   const char* type() const override { return "Dropout"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]); mask_.ReshapeLike(*b[0]); }
  protected:
@@ -145,6 +148,7 @@ class DropoutLayer : public LayerBase {        // TRAIN phase: y = x * mask, mas
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
   float ratio_;
   uint64_t seed_, offset_ = 0;
+  bool test_;
   Blob mask_;
 };
 
@@ -195,7 +199,8 @@ class AccuracyLayer : public LayerBase {       // forward only (accuracy_layer.c
 //     values, scale) into the float data blob.
 class SyntheticDataLayer : public LayerBase {
  public:
-  struct Transform { bool on = false, mirror = false; int crop = 0; float scale = 1.f; vector<float> mean_value; };
+  // train = false (TEST phase): the centre crop window instead of a random one (data_transformer.cpp:219-229)
+  struct Transform { bool on = false, mirror = false, train = true; int crop = 0; float scale = 1.f; vector<float> mean_value; };
   SyntheticDataLayer(const LayerParameter& p, const vector<vector<int>>& shapes, int num_classes, uint64_t seed, const Transform& tf)
       : LayerBase(p), shapes_(shapes), classes_(num_classes), seed_(seed), tf_(tf) {}
   const char* type() const override { return "Data"; }
@@ -237,6 +242,10 @@ class SyntheticDataLayer : public LayerBase {
   void IssueCopy(int s);
 };
 
+// A Net built with phase TEST makes a forward-only instance (the reference's test net, net.cpp / tools/caffe.cpp test()): no
+// SGDSolver, ReduceScheduler or parameter arena, no backward bookkeeping, BatchNorm on its running statistics, Dropout the identity,
+// Data layers on the centre crop window.  Its parameters come from a .caffemodel (CopyTrainedLayersFrom) or are the blobs of a TRAIN
+// instance (ShareTrainedLayersWith), and Test() scores it.
 class TrainNet {
  public:
   TrainNet(const Net& net, const SolverParameter& sp, int num_classes, uint64_t seed, int math);
@@ -272,6 +281,22 @@ class TrainNet {
   // Net::CopyTrainedLayersFrom (net.cpp): layers matched by name, blob shapes must agree; returns the number of layers copied
   int CopyTrainedLayersFrom(const string& caffemodel_path);
   const string& name() const { return name_; }
+  bool test_phase() const { return test_; }
+  bool has_solver() const { return solver_ != nullptr; }
+  // ---- TEST phase only ----
+  // Net::ShareTrainedLayersWith (net.cpp): a layer matched by name takes `train`'s parameter blobs by pointer (shapes must agree), so
+  // this net reads the weights and BatchNorm statistics the trainer keeps updating.  `train` must outlive this net.
+  void ShareTrainedLayersWith(TrainNet& train);
+  // Net::output_blobs (Net::Init's available_blobs: tops no later layer consumes, in name order) with their loss weights: the layer's
+  // loss_weight, else 1 for a loss layer's first top and 0 otherwise
+  struct Output { string name; Blob* blob; float loss_weight; };
+  const vector<Output>& outputs() const { return outputs_; }
+  void ForwardTest();                              // one forward: the database's next batch (when the net reads one), then every layer
+  // tools/caffe.cpp test(): `iterations` forwards on freshly prepared filter caches; per_batch gets every output element of every
+  // batch (iterations x sum of output counts), mean their means; returns the mean loss (sum of loss_weight * output per batch)
+  float Test(int iterations, vector<float>* per_batch, vector<float>* mean);
+  float TimedForwards(int n);                      // n ForwardTest calls bracketed by CUDA events; milliseconds
+  void ProfileForwards(int n, vector<int>* layer, vector<int>* op, vector<float>* ms);   // ProfileSteps for ForwardTest
  private:
   struct Node {
     vector<Blob*> bottom, top;
@@ -285,10 +310,13 @@ class TrainNet {
   void Forward(bool copy_input);
   void Backward(bool update);
   void PrepareFilters();                           // b2c_conv_prepare_filters over every cached conv layer (weights changed)
+  void Profile(int n, const std::function<void()>& iteration, vector<int>* layer, vector<int>* op, vector<float>* ms);
  public:
   void MarkParamsDirty() { filters_dirty_ = true; } // call after writing parameter data behind the net's back
  private:
   bool filters_dirty_ = true;
+  bool test_ = false;                              // built from a TEST-phase Net: forward only
+  vector<Output> outputs_;
   bool fuse_fanout_ = true;                        // B2C_FUSE: conv layers add their bottom gradient into a fan-out blob's diff directly
   vector<ConvolutionLayer*> cached_convs_;
   float host_loss_ = 0.f;

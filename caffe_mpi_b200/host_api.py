@@ -463,3 +463,108 @@ class Trainer:
         if getattr(self, "_h", None) and _lib is not None:
             _lib.b2h_trainer_destroy(self._h)
             self._h = None
+
+
+# ---------------------------------------------------------------------------------------------- TEST-phase net
+class Tester:
+    """A TEST-phase net (the prototxt filtered for phase TEST) run forward only: BatchNorm on its running statistics, Dropout the
+    identity, Data layers on the centre crop window.  Weights come from a .caffemodel (copy_trained_layers_from) or are shared with a
+    live Trainer (share_trained_layers_with), and test(k) scores k batches like the reference's `caffe test`."""
+
+    def __init__(self, net, batch=0, num_classes=1000, seed=1701, math=capi.MATH_FP32, net_is_text=True, default_channels=3,
+                 default_size=224):
+        L = lib()
+        vp, i = C.c_void_p, C.c_int
+        L.b2h_tester_create.restype = vp
+        L.b2h_tester_create.argtypes = [C.c_char_p, i, i, i, C.c_ulonglong, i, i, i]
+        for fn in ("b2h_tester_destroy", "b2h_tester_forward", "b2h_tester_num_outputs", "b2h_tester_has_solver", "b2h_tester_num_layers"):
+            getattr(L, fn).argtypes = [vp]
+        L.b2h_tester_copy_from.argtypes = [vp, C.c_char_p, C.POINTER(i)]
+        L.b2h_tester_share_from.argtypes = [vp, vp]
+        L.b2h_tester_output.argtypes = [vp, i, C.c_char_p, i, C.POINTER(C.c_float), C.POINTER(C.c_longlong)]
+        L.b2h_tester_test.argtypes = [vp, i, _f32, _f32, C.POINTER(C.c_float)]
+        L.b2h_tester_blob_count.argtypes = [vp, C.c_char_p]
+        L.b2h_tester_blob_count.restype = C.c_longlong
+        L.b2h_tester_blob.argtypes = [vp, C.c_char_p, i, _f32]
+        L.b2h_tester_layer.argtypes = [vp, i, C.c_char_p, C.c_char_p, i]
+        L.b2h_tester_timed_forwards.argtypes = [vp, i, C.POINTER(C.c_float)]
+        L.b2h_tester_profile.argtypes = [vp, i, i, C.POINTER(i), C.POINTER(C.c_float), C.POINTER(i)]
+        L.b2h_tester_database_batches.argtypes = [vp]
+        L.b2h_tester_database_batches.restype = C.c_longlong
+        self._trainer = None
+        self._h = L.b2h_tester_create(net.encode(), int(net_is_text), batch, num_classes, seed, math, default_channels, default_size)
+        if not self._h:
+            raise HostError(L.b2h_last_error().decode())
+
+    def copy_trained_layers_from(self, caffemodel_path):
+        """Net::CopyTrainedLayersFrom: layers matched by name; returns the number of layers copied."""
+        n = C.c_int()
+        _ck(lib().b2h_tester_copy_from(self._h, caffemodel_path.encode(), C.byref(n)))
+        return n.value
+
+    def share_trained_layers_with(self, trainer):
+        """Net::ShareTrainedLayersWith: read `trainer`'s parameter blobs (and BatchNorm statistics) in place from now on."""
+        _ck(lib().b2h_tester_share_from(self._h, trainer._h))
+        self._trainer = trainer                    # the shared blobs live in the trainer's arena
+
+    def forward(self):
+        _ck(lib().b2h_tester_forward(self._h))
+
+    def outputs(self):
+        """[(name, loss_weight, count)] of the net's output blobs, in the reference's (name) order."""
+        out = []
+        for i in range(lib().b2h_tester_num_outputs(self._h)):
+            nm, w, n = C.create_string_buffer(256), C.c_float(), C.c_longlong()
+            _ck(lib().b2h_tester_output(self._h, i, nm, 256, C.byref(w), C.byref(n)))
+            out.append((nm.value.decode(), w.value, n.value))
+        return out
+
+    def test(self, iterations):
+        """(per_batch [iterations x output elements], means [output elements], mean loss), like tools/caffe.cpp test()."""
+        width = sum(n for _, _, n in self.outputs())
+        per_batch, mean, loss = np.empty(iterations * width, np.float32), np.empty(max(width, 1), np.float32), C.c_float()
+        _ck(lib().b2h_tester_test(self._h, iterations, per_batch, mean, C.byref(loss)))
+        return per_batch.reshape(iterations, width), mean[:width], loss.value
+
+    def get_blob(self, name):
+        n = lib().b2h_tester_blob_count(self._h, name.encode())
+        if n < 0:
+            raise HostError("no blob " + name)
+        out = np.empty(n, np.float32)
+        _ck(lib().b2h_tester_blob(self._h, name.encode(), 0, out))
+        return out
+
+    def set_blob(self, name, arr):
+        _ck(lib().b2h_tester_blob(self._h, name.encode(), 1, np.ascontiguousarray(arr, np.float32).reshape(-1)))
+
+    def has_solver(self):
+        return bool(lib().b2h_tester_has_solver(self._h))
+
+    def layers(self):
+        out = []
+        for i in range(lib().b2h_tester_num_layers(self._h)):
+            a, b = C.create_string_buffer(256), C.create_string_buffer(256)
+            _ck(lib().b2h_tester_layer(self._h, i, a, b, 256))
+            out.append((a.value.decode(), b.value.decode()))
+        return out
+
+    def timed_forwards(self, n):
+        """n TEST forwards bracketed by CUDA events on the net's stream -> milliseconds."""
+        v = C.c_float()
+        _ck(lib().b2h_tester_timed_forwards(self._h, n, C.byref(v)))
+        return v.value
+
+    def profile(self, n=2):
+        """[(layer index, mean forward ms)] over n forwards, CUDA events around every layer call."""
+        cap = 8192
+        la, ms, cnt = (C.c_int * cap)(), (C.c_float * cap)(), C.c_int()
+        _ck(lib().b2h_tester_profile(self._h, n, cap, la, ms, C.byref(cnt)))
+        return [(la[i], float(ms[i])) for i in range(min(cnt.value, cap))]
+
+    def database_batches(self):
+        return lib().b2h_tester_database_batches(self._h)
+
+    def __del__(self):
+        if getattr(self, "_h", None) and _lib is not None:
+            _lib.b2h_tester_destroy(self._h)
+            self._h = None

@@ -221,6 +221,16 @@ int b2c_bn_forward_train_fused_res(int N, int C, int S, const float* x, const fl
 int b2c_bn_backward_fused_res(int N, int C, int S, const float* d_sum, const float* d_sum2, const float* y_sum, const float* x,
                               const float* save_mean, const float* save_invstd, const float* gamma, const float* beta,
                               float* dgamma, float* dbeta, float* dx, float* d_residual, void* stream);
+/* BatchNormLayer TEST phase (batch_norm_layer.cu:22-34 and stage 2, :80-90), one elementwise launch (csrc/bn_infer.cu):
+ *   y = [ReLU]( bn_y(bn_xn(x, running_mean[c], invstd[c]), gamma[c], beta[c]) [+ residual] ),  invstd[c] = 1 / sqrtf(running_var[c] + eps).
+ * DOUBLE eps: running_var already holds variance + eps (the TRAIN kernels fold eps in before the running average, as the reference's
+ * CAFFE engine does, batch_norm_layer.cpp:183-186), and the TEST branch adds eps again (powx(var + eps, -0.5)); this reproduces both.
+ * gamma/beta null <=> scale_bias false.  residual (may be null): the other bottom of an Eltwise SUM fed by this layer.  relu: the
+ * in-place ReLU after the layer (or after the sum).  Bit-identical to this entry point without relu / residual followed by
+ * b2c_relu_forward (slope 0), b2c_add or b2c_add_relu.  y may alias x.  Writes y only; the running statistics are read-only. */
+int b2c_bn_forward_inference(int N, int C, int S, const float* x, const float* gamma, const float* beta, float eps,
+                             const float* running_mean, const float* running_var, const float* residual, float* y, int relu,
+                             void* stream);
 /* AccuracyLayer::Forward (accuracy_layer.cpp:44-100), labels as float class ids, ties ranked like the reference's
  * std::greater<pair<score, index>>; `scratch`: 4 bytes of device memory. */
 int b2c_accuracy(int N, int C, int top_k, const float* scores, const float* labels, float* accuracy, void* scratch, void* stream);

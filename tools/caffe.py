@@ -8,6 +8,7 @@ source stands in (SURVEY 8d).  B2C_DATA=db makes a missing database fatal, as in
          [--snapshot=<solverstate to resume from>] [--weights=<caffemodel to fine-tune from>] [--snapshot_prefix=P]
   python -m torch.distributed.run --nproc-per-node N ... tools/caffe.py train --solver=...              (N GPUs, one rank each)
   python tools/caffe.py time --model=models/resnet50/train_val.prototxt [--iterations=50] [--batch=B]
+  python tools/caffe.py test --model=models/resnet50/train_val.prototxt --weights=x.caffemodel [--iterations=50] [--batch=B]   (1 GPU)
   python tools/caffe.py device_query
 """
 import argparse, os, sys, time
@@ -194,9 +195,40 @@ def cmd_time(args):
         log("*** Benchmark ends ***")
 
 
+def score_lines(outputs, per_batch, means, loss):
+    """The log lines of `caffe test` (tools/caffe.cpp:261-299): `outputs` = [(name, loss_weight, count)] in the net's output order,
+    `per_batch` = [iterations][output elements], `means` = [output elements], `loss` = the mean loss."""
+    names, weights = [], []
+    for name, w, n in outputs:
+        names += [name] * n
+        weights += [w] * n
+    lines = ["Batch %d, %s = %g" % (i, names[k], v) for i, row in enumerate(per_batch) for k, v in enumerate(row)]
+    lines.append("Loss: %g" % loss)
+    for k, m in enumerate(means):
+        lines.append("%s = %g%s" % (names[k], m, " (* %g = %g loss)" % (weights[k], weights[k] * m) if weights[k] else ""))
+    return lines
+
+
+def cmd_test(args):
+    from caffe_mpi_b200 import host_api
+    if not args.model:
+        sys.exit("caffe.py test: Need a model definition to score.")
+    if not args.weights:
+        sys.exit("caffe.py test: Need model weights to score.")
+    if int(os.environ.get("WORLD_SIZE", 1)) > 1:
+        sys.exit("caffe.py test: scoring runs on one GPU (start it without torch.distributed)")
+    t = host_api.Tester(args.model, batch=args.batch, num_classes=args.classes, seed=1701 if args.seed < 0 else args.seed, net_is_text=False)
+    t.copy_trained_layers_from(args.weights)
+    iters = args.iterations or 50
+    log("Running for %d iterations." % iters)
+    per_batch, means, loss = t.test(iters)
+    for ln in score_lines(t.outputs(), per_batch, means, loss):
+        log(ln)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-    ap.add_argument("command", choices=["train", "time", "device_query"])
+    ap.add_argument("command", choices=["train", "test", "time", "device_query"])
     ap.add_argument("--solver", "-solver", default="")
     ap.add_argument("--model", "-model", default="")
     ap.add_argument("--iterations", "-iterations", type=int, default=0)
@@ -205,10 +237,10 @@ def main():
     ap.add_argument("--display", type=int, default=0, help="iterations between loss lines (default: the solver file's `display`)")
     ap.add_argument("--seed", type=int, default=-1, help="default: the solver file's random_seed, else 1701")
     ap.add_argument("--snapshot", "-snapshot", default="", help="solver state (.solverstate) to resume training from")
-    ap.add_argument("--weights", "-weights", default="", help="pretrained weights (.caffemodel) to fine-tune from")
+    ap.add_argument("--weights", "-weights", default="", help="pretrained weights (.caffemodel) to fine-tune from, or to score (test)")
     ap.add_argument("--snapshot_prefix", default="", help="write <prefix>_iter_<N>.caffemodel/.solverstate after the last iteration")
     args = ap.parse_args()
-    {"train": cmd_train, "time": cmd_time, "device_query": cmd_device_query}[args.command](args)
+    {"train": cmd_train, "test": cmd_test, "time": cmd_time, "device_query": cmd_device_query}[args.command](args)
 
 
 if __name__ == "__main__":
