@@ -47,41 +47,6 @@ int sm_count() {
 static std::atomic<int> g_default_math{B2C_MATH_FP32};
 static std::atomic<int> g_default_algo{B2C_ALGO_AUTO};
 
-// kernels in the other translation units
-int launch_im2col2d(const float*, int, int, int, int, int, int, int, int, int, int, int, float*, cudaStream_t);
-int launch_col2im2d(const float*, int, int, int, int, int, int, int, int, int, int, int, float*, cudaStream_t);
-int launch_sgemm_simt(bool, bool, int, int, int, float, const float*, int, const float*, int, float, float*, int,
-                      cudaStream_t);
-int launch_conv_fwd_simt(const ConvShape&, const float*, const float*, const float*, float*, cudaStream_t);
-int launch_conv_dgrad_simt(const ConvShape&, const float*, const float*, float*, cudaStream_t);
-int launch_conv_wgrad_simt(const ConvShape&, const float*, const float*, float*, cudaStream_t);
-int launch_bias_add(int, int, int, const float*, float*, cudaStream_t);
-int launch_bias_grad(int, int, int, const float*, float*, cudaStream_t);
-// tensor-core family (conv_tc*.cu)
-bool tc_conv_supported(const ConvShape&, int op);
-size_t tc_conv_workspace(const ConvShape&, int op, int math);
-int launch_conv_tc(const ConvShape&, int op, int math, const float* a, const float* b, const float* bias, float* out,
-                   void* ws, size_t ws_bytes, const void* prepared, cudaStream_t);
-void tc_conv_prep_entry(const ConvShape&, int op, int math, const float* w, void* dst, PrepEntry* q);
-bool tc_stg_prep_entry(const ConvShape&, int op, const float* w, void* dst, PrepEntry* q);
-// bulk-copy-staged bf16x3 kernel (conv_tc_stg.cu): forward / dgrad of stride-1 "same" convolutions
-bool tc_stg_supported(const ConvShape&, int op);
-size_t tc_stg_workspace(const ConvShape&, int op);
-int launch_conv_tc_stg(const ConvShape&, int op, const float* a, const float* w, const float* bias, float* out, void* ws,
-                       size_t ws_bytes, const void* prepared, bool accumulate, cudaStream_t);
-// TMA-staged bf16x3 weight gradient (conv_tc_wgrad_stg.cu): stride-1 "same" convolutions with 1 or 9 taps
-bool tc_wgrad_stg_supported(const ConvShape&);
-size_t tc_wgrad_stg_workspace(const ConvShape&);
-int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t);
-bool tc_wgrad_stg_plan_info(const ConvShape&, WgradPlanInfo*);
-// weight-gradient route among the gather-family kernels (conv_tc_wgrad.cu) and its plan
-int tc_wgrad_route(const ConvShape&, int math, bool x_ok, bool dy_ok, bool ws_ok);
-void tc_wgrad_plan_info(const ConvShape&, int route, WgradPlanInfo*);
-bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K);
-size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K);
-int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const float* A, const float* B, float beta,
-                    float* C, int math, void* ws, size_t ws_bytes, cudaStream_t);
-
 static bool have_device() {
   static int ok = -1;
   if (ok < 0) {
@@ -126,9 +91,6 @@ static const void* prepared_filter(const b2c_conv_desc* d, int op) {
   const char* base = static_cast<const char*>(d->filter_cache);
   return op == B2C_OP_FORWARD ? base : base + cache_region_bytes(d, B2C_OP_FORWARD);
 }
-// true when `op` would take the staged kernel (so the cache holds the bf16 layout) but this call falls back to the gather
-// kernel because of unaligned activation pointers: the cache is then of no use to it
-static bool staged_geometry_only(const b2c_conv_desc* d, int op) { return use_staged(d, op); }
 
 // A layer of the implicit engine that no tensor-core kernel takes (K = C/g*kh*kw beyond the filter tile limit, a strided k > 1 data
 // gradient, ...) runs on the FFMA kernels: correct, an order of magnitude slower.  Say so instead of doing it silently -- the
@@ -267,8 +229,9 @@ extern "C" int b2c_conv_forward(const b2c_conv_desc* d, const float* x, const fl
   }
   if (use_staged(d, B2C_OP_FORWARD) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15u) == 0)
     return launch_conv_tc_stg(s, B2C_OP_FORWARD, x, w, bias, y, ws, ws_bytes, prepared_filter(d, B2C_OP_FORWARD), false, st);
+  // a staged layer that falls back here (unaligned activation pointers) has the staged kernel's bf16 layout in its cache: of no use
   if (tc_conv_supported(s, B2C_OP_FORWARD) && d->algo != B2C_ALGO_SIMT)
-    return launch_conv_tc(s, B2C_OP_FORWARD, gather_math(d), x, w, bias, y, ws, ws_bytes, staged_geometry_only(d, B2C_OP_FORWARD) ? nullptr : prepared_filter(d, B2C_OP_FORWARD), st);
+    return launch_conv_tc(s, B2C_OP_FORWARD, gather_math(d), x, w, bias, y, ws, ws_bytes, use_staged(d, B2C_OP_FORWARD) ? nullptr : prepared_filter(d, B2C_OP_FORWARD), st);
   note_simt_fallback(d, B2C_OP_FORWARD);
   return launch_conv_fwd_simt(s, x, w, bias, y, st);
 }
@@ -298,7 +261,7 @@ extern "C" int b2c_conv_backward_data(const b2c_conv_desc* d, const float* dy, c
   if (use_staged(d, B2C_OP_BACKWARD_DATA) && ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15u) == 0)
     return launch_conv_tc_stg(s, B2C_OP_BACKWARD_DATA, dy, w, nullptr, dx, ws, ws_bytes, prepared_filter(d, B2C_OP_BACKWARD_DATA), false, st);
   if (tc_conv_supported(s, B2C_OP_BACKWARD_DATA) && d->algo != B2C_ALGO_SIMT)
-    return launch_conv_tc(s, B2C_OP_BACKWARD_DATA, gather_math(d), dy, w, nullptr, dx, ws, ws_bytes, staged_geometry_only(d, B2C_OP_BACKWARD_DATA) ? nullptr : prepared_filter(d, B2C_OP_BACKWARD_DATA), st);
+    return launch_conv_tc(s, B2C_OP_BACKWARD_DATA, gather_math(d), dy, w, nullptr, dx, ws, ws_bytes, use_staged(d, B2C_OP_BACKWARD_DATA) ? nullptr : prepared_filter(d, B2C_OP_BACKWARD_DATA), st);
   note_simt_fallback(d, B2C_OP_BACKWARD_DATA);
   return launch_conv_dgrad_simt(s, dy, w, dx, st);
 }

@@ -60,6 +60,51 @@ struct WgradPlanInfo {
   bool plane;
 };
 
+// A B2C_* switch: atol of the variable, `dflt` when it is unset.  Switches are read once per process, into a function-local
+// `static const` (thread-safe initialisation).
+long env_int(const char* name, long dflt);
+
+// ---- kernels in the other translation units -----------------------------------------------------------------
+struct PrepEntry;
+int launch_im2col2d(const float*, int, int, int, int, int, int, int, int, int, int, int, float*, cudaStream_t);
+int launch_col2im2d(const float*, int, int, int, int, int, int, int, int, int, int, int, float*, cudaStream_t);
+int launch_sgemm_simt(bool, bool, int, int, int, float, const float*, int, const float*, int, float, float*, int,
+                      cudaStream_t);
+int launch_conv_fwd_simt(const ConvShape&, const float*, const float*, const float*, float*, cudaStream_t);
+int launch_conv_dgrad_simt(const ConvShape&, const float*, const float*, float*, cudaStream_t);
+int launch_conv_wgrad_simt(const ConvShape&, const float*, const float*, float*, cudaStream_t);
+int launch_bias_add(int, int, int, const float*, float*, cudaStream_t);
+int launch_bias_grad(int, int, int, const float*, float*, cudaStream_t);
+// tensor-core family (conv_tc*.cu)
+bool tc_conv_supported(const ConvShape&, int op);
+size_t tc_conv_workspace(const ConvShape&, int op, int math);
+int launch_conv_tc(const ConvShape&, int op, int math, const float* a, const float* b, const float* bias, float* out,
+                   void* ws, size_t ws_bytes, const void* prepared, cudaStream_t);
+void tc_conv_prep_entry(const ConvShape&, int op, int math, const float* w, void* dst, PrepEntry* q);
+bool tc_stg_prep_entry(const ConvShape&, int op, const float* w, void* dst, PrepEntry* q);
+// bulk-copy-staged bf16x3 kernel (conv_tc_stg.cu): forward / dgrad of stride-1 "same" convolutions
+bool tc_stg_supported(const ConvShape&, int op);
+size_t tc_stg_workspace(const ConvShape&, int op);
+int launch_conv_tc_stg(const ConvShape&, int op, const float* a, const float* w, const float* bias, float* out, void* ws,
+                       size_t ws_bytes, const void* prepared, bool accumulate, cudaStream_t);
+// gather-family weight gradient (conv_tc_wgrad.cu): the gather kernel, the TMA-fed 1x1 kernel, compaction of strided 1x1 layers
+bool tc_wgrad_supported(const ConvShape&);
+size_t tc_wgrad_workspace(const ConvShape&);
+int launch_conv_tc_wgrad(const ConvShape&, int math, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes,
+                         cudaStream_t);
+// weight-gradient route among the gather-family kernels and its plan
+int tc_wgrad_route(const ConvShape&, int math, bool x_ok, bool dy_ok, bool ws_ok);
+void tc_wgrad_plan_info(const ConvShape&, int route, WgradPlanInfo*);
+// TMA-staged bf16x3 weight gradient (conv_tc_wgrad_stg.cu): stride-1 "same" convolutions with 1 or 9 taps
+bool tc_wgrad_stg_supported(const ConvShape&);
+size_t tc_wgrad_stg_workspace(const ConvShape&);
+int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t);
+bool tc_wgrad_stg_plan_info(const ConvShape&, WgradPlanInfo*);
+bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K);
+size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K);
+int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const float* A, const float* B, float beta,
+                    float* C, int math, void* ws, size_t ws_bytes, cudaStream_t);
+
 }  // namespace b2c
 
 struct b2c_conv_desc {

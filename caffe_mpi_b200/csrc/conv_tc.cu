@@ -26,9 +26,7 @@
 // The activation operand is not TMA-staged: with NCHW the GEMM-K axis (c,i,j) is not unit-stride and
 // 7x7 maps have 196-byte channel pitches (TMA needs 16-byte multiples); see DESIGN.md.
 // fp32 math mode = 3 TF32 MMAs per K step (lo*hi, hi*lo, hi*hi); TF32 mode = 1.
-#include <cuda.h>
 #include <limits.h>
-#include <stdlib.h>
 #include <stdio.h>
 #include "b2c_common.cuh"
 #include "tc_common.cuh"
@@ -83,16 +81,6 @@ struct FwdSmem {
   static constexpr uint32_t TX_BYTES = B_STAGE;
   static_assert(STAGES >= 2, "shared memory budget");
 };
-
-__device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
 
 // KMODE 0: natural K order (c,i,j), per-element decode (any C/g).
 // KMODE 1 (C/g % 4 == 0): K order (c/4, i, j, c%4): a 16-byte chunk = 4 channels of one tap (one bounds check),
@@ -261,7 +249,7 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
         const int s = kbg % STAGES, it = kbg / STAGES;
         mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 40);
         if (elect_one()) {
-          mbar_arrive_expect_tx(bar_full + 8 * s, S::TX_BYTES);
+          arrive_expect_tx(bar_full + 8 * s, S::TX_BYTES);
           tma_load_3d(stage_b_hi(s), &map_hi, bar_full + 8 * s, kb * BK, n0, g);
           if (SPLIT) tma_load_3d(stage_b_lo(s), &map_lo, bar_full + 8 * s, kb * BK, n0, g);
         }
@@ -375,36 +363,6 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn encode_tiled() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(f);
-  }
-  return fn;
-}
-
-static int make_filter_map(CUtensorMap* map, const float* base, int Kp, int rows, int G, int n_tile) {
-  EncodeTiledFn enc = encode_tiled();
-  if (!enc) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)Kp, (cuuint64_t)rows, (cuuint64_t)G};
-  cuuint64_t strides[2] = {(cuuint64_t)Kp * 4, (cuuint64_t)Kp * 4 * (cuuint64_t)rows};
-  cuuint32_t box[3] = {32, (cuuint32_t)n_tile, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)r);
-  return B2C_OK;
-}
-
 template <int N_TILE, bool SPLIT, int KMODE>
 static int launch_fwd_inst(const FwdParams& p, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
   using S = FwdSmem<N_TILE, SPLIT>;
@@ -433,11 +391,6 @@ static int pick_n_tile(int Ntot) {
   if (Ntot > 32) return 64;
   return 32;
 }
-
-bool tc_wgrad_supported(const ConvShape& s);
-size_t tc_wgrad_workspace(const ConvShape& s);
-int launch_conv_tc_wgrad(const ConvShape& s, int math, const float* x, const float* dy, float* dw, void* ws,
-                         size_t ws_bytes, cudaStream_t st);
 
 static bool dgrad_as_fwd(const ConvShape& s) { return s.sh == 1 && s.sw == 1; }
 static bool dgrad_scatter(const ConvShape& s) { return s.kh == 1 && s.kw == 1 && s.ph == 0 && s.pw == 0 && (s.sh > 1 || s.sw > 1); }
@@ -515,37 +468,40 @@ int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const f
     }
   }
   p.Kp = padded_k(p.K);
-  static long long* prof_buf = nullptr;
-  static int prof_on = -1;
-  if (prof_on < 0) { const char* e = getenv("B2C_PROF"); prof_on = e ? atoi(e) : 0; if (prof_on) cudaMalloc(&prof_buf, 32 * sizeof(long long)); }
-  p.prof = prof_on ? prof_buf : nullptr;
-  { static int dbg = -1; if (dbg < 0) { const char* e = getenv("B2C_DBG"); dbg = e ? atoi(e) : 0; } p.dbg = dbg; }
+  static const int dbg = env_int("B2C_DBG", 0);
+  p.dbg = dbg;
   const int kmode = (p.Cg % 4 == 0) ? 1 : 0;
   if (!prepared)
     if (int rc = launch_filter_prep(&q, 1, st)) return rc;
 
   int n_tile = pick_n_tile(p.Ntot);
-  { static int force = -1; if (force < 0) { const char* e = getenv("B2C_NTILE"); force = e ? atoi(e) : 0; }
-    if ((force == 32 || force == 64 || force == 128) && force / 2 < p.Ntot) n_tile = force; }
+  static const int force = env_int("B2C_NTILE", 0);
+  if ((force == 32 || force == 64 || force == 128) && force / 2 < p.Ntot) n_tile = force;
   p.m_tiles = (p.Mtot + 127) / 128; p.n_tiles = (p.Ntot + n_tile - 1) / n_tile; p.G = s.G;
   p.total_tiles = p.m_tiles * p.n_tiles * p.G;
   alignas(64) CUtensorMap mh, ml;
-  if (int rc = make_filter_map(&mh, static_cast<const float*>(q.hi), p.Kp, q.rows, s.G, n_tile)) return rc;
-  if (int rc = make_filter_map(&ml, static_cast<const float*>(q.lo ? q.lo : q.hi), p.Kp, q.rows, s.G, n_tile)) return rc;
-  if (prof_on) {
-    cudaMemsetAsync(prof_buf, 0, 32 * sizeof(long long), st);
-    int rc = n_tile == 128 ? launch_fwd_n<128>(p, mh, ml, math, kmode, st) : n_tile == 64 ? launch_fwd_n<64>(p, mh, ml, math, kmode, st) : launch_fwd_n<32>(p, mh, ml, math, kmode, st);
+  const cuuint64_t dims[3] = {(cuuint64_t)p.Kp, (cuuint64_t)q.rows, (cuuint64_t)s.G};
+  const cuuint64_t strides[2] = {(cuuint64_t)p.Kp * 4, (cuuint64_t)p.Kp * 4 * (cuuint64_t)q.rows};
+  const cuuint32_t box[3] = {32, (cuuint32_t)n_tile, 1};
+  if (int rc = make_tensor_map_3d(&mh, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, q.hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "conv filter"))
+    return rc;
+  if (int rc = make_tensor_map_3d(&ml, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, q.lo ? q.lo : q.hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                                  "conv filter"))
+    return rc;
+  p.prof = prof_buffer(st);
+  int rc;
+  switch (n_tile) {
+    case 128: rc = launch_fwd_n<128>(p, mh, ml, math, kmode, st); break;
+    case 64: rc = launch_fwd_n<64>(p, mh, ml, math, kmode, st); break;
+    default: rc = launch_fwd_n<32>(p, mh, ml, math, kmode, st); break;
+  }
+  if (p.prof) {
     long long h[32];
-    cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
+    prof_read(p.prof, h);
     fprintf(stderr, "[prof] N_TILE=%d nkb=%d tiles=%d | producer(t0): total=%lld wait_empty=%lld store=%lld load=%lld blocks=%lld\n",
             n_tile, p.Kp / 32, p.total_tiles, h[0], h[1], h[2], h[3], h[4]);
-    return rc;
   }
-  switch (n_tile) {
-    case 128: return launch_fwd_n<128>(p, mh, ml, math, kmode, st);
-    case 64: return launch_fwd_n<64>(p, mh, ml, math, kmode, st);
-    default: return launch_fwd_n<32>(p, mh, ml, math, kmode, st);
-  }
+  return rc;
 }
 
 TC_DEBUG_EXPORT(debug_mbar_fwd)

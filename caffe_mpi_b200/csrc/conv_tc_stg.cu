@@ -34,10 +34,8 @@
 //     Tiles that span two images write the staged chunk with 16-byte st.global.
 //   * Plane mode (BWT < 128): 7x7 maps, whole image planes staged -- see Smem below.
 // dgrad of a stride-1 same convolution is the same kernel on dY with the transposed + flipped filter.
-#include <cuda.h>
 #include <cuda_bf16.h>
 #include <limits.h>
-#include <stdlib.h>
 #include <stdio.h>
 #include "b2c_common.cuh"
 #define B2C_MBAR_DEBUG 1     // this kernel records stuck mbarrier waits (tc_common.cuh)
@@ -119,12 +117,6 @@ struct Smem {
   static_assert(NSLOT >= 2, "a tile that spans two images needs two boxes per channel group");
 };
 
-__device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t smem_src, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2) : "memory");
@@ -134,29 +126,6 @@ __device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* map, uint32
   asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-template <int OFF>
-__device__ __forceinline__ float lds32(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(addr), "n"(OFF));
-  return v;
-}
-__device__ __forceinline__ void sts128u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-// fp32 pair (k even, k odd) -> packed bf16 hi word and packed bf16 lo word; element k sits in the LOW half
-// (two consecutive K elements per 32-bit word of the K-major operand tile, little endian)
-__device__ __forceinline__ void split_pack_bf16(float e, float o, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(e, o);            // .x = e (low half), .y = o
-  const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h);
-  const float he = __uint_as_float(hb << 16), ho = __uint_as_float(hb & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(e - he, o - ho);   // a - hi is exact in fp32
-  hi = hb;
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
 template <int N_TILE, int BWT>
 __global__ void __launch_bounds__(THREADS, 1)
 igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
@@ -273,10 +242,10 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
             const uint32_t src = src_base + (uint32_t)tapoff[tap];
             constexpr int CP = (int)S::PITCH;
             float v[16];
-            v[0] = lds32<0>(src); v[1] = lds32<CP>(src); v[2] = lds32<2 * CP>(src); v[3] = lds32<3 * CP>(src);
-            v[4] = lds32<4 * CP>(src); v[5] = lds32<5 * CP>(src); v[6] = lds32<6 * CP>(src); v[7] = lds32<7 * CP>(src);
-            v[8] = lds32<16 * CP>(src); v[9] = lds32<17 * CP>(src); v[10] = lds32<18 * CP>(src); v[11] = lds32<19 * CP>(src);
-            v[12] = lds32<20 * CP>(src); v[13] = lds32<21 * CP>(src); v[14] = lds32<22 * CP>(src); v[15] = lds32<23 * CP>(src);
+            v[0] = lds32i<0>(src); v[1] = lds32i<CP>(src); v[2] = lds32i<2 * CP>(src); v[3] = lds32i<3 * CP>(src);
+            v[4] = lds32i<4 * CP>(src); v[5] = lds32i<5 * CP>(src); v[6] = lds32i<6 * CP>(src); v[7] = lds32i<7 * CP>(src);
+            v[8] = lds32i<16 * CP>(src); v[9] = lds32i<17 * CP>(src); v[10] = lds32i<18 * CP>(src); v[11] = lds32i<19 * CP>(src);
+            v[12] = lds32i<20 * CP>(src); v[13] = lds32i<21 * CP>(src); v[14] = lds32i<22 * CP>(src); v[15] = lds32i<23 * CP>(src);
 #pragma unroll
             for (int o = 0; o < 2; ++o)
 #pragma unroll
@@ -506,72 +475,13 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
 
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-typedef CUresult (*StgEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static StgEncodeTiledFn stg_encode_tiled() {
-  static StgEncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<StgEncodeTiledFn>(f);
-  }
-  return fn;
-}
-static int stg_make_filter_map(CUtensorMap* map, const void* base, int Kp, int rows, int n_tile) {
-  StgEncodeTiledFn enc = stg_encode_tiled();
-  if (!enc) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)Kp, (cuuint64_t)rows, 1};
-  cuuint64_t strides[2] = {(cuuint64_t)Kp * 2, (cuuint64_t)Kp * 2 * (cuuint64_t)rows};
-  cuuint32_t box[3] = {64, (cuuint32_t)n_tile, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled (staged conv filter) failed (%d)", (int)r);
-  return B2C_OK;
-}
-
-// [N][rows][HW] fp32, box {bw, 32, 1}, no swizzle, out-of-range elements read as zero / are not written
-static int stg_make_act_map(CUtensorMap* map, const float* base, int HW, int rows, int N, int bw) {
-  StgEncodeTiledFn enc = stg_encode_tiled();
-  if (!enc) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)HW, (cuuint64_t)rows, (cuuint64_t)N};
-  cuuint64_t strides[2] = {(cuuint64_t)HW * 4, (cuuint64_t)HW * 4 * (cuuint64_t)rows};
-  cuuint32_t box[3] = {(cuuint32_t)bw, (cuuint32_t)stg::CB, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled (staged conv activations) failed (%d)", (int)r);
-  return B2C_OK;
-}
-
-// plane mode: the [N][C][HW] blob viewed as {4*HW, C/4, N}; box {4*HW, 8, 1} = 32 channels of one image
-static int stg_make_plane_map(CUtensorMap* map, const float* base, int HW, int C, int N) {
-  StgEncodeTiledFn enc = stg_encode_tiled();
-  if (!enc) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)HW * 4, (cuuint64_t)C / 4, (cuuint64_t)N};
-  cuuint64_t strides[2] = {(cuuint64_t)HW * 16, (cuuint64_t)HW * 4 * (cuuint64_t)C};
-  cuuint32_t box[3] = {(cuuint32_t)HW * 4, (cuuint32_t)stg::CB / 4, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled (staged conv, plane mode) failed (%d)", (int)r);
-  return B2C_OK;
-}
-
 static bool stg_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B2C_CONV_STAGED"); on = e ? atoi(e) : 1; }
+  static const int on = env_int("B2C_CONV_STAGED", 1);
   return on != 0;
 }
 
 static bool stg_plane_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B2C_CONV_STAGED_PLANE"); on = e ? atoi(e) : 1; }
+  static const int on = env_int("B2C_CONV_STAGED_PLANE", 1);
   return on != 0;
 }
 
@@ -670,23 +580,40 @@ int launch_conv_tc_stg(const ConvShape& s, int op, const float* a, const float* 
   p.bias = op == B2C_OP_FORWARD ? bias : nullptr;
   p.out = out;
   p.accumulate = accumulate ? 1 : 0;
-  { static int dbg = -1; if (dbg < 0) { const char* e = getenv("B2C_STG_DBG"); dbg = e ? atoi(e) : 0; } p.dbg = dbg; }
+  static const int dbg = env_int("B2C_STG_DBG", 0);
+  p.dbg = dbg;
   const int n_tile = g.Cout > 64 ? 128 : g.Cout > 32 ? 64 : 32;
   p.m_tiles = (p.Mtot + 127) / 128; p.n_tiles = (g.Cout + n_tile - 1) / n_tile; p.total_tiles = p.m_tiles * p.n_tiles;
-  static long long* prof_buf = nullptr;
-  static int prof_on = -1;
-  if (prof_on < 0) { const char* e = getenv("B2C_PROF"); prof_on = e ? atoi(e) : 0; if (prof_on) cudaMalloc(&prof_buf, 32 * sizeof(long long)); }
-  p.prof = prof_on ? prof_buf : nullptr;
-  if (prof_on) cudaMemsetAsync(prof_buf, 0, 32 * sizeof(long long), st);
+  p.prof = prof_buffer(st);
   alignas(64) CUtensorMap mh, ml, mx, my;
-  if (int rc = stg_make_filter_map(&mh, q.hi, g.Kp, g.Cout, n_tile)) return rc;
-  if (int rc = stg_make_filter_map(&ml, q.lo, g.Kp, g.Cout, n_tile)) return rc;
+  {
+    // filter: [Cout][Kp] bf16, box {64, N_TILE}, SWIZZLE_128B
+    const cuuint64_t dims[3] = {(cuuint64_t)g.Kp, (cuuint64_t)g.Cout, 1};
+    const cuuint64_t strides[2] = {(cuuint64_t)g.Kp * 2, (cuuint64_t)g.Kp * 2 * (cuuint64_t)g.Cout};
+    const cuuint32_t box[3] = {64, (cuuint32_t)n_tile, 1};
+    if (int rc = make_tensor_map_3d(&mh, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, q.hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "staged conv filter"))
+      return rc;
+    if (int rc = make_tensor_map_3d(&ml, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, q.lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "staged conv filter"))
+      return rc;
+  }
+  const cuuint64_t HW = (cuuint64_t)p.HW;
   if (g.bwt < 128) {
-    if (int rc = stg_make_plane_map(&mx, a, p.HW, g.Cin, s.N)) return rc;
+    // plane mode: the [N][C][HW] blob viewed as {4*HW, C/4, N}; box {4*HW, 8, 1} = 32 channels of one image
+    if (int rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a, {HW * 4, (cuuint64_t)g.Cin / 4, (cuuint64_t)s.N},
+                                    {HW * 16, HW * 4 * (cuuint64_t)g.Cin}, {(cuuint32_t)HW * 4, (cuuint32_t)stg::CB / 4, 1},
+                                    CU_TENSOR_MAP_SWIZZLE_NONE, "staged conv, plane mode"))
+      return rc;
     my = mx;                                                  // plane mode stores with st.global
   } else {
-    if (int rc = stg_make_act_map(&mx, a, p.HW, g.Cin, s.N, g.bwt)) return rc;
-    if (int rc = stg_make_act_map(&my, out, p.HW, g.Cout, s.N, 128)) return rc;
+    // [N][channels][HW] fp32, box {bw, 32, 1}, no swizzle
+    if (int rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a, {HW, (cuuint64_t)g.Cin, (cuuint64_t)s.N},
+                                    {HW * 4, HW * 4 * (cuuint64_t)g.Cin}, {(cuuint32_t)g.bwt, (cuuint32_t)stg::CB, 1},
+                                    CU_TENSOR_MAP_SWIZZLE_NONE, "staged conv activations"))
+      return rc;
+    if (int rc = make_tensor_map_3d(&my, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out, {HW, (cuuint64_t)g.Cout, (cuuint64_t)s.N},
+                                    {HW * 4, HW * 4 * (cuuint64_t)g.Cout}, {128, (cuuint32_t)stg::CB, 1},
+                                    CU_TENSOR_MAP_SWIZZLE_NONE, "staged conv activations"))
+      return rc;
   }
   int rc;
   switch (n_tile) {
@@ -694,9 +621,9 @@ int launch_conv_tc_stg(const ConvShape& s, int op, const float* a, const float* 
     case 64: rc = stg_launch_n<64>(g.bwt, p, mh, ml, mx, my, st); break;
     default: rc = stg_launch_n<32>(g.bwt, p, mh, ml, mx, my, st); break;
   }
-  if (rc == B2C_OK && prof_on) {
+  if (rc == B2C_OK && p.prof) {
     long long h[32];
-    cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
+    prof_read(p.prof, h);
     fprintf(stderr, "[stg-prof] N_TILE=%d BWT=%d nkb=%d groups=%d taps=%d tiles=%d | conv(t0): total=%lld kblocks=%lld | act-tma: wait_empty=%lld boxes=%lld\n",
             n_tile, g.bwt, g.nkb, g.groups, g.taps, p.total_tiles, h[0], h[3], h[4], h[5]);
     // CTA 0's consumer warpgroups, SM cycles: issue = total - wait_full - wait_order - mma_drain - epilogue (issuing MMAs, and

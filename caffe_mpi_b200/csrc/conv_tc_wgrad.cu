@@ -9,8 +9,7 @@
 // warpgroups (warps 0-7) issue wgmma from the two tiles and keep the fp32 accumulators in registers.  The
 // reduction is split across CTAs (grid.x); partial tiles go to a workspace and the tile's CTAs then add them
 // to dW in split order (splitk_fused_reduce; the reference accumulates image by image, also a fixed order).
-#include <cuda.h>
-#include <stdlib.h>
+#include <stdio.h>
 #include "b2c_common.cuh"
 #include "tc_common.cuh"
 
@@ -50,50 +49,6 @@ struct WgradSmem {
   static constexpr uint32_t PROM_OFF = TAB_OFF + TABLE;
   static constexpr uint32_t TOTAL = PROM_OFF + PROM_BYTES;
 };
-
-// ---- split-K reduction fused into the tile's own CTAs ---------------------------------------------------------------------
-// Round 1 ran a second kernel per layer (wgrad_reduce_kernel, 53 launches / 0.58 ms per ResNet-50 step).  Here the `splits` CTAs
-// of an output tile meet at a counter in the workspace once their partial tiles are in global memory -- the whole grid is one
-// wave by construction (wgrad_plan: never more CTAs than SMs), so every CTA of the tile is resident -- and then each CTA adds
-// up its 1/splits slice of the tile over the partials IN SPLIT ORDER and accumulates it into dW: the summation order of every
-// element is fixed, so the result is bit-reproducible and equal to what the separate kernel produced.
-__device__ __forceinline__ void splitk_fused_reduce(const float* __restrict__ part, float* __restrict__ dw, unsigned int* counter,
-                                                    int split, int splits, long long plane, long long tile_base, int ld, int nrows, int ncols) {
-  __syncthreads();                                   // this CTA's partial tile is complete (epilogue warps)
-  if (threadIdx.x == 0) {
-    __threadfence();
-    atomicAdd(counter, 1u);
-    const long long t0 = clock64();
-    unsigned int seen;
-    do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-      if (seen < (unsigned)splits) {
-        __nanosleep(64);
-        if (clock64() - t0 > tc::MBAR_TIMEOUT_CYCLES) asm volatile("trap;");
-      }
-    } while (seen < (unsigned)splits);
-  }
-  __syncthreads();
-  const int total = nrows * ncols;
-  const int per = (total + splits - 1) / splits;
-  const int e_end = min(total, (split + 1) * per);
-  for (int e = split * per + (int)threadIdx.x; e < e_end; e += (int)blockDim.x) {
-    const int r = e / ncols, c = e - r * ncols;
-    const long long idx = tile_base + (long long)r * ld + c;
-    // loads of 8 splits in flight, added in split order (the order, not the batching, fixes the rounding)
-    float acc = 0.0f;
-    int s2 = 0;
-    for (; s2 + 8 <= splits; s2 += 8) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = __ldcg(part + (long long)(s2 + u) * plane + idx);
-#pragma unroll
-      for (int u = 0; u < 8; ++u) acc += v[u];
-    }
-    for (; s2 < splits; ++s2) acc += __ldcg(part + (long long)s2 * plane + idx);
-    dw[idx] += acc;
-  }
-}
 
 template <int N_TILE, bool SPLIT, bool X1X1>
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -429,21 +384,6 @@ struct WgradTmaSmem {
   static constexpr uint32_t TOTAL = BAR_OFF + 256 + 1024;              // + 1024-byte alignment slack
 };
 
-__device__ __forceinline__ void wg_tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void wg_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ float4 wg_lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-
 template <int N_TILE>
 __global__ void __launch_bounds__(WT_THREADS, 1)
 wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_constant__ CUtensorMap map_dy,
@@ -489,7 +429,7 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
       const uint32_t src = stage_a(s);
 #pragma unroll 4
       for (int u = tid - NCONS * 32; u < UNITS; u += WT_CW * 32) {
-        const float4 v = wg_lds128(src + (uint32_t)u * 16u);
+        const float4 v = lds128(src + (uint32_t)u * 16u);
         float h, l0, l1, l2, l3;
         split_tf32(v.x, h, l0); split_tf32(v.y, h, l1); split_tf32(v.z, h, l2); split_tf32(v.w, h, l3);
         sts128(src + S::RAW_BYTES + (uint32_t)u * 16u, l0, l1, l2, l3);
@@ -505,9 +445,9 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
       const int s = kb % STAGES, it = kb / STAGES;
       mbar_wait_backoff(bar_empty + 8 * s, (it & 1) ^ 1, 20);
       if (elect_one()) {
-        wg_arrive_expect_tx(bar_raw + 8 * s, S::RAW_BYTES);
-        wg_tma_load_3d(stage_a(s), &map_dy, bar_raw + 8 * s, j * 32, m0, n);
-        wg_tma_load_3d(stage_b(s), &map_x, bar_raw + 8 * s, j * 32, n0, n);
+        arrive_expect_tx(bar_raw + 8 * s, S::RAW_BYTES);
+        tma_load_3d(stage_a(s), &map_dy, bar_raw + 8 * s, j * 32, m0, n);
+        tma_load_3d(stage_b(s), &map_x, bar_raw + 8 * s, j * 32, n0, n);
       }
       __syncwarp();
       if (++j == p.cpi) { j = 0; ++n; }
@@ -561,19 +501,9 @@ static WgradPlan wgrad_plan(const ConvShape& s) {
   WgradPlan pl;
   pl.n_tile = s.Kd > 32 ? 64 : 32;                  // 768 threads leave 80 registers: 32 accumulators per consumer thread
   const long long Q = (long long)s.N * s.Ho * s.Wo;
-  const long long nkb = (Q + BK - 1) / BK;
+  pl.nkb = (Q + BK - 1) / BK;
   const long long mn = (long long)((s.Og + 127) / 128) * ((s.Kd + pl.n_tile - 1) / pl.n_tile) * s.G;
-  // one wave: every CTA pays a fixed prologue + epilogue (partial tile write), so fewer, longer CTAs win;
-  // never exceed the SM count (a partial second wave costs a full CTA time)
-  long long splits = sm_count() / mn;
-  const long long max_splits = nkb / 8 > 0 ? nkb / 8 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  long long per = (nkb + splits - 1) / splits;
-  splits = (nkb + per - 1) / per;
-  pl.splits = (int)splits;
-  pl.kb_per_split = (int)per;
-  pl.nkb = nkb;
+  plan_splitk(pl.nkb, mn, 8, &pl.splits, &pl.kb_per_split);
   return pl;
 }
 
@@ -585,27 +515,19 @@ bool tc_wgrad_supported(const ConvShape& s) {
 }
 
 static WgradPlan wgrad_tma_plan(const ConvShape& s, int* cpi_out);
-// the TMA-staged bf16x3 kernel (conv_tc_wgrad_stg.cu): the dense 1x1 problem a compacted strided layer turns into goes there when it can
-bool tc_wgrad_stg_supported(const ConvShape&);
-size_t tc_wgrad_stg_workspace(const ConvShape&);
-int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t);
 static bool wgrad_tma_shape_ok(const ConvShape& s);
 static bool wgrad_compact_shape_ok(const ConvShape& s);
 static ConvShape wgrad_compact_dense_shape(const ConvShape& s);
-constexpr size_t WG_COUNTER_BYTES = 1024;      // arrival counters of the fused split-K reduction: one u32 per output tile (<= #SMs)
 size_t tc_wgrad_workspace(const ConvShape& s) {
-  const WgradPlan pl = wgrad_plan(s);
-  size_t need = pl.splits > 1 ? WG_COUNTER_BYTES + sizeof(float) * (size_t)pl.splits * s.O * s.Kd : 0;
+  size_t need = splitk_workspace_bytes(wgrad_plan(s).splits, (long long)s.O * s.Kd);
   if (wgrad_tma_shape_ok(s)) {                       // the TMA path of 1x1 layers plans its own split count
-    const WgradPlan pt = wgrad_tma_plan(s, nullptr);
-    const size_t nt = pt.splits > 1 ? WG_COUNTER_BYTES + sizeof(float) * (size_t)pt.splits * s.O * s.C : 0;
+    const size_t nt = splitk_workspace_bytes(wgrad_tma_plan(s, nullptr).splits, (long long)s.O * s.C);
     if (nt > need) need = nt;
   }
   if (wgrad_compact_shape_ok(s)) {                   // strided 1x1: compacted input + the TMA path's partials
     const ConvShape d = wgrad_compact_dense_shape(s);
-    const WgradPlan pt = wgrad_tma_plan(d, nullptr);
-    size_t part = pt.splits > 1 ? WG_COUNTER_BYTES + sizeof(float) * (size_t)pt.splits * s.O * s.C : 0;
-    if (tc_wgrad_stg_supported(d)) part = tc_wgrad_stg_workspace(d);
+    const size_t part = tc_wgrad_stg_supported(d) ? tc_wgrad_stg_workspace(d)
+                                                  : splitk_workspace_bytes(wgrad_tma_plan(d, nullptr).splits, (long long)s.O * s.C);
     const size_t nt = part + 256 + sizeof(float) * (size_t)s.N * s.C * s.Ho * s.Wo;
     if (nt > need) need = nt;
   }
@@ -614,8 +536,7 @@ size_t tc_wgrad_workspace(const ConvShape& s) {
 
 // ---- TMA path for 1x1 layers: eligibility, plan, launch -----------------------------------------------------------
 static bool wgrad_tma_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B2C_WGRAD_TMA"); on = e ? atoi(e) : 1; }
+  static const int on = env_int("B2C_WGRAD_TMA", 1);
   return on != 0;
 }
 static bool wgrad_tma_shape_ok(const ConvShape& s) {
@@ -626,45 +547,11 @@ static WgradPlan wgrad_tma_plan(const ConvShape& s, int* cpi_out) {
   WgradPlan pl;
   pl.n_tile = s.C > 64 ? 128 : s.C > 32 ? 64 : 32;  // 128 x 128 fp32 accumulators = 64 registers per consumer thread
   const int cpi = (s.Ho * s.Wo + BK - 1) / BK;
-  const long long nkb = (long long)s.N * cpi;
+  pl.nkb = (long long)s.N * cpi;
   const long long mn = (long long)((s.O + 127) / 128) * ((s.C + pl.n_tile - 1) / pl.n_tile);
-  long long splits = sm_count() / mn;
-  const long long max_splits = nkb / 8 > 0 ? nkb / 8 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  const long long per = (nkb + splits - 1) / splits;
-  pl.splits = (int)((nkb + per - 1) / per);
-  pl.kb_per_split = (int)per;
-  pl.nkb = nkb;
+  plan_splitk(pl.nkb, mn, 8, &pl.splits, &pl.kb_per_split);
   if (cpi_out) *cpi_out = cpi;
   return pl;
-}
-typedef CUresult (*WgEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static WgEncodeTiledFn wg_encode_tiled() {
-  static WgEncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<WgEncodeTiledFn>(f);
-  }
-  return fn;
-}
-// [N][rows][P] fp32, box {32, box_rows, 1}, SWIZZLE_128B, out-of-bounds elements read as zero
-static int wg_make_map(CUtensorMap* map, const float* base, long long P, int rows, int N, int box_rows) {
-  WgEncodeTiledFn enc = wg_encode_tiled();
-  if (!enc) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)P, (cuuint64_t)rows, (cuuint64_t)N};
-  cuuint64_t strides[2] = {(cuuint64_t)P * 4, (cuuint64_t)P * 4 * (cuuint64_t)rows};
-  cuuint32_t box[3] = {32, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled (wgrad) failed (%d)", (int)r);
-  return B2C_OK;
 }
 template <int N_TILE>
 static int launch_wgrad_tma_inst(const WgradTmaParams& p, const CUtensorMap& mdy, const CUtensorMap& mx, cudaStream_t st) {
@@ -680,28 +567,24 @@ static int launch_conv_tc_wgrad_tma(const ConvShape& s, const float* x, const fl
                                     cudaStream_t st) {
   int cpi = 0;
   const WgradPlan pl = wgrad_tma_plan(s, &cpi);
-  const long long P = (long long)s.Ho * s.Wo;
   WgradTmaParams p;
   p.O = s.O; p.C = s.C; p.cpi = cpi; p.nkb_total = (long long)s.N * cpi;
   p.kb_per_split = pl.kb_per_split; p.splits = pl.splits;
-  const size_t need = pl.splits > 1 ? WG_COUNTER_BYTES + sizeof(float) * (size_t)pl.splits * s.O * s.C : 0;
-  if (need && (!ws || ws_bytes < need)) return fail(B2C_ERR_WORKSPACE, "wgrad (tma): workspace too small");
-  p.out = pl.splits > 1 ? reinterpret_cast<float*>(static_cast<char*>(ws) + WG_COUNTER_BYTES) : dw;
-  p.grad = dw;
-  p.counters = static_cast<unsigned int*>(ws);
-  if (pl.splits > 1) B2C_CUDA_OK(cudaMemsetAsync(ws, 0, WG_COUNTER_BYTES, st));
+  if (int rc = bind_splitk(p, pl.splits, (long long)s.O * s.C, dw, ws, ws_bytes, st, "wgrad (tma)")) return rc;
   alignas(64) CUtensorMap mdy, mx;
-  int rc = wg_make_map(&mdy, dy, P, s.O, s.N, 128);
+  // [N][rows][P] fp32, box {32, box rows, 1}, SWIZZLE_128B
+  const cuuint64_t P = (cuuint64_t)s.Ho * s.Wo;
+  int rc = make_tensor_map_3d(&mdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dy, {P, (cuuint64_t)s.O, (cuuint64_t)s.N}, {P * 4, P * 4 * (cuuint64_t)s.O},
+                              {32, 128, 1}, CU_TENSOR_MAP_SWIZZLE_128B, "wgrad");
   if (rc) return rc;
-  rc = wg_make_map(&mx, x, P, s.C, s.N, pl.n_tile);
+  rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, x, {P, (cuuint64_t)s.C, (cuuint64_t)s.N}, {P * 4, P * 4 * (cuuint64_t)s.C},
+                          {32, (cuuint32_t)pl.n_tile, 1}, CU_TENSOR_MAP_SWIZZLE_128B, "wgrad");
   if (rc) return rc;
   switch (pl.n_tile) {
-    case 128: rc = launch_wgrad_tma_inst<128>(p, mdy, mx, st); break;
-    case 64: rc = launch_wgrad_tma_inst<64>(p, mdy, mx, st); break;
-    default: rc = launch_wgrad_tma_inst<32>(p, mdy, mx, st); break;
+    case 128: return launch_wgrad_tma_inst<128>(p, mdy, mx, st);
+    case 64: return launch_wgrad_tma_inst<64>(p, mdy, mx, st);
+    default: return launch_wgrad_tma_inst<32>(p, mdy, mx, st);
   }
-  if (rc) return rc;
-  return B2C_OK;
 }
 
 // ---- strided 1x1 layers (pad 0, stride > 1): subsample, then the TMA path ------------------------------------------
@@ -712,8 +595,7 @@ static int launch_conv_tc_wgrad_tma(const ConvShape& s, const float* x, const fl
 // sampled pixels into a dense [N][C][Ho*Wo] buffer first is one HBM-bound pass over half of X's rows, after which the
 // layer is an ordinary 1x1 / stride 1 weight gradient for the TMA-fed kernel.
 static int wgrad_compact_mode() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B2C_WGRAD_COMPACT"); on = e ? atoi(e) : 1; }
+  static const int on = env_int("B2C_WGRAD_COMPACT", 1);
   return on;
 }
 static bool wgrad_compact_shape_ok(const ConvShape& s) {
@@ -723,9 +605,7 @@ static bool wgrad_compact_shape_ok(const ConvShape& s) {
     return false;
   // with the staged kernel behind it the extra pass over X pays for every layer it takes; with the 3xTF32 TMA kernel only for
   // the wide ones (measurements above).  7x7 outputs (P = 49) exist only on the staged kernel (plane mode).
-  ConvShape d = s;
-  d.H = s.Ho; d.W = s.Wo; d.sh = d.sw = 1; d.is_1x1 = true;
-  const bool staged = tc_wgrad_stg_supported(d);
+  const bool staged = tc_wgrad_stg_supported(wgrad_compact_dense_shape(s));
   if (!(P % 4 == 0 && P >= 32)) return staged && P == 49;
   return mode == 2 || s.O > 128 || staged;
 }
@@ -774,7 +654,6 @@ int tc_wgrad_route(const ConvShape& s, int math, bool x_ok, bool dy_ok, bool ws_
   return B2C_WGRAD_ROUTE_GATHER;
 }
 
-bool tc_wgrad_stg_plan_info(const ConvShape& s, WgradPlanInfo* q);
 // the plan the planner of `route`'s kernel makes for s (compaction routes: for the dense 1x1 problem)
 void tc_wgrad_plan_info(const ConvShape& s, int route, WgradPlanInfo* q) {
   *q = WgradPlanInfo{};
@@ -799,9 +678,8 @@ int launch_conv_tc_wgrad(const ConvShape& s, int math, const float* x, const flo
   if (route == B2C_WGRAD_ROUTE_TMA_1X1) return launch_conv_tc_wgrad_tma(s, x, dy, dw, ws, ws_bytes, st);
   if (route == B2C_WGRAD_ROUTE_COMPACT_STAGED || route == B2C_WGRAD_ROUTE_COMPACT_TMA) {
     const ConvShape d = wgrad_compact_dense_shape(s);
-    const WgradPlan pt = wgrad_tma_plan(d, nullptr);
     const bool staged = route == B2C_WGRAD_ROUTE_COMPACT_STAGED;
-    const size_t part = staged ? tc_wgrad_stg_workspace(d) : pt.splits > 1 ? WG_COUNTER_BYTES + sizeof(float) * (size_t)pt.splits * s.O * s.C : 0;
+    const size_t part = staged ? tc_wgrad_stg_workspace(d) : splitk_workspace_bytes(wgrad_tma_plan(d, nullptr).splits, (long long)s.O * s.C);
     const size_t xoff = (part + 255) & ~(size_t)255;
     const size_t xbytes = sizeof(float) * (size_t)s.N * s.C * s.Ho * s.Wo;
     if (ws_bytes < xoff + xbytes) return fail(B2C_ERR_WORKSPACE, "wgrad (compact): workspace too small");
@@ -820,26 +698,17 @@ int launch_conv_tc_wgrad(const ConvShape& s, int math, const float* x, const flo
   p.Ho = s.Ho; p.Wo = s.Wo;
   p.Q = (long long)s.N * s.Ho * s.Wo;
   p.kb_per_split = pl.kb_per_split; p.splits = pl.splits;
-  static long long* prof_buf = nullptr;
-  static int prof_on = -1;
-  if (prof_on < 0) { const char* e = getenv("B2C_PROF"); prof_on = e ? atoi(e) : 0; if (prof_on) cudaMalloc(&prof_buf, 32 * sizeof(long long)); }
-  p.prof = prof_on ? prof_buf : nullptr;
-  if (prof_on) cudaMemsetAsync(prof_buf, 0, 32 * sizeof(long long), st);
-  const size_t need = pl.splits > 1 ? WG_COUNTER_BYTES + sizeof(float) * (size_t)pl.splits * s.O * s.Kd : 0;
-  if (need && (!ws || ws_bytes < need)) return fail(B2C_ERR_WORKSPACE, "wgrad: workspace too small");
-  p.out = pl.splits > 1 ? reinterpret_cast<float*>(static_cast<char*>(ws) + WG_COUNTER_BYTES) : dw;
-  p.grad = dw;
-  p.counters = static_cast<unsigned int*>(ws);
-  if (pl.splits > 1) B2C_CUDA_OK(cudaMemsetAsync(ws, 0, WG_COUNTER_BYTES, st));
+  if (int rc = bind_splitk(p, pl.splits, (long long)s.O * s.Kd, dw, ws, ws_bytes, st, "wgrad")) return rc;
+  p.prof = prof_buffer(st);
   int rc;
   switch (pl.n_tile) {
     case 64: rc = launch_wgrad_n<64>(p, s.G, math, s.is_1x1, st); break;
     default: rc = launch_wgrad_n<32>(p, s.G, math, s.is_1x1, st); break;
   }
   if (rc) return rc;
-  if (prof_on) {
+  if (p.prof) {
     long long h[32];
-    cudaMemcpy(h, prof_buf, sizeof(h), cudaMemcpyDeviceToHost);
+    prof_read(p.prof, h);
     fprintf(stderr, "[wprof] N_TILE=%d splits=%d nkb=%lld | dY-prod: loop=%lld wait_empty=%lld store=%lld | X-prod: loop=%lld wait_empty=%lld store=%lld\n",
             pl.n_tile, pl.splits, h[5], h[0], h[1], h[2], h[8], h[9], h[10]);
   }

@@ -18,11 +18,8 @@
 //     (1x1) or 72 (8 channels x 9 taps), fp32 accumulators in registers for the whole K range of the CTA (pixels past the
 //     image end are zeros in both tiles, so every K block runs all four K steps);
 //   * the reduction over pixels is split across CTAs in one wave; partial tiles meet through the fused, deterministic
-//     split-K reduction of conv_tc_wgrad.cu (arrival counter + per-CTA slice, fixed split order).
+//     split-K reduction of tc_common.cuh (arrival counter + per-CTA slice, fixed split order).
 // Three bf16 MMAs per MAC cost 1.5 TF32 MMAs (3xTF32: 3); dropped terms ~2^-17 per product.
-#include <cuda.h>
-#include <cuda_bf16.h>
-#include <stdlib.h>
 #include <stdio.h>
 #include "b2c_common.cuh"
 #define B2C_MBAR_DEBUG 1     // this kernel records stuck mbarrier waits (tc_common.cuh)
@@ -79,29 +76,9 @@ struct Cfg {
   static_assert(TOTAL <= 227u * 1024u, "shared memory budget");
 };
 
-__device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
 __device__ __forceinline__ float lds32(uint32_t addr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-  return v;
-}
-template <int OFF>
-__device__ __forceinline__ float lds32i(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(addr), "n"(OFF));
   return v;
 }
 __device__ __forceinline__ float2 lds64(uint32_t addr) {
@@ -112,58 +89,6 @@ __device__ __forceinline__ float2 lds64(uint32_t addr) {
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
-__device__ __forceinline__ void sts128u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-// fp32 pair (k even, k odd) -> packed bf16 hi word and packed bf16 lo word (element k in the low half)
-__device__ __forceinline__ void split_pack_bf16(float e, float o, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(e, o);
-  const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h);
-  const float he = __uint_as_float(hb << 16), ho = __uint_as_float(hb & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(e - he, o - ho);
-  hi = hb;
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
-// the deterministic split-K reduction shared with the other weight-gradient kernels (conv_tc_wgrad.cu has the twin)
-__device__ __forceinline__ void splitk_fused_reduce(const float* __restrict__ part, float* __restrict__ dw, unsigned int* counter,
-                                                    int split, int splits, long long plane, long long tile_base, int ld, int nrows, int ncols) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    atomicAdd(counter, 1u);
-    const long long t0 = clock64();
-    unsigned int seen;
-    do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-      if (seen < (unsigned)splits) {
-        __nanosleep(64);
-        if (clock64() - t0 > MBAR_TIMEOUT_CYCLES) asm volatile("trap;");
-      }
-    } while (seen < (unsigned)splits);
-  }
-  __syncthreads();
-  const int total = nrows * ncols;
-  const int per = (total + splits - 1) / splits;
-  const int e_end = min(total, (split + 1) * per);
-  for (int e = split * per + (int)threadIdx.x; e < e_end; e += (int)blockDim.x) {
-    const int r = e / ncols, c = e - r * ncols;
-    const long long idx = tile_base + (long long)r * ld + c;
-    // loads of 8 splits in flight, added in split order (the order, not the batching, fixes the rounding)
-    float acc = 0.0f;
-    int s2 = 0;
-    for (; s2 + 8 <= splits; s2 += 8) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = __ldcg(part + (long long)(s2 + u) * plane + idx);
-#pragma unroll
-      for (int u = 0; u < 8; ++u) acc += v[u];
-    }
-    for (; s2 < splits; ++s2) acc += __ldcg(part + (long long)s2 * plane + idx);
-    dw[idx] += acc;
-  }
-}
-
 // PLANE (7x7 maps: a 196-byte channel pitch is not a TMA stride): one K block = one whole image.  The blobs are viewed as
 // {4*H*W, channels/4, N} (four channels per tensor row), so a box of 32 rows is 128 channels x H*W pixels, contiguous; dY is read
 // with 4-byte loads (odd word pitch: conflict-free), pixels H*W..63 of the 64-wide K block are written as zeros on both operands.
@@ -430,43 +355,13 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
 
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-typedef CUresult (*WsEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static WsEncodeTiledFn ws_encode_tiled() {
-  static WsEncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<WsEncodeTiledFn>(f);
-  }
-  return fn;
-}
-// [N][rows][HW] fp32, box {bw, box_rows, 1}
-static int ws_make_map(CUtensorMap* map, const float* base, int HW, int rows, int N, int bw, int box_rows, bool swizzle128) {
-  WsEncodeTiledFn enc = ws_encode_tiled();
-  if (!enc) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)HW, (cuuint64_t)rows, (cuuint64_t)N};
-  cuuint64_t strides[2] = {(cuuint64_t)HW * 4, (cuuint64_t)HW * 4 * (cuuint64_t)rows};
-  cuuint32_t box[3] = {(cuuint32_t)bw, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2C_ERR_CUDA, "cuTensorMapEncodeTiled (staged wgrad) failed (%d)", (int)r);
-  return B2C_OK;
-}
-
 static bool wstg_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B2C_WGRAD_STAGED"); on = e ? atoi(e) : 1; }
+  static const int on = env_int("B2C_WGRAD_STAGED", 1);
   return on != 0;
 }
 struct WstgPlan { int T, cn, bwx, bpi, splits, kb_per_split; long long nkb; bool plane; };
 static bool wstg_plane_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B2C_WGRAD_STAGED_PLANE"); on = e ? atoi(e) : 1; }
+  static const int on = env_int("B2C_WGRAD_STAGED_PLANE", 1);
   return on != 0;
 }
 static bool wstg_plan(const ConvShape& s, WstgPlan* pl) {
@@ -491,17 +386,9 @@ static bool wstg_plan(const ConvShape& s, WstgPlan* pl) {
   pl->bwx = plane ? (int)HW : (need + 3) & ~3;
   pl->bpi = (int)((HW + wstg::KPX - 1) / wstg::KPX);
   pl->nkb = (long long)s.N * pl->bpi;
-  const long long mn = (long long)((s.O + 127) / 128) * ((s.C + pl->cn - 1) / pl->cn);
-  long long splits = sm_count() / mn;
-  const long long max_splits = pl->nkb / 4 > 0 ? pl->nkb / 4 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  const long long per = (pl->nkb + splits - 1) / splits;
-  pl->splits = (int)((pl->nkb + per - 1) / per);
-  pl->kb_per_split = (int)per;
+  plan_splitk(pl->nkb, (long long)((s.O + 127) / 128) * ((s.C + pl->cn - 1) / pl->cn), 4, &pl->splits, &pl->kb_per_split);
   return true;
 }
-constexpr size_t WSTG_COUNTER_BYTES = 1024;
 bool tc_wgrad_stg_supported(const ConvShape& s) { return wstg_plan(s, nullptr); }
 bool tc_wgrad_stg_plan_info(const ConvShape& s, WgradPlanInfo* q) {
   WstgPlan pl;
@@ -513,7 +400,7 @@ bool tc_wgrad_stg_plan_info(const ConvShape& s, WgradPlanInfo* q) {
 size_t tc_wgrad_stg_workspace(const ConvShape& s) {
   WstgPlan pl;
   if (!wstg_plan(s, &pl)) return 0;
-  return pl.splits > 1 ? WSTG_COUNTER_BYTES + sizeof(float) * (size_t)pl.splits * s.O * s.Kd : 0;
+  return splitk_workspace_bytes(pl.splits, (long long)s.O * s.Kd);
 }
 
 template <int T, int CN, bool PLANE>
@@ -544,20 +431,13 @@ bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K) {
 // split count of the K loop when the caller brings a workspace (b2c_sgemm_ex): one wave of CTAs, >= 4 K blocks per split
 static void gemm_tc_plan(int M, int N, int K, WstgPlan* pl) {
   pl->T = 1; pl->plane = false; pl->cn = N > 64 ? 128 : 64; pl->bwx = wstg::KPX; pl->bpi = (K + wstg::KPX - 1) / wstg::KPX; pl->nkb = pl->bpi;
-  const long long mn = (long long)((M + 127) / 128) * ((N + pl->cn - 1) / pl->cn);
-  long long splits = sm_count() / mn;
-  const long long max_splits = pl->nkb / 4 > 0 ? pl->nkb / 4 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  const long long per = (pl->nkb + splits - 1) / splits;
-  pl->splits = (int)((pl->nkb + per - 1) / per);
-  pl->kb_per_split = (int)per;
+  plan_splitk(pl->nkb, (long long)((M + 127) / 128) * ((N + pl->cn - 1) / pl->cn), 4, &pl->splits, &pl->kb_per_split);
 }
 size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K) {
   if (!tc_gemm_supported(tA, tB, M, N, K)) return 0;
   WstgPlan pl;
   gemm_tc_plan(M, N, K, &pl);
-  return pl.splits > 1 ? WSTG_COUNTER_BYTES + sizeof(float) * (size_t)pl.splits * M * N : 0;
+  return splitk_workspace_bytes(pl.splits, (long long)M * N);
 }
 int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const float* A, const float* B, float beta, float* Cm, int math,
                     void* ws, size_t ws_bytes, cudaStream_t st) {
@@ -571,35 +451,40 @@ int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const fl
   s.Ho = 1; s.Wo = K; s.Cg = N; s.Og = M; s.Kd = N; s.is_1x1 = true;
   WstgPlan pl;
   gemm_tc_plan(M, N, K, &pl);
-  const size_t need = pl.splits > 1 ? WSTG_COUNTER_BYTES + sizeof(float) * (size_t)pl.splits * M * N : 0;
-  if (!ws || ws_bytes < need || (reinterpret_cast<uintptr_t>(ws) & 15u)) { pl.splits = 1; pl.kb_per_split = pl.bpi; ws = nullptr; ws_bytes = 0; }   // no workspace: one CTA per tile walks all of K
+  if (!ws || ws_bytes < splitk_workspace_bytes(pl.splits, (long long)M * N) || (reinterpret_cast<uintptr_t>(ws) & 15u)) { pl.splits = 1; pl.kb_per_split = pl.bpi; ws = nullptr; ws_bytes = 0; }   // no workspace: one CTA per tile walks all of K
   return launch_wstg_planned(s, pl, B, A, Cm, ws, ws_bytes, st);
 }
 
 static int launch_wstg_planned(const ConvShape& s, const WstgPlan& pl, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes,
                                cudaStream_t st) {
-  const size_t need = pl.splits > 1 ? WSTG_COUNTER_BYTES + sizeof(float) * (size_t)pl.splits * s.O * s.Kd : 0;
-  if (need && (!ws || ws_bytes < need)) return fail(B2C_ERR_WORKSPACE, "staged wgrad: workspace too small");
   wstg::Params p;
   p.HW = s.H * s.W; p.H = s.H; p.W = s.W; p.C = s.C; p.O = s.O;
   p.halo = s.ph * s.W + s.pw; p.bwx = pl.bwx; p.bpi = pl.bpi; p.nkb_total = pl.nkb;
   p.kb_per_split = pl.kb_per_split; p.splits = pl.splits; p.Kd = s.Kd;
-  p.out = pl.splits > 1 ? reinterpret_cast<float*>(static_cast<char*>(ws) + WSTG_COUNTER_BYTES) : dw;
-  p.grad = dw;
-  p.counters = static_cast<unsigned int*>(ws);
-  if (pl.splits > 1) B2C_CUDA_OK(cudaMemsetAsync(ws, 0, WSTG_COUNTER_BYTES, st));
+  if (int rc = bind_splitk(p, pl.splits, (long long)s.O * s.Kd, dw, ws, ws_bytes, st, "staged wgrad")) return rc;
   alignas(64) CUtensorMap mdy, mx;
+  const cuuint64_t HW = (cuuint64_t)p.HW;
   const int c_tiles = (s.C + pl.cn - 1) / pl.cn, o_tiles = (s.O + 127) / 128;
   if (pl.plane) {
     // {4*HW, channels/4, N}: four channels per tensor row (a 16-byte-multiple pitch); box rows = tile channels / 4
-    if (int rc = ws_make_map(&mdy, dy, p.HW * 4, s.O / 4, s.N, p.HW * 4, 32, false)) return rc;
-    if (int rc = ws_make_map(&mx, x, p.HW * 4, s.C / 4, s.N, p.HW * 4, pl.cn / 4, false)) return rc;
+    if (int rc = make_tensor_map_3d(&mdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dy, {HW * 4, (cuuint64_t)s.O / 4, (cuuint64_t)s.N},
+                                    {HW * 16, HW * 16 * (cuuint64_t)(s.O / 4)}, {(cuuint32_t)HW * 4, 32, 1}, CU_TENSOR_MAP_SWIZZLE_NONE, "staged wgrad"))
+      return rc;
+    if (int rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, x, {HW * 4, (cuuint64_t)s.C / 4, (cuuint64_t)s.N},
+                                    {HW * 16, HW * 16 * (cuuint64_t)(s.C / 4)}, {(cuuint32_t)HW * 4, (cuuint32_t)pl.cn / 4, 1},
+                                    CU_TENSOR_MAP_SWIZZLE_NONE, "staged wgrad"))
+      return rc;
     if (pl.T == 9) return wstg_launch<9, 8, true>(p, mdy, mx, c_tiles, o_tiles, st);
     if (pl.cn == 128) return wstg_launch<1, 128, true>(p, mdy, mx, c_tiles, o_tiles, st);
     return wstg_launch<1, 64, true>(p, mdy, mx, c_tiles, o_tiles, st);
   }
-  if (int rc = ws_make_map(&mdy, dy, p.HW, s.O, s.N, 32, 128, true)) return rc;
-  if (int rc = ws_make_map(&mx, x, p.HW, s.C, s.N, pl.bwx, pl.cn, false)) return rc;
+  // [N][channels][HW] fp32: dY in [128 o][32 px] SWIZZLE_128B boxes, X in [CN c][bwx px] boxes
+  if (int rc = make_tensor_map_3d(&mdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dy, {HW, (cuuint64_t)s.O, (cuuint64_t)s.N}, {HW * 4, HW * 4 * (cuuint64_t)s.O},
+                                  {32, 128, 1}, CU_TENSOR_MAP_SWIZZLE_128B, "staged wgrad"))
+    return rc;
+  if (int rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, x, {HW, (cuuint64_t)s.C, (cuuint64_t)s.N}, {HW * 4, HW * 4 * (cuuint64_t)s.C},
+                                  {(cuuint32_t)pl.bwx, (cuuint32_t)pl.cn, 1}, CU_TENSOR_MAP_SWIZZLE_NONE, "staged wgrad"))
+    return rc;
   if (pl.T == 9) return wstg_launch<9, 8, false>(p, mdy, mx, c_tiles, o_tiles, st);
   if (pl.cn == 128) return wstg_launch<1, 128, false>(p, mdy, mx, c_tiles, o_tiles, st);
   return wstg_launch<1, 64, false>(p, mdy, mx, c_tiles, o_tiles, st);

@@ -695,10 +695,6 @@ extern "C" int b2c_softmax_loss_backward(int N, int C, const float* prob, const 
   return B2C_OK;
 }
 // y[n][o] += b[o] and db[o] += sum_n dy[n][o]: InnerProduct bias (inner_product_layer.cpp), via the conv bias kernels with P = 1
-namespace b2c {
-int launch_bias_add(int, int, int, const float*, float*, cudaStream_t);
-int launch_bias_grad(int, int, int, const float*, float*, cudaStream_t);
-}
 extern "C" int b2c_bias_forward(int N, int O, int P, const float* bias, float* y, void* stream) {
   NEED(bias && y, "b2c_bias_forward: null");
   return launch_bias_add(N, O, P, bias, y, as_stream(stream));

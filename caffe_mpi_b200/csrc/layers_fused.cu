@@ -477,8 +477,7 @@ int launch_bn_stats(int N, int C, int S, const float* x, float eps, float maf, i
 
 // B2C_BN_ONEPASS (default 1): statistics / reduction and the elementwise pass in one launch per BatchNorm direction
 static bool bn_onepass() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B2C_BN_ONEPASS"); on = e ? atoi(e) : 1; }
+  static const int on = env_int("B2C_BN_ONEPASS", 1);
   return on != 0;
 }
 // bytes of one parked stream of the largest slice (rank 0's) of a channel, and the shared-memory budget of one CTA when two
@@ -490,8 +489,7 @@ static size_t bn_slice_bytes(int N, int S, bool vec, unsigned cs, unsigned* unit
   return units * (vec ? 16 : 4);
 }
 static size_t bn_cache_budget() {
-  static long v = -1;
-  if (v < 0) { const char* e = getenv("B2C_BN_CACHE_KB"); v = e ? atol(e) * 1024 : 110 * 1024; }   // 0: never park (phase 2 re-reads global memory)
+  static const long v = env_int("B2C_BN_CACHE_KB", 110) * 1024;   // 0: never park (phase 2 re-reads global memory)
   return (size_t)v;
 }
 template <typename K>
@@ -522,8 +520,8 @@ static int bn_forward_fused_impl(int N, int C, int S, const float* x, const floa
   if (bn_onepass() || residual) {
     const unsigned cs = bn_cluster_size(N, C, S);
     const size_t slice = bn_slice_bytes(N, S, vec, cs, nullptr);
-    static int prefetch = -1;             // B2C_BN_PREFETCH (default 1): cp.async the slice into shared memory before the reduction
-    if (prefetch < 0) { const char* e = getenv("B2C_BN_PREFETCH"); prefetch = e ? atoi(e) : 1; }
+    // B2C_BN_PREFETCH (default 1): cp.async the slice into shared memory before the reduction
+    static const int prefetch = env_int("B2C_BN_PREFETCH", 1);
     const int park = slice <= bn_cache_budget() ? (prefetch ? 2 : 1) : 0;
     const size_t smem = park ? slice : 0;
 #define B2C_FWD0(V, R, Q, P) do { if (int rc = bn_onepass_attr(bn_fwd_onepass_kernel<V, R, Q, P>, smem)) return rc; \
@@ -583,8 +581,8 @@ static int bn_backward_fused_impl(int N, int C, int S, const float* dy, const fl
     const int park = 2 * slice <= bn_cache_budget() ? 3 : slice <= bn_cache_budget() ? (y_mask ? 2 : 1) : 0;
     const size_t smem = (size_t)(park == 3 ? 2 : park ? 1 : 0) * slice;
     const float inv_cnt1 = 1.0f / ((float)N * S);
-    static int prefetch = -1;             // B2C_BN_PREFETCH_BWD (default 1; 16.03 -> 15.88 ms per ResNet-50 step): cp.async the parked streams before the reduction
-    if (prefetch < 0) { const char* e = getenv("B2C_BN_PREFETCH_BWD"); prefetch = e ? atoi(e) : 1; }
+    // B2C_BN_PREFETCH_BWD (default 1; 16.03 -> 15.88 ms per ResNet-50 step): cp.async the parked streams before the reduction
+    static const int prefetch = env_int("B2C_BN_PREFETCH_BWD", 1);
 #define B2C_BWDP(V, M, P, Q) do { if (int rc = bn_onepass_attr(bn_bwd_onepass_kernel<V, M, P, Q>, smem)) return rc; \
     bn_launch_clustered(bn_bwd_onepass_kernel<V, M, P, Q>, cs, C, smem, stream, bn_threads(N, S, false), N, C, S, inv_cnt1, slice_units, dy, x, y_mask, save_mean, save_invstd, \
                         gamma, beta, dgamma, dbeta, dx, d_residual, dy2); } while (0)

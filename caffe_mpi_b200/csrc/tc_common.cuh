@@ -1,6 +1,8 @@
 // tc_common.cuh -- Hopper (sm_90a) building blocks for the tensor-core kernels: mbarrier, proxy fences,
 // wgmma shared-memory matrix descriptors, wgmma fence / commit / wait and the accumulator fragment map,
-// and the TF32 hi/lo split used by the fp32-equivalent (3xTF32) math mode.
+// and the TF32 hi/lo split used by the fp32-equivalent (3xTF32) math mode; TMA loads, shared-memory accessors, the bf16 hi/lo
+// split and the fused split-K reduction; and the host plumbing around them (tc_host.cu): tensor-map encoding, the split-K
+// planner and workspace, B2C_PROF buffers.
 //
 // Shared-memory operand layout used by every kernel here: K-major, no swizzle ("interleave"),
 // canonical form ((8,m),(4,2)):((4,SBO),(1,LBO)) in fp32 elements, i.e. 8-row x 16-byte core
@@ -9,8 +11,11 @@
 // land in eight different 16-byte bank groups, so both producer mappings (lanes along rows, and
 // lanes along K) store conflict-free with 128-bit st.shared.
 #pragma once
+#include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "b2c_common.cuh"
 #include "wgmma_ops.cuh"
 
 namespace b2c {
@@ -191,6 +196,123 @@ __device__ __forceinline__ void store_chunk(uint32_t hi_addr, uint32_t lo_addr, 
     sts128(hi_addr, to_tf32(v0), to_tf32(v1), to_tf32(v2), to_tf32(v3));
   }
 }
+
+__device__ __forceinline__ void sts128u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ float4 lds128(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+// addr + OFF as an immediate: a run of loads at fixed offsets shares one base register
+template <int OFF>
+__device__ __forceinline__ float lds32i(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(addr), "n"(OFF));
+  return v;
+}
+
+// ---- bf16x3 split ------------------------------------------------------------------------------------
+// fp32 pair (k even, k odd) -> packed bf16 hi word and packed bf16 lo word; element k sits in the LOW half
+// (two consecutive K elements per 32-bit word of the K-major operand tile, little endian)
+__device__ __forceinline__ void split_pack_bf16(float e, float o, uint32_t& hi, uint32_t& lo) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(e, o);            // .x = e (low half), .y = o
+  const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h);
+  const float he = __uint_as_float(hb << 16), ho = __uint_as_float(hb & 0xffff0000u);
+  const __nv_bfloat162 l = __floats2bfloat162_rn(e - he, o - ho);   // a - hi is exact in fp32
+  hi = hb;
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+// ---- TMA ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+__device__ __forceinline__ void arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+
+// ---- split-K reduction fused into the tile's own CTAs (the weight-gradient kernels and the NT GEMM) -------------------------
+// Round 1 ran a second kernel per layer (wgrad_reduce_kernel, 53 launches / 0.58 ms per ResNet-50 step).  Here the `splits` CTAs
+// of an output tile meet at a counter in the workspace once their partial tiles are in global memory -- the whole grid is one
+// wave by construction (plan_splitk: never more CTAs than SMs), so every CTA of the tile is resident -- and then each CTA adds
+// up its 1/splits slice of the tile over the partials IN SPLIT ORDER and accumulates it into dW: the summation order of every
+// element is fixed, so the result is bit-reproducible and equal to what the separate kernel produced.
+__device__ __forceinline__ void splitk_fused_reduce(const float* __restrict__ part, float* __restrict__ dw, unsigned int* counter,
+                                                    int split, int splits, long long plane, long long tile_base, int ld, int nrows, int ncols) {
+  __syncthreads();                                   // this CTA's partial tile is complete (epilogue warps)
+  if (threadIdx.x == 0) {
+    __threadfence();
+    atomicAdd(counter, 1u);
+    const long long t0 = clock64();
+    unsigned int seen;
+    do {
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
+      if (seen < (unsigned)splits) {
+        __nanosleep(64);
+        if (clock64() - t0 > MBAR_TIMEOUT_CYCLES) asm volatile("trap;");
+      }
+    } while (seen < (unsigned)splits);
+  }
+  __syncthreads();
+  const int total = nrows * ncols;
+  const int per = (total + splits - 1) / splits;
+  const int e_end = min(total, (split + 1) * per);
+  for (int e = split * per + (int)threadIdx.x; e < e_end; e += (int)blockDim.x) {
+    const int r = e / ncols, c = e - r * ncols;
+    const long long idx = tile_base + (long long)r * ld + c;
+    // loads of 8 splits in flight, added in split order (the order, not the batching, fixes the rounding)
+    float acc = 0.0f;
+    int s2 = 0;
+    for (; s2 + 8 <= splits; s2 += 8) {
+      float v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) v[u] = __ldcg(part + (long long)(s2 + u) * plane + idx);
+#pragma unroll
+      for (int u = 0; u < 8; ++u) acc += v[u];
+    }
+    for (; s2 < splits; ++s2) acc += __ldcg(part + (long long)s2 * plane + idx);
+    dw[idx] += acc;
+  }
+}
+
+// ---- host side (tc_host.cu) ----------------------------------------------------------------------------
+// cuTensorMapEncodeTiled of a 3-D tensor (no interleave, 256-byte L2 promotion, no OOB NaN fill: out-of-range elements read as
+// zero and are not written); `what` names the map in the failure message
+int make_tensor_map_3d(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, const cuuint64_t (&dims)[3],
+                       const cuuint64_t (&byte_strides)[2], const cuuint32_t (&box)[3], CUtensorMapSwizzle swizzle, const char* what);
+
+// One wave of split-K CTAs: every CTA pays a fixed prologue + epilogue (partial tile write), so fewer, longer CTAs win; never more
+// CTAs than SMs (a partial second wave costs a full CTA time), at least min_kb_per_split of the nkb K blocks per split, and the
+// split length rebalanced so no split is empty.  `tiles`: output tiles of the launch (CTAs per split).
+void plan_splitk(long long nkb, long long tiles, int min_kb_per_split, int* splits, int* kb_per_split);
+
+// split-K workspace: [arrival counters, one u32 per output tile (<= #SMs)][partials: splits x plane_elems fp32]; 0 for one split
+constexpr size_t SPLITK_COUNTER_BYTES = 1024;
+inline size_t splitk_workspace_bytes(int splits, long long plane_elems) {
+  return splits > 1 ? SPLITK_COUNTER_BYTES + sizeof(float) * (size_t)splits * (size_t)plane_elems : 0;
+}
+// Points a split-K kernel's parameters at the workspace: `out` at the partials (splits > 1) or at dW itself, `grad` at dW,
+// `counters` at the zeroed counters.  `what` names the kernel in the failure message.
+template <class P>
+int bind_splitk(P& p, int splits, long long plane_elems, float* dw, void* ws, size_t ws_bytes, cudaStream_t st, const char* what) {
+  const size_t need = splitk_workspace_bytes(splits, plane_elems);
+  if (need && (!ws || ws_bytes < need)) return fail(B2C_ERR_WORKSPACE, "%s: workspace too small", what);
+  p.out = splits > 1 ? reinterpret_cast<float*>(static_cast<char*>(ws) + SPLITK_COUNTER_BYTES) : dw;
+  p.grad = dw;
+  p.counters = static_cast<unsigned int*>(ws);
+  if (splits > 1) B2C_CUDA_OK(cudaMemsetAsync(ws, 0, SPLITK_COUNTER_BYTES, st));
+  return B2C_OK;
+}
+
+// B2C_PROF=1: a 32-word device buffer for the kernels' clock64 phase counters, zeroed on `st`; null when the switch is off
+long long* prof_buffer(cudaStream_t st);
+// the counters the last launch wrote (synchronous)
+void prof_read(const long long* buf, long long (&h)[32]);
 
 }  // namespace tc
 }  // namespace b2c
