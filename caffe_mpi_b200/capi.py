@@ -115,6 +115,8 @@ def lib():
         "b2c_sgd_update": (i, [sz, vp, vp, vp, f, f, f, i, f, i, vp]),
         "b2c_sgd_update_arena": (i, [i, C.POINTER(sz), C.POINTER(sz), C.POINTER(f), C.POINTER(f), vp, vp, vp,
                                      f, i, f, i, vp]),
+        "b2c_solver_update_arena": (i, [i, i, C.POINTER(sz), C.POINTER(sz), C.POINTER(f), C.POINTER(f), vp, vp, vp, vp,
+                                        SolverHParams, i, f, i, vp]),
         "b2c_relu_forward": (i, [sz, vp, vp, f, vp]),
         "b2c_relu_backward": (i, [sz, vp, vp, vp, f, vp]),
         "b2c_bn_forward_train": (i, [i, i, i, vp, vp, vp, f, f, i, vp, vp, vp, vp, vp, vp, vp]),
@@ -324,6 +326,26 @@ def sgd_update_arena(offsets, counts, rates, decays, g, w, h, momentum, l2=True,
     check(lib().b2c_sgd_update_arena(n, (C.c_size_t * n)(*offsets), (C.c_size_t * n)(*counts),
                                      (C.c_float * n)(*rates), (C.c_float * n)(*decays), _p(g), _p(w), _p(h),
                                      momentum, int(l2), grad_scale, int(clear_grads), _stream(stream)))
+
+
+SOLVER_KINDS = {"SGD": 0, "Nesterov": 1, "AdaGrad": 2, "RMSProp": 3, "AdaDelta": 4, "Adam": 5}   # b2c_solver_kind
+
+
+class SolverHParams(C.Structure):
+    _fields_ = [("momentum", C.c_float), ("delta", C.c_float), ("rms_decay", C.c_float), ("beta1", C.c_float),
+                ("beta2", C.c_float)]
+
+
+def solver_update_arena(kind, offsets, counts, rates, decays, g, w, h, h2=None, momentum=0.0, delta=1e-8, rms_decay=0.0,
+                        beta1=0.9, beta2=0.999, l2=True, grad_scale=1.0, clear_grads=True, stream=None):
+    """b2c_solver_update_arena: `kind` is a name of SOLVER_KINDS; h2 only for AdaDelta and Adam.  For Adam, `rates` carry the
+    bias correction sqrt(1-beta2^t)/(1-beta1^t)."""
+    n = len(offsets)
+    hp = SolverHParams(momentum, delta, rms_decay, beta1, beta2)
+    check(lib().b2c_solver_update_arena(SOLVER_KINDS[kind], n, (C.c_size_t * n)(*offsets), (C.c_size_t * n)(*counts),
+                                        (C.c_float * n)(*rates), (C.c_float * n)(*decays), _p(g), _p(w), _p(h),
+                                        _p(h2), hp, int(l2), grad_scale, int(clear_grads),
+                                        _stream(stream)))
 
 
 class Comm:

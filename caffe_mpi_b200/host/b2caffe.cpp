@@ -460,6 +460,7 @@ ParamArena::~ParamArena() {
   if (data_) cudaFree(data_);
   if (diff_) { if (diff_nccl_) b2c_comm_mem_free(diff_); else cudaFree(diff_); }
   if (hist_) cudaFree(hist_);
+  if (hist2_) cudaFree(hist2_);
 }
 void ParamArena::InitLayout(const vector<size_t>& counts) {
   offset_.clear(); count_.clear();
@@ -467,7 +468,7 @@ void ParamArena::InitLayout(const vector<size_t>& counts) {
   for (size_t c : counts) { offset_.push_back(off); count_.push_back(c); off += even(c); }
   total_ = off;
 }
-void ParamArena::Init(const vector<shared_ptr<Blob>>& params) {
+void ParamArena::Init(const vector<shared_ptr<Blob>>& params, bool second_history) {
   B2_CHECK(!data_, "arena already initialised");
   offset_.clear(); count_.clear();
   size_t off = 0;
@@ -490,6 +491,10 @@ void ParamArena::Init(const vector<shared_ptr<Blob>>& params) {
   CUDA_CHECK(cudaMemset(data_, 0, bytes));
   CUDA_CHECK(cudaMemset(diff_, 0, bytes));     // net.cpp:1367
   CUDA_CHECK(cudaMemset(hist_, 0, bytes));
+  if (second_history) {
+    CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&hist2_), bytes));
+    CUDA_CHECK(cudaMemset(hist2_, 0, bytes));
+  }
   for (size_t i = 0; i < params.size(); ++i) {
     params[i]->set_gpu_data(data_ + offset_[i]);
     params[i]->set_gpu_diff(diff_ + offset_[i]);
@@ -497,6 +502,19 @@ void ParamArena::Init(const vector<shared_ptr<Blob>>& params) {
 }
 
 // ================================================================================================ solver
+int SolverKind(const string& type) {
+  static const char* const names[] = {"SGD", "Nesterov", "AdaGrad", "RMSProp", "AdaDelta", "Adam"};   // b2c_solver_kind order
+  for (int k = 0; k < 6; ++k) if (type == names[k]) return k;
+  Fatal(__FILE__, __LINE__, "Unknown solver type: " + type + " (known types: SGD, Nesterov, AdaGrad, RMSProp, AdaDelta, Adam)");
+}
+void CheckSolverParameter(const SolverParameter& p) {
+  const int k = SolverKind(p.type);
+  if (k == B2C_SOLVER_ADAGRAD) B2_CHECK(p.momentum == 0.f, "Momentum cannot be used with AdaGrad.");
+  if (k == B2C_SOLVER_RMSPROP) {
+    B2_CHECK(p.momentum == 0.f, "Momentum cannot be used with RMSProp.");
+    B2_CHECK(p.rms_decay >= 0.f && p.rms_decay < 1.f, "rms_decay should lie between 0 and 1.");
+  }
+}
 float SGDSolver::GetLearningRate() {
   const SolverParameter& p = param_;
   if (iter_ < p.rampup_interval) {
@@ -535,29 +553,47 @@ float SGDSolver::GetMomentum() {
 void SGDSolver::SetParams(const vector<shared_ptr<Blob>>& params, const vector<ParamSpec>& specs) {
   B2_CHECK(params.size() == specs.size(), "one ParamSpec per learnable blob");
   specs_ = specs;
-  arena_.Init(params);
+  arena_.Init(params, num_histories() == 2);
 }
 void SGDSolver::ApplyUpdate(int id_from, int id_to, cudaStream_t stream) {
   B2_CHECK(param_.clip_gradients < 0, "clip_gradients is not on the BASELINE path (sgd_solver.cpp:111-128)");
   B2_CHECK(param_.regularization_type == "L2" || param_.regularization_type == "L1", "Unknown regularization type");
   const float rate = GetLearningRate();
-  const float momentum = GetMomentum();
+  // SGD keeps its momentum policy; Nesterov, AdaDelta and Adam (as beta1) read param_.momentum() directly
+  // (nesterov_solver.cpp:22, adadelta_solver.cpp:37, adam_solver.cpp:33)
+  const float momentum = kind_ == B2C_SOLVER_SGD ? GetMomentum() : param_.momentum;
+  // Adam's bias correction, folded into every segment's rate (adam_solver.cpp:42-43)
+  float correction = 1.f;
+  if (kind_ == B2C_SOLVER_ADAM) {
+    const float t = (float)(iter_ + 1);
+    correction = std::sqrt(1.f - std::pow(param_.momentum2, t)) / (1.f - std::pow(param_.momentum, t));
+  }
   if (id_to < id_from) return;
   vector<size_t> off, cnt;
   vector<float> lr, dc;
   for (int id = id_from; id <= id_to; ++id) {
     const float l = rate * specs_[id].lr_mult;                        // sgd_solver.cpp:208-210
     const float d = param_.weight_decay * specs_[id].decay_mult;      // :254-259
-    // lr_mult = decay_mult = 0 (BatchNorm statistics, batch_norm_layer.cpp): history stays 0, the blob is unchanged
-    // and its diff is never written, so the update is the identity -- left out of the fused launch
+    // lr_mult = decay_mult = 0 (BatchNorm statistics, batch_norm_layer.cpp): the diff is never written, so it stays 0 and
+    // gr = 0; every rule then leaves its histories at 0 and steps by u = 0 (each delta is clamped positive, so no 0/0), so
+    // the update is the identity for every solver type -- left out of the fused launch
     if (specs_[id].statistic && l == 0.f && d == 0.f) continue;
-    off.push_back(arena_.offset(id)); cnt.push_back(arena_.count(id)); lr.push_back(l); dc.push_back(d);
+    off.push_back(arena_.offset(id)); cnt.push_back(arena_.count(id)); lr.push_back(kind_ == B2C_SOLVER_ADAM ? l * correction : l);
+    dc.push_back(d);
   }
   const int n = (int)off.size();
   if (n == 0) return;
   const float grad_scale = 1.f / (float)Caffe::solver_count() / param_.global_grad_scale / (float)param_.iter_size;
-  B2C_CHECK(b2c_sgd_update_arena(n, off.data(), cnt.data(), lr.data(), dc.data(), arena_.diff(), arena_.data(), arena_.history(),
-                                 momentum, param_.regularization_type == "L2" ? 1 : 0, grad_scale, param_.snapshot_diff ? 0 : 1, stream));
+  const int l2 = param_.regularization_type == "L2" ? 1 : 0, clear = param_.snapshot_diff ? 0 : 1;
+  if (kind_ == B2C_SOLVER_SGD) {
+    B2C_CHECK(b2c_sgd_update_arena(n, off.data(), cnt.data(), lr.data(), dc.data(), arena_.diff(), arena_.data(), arena_.history(),
+                                   momentum, l2, grad_scale, clear, stream));
+    return;
+  }
+  b2c_solver_hparams hp;
+  hp.momentum = momentum; hp.delta = param_.delta; hp.rms_decay = param_.rms_decay; hp.beta1 = param_.momentum; hp.beta2 = param_.momentum2;
+  B2C_CHECK(b2c_solver_update_arena(kind_, n, off.data(), cnt.data(), lr.data(), dc.data(), arena_.diff(), arena_.data(), arena_.history(),
+                                    arena_.history2(), hp, l2, grad_scale, clear, stream));
 }
 
 // The streaming bucket logic of Net::ReduceAndUpdate (net.cpp:772-783,824-862), replayed over an arrival order.

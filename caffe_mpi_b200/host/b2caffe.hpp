@@ -268,12 +268,13 @@ class ConvolutionLayer : public LayerBase {
 shared_ptr<LayerBase> GetConvolutionLayer(const LayerParameter& p);   // layer_factory.cpp:53-88
 
 // ---------------------------------------------------------------------------------------------- arena
-// One contiguous device space each for parameter data, diffs and SGD history; every learnable blob's
+// One contiguous device space each for parameter data, diffs and solver history; every learnable blob's
 // data/diff is re-pointed into it at even(count) stride (net.cpp:1350-1373; the reference does diffs only).
+// AdaDelta and Adam keep a second history (history2) with the same layout; the other solvers allocate none.
 class ParamArena {
  public:
   ~ParamArena();
-  void Init(const vector<shared_ptr<Blob>>& params);
+  void Init(const vector<shared_ptr<Blob>>& params, bool second_history = false);
   void InitLayout(const vector<size_t>& counts);   // offsets only, no device memory (planning / CPU tests)
   size_t total() const { return total_; }
   size_t offset(int i) const { return offset_[i]; }
@@ -282,16 +283,19 @@ class ParamArena {
   float* data() const { return data_; }
   float* diff() const { return diff_; }
   float* history() const { return hist_; }
+  float* history2() const { return hist2_; }     // nullptr unless Init(..., second_history)
   bool diff_is_nccl_memory() const { return diff_nccl_; }
  private:
   vector<size_t> offset_, count_;
   size_t total_ = 0;
-  float *data_ = nullptr, *diff_ = nullptr, *hist_ = nullptr;
+  float *data_ = nullptr, *diff_ = nullptr, *hist_ = nullptr, *hist2_ = nullptr;
   bool diff_nccl_ = false;
 };
 
 // ---------------------------------------------------------------------------------------------- solver
 struct SolverParameter {   // caffe.proto SolverParameter (fields this path reads)
+  string type = "SGD";             // caffe.proto:269; the legacy solver_type enum (:288-297) is read into it
+  float delta = 1e-8f, momentum2 = 0.999f, rms_decay = 0.f;   // caffe.proto:272,274,278 (rms_decay declares no default)
   float base_lr = 0.01f, gamma = 0.1f, power = 1.f, momentum = 0.f, weight_decay = 0.f, min_lr = 0.f;
   float rampup_lr = 0.f, max_momentum = 0.99f, momentum_power = 1.f, clip_gradients = -1.f;
   int stepsize = 1, max_iter = 1, iter_size = 1, rampup_interval = 0;
@@ -302,12 +306,24 @@ struct SolverParameter {   // caffe.proto SolverParameter (fields this path read
   int reduce_buckets = 6;          // NetParameter.reduce_buckets (caffe.proto:140)
 };
 
+// b2c_solver_kind of a SolverParameter.type (REGISTER_SOLVER_CLASS names); an unknown type is fatal and lists the known ones
+int SolverKind(const string& type);
+// SolverKind plus the constructor sanity checks of the reference's solvers (include/caffe/sgd_solvers.hpp:84-113): AdaGrad
+// and RMSProp take no momentum, rms_decay lies in [0, 1).  Fatal on violation.
+void CheckSolverParameter(const SolverParameter& p);
+
 class P2PSync;
 
+// SGDSolver and the five solvers derived from it in the reference (Nesterov, AdaGrad, RMSProp, AdaDelta, Adam): they share the
+// lr policy, arena, bucket walk and snapshot code and differ only in the fused update ApplyUpdate launches (dispatched on
+// param().type) and in the number of history arenas.
 class SGDSolver {
  public:
-  explicit SGDSolver(const SolverParameter& p) : param_(p) {}
+  explicit SGDSolver(const SolverParameter& p) : param_(p), kind_(SolverKind(p.type)) { CheckSolverParameter(p); }
   const SolverParameter& param() const { return param_; }
+  int kind() const { return kind_; }
+  // history blobs per learnable blob: 2 for AdaDelta and Adam (AdaDeltaPreSolve / AdamPreSolve), 1 otherwise
+  int num_histories() const { return kind_ == B2C_SOLVER_ADADELTA || kind_ == B2C_SOLVER_ADAM ? 2 : 1; }
   int iter() const { return iter_; }
   void set_iter(int i) { iter_ = i; }
   int current_step() const { return current_step_; }
@@ -324,6 +340,7 @@ class SGDSolver {
   void increment_iter() { ++iter_; }
  private:
   SolverParameter param_;
+  int kind_;
   ParamArena arena_;
   vector<ParamSpec> specs_;
   int iter_ = 0, current_step_ = 0;

@@ -112,17 +112,31 @@ int b2h_conv_algo_used(void* hv, int op) {
 void b2h_conv_destroy(void* hv) { delete static_cast<ConvHandle*>(hv); }
 
 // ---- solver / scheduler ---------------------------------------------------------------------------------------
+// a solver of any type (SGD, Nesterov, AdaGrad, RMSProp, AdaDelta, Adam) with its hyperparameters; NULL on a bad type or a failed
+// sanity check
+void* b2h_solver_create_typed(const char* type, float base_lr, const char* lr_policy, float gamma, float power, int stepsize,
+                              int max_iter, float momentum, float weight_decay, const char* reg_type, int iter_size, int reduce_buckets,
+                              int nstep, const int* stepvalue, int rampup_interval, float rampup_lr, float min_lr, float delta,
+                              float momentum2, float rms_decay) {
+  try {
+    SolverParameter p;
+    p.type = type; p.delta = delta; p.momentum2 = momentum2; p.rms_decay = rms_decay;
+    p.base_lr = base_lr; p.lr_policy = lr_policy; p.gamma = gamma; p.power = power; p.stepsize = stepsize; p.max_iter = max_iter;
+    p.momentum = momentum; p.weight_decay = weight_decay; p.regularization_type = reg_type; p.iter_size = iter_size;
+    p.reduce_buckets = reduce_buckets; p.rampup_interval = rampup_interval; p.rampup_lr = rampup_lr; p.min_lr = min_lr;
+    if (nstep) p.stepvalue.assign(stepvalue, stepvalue + nstep);
+    auto* h = new SolverHandle;
+    h->solver.reset(new SGDSolver(p));
+    return h;
+  } catch (const std::exception& e) { g_err = e.what(); return nullptr; }
+}
+// an SGD solver (b2h_solver_create_typed with type "SGD" and the SolverParameter defaults of the other solvers' fields)
 void* b2h_solver_create(float base_lr, const char* lr_policy, float gamma, float power, int stepsize, int max_iter,
                         float momentum, float weight_decay, const char* reg_type, int iter_size, int reduce_buckets,
                         int nstep, const int* stepvalue, int rampup_interval, float rampup_lr, float min_lr) {
-  SolverParameter p;
-  p.base_lr = base_lr; p.lr_policy = lr_policy; p.gamma = gamma; p.power = power; p.stepsize = stepsize; p.max_iter = max_iter;
-  p.momentum = momentum; p.weight_decay = weight_decay; p.regularization_type = reg_type; p.iter_size = iter_size;
-  p.reduce_buckets = reduce_buckets; p.rampup_interval = rampup_interval; p.rampup_lr = rampup_lr; p.min_lr = min_lr;
-  if (nstep) p.stepvalue.assign(stepvalue, stepvalue + nstep);
-  auto* h = new SolverHandle;
-  h->solver.reset(new SGDSolver(p));
-  return h;
+  const SolverParameter d;
+  return b2h_solver_create_typed("SGD", base_lr, lr_policy, gamma, power, stepsize, max_iter, momentum, weight_decay, reg_type, iter_size,
+                                 reduce_buckets, nstep, stepvalue, rampup_interval, rampup_lr, min_lr, d.delta, d.momentum2, d.rms_decay);
 }
 void b2h_solver_destroy(void* hv) { delete static_cast<SolverHandle*>(hv); }
 float b2h_solver_lr_at(void* hv, int iter) {
@@ -160,12 +174,18 @@ int b2h_solver_set(void* hv, int i, int diff, const float* src) {
     CUDA_CHECK(cudaMemcpy(diff ? b.mutable_gpu_diff() : b.mutable_gpu_data(), src, sizeof(float) * b.count(), cudaMemcpyHostToDevice));
   });
 }
-int b2h_solver_get(void* hv, int i, int what, float* dst) {   // what: 0 data, 1 diff, 2 history
+// the device address of history `what` (2: history, 3: second history -- AdaDelta / Adam only) of arena slot i
+static float* history_at(SGDSolver& s, int what, int i) {
+  float* base = what == 2 ? s.arena().history() : s.arena().history2();
+  B2_CHECK(base != nullptr, "solver type " + s.param().type + " keeps no second history");
+  return base + s.arena().offset(i);
+}
+int b2h_solver_get(void* hv, int i, int what, float* dst) {   // what: 0 data, 1 diff, 2 history, 3 second history
   auto* h = static_cast<SolverHandle*>(hv);
   B2H_TRY({
     Blob& b = *h->params[i];
     CUDA_CHECK(cudaDeviceSynchronize());
-    const float* src = what == 0 ? b.gpu_data() : what == 1 ? b.gpu_diff() : h->solver->arena().history() + h->solver->arena().offset(i);
+    const float* src = what == 0 ? b.gpu_data() : what == 1 ? b.gpu_diff() : history_at(*h->solver, what, i);
     CUDA_CHECK(cudaMemcpy(dst, src, sizeof(float) * b.count(), cudaMemcpyDeviceToHost));
   });
 }
@@ -239,8 +259,9 @@ int b2h_net_layer_uses_database(void* h, int i) {
 }
 int b2h_net_reduce_buckets(void* h) { return static_cast<Net*>(h)->reduce_buckets(); }
 
-// SolverParameter from a solver.prototxt; returns an SGDSolver handle (same as b2h_solver_create)
-void* b2h_solver_from_file(const char* path_or_text, int is_text, char* net_path, int cap) {
+// SolverParameter from a solver.prototxt of any type (SGD, Nesterov, AdaGrad, RMSProp, AdaDelta, Adam; `type` or the legacy
+// `solver_type`); returns a solver handle like b2h_solver_create_typed
+void* b2h_solver_open(const char* path_or_text, int is_text, char* net_path, int cap) {
   try {
     PMessage m = is_text ? ParseTextProto(path_or_text) : ParseTextProtoFile(path_or_text);
     std::string np;
@@ -251,10 +272,26 @@ void* b2h_solver_from_file(const char* path_or_text, int is_text, char* net_path
     return h;
   } catch (const std::exception& e) { g_err = e.what(); return nullptr; }
 }
+// the same, for SGD solver files only: a caller that asked for an SGD solver is refused a file of another type
+void* b2h_solver_from_file(const char* path_or_text, int is_text, char* net_path, int cap) {
+  auto* h = static_cast<SolverHandle*>(b2h_solver_open(path_or_text, is_text, net_path, cap));
+  if (h && h->solver->kind() != B2C_SOLVER_SGD) {
+    g_err = "solver type '" + h->solver->param().type + "' asked of an SGD solver handle (SGD only; b2h_solver_open reads every type)";
+    delete h;
+    return nullptr;
+  }
+  return h;
+}
 int b2h_solver_describe(void* hv, float* base_lr, float* momentum, float* weight_decay, int* max_iter, int* iter_size, char* policy, int cap) {
   const SolverParameter& p = static_cast<SolverHandle*>(hv)->solver->param();
   *base_lr = p.base_lr; *momentum = p.momentum; *weight_decay = p.weight_decay; *max_iter = p.max_iter; *iter_size = p.iter_size;
   snprintf(policy, cap, "%s", p.lr_policy.c_str());
+  return 0;
+}
+int b2h_solver_hparams(void* hv, char* type, int cap, float* delta, float* momentum2, float* rms_decay) {
+  const SolverParameter& p = static_cast<SolverHandle*>(hv)->solver->param();
+  snprintf(type, cap, "%s", p.type.c_str());
+  *delta = p.delta; *momentum2 = p.momentum2; *rms_decay = p.rms_decay;
   return 0;
 }
 
@@ -358,14 +395,13 @@ long long b2h_trainer_param_count(void* hv, int i) {
   auto* h = static_cast<TrainerHandle*>(hv);
   return (long long)h->net->learnable_params()[h->net->trainable_ids()[i]]->count();
 }
-int b2h_trainer_param(void* hv, int i, int what, int set, float* buf) {   // what: 0 data, 1 diff, 2 history
+int b2h_trainer_param(void* hv, int i, int what, int set, float* buf) {   // what: 0 data, 1 diff, 2 history, 3 second history
   auto* h = static_cast<TrainerHandle*>(hv);
   B2H_TRY({
     const int id = h->net->trainable_ids().at(i);
     Blob& b = *h->net->learnable_params()[id];
     CUDA_CHECK(cudaDeviceSynchronize());
-    float* dev = what == 0 ? b.mutable_gpu_data() : what == 1 ? b.mutable_gpu_diff()
-                                                              : h->net->solver().arena().history() + h->net->solver().arena().offset(id);
+    float* dev = what == 0 ? b.mutable_gpu_data() : what == 1 ? b.mutable_gpu_diff() : history_at(h->net->solver(), what, id);
     if (set) { CUDA_CHECK(cudaMemcpy(dev, buf, sizeof(float) * b.count(), cudaMemcpyHostToDevice)); if (what == 0) h->net->MarkParamsDirty(); }
     else CUDA_CHECK(cudaMemcpy(buf, dev, sizeof(float) * b.count(), cudaMemcpyDeviceToHost));
   });

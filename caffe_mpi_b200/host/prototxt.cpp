@@ -453,8 +453,21 @@ SolverParameter ReadSolverParameter(const PMessage& m, std::string* net_path) {
   p.rampup_lr = (float)m.num("rampup_lr", 0.0);
   p.min_lr = (float)m.num("min_lr", 0.0);
   p.snapshot_diff = m.boolean("snapshot_diff", false);
-  const std::string type = m.str("type", "SGD");
-  if (type != "SGD") Fatal(__FILE__, __LINE__, "solver type '" + type + "' is outside this path (SGD only; REGISTER_SOLVER_CLASS(SGD), sgd_solver.cpp:357)");
+  p.delta = (float)m.num("delta", 1e-8);
+  p.momentum2 = (float)m.num("momentum2", 0.999);
+  p.rms_decay = (float)m.num("rms_decay", 0.0);
+  // the legacy solver_type enum (caffe.proto:288-297) becomes `type` as in UpgradeSolverType (upgrade_proto.cpp:1002-1040)
+  p.type = m.str("type", "SGD");
+  if (m.has("solver_type")) {
+    B2_CHECK(!m.has("type"), "Failed to upgrade solver: old solver_type field (enum) and new type field (string) cannot be both "
+                             "specified in solver proto text.");
+    static const char* const legacy[][2] = {{"SGD", "SGD"}, {"NESTEROV", "Nesterov"}, {"ADAGRAD", "AdaGrad"},
+                                            {"RMSPROP", "RMSProp"}, {"ADADELTA", "AdaDelta"}, {"ADAM", "Adam"}};
+    const std::string e = m.str("solver_type");
+    p.type.clear();
+    for (auto& l : legacy) if (e == l[0] || e == std::to_string(&l - legacy)) p.type = l[1];
+    if (p.type.empty()) Fatal(__FILE__, __LINE__, "Unknown SolverParameter solver_type: " + e + " (known: SGD, NESTEROV, ADAGRAD, RMSPROP, ADADELTA, ADAM)");
+  }
   if (net_path) *net_path = m.str("net", m.str("train_net"));
   return p;
 }

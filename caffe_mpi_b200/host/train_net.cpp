@@ -779,12 +779,14 @@ string TrainNet::Snapshot(const string& prefix) {
   WriteBinaryFile(stem + ".caffemodel", SerializeNetWeights(nw));
   SolverStateData st;
   st.iter = solver_->iter(); st.current_step = solver_->current_step(); st.learned_net = stem + ".caffemodel";
+  // the reference's history_ layout: [h_0 .. h_np-1], then for AdaDelta / Adam [h2_0 .. h2_np-1] (AdamPreSolve, adam_solver.cpp:8-16)
   ParamArena& ar = solver_->arena();
-  for (size_t i = 0; i < learnable_.size(); ++i) {
-    vector<float> h(learnable_[i]->count());
-    CUDA_CHECK(cudaMemcpy(h.data(), ar.history() + ar.offset((int)i), sizeof(float) * h.size(), cudaMemcpyDeviceToHost));
-    st.history.push_back(to_blob_data(learnable_[i]->shape(), h.data(), h.size()));
-  }
+  for (int k = 0; k < solver_->num_histories(); ++k)
+    for (size_t i = 0; i < learnable_.size(); ++i) {
+      vector<float> h(learnable_[i]->count());
+      CUDA_CHECK(cudaMemcpy(h.data(), (k ? ar.history2() : ar.history()) + ar.offset((int)i), sizeof(float) * h.size(), cudaMemcpyDeviceToHost));
+      st.history.push_back(to_blob_data(learnable_[i]->shape(), h.data(), h.size()));
+    }
   WriteBinaryFile(stem + ".solverstate", SerializeSolverState(st));
   return stem + ".solverstate";
 }
@@ -811,11 +813,14 @@ int TrainNet::CopyTrainedLayersFrom(const string& path) {
 void TrainNet::Restore(const string& state_path) {
   const SolverStateData st = ParseSolverState(ReadBinaryFile(state_path));
   if (!st.learned_net.empty()) CopyTrainedLayersFrom(st.learned_net);
-  B2_CHECK(st.history.size() == learnable_.size(), "Incorrect length of history blobs.");      // sgd_solver.cpp:334
+  const size_t np = learnable_.size();
+  B2_CHECK(st.history.size() == np * solver_->num_histories(), "Incorrect length of history blobs.");      // sgd_solver.cpp:334
   ParamArena& ar = solver_->arena();
-  for (size_t i = 0; i < learnable_.size(); ++i) {
-    B2_CHECK(st.history[i].data.size() == learnable_[i]->count(), "history blob " + std::to_string(i) + ": size mismatch");
-    CUDA_CHECK(cudaMemcpy(ar.history() + ar.offset((int)i), st.history[i].data.data(), sizeof(float) * learnable_[i]->count(), cudaMemcpyHostToDevice));
+  for (size_t j = 0; j < st.history.size(); ++j) {
+    const size_t i = j % np;
+    B2_CHECK(st.history[j].data.size() == learnable_[i]->count(), "history blob " + std::to_string(j) + ": size mismatch");
+    CUDA_CHECK(cudaMemcpy((j < np ? ar.history() : ar.history2()) + ar.offset((int)i), st.history[j].data.data(),
+                          sizeof(float) * learnable_[i]->count(), cudaMemcpyHostToDevice));
   }
   solver_->set_iter(st.iter);
   solver_->set_current_step(st.current_step);

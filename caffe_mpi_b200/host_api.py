@@ -42,6 +42,8 @@ def lib():
         L.b2h_conv_destroy.argtypes = [vp]
         L.b2h_solver_create.restype = vp
         L.b2h_solver_create.argtypes = [f, C.c_char_p, f, f, i, i, f, f, C.c_char_p, i, i, i, ip, i, f, f]
+        L.b2h_solver_create_typed.restype = vp
+        L.b2h_solver_create_typed.argtypes = [C.c_char_p, f, C.c_char_p, f, f, i, i, f, f, C.c_char_p, i, i, i, ip, i, f, f, f, f, f]
         L.b2h_solver_destroy.argtypes = [vp]
         L.b2h_solver_lr_at.argtypes = [vp, i]
         L.b2h_solver_lr_at.restype = f
@@ -118,13 +120,18 @@ class ConvolutionLayer:
 
 
 class SGDSolver:
+    """caffe::SGDSolver over a standalone arena.  `type` picks the update (SGD, Nesterov, AdaGrad, RMSProp, AdaDelta, Adam);
+    delta, momentum2 and rms_decay are the SolverParameter fields those read.  get(i, 3) is the second history (AdaDelta, Adam)."""
+
     def __init__(self, base_lr=0.01, lr_policy="fixed", gamma=0.1, power=1.0, stepsize=1, max_iter=1, momentum=0.0,
                  weight_decay=0.0, regularization_type="L2", iter_size=1, reduce_buckets=6, stepvalue=(), rampup_interval=0,
-                 rampup_lr=0.0, min_lr=0.0):
+                 rampup_lr=0.0, min_lr=0.0, type="SGD", delta=1e-8, momentum2=0.999, rms_decay=0.0):
         sv = list(stepvalue)
-        self._h = lib().b2h_solver_create(base_lr, lr_policy.encode(), gamma, power, stepsize, max_iter, momentum, weight_decay,
-                                          regularization_type.encode(), iter_size, reduce_buckets, len(sv), _ia(sv) if sv else None,
-                                          rampup_interval, rampup_lr, min_lr)
+        self._h = lib().b2h_solver_create_typed(type.encode(), base_lr, lr_policy.encode(), gamma, power, stepsize, max_iter, momentum,
+                                                weight_decay, regularization_type.encode(), iter_size, reduce_buckets, len(sv),
+                                                _ia(sv) if sv else None, rampup_interval, rampup_lr, min_lr, delta, momentum2, rms_decay)
+        if not self._h:
+            raise HostError(lib().b2h_last_error().decode())
 
     def lr_at(self, it):
         v = lib().b2h_solver_lr_at(self._h, it)
@@ -244,18 +251,24 @@ class Net:
             self._h = None
 
 
-def solver_from_prototxt(path_or_text, is_text=False):
-    """(SGDSolver, net_path) from a solver.prototxt."""
+def solver_from_prototxt(path_or_text, is_text=False, entry="b2h_solver_from_file"):
+    """(SGDSolver, net_path) from a solver.prototxt of type SGD; any other type is refused (open_solver reads every type)."""
     L = lib()
-    L.b2h_solver_from_file.restype = C.c_void_p
-    L.b2h_solver_from_file.argtypes = [C.c_char_p, C.c_int, C.c_char_p, C.c_int]
+    fn = getattr(L, entry)
+    fn.restype = C.c_void_p
+    fn.argtypes = [C.c_char_p, C.c_int, C.c_char_p, C.c_int]
     buf = C.create_string_buffer(512)
-    h = L.b2h_solver_from_file(path_or_text.encode(), int(is_text), buf, 512)
+    h = fn(path_or_text.encode(), int(is_text), buf, 512)
     if not h:
         raise HostError(L.b2h_last_error().decode())
     s = SGDSolver.__new__(SGDSolver)
     s._h = h
     return s, buf.value.decode()
+
+
+def open_solver(path_or_text, is_text=False):
+    """(solver, net_path) from a solver.prototxt of any type: `type`, or the legacy `solver_type` enum."""
+    return solver_from_prototxt(path_or_text, is_text, entry="b2h_solver_open")
 
 
 def textproto_scalar(path_or_text, key, default=None, is_text=False):
@@ -276,7 +289,11 @@ def solver_describe(s):
     d, e = C.c_int(), C.c_int()
     pol = C.create_string_buffer(64)
     L.b2h_solver_describe(s._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d), C.byref(e), pol, 64)
-    return dict(base_lr=a.value, momentum=b.value, weight_decay=c.value, max_iter=d.value, iter_size=e.value, lr_policy=pol.value.decode())
+    L.b2h_solver_hparams.argtypes = [C.c_void_p, C.c_char_p, C.c_int] + [C.POINTER(C.c_float)] * 3
+    ty, delta, m2, rho = C.create_string_buffer(64), C.c_float(), C.c_float(), C.c_float()
+    L.b2h_solver_hparams(s._h, ty, 64, C.byref(delta), C.byref(m2), C.byref(rho))
+    return dict(base_lr=a.value, momentum=b.value, weight_decay=c.value, max_iter=d.value, iter_size=e.value, lr_policy=pol.value.decode(),
+                type=ty.value.decode(), delta=delta.value, momentum2=m2.value, rms_decay=rho.value)
 
 
 # ---------------------------------------------------------------------------------------------- TrainNet
@@ -387,6 +404,7 @@ class Trainer:
         return lib().b2h_trainer_num_learnable(self._h)
 
     def get_param(self, i, what=0):
+        """what: 0 data, 1 diff, 2 history, 3 second history (AdaDelta, Adam)."""
         out = np.empty(lib().b2h_trainer_param_count(self._h, i), np.float32)
         _ck(lib().b2h_trainer_param(self._h, i, what, 0, out))
         return out

@@ -282,6 +282,40 @@ int b2c_sgd_update_arena(int nseg, const size_t* offset, const size_t* count,
                          float* g, float* w, float* h, float momentum, int l2,
                          float grad_scale, int clear_grads, void* stream);
 
+/* ---- the other solvers, fused over the arena ------------------------------------------------
+ * Same segments, host arrays and folded grad_scale as b2c_sgd_update_arena; per element, with
+ * gr = grad_scale*g + local_decay*reg(w), lr = local_rate[s]:
+ *   SGD       h = momentum*h + lr*gr; u = h                    (b2c_sgd_update_arena, bit for bit)
+ *   NESTEROV  h' = momentum*h + lr*gr; u = (1+momentum)*h' - momentum*h
+ *             replaces NesterovRegUpdateAllAndClear (src/caffe/solvers/nesterov_solver.cu:12-25)
+ *   ADAGRAD   h += gr^2; u = lr*gr / (sqrt(h) + max(delta, 1e-3))
+ *             replaces AdaGradRegUpdateAllAndClear (adagrad_solver.cu:11-23, delta clamp adagrad_solver.cpp:22)
+ *   RMSPROP   h = rms_decay*h + (1-rms_decay)*gr^2; u = lr*gr / (sqrt(h) + max(delta, 1e-4))
+ *             replaces RMSPropRegUpdateAllAndClear (rmsprop_solver.cu:12-23, rmsprop_solver.cpp:25)
+ *   ADADELTA  h = momentum*h + (1-momentum)*gr^2; gr *= sqrt((h2+d)/(h+d)); h2 = momentum*h2 + (1-momentum)*gr^2;
+ *             u = lr*gr, d = max(delta, 1e-3)
+ *             replaces AdaDeltaRegUpdateAllAndClear (adadelta_solver.cu:12-26, adadelta_solver.cpp:36)
+ *   ADAM      h = beta1*h + (1-beta1)*gr; h2 = beta2*h2 + (1-beta2)*gr^2; u = lr*h / (sqrt(h2) + max(delta, 1e-4))
+ *             replaces AdamRegUpdateAllAndClear (adam_solver.cu:11-24).  The bias correction
+ *             sqrt(1-beta2^t)/(1-beta1^t) is NOT applied here: fold it into local_rate (adam_solver.cpp:42-43).
+ * then w -= u; g = clear_grads ? 0 : u.  h2 (same offsets as h) is read only by ADADELTA and ADAM and may be NULL
+ * otherwise.  sqrt and division are IEEE-rounded.  Fields of b2c_solver_hparams a kind does not name are ignored. */
+enum b2c_solver_kind {
+  B2C_SOLVER_SGD = 0, B2C_SOLVER_NESTEROV = 1, B2C_SOLVER_ADAGRAD = 2, B2C_SOLVER_RMSPROP = 3,
+  B2C_SOLVER_ADADELTA = 4, B2C_SOLVER_ADAM = 5
+};
+typedef struct b2c_solver_hparams {
+  float momentum;   /* SGD, NESTEROV, ADADELTA */
+  float delta;      /* ADAGRAD, RMSPROP, ADADELTA, ADAM (epsilon); clamped as above */
+  float rms_decay;  /* RMSPROP */
+  float beta1;      /* ADAM (SolverParameter.momentum) */
+  float beta2;      /* ADAM (SolverParameter.momentum2) */
+} b2c_solver_hparams;
+int b2c_solver_update_arena(int kind, int nseg, const size_t* offset, const size_t* count,
+                            const float* local_rate, const float* local_decay,
+                            float* g, float* w, float* h, float* h2, b2c_solver_hparams hp,
+                            int l2, float grad_scale, int clear_grads, void* stream);
+
 /* ---- gradient exchange ---------------------------------------------------------------------
  * Replaces P2PManager/P2PSync's NCCL use (src/caffe/parallel.cpp:36-87,145-253) and the MPI
  * bootstrap (src/caffe/clusters.cpp:8-16; parallel.cpp:42-45,163-172).  One communicator per

@@ -78,13 +78,20 @@ def build_trainer(args, net, net_is_text, solver, solver_is_text):
     return t, rank, world
 
 
+def solver_hparams_text(d):
+    """The hyperparameters the solver type reads (solver_describe's dict), for the "Solving" line."""
+    keys = {"SGD": ("momentum",), "Nesterov": ("momentum",), "AdaGrad": ("delta",), "RMSProp": ("rms_decay", "delta"),
+            "AdaDelta": ("momentum", "delta"), "Adam": ("momentum", "momentum2", "delta")}[d["type"]]
+    return " ".join("%s %g" % (k, d[k]) for k in keys)
+
+
 def cmd_train(args):
     from caffe_mpi_b200 import host_api
     if not args.solver:
         sys.exit("caffe.py train: Need a solver definition to train (--solver=...)")
     if args.snapshot and args.weights:
         sys.exit("caffe.py train: Give a snapshot to resume training or weights to finetune but not both.")   # tools/caffe.cpp:166
-    s, net_path = host_api.solver_from_prototxt(args.solver)
+    s, net_path = host_api.open_solver(args.solver)
     d = host_api.solver_describe(s)
     net_path = args.model or net_path
     if not os.path.exists(net_path):
@@ -111,8 +118,8 @@ def cmd_train(args):
     snap_after = sp("snapshot_after_train", "true").lower() in ("true", "1")
     if rank == 0:
         log("Data layer: %s" % ("reading the LMDB named by data_param.source" if t.database_batches() >= 0 else "synthetic in-memory source"))
-        log("Solving %s: %d learnable blobs, lr_policy %s base_lr %g momentum %g weight_decay %g, %d iteration(s) on %d GPU(s)" %
-            (net_path, t.num_params(), d["lr_policy"], d["base_lr"], d["momentum"], d["weight_decay"], iters, world))
+        log("Solving %s with %s: %d learnable blobs, lr_policy %s base_lr %g %s weight_decay %g, %d iteration(s) on %d GPU(s)" %
+            (net_path, d["type"], t.num_params(), d["lr_policy"], d["base_lr"], solver_hparams_text(d), d["weight_decay"], iters, world))
     try:
         batch = len(t.get_blob("label"))           # images per rank and step, for the img/s figure
     except host_api.HostError:
