@@ -670,6 +670,7 @@ void P2PSync::allreduce_bucket(float* buf, size_t count) {
   CUDA_CHECK(cudaEventRecord(t.b, comm_stream_));
   timed_.push_back(t);
 }
+void P2PSync::allreduce_scores(float* buf, size_t count) { B2C_CHECK(b2c_comm_allreduce_sum(comm_, buf, count, comm_stream_)); }
 void P2PSync::collect_bucket_times(vector<size_t>* bytes, vector<float>* ms) {
   CUDA_CHECK(cudaStreamSynchronize(comm_stream_));
   for (TimedBucket& t : timed_) {

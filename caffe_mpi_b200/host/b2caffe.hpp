@@ -304,6 +304,11 @@ struct SolverParameter {   // caffe.proto SolverParameter (fields this path read
   bool snapshot_diff = false;
   float global_grad_scale = 1.f;   // NetParameter.global_grad_scale (caffe.proto:130)
   int reduce_buckets = 6;          // NetParameter.reduce_buckets (caffe.proto:140)
+  // testing (caffe.proto:184-188): one TEST net per test_iter entry, built from `net`; a pass every test_interval iterations
+  vector<int> test_iter;
+  int test_interval = 0;
+  bool test_compute_loss = false;
+  vector<string> test_fields_not_built;   // test_net, test_net_param, test_state when present: test nets from those are not built
 };
 
 // b2c_solver_kind of a SolverParameter.type (REGISTER_SOLVER_CLASS names); an unknown type is fatal and lists the known ones
@@ -378,7 +383,10 @@ class P2PSync : public SolverCallback {
   cudaStream_t comm_stream() const override { return comm_stream_; }
   void on_start(ParamArena& arena) override;                          // parallel.cpp:208-227
   void allreduce_bucket(float* buf, size_t count) override;           // parallel.cpp:245-253 (async, comm stream)
-  void soft_barrier() override;                                       // parallel.cpp: MPI_Barrier -> comm-stream drain
+  // the test scores' sum over the ranks (saveTestResults / aggregateTestResults, parallel.cpp:256-282), async on the comm stream;
+  // a sibling of allreduce_bucket so that bucket timing never counts it as a gradient bucket
+  void allreduce_scores(float* buf, size_t count);
+  void soft_barrier() override;                                      // parallel.cpp: MPI_Barrier -> comm-stream drain
   void reduce_barrier() override;
   // batch division of parallel.cpp:284-293: per-rank batch, rounded up to a multiple
   static int divide_batch_size(int total, int solver_count);

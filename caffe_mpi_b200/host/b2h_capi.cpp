@@ -294,6 +294,18 @@ int b2h_solver_hparams(void* hv, char* type, int cap, float* delta, float* momen
   *delta = p.delta; *momentum2 = p.momentum2; *rms_decay = p.rms_decay;
   return 0;
 }
+// the testing fields: returns the number of test_iter entries (the first `cap` of them land in test_iter); not_built gets the names of
+// the test-net sources present that are not built (test_net, test_net_param, test_state), space-separated
+int b2h_solver_testing(void* hv, int* test_iter, int cap, int* test_interval, int* test_compute_loss, char* not_built, int nb_cap) {
+  const SolverParameter& p = static_cast<SolverHandle*>(hv)->solver->param();
+  for (int i = 0; i < (int)p.test_iter.size() && i < cap; ++i) test_iter[i] = p.test_iter[i];
+  *test_interval = p.test_interval;
+  *test_compute_loss = p.test_compute_loss ? 1 : 0;
+  std::string nb;
+  for (const std::string& f : p.test_fields_not_built) nb += (nb.empty() ? "" : " ") + f;
+  snprintf(not_built, nb_cap, "%s", nb.c_str());
+  return (int)p.test_iter.size();
+}
 
 // first scalar value of a top-level field of a text-format message (tools/caffe.py reads SolverParameter.display / snapshot /
 // snapshot_prefix / snapshot_after_train / random_seed with it); returns 1 if present, 0 if absent, -1 on a parse error
@@ -554,6 +566,20 @@ int b2h_tester_test(void* hv, int iterations, float* per_batch, float* mean, flo
     memcpy(per_batch, pb.data(), sizeof(float) * pb.size());
     memcpy(mean, m.data(), sizeof(float) * m.size());
   });
+}
+// Solver::Test's pass (TrainNet::TestPass): scores summed on the device (over the ranks too when the tester shares a multi-GPU trainer),
+// one read at the end.  between (may be null) is called before every batch with its index; a zero return stops the pass there.
+// Returns the number of batches run (= iterations unless stopped), -1 on error; means / loss are written only for a whole pass.
+int b2h_tester_test_pass(void* hv, int iterations, float* means, float* loss, int (*between)(int)) {
+  auto* h = static_cast<TesterHandle*>(hv);
+  try {
+    vector<float> m;
+    std::function<bool(int)> hook;
+    if (between) hook = [between](int i) { return between(i) != 0; };
+    const int ran = h->net->TestPass(iterations, hook, &m, loss);
+    if (ran == iterations) memcpy(means, m.data(), sizeof(float) * m.size());
+    return ran;
+  } catch (const std::exception& e) { g_err = e.what(); return -1; }
 }
 long long b2h_tester_blob_count(void* hv, const char* name) {
   Blob* b = static_cast<TesterHandle*>(hv)->net->blob(name);

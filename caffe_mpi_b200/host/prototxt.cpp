@@ -468,6 +468,14 @@ SolverParameter ReadSolverParameter(const PMessage& m, std::string* net_path) {
     for (auto& l : legacy) if (e == l[0] || e == std::to_string(&l - legacy)) p.type = l[1];
     if (p.type.empty()) Fatal(__FILE__, __LINE__, "Unknown SolverParameter solver_type: " + e + " (known: SGD, NESTEROV, ADAGRAD, RMSPROP, ADADELTA, ADAM)");
   }
+  // testing: test nets come from the generic `net` only (Solver::InitTestNets, solver.cpp:107-185; the reference's model files
+  // use nothing else), with phase TEST and no stages.  The other sources are recorded, and refused where test nets are built
+  for (const char* f : {"test_net", "test_net_param", "test_state"})
+    if (m.has(f)) p.test_fields_not_built.push_back(f);
+  for (long long v : m.ints("test_iter")) p.test_iter.push_back((int)v);
+  p.test_interval = (int)m.integer("test_interval", 0);
+  p.test_compute_loss = m.boolean("test_compute_loss", false);
+  if (!p.test_iter.empty()) B2_CHECK(p.test_interval > 0, "(test_interval > 0 when test_iter is given)");   // solver.cpp:135-137 CHECK_GT
   if (net_path) *net_path = m.str("net", m.str("train_net"));
   return p;
 }

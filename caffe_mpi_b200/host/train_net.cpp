@@ -634,7 +634,10 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
   }
   CUDA_CHECK(cudaStreamSynchronize(S()));
 }
-TrainNet::~TrainNet() {}
+TrainNet::~TrainNet() {
+  if (pass_scored_) cudaEventDestroy(pass_scored_);
+  if (pass_reduced_) cudaEventDestroy(pass_reduced_);
+}
 
 void TrainNet::AttachSync(P2PSync* sync) {
   sync_ = sync;
@@ -848,6 +851,9 @@ void TrainNet::ShareTrainedLayersWith(TrainNet& train) {
       learnable_[nodes_[i].first_param + j] = src[j];
     }
   }
+  // a multi-GPU trainer: rank r scores its stripe of the validation database (Net::Init's TEST DataReader gets (solver_count, rank))
+  test_sync_ = train.sync_;
+  if (test_sync_ && db_data_) db_data_->set_solver(test_sync_->nranks(), test_sync_->rank());
   filters_dirty_ = true;
 }
 void TrainNet::ForwardTest() {
@@ -880,6 +886,69 @@ float TrainNet::Test(int iterations, vector<float>* per_batch, vector<float>* me
   mean->resize(width);
   for (size_t k = 0; k < width; ++k) (*mean)[k] = sum[k] / iterations;
   return loss / iterations;
+}
+int TrainNet::TestPass(int iterations, const std::function<bool(int)>& before_batch, vector<float>* mean, float* loss) {
+  const int ran = EnqueueTestPass(iterations, before_batch);
+  if (ran == iterations) ReadTestPass(mean, loss);
+  return ran;
+}
+int TrainNet::EnqueueTestPass(int iterations, const std::function<bool(int)>& before_batch) {
+  B2_CHECK(test_, "TestPass: the net was built for the TRAIN phase");
+  B2_CHECK(iterations > 0, "TestPass: iterations must be positive");
+  B2_CHECK(pass_batches_ == 0, "TestPass: the previous pass was never read");
+  // the shared weights changed since the last pass.  This stream waited for the trainer's last update at the end of its step
+  // (ReduceScheduler::end_of_iteration), so the forwards below read the updated weights; the trainer's next step is enqueued
+  // behind them on the same stream, so its updates cannot overtake them.
+  filters_dirty_ = true;
+  size_t width = 0;
+  for (const Output& o : outputs_) width += o.blob->count();
+  if (scores_.count() != std::max<size_t>(width, 1)) scores_.Reshape({(int)std::max<size_t>(width, 1)});
+  float* score = scores_.mutable_gpu_data();
+  CUDA_CHECK(cudaMemsetAsync(score, 0, sizeof(float) * scores_.count(), S()));
+  for (int i = 0; i < iterations; ++i) {
+    if (before_batch && !before_batch(i)) return i;
+    ForwardTest();
+    size_t idx = 0;
+    for (const Output& o : outputs_) {                   // 0 + v, then + v per batch: Test()'s host sums (tools/caffe.cpp:272-289)
+      B2C_CHECK(b2c_add(o.blob->count(), score + idx, o.blob->gpu_data(), score + idx, S()));
+      idx += o.blob->count();
+    }
+  }
+  if (test_sync_ && test_sync_->nranks() > 1 && width) {
+    CUDA_CHECK(cudaEventCreateWithFlags(&pass_scored_, cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventCreateWithFlags(&pass_reduced_, cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventRecord(pass_scored_, S()));                  // the last batch's scores are in the vector ...
+    CUDA_CHECK(cudaStreamWaitEvent(test_sync_->comm_stream(), pass_scored_, 0));
+    test_sync_->allreduce_scores(score, width);                      // ... before it travels
+    CUDA_CHECK(cudaEventRecord(pass_reduced_, test_sync_->comm_stream()));
+    CUDA_CHECK(cudaStreamWaitEvent(S(), pass_reduced_, 0));
+  }
+  pass_batches_ = iterations;
+  return iterations;
+}
+void TrainNet::ReadTestPass(vector<float>* mean, float* loss) {
+  B2_CHECK(pass_batches_ > 0, "ReadTestPass: no whole pass was enqueued");
+  const int batches = pass_batches_, nranks = test_sync_ ? test_sync_->nranks() : 1;
+  pass_batches_ = 0;
+  size_t width = 0;
+  for (const Output& o : outputs_) width += o.blob->count();
+  vector<float> sum(width);
+  if (width) CUDA_CHECK(cudaMemcpyAsync(sum.data(), scores_.gpu_data(), sizeof(float) * width, cudaMemcpyDeviceToHost, S()));
+  CUDA_CHECK(cudaStreamSynchronize(S()));
+  if (pass_scored_) {
+    cudaEventDestroy(pass_scored_); cudaEventDestroy(pass_reduced_);
+    pass_scored_ = pass_reduced_ = nullptr;
+  }
+  // solver.cpp:527: score / test_iterations / solver_count, with the score summed over every rank (DESIGN.md section 8)
+  mean->resize(width);
+  float l = 0.f;
+  size_t idx = 0;
+  for (const Output& o : outputs_)
+    for (size_t k = 0; k < o.blob->count(); ++k, ++idx) {
+      (*mean)[idx] = sum[idx] / batches / nranks;
+      l += o.loss_weight * sum[idx];
+    }
+  *loss = l / batches / nranks;
 }
 float TrainNet::TimedForwards(int n) {
   cudaEvent_t a, b;

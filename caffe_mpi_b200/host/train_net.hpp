@@ -285,7 +285,8 @@ class TrainNet {
   bool has_solver() const { return solver_ != nullptr; }
   // ---- TEST phase only ----
   // Net::ShareTrainedLayersWith (net.cpp): a layer matched by name takes `train`'s parameter blobs by pointer (shapes must agree), so
-  // this net reads the weights and BatchNorm statistics the trainer keeps updating.  `train` must outlive this net.
+  // this net reads the weights and BatchNorm statistics the trainer keeps updating.  `train` must outlive this net.  When `train` has
+  // a P2PSync attached (call this after AttachSync), this net's database reads the rank's stripe and TestPass sums over the ranks.
   void ShareTrainedLayersWith(TrainNet& train);
   // Net::output_blobs (Net::Init's available_blobs: tops no later layer consumes, in name order) with their loss weights: the layer's
   // loss_weight, else 1 for a loss layer's first top and 0 otherwise
@@ -295,7 +296,18 @@ class TrainNet {
   // tools/caffe.cpp test(): `iterations` forwards on freshly prepared filter caches; per_batch gets every output element of every
   // batch (iterations x sum of output counts), mean their means; returns the mean loss (sum of loss_weight * output per batch)
   float Test(int iterations, vector<float>* per_batch, vector<float>* mean);
-  float TimedForwards(int n);                      // n ForwardTest calls bracketed by CUDA events; milliseconds
+  // Solver::Test (solver.cpp:445-540) without a host read per batch: `iterations` forwards on the thread stream, each batch's outputs
+  // added (b2c_add, output order) into a device score vector -- the float sums of Test(), bit for bit.  With a trainer's P2PSync
+  // (ShareTrainedLayersWith) the vector is then summed over the ranks by one allreduce on the comm stream, ordered after the last batch
+  // by an event.  One device -> host read at the end: mean = sum / batches / ranks, loss = sum_k loss_weight_k * mean_k.
+  // before_batch (may be empty) is asked before every batch; false stops the pass.  Returns the batches run; mean and loss are
+  // written only when all `iterations` ran.  Every rank of a multi-GPU trainer must run the whole pass (the allreduce waits for all).
+  int TestPass(int iterations, const std::function<bool(int)>& before_batch, vector<float>* mean, float* loss);
+  // TestPass in its two halves: everything up to the read (returns the batches enqueued; the reduction only follows a whole pass),
+  // then the read.  Several ranks driven from one host thread enqueue every rank's pass before reading any.
+  int EnqueueTestPass(int iterations, const std::function<bool(int)>& before_batch);
+  void ReadTestPass(vector<float>* mean, float* loss);
+  float TimedForwards(int n);                     // n ForwardTest calls bracketed by CUDA events; milliseconds
   void ProfileForwards(int n, vector<int>* layer, vector<int>* op, vector<float>* ms);   // ProfileSteps for ForwardTest
  private:
   struct Node {
@@ -317,6 +329,10 @@ class TrainNet {
   bool filters_dirty_ = true;
   bool test_ = false;                              // built from a TEST-phase Net: forward only
   vector<Output> outputs_;
+  P2PSync* test_sync_ = nullptr;                   // TEST phase: the P2PSync of the trainer this net shares (TestPass's reduction)
+  Blob scores_;                                    // TEST phase: TestPass's device score vector
+  int pass_batches_ = 0;                           // batches of the enqueued, unread pass
+  cudaEvent_t pass_scored_ = nullptr, pass_reduced_ = nullptr;   // its score allreduce: after the last batch, before the read
   bool fuse_fanout_ = true;                        // B2C_FUSE: conv layers add their bottom gradient into a fan-out blob's diff directly
   vector<ConvolutionLayer*> cached_convs_;
   float host_loss_ = 0.f;

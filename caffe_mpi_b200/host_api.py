@@ -292,8 +292,16 @@ def solver_describe(s):
     L.b2h_solver_hparams.argtypes = [C.c_void_p, C.c_char_p, C.c_int] + [C.POINTER(C.c_float)] * 3
     ty, delta, m2, rho = C.create_string_buffer(64), C.c_float(), C.c_float(), C.c_float()
     L.b2h_solver_hparams(s._h, ty, 64, C.byref(delta), C.byref(m2), C.byref(rho))
+    L.b2h_solver_testing.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_char_p, C.c_int]
+    ti, interval, tcl, nb = (C.c_int * 64)(), C.c_int(), C.c_int(), C.create_string_buffer(256)
+    n = L.b2h_solver_testing(s._h, ti, 64, C.byref(interval), C.byref(tcl), nb, 256)
+    if n > 64:
+        ti = (C.c_int * n)()
+        L.b2h_solver_testing(s._h, ti, n, C.byref(interval), C.byref(tcl), nb, 256)
     return dict(base_lr=a.value, momentum=b.value, weight_decay=c.value, max_iter=d.value, iter_size=e.value, lr_policy=pol.value.decode(),
-                type=ty.value.decode(), delta=delta.value, momentum2=m2.value, rms_decay=rho.value)
+                type=ty.value.decode(), delta=delta.value, momentum2=m2.value, rms_decay=rho.value,
+                test_iter=[ti[k] for k in range(n)], test_interval=interval.value, test_compute_loss=bool(tcl.value),
+                test_fields_not_built=nb.value.decode().split())
 
 
 # ---------------------------------------------------------------------------------------------- TrainNet
@@ -543,6 +551,22 @@ class Tester:
         per_batch, mean, loss = np.empty(iterations * width, np.float32), np.empty(max(width, 1), np.float32), C.c_float()
         _ck(lib().b2h_tester_test(self._h, iterations, per_batch, mean, C.byref(loss)))
         return per_batch.reshape(iterations, width), mean[:width], loss.value
+
+    def test_pass(self, iterations, between=None):
+        """Solver::Test's pass: (means [output elements], loss) of `iterations` batches, scores summed on the device -- and over the
+        ranks when the tester shares a trainer with an attached sync -- and read once at the end.  means = sum / batches / ranks, the
+        float sums of test(); loss = sum of loss_weight * mean.  between(i), if given, is called before batch i; a false return stops the
+        pass and test_pass returns None.  (On several ranks every rank must run the whole pass.)"""
+        L = lib()
+        hook_t = C.CFUNCTYPE(C.c_int, C.c_int)
+        L.b2h_tester_test_pass.argtypes = [C.c_void_p, C.c_int, _f32, C.POINTER(C.c_float), hook_t]
+        width = sum(n for _, _, n in self.outputs())
+        mean, loss = np.empty(max(width, 1), np.float32), C.c_float()
+        hook = hook_t(lambda i: 1 if between(i) else 0) if between else hook_t()
+        ran = L.b2h_tester_test_pass(self._h, iterations, mean, C.byref(loss), hook)
+        if ran < 0:
+            raise HostError(L.b2h_last_error().decode())
+        return (mean[:width], loss.value) if ran == iterations else None
 
     def get_blob(self, name):
         n = lib().b2h_tester_blob_count(self._h, name.encode())

@@ -16,9 +16,16 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def log(msg):
+def log(msg, stream=None):
     t = time.localtime()
-    print("I%02d%02d %02d:%02d:%02d caffe.py] %s" % (t.tm_mon, t.tm_mday, t.tm_hour, t.tm_min, t.tm_sec, msg), flush=True)
+    print("I%02d%02d %02d:%02d:%02d caffe.py] %s" % (t.tm_mon, t.tm_mday, t.tm_hour, t.tm_min, t.tm_sec, msg), flush=True, file=stream or sys.stdout)
+
+
+def log_test_net(msg):
+    """The test nets' log lines go to stderr -- the stream the reference logs everything to (glog, alsologtostderr) -- so that stdout
+    carries the same lines with and without test nets: a script reading the training loss from stdout's `loss = ` never picks up a
+    test net's `Test net output #i: loss = ...`."""
+    log(msg, sys.stderr)
 
 
 def cmd_device_query(_):
@@ -32,30 +39,44 @@ def cmd_device_query(_):
     log("libb2c version %s, %d device(s)" % (v.decode() if isinstance(v, bytes) else v, n.value))
 
 
-def schedule(it, end, display, snapshot):
+def schedule(it, end, display, snapshot, test_interval=0):
     """The shell's part of Solver::Step (solver.cpp:277-345) as a plan: yields (n, iter_after, show, snap) -- run n iterations,
     after which the iteration counter reads iter_after; print the loss line if `show` (iter % display == 0, or the run is over, or
-    display is off and this is the only chunk), write a snapshot if `snap` (iter % snapshot == 0)."""
+    display is off and this is the only chunk), write a snapshot if `snap` (iter % snapshot == 0).
+
+    With test_interval > 0 (a solver with test nets) every chunk also says which test pass runs BEFORE its iterations, as a fifth
+    element: "initial" (one batch per test net) when the counter reads 0 -- Step's iter_ == 0 branch, whatever test_initialization
+    says -- and "full" (test_iter batches) at every later multiple of test_interval except the one a resumed run starts at
+    (iterations_last_ = -1 after a restore), else None.  Solve's closing pass (solver.cpp:419-423, when the final counter is a multiple
+    of test_interval) comes last as (0, end, False, False, "final"); it is skipped when training stopped early."""
+    start = it
     while it < end:
+        test = None
+        if test_interval > 0:
+            test = "initial" if it == 0 else "full" if it > start and it % test_interval == 0 else None
         nxt = end
-        for every in (display, snapshot):
+        for every in (display, snapshot, test_interval):
             if every > 0:
                 nxt = min(nxt, (it // every + 1) * every)
         n, it = nxt - it, nxt
-        yield n, it, (display > 0 and it % display == 0) or it == end, snapshot > 0 and it % snapshot == 0
+        row = (n, it, (display > 0 and it % display == 0) or it == end, snapshot > 0 and it % snapshot == 0)
+        yield row + (test,) if test_interval > 0 else row
+    if test_interval > 0 and end % test_interval == 0:
+        yield 0, end, False, False, "final"
 
 
-def rank_batch(net, net_is_text, override, solver_count):
+def rank_batch(net, net_is_text, override, solver_count, phase="TRAIN"):
     """Per-solver batch size, or 0 for "what the prototxt says".  P2PSync::divide_batch_size (parallel.cpp:284-316): with more than
     one solver (GPU) on the node, the batch_size of the net's Data layer -- or the --batch override -- is the NODE's batch and each
     solver takes total / solver_count of it, the total first rounded up to a multiple of solver_count.  Nets fed by Input /
-    DummyData layers have no data_param and are left alone, as in the reference."""
+    DummyData layers have no data_param and are left alone, as in the reference.  phase="TEST" divides the TEST Data layer's batch
+    the same way (Net::Init does it for test nets too)."""
     from caffe_mpi_b200 import host_api
     if solver_count <= 1:
         return override
     total = override
     if not total:
-        data = [l for l in host_api.Net(net, is_text=net_is_text).layers() if l[1] == "Data"]
+        data = [l for l in host_api.Net(net, phase=phase, is_text=net_is_text).layers() if l[1] == "Data"]
         if not data:
             return 0
         total = data[0][2][0]
@@ -85,6 +106,20 @@ def solver_hparams_text(d):
     return " ".join("%s %g" % (k, d[k]) for k in keys)
 
 
+def test_net_lines(outputs, means, loss, compute_loss):
+    """Solver::Test's log lines after a pass (solver.cpp:521-538): `outputs` = [(name, loss_weight, count)] in the net's output order,
+    `means` = one value per output element, `loss` = the mean loss, printed only with test_compute_loss."""
+    import numpy as np
+    lines = ["Test loss: %g" % loss] if compute_loss else []
+    i = 0
+    for name, w, n in outputs:
+        for _ in range(n):
+            m = np.float32(means[i])
+            lines.append("    Test net output #%d: %s = %g%s" % (i, name, m, " (* %g = %g loss)" % (w, np.float32(w) * m) if w else ""))
+            i += 1
+    return lines
+
+
 def cmd_train(args):
     from caffe_mpi_b200 import host_api
     if not args.solver:
@@ -94,6 +129,9 @@ def cmd_train(args):
     s, net_path = host_api.open_solver(args.solver)
     d = host_api.solver_describe(s)
     net_path = args.model or net_path
+    for f in d["test_fields_not_built"]:
+        sys.exit("caffe.py train: SolverParameter.%s is not built: test nets are built from the solver's `net` with phase TEST, one per "
+                 "test_iter entry" % f)
     if not os.path.exists(net_path):
         sys.exit("caffe.py train: net file %r named by the solver does not exist (paths are relative to the working directory)" % net_path)
     if args.seed < 0:
@@ -124,6 +162,18 @@ def cmd_train(args):
         batch = len(t.get_blob("label"))           # images per rank and step, for the img/s figure
     except host_api.HostError:
         batch = 0
+    # Solver::InitTestNets (solver.cpp:107-185): one TEST net per test_iter entry, from the solver's net file, sharing the trainer's
+    # layers by name; each rank scores its stripe of the validation database at the per-rank TEST batch
+    testers = []
+    if d["test_iter"]:
+        test_batch = rank_batch(net_path, False, 0, int(os.environ.get("LOCAL_WORLD_SIZE", world)), phase="TEST")
+        for k, n_iter in enumerate(d["test_iter"]):
+            if rank == 0:
+                log_test_net("Creating test net (#%d) specified by net file: %s" % (k, net_path))
+            te = host_api.Tester(net_path, batch=test_batch, num_classes=args.classes, seed=args.seed + rank, net_is_text=False)
+            te.share_trained_layers_with(t)
+            testers.append((te, n_iter))
+    test_every = d["test_interval"] if testers else 0
     end = t.iter() + args.iterations if args.iterations else max(d["max_iter"], t.iter())   # a resumed run goes on to max_iter
     last_snapshot = -1
     # SignalHandler (src/caffe/util/signal_handler.cpp, tools/caffe.cpp:43-48,209-214): SIGINT = stop (with a snapshot when
@@ -133,7 +183,50 @@ def cmd_train(args):
     signal.signal(signal.SIGINT, lambda *_: got.__setitem__("stop", True))
     if hasattr(signal, "SIGHUP"):
         signal.signal(signal.SIGHUP, lambda *_: got.__setitem__("snapshot", True))
-    for n, it, show, snap in schedule(t.iter(), end, display, snap_every):
+
+    def between_batches(_):
+        # Solver::Test's GetRequestedAction before every batch (solver.cpp:461-475), one GPU only: on several GPUs a rank that left
+        # a pass early would leave the others waiting in the score allreduce, so there the flags are read when the pass is over
+        nonlocal last_snapshot
+        if got["snapshot"] and rank == 0 and snap_prefix:
+            log("Snapshotting solver state to binary proto file %s" % t.snapshot(snap_prefix))
+            last_snapshot = t.iter()
+        got["snapshot"] = False
+        return not got["stop"]
+
+    def test_all(it, kind):
+        """Solver::TestAll; returns True when a SIGINT ended it ("Test interrupted.")."""
+        nonlocal last_snapshot
+        for k, (te, n_iter) in enumerate(testers):
+            if rank == 0:
+                log_test_net("Iteration %d, Testing net (#%d)" % (it, k))
+            r = te.test_pass(1 if kind == "initial" else n_iter, between_batches if world == 1 else None)
+            if r is None:
+                log_test_net("Test interrupted.")
+                return True
+            if rank == 0:
+                for ln in test_net_lines(te.outputs(), r[0], r[1], d["test_compute_loss"]):
+                    log_test_net(ln)
+        if world > 1:
+            if got["snapshot"] and rank == 0 and snap_prefix:
+                log("Snapshotting solver state to binary proto file %s" % t.snapshot(snap_prefix))
+                last_snapshot = t.iter()
+            got["snapshot"] = False
+            return got["stop"]
+        return False
+
+    mgpu = "[MultiGPU] " if world > 1 else ""
+    plan = list(schedule(t.iter(), end, display, snap_every, test_every))
+    final_test = bool(plan) and test_every > 0 and plan[-1][4] == "final"
+    interrupted = False
+    for n, it, show, snap, *test in (plan[:-1] if final_test else plan):
+        if test and test[0]:
+            t0 = time.time()
+            interrupted = test_all(it - n, test[0])
+            if interrupted:
+                break
+            if rank == 0:
+                log_test_net(mgpu + ("Initial Test completed" if test[0] == "initial" else "Tests completed in %gs" % (time.time() - t0)))
         ms = max(t.timed_steps(n, copy_input=True), 1e-6)
         assert t.iter() == it
         if got["snapshot"] and rank == 0 and snap_prefix:
@@ -151,6 +244,11 @@ def cmd_train(args):
             last_snapshot = it
     if rank == 0 and snap_prefix and last_snapshot != t.iter() and (snap_after or args.snapshot_prefix):   # solver.cpp:340-345
         log("Snapshotting solver state to binary proto file %s" % t.snapshot(snap_prefix))
+    if interrupted:
+        if rank == 0:
+            log("Optimization stopped early.")
+    elif final_test and not got["stop"]:
+        test_all(t.iter(), "final")               # Solve's extra pass after the last iteration (solver.cpp:419-423)
     if rank == 0:
         log("Optimization Done.")
 
