@@ -15,6 +15,8 @@ UNIQUE_ID_BYTES = 128
 # b2c_wgrad_route, in enum order
 WGRAD_ROUTES = ("caffe", "simt", "gather", "staged_3x3", "staged_3x3_plane", "staged_1x1", "staged_1x1_plane", "tma_1x1",
                 "compact_staged", "compact_tma")
+# b2c_conv_route, in enum order
+CONV_ROUTES = ("caffe", "simt", "gather", "gather_scatter", "staged", "staged_plane")
 
 
 class B2CError(RuntimeError):
@@ -98,6 +100,7 @@ def lib():
         "b2c_conv_workspace_bytes": (sz, [vp, i]),
         "b2c_conv_algo_used": (i, [vp, i]),
         "b2c_debug_wgrad_plan": (i, [vp, C.POINTER(i), i]),
+        "b2c_debug_conv_plan": (i, [vp, i, C.POINTER(i), i]),
         "b2c_conv_forward": (i, [vp, vp, vp, vp, vp, vp, sz, vp]),
         "b2c_conv_backward_data": (i, [vp, vp, vp, vp, vp, sz, vp]),
         "b2c_conv_backward_filter": (i, [vp, vp, vp, vp, vp, sz, vp]),
@@ -199,6 +202,14 @@ class ConvDesc:
         out = (C.c_int * 6)()
         check(lib().b2c_debug_wgrad_plan(self._h, out, 6))
         return dict(route=WGRAD_ROUTES[out[0]], splits=out[1], per=out[2], nkb=out[3], cols=out[4], bpi=out[5])
+
+    def conv_plan(self, op):
+        """b2c_debug_conv_plan: the forward (op 0) or data-gradient (op 1) route for 16-byte aligned activations and its tile
+        plan; `variant` is the gather kernel's KMODE or the staged kernel's box width BWT."""
+        out = (C.c_int * 8)()
+        check(lib().b2c_debug_conv_plan(self._h, op, out, 8))
+        return dict(route=CONV_ROUTES[out[0]], n_tile=out[1], m_tiles=out[2], n_tiles=out[3], tiles=out[4], grid=out[5],
+                    nkb=out[6], variant=out[7])
 
     def _workspace(self, op, like):
         import torch

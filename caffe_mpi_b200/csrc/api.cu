@@ -56,8 +56,12 @@ static bool have_device() {
   return ok == 1;
 }
 
+// the staged kernels run bf16x3 math: only in the fp32 math mode of the implicit engine, and not where the FFMA kernels are asked for
+static bool staged_allowed(const b2c_conv_desc* d) {
+  return d->engine != B2C_ENGINE_CAFFE && d->algo != B2C_ALGO_SIMT && d->math == B2C_MATH_FP32;
+}
 static bool use_staged(const b2c_conv_desc* d, int op) {
-  if (d->engine == B2C_ENGINE_CAFFE || d->algo == B2C_ALGO_SIMT || d->math != B2C_MATH_FP32) return false;
+  if (!staged_allowed(d)) return false;
   return op == B2C_OP_BACKWARD_FILTER ? tc_wgrad_stg_supported(d->s) : tc_stg_supported(d->s, op);
 }
 // math mode handed to the gather kernels (conv_tc.cu / conv_tc_wgrad.cu), which know FP32 (= 3xTF32) and TF32
@@ -78,12 +82,28 @@ static int wgrad_route(const b2c_conv_desc* d, bool x_ok, bool dy_ok, bool ws_ok
   return B2C_WGRAD_ROUTE_SIMT;
 }
 
+// The kernel b2c_conv_forward (op B2C_OP_FORWARD) or b2c_conv_backward_data (B2C_OP_BACKWARD_DATA) runs (b2c_conv_route), decided
+// in one place for the launches, the workspace and filter-cache sizes and b2c_debug_conv_plan.  aligned: the activation operands
+// (x and y, or dy and dx) are 16-byte aligned, which the staged kernel needs; otherwise the gather kernel.
+static int conv_route(const b2c_conv_desc* d, int op, bool aligned) {
+  if (d->engine == B2C_ENGINE_CAFFE) return B2C_CONV_ROUTE_CAFFE;
+  ConvPlanInfo q;
+  if (aligned && staged_allowed(d) && tc_stg_plan_info(d->s, op, &q))
+    return q.variant < 128 ? B2C_CONV_ROUTE_STAGED_PLANE : B2C_CONV_ROUTE_STAGED;
+  if (tc_conv_supported(d->s, op) && d->algo != B2C_ALGO_SIMT)
+    return tc_conv_scatter(d->s, op) ? B2C_CONV_ROUTE_GATHER_SCATTER : B2C_CONV_ROUTE_GATHER;
+  return B2C_CONV_ROUTE_SIMT;
+}
+static bool staged_route(int route) { return route == B2C_CONV_ROUTE_STAGED || route == B2C_CONV_ROUTE_STAGED_PLANE; }
+static bool gather_route(int route) { return route == B2C_CONV_ROUTE_GATHER || route == B2C_CONV_ROUTE_GATHER_SCATTER; }
+
 // ---- prepared-filter cache: [forward layout | dgrad layout], each region 256-byte aligned -------------------------------
+// (the layout of the route for aligned operands: a call with unaligned ones runs its own prepass)
 static size_t cache_region_bytes(const b2c_conv_desc* d, int op) {
-  if (d->engine == B2C_ENGINE_CAFFE || d->algo == B2C_ALGO_SIMT) return 0;
+  const int route = conv_route(d, op, true);
   size_t n = 0;
-  if (use_staged(d, op)) n = tc_stg_workspace(d->s, op);
-  else if (tc_conv_supported(d->s, op)) n = tc_conv_workspace(d->s, op, gather_math(d));
+  if (staged_route(route)) n = tc_stg_workspace(d->s, op);
+  else if (gather_route(route)) n = tc_conv_workspace(d->s, op, gather_math(d));
   return (n + 255) & ~(size_t)255;
 }
 static const void* prepared_filter(const b2c_conv_desc* d, int op) {
@@ -91,6 +111,11 @@ static const void* prepared_filter(const b2c_conv_desc* d, int op) {
   const char* base = static_cast<const char*>(d->filter_cache);
   return op == B2C_OP_FORWARD ? base : base + cache_region_bytes(d, B2C_OP_FORWARD);
 }
+// the prepared filter for a gather-kernel launch: none where the cache holds the staged kernel's layout
+static const void* cached_gather_filter(const b2c_conv_desc* d, int op) {
+  return staged_route(conv_route(d, op, true)) ? nullptr : prepared_filter(d, op);
+}
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // A layer of the implicit engine that no tensor-core kernel takes (K = C/g*kh*kw beyond the filter tile limit, a strided k > 1 data
 // gradient, ...) runs on the FFMA kernels: correct, an order of magnitude slower.  Say so instead of doing it silently -- the
@@ -109,6 +134,7 @@ static void note_simt_fallback(const b2c_conv_desc* d, int op) {
 
 static int resolve_algo(const b2c_conv_desc* d, int op) {
   if (d->engine == B2C_ENGINE_CAFFE) return B2C_ALGO_SIMT;  // reported family of the explicit path's GEMM
+  if (op != B2C_OP_BACKWARD_FILTER) return conv_route(d, op, true) == B2C_CONV_ROUTE_SIMT ? B2C_ALGO_SIMT : B2C_ALGO_TCGEN05;
   if (d->algo == B2C_ALGO_SIMT) return B2C_ALGO_SIMT;
   if (use_staged(d, op)) return B2C_ALGO_TCGEN05;
   return tc_conv_supported(d->s, op) ? B2C_ALGO_TCGEN05 : B2C_ALGO_SIMT;
@@ -188,8 +214,16 @@ extern "C" size_t b2c_conv_workspace_bytes(const b2c_conv_desc* d, int op) {
   const ConvShape& s = d->s;
   if (d->engine == B2C_ENGINE_CAFFE)   // one image's col buffer [Kd*G, Ho, Wo] (base_conv_layer.cpp:225-233)
     return s.is_1x1 ? 0 : sizeof(float) * (size_t)s.Kd * s.G * s.Ho * s.Wo;
-  if (use_staged(d, op)) {   // the gather kernel is the fallback for unaligned activation pointers: size for both
-    const size_t a = op == B2C_OP_BACKWARD_FILTER ? tc_wgrad_stg_workspace(s) : tc_stg_workspace(s, op);
+  if (op != B2C_OP_BACKWARD_FILTER) {
+    const int route = conv_route(d, op, true);
+    if (!staged_route(route)) return gather_route(route) ? tc_conv_workspace(s, op, gather_math(d)) : 0;
+    // the gather kernel is the fallback for unaligned activation pointers: size for both
+    const size_t a = tc_stg_workspace(s, op);
+    const size_t b = gather_route(conv_route(d, op, false)) ? tc_conv_workspace(s, op, gather_math(d)) : 0;
+    return a > b ? a : b;
+  }
+  if (use_staged(d, op)) {   // as above, for the staged weight-gradient kernel
+    const size_t a = tc_wgrad_stg_workspace(s);
     const size_t b = tc_conv_supported(s, op) ? tc_conv_workspace(s, op, gather_math(d)) : 0;
     return a > b ? a : b;
   }
@@ -208,8 +242,8 @@ extern "C" int b2c_conv_forward(const b2c_conv_desc* d, const float* x, const fl
   if (s.has_bias && !bias) return fail(B2C_ERR_INVALID, "b2c_conv_forward: bias_term set but bias is null");
   if (!s.has_bias) bias = nullptr;
   cudaStream_t st = as_stream(stream);
-  if (ws_bytes < b2c_conv_workspace_bytes(d, B2C_OP_FORWARD) || (b2c_conv_workspace_bytes(d, B2C_OP_FORWARD) && !ws))
-    return fail(B2C_ERR_WORKSPACE, "forward workspace too small");
+  const size_t need = b2c_conv_workspace_bytes(d, B2C_OP_FORWARD);
+  if (ws_bytes < need || (need && !ws)) return fail(B2C_ERR_WORKSPACE, "forward workspace too small");
   if (d->engine == B2C_ENGINE_CAFFE) {
     const int P = s.Ho * s.Wo;
     const size_t bdim = (size_t)s.C * s.H * s.W, tdim = (size_t)s.O * P;
@@ -227,11 +261,12 @@ extern "C" int b2c_conv_forward(const b2c_conv_desc* d, const float* x, const fl
     if (bias) return launch_bias_add(s.N, s.O, P, bias, y, st);
     return B2C_OK;
   }
-  if (use_staged(d, B2C_OP_FORWARD) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15u) == 0)
+  const int route = conv_route(d, B2C_OP_FORWARD, aligned16(x) && aligned16(y));
+  if (staged_route(route))
     return launch_conv_tc_stg(s, B2C_OP_FORWARD, x, w, bias, y, ws, ws_bytes, prepared_filter(d, B2C_OP_FORWARD), false, st);
   // a staged layer that falls back here (unaligned activation pointers) has the staged kernel's bf16 layout in its cache: of no use
-  if (tc_conv_supported(s, B2C_OP_FORWARD) && d->algo != B2C_ALGO_SIMT)
-    return launch_conv_tc(s, B2C_OP_FORWARD, gather_math(d), x, w, bias, y, ws, ws_bytes, use_staged(d, B2C_OP_FORWARD) ? nullptr : prepared_filter(d, B2C_OP_FORWARD), st);
+  if (gather_route(route))
+    return launch_conv_tc(s, B2C_OP_FORWARD, gather_math(d), x, w, bias, y, ws, ws_bytes, cached_gather_filter(d, B2C_OP_FORWARD), st);
   note_simt_fallback(d, B2C_OP_FORWARD);
   return launch_conv_fwd_simt(s, x, w, bias, y, st);
 }
@@ -258,10 +293,12 @@ extern "C" int b2c_conv_backward_data(const b2c_conv_desc* d, const float* dy, c
     }
     return B2C_OK;
   }
-  if (use_staged(d, B2C_OP_BACKWARD_DATA) && ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15u) == 0)
+  const int route = conv_route(d, B2C_OP_BACKWARD_DATA, aligned16(dy) && aligned16(dx));
+  if (staged_route(route))
     return launch_conv_tc_stg(s, B2C_OP_BACKWARD_DATA, dy, w, nullptr, dx, ws, ws_bytes, prepared_filter(d, B2C_OP_BACKWARD_DATA), false, st);
-  if (tc_conv_supported(s, B2C_OP_BACKWARD_DATA) && d->algo != B2C_ALGO_SIMT)
-    return launch_conv_tc(s, B2C_OP_BACKWARD_DATA, gather_math(d), dy, w, nullptr, dx, ws, ws_bytes, use_staged(d, B2C_OP_BACKWARD_DATA) ? nullptr : prepared_filter(d, B2C_OP_BACKWARD_DATA), st);
+  if (gather_route(route))
+    return launch_conv_tc(s, B2C_OP_BACKWARD_DATA, gather_math(d), dy, w, nullptr, dx, ws, ws_bytes,
+                          cached_gather_filter(d, B2C_OP_BACKWARD_DATA), st);
   note_simt_fallback(d, B2C_OP_BACKWARD_DATA);
   return launch_conv_dgrad_simt(s, dy, w, dx, st);
 }
@@ -269,13 +306,13 @@ extern "C" int b2c_conv_backward_data(const b2c_conv_desc* d, const float* dy, c
 // dx += dgrad(dy, w): the accumulation Net::Backward performs where a blob fans out (SplitLayer::Backward in the reference),
 // folded into the kernel's TMA reduce-add store.  Only the staged kernel has it; the caller asks first.
 extern "C" int b2c_conv_backward_data_accumulate_supported(const b2c_conv_desc* d) {
-  return d && use_staged(d, B2C_OP_BACKWARD_DATA) ? 1 : 0;
+  return d && staged_route(conv_route(d, B2C_OP_BACKWARD_DATA, true)) ? 1 : 0;
 }
 extern "C" int b2c_conv_backward_data_accumulate(const b2c_conv_desc* d, const float* dy, const float* w, float* dx, void* ws,
                                                  size_t ws_bytes, void* stream) {
   if (!d || !dy || !w || !dx) return fail(B2C_ERR_INVALID, "b2c_conv_backward_data_accumulate: null pointer");
   REQUIRE_DEVICE();
-  if (!use_staged(d, B2C_OP_BACKWARD_DATA) || ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15u))
+  if (!staged_route(conv_route(d, B2C_OP_BACKWARD_DATA, aligned16(dy) && aligned16(dx))))
     return fail(B2C_ERR_INVALID, "b2c_conv_backward_data_accumulate: not available for this layer (see ..._accumulate_supported)");
   const size_t need = b2c_conv_workspace_bytes(d, B2C_OP_BACKWARD_DATA);
   if (!prepared_filter(d, B2C_OP_BACKWARD_DATA) && (ws_bytes < need || (need && !ws))) return fail(B2C_ERR_WORKSPACE, "backward_data workspace too small");
@@ -326,6 +363,18 @@ extern "C" int b2c_debug_wgrad_plan(const b2c_conv_desc* d, int* out, int n) {
   return B2C_OK;
 }
 
+extern "C" int b2c_debug_conv_plan(const b2c_conv_desc* d, int op, int* out, int n) {
+  if (!d || !out || n < 8) return fail(B2C_ERR_INVALID, "b2c_debug_conv_plan: need a descriptor and 8 ints");
+  if (op != B2C_OP_FORWARD && op != B2C_OP_BACKWARD_DATA) return fail(B2C_ERR_INVALID, "b2c_debug_conv_plan: op %d is not forward or backward data", op);
+  const int route = conv_route(d, op, true);
+  ConvPlanInfo q{};
+  if (staged_route(route)) tc_stg_plan_info(d->s, op, &q);
+  else if (gather_route(route)) tc_conv_plan_info(d->s, op, &q);
+  out[0] = route; out[1] = q.n_tile; out[2] = q.m_tiles; out[3] = q.n_tiles; out[4] = q.tiles; out[5] = persistent_grid(q.tiles);
+  out[6] = q.nkb; out[7] = q.variant;
+  return B2C_OK;
+}
+
 namespace b2c {
 int debug_mbar_fwd(unsigned int*, int, int);
 int debug_mbar_stg(unsigned int*, int, int);
@@ -364,7 +413,7 @@ static int collect_prep_entries(const b2c_conv_desc* d, const float* w, void* ca
     const size_t bytes = cache_region_bytes(d, op);
     if (!bytes) continue;
     void* dst = op == B2C_OP_FORWARD ? base : base + cache_region_bytes(d, B2C_OP_FORWARD);
-    if (use_staged(d, op)) tc_stg_prep_entry(d->s, op, w, dst, &out[n++]);
+    if (staged_route(conv_route(d, op, true))) tc_stg_prep_entry(d->s, op, w, dst, &out[n++]);
     else tc_conv_prep_entry(d->s, op, gather_math(d), w, dst, &out[n++]);
   }
   return n;

@@ -60,6 +60,19 @@ struct WgradPlanInfo {
   bool plane;
 };
 
+// A forward / data-gradient kernel's tile plan as b2c_debug_conv_plan reports it: 128 x n_tile output tiles, m_tiles x n_tiles
+// per group, `tiles` in all (run by persistent_grid(tiles) CTAs); nkb K blocks per tile.  variant: KMODE of the gather kernel
+// (conv_tc.cu), BWT of the staged kernel (conv_tc_stg.cu).
+struct ConvPlanInfo {
+  int n_tile, m_tiles, n_tiles, tiles, nkb, variant;
+};
+
+// CTAs of a persistent kernel: one per SM, never more than there are tiles
+inline int persistent_grid(int tiles) {
+  const int sms = sm_count();
+  return tiles < sms ? tiles : sms;
+}
+
 // A B2C_* switch: atol of the variable, `dflt` when it is unset.  Switches are read once per process, into a function-local
 // `static const` (thread-safe initialisation).
 long env_int(const char* name, long dflt);
@@ -81,10 +94,13 @@ size_t tc_conv_workspace(const ConvShape&, int op, int math);
 int launch_conv_tc(const ConvShape&, int op, int math, const float* a, const float* b, const float* bias, float* out,
                    void* ws, size_t ws_bytes, const void* prepared, cudaStream_t);
 void tc_conv_prep_entry(const ConvShape&, int op, int math, const float* w, void* dst, PrepEntry* q);
+void tc_conv_plan_info(const ConvShape&, int op, ConvPlanInfo*);   // the launch's plan; the shape must be tc_conv_supported
+bool tc_conv_scatter(const ConvShape&, int op);   // the data gradient of a strided 1x1 layer: rows scattered into a zeroed dx
 bool tc_stg_prep_entry(const ConvShape&, int op, const float* w, void* dst, PrepEntry* q);
 // bulk-copy-staged bf16x3 kernel (conv_tc_stg.cu): forward / dgrad of stride-1 "same" convolutions
 bool tc_stg_supported(const ConvShape&, int op);
 size_t tc_stg_workspace(const ConvShape&, int op);
+bool tc_stg_plan_info(const ConvShape&, int op, ConvPlanInfo*);     // false: the shape is not staged-eligible
 int launch_conv_tc_stg(const ConvShape&, int op, const float* a, const float* w, const float* bias, float* out, void* ws,
                        size_t ws_bytes, const void* prepared, bool accumulate, cudaStream_t);
 // gather-family weight gradient (conv_tc_wgrad.cu): the gather kernel, the TMA-fed 1x1 kernel, compaction of strided 1x1 layers

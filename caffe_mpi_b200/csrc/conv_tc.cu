@@ -369,7 +369,7 @@ static int launch_fwd_inst(const FwdParams& p, const CUtensorMap& mh, const CUte
   // per-device attribute: set on every launch (a process may drive several GPUs)
   B2C_CUDA_OK(cudaFuncSetAttribute(igemm_fwd_kernel<N_TILE, SPLIT, KMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)S::TOTAL));
-  const int grid = p.total_tiles < sm_count() ? p.total_tiles : sm_count();
+  const int grid = persistent_grid(p.total_tiles);
   igemm_fwd_kernel<N_TILE, SPLIT, KMODE><<<grid, FW_THREADS, S::TOTAL, st>>>(p, mh, ml);
   B2C_POST_LAUNCH();
   return B2C_OK;
@@ -431,26 +431,21 @@ void tc_conv_prep_entry(const ConvShape& s, int op, int math, const float* w, vo
   q->lo = math == B2C_MATH_FP32 ? static_cast<void*>(wbase + q->total) : nullptr;
 }
 
-// `prepared`: the filter already in GEMM layout (b2c_conv_prepare_filter) or null = run the prepass here into `ws`
-int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const float* b, const float* bias, float* out,
-                   void* ws, size_t ws_bytes, const void* prepared, cudaStream_t st) {
-  if (op == B2C_OP_BACKWARD_FILTER) return launch_conv_tc_wgrad(s, math, a, b, out, ws, ws_bytes, st);
-  if (!prepared && (ws_bytes < tc_conv_workspace(s, op, math) || !ws)) return fail(B2C_ERR_WORKSPACE, "tensor-core conv: workspace too small");
-  FwdParams p;
-  PrepEntry q;
-  tc_conv_prep_entry(s, op, math, b, prepared ? const_cast<void*>(prepared) : ws, &q);
+// The kernel's view of `op` on shape `s`: gather geometry, GEMM extents and output strides.  Pointers, bias and the tile plan
+// are left to the caller.
+static FwdParams fwd_params(const ConvShape& s, int op) {
+  FwdParams p{};
   if (op == B2C_OP_FORWARD) {
-    p.x = a; p.Cin_tot = s.C; p.H = s.H; p.W = s.W; p.Cg = s.Cg;
+    p.Cin_tot = s.C; p.H = s.H; p.W = s.W; p.Cg = s.Cg;
     p.kh = s.kh; p.kw = s.kw; p.sh = s.sh; p.sw = s.sw; p.ph = s.ph; p.pw = s.pw; p.dh = s.dh; p.dw = s.dw;
     p.Ho = s.Ho; p.Wo = s.Wo; p.Mtot = s.N * s.Ho * s.Wo;
     p.Ntot = s.Og; p.K = s.Kd;
-    p.out = out; p.Cout_tot = s.O; p.out_plane = (long long)s.Ho * s.Wo; p.out_hs = s.Wo; p.out_ws = 1;
-    p.bias = bias;
+    p.Cout_tot = s.O; p.out_plane = (long long)s.Ho * s.Wo; p.out_hs = s.Wo; p.out_ws = 1;
   } else {
-    // a = dy [N,O,Ho,Wo], b = w, out = dx [N,C,H,W]
-    p.x = a; p.Cin_tot = s.O; p.Cg = s.Og;
+    // x = dy [N,O,Ho,Wo], out = dx [N,C,H,W]
+    p.Cin_tot = s.O; p.Cg = s.Og;
     p.Ntot = s.Cg; p.K = s.Og * s.kh * s.kw;
-    p.out = out; p.Cout_tot = s.C; p.out_plane = (long long)s.H * s.W; p.bias = nullptr;
+    p.Cout_tot = s.C; p.out_plane = (long long)s.H * s.W;
     if (dgrad_as_fwd(s)) {
       // stride-1 conv of dY with the flipped filter, pad' = (k-1)*d - p, rows = bottom pixels
       p.H = s.Ho; p.W = s.Wo;
@@ -459,8 +454,7 @@ int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const f
       p.Ho = s.H; p.Wo = s.W; p.Mtot = s.N * s.H * s.W;
       p.out_hs = s.W; p.out_ws = 1;
     } else {
-      // 1x1, stride > 1, pad 0: rows = top pixels, scatter to bottom[ho*sh][wo*sw]; the rest of dx is 0
-      B2C_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)s.N * s.C * s.H * s.W, st));
+      // 1x1, stride > 1, pad 0: rows = top pixels, scatter to bottom[ho*sh][wo*sw]; the rest of dx is 0 (memset by the launch)
       p.H = s.Ho; p.W = s.Wo;
       p.kh = 1; p.kw = 1; p.sh = 1; p.sw = 1; p.dh = 1; p.dw = 1; p.ph = 0; p.pw = 0;
       p.Ho = s.Ho; p.Wo = s.Wo; p.Mtot = s.N * s.Ho * s.Wo;
@@ -468,17 +462,50 @@ int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const f
     }
   }
   p.Kp = padded_k(p.K);
-  static const int dbg = env_int("B2C_DBG", 0);
-  p.dbg = dbg;
-  const int kmode = (p.Cg % 4 == 0) ? 1 : 0;
-  if (!prepared)
-    if (int rc = launch_filter_prep(&q, 1, st)) return rc;
+  p.G = s.G;
+  return p;
+}
 
+// The tile plan of the launch for these GEMM extents: N_TILE (pick_n_tile, or the B2C_NTILE override where it is wider than half
+// the columns), tile counts, K blocks and KMODE.
+static void plan_tiles(const FwdParams& p, ConvPlanInfo* q) {
   int n_tile = pick_n_tile(p.Ntot);
   static const int force = env_int("B2C_NTILE", 0);
   if ((force == 32 || force == 64 || force == 128) && force / 2 < p.Ntot) n_tile = force;
-  p.m_tiles = (p.Mtot + 127) / 128; p.n_tiles = (p.Ntot + n_tile - 1) / n_tile; p.G = s.G;
-  p.total_tiles = p.m_tiles * p.n_tiles * p.G;
+  q->n_tile = n_tile;
+  q->m_tiles = (p.Mtot + 127) / 128; q->n_tiles = (p.Ntot + n_tile - 1) / n_tile;
+  q->tiles = q->m_tiles * q->n_tiles * p.G;
+  q->nkb = p.Kp / BK;
+  q->variant = (p.Cg % 4 == 0) ? 1 : 0;
+}
+
+void tc_conv_plan_info(const ConvShape& s, int op, ConvPlanInfo* q) {
+  *q = ConvPlanInfo{};
+  plan_tiles(fwd_params(s, op), q);
+}
+bool tc_conv_scatter(const ConvShape& s, int op) { return op == B2C_OP_BACKWARD_DATA && !dgrad_as_fwd(s); }
+
+// `prepared`: the filter already in GEMM layout (b2c_conv_prepare_filter) or null = run the prepass here into `ws`
+int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const float* b, const float* bias, float* out,
+                   void* ws, size_t ws_bytes, const void* prepared, cudaStream_t st) {
+  if (op == B2C_OP_BACKWARD_FILTER) return launch_conv_tc_wgrad(s, math, a, b, out, ws, ws_bytes, st);
+  if (!prepared && (ws_bytes < tc_conv_workspace(s, op, math) || !ws)) return fail(B2C_ERR_WORKSPACE, "tensor-core conv: workspace too small");
+  PrepEntry q;
+  tc_conv_prep_entry(s, op, math, b, prepared ? const_cast<void*>(prepared) : ws, &q);
+  FwdParams p = fwd_params(s, op);
+  p.x = a; p.out = out;
+  p.bias = op == B2C_OP_FORWARD ? bias : nullptr;
+  if (tc_conv_scatter(s, op))
+    B2C_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)s.N * s.C * s.H * s.W, st));
+  static const int dbg = env_int("B2C_DBG", 0);
+  p.dbg = dbg;
+  if (!prepared)
+    if (int rc = launch_filter_prep(&q, 1, st)) return rc;
+
+  ConvPlanInfo plan;
+  plan_tiles(p, &plan);
+  const int n_tile = plan.n_tile, kmode = plan.variant;
+  p.m_tiles = plan.m_tiles; p.n_tiles = plan.n_tiles; p.total_tiles = plan.tiles;
   alignas(64) CUtensorMap mh, ml;
   const cuuint64_t dims[3] = {(cuuint64_t)p.Kp, (cuuint64_t)q.rows, (cuuint64_t)s.G};
   const cuuint64_t strides[2] = {(cuuint64_t)p.Kp * 4, (cuuint64_t)p.Kp * 4 * (cuuint64_t)q.rows};

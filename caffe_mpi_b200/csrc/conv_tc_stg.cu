@@ -518,6 +518,22 @@ static bool stg_geom(const ConvShape& s, int op, StgGeom* g) {
   return true;
 }
 bool tc_stg_supported(const ConvShape& s, int op) { return stg_geom(s, op, nullptr); }
+
+// The launch's tile plan: 128 consecutive flattened pixels x N_TILE output channels per tile, BWT as the variant
+static void stg_plan(const ConvShape& s, const StgGeom& g, ConvPlanInfo* q) {
+  *q = ConvPlanInfo{};
+  q->n_tile = g.Cout > 64 ? 128 : g.Cout > 32 ? 64 : 32;
+  q->m_tiles = (s.N * s.H * s.W + 127) / 128; q->n_tiles = (g.Cout + q->n_tile - 1) / q->n_tile;
+  q->tiles = q->m_tiles * q->n_tiles;
+  q->nkb = g.nkb;
+  q->variant = g.bwt;
+}
+bool tc_stg_plan_info(const ConvShape& s, int op, ConvPlanInfo* q) {
+  StgGeom g;
+  if (!stg_geom(s, op, &g)) return false;
+  stg_plan(s, g, q);
+  return true;
+}
 size_t tc_stg_workspace(const ConvShape& s, int op) {
   StgGeom g;
   if (!stg_geom(s, op, &g)) return 0;
@@ -529,7 +545,7 @@ static int stg_launch_inst(const stg::Params& p, const CUtensorMap& mh, const CU
                            cudaStream_t st) {
   using S = stg::Smem<N_TILE, BWT>;
   B2C_CUDA_OK(cudaFuncSetAttribute(stg::igemm_stg_kernel<N_TILE, BWT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
-  const int grid = p.total_tiles < sm_count() ? p.total_tiles : sm_count();
+  const int grid = persistent_grid(p.total_tiles);
   stg::igemm_stg_kernel<N_TILE, BWT><<<grid, stg::THREADS, S::TOTAL, st>>>(p, mh, ml, mx, my);
   B2C_POST_LAUNCH();
   return B2C_OK;
@@ -582,8 +598,10 @@ int launch_conv_tc_stg(const ConvShape& s, int op, const float* a, const float* 
   p.accumulate = accumulate ? 1 : 0;
   static const int dbg = env_int("B2C_STG_DBG", 0);
   p.dbg = dbg;
-  const int n_tile = g.Cout > 64 ? 128 : g.Cout > 32 ? 64 : 32;
-  p.m_tiles = (p.Mtot + 127) / 128; p.n_tiles = (g.Cout + n_tile - 1) / n_tile; p.total_tiles = p.m_tiles * p.n_tiles;
+  ConvPlanInfo plan;
+  stg_plan(s, g, &plan);
+  const int n_tile = plan.n_tile;
+  p.m_tiles = plan.m_tiles; p.n_tiles = plan.n_tiles; p.total_tiles = plan.tiles;
   p.prof = prof_buffer(st);
   alignas(64) CUtensorMap mh, ml, mx, my;
   {

@@ -349,6 +349,25 @@ typedef enum {
  * Needs n >= 6.  Pure host computation: splits follow the current device's SM count (132 without a device). */
 int b2c_debug_wgrad_plan(const b2c_conv_desc* d, int* out, int n);
 
+/* The kernel b2c_conv_forward or b2c_conv_backward_data runs for a descriptor (b2c_debug_conv_plan out[0]). */
+typedef enum {
+  B2C_CONV_ROUTE_CAFFE = 0,           /* engine CAFFE: per-image im2col / col2im + b2c_sgemm                               */
+  B2C_CONV_ROUTE_SIMT = 1,            /* FFMA direct kernels                                                               */
+  B2C_CONV_ROUTE_GATHER = 2,          /* implicit-GEMM gather kernel: the forward, or the data gradient as a stride-1       */
+                                      /* forward of dy with the flipped filter                                             */
+  B2C_CONV_ROUTE_GATHER_SCATTER = 3,  /* the gather kernel on the data gradient of a strided 1x1 layer: rows scattered     */
+                                      /* onto the stride grid of dx, the rest of dx zeroed                                  */
+  B2C_CONV_ROUTE_STAGED = 4,          /* TMA-staged bf16x3 kernel (stride-1 "same" convolutions)                            */
+  B2C_CONV_ROUTE_STAGED_PLANE = 5     /* the same in plane mode (7x7 maps: whole image planes staged)                       */
+} b2c_conv_route;
+/* Which route op B2C_OP_FORWARD or B2C_OP_BACKWARD_DATA takes for this descriptor with 16-byte-aligned activations (x and y,
+ * or dy and dx), and its tile plan: out[0] route (b2c_conv_route), [1] N_TILE, [2] 128-row M tiles, [3] N tiles per group,
+ * [4] tiles in all (x groups), [5] grid = min(tiles, SMs), [6] K blocks per tile, [7] variant: KMODE of the gather kernel
+ * (1: K in chunks of 4 channels, 0: per-element K order), BWT of the staged kernel (staged pixels per channel: 49 in plane
+ * mode, else 128, 160, 192 or 256).  The CAFFE and SIMT routes report zeros.  Needs n >= 8.  Pure host computation: the
+ * grid follows the current device's SM count (132 without a device), N_TILE the B2C_NTILE switch as the launch does. */
+int b2c_debug_conv_plan(const b2c_conv_desc* d, int op, int* out, int n);
+
 #define B2C_UNIQUE_ID_BYTES 128
 int b2c_comm_get_unique_id(void* id_out /* B2C_UNIQUE_ID_BYTES */);
 int b2c_comm_init(int nranks, int rank, const void* id, b2c_comm** out);

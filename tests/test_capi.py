@@ -68,6 +68,102 @@ def test_wgrad_plan_routes():
     assert m.lib().b2c_debug_wgrad_plan(d._h, (C.c_int * 5)(), 5) == -1
 
 
+def test_conv_plan_routes():
+    """b2c_debug_conv_plan is host-only: the route and tile plan of b2c_conv_forward (op 0) and b2c_conv_backward_data (op 1).
+    The plans are asked for in a subprocess with the device hidden, so grids follow sm_count()'s no-device value of 132."""
+    script = r"""
+import json, sys
+sys.path.insert(0, sys.argv[1])
+import caffe_mpi_b200 as m
+from caffe_mpi_b200 import capi
+def plan(N, Cin, H, W, O, k, s=1, p=None, d=1, G=1, engine=capi.ENGINE_DEFAULT, math=None, algo=None):
+    kk = k if isinstance(k, int) else k
+    p = (kk // 2 if isinstance(kk, int) else (kk[0] // 2, kk[1] // 2)) if p is None else p
+    dd = m.ConvDesc(m.ConvParams.make(N, Cin, H, W, O, k, s, p, d, G, False), engine, math, algo)
+    return [dd.conv_plan(0), dd.conv_plan(1)]
+S = [
+    plan(3, 32, 8, 16, 128, 1), plan(3, 32, 12, 15, 32, 3), plan(3, 32, 12, 16, 96, 3), plan(3, 32, 4, 63, 32, 3),
+    plan(3, 32, 4, 64, 32, 3), plan(2, 32, 8, 16, 32, 5), plan(2, 32, 8, 16, 32, 7), plan(3, 48, 8, 16, 64, 3),
+    plan(3, 32, 8, 16, 31, 3), plan(3, 32, 8, 16, 32, 3), plan(9, 32, 7, 7, 72, 3), plan(3, 32, 11, 13, 32, 3),
+    plan(2, 3, 23, 23, 32, 7, s=2, p=3), plan(1, 512, 5, 5, 32, 3, s=2, p=1), plan(1, 516, 5, 5, 32, 3, s=2, p=1),
+    plan(1, 127, 5, 5, 32, 3, s=2, p=1), plan(1, 129, 5, 5, 32, 3, s=2, p=1), plan(1, 8, 4, 4, 1024, 3, G=2),
+    plan(1, 8, 4, 4, 1032, 3, G=2), plan(2, 32, 13, 13, 64, 1, s=2, p=0), plan(16, 64, 56, 56, 256, 3, s=2, p=1),
+    plan(2, 32, 8, 16, 32, 3, math=capi.MATH_TF32), plan(2, 32, 8, 16, 32, 3, math=capi.MATH_FP32_3XTF32),
+    plan(2, 32, 8, 16, 32, 3, algo=capi.ALGO_SIMT), plan(2, 32, 8, 16, 32, 3, engine=capi.ENGINE_CAFFE),
+]
+d = m.ConvDesc(m.ConvParams.make(1, 3, 8, 8, 4, 3))
+L = m.lib()
+import ctypes as C
+refused = [L.b2c_debug_conv_plan(d._h, 0, (C.c_int * 7)(), 7), L.b2c_debug_conv_plan(d._h, 2, (C.c_int * 8)(), 8)]
+print(json.dumps([S, refused]))
+"""
+    import json
+    import os
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    for k in ("B2C_NTILE", "B2C_CONV_STAGED", "B2C_CONV_STAGED_PLANE"):
+        env.pop(k, None)
+    out = subprocess.run([sys.executable, "-c", script, root], env=env, capture_output=True, text=True, check=True).stdout
+    S, refused = json.loads(out.strip().splitlines()[-1])
+    assert refused == [-1, -1]                                        # n < 8, and the weight gradient (b2c_debug_wgrad_plan's)
+
+    def R(q, route, **want):
+        return q["route"] == route and all(q[k] == v for k, v in want.items())
+    (f, b), it = S[0], iter(S[1:])
+    # one shape per route
+    assert R(f, "staged", n_tile=128, m_tiles=3, n_tiles=1, tiles=3, grid=3, nkb=1, variant=128)      # 1x1 on 8x16: BWT 128
+    assert R(b, "staged", n_tile=32, variant=128, nkb=2)
+    f, b = next(it)
+    assert R(f, "staged", variant=160) and R(b, "staged", variant=160)                                    # need == 160
+    f, b = next(it)
+    assert R(f, "staged", variant=192, n_tile=128) and R(b, "staged", variant=192, n_tile=32)             # need 165
+    f, b = next(it)
+    assert R(f, "staged", variant=256, m_tiles=6) and R(b, "staged", variant=256)                         # need == 256
+    f, b = next(it)
+    assert R(f, "gather", variant=1) and R(b, "gather", variant=1)                                        # need 261
+    f, b = next(it)
+    assert R(f, "staged", variant=256, nkb=13) and R(b, "staged")                                         # 25 taps
+    f, b = next(it)
+    assert R(f, "gather", variant=1, nkb=49) and R(b, "gather", variant=1)                                # 49 taps
+    f, b = next(it)
+    assert R(f, "gather", n_tile=64, variant=1) and R(b, "staged", n_tile=64, variant=192)                # C = 48
+    f, b = next(it)
+    assert R(f, "gather", n_tile=32) and R(b, "gather", variant=0)                                        # Cout 31 / 32
+    f, b = next(it)
+    assert R(f, "staged", n_tile=32) and R(b, "staged", n_tile=32)
+    f, b = next(it)
+    assert R(f, "staged_plane", variant=49, n_tile=128, m_tiles=4) and R(b, "gather", variant=1)          # 7x7: plane mode
+    f, b = next(it)
+    assert R(f, "gather") and R(b, "gather")                                                              # H*W % 4 != 0
+    f, b = next(it)
+    assert R(f, "gather", n_tile=32, variant=0, nkb=5, m_tiles=3) and R(b, "simt", n_tile=0, tiles=0, grid=0, variant=0)
+    f, b = next(it)
+    assert R(f, "gather", variant=1, nkb=144)                                                             # table: 1152 chunks
+    f, b = next(it)
+    assert R(f, "simt")
+    f, b = next(it)
+    assert R(f, "gather", variant=0, nkb=36)                                                              # table: 1152 elements
+    f, b = next(it)
+    assert R(f, "simt")
+    f, b = next(it)
+    assert R(f, "gather") and R(b, "gather", variant=1, nkb=144, tiles=2)                                 # dgrad table, G = 2
+    f, b = next(it)
+    assert R(f, "gather") and R(b, "simt")
+    f, b = next(it)
+    assert R(f, "gather") and R(b, "gather_scatter", n_tile=32, variant=1)
+    f, b = next(it)
+    assert R(f, "gather", n_tile=128, m_tiles=98, n_tiles=2, tiles=196, grid=132, nkb=18, variant=1)      # more than one wave
+    for _ in range(2):                                                                                    # TF32, 3xTF32
+        f, b = next(it)
+        assert R(f, "gather") and R(b, "gather")
+    f, b = next(it)
+    assert R(f, "simt") and R(b, "simt")
+    f, b = next(it)
+    assert f == b == dict(route="caffe", n_tile=0, m_tiles=0, n_tiles=0, tiles=0, grid=0, nkb=0, variant=0)
+
+
 def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():
