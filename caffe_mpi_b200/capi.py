@@ -17,6 +17,8 @@ WGRAD_ROUTES = ("caffe", "simt", "gather", "staged_3x3", "staged_3x3_plane", "st
                 "compact_staged", "compact_tma")
 # b2c_conv_route, in enum order
 CONV_ROUTES = ("caffe", "simt", "gather", "gather_scatter", "staged", "staged_plane")
+# b2c_pool_route, in enum order
+POOL_ROUTES = ("max_scalar", "max_window", "max_bwd_row", "max_bwd_quad", "ave")
 
 
 class B2CError(RuntimeError):
@@ -132,6 +134,7 @@ def lib():
         "b2c_relu_backward2": (i, [sz, vp, vp, vp, vp, vp]),
         "b2c_pool_forward": (i, [i] * 10 + [vp, vp, vp, vp]),
         "b2c_pool_backward": (i, [i] * 10 + [vp, vp, vp, vp]),
+        "b2c_debug_pool_plan": (i, [i] * 11 + [vp, vp, C.POINTER(i), i]),
         "b2c_add": (i, [sz, vp, vp, vp, vp]),
         "b2c_softmax_loss_forward": (i, [i, i, vp, vp, vp, vp, vp]),
         "b2c_softmax_loss_backward": (i, [i, i, vp, vp, f, vp, vp]),
@@ -304,6 +307,16 @@ def col2im_nd(col, im, k, s, p, d, stream=None):
     check(lib().b2c_col2im_nd(_p(col), nax, _iarr(im.shape), _iarr(col.shape), _iarr(k), _iarr(p), _iarr(s), _iarr(d),
                               _p(im), _stream(stream)))
     return im
+
+
+def pool_plan(method, dir, NC, H, W, k, s, p, out_ptr=0, mask_ptr=0):
+    """b2c_debug_pool_plan: the kernel b2c_pool_forward (dir 0) or b2c_pool_backward (dir 1) takes for these arguments, with y / dx
+    at address out_ptr and the MAX mask at mask_ptr (integers; never dereferenced).  k, s, p: (h, w) pairs.  Raises B2CError
+    where the entry points refuse the arguments."""
+    out = (C.c_int * 5)()
+    check(lib().b2c_debug_pool_plan(method, dir, NC, H, W, k[0], k[1], s[0], s[1], p[0], p[1], C.c_void_p(out_ptr),
+                                    C.c_void_p(mask_ptr), out, 5))
+    return dict(route=POOL_ROUTES[out[0]], Ho=out[1], Wo=out[2], q=out[3], rpb=out[4])
 
 
 def sgemm(transA, transB, M, N, K, alpha, A, B, beta, Cm, stream=None):

@@ -112,14 +112,14 @@ bias_add_kernel(size_t total, int O, int P, const float* __restrict__ bias, floa
     y[idx] += __ldg(bias + (int)((idx / P) % O));
 }
 
-// db[o] += sum_{n,p} dy[n][o][p]: one block per channel, float4 loads where aligned, warp-shuffle
-// tree then a cross-warp smem stage.
+// db[o] += sum_{n,p} dy[n][o][p]: one block per channel, float4 loads where aligned (P % 4 == 0 and dy on a 16-byte boundary:
+// then every row is), warp-shuffle tree then a cross-warp smem stage.
 __global__ void __launch_bounds__(256)
 bias_grad_kernel(int N, int O, int P, const float* __restrict__ dy, float* __restrict__ db) {
   __shared__ float red[8];
   const int o = blockIdx.x;
   float acc = 0.0f;
-  const bool vec = (P % 4) == 0;
+  const bool vec = (P % 4) == 0 && (reinterpret_cast<uintptr_t>(dy) & 15) == 0;
   for (int n = 0; n < N; ++n) {
     const float* row = dy + ((size_t)n * O + o) * P;
     if (vec) {

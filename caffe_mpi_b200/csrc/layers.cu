@@ -21,8 +21,8 @@ namespace cg = cooperative_groups;
 namespace b2c {
 
 // ---- ReLU ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) relu_fwd_kernel(size_t n, const float* __restrict__ x, float* __restrict__ y, float slope) {
-  const size_t n4 = n / 4, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+__global__ void __launch_bounds__(256) relu_fwd_kernel(size_t n, int vec, const float* __restrict__ x, float* __restrict__ y, float slope) {
+  const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const float4* x4 = reinterpret_cast<const float4*>(x);
   float4* y4 = reinterpret_cast<float4*>(y);
   for (size_t i = tid; i < n4; i += step) {
@@ -32,9 +32,9 @@ __global__ void __launch_bounds__(256) relu_fwd_kernel(size_t n, const float* __
   }
   for (size_t i = n4 * 4 + tid; i < n; i += step) { const float v = x[i]; y[i] = v > 0 ? v : v * slope; }
 }
-__global__ void __launch_bounds__(256) relu_bwd_kernel(size_t n, const float* __restrict__ dy, const float* __restrict__ x,
+__global__ void __launch_bounds__(256) relu_bwd_kernel(size_t n, int vec, const float* __restrict__ dy, const float* __restrict__ x,
                                                        float* __restrict__ dx, float slope) {
-  const size_t n4 = n / 4, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const float4* d4 = reinterpret_cast<const float4*>(dy);
   const float4* x4 = reinterpret_cast<const float4*>(x);
   float4* o4 = reinterpret_cast<float4*>(dx);
@@ -425,8 +425,8 @@ pool_ave_bwd_kernel(size_t total, int H, int W, int Ho, int Wo, int kh, int kw, 
 }
 
 // ---- elementwise ----------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) add_kernel(size_t n, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y) {
-  const size_t n4 = n / 4, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+__global__ void __launch_bounds__(256) add_kernel(size_t n, int vec, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y) {
+  const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   for (size_t i = tid; i < n4; i += step) {
     const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
     reinterpret_cast<float4*>(y)[i] = make_float4(u.x + v.x, u.y + v.y, u.z + v.z, u.w + v.w);
@@ -486,14 +486,16 @@ using namespace b2c;
 extern "C" int b2c_relu_forward(size_t n, const float* x, float* y, float negative_slope, void* stream) {
   NEED(x && y, "b2c_relu_forward: null");
   if (!n) return B2C_OK;
-  relu_fwd_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, as_stream(stream)>>>(n, x, y, negative_slope);
+  const bool al = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;     // else one float at a time
+  relu_fwd_kernel<<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, x, y, negative_slope);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 extern "C" int b2c_relu_backward(size_t n, const float* dy, const float* x, float* dx, float negative_slope, void* stream) {
   NEED(dy && x && dx, "b2c_relu_backward: null");
   if (!n) return B2C_OK;
-  relu_bwd_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, as_stream(stream)>>>(n, dy, x, dx, negative_slope);
+  const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
+  relu_bwd_kernel<<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, dy, x, dx, negative_slope);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -578,70 +580,96 @@ extern "C" int b2c_mul(size_t n, const float* a, const float* b, float* y, void*
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
+// PoolingLayer::Reshape's ceil-mode extent (pooling_layer.cpp:92-107), for arguments pool_route has checked
 static int pool_out(int in, int k, int s, int p) {
   int o = (int)ceilf((float)(in + 2 * p - k) / s) + 1;
   if (p > 0 && (o - 1) * s >= in + p) --o;
   return o;
 }
+struct PoolRoute { int route, Ho, Wo, q, rpb; };
+// The one place that picks the pooling kernel; b2c_pool_forward / b2c_pool_backward launch what it returns and b2c_debug_pool_plan
+// reports it.  dir 0 = forward (out = y, mask = the MAX mask), 1 = backward (out = dx).  Pointers are compared, never dereferenced.
+// The argument checks are PoolingLayer::LayerSetUp's and Reshape's (pooling_layer.cpp:51-52,75-76), plus non-empty maps.
+static int pool_route(int method, int dir, int NC, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw, const void* out,
+                      const void* mask, PoolRoute* r) {
+  NEED(method == 0 || method == 1, "pooling: STOCHASTIC pooling is outside this path");
+  NEED(dir == 0 || dir == 1, "pooling: dir must be 0 (forward) or 1 (backward)");
+  NEED(NC > 0 && H > 0 && W > 0, "pooling: empty input");
+  NEED(kh > 0 && kw > 0, "pooling: Filter dimensions cannot be zero.");
+  NEED(sh > 0 && sw > 0, "pooling: stride must be positive");
+  NEED(ph >= 0 && pw >= 0 && ph < kh && pw < kw, "pooling: pad must lie in [0, kernel)");
+  *r = PoolRoute{B2C_POOL_ROUTE_AVE, pool_out(H, kh, sh, ph), pool_out(W, kw, sw, pw), 0, 0};
+  NEED(r->Ho >= 1 && r->Wo >= 1, "pooling: the kernel is larger than the padded input");
+  if (method == 1) return B2C_OK;
+  const bool common = kh == kw && sh == sw && ((kh == 3 && sh == 2) || (kh == 2 && sh == 2) || (kh == 3 && sh == 1));
+  if (dir == 0) {
+    const int q = r->Wo % 4 == 0 ? 4 : r->Wo % 2 == 0 ? 2 : 0;
+    const uintptr_t al = reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(mask);
+    if (common && q && (al & (q == 4 ? 15 : 7)) == 0) { r->route = B2C_POOL_ROUTE_MAX_WINDOW; r->q = q; }
+    else r->route = B2C_POOL_ROUTE_MAX_SCALAR;
+    return B2C_OK;
+  }
+  NEED((long long)NC * H < 0x7fffffffLL, "b2c_pool_backward: too many rows");
+  if (common && W % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) r->route = B2C_POOL_ROUTE_MAX_BWD_QUAD;
+  else { r->route = B2C_POOL_ROUTE_MAX_BWD_ROW; r->rpb = W >= 128 ? 1 : 128 / W; }
+  return B2C_OK;
+}
+extern "C" int b2c_debug_pool_plan(int method, int dir, int NC, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
+                                   const void* out_ptr, const void* mask_ptr, int* out, int n) {
+  NEED(out && n >= 5, "b2c_debug_pool_plan: needs out[5]");
+  PoolRoute r;
+  if (int rc = pool_route(method, dir, NC, H, W, kh, kw, sh, sw, ph, pw, out_ptr, mask_ptr, &r)) return rc;
+  out[0] = r.route; out[1] = r.Ho; out[2] = r.Wo; out[3] = r.q; out[4] = r.rpb;
+  return B2C_OK;
+}
 extern "C" int b2c_pool_forward(int method, int NC, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw, const float* x,
                                 float* y, int* mask, void* stream) {
-  NEED(x && y && NC > 0 && kh > 0 && kw > 0 && sh > 0 && sw > 0, "b2c_pool_forward: bad argument");
-  const int Ho = pool_out(H, kh, sh, ph), Wo = pool_out(W, kw, sw, pw);
+  NEED(x && y, "b2c_pool_forward: null");
+  NEED(mask || method != 0, "b2c_pool_forward: MAX needs a mask buffer");
+  PoolRoute r;
+  if (int rc = pool_route(method, 0, NC, H, W, kh, kw, sh, sw, ph, pw, y, mask, &r)) return rc;
+  const int Ho = r.Ho, Wo = r.Wo;
   const size_t total = (size_t)NC * Ho * Wo;
-  if (method == 0) {
-    NEED(mask, "b2c_pool_forward: MAX needs a mask buffer");
-    const bool common = kh == kw && sh == sw && ((kh == 3 && sh == 2) || (kh == 2 && sh == 2) || (kh == 3 && sh == 1));
-    const int q = Wo % 4 == 0 ? 4 : Wo % 2 == 0 ? 2 : 0;
-    const uintptr_t al = reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(mask);
-    if (common && q && (al & (q == 4 ? 15 : 7)) == 0) {
-      const long long groups = (long long)NC * Ho * (Wo / q);
-      const unsigned grid = grid_for((size_t)groups, 256);
-      cudaStream_t s_ = as_stream(stream);
+  cudaStream_t s_ = as_stream(stream);
+  if (r.route == B2C_POOL_ROUTE_MAX_WINDOW) {
+    const int q = r.q;
+    const long long groups = (long long)NC * Ho * (Wo / q);
+    const unsigned grid = grid_for((size_t)groups, 256);
 #define B2C_POOLF(KH, S, Q) pool_max_fwd_q_kernel<KH, KH, S, S, Q><<<grid, 256, 0, s_>>>(groups, H, W, Ho, Wo, ph, pw, x, y, mask)
-      if (kh == 3 && sh == 2) { if (q == 4) B2C_POOLF(3, 2, 4); else B2C_POOLF(3, 2, 2); }
-      else if (kh == 2) { if (q == 4) B2C_POOLF(2, 2, 4); else B2C_POOLF(2, 2, 2); }
-      else { if (q == 4) B2C_POOLF(3, 1, 4); else B2C_POOLF(3, 1, 2); }
+    if (kh == 3 && sh == 2) { if (q == 4) B2C_POOLF(3, 2, 4); else B2C_POOLF(3, 2, 2); }
+    else if (kh == 2) { if (q == 4) B2C_POOLF(2, 2, 4); else B2C_POOLF(2, 2, 2); }
+    else { if (q == 4) B2C_POOLF(3, 1, 4); else B2C_POOLF(3, 1, 2); }
 #undef B2C_POOLF
-    } else {
-      pool_max_fwd_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y, mask);
-    }
-  } else if (method == 1) {
-    pool_ave_fwd_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y);
+  } else if (r.route == B2C_POOL_ROUTE_MAX_SCALAR) {
+    pool_max_fwd_kernel<<<grid_for(total, 256), 256, 0, s_>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y, mask);
   } else {
-    return fail(B2C_ERR_INVALID, "b2c_pool_forward: STOCHASTIC pooling is outside this path");
+    pool_ave_fwd_kernel<<<grid_for(total, 256), 256, 0, s_>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y);
   }
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 extern "C" int b2c_pool_backward(int method, int NC, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw, const float* dy,
                                  const int* mask, float* dx, void* stream) {
-  NEED(dy && dx && NC > 0, "b2c_pool_backward: bad argument");
-  const int Ho = pool_out(H, kh, sh, ph), Wo = pool_out(W, kw, sw, pw);
-  const size_t total = (size_t)NC * H * W;
-  if (method == 0) {
-    NEED(mask, "b2c_pool_backward: MAX needs the forward mask");
-    {
-      const long long rows = (long long)NC * H;
-      NEED(rows < 0x7fffffffLL, "b2c_pool_backward: too many rows");
-      if (W % 4 == 0 && (reinterpret_cast<uintptr_t>(dx) & 15) == 0 && kh == kw && sh == sw &&
-          ((kh == 3 && sh == 2) || (kh == 2 && sh == 2) || (kh == 3 && sh == 1))) {
-        const long long quads = rows * (W / 4);
-        const unsigned grid = grid_for((size_t)quads, 256);
-        cudaStream_t s_ = as_stream(stream);
-        if (kh == 3 && sh == 2) pool_max_bwd_q4_kernel<3, 3, 2, 2><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
-        else if (kh == 2) pool_max_bwd_q4_kernel<2, 2, 2, 2><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
-        else pool_max_bwd_q4_kernel<3, 3, 1, 1><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
-        B2C_POST_LAUNCH();
-        return B2C_OK;
-      }
-      const long long groups = (rows + (W >= 128 ? 1 : 128 / W) - 1) / (W >= 128 ? 1 : 128 / W);
-      const int grid = (int)(groups < (long long)sm_count() * 64 ? groups : (long long)sm_count() * 64);
-      pool_max_bwd_kernel<<<grid, 128, 0, as_stream(stream)>>>((int)rows, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, mask, dx);
-    }
-  } else if (method == 1) {
-    pool_ave_bwd_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, dx);
+  NEED(dy && dx, "b2c_pool_backward: null");
+  NEED(mask || method != 0, "b2c_pool_backward: MAX needs the forward mask");
+  PoolRoute r;
+  if (int rc = pool_route(method, 1, NC, H, W, kh, kw, sh, sw, ph, pw, dx, mask, &r)) return rc;
+  const int Ho = r.Ho, Wo = r.Wo;
+  cudaStream_t s_ = as_stream(stream);
+  if (r.route == B2C_POOL_ROUTE_MAX_BWD_QUAD) {
+    const long long quads = (long long)NC * H * (W / 4);
+    const unsigned grid = grid_for((size_t)quads, 256);
+    if (kh == 3 && sh == 2) pool_max_bwd_q4_kernel<3, 3, 2, 2><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
+    else if (kh == 2) pool_max_bwd_q4_kernel<2, 2, 2, 2><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
+    else pool_max_bwd_q4_kernel<3, 3, 1, 1><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
+  } else if (r.route == B2C_POOL_ROUTE_MAX_BWD_ROW) {
+    const long long rows = (long long)NC * H;
+    const long long groups = (rows + r.rpb - 1) / r.rpb;
+    const int grid = (int)(groups < (long long)sm_count() * 64 ? groups : (long long)sm_count() * 64);
+    pool_max_bwd_kernel<<<grid, 128, 0, s_>>>((int)rows, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, mask, dx);
   } else {
-    return fail(B2C_ERR_INVALID, "b2c_pool_backward: STOCHASTIC pooling is outside this path");
+    const size_t total = (size_t)NC * H * W;
+    pool_ave_bwd_kernel<<<grid_for(total, 256), 256, 0, s_>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, dx);
   }
   B2C_POST_LAUNCH();
   return B2C_OK;
@@ -675,7 +703,8 @@ extern "C" int b2c_transpose(int rows, int cols, const float* src, float* dst, v
 extern "C" int b2c_add(size_t n, const float* a, const float* b, float* y, void* stream) {
   NEED(a && b && y, "b2c_add: null");
   if (!n) return B2C_OK;
-  add_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, as_stream(stream)>>>(n, a, b, y);
+  const bool al = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
+  add_kernel<<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, a, b, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

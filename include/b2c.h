@@ -182,7 +182,8 @@ int b2c_sgemv(int transA, int M, int N, float alpha, const float* A, const float
 
 /* ---- the non-convolution layers on ResNet-50's training path (SURVEY.md 8(f) rank 2) ----------------------------
  * fp32 NCHW, asynchronous on `stream`.  Each keeps the semantics of the reference layer's CPU code.                */
-/* ReLULayer::Forward/Backward (src/caffe/layers/relu_layer.cpp:10-41); may run in place (y == x).                  */
+/* ReLULayer::Forward/Backward (src/caffe/layers/relu_layer.cpp:10-41); may run in place (y == x).  Any 4-byte-aligned
+ * pointers: float4 passes when all of them are 16-byte aligned, one float at a time otherwise (same values either way).     */
 int b2c_relu_forward(size_t n, const float* x, float* y, float negative_slope, void* stream);
 int b2c_relu_backward(size_t n, const float* dy, const float* x, float* dx, float negative_slope, void* stream);
 /* BatchNormLayer (NVCaffe, src/caffe/layers/batch_norm_layer.cpp:140-300), TRAIN phase.  x,y,xnorm: [N,C,S].
@@ -194,7 +195,9 @@ int b2c_bn_forward_train(int N, int C, int S, const float* x, const float* gamma
 int b2c_bn_backward(int N, int C, int S, const float* dy, const float* xnorm, const float* gamma, const float* save_invstd,
                     float* dgamma, float* dbeta, float* dx, void* stream);
 /* PoolingLayer (src/caffe/layers/pooling_layer.cpp:129-318): method 0 = MAX (mask = argmax index inside the H*W
- * plane, first maximum), 1 = AVE.  NC = N*C planes; output extent is the reference's ceil mode.  dx overwritten.    */
+ * plane, first maximum), 1 = AVE.  NC = N*C planes; output extent is the reference's ceil mode.  dx overwritten.
+ * Refused like PoolingLayer::LayerSetUp / Reshape's CHECKs: kernel and stride >= 1, 0 <= pad < kernel, H, W >= 1,
+ * Ho, Wo >= 1.  The kernel chosen is b2c_debug_pool_plan's.                                                         */
 /* DataTransformer::Transform on a batch of uint8 datums (data_transformer.cpp:178-312): crop window and mirror flag per image
  * (device arrays of N), per-channel mean_values[C] or a per-pixel mean_image[C*Hd*Wd] in datum coordinates (or neither), scale.
  * out[n][c][h][w] = (datum[n][c][h_off[n]+h][w_off[n] + (mirror[n] ? crop_w-1-w : w)] - mean) * scale. */
@@ -240,7 +243,8 @@ int b2c_pool_forward(int method, int NC, int H, int W, int kh, int kw, int sh, i
                      float* y, int* mask, void* stream);
 int b2c_pool_backward(int method, int NC, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw, const float* dy,
                       const int* mask, float* dx, void* stream);
-/* y = a + b: EltwiseLayer SUM forward (eltwise_layer.cpp) and the diff accumulation of SplitLayer::Backward.        */
+/* y = a + b: EltwiseLayer SUM forward (eltwise_layer.cpp) and the diff accumulation of SplitLayer::Backward.  Alignment
+ * as b2c_relu_forward; may run in place (y == a or y == b).                                                         */
 int b2c_add(size_t n, const float* a, const float* b, float* y, void* stream);
 /* SoftmaxWithLossLayer (src/caffe/layers/softmax_loss_layer.cpp:96-160), VALID normalisation, labels as float ids:
  * forward writes prob [N,C] and *loss (device scalar); backward writes dx = (prob - onehot) * loss_weight / N.       */
@@ -367,6 +371,23 @@ typedef enum {
  * mode, else 128, 160, 192 or 256).  The CAFFE and SIMT routes report zeros.  Needs n >= 8.  Pure host computation: the
  * grid follows the current device's SM count (132 without a device), N_TILE the B2C_NTILE switch as the launch does. */
 int b2c_debug_conv_plan(const b2c_conv_desc* d, int op, int* out, int n);
+
+/* The kernel b2c_pool_forward (dir 0) or b2c_pool_backward (dir 1) runs (b2c_debug_pool_plan out[0]). */
+typedef enum {
+  B2C_POOL_ROUTE_MAX_SCALAR = 0,    /* MAX forward, one thread per output                                                      */
+  B2C_POOL_ROUTE_MAX_WINDOW = 1,    /* MAX forward, 3x3/2, 2x2/2 or 3x3/1 with Wo % Q == 0 (Q = 4 or 2) and y, mask aligned   */
+                                    /* to 4Q bytes: one thread per Q outputs of a pooled row                                  */
+  B2C_POOL_ROUTE_MAX_BWD_ROW = 2,   /* MAX backward, one 128-thread block per input row (several rows per block when W < 128) */
+  B2C_POOL_ROUTE_MAX_BWD_QUAD = 3,  /* MAX backward, the same three windows with W % 4 == 0 and dx 16-byte aligned: one        */
+                                    /* thread per four input columns                                                          */
+  B2C_POOL_ROUTE_AVE = 4            /* AVE forward or backward, one thread per output element                                 */
+} b2c_pool_route;
+/* Which kernel the pooling call with these arguments takes; out_ptr is y (dir 0) or dx (dir 1), mask_ptr the MAX mask.  The
+ * pointers are only tested for alignment, never dereferenced.  out[0] route (b2c_pool_route), [1] Ho, [2] Wo, [3] Q of the
+ * window kernel (else 0), [4] input rows per block of the row kernel (else 0).  Needs n >= 5.  Refuses (B2C_ERR_INVALID) what
+ * the entry points refuse: kernel or stride < 1, pad outside [0, kernel), H or W < 1, an empty output.  Pure host computation. */
+int b2c_debug_pool_plan(int method, int dir, int NC, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
+                        const void* out_ptr, const void* mask_ptr, int* out, int n);
 
 #define B2C_UNIQUE_ID_BYTES 128
 int b2c_comm_get_unique_id(void* id_out /* B2C_UNIQUE_ID_BYTES */);

@@ -132,6 +132,13 @@ def ip_backward(x, w, dy):
     return dw.astype(np.float32), db.astype(np.float32), dx.astype(np.float32)
 
 
+# InnerProductLayer::Backward_cpu's bias term (inner_product_layer.cpp, caffe_cpu_gemv of dy^T and the ones vector, beta = 1) and
+# the convolution's backward_cpu_bias (base_conv_layer.cpp: one gemv per image): db0 + sum over images and pixels of dy[n][o][p]
+def bias_backward(dy, db0):
+    N, O = dy.shape[:2]
+    return (db0.astype(np.float64) + dy.reshape(N, O, -1).astype(np.float64).sum(axis=(0, 2))).astype(np.float32)
+
+
 # LRNLayer ACROSS_CHANNELS: CrossChannelForward_cpu / CrossChannelBackward_cpu, src/caffe/layers/lrn_layer.cpp; the forward
 # is written the way the reference's own test states it (test_lrn_layer.cpp:61-91, ReferenceLRNForward, with k)
 def lrn_forward(x, size=5, alpha=1.0, beta=0.75, k=1.0):

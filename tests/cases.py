@@ -98,6 +98,39 @@ def sample_index(name, k, size, samples=2048):
     return np.sort(np.random.default_rng(seed).choice(size, min(samples, size), replace=False))
 
 
+GUARD = 64                                   # sentinel floats before and after a guarded buffer (256 bytes: it stays 16-byte aligned)
+SENTINEL = 0xE07B88EF                        # the bits of float32 -7.25e19
+
+
+class Guarded:
+    """n float32 (or int32: the same bits) inside a CUDA buffer whose head and tail hold a sentinel; `off` floats of misalignment.
+    As an output the n values start as NaN, so an element never written shows up; as an input, `init` fills them."""
+
+    def __init__(self, n, off=0, init=None):
+        import numpy as np
+        import torch
+        self.n, self.lo = n, GUARD + off
+        self.buf = torch.full((self.lo + n + GUARD,), float("nan"), device="cuda")
+        self.buf.view(torch.int32)[:self.lo] = SENTINEL - (1 << 32)
+        self.buf.view(torch.int32)[self.lo + n:] = SENTINEL - (1 << 32)
+        if init is not None:
+            self.buf[self.lo:self.lo + n] = torch.from_numpy(np.ascontiguousarray(init).reshape(-1).view(np.float32)).cuda()
+
+    def ptr(self):
+        import ctypes
+        return ctypes.c_void_p(self.buf[self.lo:].data_ptr())
+
+    def read(self, dtype=None):
+        """the n values (as `dtype`, default float32) after checking that nothing outside them changed"""
+        import numpy as np
+        import torch
+        torch.cuda.synchronize()
+        out = self.buf.cpu().numpy().view(np.uint32)
+        guard = np.concatenate([out[:self.lo], out[self.lo + self.n:]])
+        assert (guard == SENTINEL).all(), "write outside the output (a guard band changed)"
+        return out[self.lo:self.lo + self.n].view(dtype or np.float32)
+
+
 def rel_err(a, ref):
     """max|a-ref| / max|ref| -- the blob-level relative error the 1e-3 bar is stated in (DESIGN.md)."""
     import numpy as np

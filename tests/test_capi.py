@@ -164,6 +164,79 @@ print(json.dumps([S, refused]))
     assert f == b == dict(route="caffe", n_tile=0, m_tiles=0, n_tiles=0, tiles=0, grid=0, nkb=0, variant=0)
 
 
+def test_pool_plan_routes():
+    """b2c_debug_pool_plan is host-only: the kernel b2c_pool_forward / b2c_pool_backward pick from the shape and the alignment of
+    y, mask and dx (the routes test_layers_schedule_gpu.py runs), and the arguments PoolingLayer's CHECKs refuse"""
+    A, OFF4, OFF8 = 1 << 20, (1 << 20) + 4, (1 << 20) + 8          # 16-byte aligned, 4 and 8 bytes past it
+
+    def plan(d, NC, H, W, k, s, p, method=0, out=A, mask=A):
+        q = capi.pool_plan(method, d, NC, H, W, (k, k) if isinstance(k, int) else k, (s, s) if isinstance(s, int) else s,
+                           (p, p) if isinstance(p, int) else p, out, mask)
+        return q["route"], q["Ho"], q["Wo"], (q["q"] if d == 0 else q["rpb"])
+    # (NC, H, W, k, s, p): forward, backward
+    table = [
+        ((512, 112, 112, 3, 2, 0), ("max_window", 56, 56, 4), ("max_bwd_quad", 56, 56, 0)),
+        ((24, 56, 56, 3, 2, 0), ("max_window", 28, 28, 4), ("max_bwd_quad", 28, 28, 0)),
+        ((24, 28, 28, 3, 2, 0), ("max_window", 14, 14, 2), ("max_bwd_quad", 14, 14, 0)),
+        ((24, 14, 14, 3, 2, 0), ("max_scalar", 7, 7, 0), ("max_bwd_row", 7, 7, 9)),
+        ((24, 28, 28, 3, 1, 1), ("max_window", 28, 28, 4), ("max_bwd_quad", 28, 28, 0)),
+        ((24, 14, 14, 3, 1, 1), ("max_window", 14, 14, 2), ("max_bwd_row", 14, 14, 9)),
+        ((24, 7, 7, 3, 1, 1), ("max_scalar", 7, 7, 0), ("max_bwd_row", 7, 7, 18)),
+        ((6144, 55, 55, 3, 2, 0), ("max_scalar", 27, 27, 0), ("max_bwd_row", 27, 27, 2)),
+        ((24, 13, 13, 3, 2, 0), ("max_window", 6, 6, 2), ("max_bwd_row", 6, 6, 9)),
+        ((4, 224, 224, 2, 2, 0), ("max_window", 112, 112, 4), ("max_bwd_quad", 112, 112, 0)),
+        ((24, 14, 14, 2, 2, 0), ("max_scalar", 7, 7, 0), ("max_bwd_row", 7, 7, 9)),
+        ((12, 30, 44, 3, 2, 0), ("max_window", 15, 22, 2), ("max_bwd_quad", 15, 22, 0)),
+        ((12, 44, 30, 3, 2, 0), ("max_scalar", 22, 15, 0), ("max_bwd_row", 22, 15, 4)),
+        ((12, 10, 16, 3, 2, 0), ("max_window", 5, 8, 4), ("max_bwd_quad", 5, 8, 0)),             # ceil mode: partial last window
+        ((12, 15, 15, 3, 2, 1), ("max_window", 8, 8, 4), ("max_bwd_row", 8, 8, 8)),
+        ((12, 8, 8, 3, 2, 1), ("max_scalar", 5, 5, 0), ("max_bwd_quad", 5, 5, 0)),
+        ((12, 9, 9, 3, 2, 1), ("max_scalar", 5, 5, 0), ("max_bwd_row", 5, 5, 14)),
+        ((12, 5, 130, 3, 1, 1), ("max_window", 5, 130, 2), ("max_bwd_row", 5, 130, 1)),
+        ((12, 11, 13, (3, 2), (2, 1), (1, 0)), ("max_scalar", 6, 12, 0), ("max_bwd_row", 6, 12, 9)),
+        ((12, 6, 3, 2, 2, 0), ("max_window", 3, 2, 2), ("max_bwd_row", 3, 2, 42)),
+        ((300, 5, 1, 1, 1, 0), ("max_scalar", 5, 1, 0), ("max_bwd_row", 5, 1, 128)),
+        ((12, 9, 9, 1, 2, 0), ("max_scalar", 5, 5, 0), ("max_bwd_row", 5, 5, 14)),
+    ]
+    for args, f, b in table:
+        assert plan(0, *args) == f, (args, plan(0, *args))
+        assert plan(1, *args) == b, (args, plan(1, *args))
+    for args in ((24, 7, 7, 7, 1, 0), (24, 14, 14, 5, 3, 0), (24, 8, 8, 3, 2, 1), (24, 9, 9, 2, 2, 0), (24, 10, 14, (3, 2), (2, 3), (1, 0))):
+        assert plan(0, *args, method=1)[0] == plan(1, *args, method=1)[0] == "ave"
+    assert plan(0, 24, 10, 14, (3, 2), (2, 3), (1, 0), method=1) == ("ave", 6, 5, 0)
+    # alignment: y and mask must both sit on 4Q bytes for the window kernel, dx on 16 for the quad kernel
+    assert plan(0, 24, 56, 56, 3, 2, 0, out=OFF4)[0] == plan(0, 24, 56, 56, 3, 2, 0, mask=OFF4)[0] == "max_scalar"
+    assert plan(0, 24, 56, 56, 3, 2, 0, out=OFF8)[0] == "max_scalar"
+    assert plan(0, 24, 28, 28, 3, 2, 0, out=OFF8, mask=OFF8) == ("max_window", 14, 14, 2)
+    assert plan(1, 24, 56, 56, 3, 2, 0, out=OFF8) == ("max_bwd_row", 28, 28, 2)
+    # refused, by the query and by both entry points, before anything is launched
+    L = m.lib()
+    one = C.c_void_p(A)
+    bad = [
+        (0, 8, 8, 0, 3, 1, 1, 0, 0),          # kernel 0
+        (0, 8, 8, 3, 0, 1, 1, 0, 0),
+        (0, 8, 8, 3, 3, 0, 1, 0, 0),          # stride 0
+        (0, 8, 8, 3, 3, 1, 0, 0, 0),
+        (0, 8, 8, 3, 3, 1, 1, 3, 0),          # pad == kernel
+        (0, 8, 8, 3, 3, 1, 1, 0, 3),
+        (0, 8, 8, 3, 3, 1, 1, -1, 0),         # negative pad
+        (0, 0, 8, 3, 3, 1, 1, 0, 0),          # empty map
+        (0, 8, 0, 3, 3, 1, 1, 0, 0),
+        (0, 1, 8, 3, 3, 1, 1, 0, 0),          # H + 2 pad < kernel: no output row
+        (0, 8, 2, 5, 5, 1, 1, 1, 1),          # W + 2 pad < kernel
+        (2, 8, 8, 3, 3, 1, 1, 0, 0),          # STOCHASTIC
+    ]
+    for method, H, W, kh, kw, sh, sw, ph, pw in bad:
+        for d in (0, 1):
+            with pytest.raises(capi.B2CError):
+                capi.pool_plan(method, d, 4, H, W, (kh, kw), (sh, sw), (ph, pw), A, A)
+        assert L.b2c_pool_forward(method, 4, H, W, kh, kw, sh, sw, ph, pw, one, one, one, None) == -1
+        assert L.b2c_pool_backward(method, 4, H, W, kh, kw, sh, sw, ph, pw, one, one, one, None) == -1
+    with pytest.raises(capi.B2CError):
+        capi.pool_plan(0, 0, 0, 8, 8, (3, 3), (1, 1), (0, 0))              # no planes
+    assert L.b2c_debug_pool_plan(0, 0, 4, 8, 8, 3, 3, 1, 1, 0, 0, one, one, (C.c_int * 4)(), 4) == -1     # n < 5
+
+
 def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():

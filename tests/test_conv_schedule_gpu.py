@@ -29,7 +29,7 @@ import numpy as np
 import pytest
 
 import oracle as o
-from cases import make, tensors, rel_err
+from cases import Guarded, make, tensors, rel_err
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -38,8 +38,6 @@ import caffe_mpi_b200 as m  # noqa: E402
 from caffe_mpi_b200 import capi  # noqa: E402
 
 TOL = 1e-4
-GUARD = 64                                   # sentinel floats before and after the output (256 bytes: it stays 16-byte aligned)
-SENTINEL = np.float32(-7.25e19)
 STAGED = ("staged", "staged_plane")
 TENSOR_CORE = STAGED + ("gather", "gather_scatter")
 
@@ -173,27 +171,6 @@ CASES = [
      lambda q0, q1, S: R(q0, "gather", tiles=196, nkb=18) and q0["tiles"] > q0["grid"], None, False),
 ]
 IDS = [c[0] for c in CASES]
-
-
-class Guarded:
-    """An output of n floats inside a NaN-prefilled buffer with sentinel guard bands; `off` floats of misalignment."""
-
-    def __init__(self, n, off=0, init=None):
-        self.n, self.lo = n, GUARD + off
-        self.buf = torch.full((self.lo + n + GUARD,), float("nan"), device="cuda")
-        self.buf[:self.lo] = float(SENTINEL)
-        self.buf[self.lo + n:] = float(SENTINEL)
-        if init is not None:
-            self.buf[self.lo:self.lo + n] = dev(init.reshape(-1))
-
-    def ptr(self):
-        return ptr(self.buf[self.lo:])
-
-    def read(self):
-        out = host(self.buf)
-        guard = np.concatenate([out[:self.lo], out[self.lo + self.n:]])
-        assert (guard.view(np.int32) == SENTINEL.view(np.int32)).all(), "write outside the output (a guard band changed)"
-        return out[self.lo:self.lo + self.n]
 
 
 class Run:

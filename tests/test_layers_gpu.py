@@ -150,23 +150,6 @@ def test_batchnorm_residual_tail_is_bitwise_the_three_layers(rng, shape, two_par
         assert np.array_equal(a, b), name
 
 
-@pytest.mark.parametrize("H,k,s,pad,method", [(112, 3, 2, 0, 0), (7, 7, 1, 0, 1), (8, 3, 2, 1, 0), (9, 2, 2, 0, 1), (13, 3, 2, 0, 0), (14, 3, 1, 1, 0), (12, 3, 1, 1, 0), (16, 2, 2, 0, 0), (28, 3, 2, 0, 0), (20, 3, 2, 1, 0)])
-def test_pooling(rng, H, k, s, pad, method):
-    x = rng.standard_normal((2, 5, H, H)).astype(np.float32)
-    y, mask = lo.pool_forward(x, method, (k, k), (s, s), (pad, pad))
-    dy = rng.standard_normal(y.shape).astype(np.float32)
-    X, DY = dev(x), dev(dy)
-    Y = torch.empty(y.shape, device="cuda")
-    M = torch.empty(y.shape, dtype=torch.int32, device="cuda")
-    DX = torch.full(x.shape, 7.0, device="cuda")
-    capi.check(m.lib().b2c_pool_forward(method, 10, H, H, k, k, s, s, pad, pad, p(X), p(Y), p(M), st()))
-    capi.check(m.lib().b2c_pool_backward(method, 10, H, H, k, k, s, s, pad, pad, p(DY), p(M), p(DX), st()))
-    assert rel_err(host(Y), y) < TOL
-    if method == 0:
-        assert np.array_equal(host(M), mask)
-    assert rel_err(host(DX), lo.pool_backward(dy, mask, x.shape, method, (k, k), (s, s), (pad, pad))) < TOL
-
-
 def test_add_and_bias(rng):
     a, b = rng.standard_normal(1001).astype(np.float32), rng.standard_normal(1001).astype(np.float32)
     A, B = dev(a), dev(b)
