@@ -11,7 +11,12 @@
 //   Eltwise SUM     src/caffe/layers/eltwise_layer.cpp
 //   SoftmaxWithLoss src/caffe/layers/softmax_loss_layer.cpp:96-160  loss = -sum log p[label] / N (VALID normalisation, no
 //                                                                    ignore_label); dx = (p - onehot) * loss_weight / N
+//   Softmax         src/caffe/layers/softmax_layer.cu               over the C axis of [outer, C, inner]; dx = (dy - sum_c dy y) y
+//   Sigmoid         src/caffe/layers/sigmoid_layer.cu:9-13           y = 1 / (1 + exp(-x)); dx = dy y (1 - y)
+//   SigmoidCrossEntropyLoss  sigmoid_cross_entropy_loss_layer.cpp   the stable loss expression / N; dx = (sigmoid(x) - t) * loss_weight / N
+//   EuclideanLoss   src/caffe/layers/euclidean_loss_layer.cu        diff = a - b, loss = sum diff^2 / N / 2; dx = +-loss_weight / N * diff
 #include <float.h>
+#include <type_traits>
 #include <cooperative_groups.h>
 #include "b2c_common.cuh"
 #include "bn_common.cuh"
@@ -436,9 +441,10 @@ __global__ void __launch_bounds__(256) add_kernel(size_t n, int vec, const float
 
 // ---- softmax with loss ------------------------------------------------------------------------------------------
 // one block per sample; prob[N,C]; labels are float class ids.  The loss itself is summed by softmax_loss_sum_kernel in a fixed
-// order (an atomicAdd per sample made the last bit of the reported loss depend on block scheduling)
+// order (an atomicAdd per sample made the last bit of the reported loss depend on block scheduling).  No __restrict__: the Softmax
+// layer runs this kernel in place (prob == logits); every element is read by the thread that later writes it, before that write.
 __global__ void __launch_bounds__(256)
-softmax_loss_fwd_kernel(int C, const float* __restrict__ logits, float* __restrict__ prob) {
+softmax_loss_fwd_kernel(int C, const float* logits, float* prob) {
   const int n = blockIdx.x;
   const float* z = logits + (size_t)n * C;
   float mx = -FLT_MAX, dummy = 0.f;
@@ -476,6 +482,179 @@ softmax_loss_bwd_kernel(size_t total, int C, const float* __restrict__ prob, con
     const int c = (int)(i - n * C);
     dx[i] = (prob[i] - (c == (int)labels[n] ? 1.f : 0.f)) * scale;
   }
+}
+
+// ---- Softmax ------------------------------------------------------------------------------------------------------
+// Over the C axis of an [outer, C, inner] view.  inner == 1 runs softmax_loss_fwd_kernel above (alias-safe): one block per row.
+// inner > 1: one thread per
+// (outer, inner) column (VEC: four adjacent columns), so a warp's loads and stores run along `inner` and coalesce; each column
+// takes max, then expf(z - max) and the sum, then the scale, in the row kernel's expressions.  No __restrict__: y may be x.
+template <bool VEC>
+__global__ void __launch_bounds__(256) softmax_col_fwd_kernel(size_t cols, int C, int inner, const float* x, float* y) {
+  using V = typename std::conditional<VEC, float4, float>::type;
+  const int w = VEC ? inner / 4 : inner;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cols; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = i / w, base = o * C * w + (i - o * w);
+    const V* z = reinterpret_cast<const V*>(x) + base;
+    V* p = reinterpret_cast<V*>(y) + base;
+    if constexpr (VEC) {
+      float4 mx = make_float4(-FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX), s = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int c = 0; c < C; ++c) { const float4 v = z[(size_t)c * w]; mx.x = fmaxf(mx.x, v.x); mx.y = fmaxf(mx.y, v.y); mx.z = fmaxf(mx.z, v.z); mx.w = fmaxf(mx.w, v.w); }
+      for (int c = 0; c < C; ++c) {
+        const float4 v = z[(size_t)c * w];
+        const float4 e = make_float4(expf(v.x - mx.x), expf(v.y - mx.y), expf(v.z - mx.z), expf(v.w - mx.w));
+        p[(size_t)c * w] = e;
+        s.x += e.x; s.y += e.y; s.z += e.z; s.w += e.w;
+      }
+      const float4 inv = make_float4(1.f / s.x, 1.f / s.y, 1.f / s.z, 1.f / s.w);
+      for (int c = 0; c < C; ++c) { float4 e = p[(size_t)c * w]; e.x *= inv.x; e.y *= inv.y; e.z *= inv.z; e.w *= inv.w; p[(size_t)c * w] = e; }
+    } else {
+      float mx = -FLT_MAX, s = 0.f;
+      for (int c = 0; c < C; ++c) mx = fmaxf(mx, z[(size_t)c * w]);
+      for (int c = 0; c < C; ++c) { const float e = expf(z[(size_t)c * w] - mx); p[(size_t)c * w] = e; s += e; }
+      const float inv = 1.f / s;
+      for (int c = 0; c < C; ++c) p[(size_t)c * w] *= inv;
+    }
+  }
+}
+// dx = (dy - sum_c dy * y) * y  (softmax_layer.cu: channel dot, channel subtract, multiply by the top).  dx may be dy.
+__global__ void __launch_bounds__(256) softmax_row_bwd_kernel(int C, const float* y, const float* dy, float* dx) {
+  const size_t off = (size_t)blockIdx.x * C;
+  float dot = 0.f, dummy = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) dot += dy[off + c] * y[off + c];
+  block_sum2(dot, dummy);                          // (ends on a barrier: every dy read is done before dx may overwrite it)
+  for (int c = threadIdx.x; c < C; c += blockDim.x) dx[off + c] = (dy[off + c] - dot) * y[off + c];
+}
+template <bool VEC>
+__global__ void __launch_bounds__(256) softmax_col_bwd_kernel(size_t cols, int C, int inner, const float* y, const float* dy, float* dx) {
+  using V = typename std::conditional<VEC, float4, float>::type;
+  const int w = VEC ? inner / 4 : inner;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cols; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = i / w, base = o * C * w + (i - o * w);
+    const V* yv = reinterpret_cast<const V*>(y) + base;
+    const V* dv = reinterpret_cast<const V*>(dy) + base;
+    V* xv = reinterpret_cast<V*>(dx) + base;
+    if constexpr (VEC) {
+      float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int c = 0; c < C; ++c) {
+        const float4 a = dv[(size_t)c * w], b = yv[(size_t)c * w];
+        d.x += a.x * b.x; d.y += a.y * b.y; d.z += a.z * b.z; d.w += a.w * b.w;
+      }
+      for (int c = 0; c < C; ++c) {
+        const float4 a = dv[(size_t)c * w], b = yv[(size_t)c * w];
+        xv[(size_t)c * w] = make_float4((a.x - d.x) * b.x, (a.y - d.y) * b.y, (a.z - d.z) * b.z, (a.w - d.w) * b.w);
+      }
+    } else {
+      float d = 0.f;
+      for (int c = 0; c < C; ++c) d += dv[(size_t)c * w] * yv[(size_t)c * w];
+      for (int c = 0; c < C; ++c) xv[(size_t)c * w] = (dv[(size_t)c * w] - d) * yv[(size_t)c * w];
+    }
+  }
+}
+
+// ---- Sigmoid, SigmoidCrossEntropyLoss, EuclideanLoss ------------------------------------------------------------------
+// sigmoid_layer.cu:9-13.  The one expression b2c_sigmoid_forward and b2c_sigmoid_ce_loss_backward share.
+__device__ __forceinline__ float sigmoid_of(float x) { return 1.f / (1.f + expf(-x)); }
+
+enum EwOp { EW_SIGMOID_FWD, EW_SIGMOID_BWD, EW_SIGCE_BWD, EW_SCALE };
+// y = op(a, b, s) per element: SIGMOID_FWD sigmoid(a); SIGMOID_BWD b * a * (1 - a) with a = y, b = dy; SIGCE_BWD (sigmoid(a) - b) * s;
+// SCALE s * a.  In place allowed (no __restrict__)
+template <int OP>
+__device__ __forceinline__ float ew_apply(float a, float b, float s) {
+  if (OP == EW_SIGMOID_FWD) return sigmoid_of(a);
+  if (OP == EW_SIGMOID_BWD) return b * a * (1.f - a);
+  if (OP == EW_SIGCE_BWD) return __fmul_rn(sigmoid_of(a) - b, s);
+  return s * a;
+}
+template <int OP>
+__global__ void __launch_bounds__(256) ew_kernel(size_t n, int vec, const float* a, const float* b, float s, float* y) {
+  const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  const bool two = OP == EW_SIGMOID_BWD || OP == EW_SIGCE_BWD;
+  for (size_t i = tid; i < n4; i += step) {
+    const float4 u = reinterpret_cast<const float4*>(a)[i];
+    const float4 v = two ? reinterpret_cast<const float4*>(b)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    reinterpret_cast<float4*>(y)[i] = make_float4(ew_apply<OP>(u.x, v.x, s), ew_apply<OP>(u.y, v.y, s), ew_apply<OP>(u.z, v.z, s), ew_apply<OP>(u.w, v.w, s));
+  }
+  for (size_t i = n4 * 4 + tid; i < n; i += step) y[i] = ew_apply<OP>(a[i], two ? b[i] : 0.f, s);
+}
+
+// Loss sums: ONE thread-block cluster of LOSS_THREADS-thread CTAs (bn_stats_kernel's pattern: each CTA sums a contiguous slice, the
+// CTA sums meet in rank 0 through distributed shared memory in rank order; no atomics, no scratch, one launch).  The cluster size
+// depends only on `count`, so the summation order -- and the bits -- are the same on every call.  Terms are computed in float and
+// summed in double; the float result is formed once at the end.
+//   MODE 0 (SigmoidCrossEntropyLoss): term = x (t - [x >= 0]) - log(1 + exp(x - 2 x [x >= 0])), loss = -sum / N
+//   MODE 1 (EuclideanLoss):           d = a - b stored to diff, term = d * d, loss = sum / N / 2
+constexpr int LOSS_THREADS = 512;
+constexpr int LOSS_CLUSTER = 8;                    // the portable cluster limit
+template <int MODE>
+__device__ __forceinline__ float loss_term(float a, float b, float* d) {
+  if (MODE == 0) {
+    const float pos = a >= 0.f ? 1.f : 0.f;
+    return a * (b - pos) - logf(1.f + expf(a - 2.f * a * pos));
+  }
+  const float v = a - b;
+  *d = v;
+  return __fmul_rn(v, v);
+}
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+template <int MODE, bool VEC>
+__global__ void __launch_bounds__(LOSS_THREADS)
+loss_sum_kernel(size_t count, int N, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ diff, float* __restrict__ loss) {
+  cg::cluster_group cluster = cg::this_cluster();
+  const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
+  const size_t units = VEC ? count / 4 : count, len = (units + nranks - 1) / nranks;
+  const size_t lo = rank * len < units ? rank * len : units, hi = lo + len < units ? lo + len : units;
+  double acc = 0.0;
+  for (size_t i = lo + threadIdx.x; i < hi; i += LOSS_THREADS) {
+    if (VEC) {
+      const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
+      float4 d;
+      const float t0 = loss_term<MODE>(u.x, v.x, &d.x), t1 = loss_term<MODE>(u.y, v.y, &d.y);
+      const float t2 = loss_term<MODE>(u.z, v.z, &d.z), t3 = loss_term<MODE>(u.w, v.w, &d.w);
+      if (MODE == 1) reinterpret_cast<float4*>(diff)[i] = d;
+      acc += ((double)t0 + (double)t1) + ((double)t2 + (double)t3);
+    } else {
+      float d;
+      const float t = loss_term<MODE>(a[i], b[i], &d);
+      if (MODE == 1) diff[i] = d;
+      acc += (double)t;
+    }
+  }
+  if (VEC && rank == 0 && threadIdx.x < count % 4) {        // the float4 pass's tail
+    const size_t i = units * 4 + threadIdx.x;
+    float d;
+    const float t = loss_term<MODE>(a[i], b[i], &d);
+    if (MODE == 1) diff[i] = d;
+    acc += (double)t;
+  }
+  __shared__ double wsum[LOSS_THREADS / 32];
+  __shared__ double part;
+  acc = warp_sum_d(acc);
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < LOSS_THREADS / 32; ++w) s += wsum[w];
+    part = s;
+  }
+  cluster.sync();
+  if (rank == 0 && threadIdx.x == 0) {
+    double s = 0.0;
+    for (unsigned r = 0; r < nranks; ++r) s += *cluster.map_shared_rank(&part, r);
+    const float f = (float)s;
+    *loss = MODE == 0 ? -f / (float)N : f / (float)N / 2.f;
+  }
+  cluster.sync();                                   // remote shared memory stays valid until rank 0 has read it
+}
+// CTAs per loss cluster: one per 64K float4 units (256K values), at most LOSS_CLUSTER.  A function of the count alone.
+static inline unsigned loss_cluster_size(size_t count) {
+  unsigned cs = 1;
+  while (cs < LOSS_CLUSTER && count / (cs * 2) >= (1u << 18)) cs *= 2;
+  return cs;
 }
 
 }  // namespace b2c
@@ -722,6 +901,86 @@ extern "C" int b2c_softmax_loss_backward(int N, int C, const float* prob, const 
   softmax_loss_bwd_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(total, C, prob, labels, loss_weight / (float)N, dx);
   B2C_POST_LAUNCH();
   return B2C_OK;
+}
+static bool al16(std::initializer_list<const void*> ptrs) {
+  for (const void* p : ptrs) if (reinterpret_cast<uintptr_t>(p) & 15) return false;
+  return true;
+}
+extern "C" int b2c_softmax_forward(int outer, int C, int inner, const float* x, float* y, void* stream) {
+  NEED(x && y && outer > 0 && C > 0 && inner > 0, "b2c_softmax_forward: bad argument");
+  if (inner == 1) {                                // every [N, C] use: SoftmaxWithLoss's row kernel, so prob and this top agree bit for bit
+    softmax_loss_fwd_kernel<<<outer, 256, 0, as_stream(stream)>>>(C, x, y);
+    B2C_POST_LAUNCH();
+    return B2C_OK;
+  }
+  const bool vec = inner % 4 == 0 && al16({x, y});
+  const size_t cols = (size_t)outer * (vec ? inner / 4 : inner);
+  if (vec) softmax_col_fwd_kernel<true><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, x, y);
+  else softmax_col_fwd_kernel<false><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, x, y);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+extern "C" int b2c_softmax_backward(int outer, int C, int inner, const float* y, const float* dy, float* dx, void* stream) {
+  NEED(y && dy && dx && outer > 0 && C > 0 && inner > 0, "b2c_softmax_backward: bad argument");
+  if (inner == 1) {
+    softmax_row_bwd_kernel<<<outer, 256, 0, as_stream(stream)>>>(C, y, dy, dx);
+    B2C_POST_LAUNCH();
+    return B2C_OK;
+  }
+  const bool vec = inner % 4 == 0 && al16({y, dy, dx});
+  const size_t cols = (size_t)outer * (vec ? inner / 4 : inner);
+  if (vec) softmax_col_bwd_kernel<true><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, y, dy, dx);
+  else softmax_col_bwd_kernel<false><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, y, dy, dx);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+template <int OP>
+static int launch_ew(size_t n, const float* a, const float* b, float s, float* y, void* stream) {
+  if (!n) return B2C_OK;
+  const bool al = al16({a, b, y});                 // (b may be null: aligned)
+  ew_kernel<OP><<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, a, b, s, y);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+extern "C" int b2c_sigmoid_forward(size_t n, const float* x, float* y, void* stream) {
+  NEED(x && y, "b2c_sigmoid_forward: null");
+  return launch_ew<EW_SIGMOID_FWD>(n, x, nullptr, 0.f, y, stream);
+}
+extern "C" int b2c_sigmoid_backward(size_t n, const float* y, const float* dy, float* dx, void* stream) {
+  NEED(y && dy && dx, "b2c_sigmoid_backward: null");
+  return launch_ew<EW_SIGMOID_BWD>(n, y, dy, 0.f, dx, stream);
+}
+template <int MODE>
+static int launch_loss_sum(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream) {
+  const bool vec = al16({a, b, diff});
+  const unsigned cs = loss_cluster_size(count);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(cs, 1, 1);
+  cfg.blockDim = dim3(LOSS_THREADS, 1, 1);
+  cfg.stream = as_stream(stream);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  B2C_CUDA_OK(cudaLaunchKernelEx(&cfg, vec ? loss_sum_kernel<MODE, true> : loss_sum_kernel<MODE, false>, count, N, a, b, diff, loss));
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+extern "C" int b2c_sigmoid_ce_loss_forward(int N, size_t count, const float* x, const float* target, float* loss, void* stream) {
+  NEED(x && target && loss && N > 0 && count > 0, "b2c_sigmoid_ce_loss_forward: bad argument");
+  return launch_loss_sum<0>(N, count, x, target, nullptr, loss, stream);
+}
+extern "C" int b2c_sigmoid_ce_loss_backward(size_t count, const float* x, const float* target, float scale, float* dx, void* stream) {
+  NEED(x && target && dx, "b2c_sigmoid_ce_loss_backward: null");
+  return launch_ew<EW_SIGCE_BWD>(count, x, target, scale, dx, stream);
+}
+extern "C" int b2c_euclidean_loss_forward(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream) {
+  NEED(a && b && diff && loss && N > 0 && count > 0, "b2c_euclidean_loss_forward: bad argument");
+  return launch_loss_sum<1>(N, count, a, b, diff, loss, stream);
+}
+extern "C" int b2c_euclidean_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream) {
+  NEED(diff && dx, "b2c_euclidean_loss_backward: null");
+  return launch_ew<EW_SCALE>(count, diff, nullptr, alpha, dx, stream);
 }
 // y[n][o] += b[o] and db[o] += sum_n dy[n][o]: InnerProduct bias (inner_product_layer.cpp), via the conv bias kernels with P = 1
 extern "C" int b2c_bias_forward(int N, int O, int P, const float* bias, float* y, void* stream) {

@@ -258,6 +258,23 @@ int b2h_net_layer_uses_database(void* h, int i) {
   return i >= 0 && i < (int)ls.size() && ls[i].use_database ? 1 : 0;
 }
 int b2h_net_reduce_buckets(void* h) { return static_cast<Net*>(h)->reduce_buckets(); }
+// layer i's need-backward result (loss pruning included): bit 0 = the layer runs backward, bit 1 + b = bottom b gets a gradient
+long long b2h_net_layer_backward(void* h, int i) {
+  const auto& ls = static_cast<Net*>(h)->layers();
+  if (i < 0 || i >= (int)ls.size()) return -1;
+  long long v = ls[i].need_backward ? 1 : 0;
+  for (size_t b = 0; b < ls[i].propagate_down.size() && b < 62; ++b) if (ls[i].propagate_down[b]) v |= 2ll << b;
+  return v;
+}
+int b2h_net_layer_bottoms(void* h, int i) {
+  const auto& ls = static_cast<Net*>(h)->layers();
+  return i >= 0 && i < (int)ls.size() ? (int)ls[i].param.bottom.size() : -1;
+}
+// the blob the trainer reports as its loss (Net::loss_blob); empty when the net has none
+int b2h_net_loss_blob(void* h, char* name, int cap) {
+  snprintf(name, cap, "%s", static_cast<Net*>(h)->loss_blob().c_str());
+  return 0;
+}
 
 // SolverParameter from a solver.prototxt of any type (SGD, Nesterov, AdaGrad, RMSProp, AdaDelta, Adam; `type` or the legacy
 // `solver_type`); returns a solver handle like b2h_solver_create_typed

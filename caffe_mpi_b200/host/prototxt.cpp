@@ -174,7 +174,25 @@ int pooled_extent(int in, int k, int s, int p) {        // PoolingLayer::Reshape
   if (p > 0 && (o - 1) * s >= in + p) --o;
   return o;
 }
+int canonical_axis(int axis, const std::vector<int>& s) {  // Blob::CanonicalAxisIndex, with its message
+  const int n = (int)s.size();
+  if (axis < -n || axis >= n) {
+    std::string shp;
+    for (int d : s) shp += std::to_string(d) + " ";
+    Fatal(__FILE__, __LINE__, "axis " + std::to_string(axis) + " out of range for " + std::to_string(n) + "-D Blob with shape " + shp + "(" +
+                                  std::to_string(prod(s)) + ")");
+  }
+  return axis < 0 ? axis + n : axis;
+}
 }  // namespace
+
+int LabelBottom(const std::string& type) {
+  return type == "SoftmaxWithLoss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy" ? 1 : -1;
+}
+bool IsLossType(const std::string& ty) { return ty.size() >= 4 && ty.compare(ty.size() - 4, 4, "Loss") == 0; }
+float TopLossWeight(const NetLayer& L, size_t t) {
+  return t < L.loss_weight.size() ? L.loss_weight[t] : (IsLossType(L.param.type) && t == 0 ? 1.f : 0.f);
+}
 
 Net Net::FromFile(const std::string& path, Phase phase, int batch_override) {
   return Net(ParseTextProtoFile(path), phase, batch_override);
@@ -380,8 +398,31 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
         s[L.concat_axis] += b[L.concat_axis];
       }
       tops.push_back(s);
+    } else if (type == "Flatten") {
+      const PMessage* fp = lp.sub("flatten_param");
+      const std::vector<int>& bs = bottom_shape(0);
+      B2_CHECK(L.param.top.empty() || L.param.top[0] != L.param.bottom[0], "Flatten Layer does not allow in-place computation.");
+      L.flatten_axis = canonical_axis(fp ? (int)fp->integer("axis", 1) : 1, bs);                // flatten_layer.cpp:8-30
+      L.flatten_end_axis = canonical_axis(fp ? (int)fp->integer("end_axis", -1) : -1, bs);
+      std::vector<int> s(bs.begin(), bs.begin() + L.flatten_axis);
+      int flat = 1;
+      for (int a = L.flatten_axis; a <= L.flatten_end_axis; ++a) flat *= bs[a];
+      s.push_back(flat);
+      for (int a = L.flatten_end_axis + 1; a < (int)bs.size(); ++a) s.push_back(bs[a]);
+      tops.push_back(s);
+    } else if (type == "Softmax") {
+      const PMessage* sp = lp.sub("softmax_param");
+      L.softmax_axis = canonical_axis(sp ? (int)sp->integer("axis", 1) : 1, bottom_shape(0));   // softmax_layer.cpp:12-13
+      tops.push_back(bottom_shape(0));
     } else if (type == "SoftmaxWithLoss" || type == "EuclideanLoss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy") {
       if (const PMessage* ap = lp.sub("accuracy_param")) L.accuracy_top_k = (int)ap->integer("top_k", 1);
+      if (type == "EuclideanLoss" || type == "SigmoidCrossEntropyLoss") {
+        const std::vector<int>& a = bottom_shape(0);
+        const std::vector<int>& b = bottom_shape(1);
+        B2_CHECK(!a.empty() && !b.empty() && a[0] == b[0], "The data and label should have the same number.");   // loss_layer.cpp:19-20
+        if (type == "EuclideanLoss") B2_CHECK(prod(a, 1) == prod(b, 1), "Inputs must have the same dimension.");
+        else B2_CHECK(prod(a) == prod(b), "SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.");
+      }
       for (size_t i = 0; i < L.param.top.size(); ++i) tops.push_back({});
     } else if (type == "ReLU" && (L.relu_slope = (float)(lp.sub("relu_param") ? lp.sub("relu_param")->num("negative_slope", 0.0) : 0.0), false)) {
     } else if ((type == "LRN" || type == "Dropout") && ([&] {
@@ -400,7 +441,7 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
                    for (auto* f : q->all("coeff")) if (!f->is_msg()) L.eltwise_coeff.push_back((float)std::atof(f->scalar.c_str()));
                  }
                }(), false)) {
-    } else if (type == "ReLU" || type == "Dropout" || type == "LRN" || type == "Eltwise" || type == "Softmax" || type == "Sigmoid" ||
+    } else if (type == "ReLU" || type == "Dropout" || type == "LRN" || type == "Eltwise" || type == "Sigmoid" ||
                type == "TanH" || type == "Power" || type == "Bias" || type == "ELU" || type == "PReLU" || type == "Split") {
       for (size_t i = 0; i < std::max<size_t>(1, L.param.top.size()); ++i) tops.push_back(bottom_shape(0));
     } else {
@@ -416,6 +457,12 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       if (spec.lr_mult != 0.f) layer_bw = true;
     }
     if (is_data) layer_bw = false;
+    L.need_backward = layer_bw;
+    for (size_t i = 0; i < L.param.bottom.size(); ++i) {     // a label / target bottom never receives a gradient (LabelBottom)
+      const bool want = layer_bw && (need_bw.count(L.param.bottom[i]) ? need_bw[L.param.bottom[i]] : false);
+      L.propagate_down.push_back(want && (int)i != LabelBottom(type));
+      if (want && (int)i == LabelBottom(type)) L.label_wants_gradient = true;
+    }
     for (size_t i = 0; i < L.param.top.size(); ++i) {
       B2_CHECK(i < tops.size(), "layer '" + L.param.name + "' declares more tops than its type produces");
       shapes_[L.param.top[i]] = tops[i];
@@ -429,6 +476,37 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
     layer_top_shapes_.push_back(tops);
     layers_.push_back(std::move(L));
   }
+  // loss pruning (net.cpp:285-330, blobs_under_loss): walking back from the last layer, a layer none of whose tops has a non-zero
+  // loss weight or feeds a layer that reaches one does not run backward, and none of its bottoms gets a gradient.  (The
+  // reference's skip-propagate-down half needs propagate_down params, which this parser does not take.)
+  std::set<std::string> under_loss;
+  for (int li = (int)layers_.size() - 1; li >= 0; --li) {
+    NetLayer& L = layers_[li];
+    bool contributes = false;
+    for (size_t t = 0; t < L.param.top.size(); ++t)
+      contributes |= TopLossWeight(L, t) != 0.f || under_loss.count(L.param.top[t]) > 0;
+    if (!contributes) {
+      L.need_backward = false;
+      L.label_wants_gradient = false;
+      L.propagate_down.assign(L.param.bottom.size(), false);
+    } else {
+      for (auto& b : L.param.bottom) under_loss.insert(b);
+    }
+  }
+  // force_backward (net.cpp:342-360, after the pruning): every layer runs backward and every bottom gets a gradient except the ones
+  // a loss layer refuses (LossLayer::AllowForceBackward: the label bottom).  Data layers have nothing to propagate to.
+  if (np.boolean("force_backward", false)) {
+    for (NetLayer& L : layers_) {
+      const std::string& ty = L.param.type;
+      if (ty == "Data" || ty == "ImageData" || ty == "HDF5Data" || ty == "Input" || ty == "DummyData") continue;
+      L.need_backward = true;
+      for (size_t i = 0; i < L.propagate_down.size(); ++i)
+        if ((int)i != LabelBottom(ty)) L.propagate_down[i] = true;
+    }
+  }
+  for (ConvEntry& c : convs_) c.propagate_down = layers_[c.layer_id].propagate_down[0];
+  for (const NetLayer& L : layers_)
+    if (IsLossType(L.param.type) && !L.param.top.empty() && TopLossWeight(L, 0) != 0.f) loss_blob_ = L.param.top[0];
 }
 
 // ================================================================================================ solver

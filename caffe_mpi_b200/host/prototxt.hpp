@@ -75,7 +75,23 @@ struct NetLayer {                       // one LayerParameter after phase filter
   long long transform_random_seed = -1; // TransformationParameter.random_seed
   bool use_database = false;            // the source opened: this layer reads it (else the synthetic in-memory source stands in)
   std::vector<int> input_shape;         // Input / DummyData layers
+  int softmax_axis = 1;                 // SoftmaxParameter.axis, canonicalised against the bottom's axes
+  int flatten_axis = 1, flatten_end_axis = -1;   // FlattenParameter.axis / end_axis, canonicalised
+  // Net::Init's need-backward result (net.cpp:160-330), loss pruning included: whether the layer runs backward, and per bottom
+  // whether it receives a gradient.  TrainNet reads these; nothing else restates the rule.
+  bool need_backward = false;
+  std::vector<bool> propagate_down;
+  bool label_wants_gradient = false;    // the LabelBottom bottom needs a gradient (and the layer runs backward)
 };
+
+// The bottom a loss-like layer reads its labels / targets from, which never receives a gradient (-1: none; EuclideanLoss sends
+// gradient to both of its bottoms).  SoftmaxWithLoss, SigmoidCrossEntropyLoss and Accuracy: bottom 1.
+int LabelBottom(const std::string& type);
+// A layer type whose name ends in "Loss" (LossLayer's subclasses)
+bool IsLossType(const std::string& type);
+// LayerParameter.loss_weight of top t, defaulting as Layer::SetLossWeights / LossLayer::LayerSetUp do: 1 for the first top of a
+// layer whose type ends in "Loss", 0 otherwise
+float TopLossWeight(const NetLayer& L, size_t t);
 
 struct LearnableParam { std::string layer; int layer_id, blob_id; size_t count; std::vector<int> shape; float lr_mult, decay_mult; };
 
@@ -97,7 +113,11 @@ class Net {
   int reduce_buckets() const { return reduce_buckets_; }
   float global_grad_scale() const { return global_grad_scale_; }
   size_t learnable_count() const;
+  // the training loss a trainer reports: the first top of the last layer whose type ends in "Loss" and whose first top has a
+  // non-zero loss weight (empty: none)
+  const std::string& loss_blob() const { return loss_blob_; }
  private:
+  std::string loss_blob_;
   std::string name_;
   Phase phase_ = TRAIN;
   std::vector<NetLayer> layers_;

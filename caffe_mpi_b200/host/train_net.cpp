@@ -287,6 +287,61 @@ void SoftmaxWithLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>
                                       b[0]->mutable_gpu_diff(), S()));
 }
 
+// ================================================================================================ Softmax / Sigmoid / Flatten
+static void softmax_view(Blob* b, int axis, int* outer, int* C, int* inner) {
+  *outer = (int)b->count(0, axis); *C = b->shape(axis); *inner = (int)b->count(axis + 1);
+}
+void SoftmaxLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  int outer, C, inner;
+  softmax_view(b[0], axis_, &outer, &C, &inner);
+  B2C_CHECK(b2c_softmax_forward(outer, C, inner, b[0]->gpu_data(), t[0]->mutable_gpu_data(), S()));
+}
+void SoftmaxLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0]) return;
+  int outer, C, inner;
+  softmax_view(t[0], axis_, &outer, &C, &inner);
+  B2C_CHECK(b2c_softmax_backward(outer, C, inner, t[0]->gpu_data(), t[0]->gpu_diff(), b[0]->mutable_gpu_diff(), S()));
+}
+void SigmoidLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2C_CHECK(b2c_sigmoid_forward(b[0]->count(), b[0]->gpu_data(), t[0]->mutable_gpu_data(), S()));
+}
+void SigmoidLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0]) return;
+  B2C_CHECK(b2c_sigmoid_backward(t[0]->count(), t[0]->gpu_data(), t[0]->gpu_diff(), b[0]->mutable_gpu_diff(), S()));
+}
+void FlattenLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2_CHECK(t[0] != b[0], "Flatten Layer does not allow in-place computation.");
+  t[0]->Reshape(shape_);
+  B2_CHECK(t[0]->count() == b[0]->count(), "Flatten: top and bottom counts differ");
+}
+void FlattenLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) { t[0]->ShareData(*b[0]); }
+void FlattenLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0]) return;
+  CUDA_CHECK(cudaMemcpyAsync(b[0]->mutable_gpu_diff(), t[0]->gpu_diff(), sizeof(float) * t[0]->count(), cudaMemcpyDeviceToDevice, S()));
+}
+
+// ================================================================================================ EuclideanLoss / SigmoidCrossEntropyLoss
+void EuclideanLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2C_CHECK(b2c_euclidean_loss_forward(b[0]->shape(0), b[0]->count(), b[0]->gpu_data(), b[1]->gpu_data(), diff_.mutable_gpu_data(),
+                                       t[0]->mutable_gpu_data(), S()));
+}
+void EuclideanLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
+  for (int i = 0; i < 2; ++i) {                    // euclidean_loss_layer.cu:24-35: alpha = sign * loss_weight / num
+    if (!pd[i]) continue;
+    const float alpha = (i == 0 ? 1.f : -1.f) * loss_weight_ / (float)b[i]->shape(0);
+    B2C_CHECK(b2c_euclidean_loss_backward(b[i]->count(), diff_.gpu_data(), alpha, b[i]->mutable_gpu_diff(), S()));
+  }
+}
+void SigmoidCrossEntropyLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2C_CHECK(b2c_sigmoid_ce_loss_forward(b[0]->shape(0), b[0]->count(), b[0]->gpu_data(), b[1]->gpu_data(), t[0]->mutable_gpu_data(), S()));
+}
+void SigmoidCrossEntropyLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
+  B2_CHECK(!pd[1], "SigmoidCrossEntropyLoss Layer cannot backpropagate to label inputs.");
+  if (!pd[0]) return;
+  const float scale = loss_weight_ / (float)b[0]->shape(0);     // caffe_scal(count, loss_weight / num, bottom_diff)
+  B2C_CHECK(b2c_sigmoid_ce_loss_backward(b[0]->count(), b[0]->gpu_data(), b[1]->gpu_data(), scale, b[0]->mutable_gpu_diff(), S()));
+}
+
 // ================================================================================================ Accuracy
 void AccuracyLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   B2C_CHECK(b2c_accuracy(b[0]->shape(0), (int)b[0]->count(1), top_k_, b[0]->gpu_data(), b[1]->gpu_data(), t[0]->mutable_gpu_data(),
@@ -404,7 +459,6 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
   name_ = net.name();
   test_ = net.phase() == TEST;
   Caffe::set_random_seed(seed);
-  std::map<string, bool> need;
   vector<ParamSpec> specs;
   for (size_t li = 0; li < net.layers().size(); ++li) {
     const NetLayer& L = net.layers()[li];
@@ -460,6 +514,19 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       layer.reset(sl);
     }
     else if (type == "Accuracy") layer.reset(new AccuracyLayer(L.param, L.accuracy_top_k));     // forward only, no gradient
+    else if (type == "Softmax") layer.reset(new SoftmaxLayer(L.param, L.softmax_axis));
+    else if (type == "Sigmoid") layer.reset(new SigmoidLayer(L.param));
+    else if (type == "Flatten") layer.reset(new FlattenLayer(L.param, net.top_shape((int)li)));
+    else if (type == "EuclideanLoss") {
+      auto* el = new EuclideanLossLayer(L.param);
+      if (!L.loss_weight.empty()) el->set_loss_weight(L.loss_weight[0]);
+      layer.reset(el);
+    }
+    else if (type == "SigmoidCrossEntropyLoss") {
+      auto* sl = new SigmoidCrossEntropyLossLayer(L.param);
+      if (!L.loss_weight.empty()) sl->set_loss_weight(L.loss_weight[0]);
+      layer.reset(sl);
+    }
     else if (type == "LRN") {
       B2_CHECK(L.lrn_region == 0, "TrainNet: LRN WITHIN_CHANNEL is not built (the BASELINE nets use ACROSS_CHANNELS)");
       layer.reset(new LRNLayer(L.param, L.lrn_size, L.lrn_alpha, L.lrn_beta, L.lrn_k));
@@ -484,18 +551,15 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       specs.push_back(ps);
       ++node.num_params;
     }
-    // need-backward analysis (net.cpp:160-283)
-    bool nb = false;
+    // need-backward (net.cpp:160-330, loss pruning included) is Net's result; a TEST net runs no backward at all.  Accuracy is
+    // forward-only (accuracy_layer.hpp: "cannot backpropagate"): its top carries no loss weight, so pruning already stops it
+    node.need_backward = L.need_backward && !test_ && type != "Accuracy";
     for (size_t i = 0; i < node.bottom.size(); ++i) {
-      const bool bneed = need.count(L.param.bottom[i]) ? need[L.param.bottom[i]] : false;
-      node.propagate_down.push_back(bneed && !(type == "SoftmaxWithLoss" && i == 1));
-      nb |= bneed;
+      node.propagate_down.push_back(node.need_backward && L.propagate_down[i]);
     }
-    for (int k = 0; k < node.num_params; ++k) nb |= specs[node.first_param + k].lr_mult != 0.f;
-    if (layer.get() == data_ || type == "Accuracy" || test_) nb = false;      // Accuracy: forward-only metric (accuracy_layer.hpp: "cannot backpropagate")
-    node.need_backward = nb;
-    for (auto& tn : L.param.top) need[tn] = nb;
-    if (type == "SoftmaxWithLoss") loss_blob_ = node.top[0];
+    // the reference refuses at backward time (sigmoid_cross_entropy_loss_layer.cpp:52-55); here the graph is known up front
+    B2_CHECK(!(type == "SigmoidCrossEntropyLoss" && node.need_backward && L.label_wants_gradient),
+             "SigmoidCrossEntropyLoss Layer cannot backpropagate to label inputs.");
     node.bottom_diff_tmp.assign(node.bottom.size(), nullptr);
     layers_.push_back(layer);
     layer_names_.push_back(L.param.name);
@@ -610,6 +674,7 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       }
     }
   }
+  if (!net.loss_blob().empty()) loss_blob_ = blobs_[net.loss_blob()].get();
   if (!test_) {
     solver_.reset(new SGDSolver(sp));
     solver_->SetParams(learnable_, specs);
@@ -624,10 +689,9 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
     std::map<string, float> weight;
     for (const NetLayer& L : net.layers()) {
       for (auto& bn : L.param.bottom) available.erase(bn);
-      const bool loss = L.param.type.size() >= 4 && L.param.type.compare(L.param.type.size() - 4, 4, "Loss") == 0;
       for (size_t t = 0; t < L.param.top.size(); ++t) {
         available.insert(L.param.top[t]);
-        weight[L.param.top[t]] = t < L.loss_weight.size() ? L.loss_weight[t] : (loss && t == 0 ? 1.f : 0.f);
+        weight[L.param.top[t]] = TopLossWeight(L, t);
       }
     }
     for (const string& n : available) outputs_.push_back({n, blobs_[n].get(), weight[n]});

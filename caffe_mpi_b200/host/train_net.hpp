@@ -176,6 +176,69 @@ class SoftmaxWithLossLayer : public LayerBase {
   float loss_weight_ = 1.f;
 };
 
+// ---- layers the deploy / TEST nets and the MNIST autoencoder add (softmax_layer, sigmoid_layer, flatten_layer, euclidean_loss_layer,
+// sigmoid_cross_entropy_loss_layer .cpp) ----
+class SoftmaxLayer : public LayerBase {        // over softmax_param.axis: an [outer, C, inner] view of the bottom
+ public:
+  SoftmaxLayer(const LayerParameter& p, int axis) : LayerBase(p), axis_(axis) {}
+  const char* type() const override { return "Softmax"; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]); }
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  int axis_;
+};
+
+class SigmoidLayer : public LayerBase {
+ public:
+  using LayerBase::LayerBase;
+  const char* type() const override { return "Sigmoid"; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]); }
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+};
+
+// Launches nothing.  Forward: the top aliases the bottom's data (Blob::ShareData), re-pointed every call in case the bottom's
+// memory moved.  Backward: ONE device-to-device copy of the top's diff into the bottom's diff, not an alias: the bottom handed
+// to Backward may be a fan-out shadow blob with a private diff, and the arena may re-point diffs (set_gpu_diff) after set-up,
+// so a diff alias fixed at set-up could write a gradient nobody reads.
+class FlattenLayer : public LayerBase {
+ public:
+  FlattenLayer(const LayerParameter& p, const vector<int>& top_shape) : LayerBase(p), shape_(top_shape) {}
+  const char* type() const override { return "Flatten"; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  vector<int> shape_;
+};
+
+class EuclideanLossLayer : public LayerBase {  // loss = sum (a - b)^2 / N / 2; gradient to each propagating bottom with its sign
+ public:
+  using LayerBase::LayerBase;
+  void set_loss_weight(float w) { loss_weight_ = w; }
+  const char* type() const override { return "EuclideanLoss"; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { diff_.ReshapeLike(*b[0]); t[0]->Reshape({1}); }
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  Blob diff_;
+  float loss_weight_ = 1.f;
+};
+
+class SigmoidCrossEntropyLossLayer : public LayerBase {   // no sigmoid tensor: backward recomputes sigmoid(x)
+ public:
+  using LayerBase::LayerBase;
+  void set_loss_weight(float w) { loss_weight_ = w; }
+  const char* type() const override { return "SigmoidCrossEntropyLoss"; }
+  void Reshape(const vector<Blob*>&, const vector<Blob*>& t) override { t[0]->Reshape({1}); }
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  float loss_weight_ = 1.f;
+};
+
 class AccuracyLayer : public LayerBase {       // forward only (accuracy_layer.cpp); top[0] is a scalar
  public:
   AccuracyLayer(const LayerParameter& p, int top_k) : LayerBase(p), top_k_(top_k) {}

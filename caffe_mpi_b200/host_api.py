@@ -239,6 +239,26 @@ class Net:
     def reduce_buckets(self):
         return lib().b2h_net_reduce_buckets(self._h)
 
+    def backward_plan(self):
+        """Per layer (loss pruning included): (runs backward, [gradient to bottom b for each bottom])."""
+        L = lib()
+        L.b2h_net_layer_backward.restype = C.c_longlong
+        L.b2h_net_layer_backward.argtypes = [C.c_void_p, C.c_int]
+        L.b2h_net_layer_bottoms.argtypes = [C.c_void_p, C.c_int]
+        out = []
+        for i in range(L.b2h_net_num_layers(self._h)):
+            v = L.b2h_net_layer_backward(self._h, i)
+            out.append((bool(v & 1), [bool(v >> (1 + b) & 1) for b in range(L.b2h_net_layer_bottoms(self._h, i))]))
+        return out
+
+    def loss_blob(self):
+        """The blob a trainer of this net reports as its loss ('' when there is none)."""
+        L = lib()
+        L.b2h_net_loss_blob.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
+        buf = C.create_string_buffer(256)
+        L.b2h_net_loss_blob(self._h, buf, 256)
+        return buf.value.decode()
+
     def uses_database(self, layer_index=0):
         """True when that Data layer's data_param.source opened and the layer will read it (else: synthetic source)."""
         L = lib()

@@ -250,6 +250,27 @@ int b2c_add(size_t n, const float* a, const float* b, float* y, void* stream);
  * forward writes prob [N,C] and *loss (device scalar); backward writes dx = (prob - onehot) * loss_weight / N.       */
 int b2c_softmax_loss_forward(int N, int C, const float* logits, const float* labels, float* prob, float* loss, void* stream);
 int b2c_softmax_loss_backward(int N, int C, const float* prob, const float* labels, float loss_weight, float* dx, void* stream);
+/* SoftmaxLayer (src/caffe/layers/softmax_layer.cpp / .cu): softmax over the C axis of an [outer, C, inner] view.  inner == 1
+ * runs b2c_softmax_loss_forward's row kernel, so y is bit-identical to its prob.  Backward: dx = (dy - sum_c dy * y) * y.  Both
+ * may run in place (y == x; dx == dy).  Alignment as b2c_relu_forward (the float4 path takes four columns when inner % 4 == 0). */
+int b2c_softmax_forward(int outer, int C, int inner, const float* x, float* y, void* stream);
+int b2c_softmax_backward(int outer, int C, int inner, const float* y, const float* dy, float* dx, void* stream);
+/* SigmoidLayer (src/caffe/layers/sigmoid_layer.cu:9-13): y = 1 / (1 + exp(-x)); backward dx = dy * y * (1 - y).  Both may
+ * run in place.  Alignment as b2c_relu_forward.                                                                                */
+int b2c_sigmoid_forward(size_t n, const float* x, float* y, void* stream);
+int b2c_sigmoid_backward(size_t n, const float* y, const float* dy, float* dx, void* stream);
+/* SigmoidCrossEntropyLossLayer (src/caffe/layers/sigmoid_cross_entropy_loss_layer.cpp): *loss (device scalar) =
+ * -sum_i [x (t - [x >= 0]) - log(1 + exp(x - 2 x [x >= 0]))] / N, one launch, the same bits on every call (fixed reduction
+ * order for a given count and alignment); no sigmoid tensor is stored.  Backward: dx = (sigmoid(x) - t) * scale with
+ * scale = loss_weight / N, where sigmoid(x) is THE SAME EXPRESSION as b2c_sigmoid_forward's: dx equals
+ * (b2c_sigmoid_forward(x) - t) * scale bit for bit.  dx may be x.                                                              */
+int b2c_sigmoid_ce_loss_forward(int N, size_t count, const float* x, const float* target, float* loss, void* stream);
+int b2c_sigmoid_ce_loss_backward(size_t count, const float* x, const float* target, float scale, float* dx, void* stream);
+/* EuclideanLossLayer (src/caffe/layers/euclidean_loss_layer.cu): diff = a - b (kept for backward), *loss = sum diff^2 / N / 2
+ * (device scalar, same reduction as b2c_sigmoid_ce_loss_forward).  Backward, once per bottom that propagates: dx = alpha * diff
+ * with alpha = +-loss_weight / N.  dx may be diff.                                                                             */
+int b2c_euclidean_loss_forward(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream);
+int b2c_euclidean_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream);
 /* y[n][o][p] += bias[o];  db[o] += sum_{n,p} dy[n][o][p]  (InnerProduct bias with P = 1; conv bias with P = Ho*Wo). */
 int b2c_bias_forward(int N, int O, int P, const float* bias, float* y, void* stream);
 int b2c_bias_backward(int N, int O, int P, const float* dy, float* db, void* stream);
