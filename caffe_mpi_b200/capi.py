@@ -106,6 +106,8 @@ def lib():
         "b2c_conv_forward": (i, [vp, vp, vp, vp, vp, vp, sz, vp]),
         "b2c_conv_backward_data": (i, [vp, vp, vp, vp, vp, sz, vp]),
         "b2c_conv_backward_filter": (i, [vp, vp, vp, vp, vp, sz, vp]),
+        "b2c_conv_wgrad_split_bytes": (sz, [vp]),
+        "b2c_conv_backward_filter_split": (i, [vp, vp, vp, vp, vp, sz, vp, sz, vp]),
         "b2c_conv_backward_bias": (i, [vp, vp, vp, vp]),
         "b2c_im2col": (i, [vp] + [i] * 11 + [vp, vp]),
         "b2c_col2im": (i, [vp] + [i] * 11 + [vp, vp]),
@@ -210,9 +212,10 @@ class ConvDesc:
 
     def wgrad_plan(self):
         """b2c_debug_wgrad_plan: the weight-gradient route for 16-byte aligned operands and its split-K plan."""
-        out = (C.c_int * 6)()
-        check(lib().b2c_debug_wgrad_plan(self._h, out, 6))
-        return dict(route=WGRAD_ROUTES[out[0]], splits=out[1], per=out[2], nkb=out[3], cols=out[4], bpi=out[5])
+        out = (C.c_int * 7)()
+        check(lib().b2c_debug_wgrad_plan(self._h, out, 7))
+        return dict(route=WGRAD_ROUTES[out[0]], splits=out[1], per=out[2], nkb=out[3], cols=out[4], bpi=out[5],
+                    presplit_dy=bool(out[6]))
 
     def conv_plan(self, op):
         """b2c_debug_conv_plan: the forward (op 0) or data-gradient (op 1) route for 16-byte aligned activations and its tile
@@ -253,6 +256,20 @@ class ConvDesc:
     def backward_filter(self, x, dy, dw, stream=None):
         ws, n = self._workspace(OP_BACKWARD_FILTER, x)
         check(lib().b2c_conv_backward_filter(self._h, _p(x), _p(dy), _p(dw), ws, n, _stream(stream)))
+        return dw
+
+    def wgrad_split_bytes(self):
+        return int(lib().b2c_conv_wgrad_split_bytes(self._h))
+
+    def backward_filter_split(self, x, dy, dw, stream=None):
+        """backward_filter with the split buffer of b2c_conv_wgrad_split_bytes (dY converted to bf16 hi / lo once per call)."""
+        import torch
+        ws, n = self._workspace(OP_BACKWARD_FILTER, x)
+        need = self.wgrad_split_bytes()
+        if need and (getattr(self, "_split", None) is None or self._split.numel() < need):
+            self._split = torch.empty(need, dtype=torch.uint8, device=x.device)
+        sp = C.c_void_p(self._split.data_ptr()) if need else None
+        check(lib().b2c_conv_backward_filter_split(self._h, _p(x), _p(dy), _p(dw), ws, n, sp, need, _stream(stream)))
         return dw
 
     def backward_bias(self, dy, db, stream=None):

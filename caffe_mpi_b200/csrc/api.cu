@@ -320,8 +320,16 @@ extern "C" int b2c_conv_backward_data_accumulate(const b2c_conv_desc* d, const f
                             as_stream(stream));
 }
 
-extern "C" int b2c_conv_backward_filter(const b2c_conv_desc* d, const float* x, const float* dy, float* dw, void* ws,
-                                        size_t ws_bytes, void* stream) {
+extern "C" size_t b2c_conv_wgrad_split_bytes(const b2c_conv_desc* d) {
+  if (!d) return 0;
+  const int route = wgrad_route(d, true, true, true);
+  WgradPlanInfo q;
+  tc_wgrad_plan_info(d->s, route, &q);
+  return q.split_bytes;
+}
+
+extern "C" int b2c_conv_backward_filter_split(const b2c_conv_desc* d, const float* x, const float* dy, float* dw, void* ws,
+                                              size_t ws_bytes, void* split, size_t split_bytes, void* stream) {
   if (!d || !x || !dy || !dw) return fail(B2C_ERR_INVALID, "b2c_conv_backward_filter: null pointer");
   REQUIRE_DEVICE();
   const ConvShape& s = d->s;
@@ -347,11 +355,16 @@ extern "C" int b2c_conv_backward_filter(const b2c_conv_desc* d, const float* x, 
     return B2C_OK;
   }
   if (route >= B2C_WGRAD_ROUTE_STAGED_3X3 && route <= B2C_WGRAD_ROUTE_STAGED_1X1_PLANE)
-    return launch_conv_tc_wgrad_stg(s, x, dy, dw, ws, ws_bytes, st);
+    return launch_conv_tc_wgrad_stg(s, x, dy, dw, ws, ws_bytes, st, split, split_bytes);
   if (route != B2C_WGRAD_ROUTE_SIMT)   // the gather kernel or the TMA-fed 1x1 kernel, with or without compaction (conv_tc_wgrad.cu)
     return launch_conv_tc(s, B2C_OP_BACKWARD_FILTER, gather_math(d), x, dy, nullptr, dw, ws, ws_bytes, nullptr, st);
   note_simt_fallback(d, B2C_OP_BACKWARD_FILTER);
   return launch_conv_wgrad_simt(s, x, dy, dw, st);
+}
+
+extern "C" int b2c_conv_backward_filter(const b2c_conv_desc* d, const float* x, const float* dy, float* dw, void* ws,
+                                        size_t ws_bytes, void* stream) {
+  return b2c_conv_backward_filter_split(d, x, dy, dw, ws, ws_bytes, nullptr, 0, stream);
 }
 
 extern "C" int b2c_debug_wgrad_plan(const b2c_conv_desc* d, int* out, int n) {
@@ -360,6 +373,7 @@ extern "C" int b2c_debug_wgrad_plan(const b2c_conv_desc* d, int* out, int n) {
   WgradPlanInfo q;
   tc_wgrad_plan_info(d->s, route, &q);
   out[0] = route; out[1] = q.splits; out[2] = q.kb_per_split; out[3] = (int)q.nkb; out[4] = q.cols; out[5] = q.bpi;
+  if (n >= 7) out[6] = q.presplit;
   return B2C_OK;
 }
 

@@ -58,6 +58,8 @@ struct WgradPlanInfo {
   long long nkb;
   int cols, bpi, taps;
   bool plane;
+  int presplit;          // staged kernel: 1 where dY is split to bf16 hi / lo before the launch
+  size_t split_bytes;    // the buffer that split needs (b2c_conv_wgrad_split_bytes)
 };
 
 // A forward / data-gradient kernel's tile plan as b2c_debug_conv_plan reports it: 128 x n_tile output tiles, m_tiles x n_tiles
@@ -114,7 +116,10 @@ void tc_wgrad_plan_info(const ConvShape&, int route, WgradPlanInfo*);
 // TMA-staged bf16x3 weight gradient (conv_tc_wgrad_stg.cu): stride-1 "same" convolutions with 1 or 9 taps
 bool tc_wgrad_stg_supported(const ConvShape&);
 size_t tc_wgrad_stg_workspace(const ConvShape&);
-int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t);
+// split: the buffer for dY's bf16 hi / lo planes where the plan pre-splits it (WgradPlanInfo::split_bytes), or null to convert
+// both operands in the kernel
+int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t,
+                             void* split = nullptr, size_t split_bytes = 0);
 bool tc_wgrad_stg_plan_info(const ConvShape&, WgradPlanInfo*);
 bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K);
 size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K);

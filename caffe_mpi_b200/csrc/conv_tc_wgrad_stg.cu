@@ -39,7 +39,7 @@ constexpr int KPX = 64;                       // pixels per K block
 constexpr uint32_t DY_BYTES = 2u * 128u * 128u;   // two [128 rows][32 px] fp32 boxes
 
 struct Params {
-  int HW, H, W, C, O;
+  int N, HW, H, W, C, O;
   int halo;                // pad*W + pad
   int bwx;                 // staged pixels per X channel row (multiple of 4)
   int bpi;                 // K blocks per image = ceil(HW / 64)
@@ -51,27 +51,36 @@ struct Params {
   unsigned int* counters;
 };
 
-template <int T, int CN>
+// A_PRE: dY arrives already split into bf16 hi / lo planes (wstg_split_kernel) and TMA lands it straight in the A tiles as
+// K-major SWIZZLE_128B boxes: no raw dY ring and no converter work for it.  The freed space goes to a deeper A / B ring.
+template <int T, int CN, bool A_PRE>
 struct Cfg {
   static constexpr int NROWS = T * CN;                                  // B rows = GEMM N (one wgmma)
   static constexpr uint32_t B_PLANE = (uint32_t)NROWS * 128u;           // [NROWS][64 bf16], SW128
   static constexpr uint32_t B_STAGE = 2u * B_PLANE;                     // hi + lo
-  static constexpr int BSTAGES = 2;
-  static constexpr uint32_t A_BYTES = tile_bytes(128);                  // [128 rows][64 bf16], K-major no swizzle
+  // [128 rows][64 bf16]: SW128 as TMA writes it (A_PRE), else K-major no swizzle as the converters write it
+  static constexpr uint32_t A_BYTES = A_PRE ? 128u * 128u : tile_bytes(128);
   // raw operands as TMA delivers them.  dY and X have their own rings: the converters are done with a dY stage early
   // (it is converted into the A tile first), while X is read until the end of the block and wants two stages.
   // 3x3: X pool = 2 x [CN c][184 px] (W <= 56; wider maps, up to the 256-column TMA box, run with one X stage).
   static constexpr int NDY = 1;
   static constexpr uint32_t XMAX = (uint32_t)CN * (T == 1 ? 64u : 256u) * 4u;   // raw X box upper bound (1x1: no halo; else bwx <= 256)
   static constexpr uint32_t XPOOL = T == 1 ? 2u * XMAX : 2u * (uint32_t)CN * 184u * 4u;
+  static constexpr uint32_t DYPOOL = A_PRE ? 0u : NDY * DY_BYTES;
   static_assert(XPOOL >= XMAX, "one X stage always fits");
+  static constexpr uint32_t FIXED = DYPOOL + XPOOL + 256 + 1024;
+  static constexpr uint32_t STAGE = B_STAGE + 2u * A_BYTES;
+  static constexpr uint32_t FIT = (227u * 1024u - FIXED) / STAGE;
+  static constexpr int BSTAGES = A_PRE ? (FIT < 4u ? (int)FIT : 4) : 2;
   static constexpr uint32_t B_OFF = 0;                                  // SW128 tiles: 1024-byte aligned
   static constexpr uint32_t DY_OFF = BSTAGES * B_STAGE;                 // SW128 boxes: 1024-byte aligned
-  static constexpr uint32_t A_OFF = DY_OFF + NDY * DY_BYTES;
+  static constexpr uint32_t A_OFF = DY_OFF + DYPOOL;                    // A_PRE: SW128, 1024-byte aligned
   static constexpr uint32_t X_OFF = A_OFF + BSTAGES * 2u * A_BYTES;    // 128-byte aligned
   static constexpr uint32_t BAR_OFF = X_OFF + XPOOL;
   static constexpr uint32_t TOTAL = BAR_OFF + 256 + 1024;
   static_assert(NROWS % 8 == 0 && NROWS <= 256, "wgmma N");
+  static_assert(BSTAGES >= 2 && BSTAGES <= 4, "A / B ring depth (4 barriers per ring)");
+  static_assert(B_PLANE % 1024u == 0 && A_OFF % 1024u == 0, "SW128 tiles are 1024-byte aligned");
   static_assert(X_OFF % 128u == 0, "TMA destinations are 128-byte aligned");
   static_assert(TOTAL <= 227u * 1024u, "shared memory budget");
 };
@@ -92,10 +101,10 @@ __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
 // PLANE (7x7 maps: a 196-byte channel pitch is not a TMA stride): one K block = one whole image.  The blobs are viewed as
 // {4*H*W, channels/4, N} (four channels per tensor row), so a box of 32 rows is 128 channels x H*W pixels, contiguous; dY is read
 // with 4-byte loads (odd word pitch: conflict-free), pixels H*W..63 of the 64-wide K block are written as zeros on both operands.
-template <int T, int CN, bool PLANE>
+template <int T, int CN, bool PLANE, bool A_PRE>
 __global__ void __launch_bounds__(THREADS, 1)
 wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x) {
-  using S = Cfg<T, CN>;
+  using S = Cfg<T, CN, A_PRE>;
   using MMA = WgmmaBf16<S::NROWS>;
   constexpr int NROWS = S::NROWS, NDY = S::NDY, BST = S::BSTAGES;
   constexpr uint32_t LBO_A = tile_lbo(128);
@@ -105,8 +114,8 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   const uint32_t bar_dy_empty = bar_dy_full + 16;          // 2: converters have read the dY stage
   const uint32_t bar_x_full = bar_dy_empty + 16;           // 2: X box landed
   const uint32_t bar_x_empty = bar_x_full + 16;            // 2: converters have read the X stage
-  const uint32_t bar_b_full = bar_x_empty + 16;            // BST: A and B tiles written
-  const uint32_t bar_b_empty = bar_b_full + 16;            // BST: the MMAs of the stage have completed
+  const uint32_t bar_b_full = bar_x_empty + 16;            // BST (<= 4): A and B tiles written / landed
+  const uint32_t bar_b_empty = bar_b_full + 32;            // BST: the MMAs of the stage have completed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int split = blockIdx.x;
@@ -126,7 +135,9 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       mbar_init(bar_dy_full + 8 * s, 1); mbar_init(bar_dy_empty + 8 * s, NCW);
       mbar_init(bar_x_full + 8 * s, 1); mbar_init(bar_x_empty + 8 * s, NCW);
     }
-    for (int s = 0; s < BST; ++s) { mbar_init(bar_b_full + 8 * s, NCW); mbar_init(bar_b_empty + 8 * s, NCONS); }
+    // b_full: the converter warps that write a tile, plus the TMA warp's expect_tx for the pre-split dY boxes
+    constexpr uint32_t b_arrivals = A_PRE ? NCW + 1u : NCW;
+    for (int s = 0; s < BST; ++s) { mbar_init(bar_b_full + 8 * s, b_arrivals); mbar_init(bar_b_empty + 8 * s, NCONS); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -149,10 +160,12 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
     const uint32_t lq = (uint32_t)lane >> 2, wr_off = (uint32_t)(lane & 3) * 4u;   // 16-byte chunk / byte inside it of this lane's pixel pair
     for (int i = 0; i < nkb; ++i) {
       const int rd = i % NDY, rx = i % nx, s = i % BST;
-      mbar_wait(bar_dy_full + 8 * rd, (i / NDY) & 1);
       // ---- (a) dY -> bf16 hi / lo: this thread's row (output channel), pixels [ch2*32, ch2*32 + 32)
       uint32_t hi[16], lo[16];
-      if constexpr (PLANE) {
+      if constexpr (!A_PRE) mbar_wait(bar_dy_full + 8 * rd, (i / NDY) & 1);
+      if constexpr (A_PRE) {
+        // dY arrives split: the TMA warp lands it in the A tile
+      } else if constexpr (PLANE) {
         const uint32_t rowb = raw_dy(rd) + (uint32_t)row * (uint32_t)(p.HW * 4) + (uint32_t)(ch2 * 128);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
@@ -172,14 +185,18 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
           split_pack_bf16(v.z, v.w, hi[2 * q + 1], lo[2 * q + 1]);
         }
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_dy_empty + 8 * rd);      // the dY stage reloads while the B tile is built
+      if constexpr (!A_PRE) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_dy_empty + 8 * rd);    // the dY stage reloads while the B tile is built
+      }
       mbar_wait_backoff(bar_b_empty + 8 * s, ((i / BST) & 1) ^ 1, 32);
+      if constexpr (!A_PRE) {
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {                            // 16-byte K chunk = 8 pixels
-        const uint32_t a = a_hi(s) + (uint32_t)(ch2 * 4 + q) * LBO_A + a_row;
-        sts128u(a, hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]);
-        sts128u(a + S::A_BYTES, lo[4 * q], lo[4 * q + 1], lo[4 * q + 2], lo[4 * q + 3]);
+        for (int q = 0; q < 4; ++q) {                          // 16-byte K chunk = 8 pixels
+          const uint32_t a = a_hi(s) + (uint32_t)(ch2 * 4 + q) * LBO_A + a_row;
+          sts128u(a, hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]);
+          sts128u(a + S::A_BYTES, lo[4 * q], lo[4 * q + 1], lo[4 * q + 2], lo[4 * q + 3]);
+        }
       }
       // ---- (b) X -> B tile rows (c, tap): lanes run along the pixels, two adjacent pixels per lane
       const int col0 = j * KPX - x_start(j) + 2 * lane;       // staged column of this lane's first pixel at tap offset 0
@@ -265,7 +282,7 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
     // ================= TMA producer ================================================================================
     int n_img = (int)(kb_begin / p.bpi), j = (int)(kb_begin - (long long)n_img * p.bpi);
     for (int i = 0; i < nkb; ++i) {
-      const int rd = i % NDY, rx = i % nx;
+      const int rd = i % NDY, rx = i % nx, s = i % BST;
       mbar_wait_backoff(bar_x_empty + 8 * rx, ((i / nx) & 1) ^ 1, 32);
       if (elect_one()) {
         arrive_expect_tx(bar_x_full + 8 * rx, x_bytes);
@@ -273,6 +290,17 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
         else tma_load_3d(raw_x(rx), &map_x, bar_x_full + 8 * rx, x_start(j), c0, n_img);
       }
       __syncwarp();
+      if constexpr (A_PRE) {
+        // pre-split planes {HWp, O, 2N}: hi of image n at n, lo at N + n; rows past O read as zeros
+        mbar_wait_backoff(bar_b_empty + 8 * s, ((i / BST) & 1) ^ 1, 32);
+        if (elect_one()) {
+          const uint32_t bar = bar_b_full + 8 * s;
+          arrive_expect_tx(bar, 2u * S::A_BYTES);
+          tma_load_3d(a_hi(s), &map_dy, bar, j * KPX, m0, n_img);
+          tma_load_3d(a_hi(s) + S::A_BYTES, &map_dy, bar, j * KPX, m0, p.N + n_img);
+        }
+        __syncwarp();
+      } else {
       mbar_wait_backoff(bar_dy_empty + 8 * rd, ((i / NDY) & 1) ^ 1, 32);
       if (elect_one()) {
         arrive_expect_tx(bar_dy_full + 8 * rd, dy_bytes);
@@ -284,7 +312,17 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
         }
       }
       __syncwarp();
+      }
       if (++j == p.bpi) { j = 0; ++n_img; }
+    }
+  } else if (warp >= 4 && warp < NCONS && p.O - m0 <= 64) {
+    // ================= second consumer warpgroup of a tile whose rows [m0 + 64, m0 + 128) are all past O ==========
+    // nothing to multiply (its rows are never stored): it only keeps the stage protocol, releasing each stage as it fills
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % BST;
+      mbar_wait_backoff(bar_b_full + 8 * s, (i / BST) & 1, 32);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_b_empty + 8 * s);
     }
   } else if (warp < NCONS) {
     // ================= consumers: wgmma over the CTA's K range, then the partial tile from registers ==============
@@ -308,8 +346,14 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < KPX / 16; ++kk) {
-        const uint32_t a = a_hi(s) + 2u * kk * LBO_A + (uint32_t)cwg * 1024u;
-        const uint64_t ah = smem_desc(a, LBO_A, 128), al = smem_desc(a + S::A_BYTES, LBO_A, 128);
+        uint64_t ah, al;
+        if constexpr (A_PRE) {                     // SW128 [128 rows][64 px]: this warpgroup's 64 rows start 8 KB in
+          const uint32_t a = a_hi(s) + (uint32_t)cwg * (64u * 128u) + kk * 32;
+          ah = smem_desc_sw128(a); al = smem_desc_sw128(a + S::A_BYTES);
+        } else {
+          const uint32_t a = a_hi(s) + 2u * kk * LBO_A + (uint32_t)cwg * 1024u;
+          ah = smem_desc(a, LBO_A, 128); al = smem_desc(a + S::A_BYTES, LBO_A, 128);
+        }
         const uint64_t bh = smem_desc_sw128(b_hi(s) + kk * 32), bl = smem_desc_sw128(b_lo(s) + kk * 32);
         MMA::mma(acc, al, bh, !fresh || kk != 0);  // lo * hi
         MMA::mma(acc, ah, bl, 1);                 // hi * lo
@@ -351,6 +395,29 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
   }
 }
 
+// fp32 [N][channels][HW] -> bf16 hi plane [N][channels][HWp] followed by the lo plane (same shape), pixels HW..HWp-1 zero:
+// the dY operand wgrad_stg_kernel's A_PRE variant reads.  The split is the converters' split_pack_bf16, so the MMA tiles
+// hold the same bits either way.  One thread per 8 output pixels (one 16-byte store per plane).
+__global__ void __launch_bounds__(256)
+wstg_split_kernel(const float* __restrict__ src, uint4* __restrict__ dst, long long rows, int HW, int HWp) {
+  const int per_row = HWp / 8;
+  const long long total = rows * per_row;
+  const long long plane = total;                            // 16-byte units per plane
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / per_row;
+    const int p0 = (int)(i - r * per_row) * 8;
+    const float* row = src + r * HW;
+    float v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = p0 + e < HW ? __ldg(row + p0 + e) : 0.f;
+    uint32_t hi[4], lo[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) split_pack_bf16(v[2 * q], v[2 * q + 1], hi[q], lo[q]);
+    dst[i] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    dst[plane + i] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  }
+}
+
 }  // namespace wstg
 
 
@@ -359,7 +426,14 @@ static bool wstg_enabled() {
   static const int on = env_int("B2C_WGRAD_STAGED", 1);
   return on != 0;
 }
-struct WstgPlan { int T, cn, bwx, bpi, splits, kb_per_split; long long nkb; bool plane; };
+// a_pre: dY goes through wstg_split_kernel first (only when the caller brings the split buffer)
+struct WstgPlan { int T, cn, bwx, bpi, splits, kb_per_split; long long nkb; bool plane, a_pre; };
+// dY of a 3x3 layer is split into bf16 hi / lo planes once per call, instead of once per CTA in the converter warps, when at least
+// this many input-channel tiles (8 channels each) would convert each of its K blocks.  The split pass moves 8 bytes of HBM per
+// element.  Measured on an H100 SXM (700 W), ResNet-50 at N = 64: every 3x3 layer gains (c_tiles 8 to 64; 250 -> 210 us for res2,
+// 221 -> 167 us for res4), while no 1x1 layer does in the training step: their tiles are 64 or 128 channels wide, so a block is
+// converted by at most 16 CTAs, and the split pass over their larger dY / X costs as much as it saves.  1x1 layers never pre-split.
+constexpr int PRESPLIT_MIN_TILES = 8;
 static bool wstg_plane_enabled() {
   static const int on = env_int("B2C_WGRAD_STAGED_PLANE", 1);
   return on != 0;
@@ -386,8 +460,14 @@ static bool wstg_plan(const ConvShape& s, WstgPlan* pl) {
   pl->bwx = plane ? (int)HW : (need + 3) & ~3;
   pl->bpi = (int)((HW + wstg::KPX - 1) / wstg::KPX);
   pl->nkb = (long long)s.N * pl->bpi;
-  plan_splitk(pl->nkb, (long long)((s.O + 127) / 128) * ((s.C + pl->cn - 1) / pl->cn), 4, &pl->splits, &pl->kb_per_split);
+  const int c_tiles = (s.C + pl->cn - 1) / pl->cn, o_tiles = (s.O + 127) / 128;
+  plan_splitk(pl->nkb, (long long)o_tiles * c_tiles, 4, &pl->splits, &pl->kb_per_split);
+  pl->a_pre = T == 9 && c_tiles >= PRESPLIT_MIN_TILES;
   return true;
+}
+// pre-split dY: hi and lo planes of [N][O][bpi * 64] bf16
+static size_t wstg_split_bytes(const ConvShape& s, const WstgPlan& pl) {
+  return pl.a_pre ? (size_t)4 * s.N * s.O * pl.bpi * wstg::KPX : 0;
 }
 bool tc_wgrad_stg_supported(const ConvShape& s) { return wstg_plan(s, nullptr); }
 bool tc_wgrad_stg_plan_info(const ConvShape& s, WgradPlanInfo* q) {
@@ -395,6 +475,8 @@ bool tc_wgrad_stg_plan_info(const ConvShape& s, WgradPlanInfo* q) {
   if (!wstg_plan(s, &pl)) return false;
   q->splits = pl.splits; q->kb_per_split = pl.kb_per_split; q->nkb = pl.nkb;
   q->cols = pl.cn * pl.T; q->bpi = pl.bpi; q->taps = pl.T; q->plane = pl.plane;
+  q->presplit = pl.a_pre ? 1 : 0;
+  q->split_bytes = wstg_split_bytes(s, pl);
   return true;
 }
 size_t tc_wgrad_stg_workspace(const ConvShape& s) {
@@ -403,22 +485,27 @@ size_t tc_wgrad_stg_workspace(const ConvShape& s) {
   return splitk_workspace_bytes(pl.splits, (long long)s.O * s.Kd);
 }
 
-template <int T, int CN, bool PLANE>
+template <int T, int CN, bool PLANE, bool A_PRE = false>
 static int wstg_launch(const wstg::Params& p, const CUtensorMap& mdy, const CUtensorMap& mx, int c_tiles, int o_tiles, cudaStream_t st) {
-  using S = wstg::Cfg<T, CN>;
-  B2C_CUDA_OK(cudaFuncSetAttribute(wstg::wgrad_stg_kernel<T, CN, PLANE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
+  using S = wstg::Cfg<T, CN, A_PRE>;
+  B2C_CUDA_OK(cudaFuncSetAttribute(wstg::wgrad_stg_kernel<T, CN, PLANE, A_PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
   dim3 grid(p.splits, c_tiles, o_tiles);
-  wstg::wgrad_stg_kernel<T, CN, PLANE><<<grid, wstg::THREADS, S::TOTAL, st>>>(p, mdy, mx);
+  wstg::wgrad_stg_kernel<T, CN, PLANE, A_PRE><<<grid, wstg::THREADS, S::TOTAL, st>>>(p, mdy, mx);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
-
 static int launch_wstg_planned(const ConvShape& s, const WstgPlan& pl, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes,
-                               cudaStream_t st);
-int launch_conv_tc_wgrad_stg(const ConvShape& s, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t st) {
+                               void* split, cudaStream_t st);
+int launch_conv_tc_wgrad_stg(const ConvShape& s, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t st,
+                             void* split, size_t split_bytes) {
   WstgPlan pl;
   if (!wstg_plan(s, &pl)) return fail(B2C_ERR_INVALID, "staged wgrad: shape not eligible");
-  return launch_wstg_planned(s, pl, x, dy, dw, ws, ws_bytes, st);
+  if (!split) {
+    pl.a_pre = false;
+  } else if (split_bytes < wstg_split_bytes(s, pl) || (reinterpret_cast<uintptr_t>(split) & 15u)) {
+    return fail(B2C_ERR_WORKSPACE, "staged wgrad: split buffer too small or not 16-byte aligned");
+  }
+  return launch_wstg_planned(s, pl, x, dy, dw, ws, ws_bytes, split, st);
 }
 
 // ---- caffe_gpu_gemm, NoTrans x Trans (math_functions.cu:11-26 as InnerProductLayer::Forward_gpu calls it): C[M][N] (+)= A[M][K] * B[N][K]^T.
@@ -430,7 +517,7 @@ bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K) {
 }
 // split count of the K loop when the caller brings a workspace (b2c_sgemm_ex): one wave of CTAs, >= 4 K blocks per split
 static void gemm_tc_plan(int M, int N, int K, WstgPlan* pl) {
-  pl->T = 1; pl->plane = false; pl->cn = N > 64 ? 128 : 64; pl->bwx = wstg::KPX; pl->bpi = (K + wstg::KPX - 1) / wstg::KPX; pl->nkb = pl->bpi;
+  pl->T = 1; pl->plane = false; pl->a_pre = false; pl->cn = N > 64 ? 128 : 64; pl->bwx = wstg::KPX; pl->bpi = (K + wstg::KPX - 1) / wstg::KPX; pl->nkb = pl->bpi;
   plan_splitk(pl->nkb, (long long)((M + 127) / 128) * ((N + pl->cn - 1) / pl->cn), 4, &pl->splits, &pl->kb_per_split);
 }
 size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K) {
@@ -452,40 +539,62 @@ int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const fl
   WstgPlan pl;
   gemm_tc_plan(M, N, K, &pl);
   if (!ws || ws_bytes < splitk_workspace_bytes(pl.splits, (long long)M * N) || (reinterpret_cast<uintptr_t>(ws) & 15u)) { pl.splits = 1; pl.kb_per_split = pl.bpi; ws = nullptr; ws_bytes = 0; }   // no workspace: one CTA per tile walks all of K
-  return launch_wstg_planned(s, pl, B, A, Cm, ws, ws_bytes, st);
+  return launch_wstg_planned(s, pl, B, A, Cm, ws, ws_bytes, nullptr, st);
+}
+
+static int launch_wstg_split(const float* src, void* dst, long long rows, int HW, int HWp, cudaStream_t st) {
+  wstg::wstg_split_kernel<<<grid_for((size_t)rows * (HWp / 8), 256), 256, 0, st>>>(src, static_cast<uint4*>(dst), rows, HW, HWp);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
 }
 
 static int launch_wstg_planned(const ConvShape& s, const WstgPlan& pl, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes,
-                               cudaStream_t st) {
+                               void* split, cudaStream_t st) {
   wstg::Params p;
-  p.HW = s.H * s.W; p.H = s.H; p.W = s.W; p.C = s.C; p.O = s.O;
+  p.N = s.N; p.HW = s.H * s.W; p.H = s.H; p.W = s.W; p.C = s.C; p.O = s.O;
   p.halo = s.ph * s.W + s.pw; p.bwx = pl.bwx; p.bpi = pl.bpi; p.nkb_total = pl.nkb;
   p.kb_per_split = pl.kb_per_split; p.splits = pl.splits; p.Kd = s.Kd;
   if (int rc = bind_splitk(p, pl.splits, (long long)s.O * s.Kd, dw, ws, ws_bytes, st, "staged wgrad")) return rc;
   alignas(64) CUtensorMap mdy, mx;
   const cuuint64_t HW = (cuuint64_t)p.HW;
   const int c_tiles = (s.C + pl.cn - 1) / pl.cn, o_tiles = (s.O + 127) / 128;
-  if (pl.plane) {
+  if (pl.a_pre) {
+    // pre-split dY: {HWp, O, 2N} bf16 (hi planes of the N images, then their lo planes), [128 o][64 px] SW128 boxes
+    const int HWp = pl.bpi * wstg::KPX;
+    if (int rc = launch_wstg_split(dy, split, (long long)s.N * s.O, p.HW, HWp, st)) return rc;
+    const cuuint64_t pitch = (cuuint64_t)HWp * 2;
+    if (int rc = make_tensor_map_3d(&mdy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, split, {(cuuint64_t)HWp, (cuuint64_t)s.O, 2 * (cuuint64_t)s.N},
+                                    {pitch, pitch * (cuuint64_t)s.O}, {(cuuint32_t)wstg::KPX, 128, 1}, CU_TENSOR_MAP_SWIZZLE_128B,
+                                    "staged wgrad (pre-split dY)"))
+      return rc;
+  } else if (pl.plane) {
     // {4*HW, channels/4, N}: four channels per tensor row (a 16-byte-multiple pitch); box rows = tile channels / 4
     if (int rc = make_tensor_map_3d(&mdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dy, {HW * 4, (cuuint64_t)s.O / 4, (cuuint64_t)s.N},
                                     {HW * 16, HW * 16 * (cuuint64_t)(s.O / 4)}, {(cuuint32_t)HW * 4, 32, 1}, CU_TENSOR_MAP_SWIZZLE_NONE, "staged wgrad"))
       return rc;
+  } else {
+    // [N][channels][HW] fp32: dY in [128 o][32 px] SWIZZLE_128B boxes
+    if (int rc = make_tensor_map_3d(&mdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dy, {HW, (cuuint64_t)s.O, (cuuint64_t)s.N}, {HW * 4, HW * 4 * (cuuint64_t)s.O},
+                                    {32, 128, 1}, CU_TENSOR_MAP_SWIZZLE_128B, "staged wgrad"))
+      return rc;
+  }
+  if (pl.plane) {
     if (int rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, x, {HW * 4, (cuuint64_t)s.C / 4, (cuuint64_t)s.N},
                                     {HW * 16, HW * 16 * (cuuint64_t)(s.C / 4)}, {(cuuint32_t)HW * 4, (cuuint32_t)pl.cn / 4, 1},
                                     CU_TENSOR_MAP_SWIZZLE_NONE, "staged wgrad"))
       return rc;
-    if (pl.T == 9) return wstg_launch<9, 8, true>(p, mdy, mx, c_tiles, o_tiles, st);
+  } else {
+    // X in [CN c][bwx px] boxes
+    if (int rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, x, {HW, (cuuint64_t)s.C, (cuuint64_t)s.N}, {HW * 4, HW * 4 * (cuuint64_t)s.C},
+                                    {(cuuint32_t)pl.bwx, (cuuint32_t)pl.cn, 1}, CU_TENSOR_MAP_SWIZZLE_NONE, "staged wgrad"))
+      return rc;
+  }
+  if (pl.plane) {
+    if (pl.T == 9) return pl.a_pre ? wstg_launch<9, 8, true, true>(p, mdy, mx, c_tiles, o_tiles, st) : wstg_launch<9, 8, true>(p, mdy, mx, c_tiles, o_tiles, st);
     if (pl.cn == 128) return wstg_launch<1, 128, true>(p, mdy, mx, c_tiles, o_tiles, st);
     return wstg_launch<1, 64, true>(p, mdy, mx, c_tiles, o_tiles, st);
   }
-  // [N][channels][HW] fp32: dY in [128 o][32 px] SWIZZLE_128B boxes, X in [CN c][bwx px] boxes
-  if (int rc = make_tensor_map_3d(&mdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dy, {HW, (cuuint64_t)s.O, (cuuint64_t)s.N}, {HW * 4, HW * 4 * (cuuint64_t)s.O},
-                                  {32, 128, 1}, CU_TENSOR_MAP_SWIZZLE_128B, "staged wgrad"))
-    return rc;
-  if (int rc = make_tensor_map_3d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, x, {HW, (cuuint64_t)s.C, (cuuint64_t)s.N}, {HW * 4, HW * 4 * (cuuint64_t)s.C},
-                                  {(cuuint32_t)pl.bwx, (cuuint32_t)pl.cn, 1}, CU_TENSOR_MAP_SWIZZLE_NONE, "staged wgrad"))
-    return rc;
-  if (pl.T == 9) return wstg_launch<9, 8, false>(p, mdy, mx, c_tiles, o_tiles, st);
+  if (pl.T == 9) return pl.a_pre ? wstg_launch<9, 8, false, true>(p, mdy, mx, c_tiles, o_tiles, st) : wstg_launch<9, 8, false>(p, mdy, mx, c_tiles, o_tiles, st);
   if (pl.cn == 128) return wstg_launch<1, 128, false>(p, mdy, mx, c_tiles, o_tiles, st);
   return wstg_launch<1, 64, false>(p, mdy, mx, c_tiles, o_tiles, st);
 }

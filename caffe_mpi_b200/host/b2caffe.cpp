@@ -401,10 +401,16 @@ void ConvolutionLayer::Backward_gpu(const vector<Blob*>& top, const vector<bool>
       if (bias_term_ && param_propagate_down_[1]) B2C_CHECK(b2c_conv_backward_bias(desc_, dy, blobs_[1]->mutable_gpu_diff(), st));
       EventProfiler* prof = Caffe::profiler();
       if (param_propagate_down_[0]) {
-        const size_t need = b2c_conv_workspace_bytes(desc_, B2C_OP_BACKWARD_FILTER);
-        void* ws = need ? workspace(need) : nullptr;
+        // [the kernel's workspace | the buffer its operands are split into], both 256-byte aligned
+        const size_t need = (b2c_conv_workspace_bytes(desc_, B2C_OP_BACKWARD_FILTER) + 255) & ~(size_t)255;
+        // (only the tensor-core weight-gradient kernels take a split buffer)
+        const size_t split = algo_used(B2C_OP_BACKWARD_FILTER) == B2C_ALGO_TCGEN05 ? b2c_conv_wgrad_split_bytes(desc_) : 0;
+        char* ws = need + split ? static_cast<char*>(workspace(need + split)) : nullptr;
         const size_t h = prof ? prof->begin(EventProfiler::WGRAD, st) : 0;
-        B2C_CHECK(b2c_conv_backward_filter(desc_, bottom[i]->gpu_data(), dy, blobs_[0]->mutable_gpu_diff(), ws, ws_bytes_, st));
+        if (split)
+          B2C_CHECK(b2c_conv_backward_filter_split(desc_, bottom[i]->gpu_data(), dy, blobs_[0]->mutable_gpu_diff(), ws, need, ws + need, split, st));
+        else
+          B2C_CHECK(b2c_conv_backward_filter(desc_, bottom[i]->gpu_data(), dy, blobs_[0]->mutable_gpu_diff(), ws, need, st));
         if (prof) prof->end(h, st);
       }
       if (propagate_down[i]) {

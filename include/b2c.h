@@ -134,6 +134,13 @@ int b2c_conv_backward_data_accumulate(const b2c_conv_desc* d, const float* dy, c
                                       void* ws, size_t ws_bytes, void* stream);
 int b2c_conv_backward_filter(const b2c_conv_desc* d, const float* x, const float* dy, float* dw,
                              void* ws, size_t ws_bytes, void* stream);
+/* The same dW += ..., with a second scratch buffer of b2c_conv_wgrad_split_bytes(d) bytes (16-byte aligned, disjoint from ws):
+ * on the 3x3 layers where many thread blocks of the TMA-staged kernel would each convert the same dY block to bf16 hi / lo, one
+ * pass converts dY once into `split` before the kernel runs.  Same bits as b2c_conv_backward_filter.  split == NULL (and every
+ * layer whose size query is 0) runs exactly b2c_conv_backward_filter. */
+size_t b2c_conv_wgrad_split_bytes(const b2c_conv_desc* d);
+int b2c_conv_backward_filter_split(const b2c_conv_desc* d, const float* x, const float* dy, float* dw,
+                                   void* ws, size_t ws_bytes, void* split, size_t split_bytes, void* stream);
 /* db[o] += sum_{n,h,w} dY.  db ACCUMULATED (beta = 1).
  * Replaces backward_gpu_bias (base_conv_layer.hpp:164-168, gemv per image) /
  * cudnnConvolutionBackwardBias beta=1 (cudnn_conv_layer.cu:73-75).                   */
@@ -371,6 +378,7 @@ typedef enum {
  * and its split-K plan: out[0] route (b2c_wgrad_route), [1] splits, [2] K blocks per split, [3] K blocks in total,
  * [4] tile columns (channels x taps, or N_TILE), [5] K blocks per image (0 where the route has no per-image blocking).
  * For the compaction routes the plan is that of the dense 1x1 problem; the CAFFE and SIMT routes report zeros.
+ * With n >= 7, out[6] is 1 where b2c_conv_backward_filter_split splits dY before the staged kernel, else 0.
  * Needs n >= 6.  Pure host computation: splits follow the current device's SM count (132 without a device). */
 int b2c_debug_wgrad_plan(const b2c_conv_desc* d, int* out, int n);
 

@@ -1,4 +1,6 @@
-"""Per-layer timing of the conv kernels for one BASELINE model (CUDA events, warm, L2 flushed between reps)."""
+"""Per-layer timing of the conv kernels for one BASELINE model (CUDA events, warm, L2 flushed between reps).  The weight gradient
+is timed on both entry points: `wgrad` (b2c_conv_backward_filter) and `wsplit` (b2c_conv_backward_filter_split, split pass
+included); the `pre` column says whether the latter splits dY first."""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -13,8 +15,8 @@ math = capi.MATH_TF32 if (len(sys.argv) > 3 and sys.argv[3] == "tf32") else capi
 reps = 5
 only = os.environ.get("B2C_SWEEP_ONLY", "").split()      # e.g. "k1 s2": keep layers whose label contains every token
 flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")
-tot = {"fwd": 0.0, "dgrad": 0.0, "wgrad": 0.0}
-print(f"{'layer':34s} {'op':6s} {'us':>9s} {'TF/s':>7s} {'GB/s(alg)':>10s} {'hbm_us':>7s} {'mma_us':>7s}")
+tot = {"fwd": 0.0, "dgrad": 0.0, "wgrad": 0.0, "wsplit": 0.0}
+print(f"{'layer':34s} {'op':6s} {'us':>9s} {'TF/s':>7s} {'GB/s(alg)':>10s} {'hbm_us':>7s} {'mma_us':>7s} {'pre':>5s}")
 first = True
 for (cnt, C, H, O, k, s, p, G, bias) in MODELS[model]:
     label = f"C{C} H{H} O{O} k{k} s{s} g{G}"
@@ -31,6 +33,9 @@ for (cnt, C, H, O, k, s, p, G, bias) in MODELS[model]:
     if not first:
         ops.append(("dgrad", lambda: d.backward_data(dy, w, dx)))
     ops.append(("wgrad", lambda: d.backward_filter(x, dy, dw)))
+    ops.append(("wsplit", lambda: d.backward_filter_split(x, dy, dw)))
+    q = d.wgrad_plan()
+    pre = "dY" if q["presplit_dy"] else "-"
     first = False
     fl = prm.flops()
     byts = 4 * (x.numel() + w.numel() + y.numel())
@@ -45,5 +50,5 @@ for (cnt, C, H, O, k, s, p, G, bias) in MODELS[model]:
         us = sorted(ts)[len(ts) // 2]
         tot[name] += us * cnt
         mma_us = fl * (3 if math == capi.MATH_FP32 else 1) / 847.5e12 * 1e6
-        print(f"{cnt}x C{C} H{H} O{O} k{k} s{s} g{G:<12d} {name:6s} {us:9.1f} {fl/us/1e6:7.1f} {byts/us/1e3:10.0f} {byts/6578e9*1e6:7.1f} {mma_us:7.1f}", flush=True)
+        print(f"{cnt}x C{C} H{H} O{O} k{k} s{s} g{G:<12d} {name:6s} {us:9.1f} {fl/us/1e6:7.1f} {byts/us/1e3:10.0f} {byts/6578e9*1e6:7.1f} {mma_us:7.1f} {pre if name == 'wsplit' else '':>5s}", flush=True)
 print("totals (us, weighted by layer count):", {k: round(v) for k, v in tot.items()}, "sum", round(sum(tot.values())))
