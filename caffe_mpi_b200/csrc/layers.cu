@@ -601,6 +601,29 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// The reduction every loss-sum kernel ends with: each thread's double partial is summed per warp, the warp sums per CTA in warp
+// order, and the CTA sums over the cluster in rank order in rank 0 through distributed shared memory.  Returns the total in rank 0's
+// thread 0 (0 elsewhere).  Every thread of every CTA of the cluster must call it.
+__device__ __forceinline__ double loss_cluster_sum(double acc) {
+  cg::cluster_group cluster = cg::this_cluster();
+  const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
+  __shared__ double wsum[LOSS_THREADS / 32];
+  __shared__ double part;
+  acc = warp_sum_d(acc);
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < LOSS_THREADS / 32; ++w) s += wsum[w];
+    part = s;
+  }
+  cluster.sync();
+  double s = 0.0;
+  if (rank == 0 && threadIdx.x == 0)
+    for (unsigned r = 0; r < nranks; ++r) s += *cluster.map_shared_rank(&part, r);
+  cluster.sync();                                   // remote shared memory stays valid until rank 0 has read it
+  return s;
+}
 template <int MODE, bool VEC>
 __global__ void __launch_bounds__(LOSS_THREADS)
 loss_sum_kernel(size_t count, int N, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ diff, float* __restrict__ loss) {
@@ -631,24 +654,77 @@ loss_sum_kernel(size_t count, int N, const float* __restrict__ a, const float* _
     if (MODE == 1) diff[i] = d;
     acc += (double)t;
   }
-  __shared__ double wsum[LOSS_THREADS / 32];
-  __shared__ double part;
-  acc = warp_sum_d(acc);
-  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int w = 0; w < LOSS_THREADS / 32; ++w) s += wsum[w];
-    part = s;
-  }
-  cluster.sync();
+  const double s = loss_cluster_sum(acc);
   if (rank == 0 && threadIdx.x == 0) {
-    double s = 0.0;
-    for (unsigned r = 0; r < nranks; ++r) s += *cluster.map_shared_rank(&part, r);
     const float f = (float)s;
     *loss = MODE == 0 ? -f / (float)N : f / (float)N / 2.f;
   }
-  cluster.sync();                                   // remote shared memory stays valid until rank 0 has read it
+}
+// ContrastiveLoss (contrastive_loss_layer.cpp): one warp per pair, the lanes strided over the channels; the pair's squared distance
+// is summed in double (lane partials, then warp_sum_d) and stored as float, its term formed in float and summed by
+// loss_cluster_sum.  Pairs are split into contiguous CTA slices like loss_sum_kernel's units.
+template <bool LEGACY>
+__global__ void __launch_bounds__(LOSS_THREADS)
+contrastive_loss_kernel(int N, int C, const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ y, float margin,
+                        float* __restrict__ diff, float* __restrict__ dist_sq, float* __restrict__ loss) {
+  cg::cluster_group cluster = cg::this_cluster();
+  const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
+  const int len = (int)((N + nranks - 1) / nranks);
+  const int lo = min(N, (int)rank * len), hi = min(N, lo + len);
+  const int lane = threadIdx.x & 31;
+  double acc = 0.0;
+  for (int n = lo + (int)(threadIdx.x >> 5); n < hi; n += LOSS_THREADS / 32) {
+    const size_t base = (size_t)n * C;
+    double s = 0.0;
+    for (int c = lane; c < C; c += 32) {
+      const float d = a[base + c] - b[base + c];
+      diff[base + c] = d;
+      s += (double)__fmul_rn(d, d);
+    }
+    s = warp_sum_d(s);
+    if (lane == 0) {
+      const float d2 = (float)s;
+      dist_sq[n] = d2;
+      float term;
+      if ((int)y[n]) term = d2;                                    // similar pair
+      else if (LEGACY) term = fmaxf(margin - d2, 0.f);
+      else { const float m = fmaxf(margin - sqrtf(d2), 0.f); term = __fmul_rn(m, m); }
+      acc += (double)term;
+    }
+  }
+  const double s = loss_cluster_sum(acc);
+  if (rank == 0 && threadIdx.x == 0) *loss = (float)s / (float)N / 2.f;
+}
+// the per-pair factor of ContrastiveLoss's backward (contrastive_loss_layer.cpp Backward_cpu); *zero: the pair's gradient is 0
+__device__ __forceinline__ float contrastive_coef(float d2, float yv, float margin, int legacy, float alpha, bool* zero) {
+  *zero = false;
+  if ((int)yv) return alpha;
+  if (legacy) { *zero = !(margin - d2 > 0.f); return -alpha; }
+  const float dist = sqrtf(d2), mdist = margin - dist;
+  *zero = !(mdist > 0.f);
+  return -alpha * mdist / (dist + 1e-4f);
+}
+template <bool VEC>
+__global__ void __launch_bounds__(256)
+contrastive_bwd_kernel(int N, int C, const float* __restrict__ diff, const float* __restrict__ dist_sq, const float* __restrict__ y, float margin,
+                       int legacy, float alpha, float* __restrict__ da, float* __restrict__ db) {
+  const size_t units = VEC ? (size_t)N * C / 4 : (size_t)N * C, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x,
+               step = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = tid; i < units; i += step) {
+    const size_t n = (VEC ? i * 4 : i) / (size_t)C;
+    bool zero;
+    const float k = contrastive_coef(dist_sq[n], y[n], margin, legacy, alpha, &zero);
+    if (VEC) {
+      const float4 d = reinterpret_cast<const float4*>(diff)[i];
+      const float4 g = zero ? make_float4(0.f, 0.f, 0.f, 0.f) : make_float4(__fmul_rn(k, d.x), __fmul_rn(k, d.y), __fmul_rn(k, d.z), __fmul_rn(k, d.w));
+      reinterpret_cast<float4*>(da)[i] = g;
+      if (db) reinterpret_cast<float4*>(db)[i] = zero ? g : make_float4(-g.x, -g.y, -g.z, -g.w);
+    } else {
+      const float g = zero ? 0.f : __fmul_rn(k, diff[i]);
+      da[i] = g;
+      if (db) db[i] = zero ? 0.f : -g;
+    }
+  }
 }
 // CTAs per loss cluster: one per 64K float4 units (256K values), at most LOSS_CLUSTER.  A function of the count alone.
 static inline unsigned loss_cluster_size(size_t count) {
@@ -950,9 +1026,9 @@ extern "C" int b2c_sigmoid_backward(size_t n, const float* y, const float* dy, f
   NEED(y && dy && dx, "b2c_sigmoid_backward: null");
   return launch_ew<EW_SIGMOID_BWD>(n, y, dy, 0.f, dx, stream);
 }
-template <int MODE>
-static int launch_loss_sum(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream) {
-  const bool vec = al16({a, b, diff});
+// one cluster of loss_cluster_size(count) LOSS_THREADS-thread CTAs
+template <typename... KArgs, typename... Args>
+static int launch_loss_cluster(void (*kernel)(KArgs...), size_t count, void* stream, Args... args) {
   const unsigned cs = loss_cluster_size(count);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(cs, 1, 1);
@@ -962,9 +1038,14 @@ static int launch_loss_sum(int N, size_t count, const float* a, const float* b, 
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  B2C_CUDA_OK(cudaLaunchKernelEx(&cfg, vec ? loss_sum_kernel<MODE, true> : loss_sum_kernel<MODE, false>, count, N, a, b, diff, loss));
+  B2C_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, args...));
   B2C_POST_LAUNCH();
   return B2C_OK;
+}
+template <int MODE>
+static int launch_loss_sum(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream) {
+  const bool vec = al16({a, b, diff});
+  return launch_loss_cluster(vec ? loss_sum_kernel<MODE, true> : loss_sum_kernel<MODE, false>, count, stream, count, N, a, b, diff, loss);
 }
 extern "C" int b2c_sigmoid_ce_loss_forward(int N, size_t count, const float* x, const float* target, float* loss, void* stream) {
   NEED(x && target && loss && N > 0 && count > 0, "b2c_sigmoid_ce_loss_forward: bad argument");
@@ -981,6 +1062,22 @@ extern "C" int b2c_euclidean_loss_forward(int N, size_t count, const float* a, c
 extern "C" int b2c_euclidean_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream) {
   NEED(diff && dx, "b2c_euclidean_loss_backward: null");
   return launch_ew<EW_SCALE>(count, diff, nullptr, alpha, dx, stream);
+}
+extern "C" int b2c_contrastive_loss_forward(int N, int C, const float* a, const float* b, const float* y, float margin, int legacy, float* diff,
+                                            float* dist_sq, float* loss, void* stream) {
+  NEED(a && b && y && diff && dist_sq && loss && N > 0 && C > 0, "b2c_contrastive_loss_forward: bad argument");
+  return launch_loss_cluster(legacy ? contrastive_loss_kernel<true> : contrastive_loss_kernel<false>, (size_t)N * C, stream, N, C, a, b, y,
+                             margin, diff, dist_sq, loss);
+}
+extern "C" int b2c_contrastive_loss_backward(int N, int C, const float* diff, const float* dist_sq, const float* y, float margin, int legacy,
+                                             float alpha, float* da, float* db, void* stream) {
+  NEED(diff && dist_sq && y && da && N > 0 && C > 0, "b2c_contrastive_loss_backward: bad argument");
+  const size_t n = (size_t)N * C;
+  const bool vec = C % 4 == 0 && al16({diff, da, db});
+  if (vec) contrastive_bwd_kernel<true><<<grid_for(n / 4, 256), 256, 0, as_stream(stream)>>>(N, C, diff, dist_sq, y, margin, legacy, alpha, da, db);
+  else contrastive_bwd_kernel<false><<<grid_for(n, 256), 256, 0, as_stream(stream)>>>(N, C, diff, dist_sq, y, margin, legacy, alpha, da, db);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
 }
 // y[n][o] += b[o] and db[o] += sum_n dy[n][o]: InnerProduct bias (inner_product_layer.cpp), via the conv bias kernels with P = 1
 extern "C" int b2c_bias_forward(int N, int O, int P, const float* bias, float* y, void* stream) {

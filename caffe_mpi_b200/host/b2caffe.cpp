@@ -121,6 +121,11 @@ void Blob::ShareData(Blob& other) {
   if (data_.gpu && data_.own_gpu) cudaFree(data_.gpu);
   data_.gpu = other.mutable_gpu_data(); data_.own_gpu = false; data_.head = AT_GPU;
 }
+void Blob::ShareDiff(Blob& other) {
+  B2_CHECK(count_ == other.count(), "ShareDiff: count mismatch");
+  if (diff_.gpu && diff_.own_gpu) cudaFree(diff_.gpu);
+  diff_.gpu = other.mutable_gpu_diff(); diff_.own_gpu = false; diff_.head = AT_GPU;
+}
 void Blob::Update() {
   // data = data - 1*diff, expressed with the fused kernel: momentum 0, rate 1, no decay, keep diff
   B2C_CHECK(b2c_sgd_update(count_, mutable_gpu_diff(), mutable_gpu_data(), mutable_gpu_diff(), 0.f, 1.f, 0.f, 1, 1.f, 0,

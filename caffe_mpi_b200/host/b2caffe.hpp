@@ -128,6 +128,7 @@ class Blob {
   void set_gpu_data(float* p);
   void set_gpu_diff(float* p);
   void ShareData(Blob& other);        // alias other's device data without copying (Blob::ShareData, blob.hpp)
+  void ShareDiff(Blob& other);        // alias other's device diff without copying (Blob::ShareDiff)
   void Update();                      // data -= diff (blob.cpp:129-154), on the thread stream
   void set_diff(float v);
 
@@ -171,6 +172,11 @@ struct ConvolutionParameter {   // caffe.proto:718-786 (same names / defaults)
 struct ParamSpec {
   float lr_mult = 1.f, decay_mult = 1.f;
   bool statistic = false;   // set by TrainNet for blobs their layer never differentiates (BatchNorm mean / variance / correction)
+  // caffe.proto ParamSpec.name / share_mode and whether lr_mult / decay_mult were given: blobs that carry one name are one
+  // parameter (Net::AppendParam, net.cpp:576-666).  share_mode: STRICT = 0, PERMISSIVE = 1
+  string name;
+  bool has_lr_mult = false, has_decay_mult = false;
+  int share_mode = 0;
 };
 struct LayerParameter {
   string name, type;

@@ -252,6 +252,18 @@ int b2h_net_param(void* h, int i, size_t* count, float* lr_mult, float* decay_mu
   snprintf(layer, cap, "%s", p.layer.c_str());
   return 0;
 }
+// every layer's parameter blobs, sharers included (Net::params_): blob i's layer, ParamSpec.name, its owner's index in this list
+// (-1: it owns its storage) and its index in b2h_net_param's list (the owner's, for a sharer)
+int b2h_net_num_net_params(void* h) { return (int)static_cast<Net*>(h)->net_params().size(); }
+int b2h_net_net_param(void* h, int i, int* owner, int* learnable_id, char* layer, char* name, int cap) {
+  Net* n = static_cast<Net*>(h);
+  if (i < 0 || i >= (int)n->net_params().size()) return -1;
+  const LearnableParam& p = n->net_params()[i];
+  *owner = p.owner; *learnable_id = p.learnable_id;
+  snprintf(layer, cap, "%s", p.layer.c_str());
+  snprintf(name, cap, "%s", p.name.c_str());
+  return 0;
+}
 // 1 when layer i is a Data layer whose data_param.source opened (it will read the database), 0 otherwise
 int b2h_net_layer_uses_database(void* h, int i) {
   const auto& ls = static_cast<Net*>(h)->layers();
@@ -418,6 +430,19 @@ int b2h_trainer_blob(void* hv, const char* name, int diff, int set, float* buf) 
 }
 // parameter access by TRAINABLE index (conv / fc weights + biases, BatchNorm scale + bias -- the blobs the layers
 // differentiate); b2h_trainer_num_learnable counts every layer blob like Net::learnable_params() (BatchNorm: 5)
+// blob `blob` of layer `layer` (execution order): the Blob object's address and its device data / diff pointers.  Two layers that
+// share a named parameter report distinct objects over one storage (test_net.cpp TestSharedWeightsUpdate)
+int b2h_trainer_layer_blob(void* hv, int layer, int blob, unsigned long long* object, unsigned long long* data, unsigned long long* diff) {
+  B2H_TRY({
+    TrainNet& n = *static_cast<TrainerHandle*>(hv)->net;
+    B2_CHECK(layer >= 0 && layer < n.num_layers(), "layer index out of range");
+    auto& bl = n.layer(layer)->blobs();
+    B2_CHECK(blob >= 0 && blob < (int)bl.size(), "blob index out of range");
+    *object = (unsigned long long)(uintptr_t)bl[blob].get();
+    *data = (unsigned long long)(uintptr_t)bl[blob]->gpu_data();
+    *diff = (unsigned long long)(uintptr_t)bl[blob]->gpu_diff();
+  });
+}
 int b2h_trainer_num_params(void* hv) { return (int)static_cast<TrainerHandle*>(hv)->net->trainable_ids().size(); }
 int b2h_trainer_num_learnable(void* hv) { return (int)static_cast<TrainerHandle*>(hv)->net->learnable_params().size(); }
 long long b2h_trainer_param_count(void* hv, int i) {

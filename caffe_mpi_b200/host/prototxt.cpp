@@ -187,6 +187,7 @@ int canonical_axis(int axis, const std::vector<int>& s) {  // Blob::CanonicalAxi
 }  // namespace
 
 int LabelBottom(const std::string& type) {
+  if (type == "ContrastiveLoss") return 2;          // the similarity label (ContrastiveLossLayer::AllowForceBackward(2) is false)
   return type == "SoftmaxWithLoss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy" ? 1 : -1;
 }
 bool IsLossType(const std::string& ty) { return ty.size() >= 4 && ty.compare(ty.size() - 4, 4, "Loss") == 0; }
@@ -198,6 +199,12 @@ Net Net::FromFile(const std::string& path, Phase phase, int batch_override) {
   return Net(ParseTextProtoFile(path), phase, batch_override);
 }
 size_t Net::learnable_count() const { size_t c = 0; for (auto& p : params_) c += p.count; return c; }
+std::pair<int, int> Net::param_owner(int layer_id, int layer_blob) const {
+  for (const LearnableParam& p : net_params_)
+    if (p.layer_id == layer_id && p.layer_blob == layer_blob && p.owner >= 0)
+      return {net_params_[p.owner].layer_id, net_params_[p.owner].layer_blob};
+  return {-1, -1};
+}
 
 Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channels, int default_size) {
   name_ = np.str("name");
@@ -219,6 +226,9 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
     }
   }
   std::map<std::string, bool> need_bw;
+  std::map<std::string, int> param_names;               // param name -> its owner's index in net_params_ (Net::param_names_index_)
+  std::map<std::string, std::string> bn_stat_names;     // names given to BatchNorm statistics blobs -> the layer
+  std::vector<bool> has_lr, has_decay;                  // per learnable param: lr_mult / decay_mult given (Net::has_params_lr_)
   for (auto* lf : np.all("layer")) {
     if (!lf->is_msg()) continue;
     const PMessage& lp = *lf->msg;
@@ -231,7 +241,14 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
     for (auto* t : lp.all("top")) L.param.top.push_back(t->scalar);
     for (auto* ps : lp.all("param")) {
       ParamSpec s;
-      if (ps->is_msg()) { s.lr_mult = (float)ps->msg->num("lr_mult", 1.0); s.decay_mult = (float)ps->msg->num("decay_mult", 1.0); }
+      if (ps->is_msg()) {
+        const PMessage& m = *ps->msg;
+        s.lr_mult = (float)m.num("lr_mult", 1.0); s.decay_mult = (float)m.num("decay_mult", 1.0);
+        s.has_lr_mult = m.has("lr_mult"); s.has_decay_mult = m.has("decay_mult");
+        s.name = m.str("name");
+        const std::string sm = m.str("share_mode", "STRICT");
+        s.share_mode = (sm == "PERMISSIVE" || sm == "1") ? 1 : 0;
+      }
       L.param.param.push_back(s);
     }
     const std::string& type = L.param.type;
@@ -424,6 +441,76 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
         else B2_CHECK(prod(a) == prod(b), "SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.");
       }
       for (size_t i = 0; i < L.param.top.size(); ++i) tops.push_back({});
+    } else if (type == "Slice") {
+      const PMessage* sp = lp.sub("slice_param");
+      const std::vector<int> bs = bottom_shape(0);
+      const size_t ntop = L.param.top.size();
+      B2_CHECK(ntop >= 1, "Slice layer needs at least one top");
+      B2_CHECK(!(sp && sp->has("axis") && sp->has("slice_dim")), "Either axis or slice_dim should be specified; not both.");   // slice_layer.cpp:12-13
+      if (sp && sp->has("slice_dim")) {                                                                                   // :26-33
+        L.slice_axis = (int)sp->integer("slice_dim");
+        B2_CHECK(L.slice_axis >= 0, "casting slice_dim from uint32 to int32 produced negative result; slice_dim must satisfy 0 <= slice_dim < 32");
+        B2_CHECK(L.slice_axis < (int)bs.size(), "slice_dim out of range.");
+      } else {
+        L.slice_axis = canonical_axis(sp ? (int)sp->integer("axis", 1) : 1, bs);
+      }
+      const int extent = bs[L.slice_axis];
+      const std::vector<int> points = sp ? to_int(sp->ints("slice_point")) : std::vector<int>();
+      std::vector<int> slices;
+      if (!points.empty()) {                                                                                              // :40-56
+        if (points.size() != ntop - 1)
+          Fatal(__FILE__, __LINE__, "Check failed: slice_point_.size() == top.size() - 1 (" + std::to_string(points.size()) + " vs. " +
+                                        std::to_string(ntop - 1) + ") ");
+        if ((int)ntop > extent)
+          Fatal(__FILE__, __LINE__, "Check failed: top.size() <= bottom_slice_axis (" + std::to_string(ntop) + " vs. " + std::to_string(extent) + ") ");
+        int prev = 0;
+        for (int p : points) {
+          if (!(p > prev)) Fatal(__FILE__, __LINE__, "Check failed: slice_point_[i] > prev (" + std::to_string(p) + " vs. " + std::to_string(prev) + ") ");
+          slices.push_back(p - prev);
+          prev = p;
+        }
+        slices.push_back(extent - prev);
+        if (slices.back() < 0)                                                                                            // Blob::Reshape's CHECK
+          Fatal(__FILE__, __LINE__, "Check failed: shape[i] >= 0 (" + std::to_string(slices.back()) + " vs. 0) ");
+      } else {                                                                                                            // :57-64
+        if (extent % (int)ntop != 0)
+          Fatal(__FILE__, __LINE__, "Check failed: bottom_slice_axis % top.size() == 0 (" + std::to_string(extent % (int)ntop) + " vs. 0) Number of top blobs (" +
+                                        std::to_string(ntop) + ") should evenly divide input slice axis (" + std::to_string(extent) + ")");
+        slices.assign(ntop, extent / (int)ntop);
+      }
+      for (int s : slices) {
+        std::vector<int> t = bs;
+        t[L.slice_axis] = s;
+        tops.push_back(t);
+      }
+    } else if (type == "ContrastiveLoss") {
+      // contrastive_loss_layer.cpp:13-20 and LossLayer::Reshape, on the legacy num / channels / height / width view (Blob::LegacyShape:
+      // a missing axis reads as 1, so an [N, C] feature blob is [N, C, 1, 1])
+      const std::vector<int>& a = bottom_shape(0);
+      const std::vector<int>& b = bottom_shape(1);
+      const std::vector<int>& y = bottom_shape(2);
+      for (const std::vector<int>* s : {&a, &b, &y})
+        B2_CHECK(s->size() <= 4, "Cannot use legacy accessors on Blobs with > 4 axes.");
+      auto legacy = [](const std::vector<int>& s, int i) { return i < (int)s.size() ? s[i] : 1; };
+      auto check_eq = [](int u, int v, const char* what) {
+        if (u != v) Fatal(__FILE__, __LINE__, std::string("Check failed: ") + what + " (" + std::to_string(u) + " vs. " + std::to_string(v) + ") ");
+      };
+      check_eq(legacy(a, 1), legacy(b, 1), "bottom[0]->channels() == bottom[1]->channels()");
+      check_eq(legacy(a, 2), 1, "bottom[0]->height() == 1");
+      check_eq(legacy(a, 3), 1, "bottom[0]->width() == 1");
+      check_eq(legacy(b, 2), 1, "bottom[1]->height() == 1");
+      check_eq(legacy(b, 3), 1, "bottom[1]->width() == 1");
+      check_eq(legacy(y, 1), 1, "bottom[2]->channels() == 1");
+      check_eq(legacy(y, 2), 1, "bottom[2]->height() == 1");
+      check_eq(legacy(y, 3), 1, "bottom[2]->width() == 1");
+      B2_CHECK(!a.empty() && !b.empty() && a[0] == b[0], "The data and label should have the same number.");     // loss_layer.cpp:19-20
+      // not in the reference, which reads bottom[2][i] for every pair without checking: one label per pair
+      B2_CHECK(!y.empty() && y[0] == a[0], "ContrastiveLoss: the similarity blob needs one label per pair");
+      if (const PMessage* cp = lp.sub("contrastive_loss_param")) {
+        L.contrastive_margin = (float)cp->num("margin", 1.0);
+        L.contrastive_legacy = cp->boolean("legacy_version", false);
+      }
+      for (size_t i = 0; i < L.param.top.size(); ++i) tops.push_back({});
     } else if (type == "ReLU" && (L.relu_slope = (float)(lp.sub("relu_param") ? lp.sub("relu_param")->num("negative_slope", 0.0) : 0.0), false)) {
     } else if ((type == "LRN" || type == "Dropout") && ([&] {
                  if (const PMessage* q = lp.sub("lrn_param")) {
@@ -468,10 +555,64 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       shapes_[L.param.top[i]] = tops[i];
       need_bw[L.param.top[i]] = layer_bw;
     }
+    // parameter sharing (Net::AppendParam, net.cpp:576-666).  BatchNorm's statistics (blobs 0-2) are not learnable blobs here; a
+    // name on one of them is refused as soon as a second blob would carry it: two layers would update one running mean
+    if (type == "BatchNorm")
+      for (int i = 0; i < 3 && i < (int)L.param.param.size(); ++i) {
+        const std::string& nm = L.param.param[i].name;
+        if (nm.empty()) continue;
+        B2_CHECK(!param_names.count(nm) && !bn_stat_names.count(nm),
+                 "Cannot share param '" + nm + "' with BatchNorm layer '" + L.param.name + "' statistics blob " + std::to_string(i) +
+                     ": two layers would update one running statistic");
+        bn_stat_names[nm] = L.param.name;
+      }
     int bid = 0;
     for (auto& bl : blobs) {
       const ParamSpec spec = bl.second < (int)L.param.param.size() ? L.param.param[bl.second] : ParamSpec();
-      params_.push_back(LearnableParam{L.param.name, id, bid++, prod(bl.first), bl.first, spec.lr_mult, spec.decay_mult});
+      LearnableParam p{L.param.name, id, bid++, prod(bl.first), bl.first, spec.lr_mult, spec.decay_mult};
+      p.layer_blob = bl.second;
+      p.name = spec.name;
+      if (!spec.name.empty() && bn_stat_names.count(spec.name))
+        Fatal(__FILE__, __LINE__, "Cannot share param '" + spec.name + "' with BatchNorm layer '" + bn_stat_names[spec.name] +
+                                      "' statistics blob: two layers would update one running statistic");
+      auto it = spec.name.empty() ? param_names.end() : param_names.find(spec.name);
+      if (it == param_names.end()) {                    // anonymous, or a name seen for the first time: this blob owns it
+        if (!spec.name.empty()) param_names[spec.name] = (int)net_params_.size();
+        p.learnable_id = (int)params_.size();
+        params_.push_back(p);
+        has_lr.push_back(spec.has_lr_mult);
+        has_decay.push_back(spec.has_decay_mult);
+      } else {                                          // a sharer: same storage, same update
+        const LearnableParam& o = net_params_[it->second];
+        auto shape_str = [](const std::vector<int>& s) {
+          std::string r;
+          for (int d : s) r += std::to_string(d) + " ";
+          return r + "(" + std::to_string(prod(s)) + ")";
+        };
+        const std::string who = "Cannot share param '" + spec.name + "' owned by layer '" + o.layer + "' with layer '" + L.param.name + "'; ";
+        if (spec.share_mode == 1) {                     // PERMISSIVE: the reference then reshapes the sharer; only STRICT is built
+          B2_CHECK(p.count == o.count, who + "count mismatch.  Owner layer param shape is " + shape_str(o.shape) + "; sharing layer shape is " +
+                                           shape_str(p.shape));
+          B2_CHECK(p.shape == o.shape, who + "share_mode PERMISSIVE with a different shape is not built (only STRICT sharing is).  Owner "
+                                           "layer param shape is " + shape_str(o.shape) + "; sharing layer expects shape " + shape_str(p.shape));
+        }
+        B2_CHECK(p.shape == o.shape, who + "shape mismatch.  Owner layer param shape is " + shape_str(o.shape) + "; sharing layer expects shape " +
+                                         shape_str(p.shape));
+        p.owner = it->second;
+        p.learnable_id = o.learnable_id;
+        LearnableParam& lo = params_[o.learnable_id];
+        if (spec.has_lr_mult) {                         // net.cpp:647-664: agree where both are given, else the sharer's value is adopted
+          B2_CHECK(!has_lr[o.learnable_id] || spec.lr_mult == lo.lr_mult, "Shared param '" + spec.name + "' has mismatched lr_mult.");
+          has_lr[o.learnable_id] = true;
+          lo.lr_mult = spec.lr_mult;
+        }
+        if (spec.has_decay_mult) {
+          B2_CHECK(!has_decay[o.learnable_id] || spec.decay_mult == lo.decay_mult, "Shared param '" + spec.name + "' has mismatched decay_mult.");
+          has_decay[o.learnable_id] = true;
+          lo.decay_mult = spec.decay_mult;
+        }
+      }
+      net_params_.push_back(p);
     }
     layer_top_shapes_.push_back(tops);
     layers_.push_back(std::move(L));

@@ -77,6 +77,9 @@ struct NetLayer {                       // one LayerParameter after phase filter
   std::vector<int> input_shape;         // Input / DummyData layers
   int softmax_axis = 1;                 // SoftmaxParameter.axis, canonicalised against the bottom's axes
   int flatten_axis = 1, flatten_end_axis = -1;   // FlattenParameter.axis / end_axis, canonicalised
+  int slice_axis = 1;                   // SliceParameter.axis (canonicalised) or slice_dim; the tops' shapes carry the split
+  float contrastive_margin = 1.f;       // ContrastiveLossParameter.margin / legacy_version (caffe.proto)
+  bool contrastive_legacy = false;
   // Net::Init's need-backward result (net.cpp:160-330), loss pruning included: whether the layer runs backward, and per bottom
   // whether it receives a gradient.  TrainNet reads these; nothing else restates the rule.
   bool need_backward = false;
@@ -85,7 +88,7 @@ struct NetLayer {                       // one LayerParameter after phase filter
 };
 
 // The bottom a loss-like layer reads its labels / targets from, which never receives a gradient (-1: none; EuclideanLoss sends
-// gradient to both of its bottoms).  SoftmaxWithLoss, SigmoidCrossEntropyLoss and Accuracy: bottom 1.
+// gradient to both of its bottoms).  SoftmaxWithLoss, SigmoidCrossEntropyLoss and Accuracy: bottom 1; ContrastiveLoss: bottom 2.
 int LabelBottom(const std::string& type);
 // A layer type whose name ends in "Loss" (LossLayer's subclasses)
 bool IsLossType(const std::string& type);
@@ -93,7 +96,16 @@ bool IsLossType(const std::string& type);
 // layer whose type ends in "Loss", 0 otherwise
 float TopLossWeight(const NetLayer& L, size_t t);
 
-struct LearnableParam { std::string layer; int layer_id, blob_id; size_t count; std::vector<int> shape; float lr_mult, decay_mult; };
+// One parameter blob of a layer.  blob_id counts the layer's learnable blobs; layer_blob is its index among the layer's blobs
+// (BatchNorm's scale / bias are blobs 3 and 4).  Named blobs are shared (Net::AppendParam, net.cpp:576-666): the first blob with
+// a name owns it, a later one is a sharer with owner = the owner's index in net_params(); learnable_id indexes learnable_params().
+struct LearnableParam {
+  std::string layer; int layer_id, blob_id; size_t count; std::vector<int> shape; float lr_mult, decay_mult;
+  int layer_blob = 0;
+  std::string name;                     // ParamSpec.name, empty when anonymous
+  int owner = -1;                       // -1: this blob owns its storage
+  int learnable_id = 0;
+};
 
 struct ConvEntry { std::string name; int layer_id; b2c_conv_params p; bool propagate_down; };
 
@@ -108,7 +120,11 @@ class Net {
   const std::vector<NetLayer>& layers() const { return layers_; }
   const std::map<std::string, std::vector<int>>& blob_shapes() const { return shapes_; }
   const std::vector<int>& top_shape(int layer, int top = 0) const { return layer_top_shapes_[layer][top]; }
-  const std::vector<LearnableParam>& learnable_params() const { return params_; }   // layer order (Net::AppendParam)
+  // owners only, in layer order (Net::learnable_params_); a sharer's lr_mult / decay_mult fill in what its owner left unset
+  const std::vector<LearnableParam>& learnable_params() const { return params_; }
+  const std::vector<LearnableParam>& net_params() const { return net_params_; }   // every layer's blobs, sharers included (Net::params_)
+  // the owner of blob `layer_blob` of layer `layer_id` as (layer_id, layer_blob); (-1, -1) when the blob owns itself
+  std::pair<int, int> param_owner(int layer_id, int layer_blob) const;
   const std::vector<ConvEntry>& conv_layers() const { return convs_; }
   int reduce_buckets() const { return reduce_buckets_; }
   float global_grad_scale() const { return global_grad_scale_; }
@@ -123,7 +139,7 @@ class Net {
   std::vector<NetLayer> layers_;
   std::map<std::string, std::vector<int>> shapes_;
   std::vector<std::vector<std::vector<int>>> layer_top_shapes_;
-  std::vector<LearnableParam> params_;
+  std::vector<LearnableParam> params_, net_params_;
   std::vector<ConvEntry> convs_;
   int reduce_buckets_ = 6;
   float global_grad_scale_ = 1.f;

@@ -250,26 +250,41 @@ void ConcatLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
   }
   t[0]->Reshape(s);
 }
-void ConcatLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
-  const size_t inner = t[0]->count(2), N = t[0]->shape(0), Ct = t[0]->shape(1);
-  size_t coff = 0;
-  for (Blob* src : b) {
-    const size_t w = sizeof(float) * src->shape(1) * inner;
-    CUDA_CHECK(cudaMemcpy2DAsync(t[0]->mutable_gpu_data() + coff * inner, sizeof(float) * Ct * inner, src->gpu_data(), w, w, N,
-                                 cudaMemcpyDeviceToDevice, S()));
-    coff += src->shape(1);
+// The copies of Concat and Slice: `whole` is the parts laid side by side along `axis`, as count(0, axis) rows of which part i
+// holds a window of shape(axis) * count(axis + 1) floats.  One strided 2-D copy per part: into whole's window (gather) or out of
+// it; diff selects the diffs instead of the data.  Parts with copy[i] false (when given) are skipped but keep their window.
+static void axis_copy(Blob* whole, const vector<Blob*>& parts, int axis, bool gather, bool diff, const vector<bool>* copy) {
+  const size_t inner = whole->count(axis + 1), rows = whole->count(0, axis), pitch = sizeof(float) * whole->shape(axis) * inner;
+  size_t off = 0;
+  for (size_t i = 0; i < parts.size(); ++i) {
+    Blob* p = parts[i];
+    const size_t w = sizeof(float) * p->shape(axis) * inner;
+    if (!copy || (*copy)[i]) {
+      if (gather)
+        CUDA_CHECK(cudaMemcpy2DAsync((diff ? whole->mutable_gpu_diff() : whole->mutable_gpu_data()) + off * inner, pitch,
+                                     diff ? p->gpu_diff() : p->gpu_data(), w, w, rows, cudaMemcpyDeviceToDevice, S()));
+      else
+        CUDA_CHECK(cudaMemcpy2DAsync(diff ? p->mutable_gpu_diff() : p->mutable_gpu_data(), w,
+                                     (diff ? whole->gpu_diff() : whole->gpu_data()) + off * inner, pitch, w, rows, cudaMemcpyDeviceToDevice, S()));
+    }
+    off += p->shape(axis);
   }
 }
-void ConcatLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
-  const size_t inner = t[0]->count(2), N = t[0]->shape(0), Ct = t[0]->shape(1);
-  size_t coff = 0;
-  for (size_t i = 0; i < b.size(); ++i) {
-    const size_t w = sizeof(float) * b[i]->shape(1) * inner;
-    if (pd[i])
-      CUDA_CHECK(cudaMemcpy2DAsync(b[i]->mutable_gpu_diff(), w, t[0]->gpu_diff() + coff * inner, sizeof(float) * Ct * inner, w, N,
-                                   cudaMemcpyDeviceToDevice, S()));
-    coff += b[i]->shape(1);
+void ConcatLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) { axis_copy(t[0], b, 1, true, false, nullptr); }
+void ConcatLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) { axis_copy(t[0], b, 1, false, true, &pd); }
+void SliceLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
+  size_t count = 0;
+  for (size_t i = 0; i < t.size(); ++i) {
+    B2_CHECK(t[i] != b[0], "Slice Layer does not allow in-place computation.");
+    t[i]->Reshape(shapes_[i]);
+    count += t[i]->count();
   }
+  B2_CHECK(count == b[0]->count(), "Slice: the tops do not cover the bottom");   // slice_layer.cpp:65
+}
+void SliceLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) { axis_copy(b[0], t, axis_, false, false, nullptr); }
+void SliceLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0]) return;
+  axis_copy(b[0], t, axis_, true, true, nullptr);
 }
 
 // ================================================================================================ SoftmaxWithLoss
@@ -340,6 +355,24 @@ void SigmoidCrossEntropyLossLayer::Backward_gpu(const vector<Blob*>&, const vect
   if (!pd[0]) return;
   const float scale = loss_weight_ / (float)b[0]->shape(0);     // caffe_scal(count, loss_weight / num, bottom_diff)
   B2C_CHECK(b2c_sigmoid_ce_loss_backward(b[0]->count(), b[0]->gpu_data(), b[1]->gpu_data(), scale, b[0]->mutable_gpu_diff(), S()));
+}
+
+// ================================================================================================ ContrastiveLoss
+void ContrastiveLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2C_CHECK(b2c_contrastive_loss_forward(b[0]->shape(0), (int)b[0]->count(1), b[0]->gpu_data(), b[1]->gpu_data(), b[2]->gpu_data(), margin_,
+                                         legacy_ ? 1 : 0, diff_.mutable_gpu_data(), dist_sq_.mutable_gpu_data(), t[0]->mutable_gpu_data(), S()));
+}
+void ContrastiveLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0] && !pd[1]) return;
+  // contrastive_loss_layer.cpp Backward_cpu: alpha = +-loss_weight / num; bottom 1's gradient is bottom 0's negated
+  const int N = b[0]->shape(0), C = (int)b[0]->count(1);
+  const float alpha = loss_weight_ / (float)N;
+  if (pd[0])
+    B2C_CHECK(b2c_contrastive_loss_backward(N, C, diff_.gpu_data(), dist_sq_.gpu_data(), b[2]->gpu_data(), margin_, legacy_ ? 1 : 0, alpha,
+                                            b[0]->mutable_gpu_diff(), pd[1] ? b[1]->mutable_gpu_diff() : nullptr, S()));
+  else
+    B2C_CHECK(b2c_contrastive_loss_backward(N, C, diff_.gpu_data(), dist_sq_.gpu_data(), b[2]->gpu_data(), margin_, legacy_ ? 1 : 0, -alpha,
+                                            b[1]->mutable_gpu_diff(), nullptr, S()));
 }
 
 // ================================================================================================ Accuracy
@@ -536,20 +569,45 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       B2_CHECK(L.concat_axis == 1, "TrainNet: Concat is built for the channel axis only");
       layer.reset(new ConcatLayer(L.param));
     }
+    else if (type == "Slice") {
+      vector<vector<int>> shapes;
+      for (size_t t = 0; t < L.param.top.size(); ++t) shapes.push_back(net.top_shape((int)li, (int)t));
+      layer.reset(new SliceLayer(L.param, L.slice_axis, shapes));
+    }
+    else if (type == "ContrastiveLoss") {
+      auto* cl = new ContrastiveLossLayer(L.param, L.contrastive_margin, L.contrastive_legacy);
+      if (!L.loss_weight.empty()) cl->set_loss_weight(L.loss_weight[0]);
+      layer.reset(cl);
+    }
     else B2_CHECK(false, "TrainNet: layer type '" + type + "' is not built yet (SURVEY 8f rank 2 covers the ResNet-50 set)");
     layer->SetUp(node.bottom, node.top);
     // learnable blobs in layer order: Net::AppendParam (net.cpp:573-606) appends EVERY blob of every layer, so param ids,
     // reduce-bucket boundaries and the SolverState history list (5 blobs per BatchNorm layer) match the reference.
     // Blobs the layer never differentiates (BatchNorm mean / variance / correction, batch_norm_layer.cpp: lr_mult forced
     // to 0) are marked `statistic`; trainable_ids_ lists the rest for the trainer API.
-    node.first_param = (int)learnable_.size();
+    // A blob that shares a named parameter (Net::AppendParam, net.cpp:611-666; Net checked shapes and multipliers) is not appended:
+    // it maps to its owner's id, keeps its own Blob object, and aliases the owner's storage once the arena exists (ShareNamedParams).
     for (size_t bi = 0; bi < layer->blobs().size(); ++bi) {
-      ParamSpec ps = bi < L.param.param.size() ? L.param.param[bi] : ParamSpec();
+      const ParamSpec& own = bi < L.param.param.size() ? L.param.param[bi] : ParamSpec();
+      const std::pair<int, int> owner = net.param_owner((int)li, (int)bi);
+      if (owner.first >= 0) {
+        const Node& on = nodes_[owner.first];
+        const int id = on.param_ids[owner.second];
+        node.param_ids.push_back(id);
+        node.param_owned.push_back(false);
+        shares_.push_back({(int)li, (int)bi, owner.first, owner.second});
+        if (own.has_lr_mult && !specs[id].statistic) specs[id].lr_mult = own.lr_mult;   // the owner left it unset (else Net found them equal)
+        if (own.has_decay_mult && !specs[id].statistic) specs[id].decay_mult = own.decay_mult;
+        continue;
+      }
+      ParamSpec ps = own;
       if (!layer->param_propagate_down((int)bi)) { ps.lr_mult = 0.f; ps.decay_mult = 0.f; ps.statistic = true; }
       else trainable_ids_.push_back((int)learnable_.size());
+      if (node.first_owned < 0) node.first_owned = (int)learnable_.size();
+      node.param_ids.push_back((int)learnable_.size());
+      node.param_owned.push_back(true);
       learnable_.push_back(layer->blobs()[bi]);
       specs.push_back(ps);
-      ++node.num_params;
     }
     // need-backward (net.cpp:160-330, loss pruning included) is Net's result; a TEST net runs no backward at all.  Accuracy is
     // forward-only (accuracy_layer.hpp: "cannot backpropagate"): its top carries no loss weight, so pruning already stops it
@@ -679,6 +737,9 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
     solver_.reset(new SGDSolver(sp));
     solver_->SetParams(learnable_, specs);
   }
+  // Net::ShareWeights (net.cpp:1270-1287), after the arena re-homed the owners: every sharer blob aliases its owner's data and diff.
+  // The sharer's filler ran in SetUp; the owner's values win, with no copy either way
+  for (const Share& sh : shares_) AliasShare(sh);
   for (auto& l : layers_)
     if (auto* c = dynamic_cast<ConvolutionLayer*>(l.get()))
       if (c->EnableFilterCache()) cached_convs_.push_back(c);
@@ -718,6 +779,12 @@ size_t TrainNet::activation_floats() const {
   size_t c = 0;
   for (auto& kv : blobs_) c += kv.second->count();
   return c;
+}
+void TrainNet::AliasShare(const Share& sh) {
+  Blob* sharer = layers_[sh.layer]->blobs()[sh.blob].get();
+  Blob& owner = *layers_[sh.owner_layer]->blobs()[sh.owner_blob];
+  sharer->ShareData(owner);
+  sharer->ShareDiff(owner);
 }
 void TrainNet::PrepareFilters() {
   // one multi-tensor launch per 24 filter layouts instead of one prepass per forward and per dgrad call
@@ -762,7 +829,10 @@ void TrainNet::Backward(bool update) {
           B2C_CHECK(b2c_add(nd.bottom[i]->count(), nd.bottom[i]->gpu_diff(), nd.bottom_diff_tmp[i]->gpu_diff(), nd.bottom[i]->mutable_gpu_diff(), S()));
       if (prof) prof->end(ph, S());
     }
-    if (update && nd.num_params) sched_->on_param_ready(nd.first_param, S());     // net.cpp:738-746
+    // net.cpp:738-746: only the owner of a parameter releases it, after its own backward.  The owner of a shared parameter is the
+    // earliest layer that uses the name, so its backward runs after every sharer's has added into the shared diff; a layer that
+    // owns nothing releases nothing.  Owned ids grow with the layer index, so releases still arrive in descending id order.
+    if (update && nd.first_owned >= 0) sched_->on_param_ready(nd.first_owned, S());
   }
 }
 float TrainNet::ForwardBackward() {
@@ -900,6 +970,7 @@ float TrainNet::last_loss() { return loss_blob_ ? loss_blob_->cpu_data()[0] : 0.
 void TrainNet::ShareTrainedLayersWith(TrainNet& train) {
   B2_CHECK(test_, "ShareTrainedLayersWith: only a TEST-phase net takes another net's parameters");
   CUDA_CHECK(cudaStreamSynchronize(S()));
+  vector<bool> taken(layers_.size(), false);
   for (size_t i = 0; i < layers_.size(); ++i) {
     size_t k = 0;
     while (k < train.layer_names_.size() && train.layer_names_[k] != layer_names_[i]) ++k;
@@ -911,10 +982,15 @@ void TrainNet::ShareTrainedLayersWith(TrainNet& train) {
       B2_CHECK(src[j]->shape() == dst[j]->shape(), "Cannot share param " + std::to_string(j) + " weights from layer '" + layer_names_[i] +
                                                        "'; shape mismatch.  Source param shape is " + src[j]->shape_string() +
                                                        "; target param shape is " + dst[j]->shape_string());
-      dst[j] = src[j];
-      learnable_[nodes_[i].first_param + j] = src[j];
+      dst[j] = src[j];                             // a sharer takes the trainer's sharer blob, which aliases the trainer's owner
+      if (nodes_[i].param_owned[j]) learnable_[nodes_[i].param_ids[j]] = src[j];
     }
+    taken[i] = true;
   }
+  // a sharer in a layer the trainer does not have kept its own blob, which aliased an owner blob that may just have been replaced
+  // (and freed): point it at the owner's current storage
+  for (const Share& sh : shares_)
+    if (!taken[sh.layer]) AliasShare(sh);
   // a multi-GPU trainer: rank r scores its stripe of the validation database (Net::Init's TEST DataReader gets (solver_count, rank))
   test_sync_ = train.sync_;
   if (test_sync_ && db_data_) db_data_->set_solver(test_sync_->nranks(), test_sync_->rank());

@@ -162,6 +162,20 @@ class ConcatLayer : public LayerBase {         // along the channel axis (axis 1
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
 };
 
+// slice_layer.cpp: the bottom split along one axis into the tops, in order; Concat's strided 2-D copies with the roles swapped.
+// Backward writes the whole bottom diff: a top whose diff no layer writes contributes its zero-initialised diff.
+class SliceLayer : public LayerBase {
+ public:
+  SliceLayer(const LayerParameter& p, int axis, const vector<vector<int>>& top_shapes) : LayerBase(p), axis_(axis), shapes_(top_shapes) {}
+  const char* type() const override { return "Slice"; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  int axis_;
+  vector<vector<int>> shapes_;
+};
+
 class SoftmaxWithLossLayer : public LayerBase {
  public:
   using LayerBase::LayerBase;
@@ -236,6 +250,24 @@ class SigmoidCrossEntropyLossLayer : public LayerBase {   // no sigmoid tensor: 
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  float loss_weight_ = 1.f;
+};
+
+// contrastive_loss_layer.cpp: bottoms a, b [N, C(, 1, 1)] and the similarity label [N]; diff = a - b and dist_sq are kept for backward
+class ContrastiveLossLayer : public LayerBase {
+ public:
+  ContrastiveLossLayer(const LayerParameter& p, float margin, bool legacy) : LayerBase(p), margin_(margin), legacy_(legacy) {}
+  void set_loss_weight(float w) { loss_weight_ = w; }
+  const char* type() const override { return "ContrastiveLoss"; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override {
+    diff_.Reshape({b[0]->shape(0), (int)b[0]->count(1)}); dist_sq_.Reshape({b[0]->shape(0)}); t[0]->Reshape({1});
+  }
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  float margin_;
+  bool legacy_;
+  Blob diff_, dist_sq_;
   float loss_weight_ = 1.f;
 };
 
@@ -331,7 +363,9 @@ class TrainNet {
   Blob* blob(const string& name);
   int num_layers() const { return (int)layers_.size(); }
   LayerBase* layer(int i) { return layers_[i].get(); }
-  const vector<shared_ptr<Blob>>& learnable_params() const { return learnable_; }   // Net::learnable_params(): every layer blob
+  // Net::learnable_params(): every layer blob that owns its storage (a blob sharing a named parameter is not listed: it aliases its
+  // owner's data and diff, and its gradient adds into the owner's)
+  const vector<shared_ptr<Blob>>& learnable_params() const { return learnable_; }
   const vector<int>& trainable_ids() const { return trainable_ids_; }               // ids the layers differentiate
   size_t activation_floats() const;
   size_t input_bytes() const { return db_data_ ? db_data_->h2d_bytes() : data_ ? data_->h2d_bytes() : 0; }   // host -> device bytes of one e2e step's batch
@@ -380,11 +414,19 @@ class TrainNet {
     vector<bool> accumulate_bottom;                // per bottom: the layer itself adds into the blob's diff (no shadow blob)
     vector<bool> deferred_add;                     // per bottom: the shadow diff is added by the blob's producer (fused BatchNorm residual tail)
     bool need_backward = false;
-    int first_param = -1, num_params = 0;
+    // per layer blob: its learnable id (the owner's for a shared blob; the reference's learnable_param_ids_) and whether this layer
+    // owns it.  first_owned: the lowest learnable id this layer owns, -1 when it owns none (it then releases nothing to the reducer)
+    vector<int> param_ids;
+    vector<bool> param_owned;
+    int first_owned = -1;
   };
   void Forward(bool copy_input);
   void Backward(bool update);
   void PrepareFilters();                           // b2c_conv_prepare_filters over every cached conv layer (weights changed)
+  // a blob that shares a named parameter (Net::param_owners_): blob `blob` of layer `layer` aliases blob `owner_blob` of `owner_layer`
+  struct Share { int layer, blob, owner_layer, owner_blob; };
+  vector<Share> shares_;
+  void AliasShare(const Share& sh);                // the sharer's data and diff alias the owner's (ShareData + ShareDiff, no copy)
   void Profile(int n, const std::function<void()>& iteration, vector<int>* layer, vector<int>* op, vector<float>* ms);
  public:
   void MarkParamsDirty() { filters_dirty_ = true; } // call after writing parameter data behind the net's back

@@ -236,6 +236,19 @@ class Net:
             out.append((nm.value.decode(), cnt.value, lr.value, dc.value))
         return out
 
+    def net_params(self):
+        """Every layer's parameter blobs, sharers included: [(layer, param name, owner, learnable id)].  owner is the index of the
+        owning blob in this list (-1: the blob owns its storage); learnable id indexes learnable_params()."""
+        L = lib()
+        L.b2h_net_net_param.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_char_p, C.c_char_p, C.c_int]
+        L.b2h_net_num_net_params.argtypes = [C.c_void_p]
+        out = []
+        for i in range(L.b2h_net_num_net_params(self._h)):
+            ow, lid, nm, pn = C.c_int(), C.c_int(), C.create_string_buffer(256), C.create_string_buffer(256)
+            L.b2h_net_net_param(self._h, i, C.byref(ow), C.byref(lid), nm, pn, 256)
+            out.append((nm.value.decode(), pn.value.decode(), ow.value, lid.value))
+        return out
+
     def reduce_buckets(self):
         return lib().b2h_net_reduce_buckets(self._h)
 
@@ -442,6 +455,15 @@ class Trainer:
 
     def activation_floats(self):
         return lib().b2h_trainer_activation_floats(self._h)
+
+    def layer_blob_pointers(self, layer, blob):
+        """(Blob object address, device data pointer, device diff pointer) of blob `blob` of layer `layer` (execution order)"""
+        L = lib()
+        u = C.c_ulonglong
+        L.b2h_trainer_layer_blob.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(u), C.POINTER(u), C.POINTER(u)]
+        o, d, g = u(), u(), u()
+        _ck(L.b2h_trainer_layer_blob(self._h, layer, blob, C.byref(o), C.byref(d), C.byref(g)))
+        return o.value, d.value, g.value
 
     def database_batches(self):
         """Batches the LMDB-backed Data layer has loaded so far, or -1 when the net runs on the synthetic source."""

@@ -278,6 +278,22 @@ int b2c_sigmoid_ce_loss_backward(size_t count, const float* x, const float* targ
  * with alpha = +-loss_weight / N.  dx may be diff.                                                                             */
 int b2c_euclidean_loss_forward(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream);
 int b2c_euclidean_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream);
+/* ContrastiveLossLayer (src/caffe/layers/contrastive_loss_layer.cpp), N pairs of C-channel features a, b [N, C] and labels y [N]
+ * read as (int)y (0.7 is dissimilar, -1 similar).  Forward, one launch: diff = a - b [N, C] (kept for backward), dist_sq [N], and
+ * *loss (device scalar) = sum_n (y_n ? d2_n : max(margin - sqrt(d2_n), 0)^2) / N / 2; legacy != 0 takes max(margin - d2_n, 0) as
+ * the dissimilar term.  Rounding: dist_sq[n] = float( sum_c float(diff^2) ), each square rounded to float and the sum over the
+ * channels taken in double, then rounded once; every term is formed in float from that dist_sq and the terms are summed in
+ * double over the pairs with b2c_euclidean_loss_forward's cluster reduction (no atomics: the same bits on every call).
+ * Backward, one elementwise launch, alpha = loss_weight / N: similar pairs da = alpha * diff; dissimilar pairs with
+ * mdist = margin - sqrt(d2) > 0: da = (-alpha * mdist / (sqrt(d2) + 1e-4)) * diff (the 1e-4 is the reference's), else 0.  Legacy:
+ * da = -alpha * diff where margin - d2 > 0, else 0 -- the reference's Backward_cpu.  Its .cu kernel writes the constant -alpha
+ * with no diff factor there, which is not the derivative of the loss it computes; this follows the CPU form.  db (may be null)
+ * = -da bit for bit, except that both are +0 where the hinge zeroes a pair (as the reference's caffe_set(0)).  float4 path when diff, da and db are 16-byte aligned and C % 4 == 0, else one float at a
+ * time.  N >= 1 and C >= 1, else B2C_ERR_INVALID.                                                                           */
+int b2c_contrastive_loss_forward(int N, int C, const float* a, const float* b, const float* y, float margin, int legacy, float* diff,
+                                 float* dist_sq, float* loss, void* stream);
+int b2c_contrastive_loss_backward(int N, int C, const float* diff, const float* dist_sq, const float* y, float margin, int legacy,
+                                  float alpha, float* da, float* db, void* stream);
 /* y[n][o][p] += bias[o];  db[o] += sum_{n,p} dy[n][o][p]  (InnerProduct bias with P = 1; conv bias with P = Ho*Wo). */
 int b2c_bias_forward(int N, int O, int P, const float* bias, float* y, void* stream);
 int b2c_bias_backward(int N, int O, int P, const float* dy, float* db, void* stream);
