@@ -178,11 +178,50 @@ struct ParamSpec {
   bool has_lr_mult = false, has_decay_mult = false;
   int share_mode = 0;
 };
+// The sub-messages of caffe.proto's LayerParameter the built layers read, with the proto's names and defaults.  Net (prototxt.hpp)
+// fills them and stores what it resolves against the bottoms: canonical axes, global pooling's window, BatchNorm's eps floor.
+struct PoolingParameter { int pool = 0, kernel_h = 0, kernel_w = 0, stride_h = 1, stride_w = 1, pad_h = 0, pad_w = 0; bool global_pooling = false; };   // pool: MAX = 0, AVE = 1, STOCHASTIC = 2
+struct InnerProductParameter { int num_output = 0; bool bias_term = true; FillerParameter weight_filler, bias_filler; };
+struct BatchNormParameter {     // NVCaffe's; a scale_filler or bias_filler implies scale_bias.  The fillers' defaults: scale 1, bias 0
+  bool scale_bias = false; float eps = 1e-5f, moving_average_fraction = 0.999f; FillerParameter scale_filler{"constant", 1.f}, bias_filler;
+};
+struct ReLUParameter { float negative_slope = 0.f; };
+struct LRNParameter { int local_size = 5; float alpha = 1.f, beta = 0.75f, k = 1.f; int norm_region = 0; };   // ACROSS_CHANNELS = 0, WITHIN_CHANNEL = 1
+struct DropoutParameter { float dropout_ratio = 0.5f; };
+struct EltwiseParameter { int operation = 1; vector<float> coeff; };   // PROD = 0, SUM = 1, MAX = 2
+struct ConcatParameter { int axis = 1; };
+struct SliceParameter { int axis = 1; bool slice_dim_given = false; vector<int> slice_point; };   // axis: SliceParameter.axis or slice_dim
+struct SoftmaxParameter { int axis = 1; };
+struct FlattenParameter { int axis = 1, end_axis = -1; };
+struct AccuracyParameter { int top_k = 1; };
+struct ContrastiveLossParameter { float margin = 1.f; bool legacy_version = false; };
+struct TransformationParameter { float scale = 1.f; bool mirror = false; int crop_size = 0; vector<float> mean_value; string mean_file; long long random_seed = -1; };
+struct DataParameter {   // batch_size after Net's batch override; backend: LEVELDB = 0, LMDB = 1; parser_threads 0: automatic (see DataLayer)
+  string source; int batch_size = 0, backend = 0, parser_threads = 0; bool force_encoded_color = false, cache = false, shuffle = false;
+};
+enum Phase { TRAIN = 0, TEST = 1 };
 struct LayerParameter {
   string name, type;
   vector<string> bottom, top;
+  vector<float> loss_weight;            // one per top; see TopLossWeight (prototxt.hpp) for the default
   vector<ParamSpec> param;
+  Phase phase = TRAIN;                  // the net's phase: TEST runs BatchNorm on its running statistics and Dropout as the identity
   ConvolutionParameter convolution_param;
+  PoolingParameter pooling_param;
+  InnerProductParameter inner_product_param;
+  BatchNormParameter batch_norm_param;
+  ReLUParameter relu_param;
+  LRNParameter lrn_param;
+  DropoutParameter dropout_param;
+  EltwiseParameter eltwise_param;
+  ConcatParameter concat_param;
+  SliceParameter slice_param;
+  SoftmaxParameter softmax_param;
+  FlattenParameter flatten_param;
+  AccuracyParameter accuracy_param;
+  ContrastiveLossParameter contrastive_loss_param;
+  TransformationParameter transform_param;
+  DataParameter data_param;
 };
 
 // ---------------------------------------------------------------------------------------------- Layer
@@ -199,6 +238,7 @@ class LayerBase {
   void Backward(const vector<Blob*>& top, const vector<bool>& propagate_down, const vector<Blob*>& bottom);
   vector<shared_ptr<Blob>>& blobs() { return blobs_; }
   const LayerParameter& layer_param() const { return layer_param_; }
+  float loss_weight() const;            // the loss weight of top 0 (TopLossWeight: 1 for a *Loss type unless the prototxt says)
   virtual const char* type() const { return ""; }
   virtual int MinBottomBlobs() const { return -1; }
   virtual int MinTopBlobs() const { return -1; }

@@ -8,7 +8,7 @@
 
 namespace caffe {
 
-DataLayer::DataLayer(const NetLayer& L, uint64_t seed, bool train) : LayerBase(L.param), L_(L), seed_(seed), train_(train) {}
+DataLayer::DataLayer(const NetLayer& L, uint64_t seed) : LayerBase(L.param), seed_(seed) {}
 
 DataLayer::~DataLayer() {
   if (copy_stream_) cudaStreamSynchronize(copy_stream_);
@@ -31,43 +31,45 @@ DataLayer::~DataLayer() {
 }
 
 void DataLayer::LayerSetUp(const vector<Blob*>&, const vector<Blob*>& top) {
+  const DataParameter& dp = layer_param_.data_param;
+  const TransformationParameter& tp = layer_param_.transform_param;
   B2_CHECK(top.size() == 1 || top.size() == 2, "Data layer produces data, or data and label");
-  B2_CHECK(L_.batch_size > 0, "Data layer needs a positive batch_size");
-  N_ = L_.batch_size;
+  B2_CHECK(dp.batch_size > 0, "Data layer needs a positive batch_size");
+  N_ = dp.batch_size;
   bool encoded = false;
-  PeekDatumShape(L_.data_source, &C_, &Hd_, &Wd_, L_.force_encoded_color, &encoded);             // data_layer.cpp:176-183: shape from one datum
-  crop_h_ = L_.crop_size > 0 ? L_.crop_size : Hd_;
-  crop_w_ = L_.crop_size > 0 ? L_.crop_size : Wd_;
+  PeekDatumShape(dp.source, &C_, &Hd_, &Wd_, dp.force_encoded_color, &encoded);             // data_layer.cpp:176-183: shape from one datum
+  crop_h_ = tp.crop_size > 0 ? tp.crop_size : Hd_;
+  crop_w_ = tp.crop_size > 0 ? tp.crop_size : Wd_;
   B2_CHECK(Hd_ >= crop_h_ && Wd_ >= crop_w_, "crop_size larger than the datum");   // data_transformer.cpp:192-193
-  host_crop_ = encoded && L_.crop_size > 0 && L_.mean_file.empty();
-  if (host_crop_) Hd_ = Wd_ = L_.crop_size;                                        // the slots hold crop windows
+  host_crop_ = encoded && tp.crop_size > 0 && tp.mean_file.empty();
+  if (host_crop_) Hd_ = Wd_ = tp.crop_size;                                        // the slots hold crop windows
   top[0]->Reshape({N_, C_, crop_h_, crop_w_});
   if (top.size() > 1) top[1]->Reshape({N_});
   u8_bytes_ = (size_t)N_ * C_ * Hd_ * Wd_;
 
   // DataTransformer's constructor (data_transformer.cpp:17-40)
-  if (!L_.mean_file.empty()) {
-    B2_CHECK(L_.mean_value.empty(), "Cannot specify mean_file and mean_value at the same time");
-    const BlobData mean = ParseBlobProto(ReadBinaryFile(L_.mean_file));
+  if (!tp.mean_file.empty()) {
+    B2_CHECK(tp.mean_value.empty(), "Cannot specify mean_file and mean_value at the same time");
+    const BlobData mean = ParseBlobProto(ReadBinaryFile(tp.mean_file));
     vector<int> shp = mean.shape;
     while (shp.size() > 3 && shp.front() == 1) shp.erase(shp.begin());   // (1, C, H, W) as compute_image_mean writes it
     B2_CHECK(shp.size() == 3 && shp[0] == C_ && shp[1] == Hd_ && shp[2] == Wd_,
-             "mean_file " + L_.mean_file + " does not have the datums' channels x height x width");   // data_transformer.cpp:198-200
+             "mean_file " + tp.mean_file + " does not have the datums' channels x height x width");   // data_transformer.cpp:198-200
     CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&dev_mean_image_), sizeof(float) * mean.data.size()));
     CUDA_CHECK(cudaMemcpy(dev_mean_image_, mean.data.data(), sizeof(float) * mean.data.size(), cudaMemcpyHostToDevice));
-  } else if (!L_.mean_value.empty()) {
-    B2_CHECK(L_.mean_value.size() == 1 || (int)L_.mean_value.size() == C_, "Specify either 1 mean_value or as many as channels: " + std::to_string(C_));
-    vector<float> mv(C_, L_.mean_value[0]);
-    if ((int)L_.mean_value.size() == C_) mv = L_.mean_value;
+  } else if (!tp.mean_value.empty()) {
+    B2_CHECK(tp.mean_value.size() == 1 || (int)tp.mean_value.size() == C_, "Specify either 1 mean_value or as many as channels: " + std::to_string(C_));
+    vector<float> mv(C_, tp.mean_value[0]);
+    if ((int)tp.mean_value.size() == C_) mv = tp.mean_value;
     CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&dev_mean_values_), sizeof(float) * C_));
     CUDA_CHECK(cudaMemcpy(dev_mean_values_, mv.data(), sizeof(float) * C_, cudaMemcpyHostToDevice));
   }
 
-  if (L_.data_cache || L_.data_shuffle)
+  if (dp.cache || dp.shuffle)
     fprintf(stderr, "DataLayer '%s': data_param { cache: %s shuffle: %s } -- the database is a read-only mapping of the page cache, "
                     "so `cache` has nothing to add; `shuffle` is not built: records are read in key order (shuffle when converting)\n",
-            L_.param.name.c_str(), L_.data_cache ? "true" : "false", L_.data_shuffle ? "true" : "false");
-  parsers_ = L_.parser_threads > 0 ? L_.parser_threads : (encoded ? 6 : 1);
+            layer_param_.name.c_str(), dp.cache ? "true" : "false", dp.shuffle ? "true" : "false");
+  parsers_ = dp.parser_threads > 0 ? dp.parser_threads : (encoded ? 6 : 1);
   const int K = std::max(2, parsers_ + 1);
   slot_.resize(K);
   CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
@@ -96,21 +98,22 @@ size_t DataLayer::h2d_bytes() const { return u8_bytes_ + sizeof(int) * 3 * (size
 
 void DataLayer::EnsureStarted() {
   if (reader_) return;
+  const TransformationParameter& tp = layer_param_.transform_param;
   DataReaderParam p;
-  p.source = L_.data_source;
+  p.source = layer_param_.data_param.source;
   p.batch_size = N_;
   p.solver_count = (size_t)solver_count_;
   p.solver_rank = (size_t)solver_rank_;
   p.parser_threads = (size_t)parsers_;
-  p.force_encoded_color = L_.force_encoded_color;
-  p.host_crop = host_crop_ ? L_.crop_size : 0;
-  p.train = train_;
+  p.force_encoded_color = layer_param_.data_param.force_encoded_color;
+  p.host_crop = host_crop_ ? tp.crop_size : 0;
+  p.train = layer_param_.phase != TEST;
   reader_.reset(new DataReader(p));
   B2_CHECK(reader_->channels() == C_ && reader_->height() == Hd_ && reader_->width() == Wd_, "database changed shape between set-up and start");
   // random_seed >= 0: "Use random_seed setting for deterministic transformations" (data_transformer.cpp:733-736); otherwise every
   // solver gets its own stream (the reference: Caffe::next_seed() of a solver seeded with seed + rank, parallel.cpp:179-187)
-  const uint64_t s = L_.transform_random_seed >= 0 ? (uint64_t)L_.transform_random_seed : seed_ + 0x9E3779B9ull * (uint64_t)(solver_rank_ + 1);
-  draws_.reset(new TransformDraws(s, L_.mirror, L_.crop_size, train_));
+  const uint64_t s = tp.random_seed >= 0 ? (uint64_t)tp.random_seed : seed_ + 0x9E3779B9ull * (uint64_t)(solver_rank_ + 1);
+  draws_.reset(new TransformDraws(s, tp.mirror, tp.crop_size, p.train));
   for (int s = 0; s < (int)slot_.size(); ++s) HandToReader(s);   // slot k assembles batch k, k + K, k + 2K, ...
 }
 
@@ -133,7 +136,7 @@ void DataLayer::IssueCopy(int s) {
   // data_layer.cpp:283-296).  host_off is free: LoadBatch waited for this slot's previous copy before handing the slot back.
   unsigned char* mir = reinterpret_cast<unsigned char*>(sl.host_off + 2 * N_);
   if (host_crop_) {                                      // the windows are cut already; what is left for the device is the flip
-    for (int i = 0; i < N_; ++i) { sl.host_off[i] = sl.host_off[N_ + i] = 0; mir[i] = (L_.mirror && (sl.rand[3 * i] % 2)) ? 1 : 0; }
+    for (int i = 0; i < N_; ++i) { sl.host_off[i] = sl.host_off[N_ + i] = 0; mir[i] = (layer_param_.transform_param.mirror && (sl.rand[3 * i] % 2)) ? 1 : 0; }
   } else {
     for (int i = 0; i < N_; ++i) draws_->Draw(Hd_, Wd_, sl.host_off + i, sl.host_off + N_ + i, mir + i);
   }
@@ -150,7 +153,7 @@ void DataLayer::LoadBatch(const vector<Blob*>& top, cudaStream_t st) {
   if (!sl.in_flight) IssueCopy(cur_);                    // the first batch: nothing was prefetched yet
   CUDA_CHECK(cudaStreamWaitEvent(st, sl.copied, 0));
   B2C_CHECK(b2c_transform_u8(sl.dev_u8, N_, C_, Hd_, Wd_, crop_h_, crop_w_, sl.dev_off, sl.dev_off + N_,
-                             reinterpret_cast<const unsigned char*>(sl.dev_off + 2 * N_), dev_mean_values_, dev_mean_image_, L_.transform_scale,
+                             reinterpret_cast<const unsigned char*>(sl.dev_off + 2 * N_), dev_mean_values_, dev_mean_image_, layer_param_.transform_param.scale,
                              top[0]->mutable_gpu_data(), st));
   if (top.size() > 1)
     CUDA_CHECK(cudaMemcpyAsync(top[1]->mutable_gpu_data(), sl.dev_label, sizeof(float) * N_, cudaMemcpyDeviceToDevice, st));

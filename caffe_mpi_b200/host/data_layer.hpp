@@ -22,9 +22,9 @@ namespace caffe {
 
 class DataLayer : public LayerBase {
  public:
-  // `seed` feeds the crop / mirror stream when transform_param.random_seed is unset (the reference draws Caffe::next_seed());
-  // train = false (TEST phase): the centre crop window
-  DataLayer(const NetLayer& L, uint64_t seed, bool train = true);
+  // reads L.param's data_param and transform_param.  `seed` feeds the crop / mirror stream when transform_param.random_seed is unset
+  // (the reference draws Caffe::next_seed()); the TEST phase takes the centre crop window
+  DataLayer(const NetLayer& L, uint64_t seed);
   ~DataLayer() override;
   const char* type() const override { return "Data"; }
   void LayerSetUp(const vector<Blob*>& bottom, const vector<Blob*>& top) override;
@@ -64,9 +64,7 @@ class DataLayer : public LayerBase {
   // and 4, data_layer.cpp:85-95) becomes 1 for raw datums -- one thread's memcpy outruns the GPU -- and 6 for encoded ones: at
   // ~0.8 k decoded 256x256 JPEGs per second and thread that is what a GPU training ResNet-50 at a few thousand img/s asks for
   int parsers_ = 1;
-  NetLayer L_;
   uint64_t seed_;
-  bool train_;
   int solver_count_ = 1, solver_rank_ = 0;
   int N_ = 0, C_ = 0, Hd_ = 0, Wd_ = 0, crop_h_ = 0, crop_w_ = 0;
   size_t u8_bytes_ = 0;

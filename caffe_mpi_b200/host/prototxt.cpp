@@ -169,11 +169,6 @@ FillerParameter filler_of(const PMessage* m) {
 }
 std::vector<int> to_int(const std::vector<long long>& v) { return std::vector<int>(v.begin(), v.end()); }
 size_t prod(const std::vector<int>& s, size_t from = 0) { size_t c = 1; for (size_t i = from; i < s.size(); ++i) c *= (size_t)s[i]; return c; }
-int pooled_extent(int in, int k, int s, int p) {        // PoolingLayer::Reshape: ceil mode + last-window clip
-  int o = (int)std::ceil((float)(in + 2 * p - k) / s) + 1;
-  if (p > 0 && (o - 1) * s >= in + p) --o;
-  return o;
-}
 int canonical_axis(int axis, const std::vector<int>& s) {  // Blob::CanonicalAxisIndex, with its message
   const int n = (int)s.size();
   if (axis < -n || axis >= n) {
@@ -184,6 +179,112 @@ int canonical_axis(int axis, const std::vector<int>& s) {  // Blob::CanonicalAxi
   }
   return axis < 0 ? axis + n : axis;
 }
+// Step one of Net::Net for a layer: the LayerParameter message as written, every sub-message the built layers read included.
+// What depends on the bottoms' shapes (canonical axes, global pooling) is resolved by the shape step.
+LayerParameter read_layer(const PMessage& lp, Phase phase, int batch_override) {
+  static const PMessage none;                           // an absent sub-message reads as its defaults
+  auto sub = [&](const char* k) -> const PMessage& { const PMessage* m = lp.sub(k); return m ? *m : none; };
+  LayerParameter p;
+  p.name = lp.str("name");
+  p.type = lp.str("type");
+  p.phase = phase;
+  for (const PField* f : lp.all("loss_weight")) p.loss_weight.push_back((float)std::atof(f->scalar.c_str()));
+  for (auto* b : lp.all("bottom")) p.bottom.push_back(b->scalar);
+  for (auto* t : lp.all("top")) p.top.push_back(t->scalar);
+  for (auto* ps : lp.all("param")) {
+    ParamSpec s;
+    if (ps->is_msg()) {
+      const PMessage& m = *ps->msg;
+      s.lr_mult = (float)m.num("lr_mult", 1.0); s.decay_mult = (float)m.num("decay_mult", 1.0);
+      s.has_lr_mult = m.has("lr_mult"); s.has_decay_mult = m.has("decay_mult");
+      s.name = m.str("name");
+      const std::string sm = m.str("share_mode", "STRICT");
+      s.share_mode = (sm == "PERMISSIVE" || sm == "1") ? 1 : 0;
+    }
+    p.param.push_back(s);
+  }
+  const PMessage& cp = sub("convolution_param");
+  ConvolutionParameter& c = p.convolution_param;
+  c.num_output = (int)cp.integer("num_output");
+  c.bias_term = cp.boolean("bias_term", true);
+  c.pad = to_int(cp.ints("pad")); c.kernel_size = to_int(cp.ints("kernel_size"));
+  c.stride = to_int(cp.ints("stride")); c.dilation = to_int(cp.ints("dilation"));
+  c.pad_h = (int)cp.integer("pad_h", -1);
+  c.pad_w = (int)cp.integer("pad_w", -1);
+  c.kernel_h = (int)cp.integer("kernel_h", -1);
+  c.kernel_w = (int)cp.integer("kernel_w", -1);
+  c.stride_h = (int)cp.integer("stride_h", -1);
+  c.stride_w = (int)cp.integer("stride_w", -1);
+  c.group = (int)cp.integer("group", 1);
+  c.weight_filler = filler_of(cp.sub("weight_filler"));
+  c.bias_filler = filler_of(cp.sub("bias_filler"));
+  c.engine = engine_of(cp.str("engine", "DEFAULT"));
+  c.axis = (int)cp.integer("axis", 1);
+  c.force_nd_im2col = cp.boolean("force_nd_im2col", false);
+  const PMessage& pp = sub("pooling_param");
+  PoolingParameter& q = p.pooling_param;
+  const std::string pool = pp.str("pool", "MAX");
+  q.pool = pool == "AVE" || pool == "1" ? 1 : pool == "STOCHASTIC" || pool == "2" ? 2 : 0;
+  q.global_pooling = pp.boolean("global_pooling", false);
+  const int k = (int)pp.integer("kernel_size", 0), s = (int)pp.integer("stride", 1), pad = (int)pp.integer("pad", 0);
+  q.kernel_h = (int)pp.integer("kernel_h", k); q.kernel_w = (int)pp.integer("kernel_w", k);
+  q.stride_h = (int)pp.integer("stride_h", s); q.stride_w = (int)pp.integer("stride_w", s);
+  q.pad_h = (int)pp.integer("pad_h", pad); q.pad_w = (int)pp.integer("pad_w", pad);
+  const PMessage& ip = sub("inner_product_param");
+  p.inner_product_param.num_output = (int)ip.integer("num_output");
+  p.inner_product_param.bias_term = ip.boolean("bias_term", true);
+  p.inner_product_param.weight_filler = filler_of(ip.sub("weight_filler"));
+  p.inner_product_param.bias_filler = filler_of(ip.sub("bias_filler"));
+  const PMessage& bp = sub("batch_norm_param");
+  BatchNormParameter& bn = p.batch_norm_param;
+  bn.scale_bias = bp.boolean("scale_bias", false) || bp.has("scale_filler") || bp.has("bias_filler");
+  bn.eps = std::max((float)bp.num("eps", 1e-5), 1e-5f);
+  bn.moving_average_fraction = (float)bp.num("moving_average_fraction", 0.999);
+  if (bp.has("scale_filler")) bn.scale_filler = filler_of(bp.sub("scale_filler"));
+  if (bp.has("bias_filler")) bn.bias_filler = filler_of(bp.sub("bias_filler"));
+  p.relu_param.negative_slope = (float)sub("relu_param").num("negative_slope", 0.0);
+  const PMessage& lrn = sub("lrn_param");
+  LRNParameter& l = p.lrn_param;
+  l.local_size = (int)lrn.integer("local_size", 5); l.alpha = (float)lrn.num("alpha", 1.0); l.beta = (float)lrn.num("beta", 0.75);
+  l.k = (float)lrn.num("k", 1.0);
+  const std::string region = lrn.str("norm_region", "ACROSS_CHANNELS");
+  l.norm_region = (region == "WITHIN_CHANNEL" || region == "1") ? 1 : 0;
+  p.dropout_param.dropout_ratio = (float)sub("dropout_param").num("dropout_ratio", 0.5);
+  const std::string op = sub("eltwise_param").str("operation", "SUM");
+  p.eltwise_param.operation = (op == "PROD" || op == "0") ? 0 : (op == "MAX" || op == "2") ? 2 : 1;
+  for (auto* f : sub("eltwise_param").all("coeff")) if (!f->is_msg()) p.eltwise_param.coeff.push_back((float)std::atof(f->scalar.c_str()));
+  p.concat_param.axis = (int)sub("concat_param").integer("axis", 1);
+  const PMessage& sp = sub("slice_param");
+  B2_CHECK(!(sp.has("axis") && sp.has("slice_dim")), "Either axis or slice_dim should be specified; not both.");   // slice_layer.cpp:12-13
+  p.slice_param.slice_dim_given = sp.has("slice_dim");
+  p.slice_param.axis = (int)(sp.has("slice_dim") ? sp.integer("slice_dim") : sp.integer("axis", 1));
+  p.slice_param.slice_point = to_int(sp.ints("slice_point"));
+  p.softmax_param.axis = (int)sub("softmax_param").integer("axis", 1);
+  p.flatten_param.axis = (int)sub("flatten_param").integer("axis", 1);
+  p.flatten_param.end_axis = (int)sub("flatten_param").integer("end_axis", -1);
+  p.accuracy_param.top_k = (int)sub("accuracy_param").integer("top_k", 1);
+  p.contrastive_loss_param.margin = (float)sub("contrastive_loss_param").num("margin", 1.0);
+  p.contrastive_loss_param.legacy_version = sub("contrastive_loss_param").boolean("legacy_version", false);
+  const PMessage& tp = sub("transform_param");
+  TransformationParameter& t = p.transform_param;
+  t.crop_size = (int)tp.integer("crop_size", 0);
+  t.mirror = tp.boolean("mirror", false);
+  t.scale = (float)tp.num("scale", 1.0);
+  for (auto* f : tp.all("mean_value")) if (!f->is_msg()) t.mean_value.push_back((float)std::atof(f->scalar.c_str()));
+  t.mean_file = tp.str("mean_file");
+  t.random_seed = tp.integer("random_seed", -1);
+  const PMessage& dp = lp.sub("data_param") ? sub("data_param") : sub("image_data_param");
+  DataParameter& d = p.data_param;
+  d.batch_size = batch_override > 0 ? batch_override : (int)dp.integer("batch_size", 1);
+  d.source = dp.str("source");
+  const std::string be = dp.str("backend", "LEVELDB");
+  d.backend = (be == "LMDB" || be == "1") ? 1 : 0;
+  d.parser_threads = (int)dp.integer("parser_threads", 0);
+  d.force_encoded_color = dp.boolean("force_encoded_color", false);
+  d.cache = dp.boolean("cache", false);
+  d.shuffle = dp.boolean("shuffle", false);
+  return p;
+}
 }  // namespace
 
 int LabelBottom(const std::string& type) {
@@ -191,8 +292,19 @@ int LabelBottom(const std::string& type) {
   return type == "SoftmaxWithLoss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy" ? 1 : -1;
 }
 bool IsLossType(const std::string& ty) { return ty.size() >= 4 && ty.compare(ty.size() - 4, 4, "Loss") == 0; }
-float TopLossWeight(const NetLayer& L, size_t t) {
-  return t < L.loss_weight.size() ? L.loss_weight[t] : (IsLossType(L.param.type) && t == 0 ? 1.f : 0.f);
+float TopLossWeight(const LayerParameter& p, size_t t) {
+  return t < p.loss_weight.size() ? p.loss_weight[t] : (IsLossType(p.type) && t == 0 ? 1.f : 0.f);
+}
+float LayerBase::loss_weight() const { return TopLossWeight(layer_param_, 0); }
+int pooled_extent(int in, int k, int s, int p) {
+  int o = (int)std::ceil((float)(in + 2 * p - k) / s) + 1;
+  if (p > 0 && (o - 1) * s >= in + p) --o;
+  return o;
+}
+PoolingParameter EffectivePooling(const PoolingParameter& q, int h, int w) {
+  PoolingParameter e = q;
+  if (q.global_pooling) { e.kernel_h = h; e.kernel_w = w; e.stride_h = e.stride_w = 1; e.pad_h = e.pad_w = 0; }
+  return e;
 }
 
 Net Net::FromFile(const std::string& path, Phase phase, int batch_override) {
@@ -234,29 +346,14 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
     const PMessage& lp = *lf->msg;
     if (!layer_included(lp, phase)) continue;
     NetLayer L;
-    L.param.name = lp.str("name");
-    L.param.type = lp.str("type");
-    for (const PField* f : lp.all("loss_weight")) L.loss_weight.push_back((float)std::atof(f->scalar.c_str()));
-    for (auto* b : lp.all("bottom")) L.param.bottom.push_back(b->scalar);
-    for (auto* t : lp.all("top")) L.param.top.push_back(t->scalar);
-    for (auto* ps : lp.all("param")) {
-      ParamSpec s;
-      if (ps->is_msg()) {
-        const PMessage& m = *ps->msg;
-        s.lr_mult = (float)m.num("lr_mult", 1.0); s.decay_mult = (float)m.num("decay_mult", 1.0);
-        s.has_lr_mult = m.has("lr_mult"); s.has_decay_mult = m.has("decay_mult");
-        s.name = m.str("name");
-        const std::string sm = m.str("share_mode", "STRICT");
-        s.share_mode = (sm == "PERMISSIVE" || sm == "1") ? 1 : 0;
-      }
-      L.param.param.push_back(s);
-    }
-    const std::string& type = L.param.type;
+    L.param = read_layer(lp, phase, batch_override);
+    LayerParameter& P = L.param;
+    const std::string& type = P.type;
     const int id = (int)layers_.size();
     auto bottom_shape = [&](int i) -> const std::vector<int>& {
-      B2_CHECK(i < (int)L.param.bottom.size(), "layer " + L.param.name + " has too few bottoms");
-      auto it = shapes_.find(L.param.bottom[i]);
-      if (it == shapes_.end()) Fatal(__FILE__, __LINE__, "Unknown bottom blob '" + L.param.bottom[i] + "' (layer '" + L.param.name + "')");
+      B2_CHECK(i < (int)P.bottom.size(), "layer " + P.name + " has too few bottoms");
+      auto it = shapes_.find(P.bottom[i]);
+      if (it == shapes_.end()) Fatal(__FILE__, __LINE__, "Unknown bottom blob '" + P.bottom[i] + "' (layer '" + P.name + "')");
       return it->second;
     };
     std::vector<std::vector<int>> tops;
@@ -265,43 +362,26 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
 
     if (type == "Data" || type == "ImageData" || type == "HDF5Data") {
       is_data = true;
-      const PMessage* dp = lp.sub("data_param");
-      if (!dp) dp = lp.sub("image_data_param");
-      const PMessage* tp = lp.sub("transform_param");
-      L.batch_size = batch_override > 0 ? batch_override : (int)(dp ? dp->integer("batch_size", 1) : 1);
-      L.crop_size = (int)(tp ? tp->integer("crop_size", 0) : 0);
-      if (tp) {
-        L.has_transform = true;
-        L.mirror = tp->boolean("mirror", false);
-        L.transform_scale = (float)tp->num("scale", 1.0);
-        for (auto* f : tp->all("mean_value")) if (!f->is_msg()) L.mean_value.push_back((float)std::atof(f->scalar.c_str()));
-      }
+      const DataParameter& dp = P.data_param;
+      const int crop = P.transform_param.crop_size;
       int dc = default_channels, dh = default_size, dw = default_size;
-      if (type == "Data" && dp) {
-        L.data_source = dp->str("source");
-        const std::string be = dp->str("backend", "LEVELDB");
-        L.data_backend = (be == "LMDB" || be == "1") ? 1 : 0;
-        L.parser_threads = (int)dp->integer("parser_threads", 0);
-        L.force_encoded_color = dp->boolean("force_encoded_color", false);
-        L.data_cache = dp->boolean("cache", false);
-        L.data_shuffle = dp->boolean("shuffle", false);
-        if (tp) { L.mean_file = tp->str("mean_file"); L.transform_random_seed = tp->integer("random_seed", -1); }
+      if (type == "Data") {
         // DataLayerSetUp reads one datum to size the top blob (data_layer.cpp:176-183); so does this, when the database is there
-        L.use_database = UseDatabase(L.data_source, L.data_backend);
-        if (L.use_database) PeekDatumShape(L.data_source, &dc, &dh, &dw, L.force_encoded_color);
+        L.use_database = UseDatabase(dp.source, dp.backend);
+        if (L.use_database) PeekDatumShape(dp.source, &dc, &dh, &dw, dp.force_encoded_color);
       }
-      if (L.crop_size > 0) {
-        if (L.use_database) B2_CHECK(dh >= L.crop_size && dw >= L.crop_size, "crop_size larger than the datums of " + L.data_source);
-        dh = dw = L.crop_size;
+      if (crop > 0) {
+        if (L.use_database) B2_CHECK(dh >= crop && dw >= crop, "crop_size larger than the datums of " + dp.source);
+        dh = dw = crop;
       }
-      tops.push_back({L.batch_size, dc, dh, dw});
-      tops.push_back({L.batch_size});
+      tops.push_back({dp.batch_size, dc, dh, dw});
+      tops.push_back({dp.batch_size});
     } else if (type == "Input" || type == "DummyData") {
       is_data = true;
       const PMessage* ip = lp.sub(type == "Input" ? "input_param" : "dummy_data_param");
       B2_CHECK(ip != nullptr, type + " layer needs its parameter message");
       const auto shp = ip->all("shape");
-      for (size_t i = 0; i < L.param.top.size(); ++i) {
+      for (size_t i = 0; i < P.top.size(); ++i) {
         B2_CHECK(!shp.empty(), "Input layer needs shape");
         const PField* sf = shp[std::min(i, shp.size() - 1)];
         B2_CHECK(sf->is_msg(), type + " layer: `shape` must be a message { dim: ... }");
@@ -312,20 +392,7 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
     } else if (type == "Convolution") {
       const PMessage* cp = lp.sub("convolution_param");
       B2_CHECK(cp != nullptr, "Convolution layer without convolution_param");
-      ConvolutionParameter& c = L.param.convolution_param;
-      c.num_output = (int)cp->integer("num_output");
-      c.bias_term = cp->boolean("bias_term", true);
-      c.pad = to_int(cp->ints("pad")); c.kernel_size = to_int(cp->ints("kernel_size"));
-      c.stride = to_int(cp->ints("stride")); c.dilation = to_int(cp->ints("dilation"));
-      if (cp->has("pad_h")) c.pad_h = (int)cp->integer("pad_h"); if (cp->has("pad_w")) c.pad_w = (int)cp->integer("pad_w");
-      if (cp->has("kernel_h")) c.kernel_h = (int)cp->integer("kernel_h"); if (cp->has("kernel_w")) c.kernel_w = (int)cp->integer("kernel_w");
-      if (cp->has("stride_h")) c.stride_h = (int)cp->integer("stride_h"); if (cp->has("stride_w")) c.stride_w = (int)cp->integer("stride_w");
-      c.group = (int)cp->integer("group", 1);
-      c.weight_filler = filler_of(cp->sub("weight_filler"));
-      c.bias_filler = filler_of(cp->sub("bias_filler"));
-      c.engine = engine_of(cp->str("engine", "DEFAULT"));
-      c.axis = (int)cp->integer("axis", 1);
-      c.force_nd_im2col = cp->boolean("force_nd_im2col", false);
+      const ConvolutionParameter& c = P.convolution_param;
       const std::vector<int>& bs = bottom_shape(0);
       B2_CHECK(bs.size() == 4, "2-D convolution expects a 4-D bottom");
       auto ax = [&](const std::vector<int>& rep, int hv, int wv, int dflt, int which) {
@@ -350,89 +417,66 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       tops.push_back({p.N, p.O, Ho, Wo});
       blobs.push_back({{p.O, p.C / p.G, p.kh, p.kw}, 0});
       if (c.bias_term) blobs.push_back({{p.O}, 1});
-      const bool pd = need_bw.count(L.param.bottom[0]) ? need_bw[L.param.bottom[0]] : false;   // net.cpp:183-191,278-283
-      convs_.push_back(ConvEntry{L.param.name, id, p, pd});
+      convs_.push_back(ConvEntry{P.name, id, p, false});   // propagate_down: set once need-backward is final, below
     } else if (type == "Pooling") {
-      const PMessage* pp = lp.sub("pooling_param");
       const std::vector<int>& bs = bottom_shape(0);
       B2_CHECK(bs.size() == 4, "Pooling expects a 4-D bottom (num, channels, height, width)");   // pooling_layer.cpp:84-86
-      PoolingParameter& q = L.pooling;
-      if (pp) {
-        const std::string pool = pp->str("pool", "MAX");
-        q.pool = pool == "AVE" || pool == "1" ? 1 : pool == "STOCHASTIC" || pool == "2" ? 2 : 0;
-        q.global_pooling = pp->boolean("global_pooling", false);
-        const int k = (int)pp->integer("kernel_size", 0), s = (int)pp->integer("stride", 1), p = (int)pp->integer("pad", 0);
-        q.kernel_h = pp->has("kernel_h") ? (int)pp->integer("kernel_h") : k; q.kernel_w = pp->has("kernel_w") ? (int)pp->integer("kernel_w") : k;
-        q.stride_h = pp->has("stride_h") ? (int)pp->integer("stride_h") : s; q.stride_w = pp->has("stride_w") ? (int)pp->integer("stride_w") : s;
-        q.pad_h = pp->has("pad_h") ? (int)pp->integer("pad_h") : p; q.pad_w = pp->has("pad_w") ? (int)pp->integer("pad_w") : p;
-      }
-      if (q.global_pooling) { q.kernel_h = bs[2]; q.kernel_w = bs[3]; q.stride_h = q.stride_w = 1; q.pad_h = q.pad_w = 0; }
+      PoolingParameter& q = P.pooling_param;
+      q = EffectivePooling(q, bs[2], bs[3]);
       B2_CHECK(q.kernel_h > 0 && q.kernel_w > 0, "Filter dimensions cannot be zero.");
       B2_CHECK(q.stride_h > 0 && q.stride_w > 0 && q.pad_h >= 0 && q.pad_w >= 0, "Pooling stride must be positive and pad non-negative");
       tops.push_back({bs[0], bs[1], pooled_extent(bs[2], q.kernel_h, q.stride_h, q.pad_h), pooled_extent(bs[3], q.kernel_w, q.stride_w, q.pad_w)});
     } else if (type == "InnerProduct") {
       const PMessage* ip = lp.sub("inner_product_param");
       B2_CHECK(ip != nullptr, "InnerProduct layer without inner_product_param");
-      L.ip_num_output = (int)ip->integer("num_output");
-      L.ip_bias = ip->boolean("bias_term", true);
-      L.ip_weight_filler = filler_of(ip->sub("weight_filler"));
-      L.ip_bias_filler = filler_of(ip->sub("bias_filler"));
+      const InnerProductParameter& q = P.inner_product_param;
       const std::vector<int>& bs = bottom_shape(0);
-      B2_CHECK(bs.size() >= 2 && L.ip_num_output > 0, "InnerProduct needs a bottom with at least 2 axes and a positive num_output");
-      const int K = (int)prod(bs, 1);
-      tops.push_back({bs[0], L.ip_num_output});
-      blobs.push_back({{L.ip_num_output, K}, 0});
-      if (L.ip_bias) blobs.push_back({{L.ip_num_output}, 1});
+      B2_CHECK(bs.size() >= 2 && q.num_output > 0, "InnerProduct needs a bottom with at least 2 axes and a positive num_output");
+      tops.push_back({bs[0], q.num_output});
+      blobs.push_back({{q.num_output, (int)prod(bs, 1)}, 0});
+      if (q.bias_term) blobs.push_back({{q.num_output}, 1});
     } else if (type == "BatchNorm") {
-      const PMessage* bp = lp.sub("batch_norm_param");
-      L.bn_scale_bias = bp ? (bp->boolean("scale_bias", false) || bp->has("scale_filler") || bp->has("bias_filler")) : false;
-      if (bp) { L.bn_eps = std::max((float)bp->num("eps", 1e-5), 1e-5f); L.bn_maf = (float)bp->num("moving_average_fraction", 0.999); }
-      if (bp && bp->has("scale_filler")) { L.bn_scale_filler = filler_of(bp->sub("scale_filler")); L.bn_has_scale_filler = true; }
-      if (bp && bp->has("bias_filler")) { L.bn_bias_filler = filler_of(bp->sub("bias_filler")); L.bn_has_bias_filler = true; }
       const std::vector<int>& bs = bottom_shape(0);
       B2_CHECK(bs.size() >= 2, "BatchNorm needs a bottom with a channel axis");
       tops.push_back(bs);
       // blobs_[0..2] = running mean / variance / correction (statistics, not exchanged with the cuDNN engine:
       // include/caffe/layers/cudnn_batch_norm_layer.hpp:30-32); [3], [4] = scale, bias when scale_bias
-      if (L.bn_scale_bias) { blobs.push_back({{bs[1]}, 3}); blobs.push_back({{bs[1]}, 4}); }
+      if (P.batch_norm_param.scale_bias) { blobs.push_back({{bs[1]}, 3}); blobs.push_back({{bs[1]}, 4}); }
     } else if (type == "Scale") {
       const PMessage* sp = lp.sub("scale_param");
       const std::vector<int>& bs = bottom_shape(0);
       B2_CHECK(bs.size() >= 2, "Scale needs a bottom with a channel axis");
       tops.push_back(bs);
-      if (L.param.bottom.size() == 1) {
+      if (P.bottom.size() == 1) {
         blobs.push_back({{bs[1]}, 0});
         if (sp && sp->boolean("bias_term", false)) blobs.push_back({{bs[1]}, 1});
       }
     } else if (type == "Concat") {
-      const PMessage* cp = lp.sub("concat_param");
-      L.concat_axis = cp ? (int)cp->integer("axis", 1) : 1;
+      const int axis = P.concat_param.axis;
       std::vector<int> s = bottom_shape(0);
-      B2_CHECK(L.concat_axis >= 0 && L.concat_axis < (int)s.size(), "Concat: axis outside the bottom's axes");
-      for (size_t i = 1; i < L.param.bottom.size(); ++i) {
+      B2_CHECK(axis >= 0 && axis < (int)s.size(), "Concat: axis outside the bottom's axes");
+      for (size_t i = 1; i < P.bottom.size(); ++i) {
         const std::vector<int>& b = bottom_shape((int)i);
         B2_CHECK(b.size() == s.size(), "Concat: all inputs must have the same #axes.");
-        s[L.concat_axis] += b[L.concat_axis];
+        s[axis] += b[axis];
       }
       tops.push_back(s);
     } else if (type == "Flatten") {
-      const PMessage* fp = lp.sub("flatten_param");
+      FlattenParameter& f = P.flatten_param;
       const std::vector<int>& bs = bottom_shape(0);
-      B2_CHECK(L.param.top.empty() || L.param.top[0] != L.param.bottom[0], "Flatten Layer does not allow in-place computation.");
-      L.flatten_axis = canonical_axis(fp ? (int)fp->integer("axis", 1) : 1, bs);                // flatten_layer.cpp:8-30
-      L.flatten_end_axis = canonical_axis(fp ? (int)fp->integer("end_axis", -1) : -1, bs);
-      std::vector<int> s(bs.begin(), bs.begin() + L.flatten_axis);
+      B2_CHECK(P.top.empty() || P.top[0] != P.bottom[0], "Flatten Layer does not allow in-place computation.");
+      f.axis = canonical_axis(f.axis, bs);                                                          // flatten_layer.cpp:8-30
+      f.end_axis = canonical_axis(f.end_axis, bs);
+      std::vector<int> s(bs.begin(), bs.begin() + f.axis);
       int flat = 1;
-      for (int a = L.flatten_axis; a <= L.flatten_end_axis; ++a) flat *= bs[a];
+      for (int a = f.axis; a <= f.end_axis; ++a) flat *= bs[a];
       s.push_back(flat);
-      for (int a = L.flatten_end_axis + 1; a < (int)bs.size(); ++a) s.push_back(bs[a]);
+      for (int a = f.end_axis + 1; a < (int)bs.size(); ++a) s.push_back(bs[a]);
       tops.push_back(s);
     } else if (type == "Softmax") {
-      const PMessage* sp = lp.sub("softmax_param");
-      L.softmax_axis = canonical_axis(sp ? (int)sp->integer("axis", 1) : 1, bottom_shape(0));   // softmax_layer.cpp:12-13
+      P.softmax_param.axis = canonical_axis(P.softmax_param.axis, bottom_shape(0));                 // softmax_layer.cpp:12-13
       tops.push_back(bottom_shape(0));
     } else if (type == "SoftmaxWithLoss" || type == "EuclideanLoss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy") {
-      if (const PMessage* ap = lp.sub("accuracy_param")) L.accuracy_top_k = (int)ap->integer("top_k", 1);
       if (type == "EuclideanLoss" || type == "SigmoidCrossEntropyLoss") {
         const std::vector<int>& a = bottom_shape(0);
         const std::vector<int>& b = bottom_shape(1);
@@ -440,22 +484,20 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
         if (type == "EuclideanLoss") B2_CHECK(prod(a, 1) == prod(b, 1), "Inputs must have the same dimension.");
         else B2_CHECK(prod(a) == prod(b), "SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.");
       }
-      for (size_t i = 0; i < L.param.top.size(); ++i) tops.push_back({});
+      for (size_t i = 0; i < P.top.size(); ++i) tops.push_back({});
     } else if (type == "Slice") {
-      const PMessage* sp = lp.sub("slice_param");
+      SliceParameter& sp = P.slice_param;
       const std::vector<int> bs = bottom_shape(0);
-      const size_t ntop = L.param.top.size();
+      const size_t ntop = P.top.size();
       B2_CHECK(ntop >= 1, "Slice layer needs at least one top");
-      B2_CHECK(!(sp && sp->has("axis") && sp->has("slice_dim")), "Either axis or slice_dim should be specified; not both.");   // slice_layer.cpp:12-13
-      if (sp && sp->has("slice_dim")) {                                                                                   // :26-33
-        L.slice_axis = (int)sp->integer("slice_dim");
-        B2_CHECK(L.slice_axis >= 0, "casting slice_dim from uint32 to int32 produced negative result; slice_dim must satisfy 0 <= slice_dim < 32");
-        B2_CHECK(L.slice_axis < (int)bs.size(), "slice_dim out of range.");
+      if (sp.slice_dim_given) {                                                                                          // slice_layer.cpp:26-33
+        B2_CHECK(sp.axis >= 0, "casting slice_dim from uint32 to int32 produced negative result; slice_dim must satisfy 0 <= slice_dim < 32");
+        B2_CHECK(sp.axis < (int)bs.size(), "slice_dim out of range.");
       } else {
-        L.slice_axis = canonical_axis(sp ? (int)sp->integer("axis", 1) : 1, bs);
+        sp.axis = canonical_axis(sp.axis, bs);
       }
-      const int extent = bs[L.slice_axis];
-      const std::vector<int> points = sp ? to_int(sp->ints("slice_point")) : std::vector<int>();
+      const int extent = bs[sp.axis];
+      const std::vector<int>& points = sp.slice_point;
       std::vector<int> slices;
       if (!points.empty()) {                                                                                              // :40-56
         if (points.size() != ntop - 1)
@@ -480,7 +522,7 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       }
       for (int s : slices) {
         std::vector<int> t = bs;
-        t[L.slice_axis] = s;
+        t[sp.axis] = s;
         tops.push_back(t);
       }
     } else if (type == "ContrastiveLoss") {
@@ -506,34 +548,14 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       B2_CHECK(!a.empty() && !b.empty() && a[0] == b[0], "The data and label should have the same number.");     // loss_layer.cpp:19-20
       // not in the reference, which reads bottom[2][i] for every pair without checking: one label per pair
       B2_CHECK(!y.empty() && y[0] == a[0], "ContrastiveLoss: the similarity blob needs one label per pair");
-      if (const PMessage* cp = lp.sub("contrastive_loss_param")) {
-        L.contrastive_margin = (float)cp->num("margin", 1.0);
-        L.contrastive_legacy = cp->boolean("legacy_version", false);
-      }
-      for (size_t i = 0; i < L.param.top.size(); ++i) tops.push_back({});
-    } else if (type == "ReLU" && (L.relu_slope = (float)(lp.sub("relu_param") ? lp.sub("relu_param")->num("negative_slope", 0.0) : 0.0), false)) {
-    } else if ((type == "LRN" || type == "Dropout") && ([&] {
-                 if (const PMessage* q = lp.sub("lrn_param")) {
-                   L.lrn_size = (int)q->integer("local_size", 5); L.lrn_alpha = (float)q->num("alpha", 1.0); L.lrn_beta = (float)q->num("beta", 0.75);
-                   L.lrn_k = (float)q->num("k", 1.0);
-                   const std::string r = q->str("norm_region", "ACROSS_CHANNELS");
-                   L.lrn_region = (r == "WITHIN_CHANNEL" || r == "1") ? 1 : 0;
-                 }
-                 if (const PMessage* q = lp.sub("dropout_param")) L.dropout_ratio = (float)q->num("dropout_ratio", 0.5);
-               }(), false)) {
-    } else if (type == "Eltwise" && ([&] {
-                 if (const PMessage* q = lp.sub("eltwise_param")) {
-                   const std::string op = q->str("operation", "SUM");
-                   L.eltwise_op = (op == "PROD" || op == "0") ? 0 : (op == "MAX" || op == "2") ? 2 : 1;
-                   for (auto* f : q->all("coeff")) if (!f->is_msg()) L.eltwise_coeff.push_back((float)std::atof(f->scalar.c_str()));
-                 }
-               }(), false)) {
+      for (size_t i = 0; i < P.top.size(); ++i) tops.push_back({});
     } else if (type == "ReLU" || type == "Dropout" || type == "LRN" || type == "Eltwise" || type == "Sigmoid" ||
                type == "TanH" || type == "Power" || type == "Bias" || type == "ELU" || type == "PReLU" || type == "Split") {
-      for (size_t i = 0; i < std::max<size_t>(1, L.param.top.size()); ++i) tops.push_back(bottom_shape(0));
+      for (size_t i = 0; i < std::max<size_t>(1, P.top.size()); ++i) tops.push_back(bottom_shape(0));
     } else {
-      Fatal(__FILE__, __LINE__, "Unknown layer type: " + type + " (layer '" + L.param.name + "')");
+      Fatal(__FILE__, __LINE__, "Unknown layer type: " + type + " (layer '" + P.name + "')");
     }
+
 
     // need-backward analysis (Net::Init, net.cpp:160-283): data tops never need it; a layer needs backward if a
     // bottom does or it owns a parameter with a non-zero lr_mult
@@ -625,7 +647,7 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
     NetLayer& L = layers_[li];
     bool contributes = false;
     for (size_t t = 0; t < L.param.top.size(); ++t)
-      contributes |= TopLossWeight(L, t) != 0.f || under_loss.count(L.param.top[t]) > 0;
+      contributes |= TopLossWeight(L.param, t) != 0.f || under_loss.count(L.param.top[t]) > 0;
     if (!contributes) {
       L.need_backward = false;
       L.label_wants_gradient = false;
@@ -647,7 +669,7 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
   }
   for (ConvEntry& c : convs_) c.propagate_down = layers_[c.layer_id].propagate_down[0];
   for (const NetLayer& L : layers_)
-    if (IsLossType(L.param.type) && !L.param.top.empty() && TopLossWeight(L, 0) != 0.f) loss_blob_ = L.param.top[0];
+    if (IsLossType(L.param.type) && !L.param.top.empty() && TopLossWeight(L.param, 0) != 0.f) loss_blob_ = L.param.top[0];
 }
 
 // ================================================================================================ solver

@@ -41,45 +41,9 @@ PMessage ParseTextProto(const std::string& text);        // throws FatalError wi
 PMessage ParseTextProtoFile(const std::string& path);
 
 // ---- net description --------------------------------------------------------------------------------------------
-enum Phase { TRAIN = 0, TEST = 1 };
-
-struct PoolingParameter { int pool = 0, kernel_h = 0, kernel_w = 0, stride_h = 1, stride_w = 1, pad_h = 0, pad_w = 0; bool global_pooling = false; };
-
 struct NetLayer {                       // one LayerParameter after phase filtering
-  LayerParameter param;                 // name, type, bottom, top, ParamSpecs, convolution_param
-  PoolingParameter pooling;
-  int ip_num_output = 0;
-  bool ip_bias = true;
-  bool bn_scale_bias = false;           // NVCaffe BatchNormParameter.scale_bias
-  float bn_eps = 1e-5f, bn_maf = 0.999f; // BatchNormParameter.eps / moving_average_fraction
-  FillerParameter ip_weight_filler, ip_bias_filler;
-  float relu_slope = 0.f;
-  int eltwise_op = 1;                   // EltwiseParameter.operation: PROD = 0, SUM = 1, MAX = 2
-  std::vector<float> eltwise_coeff;
-  FillerParameter bn_scale_filler, bn_bias_filler; bool bn_has_scale_filler = false, bn_has_bias_filler = false;
-  int lrn_size = 5; float lrn_alpha = 1.f, lrn_beta = 0.75f, lrn_k = 1.f; int lrn_region = 0;   // LRNParameter (caffe.proto:1039-1055)
-  float dropout_ratio = 0.5f;           // DropoutParameter.dropout_ratio
-  std::vector<float> loss_weight;        // LayerParameter.loss_weight (one per top)
-  int concat_axis = 1;
-  int accuracy_top_k = 1;               // AccuracyParameter.top_k
-  int batch_size = 0, crop_size = 0;    // Data layers
-  bool has_transform = false, mirror = false;   // TransformationParameter (caffe.proto:436-470)
-  float transform_scale = 1.f;
-  std::vector<float> mean_value;
-  // DataParameter / TransformationParameter fields the database-backed DataLayer reads (caffe.proto:436-470, 806-849)
-  std::string data_source, mean_file;
-  int data_backend = 0;                 // DataParameter.DB: LEVELDB = 0 (the proto's default), LMDB = 1
-  int parser_threads = 0;               // 0 = automatic in the reference; one parser thread here
-  bool force_encoded_color = false;     // DataParameter.force_encoded_color
-  bool data_cache = false, data_shuffle = false;   // DataParameter.cache / shuffle (accepted; see DataLayer::LayerSetUp)
-  long long transform_random_seed = -1; // TransformationParameter.random_seed
-  bool use_database = false;            // the source opened: this layer reads it (else the synthetic in-memory source stands in)
-  std::vector<int> input_shape;         // Input / DummyData layers
-  int softmax_axis = 1;                 // SoftmaxParameter.axis, canonicalised against the bottom's axes
-  int flatten_axis = 1, flatten_end_axis = -1;   // FlattenParameter.axis / end_axis, canonicalised
-  int slice_axis = 1;                   // SliceParameter.axis (canonicalised) or slice_dim; the tops' shapes carry the split
-  float contrastive_margin = 1.f;       // ContrastiveLossParameter.margin / legacy_version (caffe.proto)
-  bool contrastive_legacy = false;
+  LayerParameter param;
+  bool use_database = false;            // a Data layer whose source opened: it reads it (else the synthetic in-memory source stands in)
   // Net::Init's need-backward result (net.cpp:160-330), loss pruning included: whether the layer runs backward, and per bottom
   // whether it receives a gradient.  TrainNet reads these; nothing else restates the rule.
   bool need_backward = false;
@@ -94,7 +58,11 @@ int LabelBottom(const std::string& type);
 bool IsLossType(const std::string& type);
 // LayerParameter.loss_weight of top t, defaulting as Layer::SetLossWeights / LossLayer::LayerSetUp do: 1 for the first top of a
 // layer whose type ends in "Loss", 0 otherwise
-float TopLossWeight(const NetLayer& L, size_t t);
+float TopLossWeight(const LayerParameter& p, size_t t);
+// PoolingLayer::Reshape's output extent: ceil mode, and the last window clipped when it would start in the padding
+int pooled_extent(int in, int k, int s, int p);
+// q over an h x w bottom: global_pooling makes the whole plane one window (stride 1, no padding)
+PoolingParameter EffectivePooling(const PoolingParameter& q, int h, int w);
 
 // One parameter blob of a layer.  blob_id counts the layer's learnable blobs; layer_blob is its index among the layer's blobs
 // (BatchNorm's scale / bias are blobs 3 and 4).  Named blobs are shared (Net::AppendParam, net.cpp:576-666): the first blob with

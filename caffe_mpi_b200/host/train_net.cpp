@@ -10,16 +10,20 @@
 namespace caffe {
 
 static cudaStream_t S() { return Caffe::thread_stream(); }
+static bool env_on(const char* name, bool dflt) {        // a 0 / 1 switch from the environment
+  const char* e = getenv(name);
+  return e ? atoi(e) != 0 : dflt;
+}
 
 // ================================================================================================ ReLU
 void ReLULayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   if (fused_away_) return;
-  B2C_CHECK(b2c_relu_forward(b[0]->count(), b[0]->gpu_data(), t[0]->mutable_gpu_data(), slope_, S()));
+  B2C_CHECK(b2c_relu_forward(b[0]->count(), b[0]->gpu_data(), t[0]->mutable_gpu_data(), negative_slope(), S()));
 }
 void ReLULayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
   if (!pd[0] || fused_away_) return;
   // in place: bottom data == top data (post-activation), same (x > 0) mask for slope 0 (relu_layer.cpp:27-41)
-  B2C_CHECK(b2c_relu_backward(b[0]->count(), t[0]->gpu_diff(), b[0]->gpu_data(), b[0]->mutable_gpu_diff(), slope_, S()));
+  B2C_CHECK(b2c_relu_backward(b[0]->count(), t[0]->gpu_diff(), b[0]->gpu_data(), b[0]->mutable_gpu_diff(), negative_slope(), S()));
 }
 
 // ================================================================================================ BatchNorm
@@ -32,8 +36,8 @@ void BatchNormLayer::LayerSetUp(const vector<Blob*>& b, const vector<Blob*>&) {
   if (scale_bias_) {
     blobs_[3].reset(new Blob(vector<int>{C}));
     blobs_[4].reset(new Blob(vector<int>{C}));
-    Fill(scale_filler_, blobs_[3].get());         // defaults: scale = 1, bias = 0 (batch_norm_layer.cpp:52-63)
-    Fill(bias_filler_, blobs_[4].get());
+    Fill(layer_param_.batch_norm_param.scale_filler, blobs_[3].get());   // batch_norm_layer.cpp:52-63
+    Fill(layer_param_.batch_norm_param.bias_filler, blobs_[4].get());
   }
   param_propagate_down_.assign(blobs_.size(), false);
   if (scale_bias_) param_propagate_down_[3] = param_propagate_down_[4] = true;
@@ -41,12 +45,12 @@ void BatchNormLayer::LayerSetUp(const vector<Blob*>& b, const vector<Blob*>&) {
 void BatchNormLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
   if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]);
   const int C = b[0]->shape(1);
-  if (!test_ && !(recompute_ && t[0] != b[0])) xnorm_.ReshapeLike(*b[0]);
+  if (layer_param_.phase != TEST && !(recompute_ && t[0] != b[0])) xnorm_.ReshapeLike(*b[0]);
   save_mean_.Reshape({C}); save_invstd_.Reshape({C}); scratch_.Reshape({2 * C});
 }
 void BatchNormLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   const int N = b[0]->shape(0), C = b[0]->shape(1), Sp = (int)(b[0]->count() / ((size_t)N * C));
-  if (test_) {
+  if (layer_param_.phase == TEST) {
     // TEST: normalise with the running statistics (batch_norm_layer.cu:22-34), [+ the residual tail's other operand], [ReLU]
     B2C_CHECK(b2c_bn_forward_inference(N, C, Sp, b[0]->gpu_data(), scale_bias_ ? blobs_[3]->gpu_data() : nullptr,
                                        scale_bias_ ? blobs_[4]->gpu_data() : nullptr, eps_, blobs_[0]->gpu_data(), blobs_[1]->gpu_data(),
@@ -103,16 +107,10 @@ void BatchNormLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>&, c
 
 // ================================================================================================ Pooling
 PoolingLayer::~PoolingLayer() { if (mask_) cudaFree(mask_); }
-static int pooled(int in, int k, int s, int p) {
-  int o = (int)std::ceil((float)(in + 2 * p - k) / s) + 1;
-  if (p > 0 && (o - 1) * s >= in + p) --o;
-  return o;
-}
 void PoolingLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
-  eff_ = q_;
-  if (q_.global_pooling) { eff_.kernel_h = b[0]->shape(2); eff_.kernel_w = b[0]->shape(3); eff_.stride_h = eff_.stride_w = 1; eff_.pad_h = eff_.pad_w = 0; }
-  t[0]->Reshape({b[0]->shape(0), b[0]->shape(1), pooled(b[0]->shape(2), eff_.kernel_h, eff_.stride_h, eff_.pad_h),
-                 pooled(b[0]->shape(3), eff_.kernel_w, eff_.stride_w, eff_.pad_w)});
+  eff_ = EffectivePooling(layer_param_.pooling_param, b[0]->shape(2), b[0]->shape(3));
+  t[0]->Reshape({b[0]->shape(0), b[0]->shape(1), pooled_extent(b[0]->shape(2), eff_.kernel_h, eff_.stride_h, eff_.pad_h),
+                 pooled_extent(b[0]->shape(3), eff_.kernel_w, eff_.stride_w, eff_.pad_w)});
   if (eff_.pool == 0 && t[0]->count() > mask_cap_) {
     if (mask_) CUDA_CHECK(cudaFree(mask_));
     CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&mask_), sizeof(int) * t[0]->count()));
@@ -157,8 +155,8 @@ void InnerProductLayer::LayerSetUp(const vector<Blob*>& b, const vector<Blob*>&)
   K_ = (int)b[0]->count(1);
   blobs_.resize(bias_ ? 2 : 1);
   blobs_[0].reset(new Blob(vector<int>{num_output_, K_}));
-  Fill(wf_, blobs_[0].get());
-  if (bias_) { blobs_[1].reset(new Blob(vector<int>{num_output_})); Fill(bf_, blobs_[1].get()); }
+  Fill(layer_param_.inner_product_param.weight_filler, blobs_[0].get());
+  if (bias_) { blobs_[1].reset(new Blob(vector<int>{num_output_})); Fill(layer_param_.inner_product_param.bias_filler, blobs_[1].get()); }
   param_propagate_down_.assign(blobs_.size(), true);
 }
 void InnerProductLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
@@ -168,8 +166,7 @@ void InnerProductLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) 
   const size_t wsb = b2c_sgemm_workspace_bytes(0, 1, M_, num_output_, K_);
   if (wsb) gemm_ws_.Reshape({(int)((wsb + 3) / 4)});
   // backward: dW = dy^T[N x M] * (x^T[K x M])^T (reduction over the batch), dx = dy[M x N] * (W^T[K x N])^T (reduction over the outputs)
-  const char* e = getenv("B2C_IP_BWD_TC");
-  const bool on = !e || atoi(e) != 0;
+  const bool on = env_on("B2C_IP_BWD_TC", true);
   // dW: the reduction runs over the batch -- only a few K blocks per 128 x 128 output tile unless the batch is large; on AlexNet
   // (batch 256, 4096 x 9216 outputs) the tile set-up and the read-modify-write epilogue cost more than the FFMA kernel saves,
   // so the batch has to be at least 512
@@ -217,22 +214,24 @@ void InnerProductLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>&
 
 // ================================================================================================ LRN / Dropout / Concat
 void LRNLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  const LRNParameter& q = layer_param_.lrn_param;
   const int N = b[0]->shape(0), C = b[0]->shape(1), Sp = (int)(b[0]->count() / ((size_t)N * C));
-  B2C_CHECK(b2c_lrn_forward(N, C, Sp, size_, alpha_, beta_, k_, b[0]->gpu_data(), scale_.mutable_gpu_data(), t[0]->mutable_gpu_data(), S()));
+  B2C_CHECK(b2c_lrn_forward(N, C, Sp, q.local_size, q.alpha, q.beta, q.k, b[0]->gpu_data(), scale_.mutable_gpu_data(), t[0]->mutable_gpu_data(), S()));
 }
 void LRNLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
   if (!pd[0]) return;
+  const LRNParameter& q = layer_param_.lrn_param;
   const int N = b[0]->shape(0), C = b[0]->shape(1), Sp = (int)(b[0]->count() / ((size_t)N * C));
-  B2C_CHECK(b2c_lrn_backward(N, C, Sp, size_, alpha_, beta_, b[0]->gpu_data(), t[0]->gpu_data(), scale_.gpu_data(), t[0]->gpu_diff(),
+  B2C_CHECK(b2c_lrn_backward(N, C, Sp, q.local_size, q.alpha, q.beta, b[0]->gpu_data(), t[0]->gpu_data(), scale_.gpu_data(), t[0]->gpu_diff(),
                              b[0]->mutable_gpu_diff(), S()));
 }
 void DropoutLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
-  if (test_) {                               // TEST: the identity (dropout_layer.cu); no mask is drawn and the stream offset stays
+  if (layer_param_.phase == TEST) {          // TEST: the identity (dropout_layer.cu); no mask is drawn and the stream offset stays
     if (t[0] != b[0])
       CUDA_CHECK(cudaMemcpyAsync(t[0]->mutable_gpu_data(), b[0]->gpu_data(), sizeof(float) * b[0]->count(), cudaMemcpyDeviceToDevice, S()));
     return;
   }
-  B2C_CHECK(b2c_dropout_mask(b[0]->count(), ratio_, seed_, offset_, mask_.mutable_gpu_data(), S()));
+  B2C_CHECK(b2c_dropout_mask(b[0]->count(), layer_param_.dropout_param.dropout_ratio, seed_, offset_, mask_.mutable_gpu_data(), S()));
   offset_ += b[0]->count();
   B2C_CHECK(b2c_mul(b[0]->count(), b[0]->gpu_data(), mask_.gpu_data(), t[0]->mutable_gpu_data(), S()));
 }
@@ -281,10 +280,10 @@ void SliceLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
   }
   B2_CHECK(count == b[0]->count(), "Slice: the tops do not cover the bottom");   // slice_layer.cpp:65
 }
-void SliceLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) { axis_copy(b[0], t, axis_, false, false, nullptr); }
+void SliceLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) { axis_copy(b[0], t, layer_param_.slice_param.axis, false, false, nullptr); }
 void SliceLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
   if (!pd[0]) return;
-  axis_copy(b[0], t, axis_, true, true, nullptr);
+  axis_copy(b[0], t, layer_param_.slice_param.axis, true, true, nullptr);
 }
 
 // ================================================================================================ SoftmaxWithLoss
@@ -298,7 +297,7 @@ void SoftmaxWithLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob
 }
 void SoftmaxWithLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
   if (!pd[0]) return;
-  B2C_CHECK(b2c_softmax_loss_backward(b[0]->shape(0), (int)b[0]->count(1), prob_.gpu_data(), b[1]->gpu_data(), loss_weight_,
+  B2C_CHECK(b2c_softmax_loss_backward(b[0]->shape(0), (int)b[0]->count(1), prob_.gpu_data(), b[1]->gpu_data(), loss_weight(),
                                       b[0]->mutable_gpu_diff(), S()));
 }
 
@@ -308,13 +307,13 @@ static void softmax_view(Blob* b, int axis, int* outer, int* C, int* inner) {
 }
 void SoftmaxLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   int outer, C, inner;
-  softmax_view(b[0], axis_, &outer, &C, &inner);
+  softmax_view(b[0], layer_param_.softmax_param.axis, &outer, &C, &inner);
   B2C_CHECK(b2c_softmax_forward(outer, C, inner, b[0]->gpu_data(), t[0]->mutable_gpu_data(), S()));
 }
 void SoftmaxLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
   if (!pd[0]) return;
   int outer, C, inner;
-  softmax_view(t[0], axis_, &outer, &C, &inner);
+  softmax_view(t[0], layer_param_.softmax_param.axis, &outer, &C, &inner);
   B2C_CHECK(b2c_softmax_backward(outer, C, inner, t[0]->gpu_data(), t[0]->gpu_diff(), b[0]->mutable_gpu_diff(), S()));
 }
 void SigmoidLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
@@ -343,7 +342,7 @@ void EuclideanLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>
 void EuclideanLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
   for (int i = 0; i < 2; ++i) {                    // euclidean_loss_layer.cu:24-35: alpha = sign * loss_weight / num
     if (!pd[i]) continue;
-    const float alpha = (i == 0 ? 1.f : -1.f) * loss_weight_ / (float)b[i]->shape(0);
+    const float alpha = (i == 0 ? 1.f : -1.f) * loss_weight() / (float)b[i]->shape(0);
     B2C_CHECK(b2c_euclidean_loss_backward(b[i]->count(), diff_.gpu_data(), alpha, b[i]->mutable_gpu_diff(), S()));
   }
 }
@@ -353,31 +352,33 @@ void SigmoidCrossEntropyLossLayer::Forward_gpu(const vector<Blob*>& b, const vec
 void SigmoidCrossEntropyLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
   B2_CHECK(!pd[1], "SigmoidCrossEntropyLoss Layer cannot backpropagate to label inputs.");
   if (!pd[0]) return;
-  const float scale = loss_weight_ / (float)b[0]->shape(0);     // caffe_scal(count, loss_weight / num, bottom_diff)
+  const float scale = loss_weight() / (float)b[0]->shape(0);     // caffe_scal(count, loss_weight / num, bottom_diff)
   B2C_CHECK(b2c_sigmoid_ce_loss_backward(b[0]->count(), b[0]->gpu_data(), b[1]->gpu_data(), scale, b[0]->mutable_gpu_diff(), S()));
 }
 
 // ================================================================================================ ContrastiveLoss
 void ContrastiveLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
-  B2C_CHECK(b2c_contrastive_loss_forward(b[0]->shape(0), (int)b[0]->count(1), b[0]->gpu_data(), b[1]->gpu_data(), b[2]->gpu_data(), margin_,
-                                         legacy_ ? 1 : 0, diff_.mutable_gpu_data(), dist_sq_.mutable_gpu_data(), t[0]->mutable_gpu_data(), S()));
+  const ContrastiveLossParameter& q = layer_param_.contrastive_loss_param;
+  B2C_CHECK(b2c_contrastive_loss_forward(b[0]->shape(0), (int)b[0]->count(1), b[0]->gpu_data(), b[1]->gpu_data(), b[2]->gpu_data(), q.margin,
+                                         q.legacy_version ? 1 : 0, diff_.mutable_gpu_data(), dist_sq_.mutable_gpu_data(), t[0]->mutable_gpu_data(), S()));
 }
 void ContrastiveLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
   if (!pd[0] && !pd[1]) return;
   // contrastive_loss_layer.cpp Backward_cpu: alpha = +-loss_weight / num; bottom 1's gradient is bottom 0's negated
+  const ContrastiveLossParameter& q = layer_param_.contrastive_loss_param;
   const int N = b[0]->shape(0), C = (int)b[0]->count(1);
-  const float alpha = loss_weight_ / (float)N;
+  const float alpha = loss_weight() / (float)N;
   if (pd[0])
-    B2C_CHECK(b2c_contrastive_loss_backward(N, C, diff_.gpu_data(), dist_sq_.gpu_data(), b[2]->gpu_data(), margin_, legacy_ ? 1 : 0, alpha,
+    B2C_CHECK(b2c_contrastive_loss_backward(N, C, diff_.gpu_data(), dist_sq_.gpu_data(), b[2]->gpu_data(), q.margin, q.legacy_version ? 1 : 0, alpha,
                                             b[0]->mutable_gpu_diff(), pd[1] ? b[1]->mutable_gpu_diff() : nullptr, S()));
   else
-    B2C_CHECK(b2c_contrastive_loss_backward(N, C, diff_.gpu_data(), dist_sq_.gpu_data(), b[2]->gpu_data(), margin_, legacy_ ? 1 : 0, -alpha,
+    B2C_CHECK(b2c_contrastive_loss_backward(N, C, diff_.gpu_data(), dist_sq_.gpu_data(), b[2]->gpu_data(), q.margin, q.legacy_version ? 1 : 0, -alpha,
                                             b[1]->mutable_gpu_diff(), nullptr, S()));
 }
 
 // ================================================================================================ Accuracy
 void AccuracyLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
-  B2C_CHECK(b2c_accuracy(b[0]->shape(0), (int)b[0]->count(1), top_k_, b[0]->gpu_data(), b[1]->gpu_data(), t[0]->mutable_gpu_data(),
+  B2C_CHECK(b2c_accuracy(b[0]->shape(0), (int)b[0]->count(1), layer_param_.accuracy_param.top_k, b[0]->gpu_data(), b[1]->gpu_data(), t[0]->mutable_gpu_data(),
                          hits_.mutable_gpu_data(), S()));
 }
 
@@ -411,10 +412,11 @@ void SyntheticDataLayer::LayerSetUp(const vector<Blob*>&, const vector<Blob*>& t
     float* l = t[1]->mutable_cpu_data();
     for (size_t i = 0; i < t[1]->count(); ++i) l[i] = (float)u(rng);
   }
-  datum_mode_ = tf_.on && tf_.crop > 0 && shapes_[0].size() == 4 && shapes_[0][2] == tf_.crop && shapes_[0][3] == tf_.crop;
+  const TransformationParameter& tf = layer_param_.transform_param;
+  datum_mode_ = tf.crop_size > 0 && shapes_[0].size() == 4 && shapes_[0][2] == tf.crop_size && shapes_[0][3] == tf.crop_size;
   if (datum_mode_) {
     const int N = shapes_[0][0], C = shapes_[0][1];
-    hd_ = wd_ = tf_.crop + 32;
+    hd_ = wd_ = tf.crop_size + 32;
     u8_bytes_ = (size_t)N * C * hd_ * wd_;
     CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&host_u8_), u8_bytes_));
     CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
@@ -429,10 +431,10 @@ void SyntheticDataLayer::LayerSetUp(const vector<Blob*>&, const vector<Blob*>& t
       uint64_t r = splitmix64(seed_ * 0x100000001B3ull + i);
       for (size_t k = 0; k < 8 && i + k < u8_bytes_; ++k, r >>= 8) host_u8_[i + k] = (unsigned char)(r & 0xff);
     }
-    if (!tf_.mean_value.empty()) {
-      B2_CHECK(tf_.mean_value.size() == 1 || (int)tf_.mean_value.size() == C, "Specify either 1 mean_value or as many as channels");
-      vector<float> mv(C, tf_.mean_value[0]);
-      if ((int)tf_.mean_value.size() == C) mv = tf_.mean_value;
+    if (!tf.mean_value.empty()) {
+      B2_CHECK(tf.mean_value.size() == 1 || (int)tf.mean_value.size() == C, "Specify either 1 mean_value or as many as channels");
+      vector<float> mv(C, tf.mean_value[0]);
+      if ((int)tf.mean_value.size() == C) mv = tf.mean_value;
       CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&dev_mean_), sizeof(float) * C));
       CUDA_CHECK(cudaMemcpy(dev_mean_, mv.data(), sizeof(float) * C, cudaMemcpyHostToDevice));
     }
@@ -452,12 +454,12 @@ void SyntheticDataLayer::LoadBatch(Blob* top, cudaStream_t st) {
     CUDA_CHECK(cudaMemcpyAsync(top->mutable_gpu_data(), host_, sizeof(float) * n0_, cudaMemcpyHostToDevice, st));
     return;
   }
-  const int N = shapes_[0][0], C = shapes_[0][1];
+  const int N = shapes_[0][0], C = shapes_[0][1], crop = layer_param_.transform_param.crop_size;
   Slot& sl = slot_[cur_];
   if (!sl.in_flight) IssueCopy(cur_);                    // first batch, or nothing was prefetched
   CUDA_CHECK(cudaStreamWaitEvent(st, sl.copied, 0));
-  B2C_CHECK(b2c_transform_u8(sl.dev_u8, N, C, hd_, wd_, tf_.crop, tf_.crop, sl.dev_off, sl.dev_off + N,
-                             reinterpret_cast<const unsigned char*>(sl.dev_off + 2 * N), dev_mean_, nullptr, tf_.scale, top->mutable_gpu_data(), st));
+  B2C_CHECK(b2c_transform_u8(sl.dev_u8, N, C, hd_, wd_, crop, crop, sl.dev_off, sl.dev_off + N,
+                             reinterpret_cast<const unsigned char*>(sl.dev_off + 2 * N), dev_mean_, nullptr, layer_param_.transform_param.scale, top->mutable_gpu_data(), st));
   CUDA_CHECK(cudaEventRecord(sl.consumed, st));
   sl.in_flight = false; sl.used = true;
   cur_ ^= 1;
@@ -465,6 +467,7 @@ void SyntheticDataLayer::LoadBatch(Blob* top, cudaStream_t st) {
 }
 void SyntheticDataLayer::IssueCopy(int s) {
   const int N = shapes_[0][0];
+  const int crop = layer_param_.transform_param.crop_size;
   Slot& sl = slot_[s];
   if (sl.used) {
     CUDA_CHECK(cudaEventSynchronize(sl.copied));         // the previous copy out of this slot's pinned offsets finished long ago
@@ -476,9 +479,9 @@ void SyntheticDataLayer::IssueCopy(int s) {
     const uint64_t base = (draws_ * (uint64_t)N + (uint64_t)i) * 3;
     const unsigned r0 = (unsigned)(splitmix64(seed_ + base) >> 33) + 1, r1 = (unsigned)(splitmix64(seed_ + base + 1) >> 33) + 1,
                    r2 = (unsigned)(splitmix64(seed_ + base + 2) >> 33) + 1;
-    mir[i] = (tf_.mirror && (r0 % 2)) ? 1 : 0;
-    sl.host_off[i] = tf_.train ? (int)(r1 % (unsigned)(hd_ - tf_.crop + 1)) : (hd_ - tf_.crop) / 2;
-    sl.host_off[N + i] = tf_.train ? (int)(r2 % (unsigned)(wd_ - tf_.crop + 1)) : (wd_ - tf_.crop) / 2;
+    mir[i] = (layer_param_.transform_param.mirror && (r0 % 2)) ? 1 : 0;
+    sl.host_off[i] = layer_param_.phase != TEST ? (int)(r1 % (unsigned)(hd_ - crop + 1)) : (hd_ - crop) / 2;
+    sl.host_off[N + i] = layer_param_.phase != TEST ? (int)(r2 % (unsigned)(wd_ - crop + 1)) : (wd_ - crop) / 2;
   }
   ++draws_;
   CUDA_CHECK(cudaMemcpyAsync(sl.dev_u8, host_u8_, u8_bytes_, cudaMemcpyHostToDevice, copy_stream_));
@@ -488,10 +491,63 @@ void SyntheticDataLayer::IssueCopy(int s) {
 }
 
 // ================================================================================================ TrainNet
+// Every layer type TrainNet builds except the data layers, from its LayerParameter.  top_shapes: the tops Net inferred
+// (Flatten and Slice take them); dropout_seed keys that layer's mask stream.
+static shared_ptr<LayerBase> CreateLayer(const LayerParameter& p, const vector<vector<int>>& top_shapes, uint64_t dropout_seed) {
+  const string& t = p.type;
+  if (t == "Convolution") return LayerRegistry::CreateLayer(p);
+  if (t == "ReLU") return std::make_shared<ReLULayer>(p);
+  if (t == "BatchNorm") return std::make_shared<BatchNormLayer>(p);
+  if (t == "Pooling") return std::make_shared<PoolingLayer>(p);
+  if (t == "Eltwise") return std::make_shared<EltwiseLayer>(p);
+  if (t == "InnerProduct") return std::make_shared<InnerProductLayer>(p);
+  if (t == "SoftmaxWithLoss") return std::make_shared<SoftmaxWithLossLayer>(p);
+  if (t == "Accuracy") return std::make_shared<AccuracyLayer>(p);
+  if (t == "Softmax") return std::make_shared<SoftmaxLayer>(p);
+  if (t == "Sigmoid") return std::make_shared<SigmoidLayer>(p);
+  if (t == "Flatten") return std::make_shared<FlattenLayer>(p, top_shapes[0]);
+  if (t == "EuclideanLoss") return std::make_shared<EuclideanLossLayer>(p);
+  if (t == "SigmoidCrossEntropyLoss") return std::make_shared<SigmoidCrossEntropyLossLayer>(p);
+  if (t == "LRN") return std::make_shared<LRNLayer>(p);
+  if (t == "Dropout") return std::make_shared<DropoutLayer>(p, dropout_seed);
+  if (t == "Concat") return std::make_shared<ConcatLayer>(p);
+  if (t == "Slice") return std::make_shared<SliceLayer>(p, top_shapes);
+  if (t == "ContrastiveLoss") return std::make_shared<ContrastiveLossLayer>(p);
+  B2_CHECK(false, "TrainNet: layer type '" + t + "' is not built yet (SURVEY 8f rank 2 covers the ResNet-50 set)");
+  return nullptr;
+}
+
 TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, uint64_t seed, int math) {
   name_ = net.name();
   test_ = net.phase() == TEST;
   Caffe::set_random_seed(seed);
+  const vector<ParamSpec> specs = BuildNodes(net, num_classes, seed, math);
+  // B2C_FUSE=0 disables every graph fusion; each pass below has its own switch as well
+  const bool fuse = env_on("B2C_FUSE", true);
+  // conv layers adding their bottom gradient straight into a fan-out blob's diff (TMA reduce-add store): measured SLOWER than
+  // the shadow blob + add pass on ResNet-50 (dgrad 3.04 -> 3.82 ms/step against 0.50 ms of adds saved; the L2 reduction
+  // units retire the 16 large accumulating stores at about half the plain-store rate), so it is opt-in: B2C_FUSE_FANOUT=1
+  fuse_fanout_ = fuse && env_on("B2C_FUSE_FANOUT", false);
+  if (fuse) FuseReLU();
+  PlanFanOutDiffs();
+  const bool fuse_res = fuse && env_on("B2C_FUSE_RES", true);
+  if (fuse_res) FuseResidualTails(env_on("B2C_FUSE_SPLIT", true));
+  if (!net.loss_blob().empty()) loss_blob_ = blobs_[net.loss_blob()].get();
+  if (!test_) {
+    solver_.reset(new SGDSolver(sp));
+    solver_->SetParams(learnable_, specs);
+  }
+  // Net::ShareWeights (net.cpp:1270-1287), after the arena re-homed the owners: every sharer blob aliases its owner's data and diff.
+  // The sharer's filler ran in SetUp; the owner's values win, with no copy either way
+  for (const Share& sh : shares_) AliasShare(sh);
+  for (auto& l : layers_)
+    if (auto* c = dynamic_cast<ConvolutionLayer*>(l.get()))
+      if (c->EnableFilterCache()) cached_convs_.push_back(c);
+  if (!test_) sched_.reset(new ReduceScheduler(solver_.get(), nullptr));
+  CollectOutputs(net);
+  CUDA_CHECK(cudaStreamSynchronize(S()));
+}
+vector<ParamSpec> TrainNet::BuildNodes(const Net& net, int num_classes, uint64_t seed, int math) {
   vector<ParamSpec> specs;
   for (size_t li = 0; li < net.layers().size(); ++li) {
     const NetLayer& L = net.layers()[li];
@@ -507,79 +563,25 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       if (!sp_) sp_.reset(new Blob());
       node.top.push_back(sp_.get());
     }
+    vector<vector<int>> shapes;
+    for (size_t t = 0; t < L.param.top.size(); ++t) shapes.push_back(net.top_shape((int)li, (int)t));
     shared_ptr<LayerBase> layer;
     if (type == "Data" && L.use_database) {
       // data_param.source opened: the layer reads it (parser threads -> pinned batch -> device transform), data_layer.hpp
       B2_CHECK(db_data_ == nullptr && data_ == nullptr, "TrainNet: one data source per net");
-      auto* d = new DataLayer(L, seed, !test_);
+      auto* d = new DataLayer(L, seed);
       layer.reset(d);
       db_data_ = d;
       db_data_node_ = (int)layers_.size();
     } else if (type == "Data" || type == "Input" || type == "DummyData" || type == "ImageData") {
-      vector<vector<int>> shapes;
-      for (size_t t = 0; t < L.param.top.size(); ++t) shapes.push_back(net.top_shape((int)li, (int)t));
-      SyntheticDataLayer::Transform tf;
-      tf.on = L.has_transform; tf.mirror = L.mirror; tf.train = !test_; tf.crop = L.crop_size; tf.scale = L.transform_scale; tf.mean_value = L.mean_value;
-      auto* d = new SyntheticDataLayer(L.param, shapes, num_classes, seed, tf);
+      auto* d = new SyntheticDataLayer(L.param, shapes, num_classes, seed);
       layer.reset(d);
       data_ = d;
-    } else if (type == "Convolution") {
+    } else {
       LayerParameter lp = L.param;
       lp.convolution_param.math = math;
-      layer = LayerRegistry::CreateLayer(lp);
-    } else if (type == "ReLU") layer.reset(new ReLULayer(L.param, L.relu_slope));
-    else if (type == "BatchNorm") {
-      auto* bn = new BatchNormLayer(L.param, L.bn_scale_bias, L.bn_eps, L.bn_maf, test_);
-      if (L.bn_has_scale_filler) bn->set_scale_filler(L.bn_scale_filler);      // batch_norm_layer.cpp:52-63
-      if (L.bn_has_bias_filler) bn->set_bias_filler(L.bn_bias_filler);
-      layer.reset(bn);
+      layer = CreateLayer(lp, shapes, seed * 0x100000001B3ull + li);
     }
-    else if (type == "Pooling") layer.reset(new PoolingLayer(L.param, L.pooling));
-    else if (type == "Eltwise") {
-      B2_CHECK(L.eltwise_op == 1, "TrainNet: Eltwise PROD / MAX are not built (the BASELINE nets use SUM)");
-      for (float c : L.eltwise_coeff) B2_CHECK(c == 1.f, "TrainNet: Eltwise SUM is built for unit coefficients only");
-      layer.reset(new EltwiseLayer(L.param));
-    }
-    else if (type == "InnerProduct") layer.reset(new InnerProductLayer(L.param, L.ip_num_output, L.ip_bias, L.ip_weight_filler, L.ip_bias_filler));
-    else if (type == "SoftmaxWithLoss") {
-      auto* sl = new SoftmaxWithLossLayer(L.param);
-      if (!L.loss_weight.empty()) sl->set_loss_weight(L.loss_weight[0]);      // GoogLeNet's auxiliary classifiers: 0.3
-      layer.reset(sl);
-    }
-    else if (type == "Accuracy") layer.reset(new AccuracyLayer(L.param, L.accuracy_top_k));     // forward only, no gradient
-    else if (type == "Softmax") layer.reset(new SoftmaxLayer(L.param, L.softmax_axis));
-    else if (type == "Sigmoid") layer.reset(new SigmoidLayer(L.param));
-    else if (type == "Flatten") layer.reset(new FlattenLayer(L.param, net.top_shape((int)li)));
-    else if (type == "EuclideanLoss") {
-      auto* el = new EuclideanLossLayer(L.param);
-      if (!L.loss_weight.empty()) el->set_loss_weight(L.loss_weight[0]);
-      layer.reset(el);
-    }
-    else if (type == "SigmoidCrossEntropyLoss") {
-      auto* sl = new SigmoidCrossEntropyLossLayer(L.param);
-      if (!L.loss_weight.empty()) sl->set_loss_weight(L.loss_weight[0]);
-      layer.reset(sl);
-    }
-    else if (type == "LRN") {
-      B2_CHECK(L.lrn_region == 0, "TrainNet: LRN WITHIN_CHANNEL is not built (the BASELINE nets use ACROSS_CHANNELS)");
-      layer.reset(new LRNLayer(L.param, L.lrn_size, L.lrn_alpha, L.lrn_beta, L.lrn_k));
-    }
-    else if (type == "Dropout") layer.reset(new DropoutLayer(L.param, L.dropout_ratio, seed * 0x100000001B3ull + li, test_));
-    else if (type == "Concat") {
-      B2_CHECK(L.concat_axis == 1, "TrainNet: Concat is built for the channel axis only");
-      layer.reset(new ConcatLayer(L.param));
-    }
-    else if (type == "Slice") {
-      vector<vector<int>> shapes;
-      for (size_t t = 0; t < L.param.top.size(); ++t) shapes.push_back(net.top_shape((int)li, (int)t));
-      layer.reset(new SliceLayer(L.param, L.slice_axis, shapes));
-    }
-    else if (type == "ContrastiveLoss") {
-      auto* cl = new ContrastiveLossLayer(L.param, L.contrastive_margin, L.contrastive_legacy);
-      if (!L.loss_weight.empty()) cl->set_loss_weight(L.loss_weight[0]);
-      layer.reset(cl);
-    }
-    else B2_CHECK(false, "TrainNet: layer type '" + type + "' is not built yet (SURVEY 8f rank 2 covers the ResNet-50 set)");
     layer->SetUp(node.bottom, node.top);
     // learnable blobs in layer order: Net::AppendParam (net.cpp:573-606) appends EVERY blob of every layer, so param ids,
     // reduce-bucket boundaries and the SolverState history list (5 blobs per BatchNorm layer) match the reference.
@@ -624,40 +626,36 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
     layer_types_.push_back(type);
     nodes_.push_back(node);
   }
-  // Fusion pass (B2C_FUSE=0 disables): BatchNorm -> in-place ReLU and Eltwise(SUM, 2 bottoms) -> in-place ReLU run as one
-  // kernel each way, and BatchNorm stops materialising x_norm (csrc/layers_fused.cu).  The ReLU layer stays in the graph as a
-  // no-op so that layer indices, names and blobs are those of the prototxt.  Results are bit-identical to the unfused graph.
-  {
-    const char* e = getenv("B2C_FUSE");
-    const bool fuse = !e || atoi(e) != 0;
-    // conv layers adding their bottom gradient straight into a fan-out blob's diff (TMA reduce-add store): measured SLOWER than
-    // the shadow blob + add pass on ResNet-50 (dgrad 3.04 -> 3.82 ms/step against 0.50 ms of adds saved; the L2 reduction
-    // units retire the 16 large accumulating stores at about half the plain-store rate), so it is opt-in: B2C_FUSE_FANOUT=1
-    const char* ef = getenv("B2C_FUSE_FANOUT");
-    fuse_fanout_ = fuse && ef && atoi(ef) != 0;
-    for (size_t i = 0; fuse && i < layers_.size(); ++i) {
-      auto* bn = dynamic_cast<BatchNormLayer*>(layers_[i].get());
-      auto* el = dynamic_cast<EltwiseLayer*>(layers_[i].get());
-      if (!bn && !el) continue;
-      const bool out_of_place = nodes_[i].top[0] != nodes_[i].bottom[0];
-      ReLULayer* relu = nullptr;
-      if (i + 1 < layers_.size()) {
-        relu = dynamic_cast<ReLULayer*>(layers_[i + 1].get());
-        if (relu && !(nodes_[i + 1].bottom[0] == nodes_[i].top[0] && nodes_[i + 1].top[0] == nodes_[i].top[0] && relu->negative_slope() == 0.f))
-          relu = nullptr;
-      }
-      if (bn && (out_of_place || test_)) {           // (TEST: the inference kernel also runs in place)
-        bn->set_fusion(true, relu != nullptr);
-        bn->Reshape(nodes_[i].bottom, nodes_[i].top);
-        if (relu) relu->set_fused_away(true);
-      } else if (el && relu && nodes_[i].bottom.size() == 2) {
-        el->set_fuse_relu(true);
-        relu->set_fused_away(true);
-      }
+  return specs;
+}
+// Fusion: BatchNorm -> in-place ReLU and Eltwise(SUM, 2 bottoms) -> in-place ReLU run as one kernel each way, and BatchNorm stops
+// materialising x_norm (csrc/layers_fused.cu).  The ReLU layer stays in the graph as a no-op so that layer indices, names and blobs
+// are those of the prototxt.  Results are bit-identical to the unfused graph.
+void TrainNet::FuseReLU() {
+  for (size_t i = 0; i < layers_.size(); ++i) {
+    auto* bn = dynamic_cast<BatchNormLayer*>(layers_[i].get());
+    auto* el = dynamic_cast<EltwiseLayer*>(layers_[i].get());
+    if (!bn && !el) continue;
+    const bool out_of_place = nodes_[i].top[0] != nodes_[i].bottom[0];
+    ReLULayer* relu = nullptr;
+    if (i + 1 < layers_.size()) {
+      relu = dynamic_cast<ReLULayer*>(layers_[i + 1].get());
+      if (relu && !(nodes_[i + 1].bottom[0] == nodes_[i].top[0] && nodes_[i + 1].top[0] == nodes_[i].top[0] && relu->negative_slope() == 0.f))
+        relu = nullptr;
+    }
+    if (bn && (out_of_place || test_)) {           // (TEST: the inference kernel also runs in place)
+      bn->set_fusion(true, relu != nullptr);
+      bn->Reshape(nodes_[i].bottom, nodes_[i].top);
+      if (relu) relu->set_fused_away(true);
+    } else if (el && relu && nodes_[i].bottom.size() == 2) {
+      el->set_fuse_relu(true);
+      relu->set_fused_away(true);
     }
   }
-  // diff accumulation where a blob fans out (insert_splits.cpp / SplitLayer::Backward): the consumer that runs FIRST in
-  // the backward pass writes the blob's diff; every other consumer writes a shadow diff that is then added in
+}
+// diff accumulation where a blob fans out (insert_splits.cpp / SplitLayer::Backward): the consumer that runs FIRST in
+// the backward pass writes the blob's diff; every other consumer writes a shadow diff that is then added in
+void TrainNet::PlanFanOutDiffs() {
   std::map<Blob*, int> writers;
   for (int li = (int)nodes_.size() - 1; li >= 0; --li) {
     Node& nd = nodes_[li];
@@ -677,87 +675,69 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
       }
     }
   }
-  // Residual tails (B2C_FUSE_RES=0 disables): BatchNorm -> Eltwise(SUM, 2 bottoms) -> in-place ReLU.  The BatchNorm that runs LAST
-  // among the producers of the sum's bottoms takes over the sum and the ReLU in both directions (csrc/layers_fused.cu, *_res): its
-  // top is not materialised, four passes over a block-output-sized tensor go away per block and step.  Conditions: the
-  // BatchNorm's top has no other consumer, nothing between it and the sum rewrites the other operand, the sum is the first
-  // backward writer of both bottoms (no shadow diffs).  A TEST net has no backward: there only the first two conditions apply.
-  {
-    const char* e = getenv("B2C_FUSE");
-    const char* er = getenv("B2C_FUSE_RES");
-    const bool fuse_res = (!e || atoi(e) != 0) && (!er || atoi(er) != 0);
-    for (size_t i = 0; fuse_res && i < layers_.size(); ++i) {
-      auto* el = dynamic_cast<EltwiseLayer*>(layers_[i].get());
-      Node& en = nodes_[i];
-      if (!el || !el->fuse_relu() || en.bottom.size() != 2 || (!test_ && !en.need_backward)) continue;
-      if (!en.accumulate_bottom.empty() || en.bottom_diff_tmp[0] || en.bottom_diff_tmp[1]) continue;
-      int prod[2] = {-1, -1};
-      for (int k = 0; k < 2; ++k)
-        for (int j = (int)i - 1; j >= 0 && prod[k] < 0; --j)
-          for (Blob* tb : nodes_[j].top) if (tb == en.bottom[k]) prod[k] = j;
-      if (prod[0] < 0 || prod[1] < 0 || prod[0] == prod[1]) continue;
-      const int k = prod[0] > prod[1] ? 0 : 1, j = prod[k];
-      auto* bn = dynamic_cast<BatchNormLayer*>(layers_[j].get());
-      if (!bn || !bn->recompute() || bn->fuse_relu() || nodes_[j].top[0] == nodes_[j].bottom[0] || (!test_ && !en.propagate_down[k])) continue;
-      int consumers = 0;
-      for (size_t l = 0; l < nodes_.size(); ++l)
-        for (Blob* bb : nodes_[l].bottom) if (bb == en.bottom[k]) ++consumers;
-      bool other_rewritten = false;
-      for (size_t l = (size_t)j + 1; l < i; ++l) {       // ... nor reads it (its backward would add into a diff this layer has yet to write)
-        for (Blob* tb : nodes_[l].top) if (tb == en.bottom[1 - k]) other_rewritten = true;
-        if (!test_) for (Blob* bb : nodes_[l].bottom) if (bb == en.bottom[1 - k]) other_rewritten = true;
-      }
-      if (consumers != 1 || other_rewritten) continue;
-      bn->set_residual(en.bottom[1 - k], en.top[0], en.propagate_down[1 - k]);
-      el->set_fused_away(true);
+}
+// Residual tails (B2C_FUSE_RES=0 disables): BatchNorm -> Eltwise(SUM, 2 bottoms) -> in-place ReLU.  The BatchNorm that runs LAST
+// among the producers of the sum's bottoms takes over the sum and the ReLU in both directions (csrc/layers_fused.cu, *_res): its
+// top is not materialised, four passes over a block-output-sized tensor go away per block and step.  Conditions: the
+// BatchNorm's top has no other consumer, nothing between it and the sum rewrites the other operand, the sum is the first
+// backward writer of both bottoms (no shadow diffs).  A TEST net has no backward: there only the first two conditions apply.
+void TrainNet::FuseResidualTails(bool fuse_split) {
+  for (size_t i = 0; i < layers_.size(); ++i) {
+    auto* el = dynamic_cast<EltwiseLayer*>(layers_[i].get());
+    Node& en = nodes_[i];
+    if (!el || !el->fuse_relu() || en.bottom.size() != 2 || (!test_ && !en.need_backward)) continue;
+    if (!en.accumulate_bottom.empty() || en.bottom_diff_tmp[0] || en.bottom_diff_tmp[1]) continue;
+    int prod[2] = {-1, -1};
+    for (int k = 0; k < 2; ++k)
+      for (int j = (int)i - 1; j >= 0 && prod[k] < 0; --j)
+        for (Blob* tb : nodes_[j].top) if (tb == en.bottom[k]) prod[k] = j;
+    if (prod[0] < 0 || prod[1] < 0 || prod[0] == prod[1]) continue;
+    const int k = prod[0] > prod[1] ? 0 : 1, j = prod[k];
+    auto* bn = dynamic_cast<BatchNormLayer*>(layers_[j].get());
+    if (!bn || !bn->recompute() || bn->fuse_relu() || nodes_[j].top[0] == nodes_[j].bottom[0] || (!test_ && !en.propagate_down[k])) continue;
+    int consumers = 0;
+    for (size_t l = 0; l < nodes_.size(); ++l)
+      for (Blob* bb : nodes_[l].bottom) if (bb == en.bottom[k]) ++consumers;
+    bool other_rewritten = false;
+    for (size_t l = (size_t)j + 1; l < i; ++l) {       // ... nor reads it (its backward would add into a diff this layer has yet to write)
+      for (Blob* tb : nodes_[l].top) if (tb == en.bottom[1 - k]) other_rewritten = true;
+      if (!test_) for (Blob* bb : nodes_[l].bottom) if (bb == en.bottom[1 - k]) other_rewritten = true;
     }
-    // a fused tail's sum blob with a second backward writer: hand the shadow diff to the tail instead of adding it in a pass of its own
-    const char* ed = getenv("B2C_FUSE_SPLIT");
-    const bool fuse_split = fuse_res && (!ed || atoi(ed) != 0);
-    std::map<Blob*, BatchNormLayer*> tails;
-    for (size_t j = 0; j < layers_.size(); ++j)
-      if (auto* bn = dynamic_cast<BatchNormLayer*>(layers_[j].get()))
-        if (bn->residual_sum()) tails[bn->residual_sum()] = bn;
-    std::map<Blob*, int> shadows;
-    for (Node& nd : nodes_)
-      for (size_t i = 0; i < nd.bottom.size(); ++i) if (nd.bottom_diff_tmp[i]) ++shadows[nd.bottom[i]];
-    for (Node& nd : nodes_) {
-      nd.deferred_add.assign(nd.bottom.size(), false);
-      for (size_t i = 0; fuse_split && i < nd.bottom.size(); ++i) {
-        if (!nd.bottom_diff_tmp[i] || shadows[nd.bottom[i]] != 1) continue;       // exactly one shadow per blob
-        auto it = tails.find(nd.bottom[i]);
-        if (it == tails.end()) continue;
-        it->second->set_sum_diff_part2(nd.bottom_diff_tmp[i]);
-        nd.deferred_add[i] = true;
-      }
+    if (consumers != 1 || other_rewritten) continue;
+    bn->set_residual(en.bottom[1 - k], en.top[0], en.propagate_down[1 - k]);
+    el->set_fused_away(true);
+  }
+  // a fused tail's sum blob with a second backward writer: hand the shadow diff to the tail instead of adding it in a pass of its own
+  std::map<Blob*, BatchNormLayer*> tails;
+  for (size_t j = 0; j < layers_.size(); ++j)
+    if (auto* bn = dynamic_cast<BatchNormLayer*>(layers_[j].get()))
+      if (bn->residual_sum()) tails[bn->residual_sum()] = bn;
+  std::map<Blob*, int> shadows;
+  for (Node& nd : nodes_)
+    for (size_t i = 0; i < nd.bottom.size(); ++i) if (nd.bottom_diff_tmp[i]) ++shadows[nd.bottom[i]];
+  for (Node& nd : nodes_) {
+    nd.deferred_add.assign(nd.bottom.size(), false);
+    for (size_t i = 0; fuse_split && i < nd.bottom.size(); ++i) {
+      if (!nd.bottom_diff_tmp[i] || shadows[nd.bottom[i]] != 1) continue;       // exactly one shadow per blob
+      auto it = tails.find(nd.bottom[i]);
+      if (it == tails.end()) continue;
+      it->second->set_sum_diff_part2(nd.bottom_diff_tmp[i]);
+      nd.deferred_add[i] = true;
     }
   }
-  if (!net.loss_blob().empty()) loss_blob_ = blobs_[net.loss_blob()].get();
-  if (!test_) {
-    solver_.reset(new SGDSolver(sp));
-    solver_->SetParams(learnable_, specs);
-  }
-  // Net::ShareWeights (net.cpp:1270-1287), after the arena re-homed the owners: every sharer blob aliases its owner's data and diff.
-  // The sharer's filler ran in SetUp; the owner's values win, with no copy either way
-  for (const Share& sh : shares_) AliasShare(sh);
-  for (auto& l : layers_)
-    if (auto* c = dynamic_cast<ConvolutionLayer*>(l.get()))
-      if (c->EnableFilterCache()) cached_convs_.push_back(c);
-  if (!test_) sched_.reset(new ReduceScheduler(solver_.get(), nullptr));
-  // output blobs and loss weights (Net::Init, net.cpp: available_blobs; Layer::SetLossWeights, LossLayer::LayerSetUp)
-  {
-    std::set<string> available;
-    std::map<string, float> weight;
-    for (const NetLayer& L : net.layers()) {
-      for (auto& bn : L.param.bottom) available.erase(bn);
-      for (size_t t = 0; t < L.param.top.size(); ++t) {
-        available.insert(L.param.top[t]);
-        weight[L.param.top[t]] = TopLossWeight(L, t);
-      }
+}
+// output blobs and loss weights (Net::Init, net.cpp: available_blobs; Layer::SetLossWeights, LossLayer::LayerSetUp)
+void TrainNet::CollectOutputs(const Net& net) {
+  std::set<string> available;
+  std::map<string, float> weight;
+  for (const NetLayer& L : net.layers()) {
+    for (auto& bn : L.param.bottom) available.erase(bn);
+    for (size_t t = 0; t < L.param.top.size(); ++t) {
+      available.insert(L.param.top[t]);
+      weight[L.param.top[t]] = TopLossWeight(L.param, t);
     }
-    for (const string& n : available) outputs_.push_back({n, blobs_[n].get(), weight[n]});
   }
-  CUDA_CHECK(cudaStreamSynchronize(S()));
+  for (const string& n : available) outputs_.push_back({n, blobs_[n].get(), weight[n]});
 }
 TrainNet::~TrainNet() {
   if (pass_scored_) cudaEventDestroy(pass_scored_);

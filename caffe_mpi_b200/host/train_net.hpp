@@ -13,28 +13,24 @@ namespace caffe {
 
 class ReLULayer : public LayerBase {
  public:
-  ReLULayer(const LayerParameter& p, float negative_slope) : LayerBase(p), slope_(negative_slope) {}
+  using LayerBase::LayerBase;
   const char* type() const override { return "ReLU"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]); }
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  float slope_;     // relu_param.negative_slope (relu_layer.cpp:13-16)
   bool fused_away_ = false;
  public:
-  float negative_slope() const { return slope_; }
+  float negative_slope() const { return layer_param_.relu_param.negative_slope; }   // relu_layer.cpp:13-16
   void set_fused_away(bool v) { fused_away_ = v; }   // the producing BatchNorm / Eltwise layer applies (and back-propagates) this ReLU
 };
 
 class BatchNormLayer : public LayerBase {      // NVCaffe BatchNorm with scale_bias (batch_norm_layer.cpp)
  public:
-  // test: the TEST phase -- normalise with the running statistics (b2c_bn_forward_inference), never write blobs 0-4
-  BatchNormLayer(const LayerParameter& p, bool scale_bias, float eps, float maf, bool test = false)
-      : LayerBase(p), scale_bias_(scale_bias), eps_(eps), maf_(maf), test_(test) {
-    scale_filler_.type = "constant"; scale_filler_.value = 1.f;
-  }
-  void set_scale_filler(const FillerParameter& f) { scale_filler_ = f; }
-  void set_bias_filler(const FillerParameter& f) { bias_filler_ = f; }
+  // TEST phase: normalise with the running statistics (b2c_bn_forward_inference), never write blobs 0-4
+  explicit BatchNormLayer(const LayerParameter& p)
+      : LayerBase(p), scale_bias_(p.batch_norm_param.scale_bias), eps_(p.batch_norm_param.eps),
+        maf_(p.batch_norm_param.moving_average_fraction) {}
   const char* type() const override { return "BatchNorm"; }
   void LayerSetUp(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
@@ -43,10 +39,8 @@ class BatchNormLayer : public LayerBase {      // NVCaffe BatchNorm with scale_b
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
   bool scale_bias_;
   float eps_, maf_;
-  FillerParameter scale_filler_, bias_filler_;
   bool fuse_relu_ = false;   // an in-place ReLU on the top blob is folded into this layer's kernels (TrainNet's fusion pass)
   bool recompute_ = false;   // do not store x_norm: backward recomputes it from the bottom blob (needs top != bottom)
-  bool test_;
   int iter_ = 0;
  public:
   void set_iter(int i) { iter_ = i; }
@@ -70,13 +64,13 @@ class BatchNormLayer : public LayerBase {      // NVCaffe BatchNorm with scale_b
 
 class PoolingLayer : public LayerBase {
  public:
-  PoolingLayer(const LayerParameter& p, const PoolingParameter& q) : LayerBase(p), q_(q) {}
+  using LayerBase::LayerBase;
   const char* type() const override { return "Pooling"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  PoolingParameter q_, eff_;
+  PoolingParameter eff_;
   int* mask_ = nullptr;
   size_t mask_cap_ = 0;
  public:
@@ -85,7 +79,10 @@ class PoolingLayer : public LayerBase {
 
 class EltwiseLayer : public LayerBase {        // SUM with unit coefficients (the only use in the BASELINE nets)
  public:
-  using LayerBase::LayerBase;
+  explicit EltwiseLayer(const LayerParameter& p) : LayerBase(p) {
+    B2_CHECK(p.eltwise_param.operation == 1, "TrainNet: Eltwise PROD / MAX are not built (the BASELINE nets use SUM)");
+    for (float c : p.eltwise_param.coeff) B2_CHECK(c == 1.f, "TrainNet: Eltwise SUM is built for unit coefficients only");
+  }
   void set_fuse_relu(bool v) { fuse_relu_ = v; }
   bool fuse_relu() const { return fuse_relu_; }
   void set_fused_away(bool v) { fused_away_ = v; }     // the BatchNorm layer that produces one of the bottoms does the sum (TrainNet's fusion pass)
@@ -102,8 +99,8 @@ class EltwiseLayer : public LayerBase {        // SUM with unit coefficients (th
 
 class InnerProductLayer : public LayerBase {
  public:
-  InnerProductLayer(const LayerParameter& p, int num_output, bool bias, const FillerParameter& wf, const FillerParameter& bf)
-      : LayerBase(p), num_output_(num_output), bias_(bias), wf_(wf), bf_(bf) {}
+  explicit InnerProductLayer(const LayerParameter& p)
+      : LayerBase(p), num_output_(p.inner_product_param.num_output), bias_(p.inner_product_param.bias_term) {}
   const char* type() const override { return "InnerProduct"; }
   void LayerSetUp(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
@@ -112,7 +109,6 @@ class InnerProductLayer : public LayerBase {
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
   int num_output_, K_ = 0, M_ = 0;
   bool bias_;
-  FillerParameter wf_, bf_;
   // forward runs on the tensor-core NoTrans x Trans GEMM (b2c_sgemm_ex): split-K scratch, and a 16-byte aligned copy of the
   // weights when their slot in the parameter arena is only 8-byte aligned (slots are padded to even counts, net.cpp:1356-1371;
   // TMA wants 16).  The copy is 4 bytes per weight once per forward -- against a 4x slower FFMA kernel.
@@ -127,34 +123,34 @@ class InnerProductLayer : public LayerBase {
 // ---- layers the AlexNet / GoogLeNet / VGG-16 nets add (parity: tests/test_layers_extra_gpu.py, test_inception_style_net_matches_oracle) ----
 class LRNLayer : public LayerBase {            // ACROSS_CHANNELS only (the BASELINE nets' use)
  public:
-  LRNLayer(const LayerParameter& p, int size, float alpha, float beta, float k) : LayerBase(p), size_(size), alpha_(alpha), beta_(beta), k_(k) {}
+  explicit LRNLayer(const LayerParameter& p) : LayerBase(p) {
+    B2_CHECK(p.lrn_param.norm_region == 0, "TrainNet: LRN WITHIN_CHANNEL is not built (the BASELINE nets use ACROSS_CHANNELS)");
+  }
   const char* type() const override { return "LRN"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { t[0]->ReshapeLike(*b[0]); scale_.ReshapeLike(*b[0]); }
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  int size_;
-  float alpha_, beta_, k_;
   Blob scale_;
 };
 
 class DropoutLayer : public LayerBase {        // TRAIN phase: y = x * mask, mask in {0, 1/(1-ratio)}; TEST phase: y = x
  public:
-  DropoutLayer(const LayerParameter& p, float ratio, uint64_t seed, bool test = false) : LayerBase(p), ratio_(ratio), seed_(seed), test_(test) {}
+  DropoutLayer(const LayerParameter& p, uint64_t seed) : LayerBase(p), seed_(seed) {}
   const char* type() const override { return "Dropout"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]); mask_.ReshapeLike(*b[0]); }
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  float ratio_;
   uint64_t seed_, offset_ = 0;
-  bool test_;
   Blob mask_;
 };
 
 class ConcatLayer : public LayerBase {         // along the channel axis (axis 1), strided 2-D copies
  public:
-  using LayerBase::LayerBase;
+  explicit ConcatLayer(const LayerParameter& p) : LayerBase(p) {
+    B2_CHECK(p.concat_param.axis == 1, "TrainNet: Concat is built for the channel axis only");
+  }
   const char* type() const override { return "Concat"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
  protected:
@@ -166,41 +162,36 @@ class ConcatLayer : public LayerBase {         // along the channel axis (axis 1
 // Backward writes the whole bottom diff: a top whose diff no layer writes contributes its zero-initialised diff.
 class SliceLayer : public LayerBase {
  public:
-  SliceLayer(const LayerParameter& p, int axis, const vector<vector<int>>& top_shapes) : LayerBase(p), axis_(axis), shapes_(top_shapes) {}
+  SliceLayer(const LayerParameter& p, const vector<vector<int>>& top_shapes) : LayerBase(p), shapes_(top_shapes) {}
   const char* type() const override { return "Slice"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  int axis_;
   vector<vector<int>> shapes_;
 };
 
 class SoftmaxWithLossLayer : public LayerBase {
  public:
   using LayerBase::LayerBase;
-  void set_loss_weight(float w) { loss_weight_ = w; }
-  float loss_weight() const { return loss_weight_; }
   const char* type() const override { return "SoftmaxWithLoss"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
   Blob prob_;
-  float loss_weight_ = 1.f;
 };
 
 // ---- layers the deploy / TEST nets and the MNIST autoencoder add (softmax_layer, sigmoid_layer, flatten_layer, euclidean_loss_layer,
 // sigmoid_cross_entropy_loss_layer .cpp) ----
 class SoftmaxLayer : public LayerBase {        // over softmax_param.axis: an [outer, C, inner] view of the bottom
  public:
-  SoftmaxLayer(const LayerParameter& p, int axis) : LayerBase(p), axis_(axis) {}
+  using LayerBase::LayerBase;
   const char* type() const override { return "Softmax"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]); }
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  int axis_;
 };
 
 class SigmoidLayer : public LayerBase {
@@ -231,33 +222,28 @@ class FlattenLayer : public LayerBase {
 class EuclideanLossLayer : public LayerBase {  // loss = sum (a - b)^2 / N / 2; gradient to each propagating bottom with its sign
  public:
   using LayerBase::LayerBase;
-  void set_loss_weight(float w) { loss_weight_ = w; }
   const char* type() const override { return "EuclideanLoss"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { diff_.ReshapeLike(*b[0]); t[0]->Reshape({1}); }
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
   Blob diff_;
-  float loss_weight_ = 1.f;
 };
 
 class SigmoidCrossEntropyLossLayer : public LayerBase {   // no sigmoid tensor: backward recomputes sigmoid(x)
  public:
   using LayerBase::LayerBase;
-  void set_loss_weight(float w) { loss_weight_ = w; }
   const char* type() const override { return "SigmoidCrossEntropyLoss"; }
   void Reshape(const vector<Blob*>&, const vector<Blob*>& t) override { t[0]->Reshape({1}); }
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  float loss_weight_ = 1.f;
 };
 
 // contrastive_loss_layer.cpp: bottoms a, b [N, C(, 1, 1)] and the similarity label [N]; diff = a - b and dist_sq are kept for backward
 class ContrastiveLossLayer : public LayerBase {
  public:
-  ContrastiveLossLayer(const LayerParameter& p, float margin, bool legacy) : LayerBase(p), margin_(margin), legacy_(legacy) {}
-  void set_loss_weight(float w) { loss_weight_ = w; }
+  using LayerBase::LayerBase;
   const char* type() const override { return "ContrastiveLoss"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override {
     diff_.Reshape({b[0]->shape(0), (int)b[0]->count(1)}); dist_sq_.Reshape({b[0]->shape(0)}); t[0]->Reshape({1});
@@ -265,24 +251,20 @@ class ContrastiveLossLayer : public LayerBase {
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  float margin_;
-  bool legacy_;
   Blob diff_, dist_sq_;
-  float loss_weight_ = 1.f;
 };
 
 class AccuracyLayer : public LayerBase {       // forward only (accuracy_layer.cpp); top[0] is a scalar
  public:
-  AccuracyLayer(const LayerParameter& p, int top_k) : LayerBase(p), top_k_(top_k) {}
+  using LayerBase::LayerBase;
   const char* type() const override { return "Accuracy"; }
   void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override {
-    B2_CHECK(top_k_ <= (int)(b[0]->count() / b[1]->count()), "top_k must be less than or equal to the number of classes.");
+    B2_CHECK(layer_param_.accuracy_param.top_k <= (int)(b[0]->count() / b[1]->count()), "top_k must be less than or equal to the number of classes.");
     t[0]->Reshape({1}); hits_.Reshape({1});
   }
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>&, const vector<bool>&, const vector<Blob*>&) override {}   // "Accuracy cannot backpropagate"
-  int top_k_;
   Blob hits_;
 };
 
@@ -294,10 +276,9 @@ class AccuracyLayer : public LayerBase {       // forward only (accuracy_layer.c
 //     values, scale) into the float data blob.
 class SyntheticDataLayer : public LayerBase {
  public:
-  // train = false (TEST phase): the centre crop window instead of a random one (data_transformer.cpp:219-229)
-  struct Transform { bool on = false, mirror = false, train = true; int crop = 0; float scale = 1.f; vector<float> mean_value; };
-  SyntheticDataLayer(const LayerParameter& p, const vector<vector<int>>& shapes, int num_classes, uint64_t seed, const Transform& tf)
-      : LayerBase(p), shapes_(shapes), classes_(num_classes), seed_(seed), tf_(tf) {}
+  // transform_param: crop, mirror, mean_value, scale; the TEST phase takes the centre crop window (data_transformer.cpp:219-229)
+  SyntheticDataLayer(const LayerParameter& p, const vector<vector<int>>& shapes, int num_classes, uint64_t seed)
+      : LayerBase(p), shapes_(shapes), classes_(num_classes), seed_(seed) {}
   const char* type() const override { return "Data"; }
   void LayerSetUp(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Reshape(const vector<Blob*>&, const vector<Blob*>&) override {}
@@ -312,7 +293,6 @@ class SyntheticDataLayer : public LayerBase {
   vector<vector<int>> shapes_;
   int classes_;
   uint64_t seed_;
-  Transform tf_;
   float* host_ = nullptr;
   size_t n0_ = 0;
   // datum mode
@@ -420,6 +400,13 @@ class TrainNet {
     vector<bool> param_owned;
     int first_owned = -1;
   };
+  // set-up, in this order: the layers and their parameter ids (sharing included), BatchNorm / Eltwise fused with the ReLU that
+  // follows, shadow diffs where a blob fans out, residual tails with their deferred shadow adds, the output blobs
+  vector<ParamSpec> BuildNodes(const Net& net, int num_classes, uint64_t seed, int math);   // returns the learnable blobs' specs
+  void FuseReLU();
+  void PlanFanOutDiffs();
+  void FuseResidualTails(bool fuse_split);
+  void CollectOutputs(const Net& net);
   void Forward(bool copy_input);
   void Backward(bool update);
   void PrepareFilters();                           // b2c_conv_prepare_filters over every cached conv layer (weights changed)
