@@ -137,6 +137,7 @@ def lib():
         "b2c_pool_forward": (i, [i] * 10 + [vp, vp, vp, vp]),
         "b2c_pool_backward": (i, [i] * 10 + [vp, vp, vp, vp]),
         "b2c_debug_pool_plan": (i, [i] * 11 + [vp, vp, C.POINTER(i), i]),
+        "b2c_debug_bn_plan": (i, [i] * 5 + [C.POINTER(vp), i, C.POINTER(i), i]),
         "b2c_add": (i, [sz, vp, vp, vp, vp]),
         "b2c_softmax_loss_forward": (i, [i, i, vp, vp, vp, vp, vp]),
         "b2c_softmax_loss_backward": (i, [i, i, vp, vp, f, vp, vp]),
@@ -344,6 +345,18 @@ def pool_plan(method, dir, NC, H, W, k, s, p, out_ptr=0, mask_ptr=0):
     check(lib().b2c_debug_pool_plan(method, dir, NC, H, W, k[0], k[1], s[0], s[1], p[0], p[1], C.c_void_p(out_ptr),
                                     C.c_void_p(mask_ptr), out, 5))
     return dict(route=POOL_ROUTES[out[0]], Ho=out[1], Wo=out[2], q=out[3], rpb=out[4])
+
+
+BN_FORMS = ("unfused", "fused", "fused_res")
+
+
+def bn_plan(dir, form, N, Cc, S, ptrs=()):
+    """b2c_debug_bn_plan: the launch a BatchNorm training call (dir 0 forward, 1 backward; form one of BN_FORMS) takes, with the
+    call's tensor pointers (ints, None for a null one) tested for alignment only"""
+    out = (C.c_int * 6)()
+    arr = (C.c_void_p * max(1, len(ptrs)))(*[p or None for p in ptrs])
+    check(lib().b2c_debug_bn_plan(dir, BN_FORMS.index(form), N, Cc, S, arr, len(ptrs), out, 6))
+    return dict(launches=out[0], cs=out[1], threads=out[2], park=out[3], prefetch=out[4], vec=bool(out[5]))
 
 
 def sgemm(transA, transB, M, N, K, alpha, A, B, beta, Cm, stream=None):

@@ -3,6 +3,7 @@
 // accumulation order.  Both files produce the same bits for the same input because they run the same code in the same order.
 #pragma once
 #include <cooperative_groups.h>
+#include <initializer_list>
 #include <stdlib.h>
 #include "b2c_common.cuh"
 
@@ -117,6 +118,69 @@ __device__ __forceinline__ void bn_channel_partial(int N, int C, int S, int c, c
   }
   a += a2; b += b2;
 }
+
+// the cluster's partial (a, b) pairs added in rank order, by every thread
+__device__ __forceinline__ void bn_cluster_sum(cooperative_groups::cluster_group& cluster, const float2* part, unsigned nranks, double& s1, double& s2) {
+  float2 v[BN_CLUSTER];
+#pragma unroll
+  for (unsigned r = 0; r < (unsigned)BN_CLUSTER; ++r) v[r] = r < nranks ? *cluster.map_shared_rank(part, r) : make_float2(0.f, 0.f);
+  s1 = 0.0; s2 = 0.0;
+#pragma unroll
+  for (unsigned r = 0; r < (unsigned)BN_CLUSTER; ++r) if (r < nranks) { s1 += v[r].x; s2 += v[r].y; }
+}
+
+// Mean and variance + eps of channel c, in every thread of the cluster.  Pass 1 sums x - k and (x - k)^2 with k = the channel's
+// first value; the variance s2/cnt - (s1/cnt)^2 then carries an fp32 summation error that grows as ((mean - k) / sigma)^2 (4e-4
+// relative for a first value 100 sigma out).  So when k lies more than 4 sigma from the mean, pass 2 sums x - m0 and (x - m0)^2
+// about pass 1's mean m0 instead: the error is then the reference's two-pass level whatever k is, and within 17x of it when pass 2
+// is skipped.  Every thread of the cluster holds the same s1, s2, so all take the same branch.  CACHE (bn_channel_partial's): pass 1
+// parks the slice in shared memory (1) or reads it from there (2); pass 2 reads the parked copy, else x again.  part[2]: the CTA's
+// partials of each pass (pass 2 writes the second slot while peers may still read the first).
+template <bool VEC, int CACHE>
+__device__ __forceinline__ void bn_channel_stats(cooperative_groups::cluster_group& cluster, int N, int C, int S, int c, const float* __restrict__ x,
+                                                 float eps, float2* part, void* cache, float& m, float& var_eps) {
+  const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
+  const double cnt = (double)N * S;
+  const float k = x[(size_t)c * S];
+  float a, b;
+  double s1, s2;
+  bn_channel_partial<VEC, 0, CACHE>(N, C, S, c, x, nullptr, k, rank, nranks, a, b, cache);
+  block_sum2(a, b);
+  if (threadIdx.x == 0) part[0] = make_float2(a, b);
+  cluster.sync();
+  bn_cluster_sum(cluster, part, nranks, s1, s2);
+  double m1 = s1 / cnt, var = s2 / cnt - m1 * m1;
+  m = (float)((double)k + m1);
+  if (m1 * m1 > 16.0 * var) {
+    const float m0 = m;
+    bn_channel_partial<VEC, 0, CACHE ? 2 : 0>(N, C, S, c, x, nullptr, m0, rank, nranks, a, b, cache);
+    block_sum2(a, b);
+    if (threadIdx.x == 0) part[1] = make_float2(a, b);
+    cluster.sync();
+    bn_cluster_sum(cluster, part + 1, nranks, s1, s2);
+    m1 = s1 / cnt;
+    var = s2 / cnt - m1 * m1;
+    m = (float)((double)m0 + m1);
+  }
+  var_eps = (float)fmax(var, 0.0) + eps;   // batch_norm_layer.cpp:183-186 (eps folded in before the average)
+}
+
+// The launch of a BatchNorm training call, chosen by bn_plan (layers_fused.cu) for every entry point and reported by
+// b2c_debug_bn_plan.  threads and cs are those of the per-channel (cluster) kernel; the two-launch forms' elementwise passes
+// always run 256-thread blocks.
+struct BnPlan {
+  int launches;            // 1: statistics / reduction and the elementwise pass in one launch; 2: two launches
+  unsigned cs;             // CTAs per channel (one thread-block cluster)
+  unsigned threads;        // threads per CTA
+  int park;                // what stays in shared memory between the phases: bit 0 = x, bit 1 = the (masked) gradient
+  int prefetch;            // the parked streams come in by cp.async before the reduction
+  bool vec;                // float4 units (S % 4 == 0 and every pointer 16-byte aligned), else one float at a time
+  size_t smem;             // dynamic shared memory per CTA
+  unsigned slice_units;    // units in the largest (rank 0's) slice of a channel
+};
+// dir 0 = forward, 1 = backward; form 0 = b2c_bn_forward_train / b2c_bn_backward, 1 = *_fused, 2 = *_fused_res.  `ptrs` are the
+// call's tensors (compared for alignment, never dereferenced).  Refuses what the entry points refuse about the shape.
+int bn_plan(int dir, int form, int N, int C, int S, std::initializer_list<const void*> ptrs, const char* who, BnPlan* p);
 
 // Largest cluster the per-channel kernels may use on this device: B2C_BN_CLUSTER (1..16, default 8 = the portable limit) capped by what the
 // device schedules -- 16-CTA clusters are a non-portable size (cudaFuncAttributeNonPortableClusterSizeAllowed); the probe kernel

@@ -56,36 +56,26 @@ __global__ void __launch_bounds__(256) relu_bwd_kernel(size_t n, int vec, const 
 // Per-channel reductions run as one thread-block CLUSTER of 1..8 CTAs per channel (sized by the host from the channel's
 // extent): each CTA streams its share of the channel's N*S values (float4 when the planes are 16-byte aligned), the eight partial sums meet in rank 0 through
 // distributed shared memory in rank order (deterministic), no scratch buffer, no atomics, one launch.
-// Statistics use sums of (x - k) and (x - k)^2 with k = the channel's first value, combined in double: one pass over
-// HBM instead of the reference's two, without the cancellation of a raw E[x^2] - E[x]^2.
+// Statistics (bn_channel_stats): sums of x - k and (x - k)^2 with k = the channel's first value, combined in double, and a second
+// pass about that mean when k lies more than 4 sigma from it, so the variance's error does not depend on any one element.
 // (geometry, cursors and block sums: bn_common.cuh, shared with the fused kernels of layers_fused.cu)
 
 template <bool VEC>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_stats_kernel(int N, int C, int S, const float* __restrict__ x, float eps, float maf, int first,
                 float* __restrict__ mean, float* __restrict__ invstd, float* __restrict__ run_mean, float* __restrict__ run_var) {
-  __shared__ float2 part;
+  __shared__ float2 part[2];
   cg::cluster_group cluster = cg::this_cluster();
-  const unsigned rank = cluster.block_rank();
   const int c = blockIdx.y;
-  const float k = x[(size_t)c * S];
-  float a, b;
-  bn_channel_partial<VEC, 0>(N, C, S, c, x, nullptr, k, rank, cluster.num_blocks(), a, b);
-  block_sum2(a, b);
-  if (threadIdx.x == 0) part = make_float2(a, b);
-  cluster.sync();
-  if (rank == 0 && threadIdx.x == 0) {
-    double s1 = 0.0, s2 = 0.0;
-    for (unsigned r = 0; r < cluster.num_blocks(); ++r) { const float2 v = *cluster.map_shared_rank(&part, r); s1 += v.x; s2 += v.y; }
-    const double cnt = (double)N * S, m1 = s1 / cnt;
-    const float m = (float)((double)k + m1);
-    const float var_eps = (float)fmax(s2 / cnt - m1 * m1, 0.0) + eps;   // batch_norm_layer.cpp:183-186 (eps folded in before the average)
+  float m, var_eps;
+  bn_channel_stats<VEC, 0>(cluster, N, C, S, c, x, eps, part, nullptr, m, var_eps);
+  if (cluster.block_rank() == 0 && threadIdx.x == 0) {
     mean[c] = m;
     invstd[c] = 1.0f / sqrtf(var_eps);
     if (first) { run_mean[c] = m; run_var[c] = var_eps; }                         // iter_ <= 1: copy (:199-204)
     else { run_mean[c] = (1.f - maf) * m + maf * run_mean[c]; run_var[c] = (1.f - maf) * var_eps + maf * run_var[c]; }
   }
-  cluster.sync();                                   // remote shared memory stays valid until rank 0 has read it
+  cluster.sync();                                   // remote shared memory stays valid until every rank has read it
 }
 // per channel: dgamma = sum dy*xn, dbeta = sum dy (both OVERWRITTEN, batch_norm_layer.cpp:247-252)
 template <bool VEC>
@@ -758,16 +748,10 @@ template <typename... Args>
 static void launch_clustered(void (*kernel)(Args...), unsigned cs, int C, void* stream, unsigned threads, Args... args) {
   bn_launch_clustered(kernel, cs, C, 0, stream, threads, args...);
 }
-static bool vec_ok(int S, std::initializer_list<const void*> ptrs) {
-  if (S % 4) return false;
-  for (const void* p : ptrs) if (reinterpret_cast<uintptr_t>(p) & 15) return false;
-  return true;
-}
 namespace b2c {
-int launch_bn_stats(int N, int C, int S, const float* x, float eps, float maf, int first, float* mean, float* invstd, float* run_mean,
-                    float* run_var, bool vec, void* stream) {
-  const unsigned cs = bn_cluster_size(N, C, S);
-  launch_clustered(vec ? bn_stats_kernel<true> : bn_stats_kernel<false>, cs, C, stream, bn_threads(N, S, true), N, C, S, x, eps, maf, first, mean, invstd, run_mean, run_var);
+int launch_bn_stats(const BnPlan& p, int N, int C, int S, const float* x, float eps, float maf, int first, float* mean, float* invstd,
+                    float* run_mean, float* run_var, void* stream) {
+  launch_clustered(p.vec ? bn_stats_kernel<true> : bn_stats_kernel<false>, p.cs, C, stream, p.threads, N, C, S, x, eps, maf, first, mean, invstd, run_mean, run_var);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -775,14 +759,12 @@ int launch_bn_stats(int N, int C, int S, const float* x, float eps, float maf, i
 extern "C" int b2c_bn_forward_train(int N, int C, int S, const float* x, const float* gamma, const float* beta, float eps,
                                     float moving_average_fraction, int first_iteration, float* running_mean, float* running_var,
                                     float* save_mean, float* save_invstd, float* xnorm, float* y, void* stream) {
-  NEED(x && y && xnorm && save_mean && save_invstd && running_mean && running_var && N > 0 && C > 0 && S > 0, "b2c_bn_forward_train: bad argument");
+  NEED(x && y && xnorm && save_mean && save_invstd && running_mean && running_var, "b2c_bn_forward_train: bad argument");
   NEED((gamma == nullptr) == (beta == nullptr), "b2c_bn_forward_train: gamma and beta go together");
-  NEED((size_t)N * S < (1ull << 31) && C <= 65535, "b2c_bn_forward_train: channel extent out of range");
-  const bool vec = vec_ok(S, {x, y, xnorm});
-  const unsigned cs = bn_cluster_size(N, C, S);
-  launch_clustered(vec ? bn_stats_kernel<true> : bn_stats_kernel<false>, cs, C, stream, bn_threads(N, S, true), N, C, S, x, eps, moving_average_fraction, first_iteration,
-                   save_mean, save_invstd, running_mean, running_var);
-  B2C_POST_LAUNCH();
+  BnPlan pl;
+  if (int rc = bn_plan(0, 0, N, C, S, {x, y, xnorm}, "b2c_bn_forward_train", &pl)) return rc;
+  const bool vec = pl.vec;
+  if (int rc = launch_bn_stats(pl, N, C, S, x, eps, moving_average_fraction, first_iteration, save_mean, save_invstd, running_mean, running_var, stream)) return rc;
   const size_t units = (size_t)N * C * (vec ? S / 4 : S);
   const unsigned blocks = (unsigned)((units + 256 * BN_EW_PER_THREAD - 1) / (256 * BN_EW_PER_THREAD));
   if (vec) bn_norm_kernel<true><<<blocks, 256, 0, as_stream(stream)>>>(units, C, S, x, save_mean, save_invstd, gamma, beta, xnorm, y);
@@ -793,9 +775,10 @@ extern "C" int b2c_bn_forward_train(int N, int C, int S, const float* x, const f
 extern "C" int b2c_bn_backward(int N, int C, int S, const float* dy, const float* xnorm, const float* gamma, const float* save_invstd,
                                float* dgamma, float* dbeta, float* dx, void* stream) {
   NEED(dy && xnorm && save_invstd && dgamma && dbeta && dx, "b2c_bn_backward: null (dgamma/dbeta double as the reduction scratch)");
-  NEED(N > 0 && C > 0 && S > 0 && (size_t)N * S < (1ull << 31) && C <= 65535, "b2c_bn_backward: channel extent out of range");
-  const bool vec = vec_ok(S, {dy, xnorm, dx});
-  launch_clustered(vec ? bn_bwd_reduce_kernel<true> : bn_bwd_reduce_kernel<false>, bn_cluster_size(N, C, S), C, stream, bn_threads(N, S, false), N, C, S, dy, xnorm, dgamma, dbeta);
+  BnPlan pl;
+  if (int rc = bn_plan(1, 0, N, C, S, {dy, xnorm, dx}, "b2c_bn_backward", &pl)) return rc;
+  const bool vec = pl.vec;
+  launch_clustered(vec ? bn_bwd_reduce_kernel<true> : bn_bwd_reduce_kernel<false>, pl.cs, C, stream, pl.threads, N, C, S, dy, xnorm, dgamma, dbeta);
   B2C_POST_LAUNCH();
   const size_t units = (size_t)N * C * (vec ? S / 4 : S);
   const unsigned blocks = (unsigned)((units + 256 * BN_EW_PER_THREAD - 1) / (256 * BN_EW_PER_THREAD));

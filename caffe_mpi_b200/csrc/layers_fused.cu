@@ -201,16 +201,6 @@ __device__ __forceinline__ void bn_walk_slice(int N, int C, unsigned units, int 
     f(off, idx, ok);
   }
 }
-// the cluster's partial (a, b) pairs added in rank order, by every thread
-__device__ __forceinline__ void bn_cluster_sum(cg::cluster_group& cluster, float2* part, unsigned nranks, double& s1, double& s2) {
-  float2 v[BN_CLUSTER];
-#pragma unroll
-  for (unsigned r = 0; r < (unsigned)BN_CLUSTER; ++r) v[r] = r < nranks ? *cluster.map_shared_rank(part, r) : make_float2(0.f, 0.f);
-  s1 = 0.0; s2 = 0.0;
-#pragma unroll
-  for (unsigned r = 0; r < (unsigned)BN_CLUSTER; ++r) if (r < nranks) { s1 += v[r].x; s2 += v[r].y; }
-}
-
 // statistics (bn_stats_kernel's code and order) + normalisation [+ residual add] [+ ReLU] of one channel per cluster
 // RES: y = [max(0, .)] (BatchNorm(x) + res) -- the Eltwise SUM (and its in-place ReLU) that consumes this layer, folded in
 // CACHE: the slice is parked in dynamic shared memory between the phases (else phase 2 reads x again from global memory / L2)
@@ -229,11 +219,10 @@ bn_fwd_onepass_kernel(int N, int C, int S, const float* __restrict__ x, const fl
                       float eps, float maf, int first, float* __restrict__ mean, float* __restrict__ invstd, float* __restrict__ run_mean,
                       float* __restrict__ run_var, const float* __restrict__ res, float* __restrict__ y) {
   extern __shared__ float4 bn_cache[];
-  __shared__ float2 part;
+  __shared__ float2 part[2];
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
   const int c = blockIdx.y;
-  const float k = x[(size_t)c * S];
   if (CACHE == 2) {
     bn_walk_slice<BN_U>(N, C, VEC ? S / 4 : S, c, rank, nranks, [&](const size_t (&off)[BN_U], const unsigned (&idx)[BN_U], const bool (&ok)[BN_U]) {
 #pragma unroll
@@ -245,16 +234,8 @@ bn_fwd_onepass_kernel(int N, int C, int S, const float* __restrict__ x, const fl
     });
     asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
   }
-  float a, b;
-  bn_channel_partial<VEC, 0, CACHE>(N, C, S, c, x, nullptr, k, rank, nranks, a, b, bn_cache);
-  block_sum2(a, b);
-  if (threadIdx.x == 0) part = make_float2(a, b);
-  cluster.sync();
-  double s1, s2;
-  bn_cluster_sum(cluster, &part, nranks, s1, s2);
-  const double cnt = (double)N * S, m1 = s1 / cnt;
-  const float m = (float)((double)k + m1);
-  const float var_eps = (float)fmax(s2 / cnt - m1 * m1, 0.0) + eps;   // batch_norm_layer.cpp:183-186 (eps folded in before the average)
+  float m, var_eps;
+  bn_channel_stats<VEC, CACHE>(cluster, N, C, S, c, x, eps, part, bn_cache, m, var_eps);
   const float is = 1.0f / sqrtf(var_eps);
   if (rank == 0 && threadIdx.x == 0) {
     mean[c] = m;
@@ -472,8 +453,8 @@ accuracy_kernel(int N, int C, int top_k, const float* __restrict__ scores, const
 __global__ void accuracy_finish_kernel(const unsigned int* hits, int N, float* acc) { *acc = (float)*hits / (float)N; }
 
 // the statistics kernel of layers.cu (same launch for the fused and the unfused forward)
-int launch_bn_stats(int N, int C, int S, const float* x, float eps, float maf, int first, float* mean, float* invstd, float* run_mean,
-                    float* run_var, bool vec, void* stream);
+int launch_bn_stats(const BnPlan& p, int N, int C, int S, const float* x, float eps, float maf, int first, float* mean, float* invstd,
+                    float* run_mean, float* run_var, void* stream);
 
 // B2C_BN_ONEPASS (default 1): statistics / reduction and the elementwise pass in one launch per BatchNorm direction
 static bool bn_onepass() {
@@ -503,31 +484,65 @@ static bool fb_vec_ok(int S, std::initializer_list<const void*> ptrs) {
   return true;
 }
 
+// The one place that picks a BatchNorm training launch (bn_common.cuh).  Every switch is read here, once per process.
+int bn_plan(int dir, int form, int N, int C, int S, std::initializer_list<const void*> ptrs, const char* who, BnPlan* p) {
+  if (dir != 0 && dir != 1) return fail(B2C_ERR_INVALID, "%s: dir must be 0 (forward) or 1 (backward)", who);
+  if (form < 0 || form > 2) return fail(B2C_ERR_INVALID, "%s: form must be 0 (unfused), 1 (fused) or 2 (fused_res)", who);
+  if (!(N > 0 && C > 0 && S > 0 && (size_t)N * S < (1ull << 31) && C <= 65535)) return fail(B2C_ERR_INVALID, "%s: channel extent out of range", who);
+  *p = BnPlan{2, bn_cluster_size(N, C, S), bn_threads(N, S, dir == 0), 0, 0, fb_vec_ok(S, ptrs), 0, 0};
+  const size_t slice = bn_slice_bytes(N, S, p->vec, p->cs, &p->slice_units);
+  if (form == 0 || (form == 1 && !bn_onepass())) return B2C_OK;
+  p->launches = 1;
+  const size_t budget = bn_cache_budget();
+  if (dir == 0) {
+    // B2C_BN_PREFETCH (default 1): cp.async the slice into shared memory before the reduction
+    static const int prefetch = env_int("B2C_BN_PREFETCH", 1);
+    p->park = slice <= budget ? 1 : 0;
+    p->prefetch = p->park && prefetch;
+  } else {
+    // both streams, one (the gradient in the residual form, x otherwise), nothing
+    // B2C_BN_PREFETCH_BWD (default 1; 16.03 -> 15.88 ms per ResNet-50 step): cp.async the parked streams before the reduction
+    static const int prefetch = env_int("B2C_BN_PREFETCH_BWD", 1);
+    p->park = 2 * slice <= budget ? 3 : slice <= budget ? (form == 2 ? 2 : 1) : 0;
+    p->prefetch = p->park && prefetch;
+  }
+  p->smem = (size_t)(p->park == 3 ? 2 : p->park ? 1 : 0) * slice;
+  return B2C_OK;
+}
+
 }  // namespace b2c
 
 using namespace b2c;
 #define FNEED(cond, msg) do { if (!(cond)) return fail(B2C_ERR_INVALID, msg); } while (0)
 
+extern "C" int b2c_debug_bn_plan(int dir, int form, int N, int C, int S, const void* const* ptrs, int nptrs, int* out, int n) {
+  FNEED(out && n >= 6, "b2c_debug_bn_plan: needs out[6]");
+  FNEED(nptrs >= 0 && nptrs <= 6 && (ptrs || !nptrs), "b2c_debug_bn_plan: at most 6 pointers");
+  const void* q[6] = {};
+  for (int i = 0; i < nptrs; ++i) q[i] = ptrs[i];
+  BnPlan p;
+  if (int rc = bn_plan(dir, form, N, C, S, {q[0], q[1], q[2], q[3], q[4], q[5]}, "b2c_debug_bn_plan", &p)) return rc;
+  out[0] = p.launches; out[1] = (int)p.cs; out[2] = (int)p.threads; out[3] = p.park; out[4] = p.prefetch; out[5] = p.vec ? 1 : 0;
+  return B2C_OK;
+}
+
 static int bn_forward_fused_impl(int N, int C, int S, const float* x, const float* gamma, const float* beta, float eps,
                                  float moving_average_fraction, int first_iteration, float* running_mean, float* running_var,
                                  float* save_mean, float* save_invstd, const float* residual, float* y, int relu, void* stream) {
-  FNEED(x && y && save_mean && save_invstd && running_mean && running_var && N > 0 && C > 0 && S > 0, "b2c_bn_forward_train_fused: bad argument");
+  FNEED(x && y && save_mean && save_invstd && running_mean && running_var, "b2c_bn_forward_train_fused: bad argument");
   FNEED((gamma == nullptr) == (beta == nullptr), "b2c_bn_forward_train_fused: gamma and beta go together");
-  FNEED((size_t)N * S < (1ull << 31) && C <= 65535, "b2c_bn_forward_train_fused: channel extent out of range");
+  BnPlan pl;
+  if (int rc = bn_plan(0, residual ? 2 : 1, N, C, S, {x, y, residual}, "b2c_bn_forward_train_fused", &pl)) return rc;
   int dev_count = 0;
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) return fail(B2C_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
-  const bool vec = fb_vec_ok(S, {x, y, residual});
-  if (bn_onepass() || residual) {
-    const unsigned cs = bn_cluster_size(N, C, S);
-    const size_t slice = bn_slice_bytes(N, S, vec, cs, nullptr);
-    // B2C_BN_PREFETCH (default 1): cp.async the slice into shared memory before the reduction
-    static const int prefetch = env_int("B2C_BN_PREFETCH", 1);
-    const int park = slice <= bn_cache_budget() ? (prefetch ? 2 : 1) : 0;
-    const size_t smem = park ? slice : 0;
+  const bool vec = pl.vec;
+  if (pl.launches == 1) {
+    const size_t smem = pl.smem;
+    const int cache = pl.park ? (pl.prefetch ? 2 : 1) : 0;     // the kernel's CACHE: parked by cp.async, by the reduction's loads, not at all
 #define B2C_FWD0(V, R, Q, P) do { if (int rc = bn_onepass_attr(bn_fwd_onepass_kernel<V, R, Q, P>, smem)) return rc; \
-    bn_launch_clustered(bn_fwd_onepass_kernel<V, R, Q, P>, cs, C, smem, stream, bn_threads(N, S, true), N, C, S, x, gamma, beta, eps, moving_average_fraction, first_iteration, \
+    bn_launch_clustered(bn_fwd_onepass_kernel<V, R, Q, P>, pl.cs, C, smem, stream, pl.threads, N, C, S, x, gamma, beta, eps, moving_average_fraction, first_iteration, \
                         save_mean, save_invstd, running_mean, running_var, residual, y); } while (0)
-#define B2C_FWD1(V, R, Q) do { if (park == 2) B2C_FWD0(V, R, Q, 2); else if (park == 1) B2C_FWD0(V, R, Q, 1); else B2C_FWD0(V, R, Q, 0); } while (0)
+#define B2C_FWD1(V, R, Q) do { if (cache == 2) B2C_FWD0(V, R, Q, 2); else if (cache == 1) B2C_FWD0(V, R, Q, 1); else B2C_FWD0(V, R, Q, 0); } while (0)
 #define B2C_FWD2(V, R) do { if (residual) B2C_FWD1(V, R, true); else B2C_FWD1(V, R, false); } while (0)
     if (vec) { if (relu) B2C_FWD2(true, true); else B2C_FWD2(true, false); }
     else { if (relu) B2C_FWD2(false, true); else B2C_FWD2(false, false); }
@@ -537,7 +552,7 @@ static int bn_forward_fused_impl(int N, int C, int S, const float* x, const floa
     B2C_POST_LAUNCH();
     return B2C_OK;
   }
-  if (int rc = launch_bn_stats(N, C, S, x, eps, moving_average_fraction, first_iteration, save_mean, save_invstd, running_mean, running_var, vec, stream)) return rc;
+  if (int rc = launch_bn_stats(pl, N, C, S, x, eps, moving_average_fraction, first_iteration, save_mean, save_invstd, running_mean, running_var, stream)) return rc;
   const size_t units = (size_t)N * C * (vec ? S / 4 : S);
   const unsigned blocks = (unsigned)((units + 256 * FB_EW - 1) / (256 * FB_EW));
   cudaStream_t st = as_stream(stream);
@@ -569,24 +584,21 @@ static int bn_backward_fused_impl(int N, int C, int S, const float* dy, const fl
                                   float* d_residual, int relu, void* stream) {
   FNEED(dy && x && save_mean && save_invstd && dgamma && dbeta && dx, "b2c_bn_backward_fused: null (dgamma/dbeta double as the reduction scratch)");
   FNEED((gamma == nullptr) == (beta == nullptr), "b2c_bn_backward_fused: gamma and beta go together");
-  FNEED(N > 0 && C > 0 && S > 0 && (size_t)N * S < (1ull << 31) && C <= 65535, "b2c_bn_backward_fused: channel extent out of range");
+  BnPlan pl;
+  if (int rc = bn_plan(1, y_mask ? 2 : 1, N, C, S, {dy, dy2, x, dx, y_mask, d_residual}, "b2c_bn_backward_fused", &pl)) return rc;
   int dev_count = 0;
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) return fail(B2C_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
-  const bool vec = fb_vec_ok(S, {dy, dy2, x, dx, y_mask, d_residual});
-  const unsigned cs = bn_cluster_size(N, C, S);
-  if (bn_onepass() || y_mask) {
-    unsigned slice_units = 0;
-    const size_t slice = bn_slice_bytes(N, S, vec, cs, &slice_units);
-    // both streams, one (the gradient in the residual form, x otherwise), nothing
-    const int park = 2 * slice <= bn_cache_budget() ? 3 : slice <= bn_cache_budget() ? (y_mask ? 2 : 1) : 0;
-    const size_t smem = (size_t)(park == 3 ? 2 : park ? 1 : 0) * slice;
+  const bool vec = pl.vec;
+  const unsigned cs = pl.cs;
+  if (pl.launches == 1) {
+    const unsigned slice_units = pl.slice_units;
+    const int park = pl.park;
+    const size_t smem = pl.smem;
     const float inv_cnt1 = 1.0f / ((float)N * S);
-    // B2C_BN_PREFETCH_BWD (default 1; 16.03 -> 15.88 ms per ResNet-50 step): cp.async the parked streams before the reduction
-    static const int prefetch = env_int("B2C_BN_PREFETCH_BWD", 1);
 #define B2C_BWDP(V, M, P, Q) do { if (int rc = bn_onepass_attr(bn_bwd_onepass_kernel<V, M, P, Q>, smem)) return rc; \
-    bn_launch_clustered(bn_bwd_onepass_kernel<V, M, P, Q>, cs, C, smem, stream, bn_threads(N, S, false), N, C, S, inv_cnt1, slice_units, dy, x, y_mask, save_mean, save_invstd, \
+    bn_launch_clustered(bn_bwd_onepass_kernel<V, M, P, Q>, cs, C, smem, stream, pl.threads, N, C, S, inv_cnt1, slice_units, dy, x, y_mask, save_mean, save_invstd, \
                         gamma, beta, dgamma, dbeta, dx, d_residual, dy2); } while (0)
-#define B2C_BWD0(V, M, P) do { if (prefetch && P) B2C_BWDP(V, M, P, true); else B2C_BWDP(V, M, P, false); } while (0)
+#define B2C_BWD0(V, M, P) do { if (pl.prefetch && P) B2C_BWDP(V, M, P, true); else B2C_BWDP(V, M, P, false); } while (0)
 #define B2C_BWD1(V, M) do { if (park == 3) B2C_BWD0(V, M, 3); else if (park == 2) B2C_BWD0(V, M, 2); else if (park == 1) B2C_BWD0(V, M, 1); else B2C_BWD0(V, M, 0); } while (0)
     if (vec) { if (y_mask) B2C_BWD1(true, 2); else if (relu) B2C_BWD1(true, 1); else B2C_BWD1(true, 0); }
     else { if (y_mask) B2C_BWD1(false, 2); else if (relu) B2C_BWD1(false, 1); else B2C_BWD1(false, 0); }
@@ -596,10 +608,10 @@ static int bn_backward_fused_impl(int N, int C, int S, const float* dy, const fl
     B2C_POST_LAUNCH();
     return B2C_OK;
   }
-  if (vec) { if (relu) bn_launch_clustered(bn_bwd_reduce_fused_kernel<true, true>, cs, C, (size_t)0, stream, bn_threads(N, S, false), N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta);
-             else bn_launch_clustered(bn_bwd_reduce_fused_kernel<true, false>, cs, C, (size_t)0, stream, bn_threads(N, S, false), N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta); }
-  else { if (relu) bn_launch_clustered(bn_bwd_reduce_fused_kernel<false, true>, cs, C, (size_t)0, stream, bn_threads(N, S, false), N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta);
-         else bn_launch_clustered(bn_bwd_reduce_fused_kernel<false, false>, cs, C, (size_t)0, stream, bn_threads(N, S, false), N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta); }
+  if (vec) { if (relu) bn_launch_clustered(bn_bwd_reduce_fused_kernel<true, true>, cs, C, (size_t)0, stream, pl.threads, N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta);
+             else bn_launch_clustered(bn_bwd_reduce_fused_kernel<true, false>, cs, C, (size_t)0, stream, pl.threads, N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta); }
+  else { if (relu) bn_launch_clustered(bn_bwd_reduce_fused_kernel<false, true>, cs, C, (size_t)0, stream, pl.threads, N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta);
+         else bn_launch_clustered(bn_bwd_reduce_fused_kernel<false, false>, cs, C, (size_t)0, stream, pl.threads, N, C, S, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta); }
   B2C_POST_LAUNCH();
   const size_t units = (size_t)N * C * (vec ? S / 4 : S);
   const unsigned blocks = (unsigned)((units + 256 * FB_EW - 1) / (256 * FB_EW));

@@ -434,6 +434,17 @@ typedef enum {
 int b2c_debug_pool_plan(int method, int dir, int NC, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
                         const void* out_ptr, const void* mask_ptr, int* out, int n);
 
+/* The launch a BatchNorm training call with these arguments takes.  dir 0 = forward, 1 = backward; form 0 = b2c_bn_forward_train /
+ * b2c_bn_backward, 1 = b2c_bn_*_fused, 2 = b2c_bn_*_fused_res.  ptrs[nptrs] (nptrs <= 6) are the call's tensors -- forward: x, y,
+ * and xnorm or residual; backward: dy, d_sum2, x or xnorm, dx, y_sum, d_residual -- only tested for 16-byte alignment, never
+ * dereferenced; null entries are ignored.  out[0] launches (1: statistics / reduction and elementwise pass in one launch, 2: two),
+ * [1] CTAs per channel (one cluster), [2] threads per CTA of the per-channel kernel, [3] what stays in shared memory between the
+ * two phases (bit 0 = x, bit 1 = the masked gradient), [4] 1 when the parked streams come in by cp.async, [5] 1 for float4 units
+ * (S % 4 == 0 and every pointer aligned), 0 for one float at a time.  Reads the B2C_BN_* switches like the entry points and the
+ * current device's SM count (132 without a device).  Needs n >= 6.  Refuses (B2C_ERR_INVALID) what the entry points refuse about
+ * the shape: N, C or S < 1, N * S >= 2^31, C > 65535.  Pure host computation. */
+int b2c_debug_bn_plan(int dir, int form, int N, int C, int S, const void* const* ptrs, int nptrs, int* out, int n);
+
 #define B2C_UNIQUE_ID_BYTES 128
 int b2c_comm_get_unique_id(void* id_out /* B2C_UNIQUE_ID_BYTES */);
 int b2c_comm_init(int nranks, int rank, const void* id, b2c_comm** out);

@@ -1,6 +1,7 @@
 """CPU tests of the drop-in boundary: libb2c.so loads, exports every symbol include/b2c.h declares,
 validates arguments like the reference's LayerSetUp CHECKs, and refuses to compute without a GPU."""
 import ctypes as C
+import os
 
 import pytest
 
@@ -235,6 +236,71 @@ def test_pool_plan_routes():
     with pytest.raises(capi.B2CError):
         capi.pool_plan(0, 0, 0, 8, 8, (3, 3), (1, 1), (0, 0))              # no planes
     assert L.b2c_debug_pool_plan(0, 0, 4, 8, 8, 3, 3, 1, 1, 0, 0, one, one, (C.c_int * 4)(), 4) == -1     # n < 5
+
+
+@pytest.mark.skipif(any(k.startswith("B2C_BN_") for k in os.environ), reason="the table is the default switches'")
+def test_bn_plan_regimes():
+    """b2c_debug_bn_plan is host-only: the launch every BatchNorm training entry point takes (the regimes test_bn_schedule_gpu.py
+    runs), at 132 SMs (an H100 SXM, and the count without a device), and the shapes the entry points refuse"""
+    A, OFF4 = 1 << 20, (1 << 20) + 4
+    sms = 132
+    try:
+        import torch
+        if torch.cuda.is_available():
+            sms = torch.cuda.get_device_properties(0).multi_processor_count
+    except Exception:
+        pass
+    if sms != 132:
+        pytest.skip(f"the table is 132 SMs' ({sms} here)")
+
+    def plan(d, form, N, Cc, H, W, ptr=A):
+        q = capi.bn_plan(d, form, N, Cc, H * W, [ptr])
+        return q["launches"], q["cs"], q["threads"], q["park"], q["prefetch"], q["vec"]
+    # (N, C, H, W): forward fused, backward fused, backward fused_res -- (launches, cs, threads, park, prefetch, float4)
+    table = [
+        ((64, 64, 112, 112), (1, 8, 512, 0, 0, True), (1, 8, 512, 0, 0, True), (1, 8, 512, 0, 0, True)),     # bn_conv1: 392 KB slices
+        ((64, 64, 56, 56), (1, 8, 512, 1, 1, True), (1, 8, 512, 1, 1, True), (1, 8, 512, 2, 1, True)),        # res2: 98 KB slices
+        ((64, 256, 56, 56), (1, 8, 512, 1, 1, True), (1, 8, 512, 1, 1, True), (1, 8, 512, 2, 1, True)),
+        ((64, 128, 28, 28), (1, 2, 512, 1, 1, True), (1, 2, 512, 1, 1, True), (1, 2, 512, 2, 1, True)),       # res3
+        ((64, 512, 28, 28), (1, 2, 512, 1, 1, True), (1, 2, 512, 1, 1, True), (1, 2, 512, 2, 1, True)),
+        ((64, 256, 14, 14), (1, 1, 256, 1, 1, True), (1, 1, 512, 3, 1, True), (1, 1, 512, 3, 1, True)),       # res4: 256-thread forward
+        ((64, 1024, 14, 14), (1, 1, 256, 1, 1, True), (1, 1, 512, 3, 1, True), (1, 1, 512, 3, 1, True)),
+        ((64, 512, 7, 7), (1, 1, 128, 1, 1, False), (1, 1, 128, 3, 1, False), (1, 1, 128, 3, 1, False)),     # res5: S = 49, scalar
+        ((64, 2048, 7, 7), (1, 1, 128, 1, 1, False), (1, 1, 128, 3, 1, False), (1, 1, 128, 3, 1, False)),
+        ((64, 40, 35, 35), (1, 4, 512, 1, 1, False), (1, 4, 512, 1, 1, False), (1, 4, 512, 2, 1, False)),     # scalar, 512 threads, cs 4
+        ((37, 70, 30, 30), (1, 2, 512, 1, 1, True), (1, 2, 512, 1, 1, True), (1, 2, 512, 2, 1, True)),        # slices end mid-plane
+    ]
+    for shape, f, b, r in table:
+        assert plan(0, "fused", *shape) == plan(0, "fused_res", *shape) == f, (shape, plan(0, "fused", *shape))
+        assert plan(1, "fused", *shape) == b, (shape, plan(1, "fused", *shape))
+        assert plan(1, "fused_res", *shape) == r, (shape, plan(1, "fused_res", *shape))
+        for d, one in ((0, f), (1, b)):          # the unfused layers: the same reduction geometry, two launches, nothing parked
+            assert plan(d, "unfused", *shape) == (2, one[1], one[2], 0, 0, one[5]), (shape, d)
+    # one pointer 4 bytes off 16-byte alignment takes every form to one float at a time; null pointers do not count
+    for d in (0, 1):
+        for form in capi.BN_FORMS:
+            assert plan(d, form, 64, 256, 14, 14, OFF4)[5] is False
+            assert capi.bn_plan(d, form, 64, 256, 196, [A, None, A])["vec"] is True
+    # refused, by the query and by the entry points, before anything is launched
+    L = m.lib()
+    one = C.c_void_p(A)
+    for N, Cc, S in ((0, 4, 4), (4, 0, 4), (4, 4, 0), (-1, 4, 4), (4, 65536, 4), (1 << 16, 4, 1 << 15)):
+        for d in (0, 1):
+            for form in capi.BN_FORMS:
+                with pytest.raises(capi.B2CError, match="channel extent out of range"):
+                    capi.bn_plan(d, form, N, Cc, S, [A])
+        assert L.b2c_bn_forward_train(N, Cc, S, one, None, None, 1e-5, 0.9, 1, one, one, one, one, one, one, None) == -1
+        assert L.b2c_bn_backward(N, Cc, S, one, one, None, one, one, one, one, None) == -1
+        assert L.b2c_bn_forward_train_fused(N, Cc, S, one, None, None, 1e-5, 0.9, 1, one, one, one, one, one, 0, None) == -1
+        assert L.b2c_bn_backward_fused(N, Cc, S, one, one, one, one, None, None, one, one, one, 0, None) == -1
+        assert L.b2c_bn_forward_train_fused_res(N, Cc, S, one, None, None, 1e-5, 0.9, 1, one, one, one, one, one, one, 1, None) == -1
+        assert L.b2c_bn_backward_fused_res(N, Cc, S, one, None, one, one, one, one, None, None, one, one, one, None, None) == -1
+    out = (C.c_int * 6)()
+    ptrs = (C.c_void_p * 1)(A)
+    assert L.b2c_debug_bn_plan(2, 0, 4, 4, 4, ptrs, 1, out, 6) == -1                  # dir
+    assert L.b2c_debug_bn_plan(0, 3, 4, 4, 4, ptrs, 1, out, 6) == -1                  # form
+    assert L.b2c_debug_bn_plan(0, 0, 4, 4, 4, ptrs, 7, out, 6) == -1                  # more than 6 pointers
+    assert L.b2c_debug_bn_plan(0, 0, 4, 4, 4, ptrs, 1, out, 5) == -1                  # n < 6
 
 
 def test_no_cpu_fallback():
