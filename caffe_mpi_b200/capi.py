@@ -19,6 +19,8 @@ WGRAD_ROUTES = ("caffe", "simt", "gather", "staged_3x3", "staged_3x3_plane", "st
 CONV_ROUTES = ("caffe", "simt", "gather", "gather_scatter", "staged", "staged_plane")
 # b2c_pool_route, in enum order
 POOL_ROUTES = ("max_scalar", "max_window", "max_bwd_row", "max_bwd_quad", "ave")
+# b2c_sgemm_route, in enum order
+SGEMM_ROUTES = ("ffma", "tc")
 
 
 class B2CError(RuntimeError):
@@ -119,6 +121,7 @@ def lib():
         "b2c_sgemm_tc_supported": (i, [i, i, i, i, i]),
         "b2c_transpose": (i, [i, i, vp, vp, vp]),
         "b2c_sgemm_ex": (i, [i, i, i, i, i, f, vp, vp, f, vp, vp, sz, vp]),
+        "b2c_debug_sgemm_plan": (i, [i, i, i, i, i, f, f, vp, vp, vp, sz, C.POINTER(i), i]),
         "b2c_sgd_update": (i, [sz, vp, vp, vp, f, f, f, i, f, i, vp]),
         "b2c_sgd_update_arena": (i, [i, C.POINTER(sz), C.POINTER(sz), C.POINTER(f), C.POINTER(f), vp, vp, vp,
                                      f, i, f, i, vp]),
@@ -372,6 +375,16 @@ def sgemm_ex(transA, transB, M, N, K, alpha, A, B, beta, Cm, stream=None):
     ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=Cm.device)
     check(L.b2c_sgemm_ex(int(transA), int(transB), M, N, K, alpha, _p(A), _p(B), beta, _p(Cm), _p(ws), nbytes, _stream(stream)))
     return Cm, nbytes
+
+
+def sgemm_plan(transA, transB, M, N, K, alpha, beta, A=0, B=0, workspace=0, workspace_bytes=0):
+    """b2c_debug_sgemm_plan: the kernel b2c_sgemm_ex takes for these arguments, with A, B and the workspace at these addresses
+    (integers; never dereferenced; 0 = null workspace)"""
+    out = (C.c_int * 7)()
+    check(lib().b2c_debug_sgemm_plan(int(transA), int(transB), M, N, K, alpha, beta, C.c_void_p(A), C.c_void_p(B),
+                                     C.c_void_p(workspace or None), workspace_bytes, out, 7))
+    return dict(route=SGEMM_ROUTES[out[0]], cols=out[1], bpi=out[2], splits=out[3], kb_per_split=out[4], m_tiles=out[5],
+                n_tiles=out[6])
 
 
 def sgemv(transA, M, N, alpha, A, x, beta, y, stream=None):

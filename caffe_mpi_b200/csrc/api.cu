@@ -461,9 +461,12 @@ extern "C" int b2c_conv_backward_bias(const b2c_conv_desc* d, const float* dy, f
   return launch_bias_grad(d->s.N, d->s.O, d->s.Ho * d->s.Wo, dy, db, as_stream(stream));
 }
 
+// NoTrans x Trans products (InnerProduct forward) run on the tensor cores, fp32-equivalent bf16x3 math, unless the default algo or
+// math rules them out; everything else -- and any alpha / beta / alignment the staged kernel does not take -- on the exact-fp32
+// FFMA kernel (sgemm_route)
+static bool sgemm_tc_allowed() { return g_default_algo != B2C_ALGO_SIMT && g_default_math == B2C_MATH_FP32; }
 extern "C" int b2c_sgemm_tc_supported(int transA, int transB, int M, int N, int K) {
-  return M > 0 && N > 0 && K > 0 && have_device() && g_default_algo != B2C_ALGO_SIMT && g_default_math == B2C_MATH_FP32 &&
-         tc_gemm_supported(transA != 0, transB != 0, M, N, K) ? 1 : 0;
+  return M > 0 && N > 0 && K > 0 && have_device() && sgemm_tc_allowed() && tc_gemm_supported(transA != 0, transB != 0, M, N, K) ? 1 : 0;
 }
 extern "C" size_t b2c_sgemm_workspace_bytes(int transA, int transB, int M, int N, int K) {
   if (M <= 0 || N <= 0 || K <= 0 || !have_device()) return 0;
@@ -479,10 +482,18 @@ extern "C" int b2c_sgemm_ex(int transA, int transB, int M, int N, int K, float a
   REQUIRE_DEVICE();
   if (M == 0 || N == 0) return B2C_OK;
   const bool tA = transA != 0, tB = transB != 0;
-  // NoTrans x Trans products (InnerProduct forward) on the tensor cores, fp32-equivalent bf16x3 math; everything else -- and any
-  // alpha / beta / alignment the staged kernel does not take -- on the exact-fp32 FFMA kernel
-  if (g_default_algo != B2C_ALGO_SIMT && g_default_math == B2C_MATH_FP32 && alpha == 1.0f && (beta == 0.0f || beta == 1.0f) &&
-      ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 15u) == 0 && tc_gemm_supported(tA, tB, M, N, K))
-    return launch_sgemm_tc(tA, tB, M, N, K, alpha, A, B, beta, C, g_default_math, workspace, workspace_bytes, as_stream(stream));
+  GemmPlan g;
+  sgemm_route(sgemm_tc_allowed(), tA, tB, M, N, K, alpha, beta, A, B, workspace, workspace_bytes, &g);
+  if (g.tc) return launch_sgemm_tc(g, M, N, K, A, B, beta, C, workspace, workspace_bytes, as_stream(stream));
   return launch_sgemm_simt(tA, tB, M, N, K, alpha, A, tA ? M : K, B, tB ? K : N, beta, C, N, as_stream(stream));
+}
+extern "C" int b2c_debug_sgemm_plan(int transA, int transB, int M, int N, int K, float alpha, float beta, const void* A, const void* B,
+                                    const void* workspace, size_t workspace_bytes, int* out, int n) {
+  if (!out || n < 7) return fail(B2C_ERR_INVALID, "b2c_debug_sgemm_plan: needs out[7]");
+  if (M < 0 || N < 0 || K < 0) return fail(B2C_ERR_INVALID, "b2c_debug_sgemm_plan: negative extent");
+  GemmPlan g;
+  sgemm_route(sgemm_tc_allowed(), transA != 0, transB != 0, M, N, K, alpha, beta, A, B, workspace, workspace_bytes, &g);
+  out[0] = g.tc ? B2C_SGEMM_ROUTE_TC : B2C_SGEMM_ROUTE_FFMA; out[1] = g.cols; out[2] = g.bpi; out[3] = g.splits;
+  out[4] = g.kb_per_split; out[5] = g.m_tiles; out[6] = g.n_tiles;
+  return B2C_OK;
 }

@@ -123,8 +123,18 @@ int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, 
 bool tc_wgrad_stg_plan_info(const ConvShape&, WgradPlanInfo*);
 bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K);
 size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K);
-int launch_sgemm_tc(bool tA, bool tB, int M, int N, int K, float alpha, const float* A, const float* B, float beta,
-                    float* C, int math, void* ws, size_t ws_bytes, cudaStream_t);
+// The kernel b2c_sgemm_ex runs and its plan, decided in one place (sgemm_route) for the launch and for b2c_debug_sgemm_plan.
+// tc: the staged 1x1 kernel (wgrad_stg_kernel<1, cols>) on 128 x cols tiles, bpi K blocks of 64, split over `splits` CTAs of
+// kb_per_split blocks each; else the FFMA kernel (sgemm_simt_kernel) on 64 x 64 tiles, bpi = kb_per_split = K steps of 16.
+struct GemmPlan {
+  bool tc;
+  int cols, bpi, splits, kb_per_split, m_tiles, n_tiles;
+};
+// tc_allowed: the default algo and math let the tensor cores run (not SIMT, fp32 math).  Pointers are only tested for alignment.
+void sgemm_route(bool tc_allowed, bool tA, bool tB, int M, int N, int K, float alpha, float beta, const void* A, const void* B,
+                 const void* ws, size_t ws_bytes, GemmPlan* g);
+int launch_sgemm_tc(const GemmPlan& g, int M, int N, int K, const float* A, const float* B, float beta, float* C, void* ws,
+                    size_t ws_bytes, cudaStream_t);
 
 }  // namespace b2c
 

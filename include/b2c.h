@@ -173,15 +173,29 @@ int b2c_sgemm(int transA, int transB, int M, int N, int K, float alpha, const fl
 /* The same product with caller-provided scratch (b2c_sgemm_workspace_bytes(...) bytes, 16-byte aligned; may be null / short: then
  * as b2c_sgemm).  With it the NoTrans x Trans tensor-core path splits the K loop over one wave of CTAs and reduces the partial
  * tiles in a fixed order (deterministic) -- InnerProduct forward at small batch is otherwise one CTA per 128 x 128 output tile. */
-/* 1 when b2c_sgemm / b2c_sgemm_ex would run this product (alpha = 1, beta in {0, 1}, 16-byte aligned operands) on the tensor cores:
- * NoTrans x Trans, K >= 64, K % 4 == 0, default math = fp32-equivalent.  Callers that can choose their operand layout
- * (InnerProductLayer::Backward_gpu with transposed copies) ask before preparing them. */
+/* 1 when b2c_sgemm_ex with its workspace would run this product (alpha = 1, beta in {0, 1}, 16-byte aligned operands) on the
+ * tensor cores: NoTrans x Trans, K >= 64, K % 4 == 0, default math = fp32-equivalent.  Callers that can choose their operand layout
+ * (InnerProductLayer::Backward_gpu with transposed copies) ask before preparing them.  Without a usable workspace a product whose
+ * K loop the planner would split runs unsplit, and on the FFMA kernel once K exceeds 256 blocks of 64 (one fp32 accumulator
+ * chain that long is not fp32-accurate); b2c_debug_sgemm_plan tells. */
 int b2c_sgemm_tc_supported(int transA, int transB, int M, int N, int K);
 size_t b2c_sgemm_workspace_bytes(int transA, int transB, int M, int N, int K);
 /* dst[c][r] = src[r][c] (rows x cols -> cols x rows), src != dst. */
 int b2c_transpose(int rows, int cols, const float* src, float* dst, void* stream);
 int b2c_sgemm_ex(int transA, int transB, int M, int N, int K, float alpha, const float* A, const float* B, float beta, float* C,
                  void* workspace, size_t workspace_bytes, void* stream);
+/* The kernel b2c_sgemm_ex runs (b2c_debug_sgemm_plan out[0]). */
+typedef enum {
+  B2C_SGEMM_ROUTE_FFMA = 0,   /* exact-fp32 FFMA kernel: one sequential fmaf chain over k per element, 64 x 64 tiles, K steps of 16 */
+  B2C_SGEMM_ROUTE_TC = 1      /* NoTrans x Trans on the staged bf16x3 tensor-core kernel: 128 x cols tiles, K blocks of 64        */
+} b2c_sgemm_route;
+/* Which kernel b2c_sgemm_ex takes for these arguments and its plan; A, B and workspace are only tested for alignment, never
+ * dereferenced.  out[0] route (b2c_sgemm_route), [1] tile columns (64 or 128), [2] K blocks in all (64 wide on the tensor cores, 16
+ * on the FFMA kernel), [3] split count of the K loop, [4] K blocks per split (1 split after a null, short or misaligned workspace),
+ * [5] M tiles, [6] N tiles.  Reads the default math and algo like the entry point.  Needs n >= 7.  Pure host computation: splits
+ * follow the current device's SM count (132 without a device). */
+int b2c_debug_sgemm_plan(int transA, int transB, int M, int N, int K, float alpha, float beta, const void* A, const void* B,
+                         const void* workspace, size_t workspace_bytes, int* out, int n);
 /* y = alpha*op(A)*x + beta*y, A row-major MxN.
  * Replaces caffe_gpu_gemv<float> -> cublasSgemv (math_functions.cu:73-82).               */
 int b2c_sgemv(int transA, int M, int N, float alpha, const float* A, const float* x,

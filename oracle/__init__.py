@@ -90,6 +90,8 @@ def lib():
         L.b2o_col2im_nd.argtypes = [_f32p, C.c_int] + [_i32p] * 6 + [_f32p]
         L.b2o_gemm.argtypes = [C.c_int] * 5 + [C.c_float, _f32p, _f32p, C.c_float, _f32p, C.c_int]
         L.b2o_gemv.argtypes = [C.c_int] * 3 + [C.c_float, _f32p, _f32p, C.c_float, _f32p, C.c_int]
+        L.b2o_gemm_ffma.argtypes = [C.c_int] * 5 + [C.c_float, _f32p, _f32p, C.c_float, _f32p, _f32p]
+        L.b2o_gemv_ffma.argtypes = [C.c_int] * 3 + [C.c_float, _f32p, _f32p, C.c_float, _f32p, _f32p]
         L.b2o_conv_forward.argtypes = [P, _f32p, _f32p, C.c_void_p, _f32p, C.c_int]
         L.b2o_conv_backward.argtypes = [P, _f32p, _f32p, _f32p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.b2o_conv_direct.argtypes = [P, _f32p, _f32p, C.c_void_p, _f32p]
@@ -160,6 +162,34 @@ def gemv(transA, M, N, alpha, A, x, beta, y, acc64=False):
     lib().b2o_gemv(int(transA), M, N, alpha, np.ascontiguousarray(A, np.float32).ravel(),
                    np.ascontiguousarray(x, np.float32), beta, y, int(acc64))
     return y
+
+
+def gemm_ffma(transA, transB, M, N, K, alpha, A, B, beta, Cm):
+    """What the product's FFMA GEMM kernel (sgemm_simt_kernel) stores, bit for bit: an array [3, M, N] of the admissible results
+    (the three ways alpha * acc + beta * c may be contracted; all equal when beta == 0).  A, B: op(A) is M x K, op(B) K x N in
+    the row-major layouts b2c_sgemm takes; Cm: C before the call."""
+    out = np.empty((3, M, N), np.float32)
+    lib().b2o_gemm_ffma(int(transA), int(transB), M, N, K, alpha, np.ascontiguousarray(A, np.float32).reshape(-1),
+                        np.ascontiguousarray(B, np.float32).reshape(-1), beta, np.ascontiguousarray(Cm, np.float32).reshape(-1),
+                        out.reshape(-1))
+    return out
+
+
+def gemv_ffma(transA, M, N, alpha, A, x, beta, y):
+    """What the product's FFMA GEMV kernels store, bit for bit: [3, len(y)] admissible results, as gemm_ffma.  A is M x N."""
+    n = N if transA else M
+    out = np.empty((3, n), np.float32)
+    lib().b2o_gemv_ffma(int(transA), M, N, alpha, np.ascontiguousarray(A, np.float32).reshape(-1),
+                        np.ascontiguousarray(x, np.float32).reshape(-1), beta, np.ascontiguousarray(y, np.float32).reshape(-1),
+                        out.reshape(-1))
+    return out
+
+
+def ffma_match(got, admissible):
+    """mask of the elements of `got` equal, bit for bit (int32 views: a zero's sign counts), to one of the admissible results"""
+    g = np.ascontiguousarray(got, np.float32).view(np.int32)
+    a = np.ascontiguousarray(admissible, np.float32).view(np.int32)
+    return (g == a[0]) | (g == a[1]) | (g == a[2])
 
 
 def conv_forward(prm, x, w, bias=None, acc64=False):

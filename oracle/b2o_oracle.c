@@ -186,6 +186,80 @@ void b2o_gemv(int transA, int M, int N, float alpha, const float* A,
 }
 
 /* ------------------------------------------------------------------------- *
+ * Bit-exact emulators of the product's FFMA GEMM / GEMV kernels
+ * (caffe_mpi_b200/csrc/sgemm_simt.cu), so a test can compare them bit for bit:
+ *   sgemm_simt_kernel: acc = fmaf(a_k, b_k, acc) for k = 0 .. 16*ceil(K/16) - 1,
+ *     starting from +0, with a_k = b_k = 0 past K (the zero-padded tail of the
+ *     last 16-wide K tile, which turns an acc of -0 into +0);
+ *   sgemv_n_kernel: lane l of a warp runs the chain over k = l, l + 32, ... < N,
+ *     then s += shfl_xor(s, o) for o = 16, 8, 4, 2, 1; lane 0's value is kept;
+ *   sgemv_t_kernel: one chain over the rows r = 0 .. M - 1.
+ * Then the store: beta == 0 gives fl(alpha * acc).  Otherwise the compiler may
+ * contract alpha * acc + beta * c either way, so out[0..2] receive the three
+ * admissible results fl(fl(a*acc) + fl(b*c)), fma(a, acc, fl(b*c)) and
+ * fma(b, c, fl(a*acc)) (identical when beta == 0).  out: 3 planes of M x N
+ * (GEMM) or of the length of y (GEMV).  C / y: the values before the call.
+ * ------------------------------------------------------------------------- */
+static void ffma_store(float alpha, float acc, float beta, float c, float* out, size_t plane, size_t idx) {
+  if (beta == 0.0f) {
+    const float v = alpha * acc;
+    out[idx] = out[plane + idx] = out[2 * plane + idx] = v;
+    return;
+  }
+  const float ta = alpha * acc, tb = beta * c;
+  out[idx] = ta + tb;
+  out[plane + idx] = fmaf(alpha, acc, tb);
+  out[2 * plane + idx] = fmaf(beta, c, ta);
+}
+void b2o_gemm_ffma(int transA, int transB, int M, int N, int K, float alpha, const float* A, const float* B, float beta,
+                   const float* C, float* out) {
+  const int lda = transA ? M : K, ldb = transB ? K : N;
+  const int kpad = (K + 15) / 16 * 16;
+  const size_t plane = (size_t)M * N;
+  /* op(B) as K x N rows so the j loop runs over contiguous memory; each element keeps its own sequential chain over k */
+  float* bt = (float*)malloc(sizeof(float) * ((size_t)K * N + 1));
+  float* acc = (float*)malloc(sizeof(float) * ((size_t)N + 1));
+  for (int k = 0; k < K; ++k)
+    for (int j = 0; j < N; ++j) bt[(size_t)k * N + j] = transB ? B[(size_t)j * ldb + k] : B[(size_t)k * ldb + j];
+  for (int i = 0; i < M; ++i) {
+    for (int j = 0; j < N; ++j) acc[j] = 0.0f;
+    for (int k = 0; k < K; ++k) {
+      const float a = transA ? A[(size_t)k * lda + i] : A[(size_t)i * lda + k];
+      const float* b = bt + (size_t)k * N;
+      for (int j = 0; j < N; ++j) acc[j] = fmaf(a, b[j], acc[j]);
+    }
+    for (int k = K; k < kpad; ++k)
+      for (int j = 0; j < N; ++j) acc[j] = fmaf(0.0f, 0.0f, acc[j]);
+    for (int j = 0; j < N; ++j) ffma_store(alpha, acc[j], beta, C[(size_t)i * N + j], out, plane, (size_t)i * N + j);
+  }
+  free(bt);
+  free(acc);
+}
+void b2o_gemv_ffma(int transA, int M, int N, float alpha, const float* A, const float* x, float beta, const float* y,
+                   float* out) {
+  if (!transA) {
+    for (int r = 0; r < M; ++r) {
+      float s[32], t[32];
+      for (int l = 0; l < 32; ++l) {
+        s[l] = 0.0f;
+        for (int k = l; k < N; k += 32) s[l] = fmaf(A[(size_t)r * N + k], x[k], s[l]);
+      }
+      for (int o = 16; o; o >>= 1) {
+        for (int l = 0; l < 32; ++l) t[l] = s[l] + s[l ^ o];
+        for (int l = 0; l < 32; ++l) s[l] = t[l];
+      }
+      ffma_store(alpha, s[0], beta, y[r], out, (size_t)M, (size_t)r);
+    }
+  } else {
+    for (int c = 0; c < N; ++c) {
+      float s = 0.0f;
+      for (int r = 0; r < M; ++r) s = fmaf(A[(size_t)r * N + c], x[r], s);
+      ffma_store(alpha, s, beta, y[c], out, (size_t)N, (size_t)c);
+    }
+  }
+}
+
+/* ------------------------------------------------------------------------- *
  * ConvolutionLayer::Forward_cpu (src/caffe/layers/conv_layer.cpp:24-40) with
  * forward_cpu_gemm / forward_cpu_bias (include/caffe/layers/base_conv_layer.hpp:36-60).
  * Per image: col = im2col(x_n) unless is_1x1_ (base_conv_layer.cpp:99-103),

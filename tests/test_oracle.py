@@ -42,6 +42,107 @@ def test_gemv_known_answers():
     assert np.array_equal(o.gemv(1, 3, 2, 1.0, A, A[:3], 0.0, np.zeros(2, np.float32)), [22, 28])
 
 
+# ---- FFMA emulators (b2o_gemm_ffma / b2o_gemv_ffma): the bit-exact yardstick of the product's FFMA GEMM / GEMV kernels ------
+U32 = 2.0 ** -24
+
+
+def gamma(n):
+    return n * U32 / (1 - n * U32)
+
+
+def test_gemm_ffma_known_answers():
+    data = np.arange(1, 13, dtype=np.float32)
+    A, B = data[:6], data
+    At = np.array([1, 4, 2, 5, 3, 6], np.float32)
+    Bt = np.array([1, 5, 9, 2, 6, 10, 3, 7, 11, 4, 8, 12], np.float32)
+    want = np.array([38, 44, 50, 56, 83, 98, 113, 128], np.float32).reshape(2, 4)
+    z = np.zeros((2, 4), np.float32)
+    for tA, tB, a, b in ((0, 0, A, B), (1, 0, At, B), (1, 1, At, Bt), (0, 1, A, Bt)):
+        out = o.gemm_ffma(tA, tB, 2, 4, 3, 1.0, a, b, 0.0, z)
+        assert np.array_equal(out, np.broadcast_to(want, out.shape)), (tA, tB)
+        # alpha and beta: 0.5 * AB + 2 * C0 is exact in every contraction
+        c0 = np.arange(8, dtype=np.float32).reshape(2, 4)
+        out = o.gemm_ffma(tA, tB, 2, 4, 3, 0.5, a, b, 2.0, c0)
+        assert np.array_equal(out, np.broadcast_to(0.5 * want + 2 * c0, out.shape))
+    # K = 0: beta * C exactly; alpha * (+0) keeps alpha's sign where beta = 0
+    c0 = np.array([[1.5, -2.0]], np.float32)
+    assert np.array_equal(o.gemm_ffma(0, 0, 1, 2, 0, 1.0, np.zeros(1, np.float32), np.zeros(1, np.float32), -2.0, c0)[0], -2 * c0)
+    neg = o.gemm_ffma(0, 0, 1, 2, 0, -3.0, np.zeros(1, np.float32), np.zeros(1, np.float32), 0.0, c0)
+    assert (neg.view(np.int32) == np.float32(-0.0).view(np.int32)).all()
+
+
+def test_gemv_ffma_known_answers():
+    A = np.arange(1, 7, dtype=np.float32)
+    assert np.array_equal(o.gemv_ffma(0, 2, 3, 1.0, A, A[:3], 0.0, np.zeros(2, np.float32))[0], [14, 32])
+    assert np.array_equal(o.gemv_ffma(1, 2, 3, 1.0, A, A[:2], 0.0, np.zeros(3, np.float32))[0], [9, 12, 15])
+    assert np.array_equal(o.gemv_ffma(0, 3, 2, 1.0, A, A[:2], 0.0, np.zeros(3, np.float32))[0], [5, 11, 17])
+    assert np.array_equal(o.gemv_ffma(1, 3, 2, 1.0, A, A[:3], 1.0, np.ones(2, np.float32))[2], [23, 29])
+
+
+def test_gemm_ffma_padded_tail_turns_minus_zero_into_plus_zero():
+    """sgemm_simt_kernel runs 16-wide K tiles with zeros past K: fmaf(0, 0, -0) = +0.  A product that underflows to -0 in the last
+    real step survives when K % 16 == 0 and is lost to the padding otherwise"""
+    for K, sign in ((16, -0.0), (15, 0.0), (1, 0.0)):
+        a = np.zeros(K, np.float32)
+        b = np.zeros(K, np.float32)
+        a[K - 1], b[K - 1] = -1e-30, 1e-30
+        got = o.gemm_ffma(0, 1, 1, 1, K, 1.0, a, b, 0.0, np.zeros((1, 1), np.float32))[0]
+        assert got.view(np.int32)[0, 0] == np.float32(sign).view(np.int32), (K, got)
+
+
+@pytest.mark.parametrize("tA,tB", [(0, 0), (0, 1), (1, 0), (1, 1)])
+@pytest.mark.parametrize("alpha,beta", [(1.0, 0.0), (-3.0, 1.0), (0.5, -2.0)])
+def test_gemm_ffma_within_classic_bound(rng, tA, tB, alpha, beta):
+    """|ffma - exact| <= gamma_{Kp + 2} (|alpha| sum_k |a_k b_k| + |beta c|): one rounding per chain step, two in the store"""
+    M, N, K = 37, 29, 100
+    a = rng.standard_normal((K, M) if tA else (M, K)).astype(np.float32)
+    b = rng.standard_normal((N, K) if tB else (K, N)).astype(np.float32)
+    c0 = rng.standard_normal((M, N)).astype(np.float32)
+    opA = (a.T if tA else a).astype(np.float64)
+    opB = (b.T if tB else b).astype(np.float64)
+    exact = alpha * (opA @ opB) + beta * c0
+    mag = abs(alpha) * (np.abs(opA) @ np.abs(opB)) + abs(beta) * np.abs(c0)
+    out = o.gemm_ffma(tA, tB, M, N, K, alpha, a, b, beta, c0)
+    for r in out:
+        assert (np.abs(r - exact) <= gamma(112 + 2) * mag).all()
+    if beta == 0.0:                                    # nothing to contract: one answer
+        assert np.array_equal(out[0], out[1]) and np.array_equal(out[0], out[2])
+    elif alpha == -3.0:                                # fl(-3 acc) rounds: the contractions differ somewhere
+        assert not np.array_equal(out[0], out[1])
+
+
+@pytest.mark.parametrize("tA", [0, 1])
+def test_gemv_ffma_within_classic_bound(rng, tA):
+    M, N = 300, 1000
+    A = rng.standard_normal((M, N)).astype(np.float32)
+    x = rng.standard_normal(M if tA else N).astype(np.float32)
+    y0 = rng.standard_normal(N if tA else M).astype(np.float32)
+    opA = (A.T if tA else A).astype(np.float64)
+    exact = 0.5 * (opA @ x) + y0
+    mag = 0.5 * (np.abs(opA) @ np.abs(x)) + np.abs(y0)
+    steps = M if tA else (N + 31) // 32 + 5            # the chain (and, NoTrans, the five butterfly adds)
+    for r in o.gemv_ffma(tA, M, N, 0.5, A, x, 1.0, y0):
+        assert (np.abs(r - exact) <= gamma(steps + 2) * mag).all()
+
+
+def test_ffma_emulators_are_order_sensitive(rng):
+    """reversing the k order changes the bits on random data: a kernel that summed in another order would fail a bit-exact check"""
+    M, N, K = 64, 64, 100
+    a = rng.standard_normal((M, K)).astype(np.float32)
+    b = rng.standard_normal((K, N)).astype(np.float32)
+    z = np.zeros((M, N), np.float32)
+    fwd = o.gemm_ffma(0, 0, M, N, K, 1.0, a, b, 0.0, z)[0]
+    rev = o.gemm_ffma(0, 0, M, N, K, 1.0, a[:, ::-1], b[::-1], 0.0, z)[0]
+    assert np.mean(fwd.view(np.int32) != rev.view(np.int32)) > 0.5
+    # the GEMV's lane-strided chains and butterfly are not a sequential sum either
+    A = rng.standard_normal((200, 1000)).astype(np.float32)
+    x = rng.standard_normal(1000).astype(np.float32)
+    n = o.gemv_ffma(0, 200, 1000, 1.0, A, x, 0.0, np.zeros(200, np.float32))[0]
+    seq = o.gemv_ffma(1, 1000, 200, 1.0, np.ascontiguousarray(A.T), x, 0.0, np.zeros(200, np.float32))[0]
+    assert np.mean(n.view(np.int32) != seq.view(np.int32)) > 0.5
+    assert np.mean(o.ffma_match(n, np.stack([seq] * 3))) < 0.5
+
+
 # ---- im2col: reference source compiled verbatim (test_im2col_kernel.cu:102-212 shapes) ------------
 # golden/im2col_ref_sha256.json: SHA-256 of what the reference's own im2col.cpp (2-D and N-D, compiled verbatim by
 # tests/golden/make_golden.py) returns for these inputs; equal digests = bit-identical outputs.
