@@ -127,6 +127,8 @@ def lib():
                                      f, i, f, i, vp]),
         "b2c_solver_update_arena": (i, [i, i, C.POINTER(sz), C.POINTER(sz), C.POINTER(f), C.POINTER(f), vp, vp, vp, vp,
                                         SolverHParams, i, f, i, vp]),
+        "b2c_debug_solver_plan": (i, [i, i, C.POINTER(sz), C.POINTER(sz), vp, vp, vp, vp, C.POINTER(i), i, C.POINTER(i),
+                                      C.POINTER(C.c_longlong)]),
         "b2c_relu_forward": (i, [sz, vp, vp, f, vp]),
         "b2c_relu_backward": (i, [sz, vp, vp, vp, f, vp]),
         "b2c_bn_forward_train": (i, [i, i, i, vp, vp, vp, f, f, i, vp, vp, vp, vp, vp, vp, vp]),
@@ -415,14 +417,31 @@ class SolverHParams(C.Structure):
 
 def solver_update_arena(kind, offsets, counts, rates, decays, g, w, h, h2=None, momentum=0.0, delta=1e-8, rms_decay=0.0,
                         beta1=0.9, beta2=0.999, l2=True, grad_scale=1.0, clear_grads=True, stream=None):
-    """b2c_solver_update_arena: `kind` is a name of SOLVER_KINDS; h2 only for AdaDelta and Adam.  For Adam, `rates` carry the
+    """b2c_solver_update_arena: `kind` is a name of SOLVER_KINDS (or a raw b2c_solver_kind); h2 only for AdaDelta and Adam.  For Adam, `rates` carry the
     bias correction sqrt(1-beta2^t)/(1-beta1^t)."""
     n = len(offsets)
     hp = SolverHParams(momentum, delta, rms_decay, beta1, beta2)
-    check(lib().b2c_solver_update_arena(SOLVER_KINDS[kind], n, (C.c_size_t * n)(*offsets), (C.c_size_t * n)(*counts),
+    check(lib().b2c_solver_update_arena(SOLVER_KINDS.get(kind, kind), n, (C.c_size_t * n)(*offsets), (C.c_size_t * n)(*counts),
                                         (C.c_float * n)(*rates), (C.c_float * n)(*decays), _p(g), _p(w), _p(h),
                                         _p(h2), hp, int(l2), grad_scale, int(clear_grads),
                                         _stream(stream)))
+
+
+def solver_plan(kind, offsets, counts, g, w, h, h2=0):
+    """b2c_debug_solver_plan: the launches b2c_solver_update_arena makes for this layout with the arenas at addresses g, w, h, h2
+    (integers; never dereferenced; 0 = null).  kind: a name of SOLVER_KINDS or a raw b2c_solver_kind.  Returns dict(launches=[(segments, blocks), ...], segs=[dict(launch, vec, blocks,
+    head, body4, tail), ...]); raises B2CError where the entry points refuse the arguments."""
+    n = len(offsets)
+    seg = (C.c_longlong * max(1, 6 * n))()
+    nl = C.c_int()
+    cap = n // 96 + 2
+    lo = (C.c_int * (2 * cap))()
+    check(lib().b2c_debug_solver_plan(SOLVER_KINDS.get(kind, kind), n, (C.c_size_t * max(1, n))(*offsets),
+                                      (C.c_size_t * max(1, n))(*counts), C.c_void_p(g or None), C.c_void_p(w or None),
+                                      C.c_void_p(h or None), C.c_void_p(h2 or None), lo, cap, C.byref(nl), seg))
+    keys = ("launch", "vec", "blocks", "head", "body4", "tail")
+    return dict(launches=[(lo[2 * i], lo[2 * i + 1]) for i in range(nl.value)],
+                segs=[dict(zip(keys, (int(v) for v in seg[6 * s:6 * s + 6]))) for s in range(n)])
 
 
 class Comm:

@@ -9,6 +9,8 @@
 // SGD / Nesterov / AdaGrad / RMSProp read and write g, w, h (24 B); AdaDelta and Adam also h2 (32 B).
 #include "b2c_common.cuh"
 
+#include <vector>
+
 namespace b2c {
 
 // Per-element rules.  Each takes gr = g*grad_scale + decay*reg(w), updates its history in place and returns the step u;
@@ -77,26 +79,46 @@ __device__ __forceinline__ void solver_elem(const R& rule, float& g, float& w, f
   g = clear ? 0.0f : u;
 }
 
+// How solver_span splits a span of n elements whose arrays start at g, w, h and h2 (null for the one-history rules): when all
+// share one 4-byte-aligned offset within 16 bytes, `head` (0-3) leading scalars, `body4` float4 units and `tail` trailing scalars;
+// otherwise one float at a time (vec false, tail n).  Arena slots are padded to an even element count (reference common.hpp:723),
+// so segments are 8-byte but not 16-byte aligned and the head peels them to a 16-byte boundary.  b2c_debug_solver_plan reports it.
+struct SpanSplit {
+  bool vec;
+  unsigned head;
+  size_t body4, tail;
+};
+__host__ __device__ __forceinline__ SpanSplit span_split(size_t n, const void* g, const void* w, const void* h, const void* h2) {
+  const unsigned mg = (unsigned)(reinterpret_cast<uintptr_t>(g) & 15u);
+  const unsigned mw = (unsigned)(reinterpret_cast<uintptr_t>(w) & 15u);
+  const unsigned mh = (unsigned)(reinterpret_cast<uintptr_t>(h) & 15u);
+  const unsigned mh2 = h2 ? (unsigned)(reinterpret_cast<uintptr_t>(h2) & 15u) : mg;
+  SpanSplit s;
+  s.vec = mg == mw && mg == mh && mg == mh2 && (mg & 3u) == 0;
+  if (!s.vec) {
+    s.head = 0; s.body4 = 0; s.tail = n;
+    return s;
+  }
+  const size_t head = ((16u - mg) & 15u) >> 2;
+  s.head = (unsigned)(head < n ? head : n);
+  s.body4 = (n - s.head) / 4;
+  s.tail = n - s.head - s.body4 * 4;
+  return s;
+}
+
 template <class R>
 __device__ __forceinline__ void solver_span(const R& rule, size_t n, float* __restrict__ g, float* __restrict__ w,
                                             float* __restrict__ h, float* __restrict__ h2, float lr, float decay, bool l2,
                                             float gscale, bool clear, size_t first, size_t step) {
   float unused = 0.f;        // h2 of the one-history rules
-  // head/tail scalars keep the float4 body aligned for arbitrary segment offsets
-  const unsigned mg = (unsigned)(reinterpret_cast<uintptr_t>(g) & 15u);
-  const unsigned mw = (unsigned)(reinterpret_cast<uintptr_t>(w) & 15u);
-  const unsigned mh = (unsigned)(reinterpret_cast<uintptr_t>(h) & 15u);
-  const unsigned mh2 = R::kH2 ? (unsigned)(reinterpret_cast<uintptr_t>(h2) & 15u) : mg;
-  if (mg == mw && mg == mh && mg == mh2 && (mg & 3u) == 0) {
-    // peel up to 3 leading elements so the body is 16-byte aligned (arena slots are padded to an even element count,
-    // reference common.hpp:723, so segments are 8-byte but not 16-byte aligned)
-    size_t head = ((16u - mg) & 15u) >> 2;
-    if (head > n) head = n;
+  const SpanSplit sp = span_split(n, g, w, h, R::kH2 ? h2 : nullptr);
+  if (sp.vec) {
+    const size_t head = sp.head;
     for (size_t i = first; i < head; i += step)
       solver_elem(rule, g[i], w[i], h[i], R::kH2 ? h2[i] : unused, lr, decay, l2, gscale, clear);
     g += head; w += head; h += head; n -= head;
     if (R::kH2) h2 += head;
-    const size_t n4 = n / 4;
+    const size_t n4 = sp.body4;
     float4* g4 = reinterpret_cast<float4*>(g);
     float4* w4 = reinterpret_cast<float4*>(w);
     float4* h4 = reinterpret_cast<float4*>(h);
@@ -157,32 +179,47 @@ solver_update_arena_kernel(const __grid_constant__ SegTable t, float* __restrict
               clear != 0, threadIdx.x, blockDim.x);
 }
 
+// The launches of one arena update: segments in order, zero counts skipped, at most SEG_MAX per launch, each segment owning
+// ceil(count / BLOCK_ELEMS) consecutive blocks; seg_launch[s] (when given) receives segment s's launch, -1 for an empty one.
+// Every segment is checked before anything is returned, so a refused call launches nothing.  rate / decay may be null (the
+// plan query): the tables then carry zeros.
+static int pack_segments(const char* who, int nseg, const size_t* offset, const size_t* count, const float* local_rate,
+                         const float* local_decay, std::vector<SegTable>* launches, int* seg_launch) {
+  for (int s = 0; s < nseg; ++s)
+    if (count[s] > 0xffffffffull) return fail(B2C_ERR_INVALID, "%s: segment %d too large", who, s);
+  launches->clear();
+  for (int s = 0; s < nseg; ++s) {
+    if (seg_launch) seg_launch[s] = -1;
+    if (count[s] == 0) continue;
+    if (launches->empty() || launches->back().nseg == SEG_MAX) {
+      launches->emplace_back();
+      launches->back().nseg = 0;
+      launches->back().block_start[0] = 0;
+    }
+    SegTable& t = launches->back();
+    const unsigned start = t.block_start[t.nseg];
+    t.offset[t.nseg] = offset[s];
+    t.count[t.nseg] = (unsigned)count[s];
+    t.lr[t.nseg] = local_rate ? local_rate[s] : 0.f;
+    t.decay[t.nseg] = local_decay ? local_decay[s] : 0.f;
+    ++t.nseg;
+    t.block_start[t.nseg] = start + (unsigned)((count[s] + BLOCK_ELEMS - 1) / BLOCK_ELEMS);
+    if (seg_launch) seg_launch[s] = (int)launches->size() - 1;
+  }
+  return B2C_OK;
+}
+
 template <class R>
 static int launch_arena(const char* who, const R& rule, int nseg, const size_t* offset, const size_t* count,
                         const float* local_rate, const float* local_decay, float* g, float* w, float* h, float* h2, int l2,
                         float grad_scale, int clear_grads, void* stream) {
   if (nseg < 0 || (nseg && (!offset || !count || !local_rate || !local_decay || !g || !w || !h || (R::kH2 && !h2))))
     return fail(B2C_ERR_INVALID, "%s: bad argument", who);
-  int s = 0;
-  while (s < nseg) {
-    SegTable t;
-    t.nseg = 0;
-    unsigned blocks = 0;
-    while (s < nseg && t.nseg < SEG_MAX) {
-      if (count[s] > 0xffffffffull) return fail(B2C_ERR_INVALID, "segment %d too large", s);
-      if (count[s] == 0) { ++s; continue; }
-      t.block_start[t.nseg] = blocks;
-      t.offset[t.nseg] = offset[s];
-      t.count[t.nseg] = (unsigned)count[s];
-      t.lr[t.nseg] = local_rate[s];
-      t.decay[t.nseg] = local_decay[s];
-      blocks += (unsigned)((count[s] + BLOCK_ELEMS - 1) / BLOCK_ELEMS);
-      ++t.nseg;
-      ++s;
-    }
-    if (!t.nseg) break;
-    t.block_start[t.nseg] = blocks;
-    solver_update_arena_kernel<R><<<blocks, 256, 0, as_stream(stream)>>>(t, g, w, h, h2, rule, l2, grad_scale, clear_grads);
+  std::vector<SegTable> launches;
+  if (const int rc = pack_segments(who, nseg, offset, count, local_rate, local_decay, &launches, nullptr)) return rc;
+  for (const SegTable& t : launches) {
+    solver_update_arena_kernel<R><<<t.block_start[t.nseg], 256, 0, as_stream(stream)>>>(t, g, w, h, h2, rule, l2, grad_scale,
+                                                                                        clear_grads);
     B2C_POST_LAUNCH();
   }
   return B2C_OK;
@@ -228,4 +265,44 @@ extern "C" int b2c_solver_update_arena(int kind, int nseg, const size_t* offset,
   }
 #undef B2C_ARENA
   return fail(B2C_ERR_INVALID, "%s: unknown solver kind %d", who, kind);
+}
+
+extern "C" int b2c_debug_solver_plan(int kind, int nseg, const size_t* offset, const size_t* count, const void* g,
+                                     const void* w, const void* h, const void* h2, int* launch_out, int max_launches,
+                                     int* nlaunch, long long* seg_out) {
+  const char* who = "b2c_debug_solver_plan";
+  bool two;
+  switch (kind) {
+    case B2C_SOLVER_SGD: case B2C_SOLVER_NESTEROV: case B2C_SOLVER_ADAGRAD: case B2C_SOLVER_RMSPROP: two = false; break;
+    case B2C_SOLVER_ADADELTA: case B2C_SOLVER_ADAM: two = true; break;
+    default: return fail(B2C_ERR_INVALID, "%s: unknown solver kind %d", who, kind);
+  }
+  if (nseg < 0 || (nseg && (!offset || !count || !g || !w || !h || (two && !h2))))
+    return fail(B2C_ERR_INVALID, "%s: bad argument", who);
+  if (!nlaunch || (nseg && !seg_out) || max_launches < 0 || (max_launches && !launch_out))
+    return fail(B2C_ERR_INVALID, "%s: null output", who);
+  std::vector<SegTable> launches;
+  std::vector<int> seg_launch(nseg);
+  if (const int rc = pack_segments(who, nseg, offset, count, nullptr, nullptr, &launches, seg_launch.data())) return rc;
+  *nlaunch = (int)launches.size();
+  if (*nlaunch > max_launches) return fail(B2C_ERR_INVALID, "%s: %d launches, launch_out holds %d", who, *nlaunch, max_launches);
+  for (int i = 0; i < *nlaunch; ++i) {
+    launch_out[2 * i] = launches[i].nseg;
+    launch_out[2 * i + 1] = (int)launches[i].block_start[launches[i].nseg];
+  }
+  auto at = [](const void* p, size_t off) { return p ? static_cast<const void*>(static_cast<const char*>(p) + off * 4) : p; };
+  for (int s = 0; s < nseg; ++s) {
+    long long* o = seg_out + 6 * (size_t)s;
+    o[0] = seg_launch[s];
+    o[1] = o[2] = o[3] = o[4] = o[5] = 0;
+    if (seg_launch[s] < 0) continue;
+    // every block of the segment splits its own BLOCK_ELEMS span, as solver_update_arena_kernel does
+    for (size_t begin = 0; begin < count[s]; begin += BLOCK_ELEMS) {
+      const size_t len = count[s] - begin < (size_t)BLOCK_ELEMS ? count[s] - begin : (size_t)BLOCK_ELEMS;
+      const size_t off = offset[s] + begin;
+      const SpanSplit sp = span_split(len, at(g, off), at(w, off), at(h, off), two ? at(h2, off) : nullptr);
+      o[1] = sp.vec; o[2] += 1; o[3] += sp.head; o[4] += (long long)sp.body4; o[5] += (long long)sp.tail;
+    }
+  }
+  return B2C_OK;
 }

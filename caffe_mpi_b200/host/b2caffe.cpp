@@ -555,9 +555,11 @@ float SGDSolver::GetMomentum() {
   if (p.momentum_policy == "poly")
     return p.momentum + (p.max_momentum - p.momentum) * std::pow(float(iter_) / float(p.max_iter), p.momentum_power);
   if (p.momentum_policy == "opt") {
+    // as the reference: a float square root, the square in double, and a clamp only when max_momentum is given
     const float lr = GetLearningRate();
-    const float m = (1.f - 0.5f * std::sqrt(lr)) * (1.f - 0.5f * std::sqrt(lr));
-    return std::min(p.max_momentum, m);
+    const double r = 1. - 0.5 * std::sqrt(lr);
+    const float m = (float)(r * r);
+    return p.has_max_momentum ? std::min(p.max_momentum, m) : m;
   }
   B2_CHECK(false, "Unknown momentum policy: " + p.momentum_policy);
 }

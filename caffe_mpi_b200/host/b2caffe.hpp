@@ -348,6 +348,7 @@ struct SolverParameter {   // caffe.proto SolverParameter (fields this path read
   vector<int> stepvalue;
   string lr_policy = "fixed", momentum_policy = "fixed", regularization_type = "L2";
   bool snapshot_diff = false;
+  bool has_max_momentum = false;   // max_momentum was given: the "opt" momentum policy clamps to it only then (sgd_solver.cpp:83-86)
   float global_grad_scale = 1.f;   // NetParameter.global_grad_scale (caffe.proto:130)
   int reduce_buckets = 6;          // NetParameter.reduce_buckets (caffe.proto:140)
   // testing (caffe.proto:184-188): one TEST net per test_iter entry, built from `net`; a pass every test_interval iterations

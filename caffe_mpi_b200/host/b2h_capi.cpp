@@ -2,6 +2,7 @@
 // (The C++ classes in b2caffe.hpp are the interface a Caffe maintainer codes against; this file only
 // marshals arrays so Python can drive them.)  Every function returns 0 / a handle, or -1 / NULL with the
 // message available from b2h_last_error().
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <memory>
@@ -142,6 +143,11 @@ void b2h_solver_destroy(void* hv) { delete static_cast<SolverHandle*>(hv); }
 float b2h_solver_lr_at(void* hv, int iter) {
   auto* h = static_cast<SolverHandle*>(hv);
   try { h->solver->set_iter(iter); return h->solver->GetLearningRate(); } catch (const std::exception& e) { g_err = e.what(); return -1.f; }
+}
+// SGD's momentum at `iter` under its momentum_policy (fixed, poly, opt); NaN with the error set on an unknown policy
+float b2h_solver_momentum_at(void* hv, int iter) {
+  auto* h = static_cast<SolverHandle*>(hv);
+  try { h->solver->set_iter(iter); return h->solver->GetMomentum(); } catch (const std::exception& e) { g_err = e.what(); return NAN; }
 }
 // bucket plan over a layout of `n` params with the given element counts (no device memory needed)
 int b2h_plan_buckets(int n, const size_t* counts, int reduce_buckets, int max_out, int* id_from, int* id_to, size_t* offset, size_t* count) {

@@ -682,6 +682,7 @@ SolverParameter ReadSolverParameter(const PMessage& m, std::string* net_path) {
   p.momentum = (float)m.num("momentum", 0.0);
   p.momentum_policy = m.str("momentum_policy", "fixed");
   p.max_momentum = (float)m.num("max_momentum", 0.99);
+  p.has_max_momentum = m.has("max_momentum");
   p.momentum_power = (float)m.num("momentum_power", 1.0);
   p.weight_decay = (float)m.num("weight_decay", 0.0);
   p.regularization_type = m.str("regularization_type", "L2");

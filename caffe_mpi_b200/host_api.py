@@ -47,6 +47,8 @@ def lib():
         L.b2h_solver_destroy.argtypes = [vp]
         L.b2h_solver_lr_at.argtypes = [vp, i]
         L.b2h_solver_lr_at.restype = f
+        L.b2h_solver_momentum_at.argtypes = [vp, i]
+        L.b2h_solver_momentum_at.restype = f
         L.b2h_plan_buckets.argtypes = [i, szp, i, i, ip, ip, szp, szp]
         L.b2h_divide_batch_size.argtypes = [i, i]
         L.b2h_solver_set_params.argtypes = [vp, i, szp, C.POINTER(f), C.POINTER(f)]
@@ -136,6 +138,13 @@ class SGDSolver:
     def lr_at(self, it):
         v = lib().b2h_solver_lr_at(self._h, it)
         if v < 0:
+            raise HostError(lib().b2h_last_error().decode())
+        return float(v)
+
+    def momentum_at(self, it):
+        """SGDSolver::GetMomentum at iteration `it` (momentum_policy fixed, poly or opt)"""
+        v = lib().b2h_solver_momentum_at(self._h, it)
+        if v != v:
             raise HostError(lib().b2h_last_error().decode())
         return float(v)
 

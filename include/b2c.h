@@ -377,6 +377,16 @@ int b2c_solver_update_arena(int kind, int nseg, const size_t* offset, const size
                             const float* local_rate, const float* local_decay,
                             float* g, float* w, float* h, float* h2, b2c_solver_hparams hp,
                             int l2, float grad_scale, int clear_grads, void* stream);
+/* The launches b2c_solver_update_arena (and, for kind SGD, b2c_sgd_update_arena) makes for this layout with the arenas at g, w,
+ * h and h2 (only tested for alignment, never dereferenced).  Segments are taken in order, zero counts skipped, at most 96 per
+ * launch, each segment owning ceil(count / 4096) blocks of 4096 elements.  *nlaunch = launches; launch_out[2i], [2i+1] = launch
+ * i's segments and blocks (max_launches entries fit).  seg_out[6s..6s+5] for segment s: its launch (-1 when count is 0), 1 when
+ * its blocks take the float4 path (g, w, h and h2 at one 4-byte-aligned offset within 16 bytes) else 0, its blocks, and summed
+ * over them the leading scalars (0-3 per block), float4 units and trailing scalars.  Refuses (B2C_ERR_INVALID) what the entry
+ * points refuse: an unknown kind, nseg < 0, a null g / w / h (h2 for ADADELTA and ADAM) or layout array, a count >= 2^32.
+ * Pure host computation. */
+int b2c_debug_solver_plan(int kind, int nseg, const size_t* offset, const size_t* count, const void* g, const void* w,
+                          const void* h, const void* h2, int* launch_out, int max_launches, int* nlaunch, long long* seg_out);
 
 /* ---- gradient exchange ---------------------------------------------------------------------
  * Replaces P2PManager/P2PSync's NCCL use (src/caffe/parallel.cpp:36-87,145-253) and the MPI

@@ -101,6 +101,13 @@ def lib():
                                         C.c_float, C.c_int, C.c_int, C.c_float]
         L.b2o_learning_rate.restype = C.c_float
         L.b2o_allreduce_avg.argtypes = [C.c_int, C.c_size_t, C.POINTER(C.c_void_p), C.c_int]
+        L.b2o_momentum.argtypes = [C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_float, C.c_int, C.c_float]
+        L.b2o_momentum.restype = C.c_float
+        L.b2o_solver_fp32.argtypes = [C.c_int, C.c_uint, C.c_size_t, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float,
+                                      C.c_float, C.c_int, C.c_float, C.c_int]
+        _f64p = np.ctypeslib.ndpointer(np.float64, flags="C_CONTIGUOUS")
+        L.b2o_solver_f64.argtypes = [C.c_int, C.c_size_t, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, C.c_float, C.c_int,
+                                     C.c_float, C.c_int, _f64p, _f64p]
         _lib = L
     return _lib
 
@@ -233,6 +240,58 @@ def learning_rate(policy, it, base_lr, gamma=0.0, power=0.0, stepsize=1, max_ite
                   rampup_interval=0, rampup_lr=0.0):
     return float(lib().b2o_learning_rate(LR_POLICIES[policy], it, base_lr, gamma, power, stepsize, max_iter, min_lr,
                                          current_step, rampup_interval, rampup_lr))
+
+
+MOMENTUM_POLICIES = {"fixed": 0, "poly": 1, "opt": 2}
+
+
+def momentum(policy, it, momentum, max_momentum=0.99, has_max_momentum=False, momentum_power=1.0, max_iter=1, lr=0.0):
+    """SGDSolver::GetMomentum at iteration `it`; lr: the learning rate at `it` ("opt")"""
+    return float(lib().b2o_momentum(MOMENTUM_POLICIES[policy], it, momentum, max_momentum, int(has_max_momentum),
+                                    momentum_power, max_iter, lr))
+
+
+# b2c_solver_kind, and the form bits b2o_solver_fp32 reads for each
+SOLVER_KINDS = {"SGD": 0, "Nesterov": 1, "AdaGrad": 2, "RMSProp": 3, "AdaDelta": 4, "Adam": 5}
+_FORM_BITS = {"SGD": 4, "Nesterov": 6, "AdaGrad": 3, "RMSProp": 4, "AdaDelta": 7, "Adam": 6}
+
+
+def solver_forms(kind):
+    """every admissible `form` of solver_fp32 for `kind`: at most one fused product per a*b + c*d site"""
+    return [f for f in range(1 << _FORM_BITS[kind]) if all((f >> b) & 3 != 3 for b in (0, 2, 4))]
+
+
+def _hp_array(hp):
+    return np.array([hp.get("momentum", 0.0), hp.get("delta", 1e-8), hp.get("rms_decay", 0.0), hp.get("beta1", 0.9),
+                     hp.get("beta2", 0.999)], np.float32)
+
+
+def _solver_inputs(g, w, h, h2):
+    g, w, h = (np.ascontiguousarray(a, np.float32).reshape(-1).copy() for a in (g, w, h))
+    h2 = np.zeros_like(h) if h2 is None else np.ascontiguousarray(h2, np.float32).reshape(-1).copy()
+    return g, w, h, h2
+
+
+def solver_fp32(kind, form, g, w, h, h2, hp, lr, decay, l2=True, grad_scale=1.0, clear_grads=True):
+    """what the fused solver kernel (sgd.cu) stores for `kind` under contraction `form` (solver_forms), bit for bit:
+    (g, w, h, h2) after the update.  hp: dict of momentum, delta (unclamped), rms_decay, beta1, beta2; for Adam, lr carries
+    the bias correction.  h2 may be None for the one-history kinds (then returned unchanged as zeros)."""
+    g, w, h, h2 = _solver_inputs(g, w, h, h2)
+    rc = lib().b2o_solver_fp32(SOLVER_KINDS[kind], form, g.size, g, w, h, h2, _hp_array(hp), lr, decay, int(l2), grad_scale,
+                               int(clear_grads))
+    if rc:
+        raise ValueError(f"form {form:#x} is not admissible for {kind}")
+    return g, w, h, h2
+
+
+def solver_f64(kind, g, w, h, h2, hp, lr, decay, l2=True, grad_scale=1.0, clear_grads=True):
+    """the same update in float64 from the same fp32 inputs: (vals, bounds), each [4, n] for g, w, h, h2, where bounds[k][i]
+    bounds |fp32 result - vals| for every admissible form (derivation at b2o_solver_f64 in b2o_oracle.c)"""
+    g, w, h, h2 = _solver_inputs(g, w, h, h2)
+    vals, bounds = np.empty((4, g.size)), np.empty((4, g.size))
+    lib().b2o_solver_f64(SOLVER_KINDS[kind], g.size, g, w, h, h2, _hp_array(hp), lr, decay, int(l2), grad_scale,
+                         int(clear_grads), vals.reshape(-1), bounds.reshape(-1))
+    return vals, bounds
 
 
 def allreduce_avg(bufs, solver_count=None):

@@ -414,6 +414,207 @@ float b2o_learning_rate(int policy, int iter, float base_lr, float gamma, float 
   }
 }
 
+/* SGDSolver::GetMomentum (sgd_solver.cpp:68-91).  policy: 0 fixed, 1 poly,
+ * 2 opt; lr is GetLearningRate at iter.  "opt" squares in double what a float
+ * sqrt gave, and clamps to max_momentum only when the solver file sets it.  */
+float b2o_momentum(int policy, int iter, float momentum, float max_momentum, int has_max_momentum,
+                   float momentum_power, int max_iter, float lr) {
+  switch (policy) {
+    case 0: return momentum;
+    case 1: return momentum + (max_momentum - momentum) * powf((float)iter / (float)max_iter, momentum_power);
+    case 2: {
+      const double r = 1.0 - 0.5 * (double)sqrtf(lr);
+      const float m = (float)(r * r);
+      return has_max_momentum && max_momentum < m ? max_momentum : m;
+    }
+    default: return -1.0f;
+  }
+}
+
+/* ------------------------------------------------------------------------- *
+ * The fused solver updates of caffe_mpi_b200/csrc/sgd.cu, one element at a
+ * time, for kind = b2c_solver_kind (0 SGD, 1 Nesterov, 2 AdaGrad, 3 RMSProp,
+ * 4 AdaDelta, 5 Adam).  hp = {momentum, delta, rms_decay, beta1, beta2}; delta
+ * is clamped as b2c_solver_update_arena does (AdaGrad / AdaDelta 1e-3,
+ * RMSProp / Adam 1e-4).  lr for Adam carries the bias correction.
+ *
+ * b2o_solver_fp32 restates the kernel in fp32, in its order of operations.
+ * Where a product meets a sum the compiler may contract to an fmaf; `form`
+ * picks, per site, a rounded product then an add (bit clear) or the fmaf (bit
+ * set).  At a site a*b + c*d at most one of its two bits may be set.
+ *   bit 0  gr = fmaf(g, s, decay*reg)              bit 1  gr = fmaf(reg, decay, g*s)
+ *   SGD       bit 2  h = fmaf(m, h, lr*gr)         bit 3  h = fmaf(lr, gr, m*h)
+ *   Nesterov  bits 2, 3 as SGD for h';             bit 4  u = fmaf(1+m, h', -(m*h))
+ *                                                  bit 5  u = fmaf(-m, h, (1+m)*h')
+ *   AdaGrad   bit 2  h = fmaf(gr, gr, h)
+ *   RMSProp   bit 2  h = fmaf(rd, h, (1-rd)*gr*gr) bit 3  h = fmaf((1-rd)*gr, gr, rd*h)
+ *   AdaDelta  bits 2, 3 as RMSProp with m for h;   bits 4, 5 the same for h2;
+ *             bit 6  w = fmaf(-lr, gr, w) (u = lr*gr rounded, for g)
+ *   Adam      bit 2  m = fmaf(m, b1, gr*(1-b1))    bit 3  m = fmaf(gr, 1-b1, m*b1)
+ *             bit 4  v = fmaf(v, b2, gr*gr*(1-b2)) bit 5  v = fmaf(gr*gr, 1-b2, v*b2)
+ * Square roots and divisions are correctly rounded, as __fsqrt_rn and
+ * __fdiv_rn.  Returns -1 for an unknown kind or an inadmissible form.
+ * ------------------------------------------------------------------------- */
+static float clamp_delta(int kind, float delta) {
+  const float lo = (kind == 2 || kind == 4) ? 1e-3f : 1e-4f;
+  return delta > lo ? delta : lo;
+}
+static int solver_form_ok(int kind, unsigned form) {
+  static const unsigned bits[6] = {0xfu, 0x3fu, 0x7u, 0xfu, 0x7fu, 0x3fu};
+  if (kind < 0 || kind > 5 || (form & ~bits[kind])) return 0;
+  for (int b = 0; b < 6; b += 2)
+    if (((form >> b) & 3u) == 3u) return 0;
+  return 1;
+}
+/* a*b + c*d with bit `lo` fusing a*b and bit lo+1 fusing c*d */
+static float mad2(unsigned form, int lo, float a, float b, float c, float d) {
+  if (form >> lo & 1u) return fmaf(a, b, c * d);
+  if (form >> (lo + 1) & 1u) return fmaf(c, d, a * b);
+  return a * b + c * d;
+}
+int b2o_solver_fp32(int kind, unsigned form, size_t n, float* g, float* w, float* h, float* h2, const float* hp, float lr,
+                    float decay, int l2, float grad_scale, int clear_grads) {
+  if (!solver_form_ok(kind, form)) return -1;
+  const float m = hp[0], delta = clamp_delta(kind, hp[1]), rd = hp[2], b1 = hp[3], b2 = hp[4];
+  for (size_t i = 0; i < n; ++i) {
+    const float reg = l2 ? w[i] : (float)((0.0f < w[i]) - (w[i] < 0.0f));
+    float gr = mad2(form, 0, g[i], grad_scale, reg, decay), u = 0.0f, wn;
+    int fused_w = 0;
+    switch (kind) {
+      case 0:
+        u = h[i] = mad2(form, 2, m, h[i], lr, gr);
+        break;
+      case 1: {
+        const float hi = h[i], hn = mad2(form, 2, m, hi, lr, gr);
+        h[i] = hn;
+        const float a = 1.0f + m;
+        u = (form >> 4 & 1u) ? fmaf(a, hn, -(m * hi)) : (form >> 5 & 1u) ? fmaf(-m, hi, a * hn) : a * hn - m * hi;
+        break;
+      }
+      case 2:
+        h[i] = (form >> 2 & 1u) ? fmaf(gr, gr, h[i]) : h[i] + gr * gr;
+        u = (lr * gr) / (sqrtf(h[i]) + delta);
+        break;
+      case 3:
+        h[i] = mad2(form, 2, rd, h[i], (1.0f - rd) * gr, gr);
+        u = (lr * gr) / (sqrtf(h[i]) + delta);
+        break;
+      case 4:
+        h[i] = mad2(form, 2, m, h[i], (1.0f - m) * gr, gr);
+        gr *= sqrtf((h2[i] + delta) / (h[i] + delta));
+        h2[i] = mad2(form, 4, m, h2[i], (1.0f - m) * gr, gr);
+        u = lr * gr;
+        fused_w = (int)(form >> 6 & 1u);
+        break;
+      case 5:
+        h[i] = mad2(form, 2, h[i], b1, gr, 1.0f - b1);
+        h2[i] = mad2(form, 4, h2[i], b2, gr * gr, 1.0f - b2);
+        u = (lr * h[i]) / (sqrtf(h2[i]) + delta);
+        break;
+    }
+    wn = fused_w ? fmaf(-lr, gr, w[i]) : w[i] - u;
+    w[i] = wn;
+    g[i] = clear_grads ? 0.0f : u;
+  }
+  return 0;
+}
+
+/* b2o_solver_f64: the same update in float64 from the same fp32 inputs and
+ * constants (1 - m, 1 + m, the clamped delta as the kernel forms them in fp32),
+ * and for each output a bound on |fp32 result - float64 result| that holds for
+ * every admissible form.
+ *
+ * Derivation.  Every fp32 operation returns fl(x) = x(1 + e) + t with |e| <=
+ * u = 2^-24 and |t| <= 2^-150 (the underflow term: half the smallest fp32
+ * subnormal; zero for sums and for an fmaf away from underflow, kept anyway).
+ * Carry for each intermediate x its float64 value X and a bound E >= |x_fp32 -
+ * X|.  Inputs and fp32 constants are exact: E = 0.  To first order, plus the
+ * second-order terms where they are cheap to keep:
+ *   x = a*b      E = |A| Eb + |B| Ea + Ea Eb + u|X| + 2^-150
+ *   x = a +- b   E = Ea + Eb + u|X| + 2^-150
+ *   x = sqrt(a)  E = min(Ea / (sqrt(A) + sqrt(max(A - Ea, 0))), sqrt(Ea)) + u|X| + 2^-150
+ *                (|sqrt(a) - sqrt(A)| = |a - A| / (sqrt(a) + sqrt(A)); sqrt is
+ *                1/2-Hoelder, so the second term holds at A = 0)
+ *   x = a / b    E = (Ea + |X| Eb) / (|B| - Eb) + u|X| + 2^-150   (|B| > Eb:
+ *                b = sqrt(h) + delta >= 1e-4 while Eb is ~1e-7 |B|)
+ * An fmaf rounds once where a rounded product then an add round twice, and
+ * its result deviates from X by no more than the unfused bound's terms, so the
+ * bound of the unfused form covers every form.  Float64's own error (2^-53
+ * per operation) is ~2^29 times smaller than each u term; the caller's test
+ * multiplies the bound by 1 + 2^-20 to cover it.
+ * vals, bounds: 4 x n arrays (g, w, h, h2 after the update; h2 rows are the
+ * input for the one-history kinds, bound 0).
+ * ------------------------------------------------------------------------- */
+typedef struct { double v, e; } b2o_ve;
+static const double U32 = 5.9604644775390625e-08, ETA32 = 7.006492321624085e-46;   /* 2^-24, 2^-150 */
+static b2o_ve ve_exact(double v) { b2o_ve r = {v, 0.0}; return r; }
+static b2o_ve ve_mul(b2o_ve a, b2o_ve b) {
+  b2o_ve r; r.v = a.v * b.v;
+  r.e = fabs(a.v) * b.e + fabs(b.v) * a.e + a.e * b.e + U32 * fabs(r.v) + ETA32;
+  return r;
+}
+static b2o_ve ve_add(b2o_ve a, b2o_ve b) { b2o_ve r; r.v = a.v + b.v; r.e = a.e + b.e + U32 * fabs(r.v) + ETA32; return r; }
+static b2o_ve ve_sub(b2o_ve a, b2o_ve b) { b2o_ve r; r.v = a.v - b.v; r.e = a.e + b.e + U32 * fabs(r.v) + ETA32; return r; }
+static b2o_ve ve_sqrt(b2o_ve a) {
+  b2o_ve r; r.v = sqrt(a.v);
+  const double lo = a.v - a.e > 0.0 ? sqrt(a.v - a.e) : 0.0;
+  const double lin = r.v > 0.0 ? a.e / (r.v + lo) : INFINITY, hol = sqrt(a.e);
+  r.e = (lin < hol ? lin : hol) + U32 * r.v + ETA32;
+  return r;
+}
+static b2o_ve ve_div(b2o_ve a, b2o_ve b) {
+  b2o_ve r; r.v = a.v / b.v;
+  r.e = (a.e + fabs(r.v) * b.e) / (fabs(b.v) - b.e) + U32 * fabs(r.v) + ETA32;
+  return r;
+}
+int b2o_solver_f64(int kind, size_t n, const float* g, const float* w, const float* h, const float* h2, const float* hp,
+                   float lr, float decay, int l2, float grad_scale, int clear_grads, double* vals, double* bounds) {
+  if (kind < 0 || kind > 5) return -1;
+  const float m = hp[0], rd = hp[2], b1 = hp[3], b2 = hp[4];
+  const b2o_ve M = ve_exact(m), D = ve_exact(clamp_delta(kind, hp[1])), RD = ve_exact(rd), B1 = ve_exact(b1), B2 = ve_exact(b2);
+  const b2o_ve LR = ve_exact(lr), DEC = ve_exact(decay), S = ve_exact(grad_scale);
+  /* 1 - m, 1 + m, ... as the kernel forms them: one fp32 rounding each, so exact inputs here */
+  const b2o_ve OM = ve_exact(1.0f - m), PM = ve_exact(1.0f + m), ORD = ve_exact(1.0f - rd), OB1 = ve_exact(1.0f - b1),
+               OB2 = ve_exact(1.0f - b2);
+  for (size_t i = 0; i < n; ++i) {
+    const b2o_ve W = ve_exact(w[i]), H = ve_exact(h[i]), H2 = ve_exact(h2 ? h2[i] : 0.0f);
+    const b2o_ve REG = ve_exact(l2 ? w[i] : (float)((0.0f < w[i]) - (w[i] < 0.0f)));
+    b2o_ve gr = ve_add(ve_mul(ve_exact(g[i]), S), ve_mul(REG, DEC)), u, hn = H, h2n = H2;
+    switch (kind) {
+      case 0: u = hn = ve_add(ve_mul(M, H), ve_mul(LR, gr)); break;
+      case 1:
+        hn = ve_add(ve_mul(M, H), ve_mul(LR, gr));
+        u = ve_sub(ve_mul(PM, hn), ve_mul(M, H));
+        break;
+      case 2:
+        hn = ve_add(H, ve_mul(gr, gr));
+        u = ve_div(ve_mul(LR, gr), ve_add(ve_sqrt(hn), D));
+        break;
+      case 3:
+        hn = ve_add(ve_mul(RD, H), ve_mul(ve_mul(ORD, gr), gr));
+        u = ve_div(ve_mul(LR, gr), ve_add(ve_sqrt(hn), D));
+        break;
+      case 4:
+        hn = ve_add(ve_mul(M, H), ve_mul(ve_mul(OM, gr), gr));
+        gr = ve_mul(gr, ve_sqrt(ve_div(ve_add(H2, D), ve_add(hn, D))));
+        h2n = ve_add(ve_mul(M, H2), ve_mul(ve_mul(OM, gr), gr));
+        u = ve_mul(LR, gr);
+        break;
+      default:
+        hn = ve_add(ve_mul(H, B1), ve_mul(gr, OB1));
+        h2n = ve_add(ve_mul(H2, B2), ve_mul(ve_mul(gr, gr), OB2));
+        u = ve_div(ve_mul(LR, hn), ve_add(ve_sqrt(h2n), D));
+        break;
+    }
+    const b2o_ve wn = ve_sub(W, u);
+    vals[i] = clear_grads ? 0.0 : u.v;            bounds[i] = clear_grads ? 0.0 : u.e;
+    vals[n + i] = wn.v;                           bounds[n + i] = wn.e;
+    vals[2 * n + i] = hn.v;                       bounds[2 * n + i] = hn.e;
+    vals[3 * n + i] = h2n.v;                      bounds[3 * n + i] = h2n.e;
+  }
+  return 0;
+}
+
 /* ------------------------------------------------------------------------- *
  * Multi-rank gradient exchange: in-place sum over ranks of a diff bucket
  * (P2PSync::allreduce_bucket, src/caffe/parallel.cpp:245-253, ncclSum) followed

@@ -135,3 +135,83 @@ def update(kind, g, w, h, h2, hp, local_rate, local_decay, t=1, **kw):
 
 KINDS = ("SGD", "Nesterov", "AdaGrad", "RMSProp", "AdaDelta", "Adam")
 TWO_HISTORIES = ("AdaDelta", "Adam")
+
+
+# ---- the fused kernels' own order (csrc/sgd.cu), for the per-element suites --------------------------------------------------
+# hyperparameters as b2c_solver_hparams names them (delta unclamped); Adam's beta1 / beta2 are SolverParameter momentum / momentum2
+KERNEL_HP = dict(momentum=0.9, delta=1e-8, rms_decay=0.95, beta1=0.9, beta2=0.999)
+DYADIC_HP = dict(momentum=0.875, delta=1e-8, rms_decay=0.875, beta1=0.875, beta2=63 / 64)
+
+
+def kernel_fp32(kind, g, w, h, h2, hp, lr, decay, l2=True, grad_scale=1.0, clear_grads=True):
+    """numpy fp32, one rounding per operation, in the kernel's order: (g, w, h, h2) after the update.  numpy never contracts a
+    product into a sum, so on data where every product that meets a sum is exact (dyadic_inputs) this is what any contraction
+    of the kernel must store.  Delta is clamped as b2c_solver_update_arena clamps it."""
+    g, w, h = (np.array(a, F).reshape(-1) for a in (g, w, h))
+    h2 = np.zeros_like(h) if h2 is None else np.array(h2, F).reshape(-1)
+    m, rd, b1, b2 = F(hp["momentum"]), F(hp["rms_decay"]), F(hp["beta1"]), F(hp["beta2"])
+    d = max(F(hp["delta"]), F(1e-3) if kind in ("AdaGrad", "AdaDelta") else F(1e-4))
+    lr, decay, one = F(lr), F(decay), F(1)
+    reg = w if l2 else (w > 0).astype(F) - (w < 0).astype(F)               # sign(+-0) = +0, as (0 < w) - (w < 0)
+    gr = g * F(grad_scale) + reg * decay
+    with np.errstate(all="ignore"):
+        if kind == "SGD":
+            h = m * h + lr * gr
+            u = h
+        elif kind == "Nesterov":
+            hi, h = h, m * h + lr * gr
+            u = (one + m) * h - m * hi
+        elif kind == "AdaGrad":
+            h = h + gr * gr
+            u = (lr * gr) / (np.sqrt(h) + d)
+        elif kind == "RMSProp":
+            h = rd * h + ((one - rd) * gr) * gr
+            u = (lr * gr) / (np.sqrt(h) + d)
+        elif kind == "AdaDelta":
+            h = m * h + ((one - m) * gr) * gr
+            gr = gr * np.sqrt((h2 + d) / (h + d))
+            h2 = m * h2 + ((one - m) * gr) * gr
+            u = lr * gr
+        else:
+            h = h * b1 + gr * (one - b1)
+            h2 = h2 * b2 + (gr * gr) * (one - b2)
+            u = (lr * h) / (np.sqrt(h2) + d)
+        w = w - u
+    return (np.zeros_like(g) if clear_grads else u.astype(F)), w.astype(F), h.astype(F), h2.astype(F)
+
+
+def dyadic_inputs(rng, n, kind):
+    """(g, w, h, h2) of small integers times powers of two: with DYADIC_HP, grad_scale 1/8, lr = odd/128 (< 16/128) and decay =
+    odd/256 (< 16/256), every product that meets a sum in the kernel is exact (at most 24 significant bits), so every contraction
+    gives the same bits -- except AdaDelta's h2 and w, which follow a rounded square root.  w holds +-0."""
+    g = rng.integers(-64, 65, n).astype(F) / F(64)
+    w = rng.integers(-64, 65, n).astype(F) / F(64)
+    w[rng.random(n) < 0.05] = F(-0.0)
+    lo = -64 if kind in ("SGD", "Nesterov", "Adam") else 0
+    h = rng.integers(lo, 65, n).astype(F) / F(256)
+    h2 = rng.integers(0, 65, n).astype(F) / F(256)
+    return g, w, h, h2
+
+
+def dyadic_rates(rng, nseg):
+    """distinct per-segment (lr, decay) pairs for dyadic_inputs"""
+    pairs = [(F(a) / F(128), F(b) / F(256)) for a in range(1, 16, 2) for b in range(1, 16, 2)]
+    idx = rng.permutation(len(pairs))
+    return [float(pairs[idx[s % len(pairs)]][0]) for s in range(nseg)], [float(pairs[idx[s % len(pairs)]][1]) for s in range(nseg)]
+
+
+def wide_inputs(rng, n, kind):
+    """(g, w, h, h2) over several binades, with +-0 in w and subnormal g, h and w: data on which the contractions of the kernel
+    give different bits (test_oracle checks that every pair of forms differs on it)"""
+    def wide():
+        return (rng.standard_normal(n) * np.exp2(rng.integers(-8, 4, n))).astype(F)
+    g, w, h, h2 = wide(), wide(), wide(), np.abs(wide())
+    if kind not in ("SGD", "Nesterov", "Adam"):
+        h = np.abs(h)
+    sub = (rng.integers(1, 1 << 20, n) * np.exp2(-149)).astype(F)        # subnormals: 2^-149 .. 2^-129
+    for a, p in ((g, 0.02), (h, 0.02), (w, 0.02)):
+        pick = rng.random(n) < p
+        a[pick] = sub[pick] * (np.sign(a[pick]) if a is not h or kind in ("SGD", "Nesterov", "Adam") else 1)
+    zero = rng.random(n) < 0.03
+    w[zero] = np.where(rng.random(int(zero.sum())) < 0.5, F(0.0), F(-0.0))
+    return g, w, h, h2

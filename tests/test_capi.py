@@ -313,3 +313,74 @@ def test_no_cpu_fallback():
     rc = L.b2c_conv_forward(d._h, one, one, one, one, None, 0, None)
     assert rc == -2 and b"no CPU fallback" in L.b2c_last_error()
     assert L.b2c_sgemm(0, 0, 2, 2, 2, 1.0, one, one, 0.0, one, None) == -2
+
+
+def test_solver_plan_regimes():
+    """b2c_debug_solver_plan is host-only: how the fused solver updates split an arena into launches (at most 96 non-empty segments
+    each, 4096 elements per block) and each block's span into leading scalars, float4 units and trailing scalars -- the regimes
+    test_solver_schedule_gpu.py runs -- and the layouts the entry points refuse"""
+    A = 1 << 20                                           # 16-byte aligned arena bases
+    G, W, H, H2 = A, 2 * A, 3 * A, 4 * A
+
+    def seg(kind, off, cnt, g=G, w=W, h=H, h2=H2):
+        q = capi.solver_plan(kind, [off], [cnt], g, w, h, h2)
+        s = q["segs"][0]
+        return s["vec"], s["blocks"], s["head"], s["body4"], s["tail"]
+    # (start mod 4, count): (float4 path, blocks, head, body4, tail), summed over the segment's blocks; every block of a segment
+    # starts at the same offset mod 4 and peels its own head
+    table = {
+        (0, 1): (1, 1, 0, 0, 1), (0, 4): (1, 1, 0, 1, 0), (0, 4095): (1, 1, 0, 1023, 3), (0, 4096): (1, 1, 0, 1024, 0),
+        (0, 4097): (1, 2, 0, 1024, 1), (1, 2): (1, 1, 2, 0, 0),              # a segment shorter than its head
+        (1, 3): (1, 1, 3, 0, 0), (1, 4): (1, 1, 3, 0, 1), (3, 1): (1, 1, 1, 0, 0), (3, 4096): (1, 1, 1, 1023, 3),
+        (2, 4097): (1, 2, 3, 1023, 2), (2, 3 * 4096 + 1): (1, 4, 7, 3069, 6), (1, 4097): (1, 2, 4, 1023, 1),
+    }
+    for (mod, cnt), want in table.items():
+        for kind in capi.SOLVER_KINDS:
+            assert seg(kind, 8 + mod, cnt) == want, (kind, mod, cnt, seg(kind, 8 + mod, cnt))
+    for mod in range(4):
+        for cnt in (1, 2, 3, 4, 5, 4095, 4096, 4097, 3 * 4096 + 1):
+            v, b, hd, b4, t = seg("Adam", 4 * 1000 + mod, cnt)
+            assert v == 1 and b == -(-cnt // 4096) and hd + 4 * b4 + t == cnt and hd <= 3 * b and t <= 3 * b
+            # a pointer 4 bytes off the others takes the segment to one float at a time; for the one-history kinds h2 is not read
+            assert seg("Adam", 4 * 1000 + mod, cnt, g=G + 4) == (0, b, 0, 0, cnt)
+            assert seg("AdaDelta", 4 * 1000 + mod, cnt, h2=H2 + 4) == (0, b, 0, 0, cnt)
+            assert seg("SGD", 4 * 1000 + mod, cnt, h2=H2 + 4) == (1, b, hd, b4, t)
+            assert seg("SGD", 4 * 1000 + mod, cnt, h2=0) == (1, b, hd, b4, t)
+            assert seg("RMSProp", 4 * 1000 + mod, cnt, w=W + 8) == (0, b, 0, 0, cnt)
+    # the largest segment the launch takes: 2^32 - 1 elements, 2^20 blocks
+    assert seg("SGD", 0, (1 << 32) - 1) == (1, 1 << 20, 0, (1 << 30) - 1, 3)
+
+    def launches(counts, kind="SGD"):
+        offs = [0] * len(counts)
+        for i in range(1, len(counts)):
+            offs[i] = offs[i - 1] + counts[i - 1] + (counts[i - 1] & 1)
+        return capi.solver_plan(kind, offs, counts, G, W, H, H2)
+    assert launches([]) == dict(launches=[], segs=[])
+    for nseg, want in ((96, [(96, 96)]), (97, [(96, 96), (1, 1)]), (192, [(96, 96), (96, 96)]),
+                       (193, [(96, 96), (96, 96), (1, 1)])):
+        q = launches([7] * nseg)
+        assert q["launches"] == want, (nseg, q["launches"])
+        assert [s["launch"] for s in q["segs"]] == [i // 96 for i in range(nseg)]
+    # zero counts take no slot and no block: here at the 96th and after the 97th non-empty position, and at the very end
+    counts = [5] * 95 + [0] + [4097] + [0] + [3] * 4 + [0]
+    q = launches(counts, "AdaDelta")
+    assert q["launches"] == [(96, 97), (4, 4)]
+    assert [s["launch"] for s in q["segs"]] == [0] * 95 + [-1, 0, -1] + [1] * 4 + [-1]
+    assert all(q["segs"][i]["blocks"] == 0 for i in (95, 97, 102))
+    assert sum(b for _, b in q["launches"]) == sum(s["blocks"] for s in q["segs"])
+    # an empty layout with null arrays is accepted, as the entry points accept it
+    assert capi.solver_plan("Adam", [], [], 0, 0, 0, 0) == dict(launches=[], segs=[])
+    # refusals: a segment of 2^32 elements anywhere (here the 99th of 100), a null h2 for the two-history kinds, a null g,
+    # an unknown kind
+    big = [5] * 100
+    big[98] = 1 << 32
+    with pytest.raises(capi.B2CError, match="segment 98 too large"):
+        launches(big)
+    for kind in ("AdaDelta", "Adam"):
+        with pytest.raises(capi.B2CError):
+            capi.solver_plan(kind, [0], [8], G, W, H, 0)
+    with pytest.raises(capi.B2CError):
+        capi.solver_plan("SGD", [0], [8], 0, W, H)
+    for kind in (-1, 6):
+        with pytest.raises(capi.B2CError, match="unknown solver kind"):
+            capi.solver_plan(kind, [0], [8], G, W, H, H2)

@@ -103,3 +103,53 @@ def test_divide_batch_size():
     assert h.divide_batch_size(512, 8) == 64
     assert h.divide_batch_size(100, 8) == 13
     assert h.divide_batch_size(32, 1) == 32
+
+
+MOMENTA = [
+    dict(momentum_policy="fixed", momentum=0.9),
+    dict(momentum_policy="fixed", momentum=0.9, max_momentum=0.5),                      # "fixed" ignores max_momentum
+    dict(momentum_policy="poly", momentum=0.5, max_momentum=0.95, momentum_power=2.0),
+    dict(momentum_policy="poly", momentum=0.5),                                           # max_momentum's default, 0.99
+    dict(momentum_policy="poly", momentum=0.9, max_momentum=0.999, momentum_power=0.5),
+    dict(momentum_policy="opt", momentum=0.9),                                            # no clamp
+    dict(momentum_policy="opt", momentum=0.9, max_momentum=0.99),
+    dict(momentum_policy="opt", momentum=0.9, max_momentum=0.995),
+]
+
+
+@pytest.mark.parametrize("cfg", MOMENTA, ids=[f'{c["momentum_policy"]}{i}' for i, c in enumerate(MOMENTA)])
+@pytest.mark.parametrize("lr", [0.01, 2e-4, 1e-4, 5e-5, 1e-6])
+def test_momentum_policy_matches_oracle(cfg, lr):
+    """SGDSolver::GetMomentum against the oracle's restatement of the reference (sgd_solver.cpp:68-91), at learning rates on both
+    sides of 1.0e-4, where the "opt" momentum (1 - sqrt(lr)/2)^2 crosses 0.99; max_momentum clamps "opt" only when it is given"""
+    fields = " ".join(f'{k}: "{v}"' if isinstance(v, str) else f"{k}: {v!r}" for k, v in cfg.items())
+    s, _ = h.open_solver(f'type: "SGD" base_lr: {lr!r} lr_policy: "fixed" max_iter: 100 {fields}', is_text=True)
+    for it in (0, 1, 10, 50, 99, 100):
+        want = o.momentum(cfg["momentum_policy"], it, cfg["momentum"], cfg.get("max_momentum", 0.99), "max_momentum" in cfg,
+                          cfg.get("momentum_power", 1.0), 100, s.lr_at(it))
+        if cfg["momentum_policy"] == "poly":
+            assert s.momentum_at(it) == pytest.approx(want, rel=1e-6), it
+        else:
+            assert s.momentum_at(it) == want, it
+    if cfg["momentum_policy"] == "opt":
+        free = float(np.float32((1.0 - 0.5 * float(np.sqrt(np.float32(lr)))) ** 2))
+        clamp = cfg.get("max_momentum", np.inf)
+        assert s.momentum_at(0) == pytest.approx(min(free, clamp), rel=1e-7)
+        if "max_momentum" not in cfg and lr <= 5e-5:
+            assert s.momentum_at(0) > 0.99                 # the reference does not clamp without max_momentum
+
+
+def test_opt_momentum_follows_the_learning_rate_schedule():
+    """"opt" reads GetLearningRate at the same iteration: a step schedule takes lr from 1e-2 through 1e-4 to 1e-6"""
+    s, _ = h.open_solver('type: "SGD" base_lr: 0.01 lr_policy: "step" gamma: 0.01 stepsize: 10 max_iter: 30 momentum: 0.9 '
+                         'momentum_policy: "opt"', is_text=True)
+    got = [s.momentum_at(it) for it in (0, 10, 20)]
+    want = [o.momentum("opt", it, 0.9, lr=s.lr_at(it)) for it in (0, 10, 20)]
+    assert got == want
+    assert got[0] == pytest.approx(0.95 ** 2, rel=1e-6) and got[2] == pytest.approx(0.9995 ** 2, rel=1e-6)
+
+
+def test_unknown_momentum_policy_is_fatal():
+    s, _ = h.open_solver('type: "SGD" base_lr: 0.01 momentum: 0.9 momentum_policy: "bogus"', is_text=True)
+    with pytest.raises(h.HostError, match="Unknown momentum policy"):
+        s.momentum_at(0)

@@ -340,3 +340,133 @@ def test_oracle_matches_golden_fixtures():
         # im2col part of the fixture is bit-exact (pure copy)
         col = o.im2col(x[0], (prm.kh, prm.kw), (prm.sh, prm.sw), (prm.ph, prm.pw), (prm.dh, prm.dw))
         assert np.array_equal(col, z[nm + "/col0"]), nm
+
+
+# ---- fused solver updates: fp32 contraction forms and the float64 restatement ------------------------------------------------
+import itertools  # noqa: E402
+
+import solver_oracle as so  # noqa: E402
+
+F32 = np.float32
+
+
+def _bits(a):
+    return np.ascontiguousarray(a, np.float32).view(np.int32)
+
+
+def test_solver_known_answers():
+    """hand-computed steps on exact values, every delta clamp, and the Adam rate"""
+    hp = dict(so.KERNEL_HP, momentum=0.5)
+    # SGD: gr = 1*0.5 + 0.125*2 = 0.75, h = 0.5*0.5 + 0.25*0.75 = 0.4375, w = 2 - 0.4375
+    g, w, h, _ = o.solver_fp32("SGD", 0, [1.0], [2.0], [0.5], None, hp, 0.25, 0.125, True, 0.5, False)
+    assert (g[0], w[0], h[0]) == (0.4375, 1.5625, 0.4375)
+    # Nesterov: h' = 0.4375 as above, u = 1.5*0.4375 - 0.5*0.5 = 0.40625
+    g, w, h, _ = o.solver_fp32("Nesterov", 0, [1.0], [2.0], [0.5], None, hp, 0.25, 0.125, True, 0.5, False)
+    assert (g[0], w[0], h[0]) == (0.40625, 1.59375, 0.4375)
+    # L1: reg = sign(w) = -1, gr = 1 - 0.25 = 0.75
+    g, w, h, _ = o.solver_fp32("SGD", 0, [1.0], [-2.0], [0.0], None, hp, 1.0, 0.25, False, 1.0, True)
+    assert (g[0], w[0], h[0]) == (0.0, -2.75, 0.75)
+    # the delta clamps: below the clamp the clamp, at it and above it delta itself
+    for kind, clamp in (("AdaGrad", F32(1e-3)), ("RMSProp", F32(1e-4)), ("AdaDelta", F32(1e-3)), ("Adam", F32(1e-4))):
+        for delta, used in ((1e-8, clamp), (float(clamp), clamp), (1e-2, F32(1e-2))):
+            p = dict(hp, delta=delta, rms_decay=0.75, momentum=0.75, beta1=0.75, beta2=0.75)
+            g, w, h, h2 = o.solver_fp32(kind, 0, [2.0], [1.0], [12.0], [5.0], p, 0.5, 0.0, True, 1.0, False)
+            if kind == "AdaGrad":       # h = 12 + 4 = 16, u = 1 / (4 + d)
+                want_h, want_u = 16.0, F32(1) / (F32(4) + used)
+            elif kind == "RMSProp":     # h = 0.75*12 + 0.25*4 = 10, u = 1 / (sqrt(10) + d)
+                want_h, want_u = 10.0, F32(1) / (np.sqrt(F32(10)) + used)
+            elif kind == "AdaDelta":    # h = 10, gr = 2 sqrt((5 + d) / (10 + d)), h2 = 0.75*5 + 0.25 gr^2, u = gr / 2
+                want_h = 10.0
+                gr = F32(2) * np.sqrt((F32(5) + used) / (F32(10) + used))
+                want_u = F32(0.5) * gr
+                assert h2[0] == F32(3.75) + (F32(0.25) * gr) * gr
+            else:                       # m = 0.75*12 + 0.25*2 = 9.5, v = 0.75*5 + 0.25*4 = 4.75, u = 0.5*9.5 / (sqrt(4.75) + d)
+                want_h, want_u = 9.5, F32(4.75) / (np.sqrt(F32(4.75)) + used)
+                assert h2[0] == 4.75
+            assert h[0] == want_h and g[0] == want_u, (kind, delta)
+            assert w[0] == F32(1) - want_u, (kind, delta)
+    # Adam's first step from zero history with the bias-corrected rate lr*sqrt(1-b2)/(1-b1) moves w by lr*sign(g), less eps's
+    # share: lr / (1 + eps / (sqrt(1-b2) |g|))
+    b1, b2, lr = 0.9, 0.999, 0.01
+    rate = float(F32(lr) * so.adam_correction(b1, b2, 1))
+    gin = np.array([3.0, -0.5, 40.0], F32)
+    g, w, h, h2 = o.solver_fp32("Adam", 0, gin, np.zeros(3), np.zeros(3), np.zeros(3), dict(hp, beta1=b1, beta2=b2), rate, 0.0,
+                                True, 1.0, False)
+    eps = 1e-4                                                  # delta 1e-8, clamped
+    np.testing.assert_allclose(-w, lr * np.sign(gin) / (1 + eps / (np.sqrt(1 - b2) * np.abs(gin))), rtol=1e-5)
+
+
+def test_solver_sign_of_zero():
+    """w = +-0 under L1 regularises by +0 (sign(0) = 0), so an otherwise zero step keeps each zero's sign; a step of -0
+    turns w = -0 into +0 (-0 - -0 = +0) -- in every form"""
+    hp = dict(so.KERNEL_HP, momentum=0.5)
+    w0 = np.array([0.0, -0.0, 0.0, -0.0], F32)
+    for form in o.solver_forms("SGD"):
+        g, w, h, _ = o.solver_fp32("SGD", form, np.zeros(4), w0, np.zeros(4), None, hp, 0.1, 0.01, False, 1.0, False)
+        assert list(_bits(w)) == list(_bits(w0)) and list(_bits(g)) == [0] * 4
+        # L1, decay 0: sign(-0) = +0 gives gr = -0 + +0 = +0, sign(-1) = -1 gives gr = -0 + -0 = -0
+        g, w, h, _ = o.solver_fp32("SGD", form, [-0.0, -0.0], [-0.0, -1.0], [-0.0, -0.0], None, hp, 0.5, 0.0, False, 1.0, False)
+        assert list(_bits(h)) == list(_bits(np.array([0.0, -0.0], F32))), form
+        assert _bits(w)[1] == _bits(F32(-1.0)) and list(_bits(g)) == list(_bits(np.array([0.0, -0.0], F32)))
+        # L2, decay 0, w = -0: gr = -0 + (-0)*0 = -0, h = -0, and w = -0 - (-0) = +0
+        g, w, h, _ = o.solver_fp32("SGD", form, [-0.0], [-0.0], [-0.0], None, hp, 0.5, 0.0, True, 1.0, False)
+        assert (_bits(h)[0], _bits(w)[0], _bits(g)[0]) == (_bits(F32(-0.0)), 0, _bits(F32(-0.0))), form
+
+
+def test_solver_subnormals_are_kept():
+    """fp32 subnormals are neither flushed on input nor on output: 3*2^-149 halved rounds to even (2*2^-149), a subnormal
+    gradient steps w by itself"""
+    tiny = F32(3 * 2.0 ** -149)
+    g, w, h, _ = o.solver_fp32("SGD", 0, [0.0], [0.0], [tiny], None, dict(so.KERNEL_HP, momentum=0.5), 0.0, 0.0, True, 1.0, False)
+    assert h[0] == F32(2 * 2.0 ** -149) and w[0] == -F32(2 * 2.0 ** -149)
+    sub = F32(2.0 ** -140)
+    g, w, h, _ = o.solver_fp32("SGD", 0, [sub], [0.0], [0.0], None, dict(so.KERNEL_HP, momentum=0.0), 1.0, 0.0, True, 1.0, False)
+    assert w[0] == -sub and h[0] == sub
+
+
+@pytest.mark.parametrize("kind", so.KINDS)
+@pytest.mark.parametrize("l2", [True, False], ids=["L2", "L1"])
+@pytest.mark.parametrize("clear", [True, False], ids=["clear", "keep"])
+def test_solver_forms_within_float64_bound_and_distinct(kind, l2, clear):
+    """every fp32 contraction form lies within the float64 restatement's derived bound on data over several binades with
+    subnormals and +-0, at every delta regime; and on that data every pair of forms differs in some element, so that a kernel
+    matching one form pins its contraction"""
+    rng = np.random.default_rng(7)
+    n = 20000
+    g, w, h, h2 = so.wide_inputs(rng, n, kind)
+    worst = 0.0
+    for delta in (1e-8, 1e-3, 1e-2):
+        hp = dict(so.KERNEL_HP, delta=delta, momentum=0.0 if kind in ("AdaGrad", "RMSProp") else 0.9)
+        vals, bounds = o.solver_f64(kind, g, w, h, h2, hp, 0.3, 0.7, l2, 1 / 3, clear)
+        outs = {}
+        for form in o.solver_forms(kind):
+            out = o.solver_fp32(kind, form, g, w, h, h2, hp, 0.3, 0.7, l2, 1 / 3, clear)
+            for k in range(4):
+                err = np.abs(out[k].astype(np.float64) - vals[k])
+                assert np.all(err <= bounds[k] * (1 + 2.0 ** -20)), (kind, form, k, float(np.max(err / np.maximum(bounds[k], 1e-300))))
+                worst = max(worst, float(np.max(err / np.maximum(bounds[k], 1e-300))))
+            outs[form] = np.concatenate([_bits(a) for a in out])
+        if delta == 1e-2:
+            same = [(a, b) for a, b in itertools.combinations(outs, 2) if np.array_equal(outs[a], outs[b])]
+            # L1: decay*sign(w) is exact, so fusing it changes nothing; clear: g is 0 in every form.  Nothing else may coincide.
+            allowed = {(a, b) for a, b in same if not l2 and (a ^ b) in (2,)}
+            assert set(same) == allowed, (kind, same[:4])
+    print(f"[solver oracle] {kind} L2={l2} clear={clear}: worst |fp32 - f64| / bound = {worst:.3f}")
+
+
+@pytest.mark.parametrize("kind", so.KINDS)
+def test_solver_dyadic_data_makes_every_form_equal(kind):
+    """on dyadic_inputs every product that meets a sum is exact, so every form equals the plain numpy fp32 restatement bit for
+    bit -- AdaDelta's h2 and w excepted (they follow a rounded square root) -- which lets the GPU suite check such data against
+    numpy whatever the compiler contracts"""
+    rng = np.random.default_rng(11)
+    g, w, h, h2 = so.dyadic_inputs(rng, 50000, kind)
+    lrs, decays = so.dyadic_rates(rng, 6)
+    for (lr, decay), l2, clear in itertools.product(zip(lrs, decays), (True, False), (True, False)):
+        want = so.kernel_fp32(kind, g, w, h, h2, so.DYADIC_HP, lr, decay, l2, 0.125, clear)
+        for form in o.solver_forms(kind):
+            got = o.solver_fp32(kind, form, g, w, h, h2, so.DYADIC_HP, lr, decay, l2, 0.125, clear)
+            for k in range(4):
+                if kind == "AdaDelta" and k in (1, 3):
+                    continue
+                assert np.array_equal(_bits(got[k]), _bits(want[k])), (kind, form, k, lr, decay, l2, clear)
