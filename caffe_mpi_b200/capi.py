@@ -129,6 +129,12 @@ def lib():
                                         SolverHParams, i, f, i, vp]),
         "b2c_debug_solver_plan": (i, [i, i, C.POINTER(sz), C.POINTER(sz), vp, vp, vp, vp, C.POINTER(i), i, C.POINTER(i),
                                       C.POINTER(C.c_longlong)]),
+        "b2c_arena_sumsq": (i, [i, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), vp, vp, vp]),
+        "b2c_clip_factor": (i, [vp, sz, C.c_double, f, vp, vp]),
+        "b2c_solver_update_arena_scaled": (i, [i, i, C.POINTER(sz), C.POINTER(sz), C.POINTER(f), C.POINTER(f), vp, vp, vp, vp,
+                                               SolverHParams, i, f, vp, i, vp]),
+        "b2c_debug_sumsq_plan": (i, [i, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), vp, C.POINTER(i), i, C.POINTER(i),
+                                     C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]),
         "b2c_relu_forward": (i, [sz, vp, vp, f, vp]),
         "b2c_relu_backward": (i, [sz, vp, vp, vp, f, vp]),
         "b2c_bn_forward_train": (i, [i, i, i, vp, vp, vp, f, f, i, vp, vp, vp, vp, vp, vp, vp]),
@@ -442,6 +448,58 @@ def solver_plan(kind, offsets, counts, g, w, h, h2=0):
     keys = ("launch", "vec", "blocks", "head", "body4", "tail")
     return dict(launches=[(lo[2 * i], lo[2 * i + 1]) for i in range(nl.value)],
                 segs=[dict(zip(keys, (int(v) for v in seg[6 * s:6 * s + 6]))) for s in range(n)])
+
+
+def solver_update_arena_scaled(kind, offsets, counts, rates, decays, g, w, h, h2=None, factor=None, momentum=0.0, delta=1e-8,
+                               rms_decay=0.0, beta1=0.9, beta2=0.999, l2=True, grad_scale=1.0, clear_grads=True, stream=None):
+    """b2c_solver_update_arena_scaled: solver_update_arena with grad_scale times the float at device address `factor` (a tensor
+    or an integer address)."""
+    n = len(offsets)
+    hp = SolverHParams(momentum, delta, rms_decay, beta1, beta2)
+    fp = C.c_void_p(factor or None) if factor is None or isinstance(factor, int) else _p(factor)
+    check(lib().b2c_solver_update_arena_scaled(SOLVER_KINDS.get(kind, kind), n, (C.c_size_t * n)(*offsets),
+                                               (C.c_size_t * n)(*counts), (C.c_float * n)(*rates), (C.c_float * n)(*decays),
+                                               _p(g), _p(w), _p(h), _p(h2), hp, int(l2), grad_scale, fp,
+                                               int(clear_grads), _stream(stream)))
+
+
+def arena_sumsq(offsets, counts, slots, g, partials, stream=None):
+    """b2c_arena_sumsq: float64 partials of sum(g^2), one per 4096-element block, block b of segment s at slots[s] + b."""
+    n = len(offsets)
+    check(lib().b2c_arena_sumsq(n, (C.c_size_t * max(1, n))(*offsets), (C.c_size_t * max(1, n))(*counts),
+                                (C.c_size_t * max(1, n))(*slots), _p(g), _p(partials), _stream(stream)))
+
+
+CLIP_STATE_BYTES = 16      # b2c_clip_state: float norm, float factor, long long clipped
+
+
+def clip_factor(partials, nslots, s_n, clip, state, stream=None):
+    """b2c_clip_factor: `state` is a device buffer of CLIP_STATE_BYTES (e.g. a 4-element float32 tensor); clip_state() reads it."""
+    check(lib().b2c_clip_factor(_p(partials), nslots, s_n, clip, _p(state), _stream(stream)))
+
+
+def clip_state(state):
+    """(norm, factor, clipped) of a b2c_clip_state held in a 4-element float32 tensor"""
+    import numpy as np
+    raw = state.detach().cpu().numpy().view(np.uint8)
+    return float(raw[0:4].view(np.float32)[0]), float(raw[4:8].view(np.float32)[0]), int(raw[8:16].view(np.int64)[0])
+
+
+def sumsq_plan(offsets, counts, slots, g):
+    """b2c_debug_sumsq_plan for the diff arena at address g (an integer; never dereferenced).  Returns dict(launches=[(segments,
+    blocks), ...], segs=[dict(launch, vec, blocks, slot, head, body4, tail), ...], npartials); raises B2CError where
+    b2c_arena_sumsq refuses the arguments."""
+    n = len(offsets)
+    seg = (C.c_longlong * max(1, 7 * n))()
+    nl, npart = C.c_int(), C.c_longlong()
+    cap = n // 96 + 2
+    lo = (C.c_int * (2 * cap))()
+    check(lib().b2c_debug_sumsq_plan(n, (C.c_size_t * max(1, n))(*offsets), (C.c_size_t * max(1, n))(*counts),
+                                     (C.c_size_t * max(1, n))(*slots), C.c_void_p(g or None), lo, cap, C.byref(nl), seg,
+                                     C.byref(npart)))
+    keys = ("launch", "vec", "blocks", "slot", "head", "body4", "tail")
+    return dict(launches=[(lo[2 * i], lo[2 * i + 1]) for i in range(nl.value)],
+                segs=[dict(zip(keys, (int(v) for v in seg[7 * s:7 * s + 7]))) for s in range(n)], npartials=npart.value)
 
 
 class Comm:

@@ -161,10 +161,19 @@ struct SegTable {
   float decay[SEG_MAX];
 };
 
-template <class R>
+// The update's grad_scale: a float argument, or (b2c_solver_update_arena_scaled) fl(grad_scale * *factor) with the factor that
+// b2c_clip_factor left in device memory, formed once per thread.  The float instantiations are the unscaled entry points.
+struct DevScale {
+  float gs;
+  const float* factor;
+};
+__device__ __forceinline__ float grad_scale_of(float gs) { return gs; }
+__device__ __forceinline__ float grad_scale_of(const DevScale& s) { return s.gs * __ldg(s.factor); }
+
+template <class R, class Scale>
 __global__ void __launch_bounds__(256)
 solver_update_arena_kernel(const __grid_constant__ SegTable t, float* __restrict__ g, float* __restrict__ w,
-                           float* __restrict__ h, float* __restrict__ h2, const R rule, int l2, float gscale, int clear) {
+                           float* __restrict__ h, float* __restrict__ h2, const R rule, int l2, const Scale gscale, int clear) {
   // binary search the owning segment
   int lo = 0, hi = t.nseg - 1;
   while (lo < hi) {
@@ -175,8 +184,8 @@ solver_update_arena_kernel(const __grid_constant__ SegTable t, float* __restrict
   size_t len = (size_t)t.count[lo] - begin;
   if (len > BLOCK_ELEMS) len = BLOCK_ELEMS;
   const size_t off = (size_t)t.offset[lo] + begin;
-  solver_span(rule, len, g + off, w + off, h + off, R::kH2 ? h2 + off : nullptr, t.lr[lo], t.decay[lo], l2 != 0, gscale,
-              clear != 0, threadIdx.x, blockDim.x);
+  solver_span(rule, len, g + off, w + off, h + off, R::kH2 ? h2 + off : nullptr, t.lr[lo], t.decay[lo], l2 != 0,
+              grad_scale_of(gscale), clear != 0, threadIdx.x, blockDim.x);
 }
 
 // The launches of one arena update: segments in order, zero counts skipped, at most SEG_MAX per launch, each segment owning
@@ -209,18 +218,116 @@ static int pack_segments(const char* who, int nseg, const size_t* offset, const 
   return B2C_OK;
 }
 
-template <class R>
+template <class R, class Scale>
 static int launch_arena(const char* who, const R& rule, int nseg, const size_t* offset, const size_t* count,
                         const float* local_rate, const float* local_decay, float* g, float* w, float* h, float* h2, int l2,
-                        float grad_scale, int clear_grads, void* stream) {
+                        Scale grad_scale, int clear_grads, void* stream) {
   if (nseg < 0 || (nseg && (!offset || !count || !local_rate || !local_decay || !g || !w || !h || (R::kH2 && !h2))))
     return fail(B2C_ERR_INVALID, "%s: bad argument", who);
   std::vector<SegTable> launches;
   if (const int rc = pack_segments(who, nseg, offset, count, local_rate, local_decay, &launches, nullptr)) return rc;
   for (const SegTable& t : launches) {
-    solver_update_arena_kernel<R><<<t.block_start[t.nseg], 256, 0, as_stream(stream)>>>(t, g, w, h, h2, rule, l2, grad_scale,
-                                                                                        clear_grads);
+    solver_update_arena_kernel<R, Scale><<<t.block_start[t.nseg], 256, 0, as_stream(stream)>>>(t, g, w, h, h2, rule, l2,
+                                                                                               grad_scale, clear_grads);
     B2C_POST_LAUNCH();
+  }
+  return B2C_OK;
+}
+
+// ---- global gradient norm (clip_gradients) ----------------------------------------------------------------------------------
+// One double partial of sum(g^2) per BLOCK_ELEMS block of each segment.  The segments travel as in the update (pack_segments),
+// with the first partial slot of each in place of its rate and decay.
+static_assert(BLOCK_ELEMS == B2C_SUMSQ_BLOCK_ELEMS, "include/b2c.h states the norm's block size");
+struct SumsqTable {
+  int nseg;
+  unsigned block_start[SEG_MAX + 1];
+  unsigned long long offset[SEG_MAX];
+  unsigned count[SEG_MAX];
+  unsigned long long slot[SEG_MAX];
+};
+
+// The sum of 256 threads' doubles in a fixed order: a shuffle tree within each warp, then the eight warps in order.  Thread 0
+// returns it.
+__device__ __forceinline__ double block_sum_fixed(double s) {
+  __shared__ double warp_sum[8];
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = s;
+  __syncthreads();
+  double tot = 0.0;
+  if (threadIdx.x == 0) {
+    tot = warp_sum[0];
+    for (int i = 1; i < 8; ++i) tot += warp_sum[i];
+  }
+  return tot;
+}
+
+__device__ __forceinline__ double sq(float x) { return (double)x * (double)x; }   // exact: 48 significant bits
+
+// Each thread sums its elements of the block in order -- the head scalars, its float4 units, the tail scalars, as span_split
+// cuts the span -- so a partial depends only on its segment's address and count.
+__global__ void __launch_bounds__(256)
+arena_sumsq_kernel(const __grid_constant__ SumsqTable t, const float* __restrict__ g, double* __restrict__ partials) {
+  int lo = 0, hi = t.nseg - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (t.block_start[mid] <= blockIdx.x) lo = mid; else hi = mid - 1;
+  }
+  const unsigned b = blockIdx.x - t.block_start[lo];
+  const size_t begin = (size_t)b * BLOCK_ELEMS;
+  size_t len = (size_t)t.count[lo] - begin;
+  if (len > BLOCK_ELEMS) len = BLOCK_ELEMS;
+  const float* p = g + t.offset[lo] + begin;
+  const SpanSplit sp = span_split(len, p, p, p, nullptr);
+  double s = 0.0;
+  size_t i = threadIdx.x;
+  if (sp.vec) {
+    for (; i < sp.head; i += blockDim.x) s += sq(p[i]);
+    const float4* p4 = reinterpret_cast<const float4*>(p + sp.head);
+    for (size_t j = threadIdx.x; j < sp.body4; j += blockDim.x) {
+      const float4 v = __ldg(p4 + j);
+      s += sq(v.x); s += sq(v.y); s += sq(v.z); s += sq(v.w);
+    }
+    i = sp.head + sp.body4 * 4 + threadIdx.x;
+  }
+  for (; i < len; i += blockDim.x) s += sq(p[i]);
+  const double tot = block_sum_fixed(s);
+  if (threadIdx.x == 0) partials[t.slot[lo] + b] = tot;
+}
+
+// One CTA: each thread sums the slots i = tid (mod 256) in order, then block_sum_fixed.
+__global__ void __launch_bounds__(256)
+clip_factor_kernel(const double* __restrict__ partials, size_t n, double s_n, float clip, b2c_clip_state* __restrict__ st) {
+  double s = 0.0;
+  for (size_t i = threadIdx.x; i < n; i += blockDim.x) s += partials[i];
+  const double tot = block_sum_fixed(s);
+  if (threadIdx.x == 0) {
+    const float norm = __double2float_rn(sqrt((s_n * s_n) * tot));
+    const bool clipped = norm > clip;                            // false for a NaN norm: the update is not scaled
+    st->norm = norm;
+    st->factor = clipped ? __fdiv_rn(clip, norm) : 1.0f;
+    if (clipped) st->clipped += 1;
+  }
+}
+
+// pack_segments with each segment's first slot; refuses what pack_segments refuses
+static int pack_sumsq(const char* who, int nseg, const size_t* offset, const size_t* count, const size_t* slot,
+                      std::vector<SumsqTable>* out, int* seg_launch) {
+  std::vector<SegTable> launches;
+  if (const int rc = pack_segments(who, nseg, offset, count, nullptr, nullptr, &launches, seg_launch)) return rc;
+  out->assign(launches.size(), SumsqTable{});
+  for (size_t l = 0; l < launches.size(); ++l) {
+    SumsqTable& q = (*out)[l];
+    q.nseg = launches[l].nseg;
+    for (int k = 0; k <= q.nseg; ++k) q.block_start[k] = launches[l].block_start[k];
+    for (int k = 0; k < q.nseg; ++k) { q.offset[k] = launches[l].offset[k]; q.count[k] = launches[l].count[k]; }
+  }
+  // segments were packed in order, so the k-th non-empty segment is the k-th entry over the launches
+  size_t l = 0;
+  int k = 0;
+  for (int s = 0; s < nseg; ++s) {
+    if (count[s] == 0) continue;
+    if (k == (*out)[l].nseg) { ++l; k = 0; }
+    (*out)[l].slot[k++] = slot[s];
   }
   return B2C_OK;
 }
@@ -247,12 +354,12 @@ extern "C" int b2c_sgd_update_arena(int nseg, const size_t* offset, const size_t
                       nullptr, l2, grad_scale, clear_grads, stream);
 }
 
-extern "C" int b2c_solver_update_arena(int kind, int nseg, const size_t* offset, const size_t* count,
-                                       const float* local_rate, const float* local_decay, float* g, float* w, float* h,
-                                       float* h2, b2c_solver_hparams hp, int l2, float grad_scale, int clear_grads,
-                                       void* stream) {
+// b2c_solver_update_arena with grad_scale a float or a DevScale
+template <class Scale>
+static int solver_update_arena(const char* who, int kind, int nseg, const size_t* offset, const size_t* count,
+                               const float* local_rate, const float* local_decay, float* g, float* w, float* h, float* h2,
+                               b2c_solver_hparams hp, int l2, Scale grad_scale, int clear_grads, void* stream) {
   // the reference clamps delta in each ComputeUpdateValue before the launch
-  const char* who = "b2c_solver_update_arena";
 #define B2C_ARENA(rule) launch_arena(who, rule, nseg, offset, count, local_rate, local_decay, g, w, h, h2, l2, grad_scale, \
                                      clear_grads, stream)
   switch (kind) {
@@ -265,6 +372,81 @@ extern "C" int b2c_solver_update_arena(int kind, int nseg, const size_t* offset,
   }
 #undef B2C_ARENA
   return fail(B2C_ERR_INVALID, "%s: unknown solver kind %d", who, kind);
+}
+
+extern "C" int b2c_solver_update_arena(int kind, int nseg, const size_t* offset, const size_t* count,
+                                       const float* local_rate, const float* local_decay, float* g, float* w, float* h,
+                                       float* h2, b2c_solver_hparams hp, int l2, float grad_scale, int clear_grads,
+                                       void* stream) {
+  return solver_update_arena("b2c_solver_update_arena", kind, nseg, offset, count, local_rate, local_decay, g, w, h, h2, hp, l2,
+                             grad_scale, clear_grads, stream);
+}
+
+extern "C" int b2c_solver_update_arena_scaled(int kind, int nseg, const size_t* offset, const size_t* count,
+                                              const float* local_rate, const float* local_decay, float* g, float* w, float* h,
+                                              float* h2, b2c_solver_hparams hp, int l2, float grad_scale, const float* factor,
+                                              int clear_grads, void* stream) {
+  const char* who = "b2c_solver_update_arena_scaled";
+  if (!factor) return fail(B2C_ERR_INVALID, "%s: null factor", who);
+  return solver_update_arena(who, kind, nseg, offset, count, local_rate, local_decay, g, w, h, h2, hp, l2,
+                             DevScale{grad_scale, factor}, clear_grads, stream);
+}
+
+extern "C" int b2c_arena_sumsq(int nseg, const size_t* offset, const size_t* count, const size_t* slot, const float* g,
+                               double* partials, void* stream) {
+  const char* who = "b2c_arena_sumsq";
+  if (nseg < 0 || (nseg && (!offset || !count || !slot || !g || !partials))) return fail(B2C_ERR_INVALID, "%s: bad argument", who);
+  std::vector<SumsqTable> launches;
+  if (const int rc = pack_sumsq(who, nseg, offset, count, slot, &launches, nullptr)) return rc;
+  for (const SumsqTable& t : launches) {
+    arena_sumsq_kernel<<<t.block_start[t.nseg], 256, 0, as_stream(stream)>>>(t, g, partials);
+    B2C_POST_LAUNCH();
+  }
+  return B2C_OK;
+}
+
+extern "C" int b2c_clip_factor(const double* partials, size_t nslots, double s_n, float clip, b2c_clip_state* state,
+                               void* stream) {
+  const char* who = "b2c_clip_factor";
+  if ((nslots && !partials) || !state) return fail(B2C_ERR_INVALID, "%s: bad argument", who);
+  if (!(clip >= 0.f) || !(s_n > 0.0) || std::isinf(s_n)) return fail(B2C_ERR_INVALID, "%s: clip %g, s_n %g", who, clip, s_n);
+  clip_factor_kernel<<<1, 256, 0, as_stream(stream)>>>(partials, nslots, s_n, clip, state);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+
+extern "C" int b2c_debug_sumsq_plan(int nseg, const size_t* offset, const size_t* count, const size_t* slot, const void* g,
+                                    int* launch_out, int max_launches, int* nlaunch, long long* seg_out, long long* npartials) {
+  const char* who = "b2c_debug_sumsq_plan";
+  if (nseg < 0 || (nseg && (!offset || !count || !slot || !g))) return fail(B2C_ERR_INVALID, "%s: bad argument", who);
+  if (!nlaunch || !npartials || (nseg && !seg_out) || max_launches < 0 || (max_launches && !launch_out))
+    return fail(B2C_ERR_INVALID, "%s: null output", who);
+  std::vector<SumsqTable> launches;
+  std::vector<int> seg_launch(nseg);
+  if (const int rc = pack_sumsq(who, nseg, offset, count, slot, &launches, seg_launch.data())) return rc;
+  *nlaunch = (int)launches.size();
+  if (*nlaunch > max_launches) return fail(B2C_ERR_INVALID, "%s: %d launches, launch_out holds %d", who, *nlaunch, max_launches);
+  for (int i = 0; i < *nlaunch; ++i) {
+    launch_out[2 * i] = launches[i].nseg;
+    launch_out[2 * i + 1] = (int)launches[i].block_start[launches[i].nseg];
+  }
+  *npartials = 0;
+  for (int s = 0; s < nseg; ++s) {
+    long long* o = seg_out + 7 * (size_t)s;
+    o[0] = seg_launch[s];
+    o[1] = o[2] = o[4] = o[5] = o[6] = 0;
+    o[3] = (long long)slot[s];
+    if (seg_launch[s] < 0) continue;
+    // every block splits its own BLOCK_ELEMS span, as arena_sumsq_kernel does
+    for (size_t begin = 0; begin < count[s]; begin += BLOCK_ELEMS) {
+      const size_t len = count[s] - begin < (size_t)BLOCK_ELEMS ? count[s] - begin : (size_t)BLOCK_ELEMS;
+      const void* p = static_cast<const char*>(g) + (offset[s] + begin) * 4;
+      const SpanSplit sp = span_split(len, p, p, p, nullptr);
+      o[1] = sp.vec; o[2] += 1; o[4] += sp.head; o[5] += (long long)sp.body4; o[6] += (long long)sp.tail;
+    }
+    if (o[3] + o[2] > *npartials) *npartials = o[3] + o[2];
+  }
+  return B2C_OK;
 }
 
 extern "C" int b2c_debug_solver_plan(int kind, int nseg, const size_t* offset, const size_t* count, const void* g,

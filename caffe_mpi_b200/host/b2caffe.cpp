@@ -563,13 +563,63 @@ float SGDSolver::GetMomentum() {
   }
   B2_CHECK(false, "Unknown momentum policy: " + p.momentum_policy);
 }
+SGDSolver::~SGDSolver() {
+  if (clip_partials_) cudaFree(clip_partials_);
+  if (clip_state_) cudaFree(clip_state_);
+}
 void SGDSolver::SetParams(const vector<shared_ptr<Blob>>& params, const vector<ParamSpec>& specs) {
   B2_CHECK(params.size() == specs.size(), "one ParamSpec per learnable blob");
   specs_ = specs;
   arena_.Init(params, num_histories() == 2);
+  if (clipping()) {
+    vector<size_t> counts;
+    for (int i = 0; i < arena_.size(); ++i) counts.push_back(arena_.count(i));
+    clip_nslots_ = ClipSlots(counts, &clip_slot_);
+    CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&clip_partials_), sizeof(double) * (clip_nslots_ ? clip_nslots_ : 1)));
+    CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&clip_state_), sizeof(b2c_clip_state)));
+    CUDA_CHECK(cudaMemset(clip_state_, 0, sizeof(b2c_clip_state)));
+  }
+}
+void SGDSolver::set_clip_gradients(float clip) {
+  B2_CHECK(arena_.size() == 0 && !arena_.data(), "clip_gradients must be set before the solver's parameters");
+  param_.clip_gradients = clip;
+}
+size_t SGDSolver::ClipSlots(const vector<size_t>& counts, vector<size_t>* slot) {
+  slot->clear();
+  size_t n = 0;
+  for (size_t c : counts) {
+    slot->push_back(n);
+    n += (c + B2C_SUMSQ_BLOCK_ELEMS - 1) / B2C_SUMSQ_BLOCK_ELEMS;
+  }
+  return n;
+}
+void SGDSolver::ClipNorm(int id_from, int id_to, cudaStream_t stream) {
+  B2_CHECK(clip_state_, "ClipNorm without clip_gradients");
+  if (id_to < id_from) return;
+  // every param, BatchNorm statistics included: their diffs stay 0, so they add exact zeros and keep the slots contiguous
+  vector<size_t> off, cnt, slot;
+  for (int id = id_from; id <= id_to; ++id) {
+    off.push_back(arena_.offset(id)); cnt.push_back(arena_.count(id)); slot.push_back(clip_slot_[id]);
+  }
+  B2C_CHECK(b2c_arena_sumsq((int)off.size(), off.data(), cnt.data(), slot.data(), arena_.diff(), clip_partials_, stream));
+}
+void SGDSolver::ClipFactor(cudaStream_t stream) {
+  B2_CHECK(clip_state_, "ClipFactor without clip_gradients");
+  // the scale the net applies before ClipGradients (net.cpp:815-817,910); Normalize's 1/iter_size comes after it
+  const double s_n = 1.0 / ((double)Caffe::solver_count() * (double)param_.global_grad_scale);
+  B2C_CHECK(b2c_clip_factor(clip_partials_, clip_nslots_, s_n, param_.clip_gradients, clip_state_, stream));
+}
+b2c_clip_state SGDSolver::ClipState() {
+  B2_CHECK(clipping(), "the solver does not clip gradients (clip_gradients < 0)");
+  B2_CHECK(clip_state_, "the solver clips gradients but has no parameters yet");
+  b2c_clip_state st;
+  CUDA_CHECK(cudaDeviceSynchronize());
+  CUDA_CHECK(cudaMemcpy(&st, clip_state_, sizeof(st), cudaMemcpyDeviceToHost));
+  return st;
 }
 void SGDSolver::ApplyUpdate(int id_from, int id_to, cudaStream_t stream) {
-  B2_CHECK(param_.clip_gradients < 0, "clip_gradients is not on the BASELINE path (sgd_solver.cpp:111-128)");
+  B2_CHECK(!clipping() || (id_from == 0 && id_to == arena_.size() - 1),
+           "with clip_gradients the update covers the whole arena: every parameter takes the one global factor");
   B2_CHECK(param_.regularization_type == "L2" || param_.regularization_type == "L1", "Unknown regularization type");
   const float rate = GetLearningRate();
   // SGD keeps its momentum policy; Nesterov, AdaDelta and Adam (as beta1) read param_.momentum() directly
@@ -598,13 +648,18 @@ void SGDSolver::ApplyUpdate(int id_from, int id_to, cudaStream_t stream) {
   if (n == 0) return;
   const float grad_scale = 1.f / (float)Caffe::solver_count() / param_.global_grad_scale / (float)param_.iter_size;
   const int l2 = param_.regularization_type == "L2" ? 1 : 0, clear = param_.snapshot_diff ? 0 : 1;
+  b2c_solver_hparams hp;
+  hp.momentum = momentum; hp.delta = param_.delta; hp.rms_decay = param_.rms_decay; hp.beta1 = param_.momentum; hp.beta2 = param_.momentum2;
+  if (clipping()) {
+    B2C_CHECK(b2c_solver_update_arena_scaled(kind_, n, off.data(), cnt.data(), lr.data(), dc.data(), arena_.diff(), arena_.data(),
+                                             arena_.history(), arena_.history2(), hp, l2, grad_scale, &clip_state_->factor, clear, stream));
+    return;
+  }
   if (kind_ == B2C_SOLVER_SGD) {
     B2C_CHECK(b2c_sgd_update_arena(n, off.data(), cnt.data(), lr.data(), dc.data(), arena_.diff(), arena_.data(), arena_.history(),
                                    momentum, l2, grad_scale, clear, stream));
     return;
   }
-  b2c_solver_hparams hp;
-  hp.momentum = momentum; hp.delta = param_.delta; hp.rms_decay = param_.rms_decay; hp.beta1 = param_.momentum; hp.beta2 = param_.momentum2;
   B2C_CHECK(b2c_solver_update_arena(kind_, n, off.data(), cnt.data(), lr.data(), dc.data(), arena_.diff(), arena_.data(), arena_.history(),
                                     arena_.history2(), hp, l2, grad_scale, clear, stream));
 }
@@ -722,7 +777,8 @@ void ReduceScheduler::flush(int b, cudaStream_t compute) {
   CUDA_CHECK(cudaEventRecord(ev_ready_, compute));           // diffs of this bucket are complete on `compute`
   CUDA_CHECK(cudaStreamWaitEvent(side, ev_ready_, 0));
   if (sync_) sync_->allreduce_bucket(solver_->arena().diff() + bk.offset, bk.count);
-  solver_->ApplyUpdate(bk.id_from, bk.id_to, side);          // chained on the same side stream
+  if (solver_->clipping()) solver_->ClipNorm(bk.id_from, bk.id_to, side);   // the update waits for the global norm
+  else solver_->ApplyUpdate(bk.id_from, bk.id_to, side);     // chained on the same side stream
 }
 void ReduceScheduler::on_param_ready(int id, cudaStream_t compute) {
   while (next_bucket_ < (int)buckets_.size() && id <= buckets_[next_bucket_].id_from) {
@@ -733,6 +789,11 @@ void ReduceScheduler::on_param_ready(int id, cudaStream_t compute) {
 void ReduceScheduler::end_of_iteration(cudaStream_t compute) {
   while (next_bucket_ < (int)buckets_.size()) { flush(next_bucket_, compute); ++next_bucket_; }
   cudaStream_t side = sync_ ? sync_->comm_stream() : update_stream_;
+  if (solver_->clipping()) {
+    // behind every bucket's partials on the same stream: every rank holds the same reduced diffs, so the same factor
+    solver_->ClipFactor(side);
+    solver_->ApplyUpdateAll(side);
+  }
   CUDA_CHECK(cudaEventRecord(ev_done_, side));
   CUDA_CHECK(cudaStreamWaitEvent(compute, ev_done_, 0));     // next forward sees the updated weights
   next_bucket_ = 0;

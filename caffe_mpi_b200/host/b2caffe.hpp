@@ -372,6 +372,9 @@ class P2PSync;
 class SGDSolver {
  public:
   explicit SGDSolver(const SolverParameter& p) : param_(p), kind_(SolverKind(p.type)) { CheckSolverParameter(p); }
+  ~SGDSolver();
+  SGDSolver(const SGDSolver&) = delete;
+  SGDSolver& operator=(const SGDSolver&) = delete;
   const SolverParameter& param() const { return param_; }
   int kind() const { return kind_; }
   // history blobs per learnable blob: 2 for AdaDelta and Adam (AdaDeltaPreSolve / AdamPreSolve), 1 otherwise
@@ -386,16 +389,34 @@ class SGDSolver {
   void SetParams(const vector<shared_ptr<Blob>>& params, const vector<ParamSpec>& specs);
   ParamArena& arena() { return arena_; }
   // ApplyUpdate for params [from, to] on `stream` (sgd_solver.cpp:143-149 + sgd_solver.cu:57-72), fused
-  // over the arena; grad_scale folds 1/solver_count, 1/global_grad_scale and 1/iter_size.
+  // over the arena; grad_scale folds 1/solver_count, 1/global_grad_scale and 1/iter_size.  With clip_gradients the update is
+  // one call over the whole arena that reads the factor ClipFactor left on the device; a partial range is refused.
   void ApplyUpdate(int id_from, int id_to, cudaStream_t stream);
   void ApplyUpdateAll(cudaStream_t stream) { ApplyUpdate(0, arena_.size() - 1, stream); }
   void increment_iter() { ++iter_; }
+  // ---- clip_gradients >= 0: one L2 norm of the whole reduced gradient per iteration, every parameter scaled by the same factor
+  // (caffe.proto:241; sgd_solver.cpp:111-128 re-clips per parameter instead, see DESIGN.md section 4)
+  bool clipping() const { return param_.clip_gradients >= 0.f; }
+  void set_clip_gradients(float clip);      // before SetParams, which allocates the norm's buffers
+  // slot[i] = the first norm partial of the arena's param i (ceil(count / B2C_SUMSQ_BLOCK_ELEMS) each, in arena order); returns
+  // the partial count
+  static size_t ClipSlots(const vector<size_t>& counts, vector<size_t>* slot);
+  // the norm partials of params [from, to] (reduced diffs) on `stream`
+  void ClipNorm(int id_from, int id_to, cudaStream_t stream);
+  // norm and factor from every partial, on `stream`, after the last ClipNorm of the iteration
+  void ClipFactor(cudaStream_t stream);
+  // the device state ClipFactor writes; synchronises the device
+  b2c_clip_state ClipState();
  private:
   SolverParameter param_;
   int kind_;
   ParamArena arena_;
   vector<ParamSpec> specs_;
   int iter_ = 0, current_step_ = 0;
+  vector<size_t> clip_slot_;
+  size_t clip_nslots_ = 0;
+  double* clip_partials_ = nullptr;
+  b2c_clip_state* clip_state_ = nullptr;
 };
 
 // Bucket plan of Net::ReduceAndUpdate (net.cpp:772-783,824-862): params arrive in reverse order (last
@@ -451,7 +472,9 @@ class P2PSync : public SolverCallback {
 
 // Event-driven Net::ReduceAndUpdate: after the backward pass has produced the diffs of bucket b on the
 // compute stream, the comm stream allreduces it and runs the fused update for its params, overlapping
-// with the remaining backward work.  No host thread, no host barrier.
+// with the remaining backward work.  No host thread, no host barrier.  With clip_gradients the bucket's
+// norm partials take the update's place, and end_of_iteration enqueues the factor and one update of the
+// whole arena behind the last bucket, on the same stream.
 class ReduceScheduler {
  public:
   ReduceScheduler(SGDSolver* solver, SolverCallback* sync);

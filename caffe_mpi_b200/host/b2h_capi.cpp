@@ -2,6 +2,7 @@
 // (The C++ classes in b2caffe.hpp are the interface a Caffe maintainer codes against; this file only
 // marshals arrays so Python can drive them.)  Every function returns 0 / a handle, or -1 / NULL with the
 // message available from b2h_last_error().
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -219,6 +220,25 @@ int b2h_solver_step(void* hv) {
   });
 }
 int b2h_solver_iter(void* hv) { return static_cast<SolverHandle*>(hv)->solver->iter(); }
+// SolverParameter.clip_gradients of a solver handle (negative: off); before b2h_solver_set_params
+int b2h_solver_set_clip_gradients(void* hv, float clip) { B2H_TRY(static_cast<SolverHandle*>(hv)->solver->set_clip_gradients(clip)); }
+static int clip_state(SGDSolver& s, float* norm, float* factor, long long* clipped) {
+  B2H_TRY({
+    const b2c_clip_state st = s.ClipState();
+    *norm = st.norm; *factor = st.factor; *clipped = st.clipped;
+  });
+}
+// the last iteration's gradient norm and factor, and the clipped iterations so far; synchronises the device
+int b2h_solver_clip_state(void* hv, float* norm, float* factor, long long* clipped) {
+  return clip_state(*static_cast<SolverHandle*>(hv)->solver, norm, factor, clipped);
+}
+// the first norm partial of each of `n` params with these counts, in arena order (no device memory); returns the partial count
+long long b2h_clip_slots(int n, const size_t* counts, size_t* slot) {
+  vector<size_t> s;
+  const size_t total = SGDSolver::ClipSlots(vector<size_t>(counts, counts + n), &s);
+  std::copy(s.begin(), s.end(), slot);
+  return (long long)total;
+}
 
 // ---- prototxt / Net -----------------------------------------------------------------------------------------------
 void* b2h_net_create(const char* path_or_text, int is_text, int phase, int batch_override, int def_channels, int def_size) {
@@ -465,6 +485,9 @@ int b2h_trainer_param(void* hv, int i, int what, int set, float* buf) {   // wha
     if (set) { CUDA_CHECK(cudaMemcpy(dev, buf, sizeof(float) * b.count(), cudaMemcpyHostToDevice)); if (what == 0) h->net->MarkParamsDirty(); }
     else CUDA_CHECK(cudaMemcpy(buf, dev, sizeof(float) * b.count(), cudaMemcpyDeviceToHost));
   });
+}
+int b2h_trainer_clip_state(void* hv, float* norm, float* factor, long long* clipped) {
+  return clip_state(static_cast<TrainerHandle*>(hv)->net->solver(), norm, factor, clipped);
 }
 int b2h_trainer_snapshot(void* hv, const char* prefix, char* state_path, int len) {
   auto* h = static_cast<TrainerHandle*>(hv);

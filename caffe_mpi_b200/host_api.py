@@ -57,6 +57,11 @@ def lib():
         L.b2h_solver_attach_sync.argtypes = [vp, i, i, C.c_char_p, i]
         L.b2h_solver_step.argtypes = [vp]
         L.b2h_solver_iter.argtypes = [vp]
+        L.b2h_solver_set_clip_gradients.argtypes = [vp, f]
+        L.b2h_solver_clip_state.argtypes = [vp, C.POINTER(f), C.POINTER(f), C.POINTER(C.c_longlong)]
+        L.b2h_trainer_clip_state.argtypes = [vp, C.POINTER(f), C.POINTER(f), C.POINTER(C.c_longlong)]
+        L.b2h_clip_slots.argtypes = [i, szp, szp]
+        L.b2h_clip_slots.restype = C.c_longlong
         _lib = L
     return _lib
 
@@ -123,17 +128,24 @@ class ConvolutionLayer:
 
 class SGDSolver:
     """caffe::SGDSolver over a standalone arena.  `type` picks the update (SGD, Nesterov, AdaGrad, RMSProp, AdaDelta, Adam);
-    delta, momentum2 and rms_decay are the SolverParameter fields those read.  get(i, 3) is the second history (AdaDelta, Adam)."""
+    delta, momentum2 and rms_decay are the SolverParameter fields those read.  get(i, 3) is the second history (AdaDelta, Adam).
+    clip_gradients >= 0 scales every step's gradient to that global L2 norm when it is larger (negative: off)."""
 
     def __init__(self, base_lr=0.01, lr_policy="fixed", gamma=0.1, power=1.0, stepsize=1, max_iter=1, momentum=0.0,
                  weight_decay=0.0, regularization_type="L2", iter_size=1, reduce_buckets=6, stepvalue=(), rampup_interval=0,
-                 rampup_lr=0.0, min_lr=0.0, type="SGD", delta=1e-8, momentum2=0.999, rms_decay=0.0):
+                 rampup_lr=0.0, min_lr=0.0, type="SGD", delta=1e-8, momentum2=0.999, rms_decay=0.0, clip_gradients=-1.0):
         sv = list(stepvalue)
         self._h = lib().b2h_solver_create_typed(type.encode(), base_lr, lr_policy.encode(), gamma, power, stepsize, max_iter, momentum,
                                                 weight_decay, regularization_type.encode(), iter_size, reduce_buckets, len(sv),
                                                 _ia(sv) if sv else None, rampup_interval, rampup_lr, min_lr, delta, momentum2, rms_decay)
         if not self._h:
             raise HostError(lib().b2h_last_error().decode())
+        if clip_gradients != -1.0:
+            _ck(lib().b2h_solver_set_clip_gradients(self._h, clip_gradients))
+
+    def clip_state(self):
+        """(norm, factor, clipped_count): the last step's gradient norm and scale factor, and the steps clipped so far."""
+        return _clip_state(lib().b2h_solver_clip_state, self._h)
 
     def lr_at(self, it):
         v = lib().b2h_solver_lr_at(self._h, it)
@@ -182,6 +194,21 @@ class SGDSolver:
         if getattr(self, "_h", None) and _lib is not None:
             _lib.b2h_solver_destroy(self._h)
             self._h = None
+
+
+def _clip_state(fn, h):
+    n, f = C.c_float(), C.c_float()
+    c = C.c_longlong()
+    _ck(fn(h, C.byref(n), C.byref(f), C.byref(c)))
+    return n.value, f.value, c.value
+
+
+def clip_slots(counts):
+    """(first norm partial of each param, partial count) for params with these element counts, in arena order"""
+    n = len(counts)
+    out = (C.c_size_t * max(1, n))()
+    total = lib().b2h_clip_slots(n, (C.c_size_t * max(1, n))(*counts), out)
+    return [out[i] for i in range(n)], int(total)
 
 
 def plan_buckets(counts, reduce_buckets=6):
@@ -420,6 +447,11 @@ class Trainer:
         n = C.c_int()
         _ck(lib().b2h_trainer_bucket_times(self._h, cap, by, ms, C.byref(n)))
         return [(int(by[i]), float(ms[i])) for i in range(min(n.value, cap))]
+
+    def clip_state(self):
+        """(norm, factor, clipped_count) with clip_gradients: the last step's L2 norm of the gradient, the factor the update used,
+        and the steps clipped so far.  Synchronises the device."""
+        return _clip_state(lib().b2h_trainer_clip_state, self._h)
 
     def clear_param_diffs(self):
         """Net::ClearParamDiffs: Step() expects zeroed diffs (the update clears them); call this after a forward_backward() made

@@ -388,6 +388,47 @@ int b2c_solver_update_arena(int kind, int nseg, const size_t* offset, const size
 int b2c_debug_solver_plan(int kind, int nseg, const size_t* offset, const size_t* count, const void* g, const void* w,
                           const void* h, const void* h2, int* launch_out, int max_launches, int* nlaunch, long long* seg_out);
 
+/* ---- gradient clipping (SolverParameter.clip_gradients) -----------------------------------------------------------------
+ * Replaces SGDSolver::ClipGradients (sgd_solver.cpp:111-128): there one float sumsq_diff per learnable blob (a cuBLAS sdot each),
+ * summed on the host, then a cublasSscal per blob.  Here the squared L2 norm of the whole diff arena is accumulated in double,
+ * bucket by bucket on the stream that reduces the gradients; one CTA turns it into a factor in device memory; the update reads
+ * the factor.  The host reads nothing on the training path.  Partials depend only on each segment's address and count, so the
+ * norm is the same whichever buckets carry the segments. */
+#define B2C_SUMSQ_BLOCK_ELEMS 4096
+/* sum(g^2) over segment s, one double per block of B2C_SUMSQ_BLOCK_ELEMS elements: block b of segment s (ceil(count[s] / 4096)
+ * blocks) writes partials[slot[s] + b].  Within a block each of 256 threads sums its elements in order in double (the head
+ * scalars that peel g to 16 bytes, its float4 units, the tail), then a shuffle tree per warp, then the eight warps in order.
+ * Segments are taken as b2c_solver_update_arena takes them: in order, zero counts skipped, at most 96 per launch.  Refuses
+ * (B2C_ERR_INVALID) nseg < 0, a null layout array, g or partials, a count >= 2^32; a refused call launches nothing. */
+int b2c_arena_sumsq(int nseg, const size_t* offset, const size_t* count, const size_t* slot, const float* g, double* partials,
+                    void* stream);
+typedef struct b2c_clip_state {
+  float norm;         /* the last iteration's L2 norm of the scaled gradient */
+  float factor;       /* the last iteration's scale: clip / norm when norm > clip, else 1 */
+  long long clipped;  /* iterations with norm > clip so far */
+} b2c_clip_state;
+/* One CTA: S = the sum of partials[0..nslots) (thread t sums the slots t mod 256 in order, then the fixed tree of
+ * b2c_arena_sumsq); norm = (float)sqrt(s_n^2 * S) formed in double, s_n = 1/(solver_count * global_grad_scale), the scale the
+ * net applies before ClipGradients (net.cpp:815-817,910); factor = norm > clip ? clip / norm : 1 in IEEE float, so a NaN norm
+ * does not scale (sgd_solver.cpp:118-127).  Writes state->norm and ->factor and counts a clipped iteration in ->clipped, which
+ * the caller zeroes once.  Refuses a null state, null partials with nslots > 0, clip < 0 or NaN, s_n not positive and finite. */
+int b2c_clip_factor(const double* partials, size_t nslots, double s_n, float clip, b2c_clip_state* state, void* stream);
+/* b2c_solver_update_arena with grad_scale replaced, once per thread, by the rounded product grad_scale * *factor (a device
+ * address, normally &state->factor of b2c_clip_factor).  Weight decay is not scaled: Regularize follows ClipGradients
+ * (sgd_solver.cpp:143-149).  A factor of 1 gives b2c_solver_update_arena's bits.  Refuses what b2c_solver_update_arena
+ * refuses, and a null factor. */
+int b2c_solver_update_arena_scaled(int kind, int nseg, const size_t* offset, const size_t* count,
+                                   const float* local_rate, const float* local_decay,
+                                   float* g, float* w, float* h, float* h2, b2c_solver_hparams hp,
+                                   int l2, float grad_scale, const float* factor, int clear_grads, void* stream);
+/* The launches b2c_arena_sumsq makes for this layout with the diff arena at g (only tested for alignment).  *nlaunch,
+ * launch_out as b2c_debug_solver_plan.  seg_out[7s..7s+6] for segment s: its launch (-1 when count is 0), 1 when its blocks take
+ * the float4 path, its blocks, its first slot, and summed over its blocks the head scalars, float4 units and tail scalars.
+ * *npartials = max(slot[s] + blocks) over the segments: the partials a workspace needs.  Refuses what b2c_arena_sumsq refuses.
+ * Pure host computation. */
+int b2c_debug_sumsq_plan(int nseg, const size_t* offset, const size_t* count, const size_t* slot, const void* g, int* launch_out,
+                         int max_launches, int* nlaunch, long long* seg_out, long long* npartials);
+
 /* ---- gradient exchange ---------------------------------------------------------------------
  * Replaces P2PManager/P2PSync's NCCL use (src/caffe/parallel.cpp:36-87,145-253) and the MPI
  * bootstrap (src/caffe/clusters.cpp:8-16; parallel.cpp:42-45,163-172).  One communicator per

@@ -154,6 +154,7 @@ def cmd_train(args):
     snap_every = int(sp("snapshot", "0"))
     snap_prefix = args.snapshot_prefix or sp("snapshot_prefix", "")
     snap_after = sp("snapshot_after_train", "true").lower() in ("true", "1")
+    clip = float(sp("clip_gradients", "-1"))
     if rank == 0:
         log("Data layer: %s" % ("reading the LMDB named by data_param.source" if t.database_batches() >= 0 else "synthetic in-memory source"))
         log("Solving %s with %s: %d learnable blobs, lr_policy %s base_lr %g %s weight_decay %g, %d iteration(s) on %d GPU(s)" %
@@ -239,6 +240,14 @@ def cmd_train(args):
             break
         if rank == 0 and show:
             log("Iteration %d (%.2f iter/s%s), loss = %.6g" % (it, n / (ms / 1e3), ", %.1f img/s" % (batch * world * n / (ms / 1e3)) if batch else "", t.loss()))
+            if clip >= 0:
+                # SGDSolver::ClipGradients' line (sgd_solver.cpp:122-125) for the last iteration, at display points only: the norm
+                # lives on the device and reading it every iteration would synchronise every step
+                import numpy as np
+                norm, factor, _ = t.clip_state()
+                if np.float32(norm) > np.float32(clip):
+                    log("Gradient clipping: scaling down gradients (L2 norm %g > %g) by scale factor %g" % (norm, np.float32(clip), factor),
+                        sys.stderr)
         if rank == 0 and snap and snap_prefix:
             log("Snapshotting solver state to binary proto file %s" % t.snapshot(snap_prefix))
             last_snapshot = it
