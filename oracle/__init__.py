@@ -95,6 +95,9 @@ def lib():
         L.b2o_conv_forward.argtypes = [P, _f32p, _f32p, C.c_void_p, _f32p, C.c_int]
         L.b2o_conv_backward.argtypes = [P, _f32p, _f32p, _f32p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.b2o_conv_direct.argtypes = [P, _f32p, _f32p, C.c_void_p, _f32p]
+        L.b2o_conv_fwd_ffma.argtypes = [P, _f32p, _f32p, C.c_void_p, _f32p]
+        L.b2o_conv_dgrad_ffma.argtypes = [P, _f32p, _f32p, _f32p]
+        L.b2o_conv_wgrad_ffma.argtypes = [P, _f32p, _f32p, _f32p]
         L.b2o_sgd_update.argtypes = [C.c_size_t, _f32p, _f32p, _f32p, C.c_float, C.c_float, C.c_float,
                                      C.c_int, C.c_float, C.c_int, C.c_int]
         L.b2o_learning_rate.argtypes = [C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int,
@@ -224,6 +227,31 @@ def conv_direct(prm, x, w, bias=None):
     lib().b2o_conv_direct(C.byref(prm), np.ascontiguousarray(x, np.float32), np.ascontiguousarray(w, np.float32),
                           _ptr(bias), y)
     return y
+
+
+def conv_fwd_ffma(prm, x, w, bias=None):
+    """What the product's FFMA forward kernel (conv_fwd_simt_kernel) stores, bit for bit: one fmaf chain per output over
+    (c, i, j) without the padded taps, then + bias"""
+    y = np.empty(prm.y_shape(), np.float32)
+    lib().b2o_conv_fwd_ffma(C.byref(prm), np.ascontiguousarray(x, np.float32), np.ascontiguousarray(w, np.float32),
+                            _ptr(None if bias is None else np.ascontiguousarray(bias, np.float32)), y)
+    return y
+
+
+def conv_dgrad_ffma(prm, w, dy):
+    """What the product's FFMA data-gradient kernel (conv_dgrad_simt_kernel) stores, bit for bit: one fmaf chain per dx element
+    over (i, j, o in the group), on-grid taps only"""
+    dx = np.empty(prm.x_shape(), np.float32)
+    lib().b2o_conv_dgrad_ffma(C.byref(prm), np.ascontiguousarray(dy, np.float32), np.ascontiguousarray(w, np.float32), dx)
+    return dx
+
+
+def conv_wgrad_ffma(prm, x, dy, dw0=None):
+    """What the product's FFMA weight-gradient kernel (conv_wgrad_simt_kernel) leaves in dw, bit for bit, starting from dw0
+    (zeros when None): 256 lane-strided chains, the warp butterflies, the 8 warp partials in order, one add onto dw0"""
+    dw = np.zeros(prm.w_shape(), np.float32) if dw0 is None else np.ascontiguousarray(dw0, np.float32).reshape(prm.w_shape()).copy()
+    lib().b2o_conv_wgrad_ffma(C.byref(prm), np.ascontiguousarray(x, np.float32), np.ascontiguousarray(dy, np.float32), dw)
+    return dw
 
 
 def sgd_update(g, w, h, momentum, local_rate, local_decay, l2=True, grad_scale=1.0, iter_size=1, clear_grads=True):

@@ -260,6 +260,121 @@ void b2o_gemv_ffma(int transA, int M, int N, float alpha, const float* A, const 
 }
 
 /* ------------------------------------------------------------------------- *
+ * Bit-exact restatements of the product's FFMA direct-convolution kernels
+ * (caffe_mpi_b200/csrc/conv_simt.cu), so a test can compare them bit for bit.
+ * Each output element is one fmaf chain starting from +0; a tap that falls in
+ * the padding (or, for the data gradient, off the stride grid) is skipped, not
+ * multiplied by 0, so no chain ever sees a padded zero.
+ * ------------------------------------------------------------------------- */
+/* conv_fwd_simt_kernel: per y[n][o][ho][wo]
+ *   acc = fmaf(x, w, acc) over c (0 .. Cg-1), then i, then j     (:27-35)
+ *   skipping (unsigned)h >= H (:30) and (unsigned)ww >= W (:33);
+ *   then one acc += bias[o] (:37), the bias never inside the chain. */
+void b2o_conv_fwd_ffma(const b2o_conv_params* p, const float* x, const float* w, const float* bias, float* y) {
+  const int Ho = b2o_out_h(p), Wo = b2o_out_w(p);
+  const int Cg = p->C / p->G, Og = p->O / p->G, Kd = Cg * p->kh * p->kw;
+  size_t idx = 0;
+  for (int n = 0; n < p->N; ++n)
+    for (int o = 0; o < p->O; ++o) {
+      const float* xg = x + ((size_t)n * p->C + (size_t)(o / Og) * Cg) * p->H * p->W;
+      const float* wr = w + (size_t)o * Kd;
+      for (int ho = 0; ho < Ho; ++ho)
+        for (int wo = 0; wo < Wo; ++wo, ++idx) {
+          float acc = 0.0f;
+          for (int c = 0; c < Cg; ++c)
+            for (int i = 0; i < p->kh; ++i) {
+              const int h = ho * p->sh - p->ph + i * p->dh;
+              if (h < 0 || h >= p->H) continue;
+              for (int j = 0; j < p->kw; ++j) {
+                const int ww = wo * p->sw - p->pw + j * p->dw;
+                if (ww < 0 || ww >= p->W) continue;
+                acc = fmaf(xg[((size_t)c * p->H + h) * p->W + ww], wr[(c * p->kh + i) * p->kw + j], acc);
+              }
+            }
+          if (p->has_bias && bias) acc += bias[o];
+          y[idx] = acc;
+        }
+    }
+}
+
+/* conv_dgrad_simt_kernel: per dx[n][c][h][w], g = c / Cg, cg = c % Cg
+ *   for i: hh = h + ph - i*dh; skip hh < 0 or hh % sh != 0; ho = hh / sh; skip ho >= Ho   (:53-57)
+ *     for j: the same for w                                                               (:58-62)
+ *       for o in the group (0 .. Og-1): acc = fmaf(dy[n][g*Og+o][ho][wo], w[g*Og+o][cg][i][j], acc)   (:65-66)
+ *   then dx = acc, overwritten (:69). */
+void b2o_conv_dgrad_ffma(const b2o_conv_params* p, const float* dy, const float* w, float* dx) {
+  const int Ho = b2o_out_h(p), Wo = b2o_out_w(p);
+  const int Cg = p->C / p->G, Og = p->O / p->G, Kd = Cg * p->kh * p->kw;
+  size_t idx = 0;
+  for (int n = 0; n < p->N; ++n)
+    for (int c = 0; c < p->C; ++c) {
+      const int g = c / Cg, cg = c - g * Cg;
+      for (int h = 0; h < p->H; ++h)
+        for (int ww = 0; ww < p->W; ++ww, ++idx) {
+          float acc = 0.0f;
+          for (int i = 0; i < p->kh; ++i) {
+            const int hh = h + p->ph - i * p->dh;
+            if (hh < 0 || hh % p->sh) continue;
+            const int ho = hh / p->sh;
+            if (ho >= Ho) continue;
+            for (int j = 0; j < p->kw; ++j) {
+              const int wv = ww + p->pw - j * p->dw;
+              if (wv < 0 || wv % p->sw) continue;
+              const int wo = wv / p->sw;
+              if (wo >= Wo) continue;
+              const float* dyp = dy + (((size_t)n * p->O + (size_t)g * Og) * Ho + ho) * Wo + wo;
+              const float* wp = w + (((size_t)g * Og * Cg + cg) * p->kh + i) * p->kw + j;
+              for (int o = 0; o < Og; ++o) acc = fmaf(dyp[(size_t)o * Ho * Wo], wp[(size_t)o * Kd], acc);
+            }
+          }
+          dx[idx] = acc;
+        }
+    }
+}
+
+/* conv_wgrad_simt_kernel: one block of 256 threads per (o, cg); per tap (i, j)   (:82-83)
+ *   thread t: acc = fmaf(dy[n][o][p], x[n][g*Cg+cg][h][w], acc) for q = t, t + 256, ... < N*Ho*Wo,
+ *     n = q / P, p = q % P, skipping taps in the padding                          (:85-92)
+ *   each warp: acc += shfl_xor(acc, off) for off = 16, 8, 4, 2, 1; lane 0 stores  (:94-95)
+ *   thread 0: t = 0; t += red[k] for the 8 warps in order                         (:98-99)
+ *   dw += t, once, onto what dw held (accumulated, :100). */
+void b2o_conv_wgrad_ffma(const b2o_conv_params* p, const float* x, const float* dy, float* dw) {
+  const int Ho = b2o_out_h(p), Wo = b2o_out_w(p), P = Ho * Wo;
+  const int Cg = p->C / p->G, Og = p->O / p->G;
+  const size_t Q = (size_t)p->N * P;
+  float part[256], t[32];
+  for (int o = 0; o < p->O; ++o)
+    for (int cg = 0; cg < Cg; ++cg) {
+      const int c = (o / Og) * Cg + cg;
+      for (int i = 0; i < p->kh; ++i)
+        for (int j = 0; j < p->kw; ++j) {
+          for (int th = 0; th < 256; ++th) {
+            float acc = 0.0f;
+            for (size_t q = (size_t)th; q < Q; q += 256) {
+              const int n = (int)(q / P), pp = (int)(q - (size_t)n * P);
+              const int ho = pp / Wo, wo = pp - ho * Wo;
+              const int h = ho * p->sh - p->ph + i * p->dh, ww = wo * p->sw - p->pw + j * p->dw;
+              if (h < 0 || h >= p->H || ww < 0 || ww >= p->W) continue;
+              acc = fmaf(dy[((size_t)n * p->O + o) * P + pp], x[(((size_t)n * p->C + c) * p->H + h) * p->W + ww], acc);
+            }
+            part[th] = acc;
+          }
+          float tot = 0.0f;
+          for (int wp = 0; wp < 8; ++wp) {
+            float* s = part + 32 * wp;
+            for (int off = 16; off; off >>= 1) {
+              for (int l = 0; l < 32; ++l) t[l] = s[l] + s[l ^ off];
+              for (int l = 0; l < 32; ++l) s[l] = t[l];
+            }
+            tot += s[0];
+          }
+          float* d = dw + (((size_t)o * Cg + cg) * p->kh + i) * p->kw + j;
+          *d += tot;
+        }
+    }
+}
+
+/* ------------------------------------------------------------------------- *
  * ConvolutionLayer::Forward_cpu (src/caffe/layers/conv_layer.cpp:24-40) with
  * forward_cpu_gemm / forward_cpu_bias (include/caffe/layers/base_conv_layer.hpp:36-60).
  * Per image: col = im2col(x_n) unless is_1x1_ (base_conv_layer.cpp:99-103),
