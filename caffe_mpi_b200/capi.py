@@ -21,6 +21,8 @@ CONV_ROUTES = ("caffe", "simt", "gather", "gather_scatter", "staged", "staged_pl
 POOL_ROUTES = ("max_scalar", "max_window", "max_bwd_row", "max_bwd_quad", "ave")
 # b2c_sgemm_route, in enum order
 SGEMM_ROUTES = ("ffma", "tc")
+# b2c_deconv_route, in enum order
+DECONV_ROUTES = ("dual", "phase", "depthwise")
 
 
 class B2CError(RuntimeError):
@@ -168,6 +170,21 @@ def lib():
         "b2c_lrn_backward": (i, [i, i, i, i, f, f, vp, vp, vp, vp, vp, vp]),
         "b2c_dropout_mask": (i, [sz, f, C.c_ulonglong, C.c_ulonglong, vp, vp]),
         "b2c_mul": (i, [sz, vp, vp, vp, vp]),
+        "b2c_deconv_desc_create": (i, [P, i, C.POINTER(vp)]),
+        "b2c_deconv_desc_destroy": (i, [vp]),
+        "b2c_deconv_desc_set_math": (i, [vp, i]),
+        "b2c_deconv_desc_set_algo": (i, [vp, i]),
+        "b2c_deconv_out_shape": (i, [vp, C.POINTER(i), C.POINTER(i)]),
+        "b2c_deconv_workspace_bytes": (sz, [vp, i]),
+        "b2c_deconv_forward": (i, [vp, vp, vp, vp, vp, vp, sz, vp]),
+        "b2c_deconv_backward_data": (i, [vp, vp, vp, vp, vp, sz, vp]),
+        "b2c_deconv_backward_filter": (i, [vp, vp, vp, vp, vp, sz, vp]),
+        "b2c_deconv_wgrad_split_bytes": (sz, [vp]),
+        "b2c_deconv_backward_filter_split": (i, [vp, vp, vp, vp, vp, sz, vp, sz, vp]),
+        "b2c_deconv_backward_bias": (i, [vp, vp, vp, vp]),
+        "b2c_debug_deconv_plan": (i, [vp, i, C.POINTER(i), i]),
+        "b2c_crop_forward": (i, [i, C.POINTER(i), C.POINTER(i), C.POINTER(i), vp, vp, vp]),
+        "b2c_crop_backward": (i, [i, C.POINTER(i), C.POINTER(i), C.POINTER(i), vp, vp, vp]),
         "b2c_comm_get_unique_id": (i, [vp]),
         "b2c_comm_init": (i, [i, i, vp, C.POINTER(vp)]),
         "b2c_comm_destroy": (i, [vp]),
@@ -316,6 +333,113 @@ class ConvDesc:
         L = lib()
         L.b2c_conv_desc_bind_filter_cache.argtypes = [C.c_void_p, C.c_void_p]
         check(L.b2c_conv_desc_bind_filter_cache(self._h, None))
+
+
+class DeconvDesc:
+    """b2c_deconv_desc owner: a transposed convolution given by its own parameters (ConvParams with Cin = bottom channels,
+    O = num_output, H, W = bottom extent).  Methods take torch CUDA tensors, like ConvDesc's."""
+
+    def __init__(self, params, engine=ENGINE_DEFAULT, math=None, algo=None):
+        self.params = params
+        h = C.c_void_p()
+        check(lib().b2c_deconv_desc_create(C.byref(params), engine, C.byref(h)))
+        self._h = h
+        if math is not None:
+            check(lib().b2c_deconv_desc_set_math(h, math))
+        if algo is not None:
+            check(lib().b2c_deconv_desc_set_algo(h, algo))
+        self._ws = None
+        self._split = None
+
+    def __del__(self):
+        if getattr(self, "_h", None) and _lib is not None:
+            _lib.b2c_deconv_desc_destroy(self._h)
+            self._h = None
+
+    def out_shape(self):
+        ht, wt = C.c_int(), C.c_int()
+        check(lib().b2c_deconv_out_shape(self._h, C.byref(ht), C.byref(wt)))
+        return ht.value, wt.value
+
+    def x_shape(self):
+        p = self.params
+        return (p.N, p.C, p.H, p.W)
+
+    def w_shape(self):
+        p = self.params
+        return (p.C, p.O // p.G, p.kh, p.kw)
+
+    def y_shape(self):
+        p = self.params
+        return (p.N, p.O) + self.out_shape()
+
+    def workspace_bytes(self, op):
+        return int(lib().b2c_deconv_workspace_bytes(self._h, op))
+
+    def plan(self, op):
+        """b2c_debug_deconv_plan: route, the dual's own route (DUAL route) and, on the phase route, (taps, tiles) per phase."""
+        n = 3 + 2 * self.params.sh * self.params.sw
+        out = (C.c_int * n)()
+        check(lib().b2c_debug_deconv_plan(self._h, op, out, n))
+        ph = [(out[3 + 2 * k], out[4 + 2 * k]) for k in range(out[2])]
+        return dict(route=DECONV_ROUTES[out[0]], dual_route=out[1], phases=out[2], phase_taps=[t for t, _ in ph],
+                    phase_tiles=[t for _, t in ph])
+
+    def _workspace(self, op, like):
+        import torch
+        need = self.workspace_bytes(op)
+        if need == 0:
+            return None, 0
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=like.device)
+        return C.c_void_p(self._ws.data_ptr()), self._ws.numel()
+
+    def forward(self, x, w, bias, y, stream=None):
+        ws, n = self._workspace(OP_FORWARD, x)
+        check(lib().b2c_deconv_forward(self._h, _p(x), _p(w), _p(bias), _p(y), ws, n, _stream(stream)))
+        return y
+
+    def backward_data(self, dy, w, dx, stream=None):
+        ws, n = self._workspace(OP_BACKWARD_DATA, dy)
+        check(lib().b2c_deconv_backward_data(self._h, _p(dy), _p(w), _p(dx), ws, n, _stream(stream)))
+        return dx
+
+    def backward_filter(self, x, dy, dw, stream=None):
+        ws, n = self._workspace(OP_BACKWARD_FILTER, x)
+        check(lib().b2c_deconv_backward_filter(self._h, _p(x), _p(dy), _p(dw), ws, n, _stream(stream)))
+        return dw
+
+    def wgrad_split_bytes(self):
+        return int(lib().b2c_deconv_wgrad_split_bytes(self._h))
+
+    def backward_filter_split(self, x, dy, dw, stream=None):
+        import torch
+        ws, n = self._workspace(OP_BACKWARD_FILTER, x)
+        need = self.wgrad_split_bytes()
+        if need and (self._split is None or self._split.numel() < need):
+            self._split = torch.empty(need, dtype=torch.uint8, device=x.device)
+        sp = C.c_void_p(self._split.data_ptr()) if need else None
+        check(lib().b2c_deconv_backward_filter_split(self._h, _p(x), _p(dy), _p(dw), ws, n, sp, need, _stream(stream)))
+        return dw
+
+    def backward_bias(self, dy, db, stream=None):
+        check(lib().b2c_deconv_backward_bias(self._h, _p(dy), _p(db), _stream(stream)))
+        return db
+
+
+def crop_forward(bottom, top, offsets, stream=None):
+    """b2c_crop_forward: top = bottom[offsets : offsets + top.shape] (offsets over every axis)."""
+    nax = bottom.dim()
+    check(lib().b2c_crop_forward(nax, _iarr(bottom.shape), _iarr(top.shape), _iarr(offsets), _p(bottom), _p(top), _stream(stream)))
+    return top
+
+
+def crop_backward(top_diff, bottom_diff, offsets, stream=None):
+    """b2c_crop_backward: bottom_diff = 0, then the top diff copied into the window."""
+    nax = bottom_diff.dim()
+    check(lib().b2c_crop_backward(nax, _iarr(bottom_diff.shape), _iarr(top_diff.shape), _iarr(offsets), _p(top_diff),
+                                  _p(bottom_diff), _stream(stream)))
+    return bottom_diff
 
 
 def im2col(im, col, k, s, p, d, stream=None):

@@ -121,6 +121,19 @@ size_t tc_wgrad_stg_workspace(const ConvShape&);
 int launch_conv_tc_wgrad_stg(const ConvShape&, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t,
                              void* split = nullptr, size_t split_bytes = 0);
 bool tc_wgrad_stg_plan_info(const ConvShape&, WgradPlanInfo*);
+// One output phase of a strided transposed convolution along one axis (deconv.cu): the outputs t = t0 + s*m, m < M, are the
+// stride-1 correlation of the bottom with n taps of the filter (tap l reads filter tap i0 + (n-1-l)*L), dilation dd, pad `pad`
+// (negative where the phase's first output lies beyond the pad).  n == 0: no tap reaches these outputs.
+struct DeconvPhaseAxis { int t0, M, n, i0, L, dd, pad; };
+// The gather kernel (conv_tc.cu) on phase (a, b) of the transposed convolution whose dual convolution is `dual` (dual input = the
+// transposed convolution's top, dual output = its bottom): x = bottom, out = top (only the phase's lattice is written, + bias).
+bool tc_deconv_phase_supported(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b);
+size_t tc_deconv_phase_prep_bytes(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, int math);
+void tc_deconv_phase_prep_entry(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, int math, const float* w,
+                                void* dst, PrepEntry* q);
+void tc_deconv_phase_plan_info(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, ConvPlanInfo* q);
+int launch_deconv_phase_tc(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, int math, const float* x,
+                           const float* bias, float* out, const PrepEntry& q, cudaStream_t st);
 bool tc_gemm_supported(bool tA, bool tB, int M, int N, int K);
 size_t tc_gemm_workspace(bool tA, bool tB, int M, int N, int K);
 // The kernel b2c_sgemm_ex runs and its plan, decided in one place (sgemm_route) for the launch and for b2c_debug_sgemm_plan.

@@ -485,6 +485,8 @@ void tc_conv_plan_info(const ConvShape& s, int op, ConvPlanInfo* q) {
 }
 bool tc_conv_scatter(const ConvShape& s, int op) { return op == B2C_OP_BACKWARD_DATA && !dgrad_as_fwd(s); }
 
+static int launch_gather(FwdParams& p, const PrepEntry& q, int math, cudaStream_t st);
+
 // `prepared`: the filter already in GEMM layout (b2c_conv_prepare_filter) or null = run the prepass here into `ws`
 int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const float* b, const float* bias, float* out,
                    void* ws, size_t ws_bytes, const void* prepared, cudaStream_t st) {
@@ -501,13 +503,18 @@ int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const f
   p.dbg = dbg;
   if (!prepared)
     if (int rc = launch_filter_prep(&q, 1, st)) return rc;
+  return launch_gather(p, q, math, st);
+}
 
+// The gather kernel on the GEMM `p` describes, its filter operand prepared in q's planes (geometry, pointers and bias set by the
+// caller; the tile plan and the debug switches set here).
+static int launch_gather(FwdParams& p, const PrepEntry& q, int math, cudaStream_t st) {
   ConvPlanInfo plan;
   plan_tiles(p, &plan);
   const int n_tile = plan.n_tile, kmode = plan.variant;
   p.m_tiles = plan.m_tiles; p.n_tiles = plan.n_tiles; p.total_tiles = plan.tiles;
   alignas(64) CUtensorMap mh, ml;
-  const cuuint64_t dims[3] = {(cuuint64_t)p.Kp, (cuuint64_t)q.rows, (cuuint64_t)s.G};
+  const cuuint64_t dims[3] = {(cuuint64_t)p.Kp, (cuuint64_t)q.rows, (cuuint64_t)p.G};
   const cuuint64_t strides[2] = {(cuuint64_t)p.Kp * 4, (cuuint64_t)p.Kp * 4 * (cuuint64_t)q.rows};
   const cuuint32_t box[3] = {32, (cuuint32_t)n_tile, 1};
   if (int rc = make_tensor_map_3d(&mh, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, q.hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "conv filter"))
@@ -529,6 +536,57 @@ int launch_conv_tc(const ConvShape& s, int op, int math, const float* a, const f
             n_tile, p.Kp / 32, p.total_tiles, h[0], h[1], h[2], h[3], h[4]);
   }
   return rc;
+}
+
+// ---- transposed convolution, one output phase (deconv.cu): a stride-1 gather GEMM over the bottom whose epilogue writes the
+// phase's lattice of the top through out_hs / out_ws, starting at (a.t0, b.t0)
+static FwdParams deconv_phase_params(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b) {
+  FwdParams p{};
+  p.Cin_tot = dual.O; p.Cg = dual.Og; p.H = dual.Ho; p.W = dual.Wo;
+  p.kh = a.n; p.kw = b.n; p.sh = 1; p.sw = 1; p.ph = a.pad; p.pw = b.pad; p.dh = a.dd; p.dw = b.dd;
+  p.Ho = a.M; p.Wo = b.M; p.Mtot = dual.N * a.M * b.M;
+  p.Ntot = dual.Cg; p.K = dual.Og * a.n * b.n; p.Kp = padded_k(p.K);
+  p.Cout_tot = dual.C; p.out_plane = (long long)dual.H * dual.W; p.out_hs = dual.sh * dual.W; p.out_ws = dual.sw;
+  p.G = dual.G;
+  return p;
+}
+bool tc_deconv_phase_supported(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b) {
+  if ((long long)dual.N * a.M * b.M > 0x7fffffffLL || (long long)dual.N * dual.Ho * dual.Wo > 0x7fffffffLL) return false;
+  if ((long long)dual.O * dual.Ho * dual.Wo >= 0x7fffffffLL || (long long)dual.C * dual.H * dual.W >= 0x7fffffffLL) return false;
+  if ((a.n - 1) * a.dd > 0x7fff || (b.n - 1) * b.dd > 0x7fff) return false;
+  const int Kp = padded_k(dual.Og * a.n * b.n);
+  return (dual.Og % 4 == 0 ? Kp / 4 : Kp) <= TAB_ENTRIES;
+}
+size_t tc_deconv_phase_prep_bytes(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, int math) {
+  const size_t np = math == B2C_MATH_FP32 ? 2 : 1;
+  return sizeof(float) * np * (size_t)dual.G * dual.Cg * padded_k(dual.Og * a.n * b.n);
+}
+// dst: 256-byte aligned, tc_deconv_phase_prep_bytes long
+void tc_deconv_phase_prep_entry(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, int math, const float* w,
+                                void* dst, PrepEntry* q) {
+  *q = PrepEntry{};
+  float* wbase = static_cast<float*>(dst);
+  q->w = w; q->kind = 0; q->G = dual.G; q->Og = dual.Og; q->Cg = dual.Cg; q->taps = a.n * b.n;
+  q->mode = 2; q->rows = dual.Cg;
+  q->K = dual.Og * a.n * b.n; q->Kp = padded_k(q->K);
+  q->tap_major = (dual.Og % 4 == 0) ? 1 : 0;
+  q->flip = 0; q->kch = dual.Og;
+  q->src_taps = dual.kh * dual.kw; q->src_kw = dual.kw; q->sub_kh = a.n; q->sub_kw = b.n;
+  q->i0h = a.i0; q->i0w = b.i0; q->Lh = a.L; q->Lw = b.L;
+  q->total = (long long)dual.G * q->rows * q->Kp;
+  q->hi = wbase;
+  q->lo = math == B2C_MATH_FP32 ? static_cast<void*>(wbase + q->total) : nullptr;
+}
+void tc_deconv_phase_plan_info(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, ConvPlanInfo* q) {
+  *q = ConvPlanInfo{};
+  plan_tiles(deconv_phase_params(dual, a, b), q);
+}
+int launch_deconv_phase_tc(const ConvShape& dual, const DeconvPhaseAxis& a, const DeconvPhaseAxis& b, int math, const float* x,
+                           const float* bias, float* out, const PrepEntry& q, cudaStream_t st) {
+  FwdParams p = deconv_phase_params(dual, a, b);
+  p.x = x; p.bias = bias;
+  p.out = out + (long long)a.t0 * dual.W + b.t0;
+  return launch_gather(p, q, math, st);
 }
 
 TC_DEBUG_EXPORT(debug_mbar_fwd)

@@ -32,7 +32,13 @@ filter_prep_multi_kernel(const __grid_constant__ PrepBatch b) {
     if (valid) {
       if (q.flip) tap = q.taps - 1 - tap;
       const int o = q.mode == 0 ? row : ch, c = q.mode == 0 ? ch : row;
-      v = __ldg(q.w + (((long long)g * q.Og + o) * q.Cg + c) * q.taps + tap);
+      int taps = q.taps;
+      if (q.mode == 2) {
+        const int a = tap / q.sub_kw, bb = tap - a * q.sub_kw;
+        tap = (q.i0h + (q.sub_kh - 1 - a) * q.Lh) * q.src_kw + q.i0w + (q.sub_kw - 1 - bb) * q.Lw;
+        taps = q.src_taps;
+      }
+      v = __ldg(q.w + (((long long)g * q.Og + o) * q.Cg + c) * taps + tap);
     }
     if (q.kind == 1) {
       const __nv_bfloat16 h = __float2bfloat16_rn(v);

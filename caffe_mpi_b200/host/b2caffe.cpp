@@ -161,6 +161,16 @@ void Fill(const FillerParameter& f, Blob* b) {
   } else if (f.type == "msra") {                       // filler.hpp:381: N(0, sqrt(2/n))
     std::normal_distribution<float> g(0.f, std::sqrt(2.f / nval));
     for (size_t i = 0; i < n; ++i) d[i] = g(rng);
+  } else if (f.type == "bilinear") {                   // filler.hpp BilinearFiller, as the modelled reference writes it:
+    B2_CHECK(b->num_axes() == 4, "Blob must be 4 dim.");
+    B2_CHECK(b->shape(3) == b->shape(2), "Filter must be square");
+    const int k = b->shape(3);
+    const int f2 = k / 2;                                // ceil(width / 2) with integer division: k / 2 for odd k too
+    const float c = (2 * f2 - 1 - f2 % 2) / (2.f * f2);
+    for (size_t i = 0; i < n; ++i) {
+      const float x = (float)(i % k), y = (float)((i / k) % k);
+      d[i] = (float)((1. - std::fabs(x / f2 - c)) * (1. - std::fabs(y / f2 - c)));
+    }
   } else {
     B2_CHECK(false, "Unknown filler name: " + f.type);
   }
@@ -289,7 +299,7 @@ void ConvolutionLayer::LayerSetUp(const vector<Blob*>& bottom, const vector<Blob
   group_ = cp.group;
   B2_CHECK(channels_ % group_ == 0, "channels not divisible by group");
   B2_CHECK(num_output_ % group_ == 0, "Number of output should be multiples of group.");
-  vector<int> wshape{num_output_, channels_ / group_};
+  vector<int> wshape = reverse_dimensions() ? vector<int>{channels_, num_output_ / group_} : vector<int>{num_output_, channels_ / group_};
   for (int k : kernel_shape_) wshape.push_back(k);
   bias_term_ = cp.bias_term;
   if (!blobs_.empty()) {
@@ -461,6 +471,130 @@ void ConvolutionLayer::Backward_gpu(const vector<Blob*>& top, const vector<bool>
                               col + (size_t)g * Kd * P, st));
         B2C_CHECK(b2c_col2im_nd(col, num_spatial_axes_, im_shape.data(), col_shape.data(), kernel_shape_.data(), pad_.data(),
                                 stride_.data(), dilation_.data(), bottom[i]->mutable_gpu_diff() + n * bdim, st));
+      }
+    }
+  }
+}
+
+// ================================================================================================ Deconvolution
+static shared_ptr<LayerBase> GetDeconvolutionLayer(const LayerParameter& p) { return shared_ptr<LayerBase>(new DeconvolutionLayer(p)); }
+REGISTER_LAYER_CREATOR(Deconvolution, GetDeconvolutionLayer);
+
+DeconvolutionLayer::~DeconvolutionLayer() { if (ddesc_) b2c_deconv_desc_destroy(ddesc_); }
+
+void DeconvolutionLayer::compute_output_shape() {   // deconv_layer.cpp:7-22
+  output_shape_.clear();
+  for (int i = 0; i < num_spatial_axes_; ++i) {
+    const int in = bottom_shape_[channel_axis_ + 1 + i];
+    const int ext = dilation_[i] * (kernel_shape_[i] - 1) + 1;
+    output_shape_.push_back(stride_[i] * (in - 1) + ext - 2 * pad_[i]);
+  }
+}
+
+void DeconvolutionLayer::Reshape(const vector<Blob*>& bottom, const vector<Blob*>& top) {
+  const int first_spatial = channel_axis_ + 1;
+  B2_CHECK(bottom[0]->num_axes() == first_spatial + num_spatial_axes_, "bottom num_axes may not change.");
+  num_ = (int)bottom[0]->count(0, channel_axis_);
+  B2_CHECK(bottom[0]->shape(channel_axis_) == channels_, "Input size incompatible with convolution kernel.");
+  for (size_t i = 1; i < bottom.size(); ++i) B2_CHECK(bottom[0]->shape() == bottom[i]->shape(), "All inputs must have the same shape.");
+  bottom_shape_ = bottom[0]->shape();
+  compute_output_shape();
+  vector<int> tshape(bottom_shape_.begin(), bottom_shape_.begin() + channel_axis_);
+  tshape.push_back(num_output_);
+  for (int o : output_shape_) { B2_CHECK(o > 0, "Deconvolution: non-positive output extent (pad larger than the upsampled input)"); tshape.push_back(o); }
+  for (Blob* t : top) t->Reshape(tshape);
+  if (num_spatial_axes_ == 2 && !layer_param_.convolution_param.force_nd_im2col) {
+    b2c_conv_params p{num_, channels_, bottom_shape_[first_spatial], bottom_shape_[first_spatial + 1], num_output_, group_,
+                      kernel_shape_[0], kernel_shape_[1], stride_[0], stride_[1], pad_[0], pad_[1], dilation_[0], dilation_[1],
+                      bias_term_ ? 1 : 0};
+    if (!ddesc_ || memcmp(&p, &ddesc_params_, sizeof(p)) != 0) {
+      if (ddesc_) b2c_deconv_desc_destroy(ddesc_);
+      ddesc_ = nullptr;
+      B2C_CHECK(b2c_deconv_desc_create(&p, layer_param_.convolution_param.engine, &ddesc_));
+      B2C_CHECK(b2c_deconv_desc_set_math(ddesc_, layer_param_.convolution_param.math));
+      ddesc_params_ = p;
+    }
+  }
+}
+
+// N-D helpers: the top is the dual convolution's "image" [O, top spatial], the col buffer [Kd*G, bottom spatial] with
+// Kd = (O/G)*prod(k) (BaseConvolutionLayer with reverse_dimensions: conv_in_channels_ = O, conv_out_channels_ = C)
+void DeconvolutionLayer::Forward_gpu(const vector<Blob*>& bottom, const vector<Blob*>& top) {
+  cudaStream_t st = Caffe::thread_stream();
+  const float* w = blobs_[0]->gpu_data();
+  const float* b = bias_term_ ? blobs_[1]->gpu_data() : nullptr;
+  for (size_t i = 0; i < bottom.size(); ++i) {
+    if (ddesc_) {
+      const size_t need = b2c_deconv_workspace_bytes(ddesc_, B2C_OP_FORWARD);
+      void* ws = need ? workspace(need) : nullptr;
+      B2C_CHECK(b2c_deconv_forward(ddesc_, bottom[i]->gpu_data(), w, b, top[i]->mutable_gpu_data(), ws, ws_bytes_, st));
+      continue;
+    }
+    // deconv_layer.cu Forward_gpu: backward_gpu_gemm (GEMM + col2im_nd) per image, then the bias (one add per element)
+    vector<int> im_shape{num_output_}, col_shape{(int)blobs_[0]->count(1) * group_};
+    size_t Pb = 1, Pt = 1;
+    for (int a = 0; a < num_spatial_axes_; ++a) {
+      im_shape.push_back(output_shape_[a]); col_shape.push_back(bottom_shape_[channel_axis_ + 1 + a]);
+      Pb *= (size_t)bottom_shape_[channel_axis_ + 1 + a]; Pt *= (size_t)output_shape_[a];
+    }
+    const int Kd = (int)blobs_[0]->count(1), Cg = channels_ / group_;
+    float* col = static_cast<float*>(workspace(sizeof(float) * (size_t)Kd * group_ * Pb));
+    const size_t bdim = bottom[i]->count(channel_axis_), tdim = top[i]->count(channel_axis_);
+    for (int n = 0; n < num_; ++n) {
+      for (int g = 0; g < group_; ++g)
+        B2C_CHECK(b2c_sgemm(1, 0, Kd, (int)Pb, Cg, 1.f, w + (size_t)g * Cg * Kd, bottom[i]->gpu_data() + n * bdim + (size_t)g * Cg * Pb, 0.f,
+                            col + (size_t)g * Kd * Pb, st));
+      B2C_CHECK(b2c_col2im_nd(col, num_spatial_axes_, im_shape.data(), col_shape.data(), kernel_shape_.data(), pad_.data(), stride_.data(),
+                              dilation_.data(), top[i]->mutable_gpu_data() + n * tdim, st));
+    }
+    if (b) B2C_CHECK(b2c_bias_forward(num_, num_output_, (int)Pt, b, top[i]->mutable_gpu_data(), st));
+  }
+}
+
+void DeconvolutionLayer::Backward_gpu(const vector<Blob*>& top, const vector<bool>& propagate_down, const vector<Blob*>& bottom) {
+  cudaStream_t st = Caffe::thread_stream();
+  const float* w = blobs_[0]->gpu_data();
+  for (size_t i = 0; i < top.size(); ++i) {
+    const float* dy = top[i]->gpu_diff();
+    if (ddesc_) {
+      if (bias_term_ && param_propagate_down_[1]) B2C_CHECK(b2c_deconv_backward_bias(ddesc_, dy, blobs_[1]->mutable_gpu_diff(), st));
+      if (param_propagate_down_[0]) {
+        const size_t need = (b2c_deconv_workspace_bytes(ddesc_, B2C_OP_BACKWARD_FILTER) + 255) & ~(size_t)255;
+        const size_t split = b2c_deconv_wgrad_split_bytes(ddesc_);
+        char* ws = need + split ? static_cast<char*>(workspace(need + split)) : nullptr;
+        B2C_CHECK(b2c_deconv_backward_filter_split(ddesc_, bottom[i]->gpu_data(), dy, blobs_[0]->mutable_gpu_diff(), ws, need,
+                                                   split ? ws + need : nullptr, split, st));
+      }
+      if (propagate_down[i]) {
+        const size_t need = b2c_deconv_workspace_bytes(ddesc_, B2C_OP_BACKWARD_DATA);
+        void* ws = need ? workspace(need) : nullptr;
+        B2C_CHECK(b2c_deconv_backward_data(ddesc_, dy, w, bottom[i]->mutable_gpu_diff(), ws, ws_bytes_, st));
+      }
+      continue;
+    }
+    // deconv_layer.cu Backward_gpu: bias gradient; per image im2col_nd of the top diff, then the weight GEMM
+    // (weight_gpu_gemm(top_diff, bottom_data)) and the bottom GEMM (forward_gpu_gemm(top_diff, weights))
+    vector<int> im_shape{num_output_}, col_shape{(int)blobs_[0]->count(1) * group_};
+    size_t Pb = 1, Pt = 1;
+    for (int a = 0; a < num_spatial_axes_; ++a) {
+      im_shape.push_back(output_shape_[a]); col_shape.push_back(bottom_shape_[channel_axis_ + 1 + a]);
+      Pb *= (size_t)bottom_shape_[channel_axis_ + 1 + a]; Pt *= (size_t)output_shape_[a];
+    }
+    const int Kd = (int)blobs_[0]->count(1), Cg = channels_ / group_;
+    float* col = static_cast<float*>(workspace(sizeof(float) * (size_t)Kd * group_ * Pb));
+    const size_t bdim = bottom[i]->count(channel_axis_), tdim = top[i]->count(channel_axis_);
+    if (bias_term_ && param_propagate_down_[1]) B2C_CHECK(b2c_bias_backward(num_, num_output_, (int)Pt, dy, blobs_[1]->mutable_gpu_diff(), st));
+    if (!param_propagate_down_[0] && !propagate_down[i]) continue;
+    for (int n = 0; n < num_; ++n) {
+      B2C_CHECK(b2c_im2col_nd(dy + n * tdim, num_spatial_axes_, im_shape.data(), col_shape.data(), kernel_shape_.data(), pad_.data(),
+                              stride_.data(), dilation_.data(), col, st));
+      for (int g = 0; g < group_; ++g) {
+        if (param_propagate_down_[0])
+          B2C_CHECK(b2c_sgemm(0, 1, Cg, Kd, (int)Pb, 1.f, bottom[i]->gpu_data() + n * bdim + (size_t)g * Cg * Pb, col + (size_t)g * Kd * Pb,
+                              1.f, blobs_[0]->mutable_gpu_diff() + (size_t)g * Cg * Kd, st));
+        if (propagate_down[i])
+          B2C_CHECK(b2c_sgemm(0, 0, Cg, (int)Pb, Kd, 1.f, w + (size_t)g * Cg * Kd, col + (size_t)g * Kd * Pb, 0.f,
+                              bottom[i]->mutable_gpu_diff() + n * bdim + (size_t)g * Cg * Pb, st));
       }
     }
   }

@@ -194,6 +194,7 @@ struct SliceParameter { int axis = 1; bool slice_dim_given = false; vector<int> 
 struct SoftmaxParameter { int axis = 1; };
 struct FlattenParameter { int axis = 1, end_axis = -1; };
 struct AccuracyParameter { int top_k = 1; };
+struct CropParameter { int axis = 2; vector<int> offset; };   // caffe.proto CropParameter; Net resolves `axis` to a canonical index
 struct ContrastiveLossParameter { float margin = 1.f; bool legacy_version = false; };
 struct TransformationParameter { float scale = 1.f; bool mirror = false; int crop_size = 0; vector<float> mean_value; string mean_file; long long random_seed = -1; };
 struct DataParameter {   // batch_size after Net's batch override; backend: LEVELDB = 0, LMDB = 1; parser_threads 0: automatic (see DataLayer)
@@ -219,6 +220,7 @@ struct LayerParameter {
   SoftmaxParameter softmax_param;
   FlattenParameter flatten_param;
   AccuracyParameter accuracy_param;
+  CropParameter crop_param;
   ContrastiveLossParameter contrastive_loss_param;
   TransformationParameter transform_param;
   DataParameter data_param;
@@ -288,7 +290,7 @@ class ConvolutionLayer : public LayerBase {
   // Prepared-filter cache (include/b2c.h "Prepared filters"): an owner of the iteration (TrainNet) enables it and then calls
   // b2c_conv_prepare_filters for all layers after every weight change; without it every Forward / Backward call re-derives
   // the GEMM-ordered filter copy itself.  Returns false when the layer has nothing to cache (CAFFE engine, SIMT, N-D).
-  bool EnableFilterCache();
+  virtual bool EnableFilterCache();
   bool SupportsBottomDiffAccumulate(int) const override { return desc_ && b2c_conv_backward_data_accumulate_supported(desc_) != 0; }
   const b2c_conv_desc* desc() const { return desc_; }
   void* filter_cache() const { return fcache_; }
@@ -297,7 +299,9 @@ class ConvolutionLayer : public LayerBase {
   void Forward_gpu(const vector<Blob*>& bottom, const vector<Blob*>& top) override;     // conv_layer.cu:7-23
   void Backward_gpu(const vector<Blob*>& top, const vector<bool>& propagate_down,
                     const vector<Blob*>& bottom) override;                              // conv_layer.cu:25-57
-  void compute_output_shape();                                                          // conv_layer.cpp:7-22
+  virtual void compute_output_shape();                                                  // conv_layer.cpp:7-22
+  // DeconvolutionLayer: the weight blob is [C, num_output/G, k...] (BaseConvolutionLayer::reverse_dimensions)
+  virtual bool reverse_dimensions() const { return false; }
   void* workspace(size_t bytes);
 
   vector<int> kernel_shape_, stride_, pad_, dilation_, output_shape_, bottom_shape_;
@@ -312,6 +316,31 @@ class ConvolutionLayer : public LayerBase {
   bool fcache_on_ = false;
 };
 shared_ptr<LayerBase> GetConvolutionLayer(const LayerParameter& p);   // layer_factory.cpp:53-88
+
+// ---------------------------------------------------------------------------------------------- Deconvolution
+// src/caffe/layers/deconv_layer.{cpp,cu}: ConvolutionLayer's set-up checks and fillers with the weight blob [C, num_output/G, k...]
+// and the output extent s*(in-1) + d*(k-1) + 1 - 2p.  2-D layers run b2c_deconv_* (include/b2c.h); N-D layers and
+// force_nd_im2col the literal per-image GEMM + col2im_nd of the reference.  Several bottom / top pairs share one weight set.
+// It stays out of TrainNet's per-iteration filter cache: EnableFilterCache returns false (its phase route prepares the phase
+// sub-filters inside each forward call, and its dual routes run their own prepass).
+class DeconvolutionLayer : public ConvolutionLayer {
+ public:
+  explicit DeconvolutionLayer(const LayerParameter& p) : ConvolutionLayer(p) {}
+  ~DeconvolutionLayer() override;
+  void Reshape(const vector<Blob*>& bottom, const vector<Blob*>& top) override;
+  const char* type() const override { return "Deconvolution"; }
+  bool EnableFilterCache() override { return false; }
+  bool SupportsBottomDiffAccumulate(int) const override { return false; }
+  const b2c_deconv_desc* deconv_desc() const { return ddesc_; }
+
+ protected:
+  void Forward_gpu(const vector<Blob*>& bottom, const vector<Blob*>& top) override;
+  void Backward_gpu(const vector<Blob*>& top, const vector<bool>& propagate_down, const vector<Blob*>& bottom) override;
+  void compute_output_shape() override;
+  bool reverse_dimensions() const override { return true; }
+  b2c_deconv_desc* ddesc_ = nullptr;
+  b2c_conv_params ddesc_params_{};
+};
 
 // ---------------------------------------------------------------------------------------------- arena
 // One contiguous device space each for parameter data, diffs and solver history; every learnable blob's

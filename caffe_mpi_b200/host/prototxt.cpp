@@ -254,6 +254,8 @@ LayerParameter read_layer(const PMessage& lp, Phase phase, int batch_override) {
   p.eltwise_param.operation = (op == "PROD" || op == "0") ? 0 : (op == "MAX" || op == "2") ? 2 : 1;
   for (auto* f : sub("eltwise_param").all("coeff")) if (!f->is_msg()) p.eltwise_param.coeff.push_back((float)std::atof(f->scalar.c_str()));
   p.concat_param.axis = (int)sub("concat_param").integer("axis", 1);
+  p.crop_param.axis = (int)sub("crop_param").integer("axis", 2);
+  for (long long v : sub("crop_param").ints("offset")) p.crop_param.offset.push_back((int)v);
   const PMessage& sp = sub("slice_param");
   B2_CHECK(!(sp.has("axis") && sp.has("slice_dim")), "Either axis or slice_dim should be specified; not both.");   // slice_layer.cpp:12-13
   p.slice_param.slice_dim_given = sp.has("slice_dim");
@@ -289,6 +291,7 @@ LayerParameter read_layer(const PMessage& lp, Phase phase, int batch_override) {
 
 int LabelBottom(const std::string& type) {
   if (type == "ContrastiveLoss") return 2;          // the similarity label (ContrastiveLossLayer::AllowForceBackward(2) is false)
+  if (type == "Crop") return 1;                     // the reference blob: a shape, never a gradient
   return type == "SoftmaxWithLoss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy" ? 1 : -1;
 }
 bool IsLossType(const std::string& ty) { return ty.size() >= 4 && ty.compare(ty.size() - 4, 4, "Loss") == 0; }
@@ -300,6 +303,32 @@ int pooled_extent(int in, int k, int s, int p) {
   int o = (int)std::ceil((float)(in + 2 * p - k) / s) + 1;
   if (p > 0 && (o - 1) * s >= in + p) --o;
   return o;
+}
+void CropShape(const std::vector<int>& bottom, const std::vector<int>& ref, const CropParameter& q, std::vector<int>* top,
+               std::vector<int>* offsets) {
+  const int nax = (int)bottom.size();
+  auto check_eq = [](long long u, long long v, const std::string& what) {
+    if (u != v) Fatal(__FILE__, __LINE__, "Check failed: " + what + " (" + std::to_string(u) + " vs. " + std::to_string(v) + ") ");
+  };
+  check_eq(nax, (long long)ref.size(), "bottom[0]->num_axes() == bottom[1]->num_axes()");
+  if (q.axis < -nax || q.axis >= nax)                                 // Blob::CanonicalAxisIndex
+    Fatal(__FILE__, __LINE__, "axis " + std::to_string(q.axis) + " out of range for " + std::to_string(nax) + "-D Blob with shape");
+  const int start = q.axis < 0 ? q.axis + nax : q.axis;
+  if (q.offset.size() > 1)
+    check_eq((long long)q.offset.size(), nax - start,
+             "param.offset_size() == num_dims - start_axis number of offset values specified must be equal to the number of dimensions "
+             "following axis.");
+  *top = bottom;
+  offsets->assign(nax, 0);
+  for (int i = start; i < nax; ++i) {
+    const int o = q.offset.empty() ? 0 : q.offset.size() == 1 ? q.offset[0] : q.offset[i - start];
+    (*top)[i] = ref[i];
+    if (!(bottom[i] - o >= ref[i]))
+      Fatal(__FILE__, __LINE__, "Check failed: bottom[0]->shape(i) - crop_offset >= bottom[1]->shape(i) (" + std::to_string(bottom[i] - o) +
+                                    " vs. " + std::to_string(ref[i]) + ") invalid crop parameters in dimension: " + std::to_string(i));
+    B2_CHECK(o >= 0, "Crop: negative offset in dimension " + std::to_string(i));
+    (*offsets)[i] = o;
+  }
 }
 PoolingParameter EffectivePooling(const PoolingParameter& q, int h, int w) {
   PoolingParameter e = q;
@@ -418,6 +447,45 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       blobs.push_back({{p.O, p.C / p.G, p.kh, p.kw}, 0});
       if (c.bias_term) blobs.push_back({{p.O}, 1});
       convs_.push_back(ConvEntry{P.name, id, p, false});   // propagate_down: set once need-backward is final, below
+    } else if (type == "Deconvolution") {
+      // ConvolutionLayer's checks (base_conv_layer.cpp), the output extent of deconv_layer.cpp:7-22, weights [C, O/G, k...]
+      B2_CHECK(lp.sub("convolution_param") != nullptr, "Deconvolution layer without convolution_param");
+      const ConvolutionParameter& c = P.convolution_param;
+      const std::vector<int>& bs = bottom_shape(0);
+      const int caxis = canonical_axis(c.axis, bs), nsp = (int)bs.size() - caxis - 1;
+      B2_CHECK(nsp >= 1, "convolution needs at least one spatial axis");
+      auto ax = [&](const std::vector<int>& rep, int hv, int wv, int dflt, int i, const char* what) {
+        if (hv >= 0 || wv >= 0) {
+          B2_CHECK(nsp == 2, std::string(what) + "_h & " + what + "_w can only be used for 2D convolution.");
+          B2_CHECK(rep.empty(), std::string("Either ") + what + " or " + what + "_h/w should be specified; not both.");
+          return std::max(i == 0 ? hv : wv, 0);       // the unset one of the pair reads as the proto's 0
+        }
+        B2_CHECK(rep.size() <= 1 || (int)rep.size() == nsp, std::string(what) + " must be specified once, or once per spatial dimension");
+        return rep.empty() ? dflt : rep[rep.size() == 1 ? 0 : i];
+      };
+      B2_CHECK(c.num_output > 0 && c.group > 0, "num_output and group must be positive");
+      B2_CHECK(bs[caxis] % c.group == 0 && c.num_output % c.group == 0, "channels / num_output must be multiples of group");
+      std::vector<int> top(bs.begin(), bs.begin() + caxis + 1), wshape{bs[caxis], c.num_output / c.group};
+      top[caxis] = c.num_output;
+      for (int i = 0; i < nsp; ++i) {
+        const int k = ax(c.kernel_size, c.kernel_h, c.kernel_w, 0, i, "kernel_size"), s = ax(c.stride, c.stride_h, c.stride_w, 1, i, "stride");
+        const int pd = ax(c.pad, c.pad_h, c.pad_w, 0, i, "pad"), d = ax(c.dilation, -1, -1, 1, i, "dilation");
+        B2_CHECK(k > 0, "Filter dimensions must be nonzero.");
+        B2_CHECK(s > 0, "Stride dimensions must be nonzero.");
+        B2_CHECK(d > 0 && pd >= 0, "dilation must be positive and pad non-negative");
+        const int o = s * (bs[caxis + 1 + i] - 1) + d * (k - 1) + 1 - 2 * pd;
+        B2_CHECK(o > 0, "Deconvolution: non-positive output extent (pad larger than the upsampled input)");
+        top.push_back(o);
+        wshape.push_back(k);
+      }
+      tops.push_back(top);
+      blobs.push_back({wshape, 0});
+      if (c.bias_term) blobs.push_back({{c.num_output}, 1});
+    } else if (type == "Crop") {
+      std::vector<int> top, offsets;
+      B2_CHECK(P.bottom.size() == 2, "Crop Layer takes 2 bottom blobs: the blob to crop and the one whose shape it takes");
+      CropShape(bottom_shape(0), bottom_shape(1), P.crop_param, &top, &offsets);
+      tops.push_back(top);
     } else if (type == "Pooling") {
       const std::vector<int>& bs = bottom_shape(0);
       B2_CHECK(bs.size() == 4, "Pooling expects a 4-D bottom (num, channels, height, width)");   // pooling_layer.cpp:84-86

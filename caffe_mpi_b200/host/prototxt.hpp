@@ -52,7 +52,8 @@ struct NetLayer {                       // one LayerParameter after phase filter
 };
 
 // The bottom a loss-like layer reads its labels / targets from, which never receives a gradient (-1: none; EuclideanLoss sends
-// gradient to both of its bottoms).  SoftmaxWithLoss, SigmoidCrossEntropyLoss and Accuracy: bottom 1; ContrastiveLoss: bottom 2.
+// gradient to both of its bottoms).  SoftmaxWithLoss, SigmoidCrossEntropyLoss and Accuracy: bottom 1; ContrastiveLoss: bottom 2;
+// Crop: bottom 1, which only supplies the shape (CropLayer::Backward_gpu never writes it).
 int LabelBottom(const std::string& type);
 // A layer type whose name ends in "Loss" (LossLayer's subclasses)
 bool IsLossType(const std::string& type);
@@ -63,6 +64,11 @@ float TopLossWeight(const LayerParameter& p, size_t t);
 int pooled_extent(int in, int k, int s, int p);
 // q over an h x w bottom: global_pooling makes the whole plane one window (stride 1, no padding)
 PoolingParameter EffectivePooling(const PoolingParameter& q, int h, int w);
+// CropLayer::Reshape (crop_layer.cpp): the top takes `ref`'s extents from crop_param.axis on (negative counts from the end), the
+// axes before keep the bottom's; one offset for every cropped axis or one per cropped axis, none = 0.  Fills the top shape and
+// the offset of every axis; fatal with the reference's messages where it CHECK-fails.
+void CropShape(const std::vector<int>& bottom, const std::vector<int>& ref, const CropParameter& q, std::vector<int>* top,
+               std::vector<int>* offsets);
 
 // One parameter blob of a layer.  blob_id counts the layer's learnable blobs; layer_blob is its index among the layer's blobs
 // (BatchNorm's scale / bias are blobs 3 and 4).  Named blobs are shared (Net::AppendParam, net.cpp:576-666): the first blob with

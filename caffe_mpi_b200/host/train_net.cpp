@@ -316,6 +316,20 @@ void SoftmaxLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, 
   softmax_view(t[0], layer_param_.softmax_param.axis, &outer, &C, &inner);
   B2C_CHECK(b2c_softmax_backward(outer, C, inner, t[0]->gpu_data(), t[0]->gpu_diff(), b[0]->mutable_gpu_diff(), S()));
 }
+void CropLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
+  vector<int> top;
+  CropShape(b[0]->shape(), b[1]->shape(), layer_param_.crop_param, &top, &offsets_);
+  t[0]->Reshape(top);
+}
+void CropLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2C_CHECK(b2c_crop_forward(b[0]->num_axes(), b[0]->shape().data(), t[0]->shape().data(), offsets_.data(), b[0]->gpu_data(),
+                             t[0]->mutable_gpu_data(), Caffe::thread_stream()));
+}
+void CropLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0]) return;
+  B2C_CHECK(b2c_crop_backward(b[0]->num_axes(), b[0]->shape().data(), t[0]->shape().data(), offsets_.data(), t[0]->gpu_diff(),
+                              b[0]->mutable_gpu_diff(), Caffe::thread_stream()));
+}
 void SigmoidLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   B2C_CHECK(b2c_sigmoid_forward(b[0]->count(), b[0]->gpu_data(), t[0]->mutable_gpu_data(), S()));
 }
@@ -513,6 +527,8 @@ static shared_ptr<LayerBase> CreateLayer(const LayerParameter& p, const vector<v
   if (t == "Concat") return std::make_shared<ConcatLayer>(p);
   if (t == "Slice") return std::make_shared<SliceLayer>(p, top_shapes);
   if (t == "ContrastiveLoss") return std::make_shared<ContrastiveLossLayer>(p);
+  if (t == "Deconvolution") return LayerRegistry::CreateLayer(p);
+  if (t == "Crop") return std::make_shared<CropLayer>(p);
   B2_CHECK(false, "TrainNet: layer type '" + t + "' is not built yet (SURVEY 8f rank 2 covers the ResNet-50 set)");
   return nullptr;
 }

@@ -241,6 +241,20 @@ class SigmoidCrossEntropyLossLayer : public LayerBase {   // no sigmoid tensor: 
 };
 
 // contrastive_loss_layer.cpp: bottoms a, b [N, C(, 1, 1)] and the similarity label [N]; diff = a - b and dist_sq are kept for backward
+// CropLayer (crop_layer.cpp / .cu): top = bottom[0]'s window of bottom[1]'s extents (CropShape); backward zero-fills bottom[0]'s
+// diff and copies the top diff into the window.  bottom[1] supplies only a shape and never receives a gradient (LabelBottom).
+class CropLayer : public LayerBase {
+ public:
+  using LayerBase::LayerBase;
+  const char* type() const override { return "Crop"; }
+  int MinBottomBlobs() const override { return 2; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  vector<int> offsets_;
+};
+
 class ContrastiveLossLayer : public LayerBase {
  public:
   using LayerBase::LayerBase;

@@ -146,6 +146,64 @@ int b2c_conv_backward_filter_split(const b2c_conv_desc* d, const float* x, const
  * cudnnConvolutionBackwardBias beta=1 (cudnn_conv_layer.cu:73-75).                   */
 int b2c_conv_backward_bias(const b2c_conv_desc* d, const float* dy, float* db, void* stream);
 
+/* ---- transposed convolution (DeconvolutionLayer, src/caffe/layers/deconv_layer.{cpp,cu}) ----------------------------------
+ * The descriptor takes the deconvolution's own parameters and bottom shape: b2c_conv_params with C = bottom channels, H, W = bottom
+ * extent, O = num_output.  Top extent Ht = sh*(H-1) + dh*(kh-1) + 1 - 2*ph (deconv_layer.cpp:7-22; a non-positive extent is
+ * refused), weights [C, O/G, kh, kw], bias [O].  Internally it holds the DUAL convolution (input = the top [N, O, Ht, Wt], output =
+ * the bottom, filter = the same weight blob), so math / algo / engine mean what they mean for b2c_conv_desc.  Same calling rules
+ * as the b2c_conv_* entry points: y and dx overwritten, dw and db accumulated. */
+typedef struct b2c_deconv_desc b2c_deconv_desc;
+int b2c_deconv_desc_create(const b2c_conv_params* p, int engine, b2c_deconv_desc** out);
+int b2c_deconv_desc_destroy(b2c_deconv_desc* d);
+int b2c_deconv_desc_set_math(b2c_deconv_desc* d, int math);
+int b2c_deconv_desc_set_algo(b2c_deconv_desc* d, int algo);
+int b2c_deconv_out_shape(const b2c_deconv_desc* d, int* Ht, int* Wt);
+size_t b2c_deconv_workspace_bytes(const b2c_deconv_desc* d, int op);
+/* y = deconv(x, W) (+ bias): the dual's data gradient. */
+int b2c_deconv_forward(const b2c_deconv_desc* d, const float* x, const float* w, const float* bias, float* y, void* ws,
+                       size_t ws_bytes, void* stream);
+/* dx = the dual's forward of dy (no bias). */
+int b2c_deconv_backward_data(const b2c_deconv_desc* d, const float* dy, const float* w, float* dx, void* ws, size_t ws_bytes,
+                             void* stream);
+/* dW += the dual's weight gradient with X = dy (top diff) and dY = x (bottom data); the _split form as
+ * b2c_conv_backward_filter_split, with a buffer of b2c_deconv_wgrad_split_bytes(d) bytes. */
+int b2c_deconv_backward_filter(const b2c_deconv_desc* d, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes,
+                               void* stream);
+size_t b2c_deconv_wgrad_split_bytes(const b2c_deconv_desc* d);
+int b2c_deconv_backward_filter_split(const b2c_deconv_desc* d, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes,
+                                     void* split, size_t split_bytes, void* stream);
+/* db[o] += sum_{n,h,w} dy[n][o][h][w] (b2c_bias_backward over the top diff). */
+int b2c_deconv_backward_bias(const b2c_deconv_desc* d, const float* dy, float* db, void* stream);
+typedef enum {
+  B2C_DECONV_ROUTE_DUAL = 0,       /* the dual convolution's routes: forward = b2c_conv_backward_data (+ one bias pass), backward    */
+                                   /* data = b2c_conv_forward, weight gradient = b2c_conv_backward_filter[_split]                    */
+  B2C_DECONV_ROUTE_PHASE = 1,      /* forward of a strided layer with k > 1 (not engine CAFFE): sh*sw stride-1 gather-kernel launches */
+                                   /* on the bottom, one per output phase, each writing its lattice of the top with the bias fused   */
+  B2C_DECONV_ROUTE_DEPTHWISE = 2   /* group == C == num_output, every op, except under engine CAFFE (always the DUAL route): direct  */
+                                   /* fp32 kernels.  Forward and data gradient: per                                                  */
+                                   /* output, taps i ascending then j ascending (on-grid, in-bounds taps only), each product rounded  */
+                                   /* to fp32 then added (no FMA) from +0, bias added last.  Weight gradient per (c, i, j): 256       */
+                                   /* lane-strided chains over the flattened (n, h, w), an xor butterfly per warp, the 8 warp         */
+                                   /* partials in order, one add onto dW -- the same bits on every call                               */
+} b2c_deconv_route;
+/* The route of op (b2c_conv_op) for this descriptor: out[0] route (b2c_deconv_route), [1] for the DUAL route the dual's own route
+ * (b2c_conv_route of its b2c_debug_conv_plan, or b2c_wgrad_route for the weight gradient), else -1; [2] phases (sh*sw on the PHASE
+ * route, else 0); then per phase k (phase (t0h, t0w) = (k / sw, k % sw): outputs t0h + sh*m, t0w + sw*m'), [3 + 2k] its taps
+ * (0: only the bias is written) and [4 + 2k] its gather-kernel tiles.  Needs n >= 3, and n >= 3 + 2*phases on the PHASE route.
+ * Pure host computation. */
+int b2c_debug_deconv_plan(const b2c_deconv_desc* d, int op, int* out, int n);
+
+/* ---- Crop (CropLayer, src/caffe/layers/crop_layer.{cpp,cu}) ------------------------------------------------------------------
+ * N-D (1..32 axes) window copy; shapes and per-axis offsets are HOST int arrays over every axis (0 offset on the uncropped ones).
+ * Forward: top = bottom[offsets : offsets + top_shape].  Backward: bottom_diff zero-filled, then the top diff copied into the
+ * window.  16-byte units when the innermost top extent, offset and bottom extent are multiples of 4 and both pointers 16-byte
+ * aligned, else one float at a time (the same values).  Refuses (B2C_ERR_INVALID) num_axes outside [1, 32], negative extents or
+ * offsets, and a window that leaves the bottom ("invalid crop parameters in dimension: i", crop_layer.cpp). */
+int b2c_crop_forward(int num_axes, const int* bottom_shape, const int* top_shape, const int* offsets, const float* bottom, float* top,
+                     void* stream);
+int b2c_crop_backward(int num_axes, const int* bottom_shape, const int* top_shape, const int* offsets, const float* top_diff,
+                      float* bottom_diff, void* stream);
+
 /* ---- im2col / col2im ----------------------------------------------------------------
  * One image [C,H,W] <-> [C*kh*kw, Ho, Wo].  Replace im2col_gpu / col2im_gpu
  * (src/caffe/util/im2col.cu:42-62, 298-317).  col2im OVERWRITES im and adds the
