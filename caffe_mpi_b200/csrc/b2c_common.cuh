@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <atomic>
 #include <string>
+#include <utility>
 
 #include "../../include/b2c.h"
 
@@ -34,6 +35,34 @@ extern std::atomic<uint64_t> g_launches;
   } while (0)
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// ---- programmatic dependent launch (DESIGN §3b) ----------------------------------------------------------------
+// Every kernel of a training step is launched by launch_pdl, so its launch overlaps the end of the kernel before it on the
+// stream instead of following that kernel's completion.  Such a kernel touches no global memory before pdl_wait(), which
+// returns once every prerequisite grid has completed and its writes are visible; it is a no-op in a kernel launched without
+// the attribute.  No kernel issues griddepcontrol.launch_dependents: each grid lets the next one launch as its CTAs exit, which
+// measured faster than triggering early (DESIGN §3b), and it keeps the chain transitive.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// kernel<<<grid, block, smem, st>>>(args...) with programmatic stream serialization; cluster > 0: in thread-block clusters of
+// `cluster` CTAs along x.  The caller follows it with B2C_POST_LAUNCH(), which counts the launch and reports a launch error.
+template <typename... KArgs, typename... Args>
+inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, unsigned cluster,
+                       Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = cluster; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = cluster ? 2 : 1;
+  cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
 
 // The reference sizes grids as ceil(n/512) with 512-thread blocks
 // (include/caffe/util/device_alternate.hpp:91-96).  Here element-wise grids are capped at a

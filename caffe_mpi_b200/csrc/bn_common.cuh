@@ -233,17 +233,8 @@ static inline unsigned bn_threads(int N, int S, bool forward) {
 }
 template <typename... Args>
 static inline void bn_launch_clustered(void (*kernel)(Args...), unsigned cs, int C, size_t smem_pad, void* stream, unsigned threads, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(cs, C, 1);
-  cfg.blockDim = dim3(threads, 1, 1);
-  cfg.dynamicSmemBytes = smem_pad;
-  cfg.stream = as_stream(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
   if (cs > 8) cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-  cudaLaunchKernelEx(&cfg, kernel, args...);
+  launch_pdl(kernel, dim3(cs, C, 1), dim3(threads, 1, 1), smem_pad, as_stream(stream), cs, args...);
 }
 
 }  // namespace b2c

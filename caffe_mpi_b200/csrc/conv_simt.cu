@@ -107,6 +107,7 @@ conv_wgrad_simt_kernel(ConvShape s, const float* __restrict__ x, const float* __
 // y[n][o][p] += bias[o]
 __global__ void __launch_bounds__(256)
 bias_add_kernel(size_t total, int O, int P, const float* __restrict__ bias, float* __restrict__ y) {
+  pdl_wait();
   for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (size_t)gridDim.x * blockDim.x)
     y[idx] += __ldg(bias + (int)((idx / P) % O));
@@ -116,6 +117,7 @@ bias_add_kernel(size_t total, int O, int P, const float* __restrict__ bias, floa
 // then every row is), warp-shuffle tree then a cross-warp smem stage.
 __global__ void __launch_bounds__(256)
 bias_grad_kernel(int N, int O, int P, const float* __restrict__ dy, float* __restrict__ db) {
+  pdl_wait();
   __shared__ float red[8];
   const int o = blockIdx.x;
   float acc = 0.0f;
@@ -164,12 +166,12 @@ int launch_conv_wgrad_simt(const ConvShape& s, const float* x, const float* dy, 
 }
 int launch_bias_add(int N, int O, int P, const float* bias, float* y, cudaStream_t st) {
   const size_t total = (size_t)N * O * P;
-  bias_add_kernel<<<grid_for(total, 256), 256, 0, st>>>(total, O, P, bias, y);
+  launch_pdl(bias_add_kernel, grid_for(total, 256), 256, 0, st, 0, total, O, P, bias, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 int launch_bias_grad(int N, int O, int P, const float* dy, float* db, cudaStream_t st) {
-  bias_grad_kernel<<<O, 256, 0, st>>>(N, O, P, dy, db);
+  launch_pdl(bias_grad_kernel, O, 256, 0, st, 0, N, O, P, dy, db);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

@@ -130,6 +130,7 @@ igemm_fwd_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ CU
     }
   }
   __syncthreads();
+  pdl_wait();      // everything above is shared-memory and barrier set-up
 
   auto stage_b_hi = [&](int s) { return sbase + s * S::STAGE; };
   auto stage_b_lo = [&](int s) { return sbase + s * S::STAGE + S::B_BYTES; };
@@ -370,7 +371,7 @@ static int launch_fwd_inst(const FwdParams& p, const CUtensorMap& mh, const CUte
   B2C_CUDA_OK(cudaFuncSetAttribute(igemm_fwd_kernel<N_TILE, SPLIT, KMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)S::TOTAL));
   const int grid = persistent_grid(p.total_tiles);
-  igemm_fwd_kernel<N_TILE, SPLIT, KMODE><<<grid, FW_THREADS, S::TOTAL, st>>>(p, mh, ml);
+  launch_pdl(igemm_fwd_kernel<N_TILE, SPLIT, KMODE>, grid, FW_THREADS, S::TOTAL, st, 0, p, mh, ml);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

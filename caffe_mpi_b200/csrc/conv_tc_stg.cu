@@ -157,6 +157,7 @@ igemm_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
     tapoff[tid] = ((i - p.ph) * p.W + (j - p.pw)) * 4;          // byte offset inside a staged channel row
   }
   __syncthreads();
+  pdl_wait();      // everything above is shared-memory and barrier set-up
 
   auto stage_b_hi = [&](int s) { return sbase + (uint32_t)s * 2u * S::B_BYTES; };
   auto stage_b_lo = [&](int s) { return sbase + (uint32_t)s * 2u * S::B_BYTES + S::B_BYTES; };
@@ -546,7 +547,7 @@ static int stg_launch_inst(const stg::Params& p, const CUtensorMap& mh, const CU
   using S = stg::Smem<N_TILE, BWT>;
   B2C_CUDA_OK(cudaFuncSetAttribute(stg::igemm_stg_kernel<N_TILE, BWT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
   const int grid = persistent_grid(p.total_tiles);
-  stg::igemm_stg_kernel<N_TILE, BWT><<<grid, stg::THREADS, S::TOTAL, st>>>(p, mh, ml, mx, my);
+  launch_pdl(stg::igemm_stg_kernel<N_TILE, BWT>, grid, stg::THREADS, S::TOTAL, st, 0, p, mh, ml, mx, my);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

@@ -91,6 +91,7 @@ igemm_wgrad_kernel(const __grid_constant__ WgradParams p) {
     rowtab[r] = e;
   }
   __syncthreads();
+  pdl_wait();      // everything above is shared-memory and barrier set-up
 
   constexpr uint32_t LBO_A = tile_lbo(128), LBO_B = tile_lbo(N_TILE);
   auto stage_a_hi = [&](int s) { return sbase + s * S::STAGE; };
@@ -416,6 +417,7 @@ wgrad1x1_tma_kernel(const __grid_constant__ WgradTmaParams p, const __grid_const
     fence_barrier_init();
   }
   __syncthreads();
+  pdl_wait();      // everything above is shared-memory and barrier set-up
 
   auto stage_a = [&](int s) { return sbase + (uint32_t)s * S::STAGE; };            // raw dY tile (hi operand)
   auto stage_b = [&](int s) { return sbase + (uint32_t)s * S::STAGE + S::A_BYTES; };  // raw X tile
@@ -559,7 +561,7 @@ static int launch_wgrad_tma_inst(const WgradTmaParams& p, const CUtensorMap& mdy
   // per-device attribute: set on every launch (a process may drive several GPUs)
   B2C_CUDA_OK(cudaFuncSetAttribute(wgrad1x1_tma_kernel<N_TILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
   dim3 grid(p.splits, (p.C + N_TILE - 1) / N_TILE, (p.O + 127) / 128);
-  wgrad1x1_tma_kernel<N_TILE><<<grid, WT_THREADS, S::TOTAL, st>>>(p, mdy, mx);
+  launch_pdl(wgrad1x1_tma_kernel<N_TILE>, grid, WT_THREADS, S::TOTAL, st, 0, p, mdy, mx);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -616,6 +618,7 @@ static ConvShape wgrad_compact_dense_shape(const ConvShape& s) {
 }
 __global__ void __launch_bounds__(256)
 subsample_kernel(const float* __restrict__ x, float* __restrict__ y, long long planes, int H, int W, int Ho, int Wo, int sh, int sw) {
+  pdl_wait();
   const long long total = planes * Ho * Wo;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int wo = (int)(i % Wo);
@@ -633,7 +636,7 @@ static int launch_wgrad_inst(const WgradParams& p, int G, cudaStream_t st) {
   B2C_CUDA_OK(cudaFuncSetAttribute(igemm_wgrad_kernel<N_TILE, SPLIT, X1X1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)S::TOTAL));
   dim3 grid(p.splits, (p.Kd + N_TILE - 1) / N_TILE, G * ((p.Og + 127) / 128));
-  igemm_wgrad_kernel<N_TILE, SPLIT, X1X1><<<grid, WG_THREADS, S::TOTAL, st>>>(p);
+  launch_pdl(igemm_wgrad_kernel<N_TILE, SPLIT, X1X1>, grid, WG_THREADS, S::TOTAL, st, 0, p);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -685,7 +688,7 @@ int launch_conv_tc_wgrad(const ConvShape& s, int math, const float* x, const flo
     if (ws_bytes < xoff + xbytes) return fail(B2C_ERR_WORKSPACE, "wgrad (compact): workspace too small");
     float* xc = reinterpret_cast<float*>(static_cast<char*>(ws) + xoff);       // 16-byte aligned: ws is, xoff is a multiple of 256
     const long long planes = (long long)s.N * s.C;
-    subsample_kernel<<<grid_for((size_t)(planes * s.Ho * s.Wo), 256), 256, 0, st>>>(x, xc, planes, s.H, s.W, s.Ho, s.Wo, s.sh, s.sw);
+    launch_pdl(subsample_kernel, grid_for((size_t)(planes * s.Ho * s.Wo), 256), 256, 0, st, 0, x, xc, planes, s.H, s.W, s.Ho, s.Wo, s.sh, s.sw);
     B2C_POST_LAUNCH();
     if (staged) return launch_conv_tc_wgrad_stg(d, xc, dy, dw, ws, part, st);
     return launch_conv_tc_wgrad_tma(d, xc, dy, dw, ws, part, st);

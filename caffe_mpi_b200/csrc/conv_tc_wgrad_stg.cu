@@ -141,6 +141,7 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
     fence_barrier_init();
   }
   __syncthreads();
+  pdl_wait();      // everything above is shared-memory and barrier set-up
 
   auto b_hi = [&](int s) { return sbase + S::B_OFF + (uint32_t)s * S::B_STAGE; };
   auto b_lo = [&](int s) { return sbase + S::B_OFF + (uint32_t)s * S::B_STAGE + S::B_PLANE; };
@@ -400,6 +401,7 @@ wgrad_stg_kernel(const __grid_constant__ Params p, const __grid_constant__ CUten
 // hold the same bits either way.  One thread per 8 output pixels (one 16-byte store per plane).
 __global__ void __launch_bounds__(256)
 wstg_split_kernel(const float* __restrict__ src, uint4* __restrict__ dst, long long rows, int HW, int HWp) {
+  pdl_wait();
   const int per_row = HWp / 8;
   const long long total = rows * per_row;
   const long long plane = total;                            // 16-byte units per plane
@@ -490,7 +492,7 @@ static int wstg_launch(const wstg::Params& p, const CUtensorMap& mdy, const CUte
   using S = wstg::Cfg<T, CN, A_PRE>;
   B2C_CUDA_OK(cudaFuncSetAttribute(wstg::wgrad_stg_kernel<T, CN, PLANE, A_PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
   dim3 grid(p.splits, c_tiles, o_tiles);
-  wstg::wgrad_stg_kernel<T, CN, PLANE, A_PRE><<<grid, wstg::THREADS, S::TOTAL, st>>>(p, mdy, mx);
+  launch_pdl(wstg::wgrad_stg_kernel<T, CN, PLANE, A_PRE>, grid, wstg::THREADS, S::TOTAL, st, 0, p, mdy, mx);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -569,7 +571,7 @@ int launch_sgemm_tc(const GemmPlan& g, int M, int N, int K, const float* A, cons
 }
 
 static int launch_wstg_split(const float* src, void* dst, long long rows, int HW, int HWp, cudaStream_t st) {
-  wstg::wstg_split_kernel<<<grid_for((size_t)rows * (HWp / 8), 256), 256, 0, st>>>(src, static_cast<uint4*>(dst), rows, HW, HWp);
+  launch_pdl(wstg::wstg_split_kernel, grid_for((size_t)rows * (HWp / 8), 256), 256, 0, st, 0, src, static_cast<uint4*>(dst), rows, HW, HWp);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

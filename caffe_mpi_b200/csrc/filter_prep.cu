@@ -9,6 +9,7 @@ using namespace tc;
 
 __global__ void __launch_bounds__(256)
 filter_prep_multi_kernel(const __grid_constant__ PrepBatch b) {
+  pdl_wait();
   const PrepEntry& q = b.e[blockIdx.y];
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < q.total; idx += (long long)gridDim.x * blockDim.x) {
     const int kp = (int)(idx % q.Kp);
@@ -63,7 +64,7 @@ int launch_filter_prep(const PrepEntry* entries, int n, cudaStream_t st) {
     for (int i = 0; i < m; ++i) { b.e[i] = entries[i0 + i]; if (b.e[i].total > biggest) biggest = b.e[i].total; }
     for (int i = m; i < PREP_BATCH; ++i) { b.e[i] = PrepEntry{}; }
     dim3 grid((unsigned)grid_for((size_t)biggest, 256, 4), (unsigned)m);
-    filter_prep_multi_kernel<<<grid, 256, 0, st>>>(b);
+    launch_pdl(filter_prep_multi_kernel, grid, 256, 0, st, 0, b);
     B2C_POST_LAUNCH();
   }
   return B2C_OK;

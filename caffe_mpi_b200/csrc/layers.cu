@@ -27,6 +27,7 @@ namespace b2c {
 
 // ---- ReLU ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) relu_fwd_kernel(size_t n, int vec, const float* __restrict__ x, float* __restrict__ y, float slope) {
+  pdl_wait();
   const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const float4* x4 = reinterpret_cast<const float4*>(x);
   float4* y4 = reinterpret_cast<float4*>(y);
@@ -39,6 +40,7 @@ __global__ void __launch_bounds__(256) relu_fwd_kernel(size_t n, int vec, const 
 }
 __global__ void __launch_bounds__(256) relu_bwd_kernel(size_t n, int vec, const float* __restrict__ dy, const float* __restrict__ x,
                                                        float* __restrict__ dx, float slope) {
+  pdl_wait();
   const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const float4* d4 = reinterpret_cast<const float4*>(dy);
   const float4* x4 = reinterpret_cast<const float4*>(x);
@@ -64,6 +66,7 @@ template <bool VEC>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_stats_kernel(int N, int C, int S, const float* __restrict__ x, float eps, float maf, int first,
                 float* __restrict__ mean, float* __restrict__ invstd, float* __restrict__ run_mean, float* __restrict__ run_var) {
+  pdl_wait();
   __shared__ float2 part[2];
   cg::cluster_group cluster = cg::this_cluster();
   const int c = blockIdx.y;
@@ -82,6 +85,7 @@ template <bool VEC>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_bwd_reduce_kernel(int N, int C, int S, const float* __restrict__ dy, const float* __restrict__ xnorm,
                      float* __restrict__ sum_dy_xn, float* __restrict__ sum_dy) {
+  pdl_wait();
   __shared__ float2 part;
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank();
@@ -111,6 +115,7 @@ template <bool VEC>
 __global__ void __launch_bounds__(256)
 bn_norm_kernel(size_t total_units, int C, int S, const float* __restrict__ x, const float* __restrict__ mean, const float* __restrict__ invstd,
                const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ xnorm, float* __restrict__ y) {
+  pdl_wait();
   const unsigned units = VEC ? S / 4 : S;
   size_t i = (size_t)blockIdx.x * (256 * BN_EW_PER_THREAD) + threadIdx.x;
   if (i >= total_units) return;
@@ -141,6 +146,7 @@ __global__ void __launch_bounds__(256)
 bn_bwd_dx_kernel(size_t total_units, int C, int S, float inv_cnt, const float* __restrict__ dy, const float* __restrict__ xnorm,
                  const float* __restrict__ gamma, const float* __restrict__ invstd, const float* __restrict__ sum_dy_xn,
                  const float* __restrict__ sum_dy, float* __restrict__ dx) {
+  pdl_wait();
   const unsigned units = VEC ? S / 4 : S;
   size_t i = (size_t)blockIdx.x * (256 * BN_EW_PER_THREAD) + threadIdx.x;
   if (i >= total_units) return;
@@ -172,6 +178,7 @@ __device__ __forceinline__ float lrn_pow_neg(float s, float beta) {
 __global__ void __launch_bounds__(256)
 lrn_fwd_kernel(int N, int C, int S, int size, float alpha_over_size, float beta, float k, const float* __restrict__ x,
                float* __restrict__ scale, float* __restrict__ y) {
+  pdl_wait();
   const long long total = (long long)N * S;
   const int pre = (size - 1) / 2;                              // lrn_layer.cpp: pre_pad_
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -194,6 +201,7 @@ lrn_fwd_kernel(int N, int C, int S, int size, float alpha_over_size, float beta,
 __global__ void __launch_bounds__(256)
 lrn_bwd_kernel(int N, int C, int S, int size, float cache_ratio, float beta, const float* __restrict__ x, const float* __restrict__ y,
                const float* __restrict__ scale, const float* __restrict__ dy, float* __restrict__ dx) {
+  pdl_wait();
   const long long total = (long long)N * S;
   const int ipp = size - (size + 1) / 2;                       // lrn_layer.cpp: inverse_pre_pad
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -220,12 +228,14 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long z) {
 }
 __global__ void __launch_bounds__(256)
 dropout_mask_kernel(size_t n, unsigned threshold24, float scale, unsigned long long seed, unsigned long long offset, float* __restrict__ mask) {
+  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const unsigned u = (unsigned)(splitmix64(seed + offset + i) >> 40);      // 24 uniform bits
     mask[i] = u >= threshold24 ? scale : 0.f;
   }
 }
 __global__ void __launch_bounds__(256) mul_kernel(size_t n, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y) {
+  pdl_wait();
   const size_t n4 = n / 4, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   for (size_t i = tid; i < n4; i += step) {
     const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
@@ -238,6 +248,7 @@ __global__ void __launch_bounds__(256) mul_kernel(size_t n, const float* __restr
 __global__ void __launch_bounds__(256)
 pool_max_fwd_kernel(size_t total, int H, int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw,
                     const float* __restrict__ x, float* __restrict__ y, int* __restrict__ mask) {
+  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int wo = (int)(i % Wo), ho = (int)((i / Wo) % Ho);
     const size_t nc = i / ((size_t)Wo * Ho);
@@ -263,6 +274,7 @@ template <int KH, int KW, int SH, int SW, int Q>
 __global__ void __launch_bounds__(256)
 pool_max_fwd_q_kernel(long long groups, int H, int W, int Ho, int Wo, int ph, int pw, const float* __restrict__ x,
                       float* __restrict__ y, int* __restrict__ mask) {
+  pdl_wait();
   constexpr int NCOL = (Q - 1) * SW + KW;
   const int Wq = Wo / Q;
   for (long long gidx = (long long)blockIdx.x * blockDim.x + threadIdx.x; gidx < groups; gidx += (long long)gridDim.x * blockDim.x) {
@@ -309,6 +321,7 @@ pool_max_fwd_q_kernel(long long groups, int H, int W, int Ho, int Wo, int ph, in
 __global__ void __launch_bounds__(128)
 pool_max_bwd_kernel(int rows, int H, int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw,
                     const float* __restrict__ dy, const int* __restrict__ mask, float* __restrict__ dx) {
+  pdl_wait();
   const int rpb = W >= 128 ? 1 : 128 / W;                    // input rows per block (narrow maps: several rows share the 128 threads)
   const int tr = rpb == 1 ? 0 : (int)threadIdx.x / W;        // this thread's row inside the block's group, first column
   const int tw = rpb == 1 ? (int)threadIdx.x : (int)threadIdx.x - tr * W;
@@ -340,6 +353,7 @@ template <int KH, int KW, int SH, int SW>
 __global__ void __launch_bounds__(256)
 pool_max_bwd_q4_kernel(long long quads, int H, int W, int Ho, int Wo, int ph, int pw, const float* __restrict__ dy,
                        const int* __restrict__ mask, float* __restrict__ dx) {
+  pdl_wait();
   constexpr int MA = (KH + SH - 1) / SH;                        // pooled rows an input row can sit in
   constexpr int NB = (3 + KW - 1) / SW + 1;                    // pooled columns four consecutive input columns can sit in
   const int Wq = W / 4;
@@ -385,6 +399,7 @@ pool_max_bwd_q4_kernel(long long quads, int H, int W, int Ho, int Wo, int ph, in
 __global__ void __launch_bounds__(256)
 pool_ave_fwd_kernel(size_t total, int H, int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw,
                     const float* __restrict__ x, float* __restrict__ y) {
+  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int wo = (int)(i % Wo), ho = (int)((i / Wo) % Ho);
     const size_t nc = i / ((size_t)Wo * Ho);
@@ -402,6 +417,7 @@ pool_ave_fwd_kernel(size_t total, int H, int W, int Ho, int Wo, int kh, int kw, 
 __global__ void __launch_bounds__(256)
 pool_ave_bwd_kernel(size_t total, int H, int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw,
                     const float* __restrict__ dy, float* __restrict__ dx) {
+  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int w = (int)(i % W) + pw, h = (int)((i / W) % H) + ph;
     const size_t nc = i / ((size_t)W * H);
@@ -421,6 +437,7 @@ pool_ave_bwd_kernel(size_t total, int H, int W, int Ho, int Wo, int kh, int kw, 
 
 // ---- elementwise ----------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) add_kernel(size_t n, int vec, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y) {
+  pdl_wait();
   const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   for (size_t i = tid; i < n4; i += step) {
     const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
@@ -435,6 +452,7 @@ __global__ void __launch_bounds__(256) add_kernel(size_t n, int vec, const float
 // layer runs this kernel in place (prob == logits); every element is read by the thread that later writes it, before that write.
 __global__ void __launch_bounds__(256)
 softmax_loss_fwd_kernel(int C, const float* logits, float* prob) {
+  pdl_wait();
   const int n = blockIdx.x;
   const float* z = logits + (size_t)n * C;
   float mx = -FLT_MAX, dummy = 0.f;
@@ -455,6 +473,7 @@ softmax_loss_fwd_kernel(int C, const float* logits, float* prob) {
 // loss = scale * sum_n -log(max(prob[n][label[n]], FLT_MIN))   (softmax_loss_layer.cpp:100-116); one block, fixed summation order
 __global__ void __launch_bounds__(256)
 softmax_loss_sum_kernel(int N, int C, const float* __restrict__ prob, const float* __restrict__ labels, float scale, float* __restrict__ loss) {
+  pdl_wait();
   float s = 0.f, dummy = 0.f;
   for (int n = threadIdx.x; n < N; n += blockDim.x) {
     // the reference DCHECKs 0 <= label < C (:108-109); an out-of-range label must not read out of bounds
@@ -467,6 +486,7 @@ softmax_loss_sum_kernel(int N, int C, const float* __restrict__ prob, const floa
 __global__ void __launch_bounds__(256)
 softmax_loss_bwd_kernel(size_t total, int C, const float* __restrict__ prob, const float* __restrict__ labels, float scale,
                         float* __restrict__ dx) {
+  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const size_t n = i / C;
     const int c = (int)(i - n * C);
@@ -481,6 +501,7 @@ softmax_loss_bwd_kernel(size_t total, int C, const float* __restrict__ prob, con
 // takes max, then expf(z - max) and the sum, then the scale, in the row kernel's expressions.  No __restrict__: y may be x.
 template <bool VEC>
 __global__ void __launch_bounds__(256) softmax_col_fwd_kernel(size_t cols, int C, int inner, const float* x, float* y) {
+  pdl_wait();
   using V = typename std::conditional<VEC, float4, float>::type;
   const int w = VEC ? inner / 4 : inner;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cols; i += (size_t)gridDim.x * blockDim.x) {
@@ -509,6 +530,7 @@ __global__ void __launch_bounds__(256) softmax_col_fwd_kernel(size_t cols, int C
 }
 // dx = (dy - sum_c dy * y) * y  (softmax_layer.cu: channel dot, channel subtract, multiply by the top).  dx may be dy.
 __global__ void __launch_bounds__(256) softmax_row_bwd_kernel(int C, const float* y, const float* dy, float* dx) {
+  pdl_wait();
   const size_t off = (size_t)blockIdx.x * C;
   float dot = 0.f, dummy = 0.f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) dot += dy[off + c] * y[off + c];
@@ -517,6 +539,7 @@ __global__ void __launch_bounds__(256) softmax_row_bwd_kernel(int C, const float
 }
 template <bool VEC>
 __global__ void __launch_bounds__(256) softmax_col_bwd_kernel(size_t cols, int C, int inner, const float* y, const float* dy, float* dx) {
+  pdl_wait();
   using V = typename std::conditional<VEC, float4, float>::type;
   const int w = VEC ? inner / 4 : inner;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cols; i += (size_t)gridDim.x * blockDim.x) {
@@ -558,6 +581,7 @@ __device__ __forceinline__ float ew_apply(float a, float b, float s) {
 }
 template <int OP>
 __global__ void __launch_bounds__(256) ew_kernel(size_t n, int vec, const float* a, const float* b, float s, float* y) {
+  pdl_wait();
   const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const bool two = OP == EW_SIGMOID_BWD || OP == EW_SIGCE_BWD;
   for (size_t i = tid; i < n4; i += step) {
@@ -617,6 +641,7 @@ __device__ __forceinline__ double loss_cluster_sum(double acc) {
 template <int MODE, bool VEC>
 __global__ void __launch_bounds__(LOSS_THREADS)
 loss_sum_kernel(size_t count, int N, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ diff, float* __restrict__ loss) {
+  pdl_wait();
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
   const size_t units = VEC ? count / 4 : count, len = (units + nranks - 1) / nranks;
@@ -657,6 +682,7 @@ template <bool LEGACY>
 __global__ void __launch_bounds__(LOSS_THREADS)
 contrastive_loss_kernel(int N, int C, const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ y, float margin,
                         float* __restrict__ diff, float* __restrict__ dist_sq, float* __restrict__ loss) {
+  pdl_wait();
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
   const int len = (int)((N + nranks - 1) / nranks);
@@ -698,6 +724,7 @@ template <bool VEC>
 __global__ void __launch_bounds__(256)
 contrastive_bwd_kernel(int N, int C, const float* __restrict__ diff, const float* __restrict__ dist_sq, const float* __restrict__ y, float margin,
                        int legacy, float alpha, float* __restrict__ da, float* __restrict__ db) {
+  pdl_wait();
   const size_t units = VEC ? (size_t)N * C / 4 : (size_t)N * C, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x,
                step = (size_t)gridDim.x * blockDim.x;
   for (size_t i = tid; i < units; i += step) {
@@ -732,7 +759,7 @@ extern "C" int b2c_relu_forward(size_t n, const float* x, float* y, float negati
   NEED(x && y, "b2c_relu_forward: null");
   if (!n) return B2C_OK;
   const bool al = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;     // else one float at a time
-  relu_fwd_kernel<<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, x, y, negative_slope);
+  launch_pdl(relu_fwd_kernel, grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream), 0, n, al ? 1 : 0, x, y, negative_slope);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -740,7 +767,7 @@ extern "C" int b2c_relu_backward(size_t n, const float* dy, const float* x, floa
   NEED(dy && x && dx, "b2c_relu_backward: null");
   if (!n) return B2C_OK;
   const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
-  relu_bwd_kernel<<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, dy, x, dx, negative_slope);
+  launch_pdl(relu_bwd_kernel, grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream), 0, n, al ? 1 : 0, dy, x, dx, negative_slope);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -767,8 +794,8 @@ extern "C" int b2c_bn_forward_train(int N, int C, int S, const float* x, const f
   if (int rc = launch_bn_stats(pl, N, C, S, x, eps, moving_average_fraction, first_iteration, save_mean, save_invstd, running_mean, running_var, stream)) return rc;
   const size_t units = (size_t)N * C * (vec ? S / 4 : S);
   const unsigned blocks = (unsigned)((units + 256 * BN_EW_PER_THREAD - 1) / (256 * BN_EW_PER_THREAD));
-  if (vec) bn_norm_kernel<true><<<blocks, 256, 0, as_stream(stream)>>>(units, C, S, x, save_mean, save_invstd, gamma, beta, xnorm, y);
-  else bn_norm_kernel<false><<<blocks, 256, 0, as_stream(stream)>>>(units, C, S, x, save_mean, save_invstd, gamma, beta, xnorm, y);
+  if (vec) launch_pdl(bn_norm_kernel<true>, blocks, 256, 0, as_stream(stream), 0, units, C, S, x, save_mean, save_invstd, gamma, beta, xnorm, y);
+  else launch_pdl(bn_norm_kernel<false>, blocks, 256, 0, as_stream(stream), 0, units, C, S, x, save_mean, save_invstd, gamma, beta, xnorm, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -783,22 +810,22 @@ extern "C" int b2c_bn_backward(int N, int C, int S, const float* dy, const float
   const size_t units = (size_t)N * C * (vec ? S / 4 : S);
   const unsigned blocks = (unsigned)((units + 256 * BN_EW_PER_THREAD - 1) / (256 * BN_EW_PER_THREAD));
   const float inv_cnt = 1.0f / ((float)N * S);
-  if (vec) bn_bwd_dx_kernel<true><<<blocks, 256, 0, as_stream(stream)>>>(units, C, S, inv_cnt, dy, xnorm, gamma, save_invstd, dgamma, dbeta, dx);
-  else bn_bwd_dx_kernel<false><<<blocks, 256, 0, as_stream(stream)>>>(units, C, S, inv_cnt, dy, xnorm, gamma, save_invstd, dgamma, dbeta, dx);
+  if (vec) launch_pdl(bn_bwd_dx_kernel<true>, blocks, 256, 0, as_stream(stream), 0, units, C, S, inv_cnt, dy, xnorm, gamma, save_invstd, dgamma, dbeta, dx);
+  else launch_pdl(bn_bwd_dx_kernel<false>, blocks, 256, 0, as_stream(stream), 0, units, C, S, inv_cnt, dy, xnorm, gamma, save_invstd, dgamma, dbeta, dx);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 extern "C" int b2c_lrn_forward(int N, int C, int S, int local_size, float alpha, float beta, float k, const float* x, float* scale,
                                float* y, void* stream) {
   NEED(x && scale && y && N > 0 && C > 0 && S > 0 && local_size > 0 && (local_size & 1), "b2c_lrn_forward: bad argument (LRN only supports odd values for local_size)");
-  lrn_fwd_kernel<<<grid_for((size_t)N * S, 256), 256, 0, as_stream(stream)>>>(N, C, S, local_size, alpha / local_size, beta, k, x, scale, y);
+  launch_pdl(lrn_fwd_kernel, grid_for((size_t)N * S, 256), 256, 0, as_stream(stream), 0, N, C, S, local_size, alpha / local_size, beta, k, x, scale, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 extern "C" int b2c_lrn_backward(int N, int C, int S, int local_size, float alpha, float beta, const float* x, const float* y,
                                 const float* scale, const float* dy, float* dx, void* stream) {
   NEED(x && y && scale && dy && dx && N > 0 && C > 0 && S > 0 && local_size > 0, "b2c_lrn_backward: bad argument");
-  lrn_bwd_kernel<<<grid_for((size_t)N * S, 256), 256, 0, as_stream(stream)>>>(N, C, S, local_size, 2.f * alpha * beta / local_size, beta, x, y, scale, dy, dx);
+  launch_pdl(lrn_bwd_kernel, grid_for((size_t)N * S, 256), 256, 0, as_stream(stream), 0, N, C, S, local_size, 2.f * alpha * beta / local_size, beta, x, y, scale, dy, dx);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -806,7 +833,7 @@ extern "C" int b2c_dropout_mask(size_t n, float ratio, unsigned long long seed, 
   NEED(mask && ratio >= 0.f && ratio < 1.f, "b2c_dropout_mask: dropout_ratio must be in [0, 1)");
   if (!n) return B2C_OK;
   const unsigned thr = (unsigned)((double)ratio * 16777216.0);
-  dropout_mask_kernel<<<grid_for(n, 256), 256, 0, as_stream(stream)>>>(n, thr, 1.0f / (1.0f - ratio), seed, offset, mask);
+  launch_pdl(dropout_mask_kernel, grid_for(n, 256), 256, 0, as_stream(stream), 0, n, thr, 1.0f / (1.0f - ratio), seed, offset, mask);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -814,7 +841,7 @@ extern "C" int b2c_mul(size_t n, const float* a, const float* b, float* y, void*
   NEED(a && b && y, "b2c_mul: null");
   if (!n) return B2C_OK;
   NEED(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(y)) & 15) == 0, "b2c_mul: pointers must be 16-byte aligned");
-  mul_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, as_stream(stream)>>>(n, a, b, y);
+  launch_pdl(mul_kernel, grid_for((n + 3) / 4, 256), 256, 0, as_stream(stream), 0, n, a, b, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -873,15 +900,15 @@ extern "C" int b2c_pool_forward(int method, int NC, int H, int W, int kh, int kw
     const int q = r.q;
     const long long groups = (long long)NC * Ho * (Wo / q);
     const unsigned grid = grid_for((size_t)groups, 256);
-#define B2C_POOLF(KH, S, Q) pool_max_fwd_q_kernel<KH, KH, S, S, Q><<<grid, 256, 0, s_>>>(groups, H, W, Ho, Wo, ph, pw, x, y, mask)
+#define B2C_POOLF(KH, S, Q) launch_pdl(pool_max_fwd_q_kernel<KH, KH, S, S, Q>, grid, 256, 0, s_, 0, groups, H, W, Ho, Wo, ph, pw, x, y, mask)
     if (kh == 3 && sh == 2) { if (q == 4) B2C_POOLF(3, 2, 4); else B2C_POOLF(3, 2, 2); }
     else if (kh == 2) { if (q == 4) B2C_POOLF(2, 2, 4); else B2C_POOLF(2, 2, 2); }
     else { if (q == 4) B2C_POOLF(3, 1, 4); else B2C_POOLF(3, 1, 2); }
 #undef B2C_POOLF
   } else if (r.route == B2C_POOL_ROUTE_MAX_SCALAR) {
-    pool_max_fwd_kernel<<<grid_for(total, 256), 256, 0, s_>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y, mask);
+    launch_pdl(pool_max_fwd_kernel, grid_for(total, 256), 256, 0, s_, 0, total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y, mask);
   } else {
-    pool_ave_fwd_kernel<<<grid_for(total, 256), 256, 0, s_>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y);
+    launch_pdl(pool_ave_fwd_kernel, grid_for(total, 256), 256, 0, s_, 0, total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, x, y);
   }
   B2C_POST_LAUNCH();
   return B2C_OK;
@@ -897,17 +924,17 @@ extern "C" int b2c_pool_backward(int method, int NC, int H, int W, int kh, int k
   if (r.route == B2C_POOL_ROUTE_MAX_BWD_QUAD) {
     const long long quads = (long long)NC * H * (W / 4);
     const unsigned grid = grid_for((size_t)quads, 256);
-    if (kh == 3 && sh == 2) pool_max_bwd_q4_kernel<3, 3, 2, 2><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
-    else if (kh == 2) pool_max_bwd_q4_kernel<2, 2, 2, 2><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
-    else pool_max_bwd_q4_kernel<3, 3, 1, 1><<<grid, 256, 0, s_>>>(quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
+    if (kh == 3 && sh == 2) launch_pdl(pool_max_bwd_q4_kernel<3, 3, 2, 2>, grid, 256, 0, s_, 0, quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
+    else if (kh == 2) launch_pdl(pool_max_bwd_q4_kernel<2, 2, 2, 2>, grid, 256, 0, s_, 0, quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
+    else launch_pdl(pool_max_bwd_q4_kernel<3, 3, 1, 1>, grid, 256, 0, s_, 0, quads, H, W, Ho, Wo, ph, pw, dy, mask, dx);
   } else if (r.route == B2C_POOL_ROUTE_MAX_BWD_ROW) {
     const long long rows = (long long)NC * H;
     const long long groups = (rows + r.rpb - 1) / r.rpb;
     const int grid = (int)(groups < (long long)sm_count() * 64 ? groups : (long long)sm_count() * 64);
-    pool_max_bwd_kernel<<<grid, 128, 0, s_>>>((int)rows, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, mask, dx);
+    launch_pdl(pool_max_bwd_kernel, grid, 128, 0, s_, 0, (int)rows, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, mask, dx);
   } else {
     const size_t total = (size_t)NC * H * W;
-    pool_ave_bwd_kernel<<<grid_for(total, 256), 256, 0, s_>>>(total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, dx);
+    launch_pdl(pool_ave_bwd_kernel, grid_for(total, 256), 256, 0, s_, 0, total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dy, dx);
   }
   B2C_POST_LAUNCH();
   return B2C_OK;
@@ -915,6 +942,7 @@ extern "C" int b2c_pool_backward(int method, int NC, int H, int W, int kh, int k
 // dst[c][r] = src[r][c]: 32 x 32 tiles through shared memory (padded: conflict-free both ways), coalesced reads and writes
 __global__ void __launch_bounds__(256)
 transpose_kernel(int rows, int cols, const float* __restrict__ src, float* __restrict__ dst) {
+  pdl_wait();
   __shared__ float tile[32][33];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;             // 32 x 8 threads
   const long long c0 = (long long)blockIdx.x * 32, r0 = (long long)blockIdx.y * 32;
@@ -934,7 +962,7 @@ extern "C" int b2c_transpose(int rows, int cols, const float* src, float* dst, v
   NEED(src && dst && rows > 0 && cols > 0 && src != dst, "b2c_transpose: bad argument");
   dim3 grid((cols + 31) / 32, (rows + 31) / 32);
   NEED(grid.y <= 65535, "b2c_transpose: too many rows");
-  transpose_kernel<<<grid, 256, 0, as_stream(stream)>>>(rows, cols, src, dst);
+  launch_pdl(transpose_kernel, grid, 256, 0, as_stream(stream), 0, rows, cols, src, dst);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -942,22 +970,22 @@ extern "C" int b2c_add(size_t n, const float* a, const float* b, float* y, void*
   NEED(a && b && y, "b2c_add: null");
   if (!n) return B2C_OK;
   const bool al = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
-  add_kernel<<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, a, b, y);
+  launch_pdl(add_kernel, grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream), 0, n, al ? 1 : 0, a, b, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 extern "C" int b2c_softmax_loss_forward(int N, int C, const float* logits, const float* labels, float* prob, float* loss, void* stream) {
   NEED(logits && labels && prob && loss && N > 0 && C > 0, "b2c_softmax_loss_forward: bad argument");
-  softmax_loss_fwd_kernel<<<N, 256, 0, as_stream(stream)>>>(C, logits, prob);
+  launch_pdl(softmax_loss_fwd_kernel, N, 256, 0, as_stream(stream), 0, C, logits, prob);
   B2C_POST_LAUNCH();
-  softmax_loss_sum_kernel<<<1, 256, 0, as_stream(stream)>>>(N, C, prob, labels, 1.0f / (float)N, loss);   // VALID normalisation, no ignore_label
+  launch_pdl(softmax_loss_sum_kernel, 1, 256, 0, as_stream(stream), 0, N, C, prob, labels, 1.0f / (float)N, loss);   // VALID normalisation, no ignore_label
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 extern "C" int b2c_softmax_loss_backward(int N, int C, const float* prob, const float* labels, float loss_weight, float* dx, void* stream) {
   NEED(prob && labels && dx && N > 0 && C > 0, "b2c_softmax_loss_backward: bad argument");
   const size_t total = (size_t)N * C;
-  softmax_loss_bwd_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(total, C, prob, labels, loss_weight / (float)N, dx);
+  launch_pdl(softmax_loss_bwd_kernel, grid_for(total, 256), 256, 0, as_stream(stream), 0, total, C, prob, labels, loss_weight / (float)N, dx);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -968,28 +996,28 @@ static bool al16(std::initializer_list<const void*> ptrs) {
 extern "C" int b2c_softmax_forward(int outer, int C, int inner, const float* x, float* y, void* stream) {
   NEED(x && y && outer > 0 && C > 0 && inner > 0, "b2c_softmax_forward: bad argument");
   if (inner == 1) {                                // every [N, C] use: SoftmaxWithLoss's row kernel, so prob and this top agree bit for bit
-    softmax_loss_fwd_kernel<<<outer, 256, 0, as_stream(stream)>>>(C, x, y);
+    launch_pdl(softmax_loss_fwd_kernel, outer, 256, 0, as_stream(stream), 0, C, x, y);
     B2C_POST_LAUNCH();
     return B2C_OK;
   }
   const bool vec = inner % 4 == 0 && al16({x, y});
   const size_t cols = (size_t)outer * (vec ? inner / 4 : inner);
-  if (vec) softmax_col_fwd_kernel<true><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, x, y);
-  else softmax_col_fwd_kernel<false><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, x, y);
+  if (vec) launch_pdl(softmax_col_fwd_kernel<true>, grid_for(cols, 256), 256, 0, as_stream(stream), 0, cols, C, inner, x, y);
+  else launch_pdl(softmax_col_fwd_kernel<false>, grid_for(cols, 256), 256, 0, as_stream(stream), 0, cols, C, inner, x, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
 extern "C" int b2c_softmax_backward(int outer, int C, int inner, const float* y, const float* dy, float* dx, void* stream) {
   NEED(y && dy && dx && outer > 0 && C > 0 && inner > 0, "b2c_softmax_backward: bad argument");
   if (inner == 1) {
-    softmax_row_bwd_kernel<<<outer, 256, 0, as_stream(stream)>>>(C, y, dy, dx);
+    launch_pdl(softmax_row_bwd_kernel, outer, 256, 0, as_stream(stream), 0, C, y, dy, dx);
     B2C_POST_LAUNCH();
     return B2C_OK;
   }
   const bool vec = inner % 4 == 0 && al16({y, dy, dx});
   const size_t cols = (size_t)outer * (vec ? inner / 4 : inner);
-  if (vec) softmax_col_bwd_kernel<true><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, y, dy, dx);
-  else softmax_col_bwd_kernel<false><<<grid_for(cols, 256), 256, 0, as_stream(stream)>>>(cols, C, inner, y, dy, dx);
+  if (vec) launch_pdl(softmax_col_bwd_kernel<true>, grid_for(cols, 256), 256, 0, as_stream(stream), 0, cols, C, inner, y, dy, dx);
+  else launch_pdl(softmax_col_bwd_kernel<false>, grid_for(cols, 256), 256, 0, as_stream(stream), 0, cols, C, inner, y, dy, dx);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -997,7 +1025,7 @@ template <int OP>
 static int launch_ew(size_t n, const float* a, const float* b, float s, float* y, void* stream) {
   if (!n) return B2C_OK;
   const bool al = al16({a, b, y});                 // (b may be null: aligned)
-  ew_kernel<OP><<<grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, a, b, s, y);
+  launch_pdl(ew_kernel<OP>, grid_for(al ? (n + 3) / 4 : n, 256), 256, 0, as_stream(stream), 0, n, al ? 1 : 0, a, b, s, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -1013,15 +1041,7 @@ extern "C" int b2c_sigmoid_backward(size_t n, const float* y, const float* dy, f
 template <typename... KArgs, typename... Args>
 static int launch_loss_cluster(void (*kernel)(KArgs...), size_t count, void* stream, Args... args) {
   const unsigned cs = loss_cluster_size(count);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(cs, 1, 1);
-  cfg.blockDim = dim3(LOSS_THREADS, 1, 1);
-  cfg.stream = as_stream(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  B2C_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, args...));
+  launch_pdl(kernel, dim3(cs, 1, 1), dim3(LOSS_THREADS, 1, 1), 0, as_stream(stream), cs, args...);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -1057,8 +1077,8 @@ extern "C" int b2c_contrastive_loss_backward(int N, int C, const float* diff, co
   NEED(diff && dist_sq && y && da && N > 0 && C > 0, "b2c_contrastive_loss_backward: bad argument");
   const size_t n = (size_t)N * C;
   const bool vec = C % 4 == 0 && al16({diff, da, db});
-  if (vec) contrastive_bwd_kernel<true><<<grid_for(n / 4, 256), 256, 0, as_stream(stream)>>>(N, C, diff, dist_sq, y, margin, legacy, alpha, da, db);
-  else contrastive_bwd_kernel<false><<<grid_for(n, 256), 256, 0, as_stream(stream)>>>(N, C, diff, dist_sq, y, margin, legacy, alpha, da, db);
+  if (vec) launch_pdl(contrastive_bwd_kernel<true>, grid_for(n / 4, 256), 256, 0, as_stream(stream), 0, N, C, diff, dist_sq, y, margin, legacy, alpha, da, db);
+  else launch_pdl(contrastive_bwd_kernel<false>, grid_for(n, 256), 256, 0, as_stream(stream), 0, N, C, diff, dist_sq, y, margin, legacy, alpha, da, db);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

@@ -37,6 +37,7 @@ template <bool VEC, bool RELU>
 __global__ void __launch_bounds__(256)
 bn_norm_fused_kernel(size_t total_units, int C, int S, const float* __restrict__ x, const float* __restrict__ mean,
                      const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y) {
+  pdl_wait();
   const unsigned units = VEC ? S / 4 : S;
   size_t i = (size_t)blockIdx.x * (256 * FB_EW) + threadIdx.x;
   if (i >= total_units) return;
@@ -151,6 +152,7 @@ __global__ void __launch_bounds__(BN_THREADS)
 bn_bwd_reduce_fused_kernel(int N, int C, int S, const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
                            const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
                            float* __restrict__ sum_dy_xn, float* __restrict__ sum_dy) {
+  pdl_wait();
   __shared__ float2 part;
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank(), nranks = cluster.num_blocks();
@@ -218,6 +220,7 @@ __global__ void __launch_bounds__(BN_THREADS, 2)
 bn_fwd_onepass_kernel(int N, int C, int S, const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
                       float eps, float maf, int first, float* __restrict__ mean, float* __restrict__ invstd, float* __restrict__ run_mean,
                       float* __restrict__ run_var, const float* __restrict__ res, float* __restrict__ y) {
+  pdl_wait();
   extern __shared__ float4 bn_cache[];
   __shared__ float2 part[2];
   cg::cluster_group cluster = cg::this_cluster();
@@ -286,6 +289,7 @@ bn_bwd_onepass_kernel(int N, int C, int S, float inv_cnt, unsigned slice_units, 
                       const float* __restrict__ ym, const float* __restrict__ mean, const float* __restrict__ invstd,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ sum_dy_xn,
                       float* __restrict__ sum_dy, float* __restrict__ dx, float* __restrict__ d_res, const float* __restrict__ dy2) {
+  pdl_wait();
   constexpr int U = MASK == 2 ? 2 : BN_U;           // three input streams in the residual form: fewer units in flight per stream (64 registers)
   extern __shared__ float4 bn_cache[];
   __shared__ float2 part;
@@ -385,6 +389,7 @@ __global__ void __launch_bounds__(256)
 bn_bwd_dx_fused_kernel(size_t total_units, int C, int S, float inv_cnt, const float* __restrict__ dy, const float* __restrict__ x,
                        const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
                        const float* __restrict__ beta, const float* __restrict__ sum_dy_xn, const float* __restrict__ sum_dy, float* __restrict__ dx) {
+  pdl_wait();
   const unsigned units = VEC ? S / 4 : S;
   size_t i = (size_t)blockIdx.x * (256 * FB_EW) + threadIdx.x;
   if (i >= total_units) return;
@@ -411,6 +416,7 @@ bn_bwd_dx_fused_kernel(size_t total_units, int C, int S, float inv_cnt, const fl
 }
 
 __global__ void __launch_bounds__(256) add_relu_kernel(size_t n, int vec, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y) {
+  pdl_wait();
   const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   for (size_t i = tid; i < n4; i += step) {
     const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
@@ -420,6 +426,7 @@ __global__ void __launch_bounds__(256) add_relu_kernel(size_t n, int vec, const 
 }
 __global__ void __launch_bounds__(256)
 relu_bwd2_kernel(size_t n, int vec, const float* __restrict__ dy, const float* __restrict__ y, float* __restrict__ dxa, float* __restrict__ dxb) {
+  pdl_wait();
   const size_t n4 = vec ? n / 4 : 0, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   for (size_t i = tid; i < n4; i += step) {
     const float4 d = reinterpret_cast<const float4*>(dy)[i], v = reinterpret_cast<const float4*>(y)[i];
@@ -438,6 +445,7 @@ relu_bwd2_kernel(size_t n, int vec, const float* __restrict__ dy, const float* _
 // ordered like std::greater<pair<float,int>> (equal scores: the HIGHER class index ranks first).  One warp per sample.
 __global__ void __launch_bounds__(256)
 accuracy_kernel(int N, int C, int top_k, const float* __restrict__ scores, const float* __restrict__ labels, unsigned int* __restrict__ hits) {
+  pdl_wait();
   const int warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (warp >= N) return;
   const int lab = (int)labels[warp];
@@ -450,7 +458,7 @@ accuracy_kernel(int N, int C, int top_k, const float* __restrict__ scores, const
   for (int o = 16; o; o >>= 1) above += __shfl_xor_sync(0xffffffffu, above, o);
   if (lane == 0 && above < top_k) atomicAdd(hits, 1u);
 }
-__global__ void accuracy_finish_kernel(const unsigned int* hits, int N, float* acc) { *acc = (float)*hits / (float)N; }
+__global__ void accuracy_finish_kernel(const unsigned int* hits, int N, float* acc) { pdl_wait(); *acc = (float)*hits / (float)N; }
 
 // the statistics kernel of layers.cu (same launch for the fused and the unfused forward)
 int launch_bn_stats(const BnPlan& p, int N, int C, int S, const float* x, float eps, float maf, int first, float* mean, float* invstd,
@@ -556,10 +564,10 @@ static int bn_forward_fused_impl(int N, int C, int S, const float* x, const floa
   const size_t units = (size_t)N * C * (vec ? S / 4 : S);
   const unsigned blocks = (unsigned)((units + 256 * FB_EW - 1) / (256 * FB_EW));
   cudaStream_t st = as_stream(stream);
-  if (vec) { if (relu) bn_norm_fused_kernel<true, true><<<blocks, 256, 0, st>>>(units, C, S, x, save_mean, save_invstd, gamma, beta, y);
-             else bn_norm_fused_kernel<true, false><<<blocks, 256, 0, st>>>(units, C, S, x, save_mean, save_invstd, gamma, beta, y); }
-  else { if (relu) bn_norm_fused_kernel<false, true><<<blocks, 256, 0, st>>>(units, C, S, x, save_mean, save_invstd, gamma, beta, y);
-         else bn_norm_fused_kernel<false, false><<<blocks, 256, 0, st>>>(units, C, S, x, save_mean, save_invstd, gamma, beta, y); }
+  if (vec) { if (relu) launch_pdl(bn_norm_fused_kernel<true, true>, blocks, 256, 0, st, 0, units, C, S, x, save_mean, save_invstd, gamma, beta, y);
+             else launch_pdl(bn_norm_fused_kernel<true, false>, blocks, 256, 0, st, 0, units, C, S, x, save_mean, save_invstd, gamma, beta, y); }
+  else { if (relu) launch_pdl(bn_norm_fused_kernel<false, true>, blocks, 256, 0, st, 0, units, C, S, x, save_mean, save_invstd, gamma, beta, y);
+         else launch_pdl(bn_norm_fused_kernel<false, false>, blocks, 256, 0, st, 0, units, C, S, x, save_mean, save_invstd, gamma, beta, y); }
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -617,10 +625,10 @@ static int bn_backward_fused_impl(int N, int C, int S, const float* dy, const fl
   const unsigned blocks = (unsigned)((units + 256 * FB_EW - 1) / (256 * FB_EW));
   const float inv_cnt = 1.0f / ((float)N * S);
   cudaStream_t st = as_stream(stream);
-  if (vec) { if (relu) bn_bwd_dx_fused_kernel<true, true><<<blocks, 256, 0, st>>>(units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx);
-             else bn_bwd_dx_fused_kernel<true, false><<<blocks, 256, 0, st>>>(units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx); }
-  else { if (relu) bn_bwd_dx_fused_kernel<false, true><<<blocks, 256, 0, st>>>(units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx);
-         else bn_bwd_dx_fused_kernel<false, false><<<blocks, 256, 0, st>>>(units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx); }
+  if (vec) { if (relu) launch_pdl(bn_bwd_dx_fused_kernel<true, true>, blocks, 256, 0, st, 0, units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx);
+             else launch_pdl(bn_bwd_dx_fused_kernel<true, false>, blocks, 256, 0, st, 0, units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx); }
+  else { if (relu) launch_pdl(bn_bwd_dx_fused_kernel<false, true>, blocks, 256, 0, st, 0, units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx);
+         else launch_pdl(bn_bwd_dx_fused_kernel<false, false>, blocks, 256, 0, st, 0, units, C, S, inv_cnt, dy, x, save_mean, save_invstd, gamma, beta, dgamma, dbeta, dx); }
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -646,7 +654,7 @@ extern "C" int b2c_add_relu(size_t n, const float* a, const float* b, float* y, 
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) return fail(B2C_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
   if (!n) return B2C_OK;
   const bool al = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
-  add_relu_kernel<<<grid_for(al ? n / 4 + 1 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, a, b, y);
+  launch_pdl(add_relu_kernel, grid_for(al ? n / 4 + 1 : n, 256), 256, 0, as_stream(stream), 0, n, al ? 1 : 0, a, b, y);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -657,7 +665,7 @@ extern "C" int b2c_relu_backward2(size_t n, const float* dy, const float* y, flo
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) return fail(B2C_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
   if (!n) return B2C_OK;
   const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dx_a) | reinterpret_cast<uintptr_t>(dx_b)) & 15) == 0;
-  relu_bwd2_kernel<<<grid_for(al ? n / 4 + 1 : n, 256), 256, 0, as_stream(stream)>>>(n, al ? 1 : 0, dy, y, dx_a, dx_b);
+  launch_pdl(relu_bwd2_kernel, grid_for(al ? n / 4 + 1 : n, 256), 256, 0, as_stream(stream), 0, n, al ? 1 : 0, dy, y, dx_a, dx_b);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -669,9 +677,9 @@ extern "C" int b2c_accuracy(int N, int C, int top_k, const float* scores, const 
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) return fail(B2C_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
   cudaStream_t st = as_stream(stream);
   B2C_CUDA_OK(cudaMemsetAsync(scratch, 0, 4, st));
-  accuracy_kernel<<<(N * 32 + 255) / 256, 256, 0, st>>>(N, C, top_k, scores, labels, static_cast<unsigned int*>(scratch));
+  launch_pdl(accuracy_kernel, (N * 32 + 255) / 256, 256, 0, st, 0, N, C, top_k, scores, labels, static_cast<unsigned int*>(scratch));
   B2C_POST_LAUNCH();
-  accuracy_finish_kernel<<<1, 1, 0, st>>>(static_cast<const unsigned int*>(scratch), N, accuracy);
+  launch_pdl(accuracy_finish_kernel, 1, 1, 0, st, 0, static_cast<const unsigned int*>(scratch), N, accuracy);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

@@ -144,6 +144,7 @@ __device__ __forceinline__ void solver_span(const R& rule, size_t n, float* __re
 __global__ void __launch_bounds__(256)
 sgd_update_kernel(size_t n, float* __restrict__ g, float* __restrict__ w, float* __restrict__ h, float momentum,
                   float lr, float decay, int l2, float gscale, int clear) {
+  pdl_wait();
   solver_span(SgdRule{momentum}, n, g, w, h, nullptr, lr, decay, l2 != 0, gscale, clear != 0,
               (size_t)blockIdx.x * blockDim.x + threadIdx.x, (size_t)gridDim.x * blockDim.x);
 }
@@ -174,6 +175,7 @@ template <class R, class Scale>
 __global__ void __launch_bounds__(256)
 solver_update_arena_kernel(const __grid_constant__ SegTable t, float* __restrict__ g, float* __restrict__ w,
                            float* __restrict__ h, float* __restrict__ h2, const R rule, int l2, const Scale gscale, int clear) {
+  pdl_wait();
   // binary search the owning segment
   int lo = 0, hi = t.nseg - 1;
   while (lo < hi) {
@@ -227,7 +229,7 @@ static int launch_arena(const char* who, const R& rule, int nseg, const size_t* 
   std::vector<SegTable> launches;
   if (const int rc = pack_segments(who, nseg, offset, count, local_rate, local_decay, &launches, nullptr)) return rc;
   for (const SegTable& t : launches) {
-    solver_update_arena_kernel<R, Scale><<<t.block_start[t.nseg], 256, 0, as_stream(stream)>>>(t, g, w, h, h2, rule, l2,
+    launch_pdl(solver_update_arena_kernel<R, Scale>, t.block_start[t.nseg], 256, 0, as_stream(stream), 0, t, g, w, h, h2, rule, l2,
                                                                                                grad_scale, clear_grads);
     B2C_POST_LAUNCH();
   }
@@ -267,6 +269,7 @@ __device__ __forceinline__ double sq(float x) { return (double)x * (double)x; } 
 // cuts the span -- so a partial depends only on its segment's address and count.
 __global__ void __launch_bounds__(256)
 arena_sumsq_kernel(const __grid_constant__ SumsqTable t, const float* __restrict__ g, double* __restrict__ partials) {
+  pdl_wait();
   int lo = 0, hi = t.nseg - 1;
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
@@ -297,6 +300,7 @@ arena_sumsq_kernel(const __grid_constant__ SumsqTable t, const float* __restrict
 // One CTA: each thread sums the slots i = tid (mod 256) in order, then block_sum_fixed.
 __global__ void __launch_bounds__(256)
 clip_factor_kernel(const double* __restrict__ partials, size_t n, double s_n, float clip, b2c_clip_state* __restrict__ st) {
+  pdl_wait();
   double s = 0.0;
   for (size_t i = threadIdx.x; i < n; i += blockDim.x) s += partials[i];
   const double tot = block_sum_fixed(s);
@@ -340,7 +344,7 @@ extern "C" int b2c_sgd_update(size_t n, float* g, float* w, float* h, float mome
                               float local_decay, int l2, float grad_scale, int clear_grads, void* stream) {
   if (!g || !w || !h) return fail(B2C_ERR_INVALID, "b2c_sgd_update: null pointer");
   if (n == 0) return B2C_OK;
-  sgd_update_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, as_stream(stream)>>>(n, g, w, h, momentum, local_rate,
+  launch_pdl(sgd_update_kernel, grid_for((n + 3) / 4, 256), 256, 0, as_stream(stream), 0, n, g, w, h, momentum, local_rate,
                                                                                local_decay, l2, grad_scale,
                                                                                clear_grads);
   B2C_POST_LAUNCH();
@@ -399,7 +403,7 @@ extern "C" int b2c_arena_sumsq(int nseg, const size_t* offset, const size_t* cou
   std::vector<SumsqTable> launches;
   if (const int rc = pack_sumsq(who, nseg, offset, count, slot, &launches, nullptr)) return rc;
   for (const SumsqTable& t : launches) {
-    arena_sumsq_kernel<<<t.block_start[t.nseg], 256, 0, as_stream(stream)>>>(t, g, partials);
+    launch_pdl(arena_sumsq_kernel, t.block_start[t.nseg], 256, 0, as_stream(stream), 0, t, g, partials);
     B2C_POST_LAUNCH();
   }
   return B2C_OK;
@@ -410,7 +414,7 @@ extern "C" int b2c_clip_factor(const double* partials, size_t nslots, double s_n
   const char* who = "b2c_clip_factor";
   if ((nslots && !partials) || !state) return fail(B2C_ERR_INVALID, "%s: bad argument", who);
   if (!(clip >= 0.f) || !(s_n > 0.0) || std::isinf(s_n)) return fail(B2C_ERR_INVALID, "%s: clip %g, s_n %g", who, clip, s_n);
-  clip_factor_kernel<<<1, 256, 0, as_stream(stream)>>>(partials, nslots, s_n, clip, state);
+  launch_pdl(clip_factor_kernel, 1, 256, 0, as_stream(stream), 0, partials, nslots, s_n, clip, state);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

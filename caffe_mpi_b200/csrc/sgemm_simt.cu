@@ -16,6 +16,7 @@ template <bool TA, bool TB>
 __global__ void __launch_bounds__(256)
 sgemm_simt_kernel(int M, int N, int K, float alpha, const float* __restrict__ A, int lda,
                   const float* __restrict__ B, int ldb, float beta, float* __restrict__ C, int ldc) {
+  pdl_wait();
   __shared__ float As[2][TK][TM + 4];
   __shared__ float Bs[2][TK][TN + 4];
   const int tid = threadIdx.x;
@@ -85,10 +86,10 @@ int launch_sgemm_simt(bool tA, bool tB, int M, int N, int K, float alpha, const 
   if (M <= 0 || N <= 0) return B2C_OK;
   dim3 grid((N + TN - 1) / TN, (M + TM - 1) / TM);
   if (grid.y > 65535) return fail(B2C_ERR_INVALID, "sgemm: M too large for the SIMT path");
-  if (!tA && !tB) sgemm_simt_kernel<false, false><<<grid, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
-  else if (tA && !tB) sgemm_simt_kernel<true, false><<<grid, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
-  else if (!tA && tB) sgemm_simt_kernel<false, true><<<grid, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
-  else sgemm_simt_kernel<true, true><<<grid, 256, 0, st>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
+  if (!tA && !tB) launch_pdl(sgemm_simt_kernel<false, false>, grid, 256, 0, st, 0, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
+  else if (tA && !tB) launch_pdl(sgemm_simt_kernel<true, false>, grid, 256, 0, st, 0, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
+  else if (!tA && tB) launch_pdl(sgemm_simt_kernel<false, true>, grid, 256, 0, st, 0, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
+  else launch_pdl(sgemm_simt_kernel<true, true>, grid, 256, 0, st, 0, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }
@@ -98,6 +99,7 @@ int launch_sgemm_simt(bool tA, bool tB, int M, int N, int K, float alpha, const 
 __global__ void __launch_bounds__(256)
 sgemv_n_kernel(int M, int N, float alpha, const float* __restrict__ A, const float* __restrict__ x, float beta,
                float* __restrict__ y) {
+  pdl_wait();
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int row = warp; row < M; row += nwarps) {
@@ -113,6 +115,7 @@ sgemv_n_kernel(int M, int N, float alpha, const float* __restrict__ A, const flo
 __global__ void __launch_bounds__(256)
 sgemv_t_kernel(int M, int N, float alpha, const float* __restrict__ A, const float* __restrict__ x, float beta,
                float* __restrict__ y) {
+  pdl_wait();
   for (int col = blockIdx.x * blockDim.x + threadIdx.x; col < N; col += gridDim.x * blockDim.x) {
     float s = 0.0f;
     for (int r = 0; r < M; ++r) s = fmaf(__ldg(A + (size_t)r * N + col), __ldg(x + r), s);
@@ -128,9 +131,9 @@ extern "C" int b2c_sgemv(int transA, int M, int N, float alpha, const float* A, 
                          float* y, void* stream) {
   if (!A || !x || !y || M <= 0 || N <= 0) return fail(B2C_ERR_INVALID, "b2c_sgemv: bad argument");
   if (!transA) {
-    sgemv_n_kernel<<<grid_for((size_t)M * 32, 256), 256, 0, as_stream(stream)>>>(M, N, alpha, A, x, beta, y);
+    launch_pdl(sgemv_n_kernel, grid_for((size_t)M * 32, 256), 256, 0, as_stream(stream), 0, M, N, alpha, A, x, beta, y);
   } else {
-    sgemv_t_kernel<<<grid_for((size_t)N, 256), 256, 0, as_stream(stream)>>>(M, N, alpha, A, x, beta, y);
+    launch_pdl(sgemv_t_kernel, grid_for((size_t)N, 256), 256, 0, as_stream(stream), 0, M, N, alpha, A, x, beta, y);
   }
   B2C_POST_LAUNCH();
   return B2C_OK;

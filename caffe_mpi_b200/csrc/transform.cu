@@ -15,6 +15,7 @@ __global__ void __launch_bounds__(256)
 transform_u8_kernel(const unsigned char* __restrict__ src, int N, int C, int Hd, int Wd, int Hc, int Wc, const int* __restrict__ h_off,
                     const int* __restrict__ w_off, const unsigned char* __restrict__ mirror, const float* __restrict__ mean_values,
                     const float* __restrict__ mean_image, float scale, float* __restrict__ dst) {
+  pdl_wait();
   const int wq = (Wc + 3) / 4;                              // 4-pixel groups per output row
   const long long total = (long long)N * C * Hc * wq;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -61,7 +62,7 @@ extern "C" int b2c_transform_u8(const unsigned char* src, int N, int C, int Hd, 
   int dev_count = 0;
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) return fail(B2C_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
   const size_t units = (size_t)N * C * crop_h * ((crop_w + 3) / 4);
-  transform_u8_kernel<<<grid_for(units, 256), 256, 0, as_stream(stream)>>>(src, N, C, Hd, Wd, crop_h, crop_w, h_off, w_off, mirror, mean_values,
+  launch_pdl(transform_u8_kernel, grid_for(units, 256), 256, 0, as_stream(stream), 0, src, N, C, Hd, Wd, crop_h, crop_w, h_off, w_off, mirror, mean_values,
                                                                          mean_image, scale, dst);
   B2C_POST_LAUNCH();
   return B2C_OK;
