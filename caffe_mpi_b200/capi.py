@@ -23,6 +23,9 @@ POOL_ROUTES = ("max_scalar", "max_window", "max_bwd_row", "max_bwd_quad", "ave")
 SGEMM_ROUTES = ("ffma", "tc")
 # b2c_deconv_route, in enum order
 DECONV_ROUTES = ("dual", "phase", "depthwise")
+# b2c_softmax_loss_route and b2c_loss_normalization, in enum order
+SOFTMAX_LOSS_ROUTES = ("row", "column", "column_f4")
+LOSS_NORMS = ("FULL", "VALID", "BATCH_SIZE", "NONE")
 
 
 class B2CError(RuntimeError):
@@ -154,6 +157,11 @@ def lib():
         "b2c_add": (i, [sz, vp, vp, vp, vp]),
         "b2c_softmax_loss_forward": (i, [i, i, vp, vp, vp, vp, vp]),
         "b2c_softmax_loss_backward": (i, [i, i, vp, vp, f, vp, vp]),
+        "b2c_softmax_loss_workspace": (i, [i, i, i, C.POINTER(sz)]),
+        "b2c_softmax_loss_forward_ex": (i, [i, i, i, vp, vp, i, i, i, vp, vp, vp, vp, vp]),
+        "b2c_softmax_loss_backward_ex": (i, [i, i, i, vp, vp, i, i, vp, f, vp, vp]),
+        "b2c_debug_softmax_loss_plan": (i, [i, i, i, vp, vp, C.POINTER(i), i]),
+        "b2c_accuracy_ex": (i, [i, i, i, i, vp, vp, i, i, vp, vp, vp, vp]),
         "b2c_softmax_forward": (i, [i, i, i, vp, vp, vp]),
         "b2c_softmax_backward": (i, [i, i, i, vp, vp, vp, vp]),
         "b2c_sigmoid_forward": (i, [sz, vp, vp, vp]),
@@ -483,6 +491,39 @@ def pool_plan(method, dir, NC, H, W, k, s, p, out_ptr=0, mask_ptr=0):
 
 
 BN_FORMS = ("unfused", "fused", "fused_res")
+
+
+def softmax_loss_plan(outer, Cc, inner, logits_ptr=0, prob_ptr=0):
+    """b2c_debug_softmax_loss_plan: the forward route of b2c_softmax_loss_forward_ex with logits / prob at these addresses, the
+    pixels per chunk, the chunks and the workspace bytes."""
+    out = (C.c_int * 4)()
+    check(lib().b2c_debug_softmax_loss_plan(outer, Cc, inner, C.c_void_p(logits_ptr), C.c_void_p(prob_ptr), out, 4))
+    return {"route": SOFTMAX_LOSS_ROUTES[out[0]], "chunk": out[1], "slots": out[2], "workspace": out[3]}
+
+
+def softmax_loss_workspace(outer, Cc, inner):
+    n = C.c_size_t()
+    check(lib().b2c_softmax_loss_workspace(outer, Cc, inner, C.byref(n)))
+    return n.value
+
+
+def softmax_loss_forward_ex(outer, Cc, inner, logits, labels, prob, loss, normalizer, workspace, ignore_label=None,
+                            norm="VALID", stream=None):
+    """b2c_softmax_loss_forward_ex on torch CUDA tensors; ignore_label None = not set; norm one of LOSS_NORMS."""
+    check(lib().b2c_softmax_loss_forward_ex(outer, Cc, inner, _p(logits), _p(labels), int(ignore_label is not None),
+                                            int(ignore_label or 0), LOSS_NORMS.index(norm), _p(prob), _p(loss), _p(normalizer),
+                                            _p(workspace), _stream(stream)))
+
+
+def softmax_loss_backward_ex(outer, Cc, inner, prob, labels, normalizer, loss_weight, dx, ignore_label=None, stream=None):
+    check(lib().b2c_softmax_loss_backward_ex(outer, Cc, inner, _p(prob), _p(labels), int(ignore_label is not None),
+                                             int(ignore_label or 0), _p(normalizer), loss_weight, _p(dx), _stream(stream)))
+
+
+def accuracy_ex(outer, Cc, inner, top_k, scores, labels, accuracy, per_class, scratch, ignore_label=None, stream=None):
+    """b2c_accuracy_ex; per_class may be None; scratch holds 8 + 8 * Cc bytes (8 without per_class)."""
+    check(lib().b2c_accuracy_ex(outer, Cc, inner, top_k, _p(scores), _p(labels), int(ignore_label is not None), int(ignore_label or 0),
+                                _p(accuracy), _p(per_class), _p(scratch), _stream(stream)))
 
 
 def bn_plan(dir, form, N, Cc, S, ptrs=()):

@@ -11,6 +11,7 @@
 //   Eltwise SUM     src/caffe/layers/eltwise_layer.cpp
 //   SoftmaxWithLoss src/caffe/layers/softmax_loss_layer.cpp:96-160  loss = -sum log p[label] / N (VALID normalisation, no
 //                                                                    ignore_label); dx = (p - onehot) * loss_weight / N
+//                   the _ex forms: per (outer, inner) pixel, ignore_label, FULL / VALID / BATCH_SIZE / NONE normalizers
 //   Softmax         src/caffe/layers/softmax_layer.cu               over the C axis of [outer, C, inner]; dx = (dy - sum_c dy y) y
 //   Sigmoid         src/caffe/layers/sigmoid_layer.cu:9-13           y = 1 / (1 + exp(-x)); dx = dy y (1 - y)
 //   SigmoidCrossEntropyLoss  sigmoid_cross_entropy_loss_layer.cpp   the stable loss expression / N; dx = (sigmoid(x) - t) * loss_weight / N
@@ -494,11 +495,42 @@ softmax_loss_bwd_kernel(size_t total, int C, const float* __restrict__ prob, con
   }
 }
 
+// a warp's double sum in a fixed shuffle tree (the loss reductions below)
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
 // ---- Softmax ------------------------------------------------------------------------------------------------------
 // Over the C axis of an [outer, C, inner] view.  inner == 1 runs softmax_loss_fwd_kernel above (alias-safe): one block per row.
 // inner > 1: one thread per
 // (outer, inner) column (VEC: four adjacent columns), so a warp's loads and stores run along `inner` and coalesce; each column
 // takes max, then expf(z - max) and the sum, then the scale, in the row kernel's expressions.  No __restrict__: y may be x.
+// softmax_col is the one column (VEC: four columns) the Softmax layer's kernel and SoftmaxWithLoss's column route both compute, so
+// their prob agree bit for bit.  z and p point at channel 0 of the column; w is the channel stride in units of V.
+template <bool VEC>
+__device__ __forceinline__ void softmax_col(const typename std::conditional<VEC, float4, float>::type* z,
+                                            typename std::conditional<VEC, float4, float>::type* p, int C, int w) {
+  if constexpr (VEC) {
+    float4 mx = make_float4(-FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX), s = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int c = 0; c < C; ++c) { const float4 v = z[(size_t)c * w]; mx.x = fmaxf(mx.x, v.x); mx.y = fmaxf(mx.y, v.y); mx.z = fmaxf(mx.z, v.z); mx.w = fmaxf(mx.w, v.w); }
+    for (int c = 0; c < C; ++c) {
+      const float4 v = z[(size_t)c * w];
+      const float4 e = make_float4(expf(v.x - mx.x), expf(v.y - mx.y), expf(v.z - mx.z), expf(v.w - mx.w));
+      p[(size_t)c * w] = e;
+      s.x += e.x; s.y += e.y; s.z += e.z; s.w += e.w;
+    }
+    const float4 inv = make_float4(1.f / s.x, 1.f / s.y, 1.f / s.z, 1.f / s.w);
+    for (int c = 0; c < C; ++c) { float4 e = p[(size_t)c * w]; e.x *= inv.x; e.y *= inv.y; e.z *= inv.z; e.w *= inv.w; p[(size_t)c * w] = e; }
+  } else {
+    float mx = -FLT_MAX, s = 0.f;
+    for (int c = 0; c < C; ++c) mx = fmaxf(mx, z[(size_t)c * w]);
+    for (int c = 0; c < C; ++c) { const float e = expf(z[(size_t)c * w] - mx); p[(size_t)c * w] = e; s += e; }
+    const float inv = 1.f / s;
+    for (int c = 0; c < C; ++c) p[(size_t)c * w] *= inv;
+  }
+}
 template <bool VEC>
 __global__ void __launch_bounds__(256) softmax_col_fwd_kernel(size_t cols, int C, int inner, const float* x, float* y) {
   pdl_wait();
@@ -506,26 +538,153 @@ __global__ void __launch_bounds__(256) softmax_col_fwd_kernel(size_t cols, int C
   const int w = VEC ? inner / 4 : inner;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cols; i += (size_t)gridDim.x * blockDim.x) {
     const size_t o = i / w, base = o * C * w + (i - o * w);
-    const V* z = reinterpret_cast<const V*>(x) + base;
-    V* p = reinterpret_cast<V*>(y) + base;
-    if constexpr (VEC) {
-      float4 mx = make_float4(-FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX), s = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int c = 0; c < C; ++c) { const float4 v = z[(size_t)c * w]; mx.x = fmaxf(mx.x, v.x); mx.y = fmaxf(mx.y, v.y); mx.z = fmaxf(mx.z, v.z); mx.w = fmaxf(mx.w, v.w); }
-      for (int c = 0; c < C; ++c) {
-        const float4 v = z[(size_t)c * w];
-        const float4 e = make_float4(expf(v.x - mx.x), expf(v.y - mx.y), expf(v.z - mx.z), expf(v.w - mx.w));
-        p[(size_t)c * w] = e;
-        s.x += e.x; s.y += e.y; s.z += e.z; s.w += e.w;
+    softmax_col<VEC>(reinterpret_cast<const V*>(x) + base, reinterpret_cast<V*>(y) + base, C, w);
+  }
+}
+
+// ---- SoftmaxWithLoss over spatial positions, with ignore_label and the normalization modes (softmax_loss_layer.cpp) ----------
+// A "pixel" is one (outer, inner) column of the [outer, C, inner] view; its label is labels[o * inner + i], a float class id read
+// as (int).  Pixels are cut into chunks of SL_CHUNK; chunk k is one CTA, its thread t owns the four pixels 4t .. 4t+3 of the chunk
+// and sums their terms as ((t0 + t1) + (t2 + t3)) in double; the CTA then sums its threads with a shuffle tree per warp and the
+// warps in order into slot k.  Every slot is a function of the shape and the data alone.
+constexpr int SL_CHUNK = 1024;
+enum SlRoute { SL_ROW = 0, SL_COL = 1, SL_COL4 = 2 };        // b2c_softmax_loss_route
+// the CTA-wide end of the chunk kernels: slot k = the CTA's double sum (threads in a fixed tree) and its integer count
+__device__ __forceinline__ void sl_chunk_store(double acc, int cnt, double* __restrict__ part, int* __restrict__ valid) {
+  __shared__ double wsum[8];
+  __shared__ int wcnt[8];
+  acc = warp_sum_d(acc);
+#pragma unroll
+  for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if ((threadIdx.x & 31) == 0) { wsum[threadIdx.x >> 5] = acc; wcnt[threadIdx.x >> 5] = cnt; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    int n = 0;
+    for (int w = 0; w < 8; ++w) { s += wsum[w]; n += wcnt[w]; }
+    part[blockIdx.x] = s;
+    valid[blockIdx.x] = n;
+  }
+}
+// -log(max(p[label], FLT_MIN)) for one pixel (softmax_loss_layer.cpp:104-115), 0 and not counted when the label is ignored.  An
+// out-of-range label that is not ignored reads the nearest class instead, as softmax_loss_sum_kernel does.
+__device__ __forceinline__ float sl_term(const float* prob, size_t pix, int C, int inner, const float* labels, int has_ignore,
+                                         int ignore_label, int* cnt) {
+  const int lab = (int)labels[pix];
+  if (has_ignore && lab == ignore_label) return 0.f;
+  ++*cnt;
+  const size_t o = pix / (size_t)inner, i = pix - o * inner;
+  const int l = min(max(lab, 0), C - 1);
+  return -logf(fmaxf(prob[(o * C + l) * inner + i], FLT_MIN));
+}
+// ROUTE SL_ROW: prob is already there (softmax_loss_fwd_kernel); SL_COL: the chunk's softmax first, thread t computing pixels
+// t, t + 256, t + 512, t + 768 (softmax_col<false>, so a warp's loads coalesce along inner), then a barrier; SL_COL4: the thread's four
+// pixels are one float4 column (inner % 4 == 0, x and prob 16-byte aligned).  Either way the terms are then formed and summed in the
+// same order.  No __restrict__ on x / prob: prob elements are read back after they are written.
+template <int ROUTE>
+__global__ void __launch_bounds__(256)
+softmax_loss_chunk_kernel(long long pixels, int C, int inner, const float* x, const float* __restrict__ labels, int has_ignore,
+                          int ignore_label, float* prob, double* __restrict__ part, int* __restrict__ valid) {
+  pdl_wait();
+  const long long p0 = (long long)blockIdx.x * SL_CHUNK + 4 * (long long)threadIdx.x;
+  float t[4] = {0.f, 0.f, 0.f, 0.f};
+  int cnt = 0;
+  if (ROUTE == SL_COL) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long pix = (long long)blockIdx.x * SL_CHUNK + k * 256 + threadIdx.x;
+      if (pix < pixels) {
+        const size_t o = (size_t)pix / inner, base = o * C * inner + ((size_t)pix - o * inner);
+        softmax_col<false>(x + base, prob + base, C, inner);
       }
-      const float4 inv = make_float4(1.f / s.x, 1.f / s.y, 1.f / s.z, 1.f / s.w);
-      for (int c = 0; c < C; ++c) { float4 e = p[(size_t)c * w]; e.x *= inv.x; e.y *= inv.y; e.z *= inv.z; e.w *= inv.w; p[(size_t)c * w] = e; }
-    } else {
-      float mx = -FLT_MAX, s = 0.f;
-      for (int c = 0; c < C; ++c) mx = fmaxf(mx, z[(size_t)c * w]);
-      for (int c = 0; c < C; ++c) { const float e = expf(z[(size_t)c * w] - mx); p[(size_t)c * w] = e; s += e; }
-      const float inv = 1.f / s;
-      for (int c = 0; c < C; ++c) p[(size_t)c * w] *= inv;
     }
+    __syncthreads();                                         // the terms below read prob written by other threads of the CTA
+  }
+  if (p0 < pixels) {
+    if (ROUTE == SL_COL4) {
+      const size_t o = (size_t)p0 / inner, base = (o * C * inner + ((size_t)p0 - o * inner)) / 4;
+      softmax_col<true>(reinterpret_cast<const float4*>(x) + base, reinterpret_cast<float4*>(prob) + base, C, inner / 4);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long pix = p0 + k;
+      if (pix >= pixels) break;
+      t[k] = sl_term(prob, (size_t)pix, C, inner, labels, has_ignore, ignore_label, &cnt);
+    }
+  }
+  sl_chunk_store(((double)t[0] + (double)t[1]) + ((double)t[2] + (double)t[3]), cnt, part, valid);
+}
+// One CTA: the slots in index order (thread t sums slots t, t + 256, ... in double, then sl_chunk_store's tree), the normalizer of
+// get_normalizer (softmax_loss_layer.cpp:65-92) floored at 1, *loss = (float)sum / normalizer; *normalizer stays on the device for
+// the backward.  mode: b2c_loss_normalization.
+__global__ void __launch_bounds__(256)
+softmax_loss_finalize_kernel(int slots, long long outer, long long pixels, int has_ignore, int mode, const double* __restrict__ part,
+                             const int* __restrict__ valid, float* __restrict__ loss, float* __restrict__ normalizer) {
+  pdl_wait();
+  double acc = 0.0;
+  long long n = 0;
+  for (int s = threadIdx.x; s < slots; s += 256) { acc += part[s]; n += valid[s]; }
+  __shared__ double wsum[8];
+  __shared__ long long wcnt[8];
+  acc = warp_sum_d(acc);
+#pragma unroll
+  for (int o = 16; o; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31) == 0) { wsum[threadIdx.x >> 5] = acc; wcnt[threadIdx.x >> 5] = n; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    long long v = 0;
+    for (int w = 0; w < 8; ++w) { s += wsum[w]; v += wcnt[w]; }
+    float norm = 1.f;
+    if (mode == B2C_LOSS_NORM_FULL) norm = (float)pixels;
+    else if (mode == B2C_LOSS_NORM_VALID) norm = has_ignore ? (float)v : (float)pixels;
+    else if (mode == B2C_LOSS_NORM_BATCH_SIZE) norm = (float)outer;
+    norm = fmaxf(1.f, norm);
+    *normalizer = norm;
+    *loss = (float)s / norm;
+  }
+}
+// dx = (prob - onehot) * s, s = loss_weight / *normalizer rounded once per thread; every channel of an ignored pixel is 0.  An
+// out-of-range label subtracts nothing.  Column route: one thread per pixel column (VEC: four, float4 along inner); row route
+// (inner == 1): one thread per element.
+template <bool VEC>
+__global__ void __launch_bounds__(256)
+softmax_loss_bwd_col_kernel(size_t cols, int C, int inner, const float* __restrict__ prob, const float* __restrict__ labels, int has_ignore,
+                            int ignore_label, const float* __restrict__ normalizer, float loss_weight, float* __restrict__ dx) {
+  pdl_wait();
+  using V = typename std::conditional<VEC, float4, float>::type;
+  const float s = loss_weight / *normalizer;
+  const int w = VEC ? inner / 4 : inner;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cols; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = i / w, base = o * C * w + (i - o * w);
+    const V* p = reinterpret_cast<const V*>(prob) + base;
+    V* d = reinterpret_cast<V*>(dx) + base;
+    if constexpr (VEC) {
+      const float4 lf = reinterpret_cast<const float4*>(labels)[i];
+      const int l0 = (int)lf.x, l1 = (int)lf.y, l2 = (int)lf.z, l3 = (int)lf.w;
+      const bool k0 = !(has_ignore && l0 == ignore_label), k1 = !(has_ignore && l1 == ignore_label),
+                 k2 = !(has_ignore && l2 == ignore_label), k3 = !(has_ignore && l3 == ignore_label);
+      for (int c = 0; c < C; ++c) {
+        const float4 v = p[(size_t)c * w];
+        d[(size_t)c * w] = make_float4(k0 ? __fmul_rn(v.x - (c == l0 ? 1.f : 0.f), s) : 0.f, k1 ? __fmul_rn(v.y - (c == l1 ? 1.f : 0.f), s) : 0.f,
+                                       k2 ? __fmul_rn(v.z - (c == l2 ? 1.f : 0.f), s) : 0.f, k3 ? __fmul_rn(v.w - (c == l3 ? 1.f : 0.f), s) : 0.f);
+      }
+    } else {
+      const int l = (int)labels[i];
+      const bool keep = !(has_ignore && l == ignore_label);
+      for (int c = 0; c < C; ++c) d[(size_t)c * w] = keep ? __fmul_rn(p[(size_t)c * w] - (c == l ? 1.f : 0.f), s) : 0.f;
+    }
+  }
+}
+__global__ void __launch_bounds__(256)
+softmax_loss_bwd_row_kernel(size_t total, int C, const float* __restrict__ prob, const float* __restrict__ labels, int has_ignore,
+                            int ignore_label, const float* __restrict__ normalizer, float loss_weight, float* __restrict__ dx) {
+  pdl_wait();
+  const float s = loss_weight / *normalizer;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t n = i / C;
+    const int c = (int)(i - n * C), l = (int)labels[n];
+    dx[i] = (has_ignore && l == ignore_label) ? 0.f : __fmul_rn(prob[i] - (c == l ? 1.f : 0.f), s);
   }
 }
 // dx = (dy - sum_c dy * y) * y  (softmax_layer.cu: channel dot, channel subtract, multiply by the top).  dx may be dy.
@@ -609,11 +768,6 @@ __device__ __forceinline__ float loss_term(float a, float b, float* d) {
   const float v = a - b;
   *d = v;
   return __fmul_rn(v, v);
-}
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
 }
 // The reduction every loss-sum kernel ends with: each thread's double partial is summed per warp, the warp sums per CTA in warp
 // order, and the CTA sums over the cluster in rank order in rank 0 through distributed shared memory.  Returns the total in rank 0's
@@ -1018,6 +1172,79 @@ extern "C" int b2c_softmax_backward(int outer, int C, int inner, const float* y,
   const size_t cols = (size_t)outer * (vec ? inner / 4 : inner);
   if (vec) launch_pdl(softmax_col_bwd_kernel<true>, grid_for(cols, 256), 256, 0, as_stream(stream), 0, cols, C, inner, y, dy, dx);
   else launch_pdl(softmax_col_bwd_kernel<false>, grid_for(cols, 256), 256, 0, as_stream(stream), 0, cols, C, inner, y, dy, dx);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+struct SoftmaxLossPlan { int route; long long pixels, slots; size_t ws_bytes; };
+// The one place the softmax-loss forward route is chosen: b2c_softmax_loss_forward_ex launches it, the plan query reports it.
+static int softmax_loss_plan(int outer, int C, int inner, const void* logits, const void* prob, SoftmaxLossPlan* pl) {
+  NEED(outer > 0 && C > 0 && inner > 0, "softmax loss: outer, C and inner must be positive");
+  NEED((long long)outer * inner <= (1ll << 62) / C, "softmax loss: tensor too large");
+  pl->pixels = (long long)outer * inner;
+  pl->slots = (pl->pixels + SL_CHUNK - 1) / SL_CHUNK;
+  NEED(pl->slots <= 0x7fffffffLL, "softmax loss: too many pixels");
+  pl->route = inner == 1 ? SL_ROW : inner % 4 == 0 && al16({logits, prob}) ? SL_COL4 : SL_COL;
+  pl->ws_bytes = ((size_t)pl->slots * (sizeof(double) + sizeof(int)) + 15) / 16 * 16;
+  return B2C_OK;
+}
+extern "C" int b2c_softmax_loss_workspace(int outer, int C, int inner, size_t* bytes) {
+  NEED(bytes, "b2c_softmax_loss_workspace: null");
+  SoftmaxLossPlan pl{};
+  if (int rc = softmax_loss_plan(outer, C, inner, nullptr, nullptr, &pl)) return rc;
+  *bytes = pl.ws_bytes;
+  return B2C_OK;
+}
+extern "C" int b2c_debug_softmax_loss_plan(int outer, int C, int inner, const void* logits, const void* prob, int* out, int n) {
+  NEED(out && n >= 4, "b2c_debug_softmax_loss_plan: needs out[4]");
+  SoftmaxLossPlan pl{};
+  if (int rc = softmax_loss_plan(outer, C, inner, logits, prob, &pl)) return rc;
+  out[0] = pl.route; out[1] = SL_CHUNK; out[2] = (int)pl.slots; out[3] = (int)pl.ws_bytes;
+  return B2C_OK;
+}
+extern "C" int b2c_softmax_loss_forward_ex(int outer, int C, int inner, const float* logits, const float* labels, int has_ignore, int ignore_label,
+                                           int norm_mode, float* prob, float* loss, float* normalizer, void* workspace, void* stream) {
+  NEED(logits && labels && prob && loss && normalizer && workspace, "b2c_softmax_loss_forward_ex: null");
+  NEED(norm_mode >= B2C_LOSS_NORM_FULL && norm_mode <= B2C_LOSS_NORM_NONE, "b2c_softmax_loss_forward_ex: Unknown normalization mode");
+  NEED(al16({workspace}), "b2c_softmax_loss_forward_ex: workspace must be 16-byte aligned");
+  SoftmaxLossPlan pl{};
+  if (int rc = softmax_loss_plan(outer, C, inner, logits, prob, &pl)) return rc;
+  cudaStream_t st = as_stream(stream);
+  double* part = static_cast<double*>(workspace);
+  int* valid = reinterpret_cast<int*>(part + pl.slots);
+  const int hi = has_ignore ? 1 : 0;
+  const unsigned grid = (unsigned)pl.slots;
+  if (pl.route == SL_ROW) {
+    launch_pdl(softmax_loss_fwd_kernel, outer, 256, 0, st, 0, C, logits, prob);
+    B2C_POST_LAUNCH();
+    launch_pdl(softmax_loss_chunk_kernel<SL_ROW>, grid, 256, 0, st, 0, pl.pixels, C, inner, logits, labels, hi, ignore_label, prob, part, valid);
+  } else if (pl.route == SL_COL4) {
+    launch_pdl(softmax_loss_chunk_kernel<SL_COL4>, grid, 256, 0, st, 0, pl.pixels, C, inner, logits, labels, hi, ignore_label, prob, part, valid);
+  } else {
+    launch_pdl(softmax_loss_chunk_kernel<SL_COL>, grid, 256, 0, st, 0, pl.pixels, C, inner, logits, labels, hi, ignore_label, prob, part, valid);
+  }
+  B2C_POST_LAUNCH();
+  launch_pdl(softmax_loss_finalize_kernel, 1, 256, 0, st, 0, (int)pl.slots, (long long)outer, pl.pixels, hi, norm_mode,
+             (const double*)part, (const int*)valid, loss, normalizer);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+extern "C" int b2c_softmax_loss_backward_ex(int outer, int C, int inner, const float* prob, const float* labels, int has_ignore, int ignore_label,
+                                            const float* normalizer, float loss_weight, float* dx, void* stream) {
+  NEED(prob && labels && normalizer && dx, "b2c_softmax_loss_backward_ex: null");
+  SoftmaxLossPlan pl{};
+  if (int rc = softmax_loss_plan(outer, C, inner, prob, dx, &pl)) return rc;
+  cudaStream_t st = as_stream(stream);
+  const int hi = has_ignore ? 1 : 0;
+  if (inner == 1) {
+    const size_t total = (size_t)outer * C;
+    launch_pdl(softmax_loss_bwd_row_kernel, grid_for(total, 256), 256, 0, st, 0, total, C, prob, labels, hi, ignore_label, normalizer, loss_weight, dx);
+  } else if (inner % 4 == 0 && al16({prob, labels, dx})) {
+    const size_t cols = (size_t)pl.pixels / 4;
+    launch_pdl(softmax_loss_bwd_col_kernel<true>, grid_for(cols, 256), 256, 0, st, 0, cols, C, inner, prob, labels, hi, ignore_label, normalizer, loss_weight, dx);
+  } else {
+    const size_t cols = (size_t)pl.pixels;
+    launch_pdl(softmax_loss_bwd_col_kernel<false>, grid_for(cols, 256), 256, 0, st, 0, cols, C, inner, prob, labels, hi, ignore_label, normalizer, loss_weight, dx);
+  }
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

@@ -459,6 +459,90 @@ accuracy_kernel(int N, int C, int top_k, const float* __restrict__ scores, const
   if (lane == 0 && above < top_k) atomicAdd(hits, 1u);
 }
 __global__ void accuracy_finish_kernel(const unsigned int* hits, int N, float* acc) { pdl_wait(); *acc = (float)*hits / (float)N; }
+// The [outer, C, inner] form with ignore_label and the per-class counters (b2c_accuracy_ex).  cnt = {hits, counted pixels}, then
+// hits_c[C] and num_c[C] when per-class counting is on (per_class != 0).  Integer atomics: the same counts in any order.
+__device__ __forceinline__ void accuracy_record(int lab, int C, bool hit, int per_class, unsigned int* __restrict__ cnt) {
+  atomicAdd(cnt + 1, 1u);
+  if (hit) atomicAdd(cnt, 1u);
+  if (per_class && lab >= 0 && lab < C) {
+    atomicAdd(cnt + 2 + C + lab, 1u);
+    if (hit) atomicAdd(cnt + 2 + lab, 1u);
+  }
+}
+// inner == 1: one warp per sample, as accuracy_kernel
+__global__ void __launch_bounds__(256)
+accuracy_row_ex_kernel(int N, int C, int top_k, const float* __restrict__ scores, const float* __restrict__ labels, int has_ignore, int ignore_label,
+                       int per_class, unsigned int* __restrict__ cnt) {
+  pdl_wait();
+  const int warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (warp >= N) return;
+  const int lab = (int)labels[warp];
+  if (has_ignore && lab == ignore_label) return;
+  const bool in = lab >= 0 && lab < C;
+  int above = 0;
+  if (in) {
+    const float* z = scores + (size_t)warp * C;
+    const float zl = z[lab];
+    for (int j = lane; j < C; j += 32) { const float v = z[j]; above += (v > zl || (v == zl && j > lab)) ? 1 : 0; }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) above += __shfl_xor_sync(0xffffffffu, above, o);
+  }
+  if (lane == 0) accuracy_record(lab, C, in && above < top_k, per_class, cnt);
+}
+// inner > 1: one thread per pixel column, loads coalesced along inner.  Each thread keeps its hits and count in registers, the warp
+// sums them and adds once per warp; the per-class counters live in shared memory (smem != 0, 8 * C bytes) and each CTA adds its
+// non-zero ones to the global counters at the end, so no global address takes an atomic per pixel.
+__global__ void __launch_bounds__(256)
+accuracy_col_kernel(long long pixels, int C, int inner, int top_k, const float* __restrict__ scores, const float* __restrict__ labels,
+                    int has_ignore, int ignore_label, int per_class, int smem, unsigned int* __restrict__ cnt) {
+  pdl_wait();
+  extern __shared__ unsigned int pc_smem[];                   // hits_c[C], num_c[C]
+  unsigned int* pc = smem ? pc_smem : cnt + 2;
+  if (smem) {
+    for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) pc_smem[c] = 0u;
+    __syncthreads();
+  }
+  unsigned int hits = 0, count = 0;
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < pixels; p += (long long)gridDim.x * blockDim.x) {
+    const int lab = (int)labels[p];
+    if (has_ignore && lab == ignore_label) continue;
+    ++count;
+    if (lab < 0 || lab >= C) continue;                       // out of range: a miss, no class touched
+    const long long o = p / inner;
+    const float* z = scores + (size_t)o * C * inner + (size_t)(p - o * inner);
+    const float zl = z[(size_t)lab * inner];
+    int above = 0;
+    for (int j = 0; j < C; ++j) { const float v = z[(size_t)j * inner]; above += (v > zl || (v == zl && j > lab)) ? 1 : 0; }
+    const bool hit = above < top_k;
+    hits += hit ? 1u : 0u;
+    if (per_class) {
+      atomicAdd(pc + C + lab, 1u);
+      if (hit) atomicAdd(pc + lab, 1u);
+    }
+  }
+  hits = __reduce_add_sync(0xffffffffu, hits);
+  count = __reduce_add_sync(0xffffffffu, count);
+  if ((threadIdx.x & 31) == 0) {
+    if (hits) atomicAdd(cnt, hits);
+    if (count) atomicAdd(cnt + 1, count);
+  }
+  if (smem) {
+    __syncthreads();
+    for (int c = threadIdx.x; c < 2 * C; c += blockDim.x)
+      if (pc_smem[c]) atomicAdd(cnt + 2 + c, pc_smem[c]);
+  }
+}
+// accuracy = hits / count (accuracy_layer.cpp:94, NaN for 0 / 0); per_class[c] = num_c == 0 ? 0 : hits_c / num_c (:95-100)
+__global__ void __launch_bounds__(256)
+accuracy_ex_finish_kernel(int C, const unsigned int* __restrict__ cnt, float* __restrict__ acc, float* __restrict__ per_class) {
+  pdl_wait();
+  if (blockIdx.x == 0 && threadIdx.x == 0) *acc = (float)cnt[0] / (float)cnt[1];
+  if (per_class)
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < C; c += gridDim.x * blockDim.x) {
+      const float num = (float)cnt[2 + C + c];
+      per_class[c] = num == 0.f ? 0.f : (float)cnt[2 + c] / num;
+    }
+}
 
 // the statistics kernel of layers.cu (same launch for the fused and the unfused forward)
 int launch_bn_stats(const BnPlan& p, int N, int C, int S, const float* x, float eps, float maf, int first, float* mean, float* invstd,
@@ -680,6 +764,32 @@ extern "C" int b2c_accuracy(int N, int C, int top_k, const float* scores, const 
   launch_pdl(accuracy_kernel, (N * 32 + 255) / 256, 256, 0, st, 0, N, C, top_k, scores, labels, static_cast<unsigned int*>(scratch));
   B2C_POST_LAUNCH();
   launch_pdl(accuracy_finish_kernel, 1, 1, 0, st, 0, static_cast<const unsigned int*>(scratch), N, accuracy);
+  B2C_POST_LAUNCH();
+  return B2C_OK;
+}
+extern "C" int b2c_accuracy_ex(int outer, int C, int inner, int top_k, const float* scores, const float* labels, int has_ignore, int ignore_label,
+                               float* accuracy, float* per_class, void* scratch, void* stream) {
+  FNEED(scores && labels && accuracy && scratch, "b2c_accuracy_ex: null");
+  FNEED(outer > 0 && C > 0 && inner > 0 && (long long)outer * inner <= (1ll << 62) / C, "b2c_accuracy_ex: bad shape");
+  FNEED(top_k > 0 && top_k <= C, "b2c_accuracy_ex: top_k must be less than or equal to the number of classes.");
+  FNEED(inner > 1 || outer <= 0x7fffffff / 32, "b2c_accuracy_ex: too many samples");
+  int dev_count = 0;
+  if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) return fail(B2C_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
+  cudaStream_t st = as_stream(stream);
+  unsigned int* cnt = static_cast<unsigned int*>(scratch);
+  const int pc = per_class ? 1 : 0;
+  B2C_CUDA_OK(cudaMemsetAsync(scratch, 0, sizeof(unsigned int) * (2 + (pc ? 2 * (size_t)C : 0)), st));
+  const int hi = has_ignore ? 1 : 0;
+  if (inner == 1) {
+    launch_pdl(accuracy_row_ex_kernel, (unsigned)(((long long)outer * 32 + 255) / 256), 256, 0, st, 0, outer, C, top_k, scores, labels, hi, ignore_label, pc, cnt);
+  } else {
+    const long long pixels = (long long)outer * inner;
+    const int smem = pc && C <= 6144 ? 1 : 0;                // per-class counters in shared memory up to the 48 KB default
+    launch_pdl(accuracy_col_kernel, grid_for((size_t)pixels, 256), 256, smem ? 8 * (size_t)C : 0, st, 0, pixels, C, inner, top_k, scores, labels,
+               hi, ignore_label, pc, smem, cnt);
+  }
+  B2C_POST_LAUNCH();
+  launch_pdl(accuracy_ex_finish_kernel, pc ? (C + 255) / 256 : 1, 256, 0, st, 0, C, (const unsigned int*)cnt, accuracy, per_class);
   B2C_POST_LAUNCH();
   return B2C_OK;
 }

@@ -193,7 +193,10 @@ struct ConcatParameter { int axis = 1; };
 struct SliceParameter { int axis = 1; bool slice_dim_given = false; vector<int> slice_point; };   // axis: SliceParameter.axis or slice_dim
 struct SoftmaxParameter { int axis = 1; };
 struct FlattenParameter { int axis = 1, end_axis = -1; };
-struct AccuracyParameter { int top_k = 1; };
+struct AccuracyParameter { int top_k = 1, axis = 1; bool has_ignore_label = false; int ignore_label = 0; };   // Net resolves `axis`
+// caffe.proto LossParameter; normalization: FULL = 0, VALID = 1, BATCH_SIZE = 2, NONE = 3 (b2c_loss_normalization), with the legacy
+// `normalize` already folded in (false: BATCH_SIZE, true: VALID) when `normalization` is absent
+struct LossParameter { bool has_ignore_label = false; int ignore_label = 0; int normalization = 1; };
 struct CropParameter { int axis = 2; vector<int> offset; };   // caffe.proto CropParameter; Net resolves `axis` to a canonical index
 struct ContrastiveLossParameter { float margin = 1.f; bool legacy_version = false; };
 struct TransformationParameter { float scale = 1.f; bool mirror = false; int crop_size = 0; vector<float> mean_value; string mean_file; long long random_seed = -1; };
@@ -220,6 +223,7 @@ struct LayerParameter {
   SoftmaxParameter softmax_param;
   FlattenParameter flatten_param;
   AccuracyParameter accuracy_param;
+  LossParameter loss_param;
   CropParameter crop_param;
   ContrastiveLossParameter contrastive_loss_param;
   TransformationParameter transform_param;

@@ -260,6 +260,27 @@ int b2h_net_layer(void* h, int i, char* name, char* type, int cap, int* naxes, i
   for (size_t k = 0; k < s.size() && k < 8; ++k) top_shape[k] = s[k];
   return 0;
 }
+// top t of layer i: its shape as Net inferred it (-1 when there is no such top)
+int b2h_net_top_shape(void* h, int i, int t, int* naxes, int* top_shape) {
+  Net* n = static_cast<Net*>(h);
+  if (i < 0 || i >= (int)n->layers().size() || t < 0 || t >= (int)n->layers()[i].param.top.size()) return -1;
+  const std::vector<int>& s = n->top_shape(i, t);
+  *naxes = (int)s.size();
+  for (size_t k = 0; k < s.size() && k < 8; ++k) top_shape[k] = s[k];
+  return 0;
+}
+// the class-axis parameters of layer i as the layers read them (axes canonical): out[0] softmax_param.axis, [1] loss_param has
+// ignore_label, [2] its ignore_label, [3] its normalization (b2c_loss_normalization, `normalize` folded in), [4] accuracy_param.axis,
+// [5] top_k, [6] has ignore_label, [7] its ignore_label
+int b2h_net_loss_params(void* h, int i, int* out, int n) {
+  Net* net = static_cast<Net*>(h);
+  if (i < 0 || i >= (int)net->layers().size() || n < 8) return -1;
+  const LayerParameter& p = net->layers()[i].param;
+  const int v[8] = {p.softmax_param.axis, p.loss_param.has_ignore_label, p.loss_param.ignore_label, p.loss_param.normalization,
+                    p.accuracy_param.axis, p.accuracy_param.top_k, p.accuracy_param.has_ignore_label, p.accuracy_param.ignore_label};
+  for (int k = 0; k < 8; ++k) out[k] = v[k];
+  return 0;
+}
 int b2h_net_num_convs(void* h) { return (int)static_cast<Net*>(h)->conv_layers().size(); }
 int b2h_net_conv(void* h, int i, b2c_conv_params* out, int* propagate_down, char* name, int cap) {
   Net* n = static_cast<Net*>(h);

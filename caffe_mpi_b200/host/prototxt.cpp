@@ -264,7 +264,23 @@ LayerParameter read_layer(const PMessage& lp, Phase phase, int batch_override) {
   p.softmax_param.axis = (int)sub("softmax_param").integer("axis", 1);
   p.flatten_param.axis = (int)sub("flatten_param").integer("axis", 1);
   p.flatten_param.end_axis = (int)sub("flatten_param").integer("end_axis", -1);
-  p.accuracy_param.top_k = (int)sub("accuracy_param").integer("top_k", 1);
+  const PMessage& ap = sub("accuracy_param");
+  p.accuracy_param.top_k = (int)ap.integer("top_k", 1);
+  p.accuracy_param.axis = (int)ap.integer("axis", 1);
+  p.accuracy_param.has_ignore_label = ap.has("ignore_label");
+  p.accuracy_param.ignore_label = (int)ap.integer("ignore_label", 0);
+  const PMessage& lsp = sub("loss_param");                     // softmax_loss_layer.cpp:29-40
+  p.loss_param.has_ignore_label = lsp.has("ignore_label");
+  p.loss_param.ignore_label = (int)lsp.integer("ignore_label", 0);
+  if (lsp.has("normalization")) {
+    const std::string nm = lsp.str("normalization");
+    static const char* names[] = {"FULL", "VALID", "BATCH_SIZE", "NONE"};
+    p.loss_param.normalization = -1;
+    for (int i = 0; i < 4; ++i) if (nm == names[i] || nm == std::to_string(i)) p.loss_param.normalization = i;
+    B2_CHECK(p.loss_param.normalization >= 0, "Unknown normalization mode: " + nm);
+  } else if (lsp.has("normalize")) {
+    p.loss_param.normalization = lsp.boolean("normalize", true) ? 1 : 2;
+  }
   p.contrastive_loss_param.margin = (float)sub("contrastive_loss_param").num("margin", 1.0);
   p.contrastive_loss_param.legacy_version = sub("contrastive_loss_param").boolean("legacy_version", false);
   const PMessage& tp = sub("transform_param");
@@ -553,6 +569,24 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
         else B2_CHECK(prod(a) == prod(b), "SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.");
       }
       for (size_t i = 0; i < P.top.size(); ++i) tops.push_back({});
+      if (type == "SoftmaxWithLoss" || type == "Accuracy") {
+        // softmax_loss_layer.cpp:47-61, accuracy_layer.cpp:21-42: the class axis, the [outer, C, inner] view, one label per pixel
+        const std::vector<int>& a = bottom_shape(0);
+        const size_t labels = prod(bottom_shape(1));
+        if (type == "Accuracy")
+          B2_CHECK(labels > 0 && P.accuracy_param.top_k <= (long long)(prod(a) / labels), "top_k must be less than or equal to the number of classes.");
+        int& axis = type == "Accuracy" ? P.accuracy_param.axis : P.softmax_param.axis;
+        axis = canonical_axis(axis, a);
+        const size_t outer = prod(std::vector<int>(a.begin(), a.begin() + axis)), inner = prod(a, axis + 1);
+        // nets of the [N, C] form without ignore_label or a second top are checked by the layers' Reshape, as they always were
+        const bool spatial = inner > 1 || tops.size() > 1 || (type == "Accuracy" ? P.accuracy_param.has_ignore_label : P.loss_param.has_ignore_label);
+        if (spatial && outer * inner != labels)
+          Fatal(__FILE__, __LINE__, "Check failed: outer_num_ * inner_num_ == bottom[1]->count() (" + std::to_string(outer * inner) + " vs. " +
+                                        std::to_string(labels) + ") Number of labels must match number of predictions; e.g., if " +
+                                        (type == "Accuracy" ? "label" : "softmax") + " axis == 1 and prediction shape is (N, C, H, W), label count "
+                                        "(number of labels) must be N*H*W, with integer values in {0, 1, ..., C-1}.");
+        if (tops.size() > 1) tops[1] = type == "Accuracy" ? std::vector<int>{a[axis]} : a;
+      }
     } else if (type == "Slice") {
       SliceParameter& sp = P.slice_param;
       const std::vector<int> bs = bottom_shape(0);

@@ -287,24 +287,46 @@ void SliceLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, co
 }
 
 // ================================================================================================ SoftmaxWithLoss
-void SoftmaxWithLossLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
-  prob_.ReshapeLike(*b[0]);
-  t[0]->Reshape({1});
-}
-void SoftmaxWithLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
-  B2C_CHECK(b2c_softmax_loss_forward(b[0]->shape(0), (int)b[0]->count(1), b[0]->gpu_data(), b[1]->gpu_data(), prob_.mutable_gpu_data(),
-                                     t[0]->mutable_gpu_data(), S()));
-}
-void SoftmaxWithLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
-  if (!pd[0]) return;
-  B2C_CHECK(b2c_softmax_loss_backward(b[0]->shape(0), (int)b[0]->count(1), prob_.gpu_data(), b[1]->gpu_data(), loss_weight(),
-                                      b[0]->mutable_gpu_diff(), S()));
-}
-
-// ================================================================================================ Softmax / Sigmoid / Flatten
 static void softmax_view(Blob* b, int axis, int* outer, int* C, int* inner) {
   *outer = (int)b->count(0, axis); *C = b->shape(axis); *inner = (int)b->count(axis + 1);
 }
+void SoftmaxWithLossLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
+  const LossParameter& q = layer_param_.loss_param;
+  softmax_view(b[0], layer_param_.softmax_param.axis, &outer_, &C_, &inner_);
+  B2_CHECK((size_t)outer_ * inner_ == b[1]->count(), "Number of labels must match number of predictions; e.g., if softmax axis == 1 and "
+           "prediction shape is (N, C, H, W), label count (number of labels) must be N*H*W, with integer values in {0, 1, ..., C-1}.");
+  legacy_ = inner_ == 1 && !q.has_ignore_label && q.normalization != B2C_LOSS_NORM_NONE && t.size() == 1;
+  prob_.ReshapeLike(*b[0]);
+  t[0]->Reshape({1});
+  if (t.size() > 1) t[1]->ReshapeLike(*b[0]);
+  if (!legacy_) {
+    size_t bytes = 0;
+    B2C_CHECK(b2c_softmax_loss_workspace(outer_, C_, inner_, &bytes));
+    workspace_.Reshape({(int)(bytes / sizeof(float))});
+    normalizer_.Reshape({1});
+  }
+}
+void SoftmaxWithLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  const LossParameter& q = layer_param_.loss_param;
+  if (legacy_)
+    B2C_CHECK(b2c_softmax_loss_forward(outer_, C_, b[0]->gpu_data(), b[1]->gpu_data(), prob_.mutable_gpu_data(), t[0]->mutable_gpu_data(), S()));
+  else
+    B2C_CHECK(b2c_softmax_loss_forward_ex(outer_, C_, inner_, b[0]->gpu_data(), b[1]->gpu_data(), q.has_ignore_label ? 1 : 0, q.ignore_label,
+                                          q.normalization, prob_.mutable_gpu_data(), t[0]->mutable_gpu_data(), normalizer_.mutable_gpu_data(),
+                                          workspace_.mutable_gpu_data(), S()));
+  if (t.size() > 1) t[1]->ShareData(prob_);
+}
+void SoftmaxWithLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0]) return;
+  const LossParameter& q = layer_param_.loss_param;
+  if (legacy_)
+    B2C_CHECK(b2c_softmax_loss_backward(outer_, C_, prob_.gpu_data(), b[1]->gpu_data(), loss_weight(), b[0]->mutable_gpu_diff(), S()));
+  else
+    B2C_CHECK(b2c_softmax_loss_backward_ex(outer_, C_, inner_, prob_.gpu_data(), b[1]->gpu_data(), q.has_ignore_label ? 1 : 0, q.ignore_label,
+                                           normalizer_.gpu_data(), loss_weight(), b[0]->mutable_gpu_diff(), S()));
+}
+
+// ================================================================================================ Softmax / Sigmoid / Flatten
 void SoftmaxLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   int outer, C, inner;
   softmax_view(b[0], layer_param_.softmax_param.axis, &outer, &C, &inner);
@@ -391,9 +413,24 @@ void ContrastiveLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>
 }
 
 // ================================================================================================ Accuracy
+void AccuracyLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
+  const AccuracyParameter& q = layer_param_.accuracy_param;
+  B2_CHECK(q.top_k <= (int)(b[0]->count() / b[1]->count()), "top_k must be less than or equal to the number of classes.");
+  softmax_view(b[0], q.axis, &outer_, &C_, &inner_);
+  B2_CHECK((size_t)outer_ * inner_ == b[1]->count(), "Number of labels must match number of predictions; e.g., if label axis == 1 and "
+           "prediction shape is (N, C, H, W), label count (number of labels) must be N*H*W, with integer values in {0, 1, ..., C-1}.");
+  legacy_ = inner_ == 1 && !q.has_ignore_label && t.size() == 1;
+  t[0]->Reshape({1});
+  if (t.size() > 1) t[1]->Reshape({C_});
+  hits_.Reshape({legacy_ ? 1 : 2 + (t.size() > 1 ? 2 * C_ : 0)});        // b2c_accuracy_ex's scratch: 8 + 8 * C bytes with the per-class top
+}
 void AccuracyLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
-  B2C_CHECK(b2c_accuracy(b[0]->shape(0), (int)b[0]->count(1), layer_param_.accuracy_param.top_k, b[0]->gpu_data(), b[1]->gpu_data(), t[0]->mutable_gpu_data(),
-                         hits_.mutable_gpu_data(), S()));
+  const AccuracyParameter& q = layer_param_.accuracy_param;
+  if (legacy_)
+    B2C_CHECK(b2c_accuracy(outer_, C_, q.top_k, b[0]->gpu_data(), b[1]->gpu_data(), t[0]->mutable_gpu_data(), hits_.mutable_gpu_data(), S()));
+  else
+    B2C_CHECK(b2c_accuracy_ex(outer_, C_, inner_, q.top_k, b[0]->gpu_data(), b[1]->gpu_data(), q.has_ignore_label ? 1 : 0, q.ignore_label,
+                              t[0]->mutable_gpu_data(), t.size() > 1 ? t[1]->mutable_gpu_data() : nullptr, hits_.mutable_gpu_data(), S()));
 }
 
 // ================================================================================================ synthetic data
@@ -634,8 +671,9 @@ vector<ParamSpec> TrainNet::BuildNodes(const Net& net, int num_classes, uint64_t
       node.propagate_down.push_back(node.need_backward && L.propagate_down[i]);
     }
     // the reference refuses at backward time (sigmoid_cross_entropy_loss_layer.cpp:52-55); here the graph is known up front
-    B2_CHECK(!(type == "SigmoidCrossEntropyLoss" && node.need_backward && L.label_wants_gradient),
-             "SigmoidCrossEntropyLoss Layer cannot backpropagate to label inputs.");
+    // (softmax_loss_layer.cpp:128-130 likewise)
+    B2_CHECK(!((type == "SigmoidCrossEntropyLoss" || type == "SoftmaxWithLoss") && node.need_backward && L.label_wants_gradient),
+             type + " Layer cannot backpropagate to label inputs.");
     node.bottom_diff_tmp.assign(node.bottom.size(), nullptr);
     layers_.push_back(layer);
     layer_names_.push_back(L.param.name);

@@ -171,6 +171,10 @@ class SliceLayer : public LayerBase {
   vector<vector<int>> shapes_;
 };
 
+// softmax_loss_layer.cpp over the [outer, C, inner] view of softmax_param.axis (canonical: Net resolved it), with loss_param's
+// ignore_label and normalization; top 1 (optional) shares prob_.  The legacy case -- inner == 1, no ignore_label, a normalizer of
+// outer (VALID, FULL or BATCH_SIZE), one top -- runs b2c_softmax_loss_forward / _backward with the arguments it always had; every
+// other case b2c_softmax_loss_forward_ex / _backward_ex, with the normalizer kept on the device between the two.
 class SoftmaxWithLossLayer : public LayerBase {
  public:
   using LayerBase::LayerBase;
@@ -179,7 +183,9 @@ class SoftmaxWithLossLayer : public LayerBase {
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
-  Blob prob_;
+  Blob prob_, workspace_, normalizer_;
+  int outer_ = 0, C_ = 0, inner_ = 0;
+  bool legacy_ = true;
 };
 
 // ---- layers the deploy / TEST nets and the MNIST autoencoder add (softmax_layer, sigmoid_layer, flatten_layer, euclidean_loss_layer,
@@ -268,18 +274,20 @@ class ContrastiveLossLayer : public LayerBase {
   Blob diff_, dist_sq_;
 };
 
-class AccuracyLayer : public LayerBase {       // forward only (accuracy_layer.cpp); top[0] is a scalar
+// forward only (accuracy_layer.cpp) over the [outer, C, inner] view of accuracy_param.axis (canonical); top[0] is a scalar, top[1]
+// (optional) the per-class accuracy [C].  The legacy case -- inner == 1, no ignore_label, one top -- runs b2c_accuracy as it always
+// did; every other case b2c_accuracy_ex.
+class AccuracyLayer : public LayerBase {
  public:
   using LayerBase::LayerBase;
   const char* type() const override { return "Accuracy"; }
-  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override {
-    B2_CHECK(layer_param_.accuracy_param.top_k <= (int)(b[0]->count() / b[1]->count()), "top_k must be less than or equal to the number of classes.");
-    t[0]->Reshape({1}); hits_.Reshape({1});
-  }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
  protected:
   void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
   void Backward_gpu(const vector<Blob*>&, const vector<bool>&, const vector<Blob*>&) override {}   // "Accuracy cannot backpropagate"
   Blob hits_;
+  int outer_ = 0, C_ = 0, inner_ = 0;
+  bool legacy_ = true;
 };
 
 // Synthetic in-memory source standing in for DataLayer's LMDB reader (SURVEY 8d / 8f rank 4).  Two forms:

@@ -252,6 +252,24 @@ class Net:
             out.append((nm.value.decode(), ty.value.decode(), tuple(shp[k] for k in range(na.value))))
         return out
 
+    def top_shape(self, layer, top):
+        """The shape Net inferred for top `top` of layer `layer`."""
+        L = lib()
+        L.b2h_net_top_shape.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        na, shp = C.c_int(), (C.c_int * 8)()
+        _ck(L.b2h_net_top_shape(self._h, layer, top, C.byref(na), shp))
+        return tuple(shp[k] for k in range(na.value))
+
+    def loss_params(self, layer):
+        """The class-axis parameters of a layer: softmax_param.axis, loss_param (ignore_label or None, normalization name) and
+        accuracy_param (axis, top_k, ignore_label or None), axes canonical."""
+        L = lib()
+        L.b2h_net_loss_params.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_int]
+        o = (C.c_int * 8)()
+        _ck(L.b2h_net_loss_params(self._h, layer, o, 8))
+        return {"softmax_axis": o[0], "ignore_label": o[2] if o[1] else None, "normalization": capi.LOSS_NORMS[o[3]],
+                "accuracy_axis": o[4], "top_k": o[5], "accuracy_ignore_label": o[7] if o[6] else None}
+
     def conv_layers(self):
         L = lib()
         L.b2h_net_conv.argtypes = [C.c_void_p, C.c_int, C.POINTER(capi.ConvParams), C.POINTER(C.c_int), C.c_char_p, C.c_int]

@@ -329,6 +329,44 @@ int b2c_add(size_t n, const float* a, const float* b, float* y, void* stream);
  * forward writes prob [N,C] and *loss (device scalar); backward writes dx = (prob - onehot) * loss_weight / N.       */
 int b2c_softmax_loss_forward(int N, int C, const float* logits, const float* labels, float* prob, float* loss, void* stream);
 int b2c_softmax_loss_backward(int N, int C, const float* prob, const float* labels, float loss_weight, float* dx, void* stream);
+/* SoftmaxWithLossLayer over an [outer, C, inner] view (softmax_loss_layer.cpp:44-160): one softmax over C per (outer, inner)
+ * pixel, LossParameter.ignore_label and .normalization (caffe.proto NormalizationMode).  labels[outer * inner] are float class ids
+ * read as (int).  A pixel whose label equals ignore_label (has_ignore != 0) adds no term and is not counted.
+ * Forward: prob as b2c_softmax_forward on the same logits, bit for bit; *loss (device) = (float)S / norm with S = the sum over the
+ * counted pixels of -log(max(prob[label], FLT_MIN)), taken in double in a fixed order: pixels in chunks of 1024, one double per
+ * chunk (its threads' four-pixel sums in a fixed tree), the chunks in index order.  The bits depend on the shape and the data
+ * only, never on the device or the alignment.  norm (get_normalizer, floored at 1): FULL outer * inner; VALID the counted
+ * pixels when has_ignore, else outer * inner; BATCH_SIZE outer; NONE 1.  *normalizer (device float) receives it for the backward;
+ * nothing is read back to the host.  workspace: b2c_softmax_loss_workspace bytes of device memory, 16-byte aligned.
+ * Backward: dx = (prob - onehot) * s with s = loss_weight / *normalizer rounded once; every channel of an ignored pixel is 0.
+ * A label that is not ignored and lies outside [0, C): the forward reads class min(max(label, 0), C - 1) and the backward
+ * subtracts nothing, so no access leaves the tensors (the reference DCHECKs the range).
+ * Routes (b2c_debug_softmax_loss_plan): inner == 1 the row kernel of b2c_softmax_loss_forward, then a masked pass over the rows;
+ * inner > 1 one fused pass, a thread per pixel column, four columns as float4 when inner % 4 == 0 and logits, prob are 16-byte
+ * aligned.  The backward takes float4 along inner when inner % 4 == 0 and prob, labels, dx are aligned.
+ * outer, C, inner >= 1 and outer * C * inner < 2^62, else B2C_ERR_INVALID. */
+typedef enum {
+  B2C_LOSS_NORM_FULL = 0, B2C_LOSS_NORM_VALID = 1, B2C_LOSS_NORM_BATCH_SIZE = 2, B2C_LOSS_NORM_NONE = 3
+} b2c_loss_normalization;
+typedef enum { B2C_SOFTMAX_LOSS_ROUTE_ROW = 0, B2C_SOFTMAX_LOSS_ROUTE_COLUMN = 1, B2C_SOFTMAX_LOSS_ROUTE_COLUMN_F4 = 2 } b2c_softmax_loss_route;
+int b2c_softmax_loss_workspace(int outer, int C, int inner, size_t* bytes);
+int b2c_softmax_loss_forward_ex(int outer, int C, int inner, const float* logits, const float* labels, int has_ignore, int ignore_label,
+                                int norm_mode, float* prob, float* loss, float* normalizer, void* workspace, void* stream);
+int b2c_softmax_loss_backward_ex(int outer, int C, int inner, const float* prob, const float* labels, int has_ignore, int ignore_label,
+                                 const float* normalizer, float loss_weight, float* dx, void* stream);
+/* The forward route b2c_softmax_loss_forward_ex takes with logits and prob at these addresses (only tested for alignment):
+ * out[0] route (b2c_softmax_loss_route), [1] pixels per chunk, [2] chunks (the workspace's slots), [3] workspace bytes.  Needs
+ * n >= 4.  Refuses what the entry points refuse.  Pure host computation. */
+int b2c_debug_softmax_loss_plan(int outer, int C, int inner, const void* logits, const void* prob, int* out, int n);
+/* AccuracyLayer over an [outer, C, inner] view (accuracy_layer.cpp:21-101) with AccuracyParameter.ignore_label and the per-class
+ * top.  A pixel is a hit when fewer than top_k classes rank above its label in the order of std::greater<pair<score, index>> (on
+ * equal scores the larger index ranks first).  Pixels whose label is ignored are skipped; a label outside [0, C) that is not
+ * ignored is counted as a miss and touches no per-class counter.  *accuracy = hits / counted pixels (NaN when none is counted,
+ * as the reference's accuracy / count); per_class[c] (may be null) = hits_c / pixels labelled c, or 0 when none is.  Counts are
+ * integers: the result is exact and the same on every call.  scratch: 8 + 8 * C bytes of device memory (8 without per_class).
+ * top_k in [1, C]. */
+int b2c_accuracy_ex(int outer, int C, int inner, int top_k, const float* scores, const float* labels, int has_ignore, int ignore_label,
+                    float* accuracy, float* per_class, void* scratch, void* stream);
 /* SoftmaxLayer (src/caffe/layers/softmax_layer.cpp / .cu): softmax over the C axis of an [outer, C, inner] view.  inner == 1
  * runs b2c_softmax_loss_forward's row kernel, so y is bit-identical to its prob.  Backward: dx = (dy - sum_c dy * y) * y.  Both
  * may run in place (y == x; dx == dy).  Alignment as b2c_relu_forward (the float4 path takes four columns when inner % 4 == 0). */
