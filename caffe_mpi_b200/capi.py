@@ -26,6 +26,8 @@ DECONV_ROUTES = ("dual", "phase", "depthwise")
 # b2c_softmax_loss_route and b2c_loss_normalization, in enum order
 SOFTMAX_LOSS_ROUTES = ("row", "column", "column_f4")
 LOSS_NORMS = ("FULL", "VALID", "BATCH_SIZE", "NONE")
+# b2c_neuron_kind, in enum order
+NEURON_KINDS = ("ELU", "POWER", "ABSVAL", "BNLL", "EXP", "LOG", "THRESHOLD")
 
 
 class B2CError(RuntimeError):
@@ -166,6 +168,12 @@ def lib():
         "b2c_softmax_backward": (i, [i, i, i, vp, vp, vp, vp]),
         "b2c_sigmoid_forward": (i, [sz, vp, vp, vp]),
         "b2c_sigmoid_backward": (i, [sz, vp, vp, vp, vp]),
+        "b2c_neuron_forward": (i, [i, sz, vp, vp, f, f, f, vp]),
+        "b2c_neuron_backward": (i, [i, sz, vp, vp, vp, vp, f, f, f, vp]),
+        "b2c_prelu_forward": (i, [i, i, i, i, vp, vp, vp, vp, vp]),
+        "b2c_prelu_workspace_bytes": (i, [i, i, i, i, C.POINTER(sz)]),
+        "b2c_prelu_backward": (i, [i, i, i, i, vp, vp, vp, vp, vp, vp, sz, vp]),
+        "b2c_debug_neuron_plan": (i, [i, i, i, i, i, i, C.POINTER(vp), i, C.POINTER(i), i]),
         "b2c_sigmoid_ce_loss_forward": (i, [i, sz, vp, vp, vp, vp]),
         "b2c_sigmoid_ce_loss_backward": (i, [sz, vp, vp, f, vp, vp]),
         "b2c_euclidean_loss_forward": (i, [i, sz, vp, vp, vp, vp, vp]),
@@ -524,6 +532,50 @@ def accuracy_ex(outer, Cc, inner, top_k, scores, labels, accuracy, per_class, sc
     """b2c_accuracy_ex; per_class may be None; scratch holds 8 + 8 * Cc bytes (8 without per_class)."""
     check(lib().b2c_accuracy_ex(outer, Cc, inner, top_k, _p(scores), _p(labels), int(ignore_label is not None), int(ignore_label or 0),
                                 _p(accuracy), _p(per_class), _p(scratch), _stream(stream)))
+
+
+def neuron_forward(kind, x, y, p=(0.0, 0.0, 0.0), stream=None):
+    """b2c_neuron_forward on torch CUDA tensors; kind one of NEURON_KINDS; p the kind's (p0, p1, p2)."""
+    p = tuple(p) + (0.0,) * (3 - len(p))
+    check(lib().b2c_neuron_forward(NEURON_KINDS.index(kind), x.numel(), _p(x), _p(y), *p, _stream(stream)))
+
+
+def neuron_backward(kind, x, y, dy, dx, p=(0.0, 0.0, 0.0), stream=None):
+    """b2c_neuron_backward; x / y may be None where the kind's rule does not read them."""
+    p = tuple(p) + (0.0,) * (3 - len(p))
+    check(lib().b2c_neuron_backward(NEURON_KINDS.index(kind), dy.numel(), _p(x), _p(y), _p(dy), _p(dx), *p, _stream(stream)))
+
+
+def prelu_forward(N, Cc, dim, shared, x, slope, y, x_keep=None, stream=None):
+    check(lib().b2c_prelu_forward(N, Cc, dim, int(bool(shared)), _p(x), _p(slope), _p(y), _p(x_keep), _stream(stream)))
+
+
+def prelu_workspace_bytes(N, Cc, dim, shared):
+    n = C.c_size_t()
+    check(lib().b2c_prelu_workspace_bytes(N, Cc, dim, int(bool(shared)), C.byref(n)))
+    return n.value
+
+
+def prelu_backward(N, Cc, dim, shared, x, dy, slope, dx, dslope, workspace=None, stream=None):
+    """b2c_prelu_backward; dx and dslope may be None; dslope is added into.  workspace: a torch uint8 / float tensor of at least
+    prelu_workspace_bytes, or None when that is 0."""
+    nbytes = 0 if workspace is None else workspace.numel() * workspace.element_size()
+    check(lib().b2c_prelu_backward(N, Cc, dim, int(bool(shared)), _p(x), _p(dy), _p(slope), _p(dx), _p(dslope), _p(workspace), nbytes,
+                                   _stream(stream)))
+
+
+NEURON_PLAN_OPS = ("forward", "backward", "prelu_forward", "prelu_backward")
+
+
+def neuron_plan(op, N, Cc=1, dim=1, shared=False, kind="ELU", ptrs=()):
+    """b2c_debug_neuron_plan: the launch of an elementwise neuron call over N values (op "forward" / "backward") or of a PReLU call
+    (op "prelu_forward" / "prelu_backward") with the call's tensor pointers (ints, None for a null one) tested for alignment only."""
+    out = (C.c_int * 7)()
+    arr = (C.c_void_p * max(1, len(ptrs)))(*[p or None for p in ptrs])
+    check(lib().b2c_debug_neuron_plan(NEURON_PLAN_OPS.index(op), NEURON_KINDS.index(kind), N, Cc, dim, int(bool(shared)), arr, len(ptrs),
+                                      out, 7))
+    return dict(vec=bool(out[0]), ctas=out[1], threads=out[2], blocks_per_channel=out[3], stripe=out[4], channels=out[5],
+                workspace=out[6])
 
 
 def bn_plan(dir, form, N, Cc, S, ptrs=()):

@@ -141,7 +141,7 @@ void Fill(const FillerParameter& f, Blob* b) {
   float* d = b->mutable_cpu_data();
   const size_t n = b->count();
   std::mt19937& rng = Caffe::rng();
-  const int fan_in = (int)(n / std::max(1, b->shape(0)));
+  const int fan_in = (int)(n / std::max(1, b->num_axes() > 0 ? b->shape(0) : 1));   // a 0-axis blob (count 1) has fan-in 1
   const int fan_out = b->num_axes() > 1 ? (int)(n / std::max(1, b->shape(1))) : (int)n;
   float nval = (float)fan_in;                          // FAN_IN
   if (f.variance_norm == 2) nval = (fan_in + fan_out) / 2.f;   // AVERAGE

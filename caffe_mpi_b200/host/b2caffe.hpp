@@ -186,6 +186,14 @@ struct BatchNormParameter {     // NVCaffe's; a scale_filler or bias_filler impl
   bool scale_bias = false; float eps = 1e-5f, moving_average_fraction = 0.999f; FillerParameter scale_filler{"constant", 1.f}, bias_filler;
 };
 struct ReLUParameter { float negative_slope = 0.f; };
+// caffe.proto's PReLUParameter (filler: constant 0.25 when absent), ELUParameter, PowerParameter, ExpParameter, LogParameter and
+// ThresholdParameter, with their defaults (base -1: e)
+struct PReLUParameter { FillerParameter filler{"constant", 0.25f}; bool channel_shared = false; };
+struct ELUParameter { float alpha = 1.f; };
+struct PowerParameter { float power = 1.f, scale = 1.f, shift = 0.f; };
+struct ExpParameter { float base = -1.f, scale = 1.f, shift = 0.f; };
+struct LogParameter { float base = -1.f, scale = 1.f, shift = 0.f; };
+struct ThresholdParameter { float threshold = 0.f; };
 struct LRNParameter { int local_size = 5; float alpha = 1.f, beta = 0.75f, k = 1.f; int norm_region = 0; };   // ACROSS_CHANNELS = 0, WITHIN_CHANNEL = 1
 struct DropoutParameter { float dropout_ratio = 0.5f; };
 struct EltwiseParameter { int operation = 1; vector<float> coeff; };   // PROD = 0, SUM = 1, MAX = 2
@@ -215,6 +223,12 @@ struct LayerParameter {
   InnerProductParameter inner_product_param;
   BatchNormParameter batch_norm_param;
   ReLUParameter relu_param;
+  PReLUParameter prelu_param;
+  ELUParameter elu_param;
+  PowerParameter power_param;
+  ExpParameter exp_param;
+  LogParameter log_param;
+  ThresholdParameter threshold_param;
   LRNParameter lrn_param;
   DropoutParameter dropout_param;
   EltwiseParameter eltwise_param;

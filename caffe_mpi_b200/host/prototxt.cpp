@@ -243,6 +243,16 @@ LayerParameter read_layer(const PMessage& lp, Phase phase, int batch_override) {
   if (bp.has("scale_filler")) bn.scale_filler = filler_of(bp.sub("scale_filler"));
   if (bp.has("bias_filler")) bn.bias_filler = filler_of(bp.sub("bias_filler"));
   p.relu_param.negative_slope = (float)sub("relu_param").num("negative_slope", 0.0);
+  if (sub("prelu_param").has("filler")) p.prelu_param.filler = filler_of(sub("prelu_param").sub("filler"));
+  p.prelu_param.channel_shared = sub("prelu_param").boolean("channel_shared", false);
+  p.elu_param.alpha = (float)sub("elu_param").num("alpha", 1.0);
+  const PMessage& pw = sub("power_param");
+  p.power_param.power = (float)pw.num("power", 1.0); p.power_param.scale = (float)pw.num("scale", 1.0); p.power_param.shift = (float)pw.num("shift", 0.0);
+  const PMessage& ep = sub("exp_param");
+  p.exp_param.base = (float)ep.num("base", -1.0); p.exp_param.scale = (float)ep.num("scale", 1.0); p.exp_param.shift = (float)ep.num("shift", 0.0);
+  const PMessage& lg = sub("log_param");
+  p.log_param.base = (float)lg.num("base", -1.0); p.log_param.scale = (float)lg.num("scale", 1.0); p.log_param.shift = (float)lg.num("shift", 0.0);
+  p.threshold_param.threshold = (float)sub("threshold_param").num("threshold", 0.0);
   const PMessage& lrn = sub("lrn_param");
   LRNParameter& l = p.lrn_param;
   l.local_size = (int)lrn.integer("local_size", 5); l.alpha = (float)lrn.num("alpha", 1.0); l.beta = (float)lrn.num("beta", 0.75);
@@ -651,8 +661,19 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       // not in the reference, which reads bottom[2][i] for every pair without checking: one label per pair
       B2_CHECK(!y.empty() && y[0] == a[0], "ContrastiveLoss: the similarity blob needs one label per pair");
       for (size_t i = 0; i < P.top.size(); ++i) tops.push_back({});
+    } else if (type == "PReLU") {
+      const std::vector<int>& bs = bottom_shape(0);
+      B2_CHECK(bs.size() >= 2, "Number of axes of bottom blob must be >=2.");                              // prelu_layer.cpp:12-13
+      tops.push_back(bs);
+      // blobs_[0]: the negative slopes, one per channel, or a 0-axis blob (count 1) when channel_shared (prelu_layer.cpp:20-25)
+      blobs.push_back({P.prelu_param.channel_shared ? std::vector<int>{} : std::vector<int>{bs[1]}, 0});
+    } else if (type == "Exp" || type == "Log") {
+      const float base = type == "Exp" ? P.exp_param.base : P.log_param.base;
+      B2_CHECK(base == -1.f || base > 0.f, "base must be strictly positive.");                            // exp_layer.cpp:13-15, log_layer.cpp:13-15
+      tops.push_back(bottom_shape(0));
     } else if (type == "ReLU" || type == "Dropout" || type == "LRN" || type == "Eltwise" || type == "Sigmoid" ||
-               type == "TanH" || type == "Power" || type == "Bias" || type == "ELU" || type == "PReLU" || type == "Split") {
+               type == "TanH" || type == "Power" || type == "Bias" || type == "ELU" || type == "Split" || type == "AbsVal" ||
+               type == "BNLL" || type == "Threshold") {
       for (size_t i = 0; i < std::max<size_t>(1, P.top.size()); ++i) tops.push_back(bottom_shape(0));
     } else {
       Fatal(__FILE__, __LINE__, "Unknown layer type: " + type + " (layer '" + P.name + "')");

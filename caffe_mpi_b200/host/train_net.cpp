@@ -3,6 +3,7 @@
 #include "proto_wire.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <cstdlib>
 #include <set>
@@ -359,6 +360,113 @@ void SigmoidLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, 
   if (!pd[0]) return;
   B2C_CHECK(b2c_sigmoid_backward(t[0]->count(), t[0]->gpu_data(), t[0]->gpu_diff(), b[0]->mutable_gpu_diff(), S()));
 }
+
+// ================================================================================================ NeuronLayer / PReLU
+NeuronLayer::NeuronLayer(const LayerParameter& p) : LayerBase(p) {
+  const string& t = p.type;
+  if (t == "ELU") {
+    kind_ = B2C_NEURON_ELU;
+    fwd_[0] = bwd_[0] = p.elu_param.alpha;
+  } else if (t == "Power") {                              // power_layer.cpp:9-16 (diff_scale = power * scale: the kernel rounds it)
+    kind_ = B2C_NEURON_POWER;
+    fwd_[0] = bwd_[0] = p.power_param.power; fwd_[1] = bwd_[1] = p.power_param.scale; fwd_[2] = bwd_[2] = p.power_param.shift;
+  } else if (t == "AbsVal") {
+    kind_ = B2C_NEURON_ABSVAL;
+  } else if (t == "BNLL") {
+    kind_ = B2C_NEURON_BNLL;
+  } else if (t == "Exp") {                                // exp_layer.cpp:9-29
+    kind_ = B2C_NEURON_EXP;
+    const ExpParameter& q = p.exp_param;
+    B2_CHECK(q.base == -1.f || q.base > 0.f, "base must be strictly positive.");
+    const float log_base = q.base == -1.f ? 1.f : std::log(q.base);
+    B2_CHECK(!std::isnan(log_base) && !std::isinf(log_base), "NaN / Inf result: log(base)");
+    const float inner = log_base * q.scale;
+    const float outer = q.shift == 0.f ? 1.f : (q.base != -1.f ? std::pow(q.base, q.shift) : std::exp(q.shift));
+    fwd_[0] = bwd_[0] = inner;
+    fwd_[1] = outer;
+  } else if (t == "Log") {                                // log_layer.cpp:9-35
+    kind_ = B2C_NEURON_LOG;
+    const LogParameter& q = p.log_param;
+    B2_CHECK(q.base == -1.f || q.base > 0.f, "base must be strictly positive.");
+    const float log_base = q.base == -1.f ? 1.f : std::log(q.base);
+    B2_CHECK(!std::isnan(log_base) && !std::isinf(log_base), "NaN / Inf result: log(base)");
+    const float base_scale = 1.f / log_base;
+    B2_CHECK(!std::isnan(base_scale) && !std::isinf(base_scale), "NaN / Inf result: 1/log(base)");
+    fwd_[0] = bwd_[0] = q.scale; fwd_[1] = bwd_[1] = q.shift;
+    fwd_[2] = base_scale;
+    bwd_[2] = q.scale / log_base;                         // backward_num_scale
+  } else if (t == "Threshold") {
+    kind_ = B2C_NEURON_THRESHOLD;
+    fwd_[0] = p.threshold_param.threshold;
+  } else {
+    B2_CHECK(false, "NeuronLayer: unknown type " + t);
+  }
+}
+void NeuronLayer::LayerSetUp(const vector<Blob*>& b, const vector<Blob*>& t) {
+  if (kind_ == B2C_NEURON_ABSVAL) B2_CHECK(t[0] != b[0], "AbsVal Layer does not allow in-place computation.");   // absval_layer.cpp:10-11
+}
+bool NeuronLayer::backward_reads_bottom() const {
+  switch (kind_) {
+    case B2C_NEURON_ABSVAL: case B2C_NEURON_BNLL: case B2C_NEURON_LOG: return true;
+    case B2C_NEURON_POWER: {
+      const float power = bwd_[0], diff_scale = bwd_[0] * bwd_[1];
+      return !(diff_scale == 0.f || power == 1.f);       // the constant branch reads neither x nor y
+    }
+    default: return false;                                // ELU: in place the top stands in for x (same sign for alpha >= 0); Exp reads y
+  }
+}
+void NeuronLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2C_CHECK(b2c_neuron_forward(kind_, b[0]->count(), b[0]->gpu_data(), t[0]->mutable_gpu_data(), fwd_[0], fwd_[1], fwd_[2], S()));
+}
+void NeuronLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
+  if (!pd[0]) return;
+  B2_CHECK(kind_ != B2C_NEURON_THRESHOLD, "Threshold Layer has no backward.");
+  B2C_CHECK(b2c_neuron_backward(kind_, b[0]->count(), b[0]->gpu_data(), t[0]->gpu_data(), t[0]->gpu_diff(), b[0]->mutable_gpu_diff(), bwd_[0],
+                                bwd_[1], bwd_[2], S()));
+}
+void PReLULayer::view(const Blob* b, int* N, int* C, int* dim) const {
+  *N = b->shape(0); *C = b->shape(1); *dim = (int)b->count(2);
+}
+void PReLULayer::LayerSetUp(const vector<Blob*>& b, const vector<Blob*>&) {
+  B2_CHECK(b[0]->num_axes() >= 2, "Number of axes of bottom blob must be >=2.");   // prelu_layer.cpp:12-38
+  const PReLUParameter& q = layer_param_.prelu_param;
+  blobs_.resize(1);
+  blobs_[0].reset(new Blob(q.channel_shared ? vector<int>{} : vector<int>{b[0]->shape(1)}));
+  Fill(q.filler, blobs_[0].get());
+  param_propagate_down_.assign(1, true);
+}
+void PReLULayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2_CHECK(b[0]->num_axes() >= 2, "Number of axes of bottom blob must be >=2.");
+  if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]);
+  if (keep_bottom_) x_keep_.ReshapeLike(*b[0]);
+  int N, C, dim;
+  view(b[0], &N, &C, &dim);
+  size_t bytes = 0;
+  B2C_CHECK(b2c_prelu_workspace_bytes(N, C, dim, layer_param_.prelu_param.channel_shared ? 1 : 0, &bytes));
+  if (bytes != workspace_bytes_) {            // b2c_prelu_backward wants its counters zero once; every call leaves them so
+    workspace_bytes_ = bytes;
+    workspace_.Reshape({(int)((bytes + sizeof(float) - 1) / sizeof(float))});
+    if (bytes) CUDA_CHECK(cudaMemsetAsync(workspace_.mutable_gpu_data(), 0, bytes, S()));
+  }
+}
+void PReLULayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  int N, C, dim;
+  view(b[0], &N, &C, &dim);
+  B2C_CHECK(b2c_prelu_forward(N, C, dim, layer_param_.prelu_param.channel_shared ? 1 : 0, b[0]->gpu_data(), blobs_[0]->gpu_data(),
+                              t[0]->mutable_gpu_data(), keep_bottom_ ? x_keep_.mutable_gpu_data() : nullptr, S()));
+}
+void PReLULayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) {
+  const bool dslope = param_propagate_down_[0];
+  if (!pd[0] && !dslope) return;
+  int N, C, dim;
+  view(b[0], &N, &C, &dim);
+  // in place: the backward reads the x the forward kept; dx is written over dy element by element (top diff == bottom diff)
+  const float* x = keep_bottom_ ? x_keep_.gpu_data() : b[0]->gpu_data();
+  B2C_CHECK(b2c_prelu_backward(N, C, dim, layer_param_.prelu_param.channel_shared ? 1 : 0, x, t[0]->gpu_diff(), blobs_[0]->gpu_data(),
+                               pd[0] ? b[0]->mutable_gpu_diff() : nullptr, dslope ? blobs_[0]->mutable_gpu_diff() : nullptr,
+                               workspace_.count() ? workspace_.mutable_gpu_data() : nullptr, sizeof(float) * workspace_.count(), S()));
+}
+
 void FlattenLayer::Reshape(const vector<Blob*>& b, const vector<Blob*>& t) {
   B2_CHECK(t[0] != b[0], "Flatten Layer does not allow in-place computation.");
   t[0]->Reshape(shape_);
@@ -566,6 +674,8 @@ static shared_ptr<LayerBase> CreateLayer(const LayerParameter& p, const vector<v
   if (t == "ContrastiveLoss") return std::make_shared<ContrastiveLossLayer>(p);
   if (t == "Deconvolution") return LayerRegistry::CreateLayer(p);
   if (t == "Crop") return std::make_shared<CropLayer>(p);
+  if (t == "PReLU") return std::make_shared<PReLULayer>(p);
+  if (t == "ELU" || t == "Power" || t == "AbsVal" || t == "BNLL" || t == "Exp" || t == "Log" || t == "Threshold") return std::make_shared<NeuronLayer>(p);
   B2_CHECK(false, "TrainNet: layer type '" + t + "' is not built yet (SURVEY 8f rank 2 covers the ResNet-50 set)");
   return nullptr;
 }
@@ -674,6 +784,15 @@ vector<ParamSpec> TrainNet::BuildNodes(const Net& net, int num_classes, uint64_t
     // (softmax_loss_layer.cpp:128-130 likewise)
     B2_CHECK(!((type == "SigmoidCrossEntropyLoss" || type == "SoftmaxWithLoss") && node.need_backward && L.label_wants_gradient),
              type + " Layer cannot backpropagate to label inputs.");
+    // the neuron layers' in-place and backward limits, known once need-backward is (the reference meets them at run time, or not at all)
+    const bool in_place = !node.top.empty() && !node.bottom.empty() && node.top[0] == node.bottom[0];
+    if (auto* nl = dynamic_cast<NeuronLayer*>(layer.get())) {
+      B2_CHECK(!(type == "Threshold" && node.propagate_down[0]), "Threshold Layer cannot backpropagate: its bottom '" + L.param.bottom[0] +
+                                                                     "' needs a gradient, and the layer has no backward.");
+      B2_CHECK(!(in_place && node.propagate_down[0] && nl->backward_reads_bottom()),
+               type + " Layer does not allow in-place computation when it runs backward: its backward reads the bottom the top overwrites.");
+    }
+    if (auto* pr = dynamic_cast<PReLULayer*>(layer.get())) pr->set_keep_bottom(in_place && node.need_backward);
     node.bottom_diff_tmp.assign(node.bottom.size(), nullptr);
     layers_.push_back(layer);
     layer_names_.push_back(L.param.name);

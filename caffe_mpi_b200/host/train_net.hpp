@@ -210,6 +210,44 @@ class SigmoidLayer : public LayerBase {
   void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
 };
 
+// ELU, Power, AbsVal, BNLL, Exp, Log and Threshold (their *_layer.cpp / .cu): b2c_neuron_forward / _backward with the constants
+// each reference LayerSetUp derives, in float.  In place: AbsVal refuses it always (absval_layer.cpp); BNLL, Log and the Power
+// branches that read x refuse it when the layer runs backward (TrainNet checks that at build time), where the reference would
+// differentiate at the overwritten bottom.  ELU in place reads the top as the bottom, as the reference does.  Threshold has no
+// backward: TrainNet refuses a net in which its bottom would need a gradient.
+class NeuronLayer : public LayerBase {
+ public:
+  explicit NeuronLayer(const LayerParameter& p);
+  const char* type() const override { return layer_param_.type.c_str(); }
+  void LayerSetUp(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { if (t[0] != b[0]) t[0]->ReshapeLike(*b[0]); }
+  bool backward_reads_bottom() const;   // the backward rule reads x (so an in-place layer would read y in its place)
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  int kind_ = 0;
+  float fwd_[3] = {0.f, 0.f, 0.f}, bwd_[3] = {0.f, 0.f, 0.f};   // p0..p2 of b2c_neuron_forward / _backward
+};
+
+// prelu_layer.cpp / .cu: blobs_[0] the slopes, [C] or the 0-axis blob when channel_shared, filled by prelu_param.filler.  In place
+// with a backward, the forward also keeps a copy of x (x_keep, the reference's bottom_memory_) in the same pass.  The backward is
+// one pass for dx and the slope gradient, which it adds into blobs_[0]'s diff (b2c_prelu_backward, deterministic).
+class PReLULayer : public LayerBase {
+ public:
+  using LayerBase::LayerBase;
+  const char* type() const override { return "PReLU"; }
+  void LayerSetUp(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void set_keep_bottom(bool v) { keep_bottom_ = v; }   // TrainNet: in place and running backward
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  void view(const Blob* b, int* N, int* C, int* dim) const;
+  bool keep_bottom_ = false;
+  Blob x_keep_, workspace_;
+  size_t workspace_bytes_ = 0;
+};
+
 // Launches nothing.  Forward: the top aliases the bottom's data (Blob::ShareData), re-pointed every call in case the bottom's
 // memory moved.  Backward: ONE device-to-device copy of the top's diff into the bottom's diff, not an alias: the bottom handed
 // to Backward may be a fan-out shadow blob with a private diff, and the arena may re-point diffs (set_gpu_diff) after set-up,

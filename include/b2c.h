@@ -376,6 +376,59 @@ int b2c_softmax_backward(int outer, int C, int inner, const float* y, const floa
  * run in place.  Alignment as b2c_relu_forward.                                                                                */
 int b2c_sigmoid_forward(size_t n, const float* x, float* y, void* stream);
 int b2c_sigmoid_backward(size_t n, const float* y, const float* dy, float* dx, void* stream);
+/* The elementwise NeuronLayers (src/caffe/layers/{elu,power,absval,bnll,exp,log,threshold}_layer): one kernel template over
+ * the per-element rules, each the reference's own expression in its operation order and types, with no contraction into FMA.
+ * p0..p2 per kind -- the derived constants as the layer's LayerSetUp computes them in float on the host:
+ *   ELU        p0 alpha.                                  dx = x > 0 ? dy : dy * (y + alpha); reads x, y
+ *   POWER      p0 power, p1 scale, p2 shift; diff_scale = power * scale rounded to float in the kernel, as LayerSetUp does.
+ *              Forward: diff_scale == 0 gives the constant (power == 0 ? 1 : powf(shift, power)), else powf(shift + scale x, power)
+ *              with the scale / shift / power steps skipped where they are 1 / 0 / 1.  Backward (power_layer.cu):
+ *              diff_scale == 0 or power == 1: dx = dy * diff_scale (reads neither x nor y); power == 2: dy * (diff_scale * scale * x
+ *              [+ diff_scale * shift]) (reads x); shift == 0: dy * (power * (y / x)); else dy * (diff_scale * (y / (shift + scale x)))
+ *              (both read x and y)
+ *   ABSVAL     no parameter.                              dx = sign(x) * dy; reads x
+ *   BNLL       no parameter; exp(min(x, 50)) in the backward.   reads x
+ *   EXP        p0 inner_scale = log(base) * scale, p1 outer_scale = base^shift.   dx = inner_scale * (y * dy); reads y
+ *   LOG        p0 scale, p1 shift, p2 base_scale = 1 / log(base) (forward) or backward_num_scale = scale / log(base) (backward).
+ *              dx = dy * (p2 * powf(shift + scale x, -1)); reads x
+ *   THRESHOLD  p0 threshold; y = x > threshold ? 1 : 0.  Forward only: b2c_neuron_backward refuses it.
+ * expf / logf / powf, built without fast-math.  Backward reads only the pointers its rule needs (listed above); the others may be
+ * null.  Both directions may run in place (y == x; dx == dy): each element is read before the same thread writes it.  Alignment as
+ * b2c_relu_forward: float4 when every pointer the call reads or writes is 16-byte aligned, one float at a time otherwise, the same
+ * values either way.  Refuses (B2C_ERR_INVALID) an unknown kind and a null pointer the rule needs. */
+typedef enum {
+  B2C_NEURON_ELU = 0, B2C_NEURON_POWER = 1, B2C_NEURON_ABSVAL = 2, B2C_NEURON_BNLL = 3, B2C_NEURON_EXP = 4, B2C_NEURON_LOG = 5,
+  B2C_NEURON_THRESHOLD = 6
+} b2c_neuron_kind;
+int b2c_neuron_forward(int kind, size_t n, const float* x, float* y, float p0, float p1, float p2, void* stream);
+int b2c_neuron_backward(int kind, size_t n, const float* x, const float* y, const float* dy, float* dx, float p0, float p1, float p2,
+                        void* stream);
+/* PReLULayer (src/caffe/layers/prelu_layer.cu) over x [N, C, dim] (channels = shape(1), dim = count(2)); slope has C values, or
+ * one when `shared` (channel_shared: every value uses slope[0]).
+ * Forward: y = x > 0 ? x : x * slope[c].  y may be x.  x_keep (may be null; not x or y): the same pass also writes a copy of x
+ * there -- what the backward of an in-place layer needs (the reference's caffe_copy into bottom_memory_).
+ * Backward, one pass reading x and dy: dx = dy * ((x > 0) + (x <= 0) * slope[c]) when dx is not null (dx may be dy, not x); when
+ * dslope is not null, dslope[c] += sum over the channel of dy * x * (x <= 0) -- ADDED, as Caffe accumulates parameter diffs.  The
+ * sum is deterministic, with no float atomics: each thread adds a fixed stripe of the channel in fp32, the CTA a fixed tree of its
+ * threads; with several CTAs per channel the last to arrive at the channel's counter sums their partials in double (fixed runs,
+ * then a fixed tree) and rounds once.  The orders depend on the shape only, never on the device or the data: the same bits on
+ * every call.  ws: b2c_prelu_workspace_bytes of device memory, 16-byte aligned (may be null when that is 0, or when dslope is
+ * null), ZEROED BEFORE ITS FIRST USE: each call leaves its counters zero again, so a workspace is zeroed once, when it is
+ * allocated, and nothing but the kernel runs on `stream`.  The workspace size depends on the shape only, not on the pointers'
+ * alignment.  Both null dx and dslope: nothing is launched.
+ * Float4 units when dim (C * dim when shared) % 4 == 0 and every tensor pointer is 16-byte aligned, else one float at a time.
+ * Refuses (B2C_ERR_INVALID) N, C or dim < 1 and a channel of N * dim >= 2^31 values (N * C * dim when shared). */
+int b2c_prelu_forward(int N, int C, int dim, int shared, const float* x, const float* slope, float* y, float* x_keep, void* stream);
+int b2c_prelu_workspace_bytes(int N, int C, int dim, int shared, size_t* bytes);
+int b2c_prelu_backward(int N, int C, int dim, int shared, const float* x, const float* dy, const float* slope, float* dx, float* dslope,
+                       void* ws, size_t ws_bytes, void* stream);
+/* The launch of a neuron call.  op 0 / 1: b2c_neuron_forward / _backward of `kind` over N values (C, dim, shared unused); op 2 / 3:
+ * b2c_prelu_forward / _backward.  ptrs[nptrs] (nptrs <= 4): the call's tensors, only tested for 16-byte alignment, null entries
+ * ignored (for PReLU the first three: x, y or dy, x_keep or dx).  out[0] 1 for float4 units, [1] CTAs, [2] threads per CTA,
+ * [3] CTAs per channel (PReLU; 1 otherwise), [4] stripe: values per thread (PReLU; 0 otherwise), [5] channels of the reduction
+ * (C, or 1 when shared), [6] workspace bytes (op 3; 0 otherwise).  Needs n >= 7.  Refuses what the entry points refuse about the
+ * shape and kind.  Pure host computation, independent of the device for PReLU. */
+int b2c_debug_neuron_plan(int op, int kind, int N, int C, int dim, int shared, const void* const* ptrs, int nptrs, int* out, int n);
 /* SigmoidCrossEntropyLossLayer (src/caffe/layers/sigmoid_cross_entropy_loss_layer.cpp): *loss (device scalar) =
  * -sum_i [x (t - [x >= 0]) - log(1 + exp(x - 2 x [x >= 0]))] / N, one launch, the same bits on every call (fixed reduction
  * order for a given count and alignment); no sigmoid tensor is stored.  Backward: dx = (sigmoid(x) - t) * scale with
