@@ -22,7 +22,8 @@ The blob-level bar divides by max|ref|, so an error confined to small elements (
 channel of a ragged tile) can hide under it.  The exact-integer test closes that gap: x, w, dy and the bias are integers in
 [-4, 4], which bf16 and TF32 hold exactly (their lo terms are 0) and whose partial sums are integers below 2^24, so every
 element of y and dx must EQUAL the oracle in every math mode.  A wrong tap mask, row wrap, flip or channel offset moves some
-element by an integer.  This check cannot see a dropped lo term (lo is 0 here); the float parity above covers that."""
+element by an integer.  This check cannot see a dropped lo term (lo is 0 here); test_conv_precision_gpu.py checks the lo
+half of the split element by element (an exact split-term probe and a per-element error bound)."""
 import ctypes as C
 
 import numpy as np
