@@ -178,6 +178,8 @@ def lib():
         "b2c_sigmoid_ce_loss_backward": (i, [sz, vp, vp, f, vp, vp]),
         "b2c_euclidean_loss_forward": (i, [i, sz, vp, vp, vp, vp, vp]),
         "b2c_euclidean_loss_backward": (i, [sz, vp, f, vp, vp]),
+        "b2c_l1_loss_forward": (i, [i, sz, vp, vp, vp, vp, vp]),
+        "b2c_l1_loss_backward": (i, [sz, vp, f, vp, vp]),
         "b2c_contrastive_loss_forward": (i, [i, i, vp, vp, vp, f, i, vp, vp, vp, vp]),
         "b2c_contrastive_loss_backward": (i, [i, i, vp, vp, vp, f, i, f, vp, vp, vp]),
         "b2c_bias_forward": (i, [i, i, i, vp, vp, vp]),

@@ -16,6 +16,7 @@
 //   Sigmoid         src/caffe/layers/sigmoid_layer.cu:9-13           y = 1 / (1 + exp(-x)); dx = dy y (1 - y)
 //   SigmoidCrossEntropyLoss  sigmoid_cross_entropy_loss_layer.cpp   the stable loss expression / N; dx = (sigmoid(x) - t) * loss_weight / N
 //   EuclideanLoss   src/caffe/layers/euclidean_loss_layer.cu        diff = a - b, loss = sum diff^2 / N / 2; dx = +-loss_weight / N * diff
+//   L1Loss          src/caffe/layers/l1_loss_layer.cu:11-43          diff = a - b, loss = sum |diff| / N; dx = +-loss_weight / N * sign(diff)
 #include <float.h>
 #include <type_traits>
 #include <cooperative_groups.h>
@@ -724,18 +725,20 @@ __global__ void __launch_bounds__(256) softmax_col_bwd_kernel(size_t cols, int C
   }
 }
 
-// ---- Sigmoid, SigmoidCrossEntropyLoss, EuclideanLoss ------------------------------------------------------------------
+// ---- Sigmoid, SigmoidCrossEntropyLoss, EuclideanLoss, L1Loss ---------------------------------------------------------------
 // sigmoid_layer.cu:9-13.  The one expression b2c_sigmoid_forward and b2c_sigmoid_ce_loss_backward share.
 __device__ __forceinline__ float sigmoid_of(float x) { return 1.f / (1.f + expf(-x)); }
 
-enum EwOp { EW_SIGMOID_FWD, EW_SIGMOID_BWD, EW_SIGCE_BWD, EW_SCALE };
+enum EwOp { EW_SIGMOID_FWD, EW_SIGMOID_BWD, EW_SIGCE_BWD, EW_SCALE, EW_SIGN_SCALE };
 // y = op(a, b, s) per element: SIGMOID_FWD sigmoid(a); SIGMOID_BWD b * a * (1 - a) with a = y, b = dy; SIGCE_BWD (sigmoid(a) - b) * s;
-// SCALE s * a.  In place allowed (no __restrict__)
+// SCALE s * a; SIGN_SCALE s * sign(a) with sign(0) = sign(NaN) = 0, and +0 there (caffe_gpu_sign, then axpby's 0 * y + s * sign).
+// In place allowed (no __restrict__)
 template <int OP>
 __device__ __forceinline__ float ew_apply(float a, float b, float s) {
   if (OP == EW_SIGMOID_FWD) return sigmoid_of(a);
   if (OP == EW_SIGMOID_BWD) return b * a * (1.f - a);
   if (OP == EW_SIGCE_BWD) return __fmul_rn(sigmoid_of(a) - b, s);
+  if (OP == EW_SIGN_SCALE) return a > 0.f ? s : a < 0.f ? -s : 0.f;
   return s * a;
 }
 template <int OP>
@@ -757,6 +760,7 @@ __global__ void __launch_bounds__(256) ew_kernel(size_t n, int vec, const float*
 // summed in double; the float result is formed once at the end.
 //   MODE 0 (SigmoidCrossEntropyLoss): term = x (t - [x >= 0]) - log(1 + exp(x - 2 x [x >= 0])), loss = -sum / N
 //   MODE 1 (EuclideanLoss):           d = a - b stored to diff, term = d * d, loss = sum / N / 2
+//   MODE 2 (L1Loss):                  d = a - b stored to diff, term = |d|,  loss = sum / N
 constexpr int LOSS_THREADS = 512;
 constexpr int LOSS_CLUSTER = 8;                    // the portable cluster limit
 template <int MODE>
@@ -767,7 +771,7 @@ __device__ __forceinline__ float loss_term(float a, float b, float* d) {
   }
   const float v = a - b;
   *d = v;
-  return __fmul_rn(v, v);
+  return MODE == 1 ? __fmul_rn(v, v) : fabsf(v);
 }
 // The reduction every loss-sum kernel ends with: each thread's double partial is summed per warp, the warp sums per CTA in warp
 // order, and the CTA sums over the cluster in rank order in rank 0 through distributed shared memory.  Returns the total in rank 0's
@@ -807,12 +811,12 @@ loss_sum_kernel(size_t count, int N, const float* __restrict__ a, const float* _
       float4 d;
       const float t0 = loss_term<MODE>(u.x, v.x, &d.x), t1 = loss_term<MODE>(u.y, v.y, &d.y);
       const float t2 = loss_term<MODE>(u.z, v.z, &d.z), t3 = loss_term<MODE>(u.w, v.w, &d.w);
-      if (MODE == 1) reinterpret_cast<float4*>(diff)[i] = d;
+      if (MODE != 0) reinterpret_cast<float4*>(diff)[i] = d;
       acc += ((double)t0 + (double)t1) + ((double)t2 + (double)t3);
     } else {
       float d;
       const float t = loss_term<MODE>(a[i], b[i], &d);
-      if (MODE == 1) diff[i] = d;
+      if (MODE != 0) diff[i] = d;
       acc += (double)t;
     }
   }
@@ -820,13 +824,13 @@ loss_sum_kernel(size_t count, int N, const float* __restrict__ a, const float* _
     const size_t i = units * 4 + threadIdx.x;
     float d;
     const float t = loss_term<MODE>(a[i], b[i], &d);
-    if (MODE == 1) diff[i] = d;
+    if (MODE != 0) diff[i] = d;
     acc += (double)t;
   }
   const double s = loss_cluster_sum(acc);
   if (rank == 0 && threadIdx.x == 0) {
     const float f = (float)s;
-    *loss = MODE == 0 ? -f / (float)N : f / (float)N / 2.f;
+    *loss = MODE == 0 ? -f / (float)N : MODE == 1 ? f / (float)N / 2.f : f / (float)N;
   }
 }
 // ContrastiveLoss (contrastive_loss_layer.cpp): one warp per pair, the lanes strided over the channels; the pair's squared distance
@@ -1292,6 +1296,14 @@ extern "C" int b2c_euclidean_loss_forward(int N, size_t count, const float* a, c
 extern "C" int b2c_euclidean_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream) {
   NEED(diff && dx, "b2c_euclidean_loss_backward: null");
   return launch_ew<EW_SCALE>(count, diff, nullptr, alpha, dx, stream);
+}
+extern "C" int b2c_l1_loss_forward(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream) {
+  NEED(a && b && diff && loss && N > 0 && count > 0, "b2c_l1_loss_forward: bad argument");
+  return launch_loss_sum<2>(N, count, a, b, diff, loss, stream);
+}
+extern "C" int b2c_l1_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream) {
+  NEED(diff && dx, "b2c_l1_loss_backward: null");
+  return launch_ew<EW_SIGN_SCALE>(count, diff, nullptr, alpha, dx, stream);
 }
 extern "C" int b2c_contrastive_loss_forward(int N, int C, const float* a, const float* b, const float* y, float margin, int legacy, float* diff,
                                             float* dist_sq, float* loss, void* stream) {

@@ -185,13 +185,17 @@ class DataReader:
         lib().b2h_data_reader_info(self._h, chw, C.byref(n), C.byref(fc))
         self.shape = (chw[0], chw[1], chw[2])
         self.entries, self.full_cycle, self.batch_size = n.value, fc.value, batch_size
+        db = LMDB(source)                                # the batches are floats when the first datum carries float_data only
+        first = datum_parse(db.current()[1])
+        db.close()
+        self.dtype = np.float32 if first["float_data"] and not first["data"] else np.uint8
 
     def first_record(self, batch):
         return lib().b2h_data_reader_first_record(self._h, batch)
 
     def next(self):
-        """(data uint8 [B][C][H][W], label float32 [B], record_id uint32 [B], batch_id)"""
-        data = np.empty((self.batch_size,) + self.shape, np.uint8)
+        """(data [B][C][H][W] of self.dtype, label float32 [B], record_id uint32 [B], batch_id)"""
+        data = np.empty((self.batch_size,) + self.shape, self.dtype)
         label = np.empty(self.batch_size, np.float32)
         ids = np.empty(self.batch_size, np.uint32)
         bid = C.c_longlong()

@@ -8,7 +8,17 @@
 
 namespace caffe {
 
-DataLayer::DataLayer(const NetLayer& L, uint64_t seed) : LayerBase(L.param), seed_(seed) {}
+DataLayer::DataLayer(const NetLayer& L, uint64_t seed, int parser_threads)
+    : LayerBase(L.param), parsers_(parser_threads > 0 ? parser_threads : 0), seed_(seed) {}
+
+int DataLayer::ParserThreads(const NetLayer& L) {
+  const DataParameter& dp = L.param.data_param;
+  if (dp.parser_threads > 0) return dp.parser_threads;
+  int c = 0, h = 0, w = 0;
+  bool encoded = false;
+  PeekDatumShape(dp.source, &c, &h, &w, dp.force_encoded_color, &encoded);
+  return encoded ? 6 : 1;
+}
 
 DataLayer::~DataLayer() {
   if (copy_stream_) cudaStreamSynchronize(copy_stream_);
@@ -37,7 +47,9 @@ void DataLayer::LayerSetUp(const vector<Blob*>&, const vector<Blob*>& top) {
   B2_CHECK(dp.batch_size > 0, "Data layer needs a positive batch_size");
   N_ = dp.batch_size;
   bool encoded = false;
-  PeekDatumShape(dp.source, &C_, &Hd_, &Wd_, dp.force_encoded_color, &encoded);             // data_layer.cpp:176-183: shape from one datum
+  PeekDatumShape(dp.source, &C_, &Hd_, &Wd_, dp.force_encoded_color, &encoded, &float_);    // data_layer.cpp:176-183: shape from one datum
+  B2_CHECK(!float_ || FloatDatumsTakeNoTransform(tp.scale, tp.mirror, tp.crop_size, !tp.mean_value.empty() || !tp.mean_file.empty()),
+           "Data layer '" + layer_param_.name + "': " + kFloatDatumTransformMsg);
   crop_h_ = tp.crop_size > 0 ? tp.crop_size : Hd_;
   crop_w_ = tp.crop_size > 0 ? tp.crop_size : Wd_;
   B2_CHECK(Hd_ >= crop_h_ && Wd_ >= crop_w_, "crop_size larger than the datum");   // data_transformer.cpp:192-193
@@ -45,7 +57,7 @@ void DataLayer::LayerSetUp(const vector<Blob*>&, const vector<Blob*>& top) {
   if (host_crop_) Hd_ = Wd_ = tp.crop_size;                                        // the slots hold crop windows
   top[0]->Reshape({N_, C_, crop_h_, crop_w_});
   if (top.size() > 1) top[1]->Reshape({N_});
-  u8_bytes_ = (size_t)N_ * C_ * Hd_ * Wd_;
+  batch_bytes_ = (size_t)N_ * C_ * Hd_ * Wd_ * (float_ ? sizeof(float) : 1);
 
   // DataTransformer's constructor (data_transformer.cpp:17-40)
   if (!tp.mean_file.empty()) {
@@ -69,16 +81,16 @@ void DataLayer::LayerSetUp(const vector<Blob*>&, const vector<Blob*>& top) {
     fprintf(stderr, "DataLayer '%s': data_param { cache: %s shuffle: %s } -- the database is a read-only mapping of the page cache, "
                     "so `cache` has nothing to add; `shuffle` is not built: records are read in key order (shuffle when converting)\n",
             layer_param_.name.c_str(), dp.cache ? "true" : "false", dp.shuffle ? "true" : "false");
-  parsers_ = dp.parser_threads > 0 ? dp.parser_threads : (encoded ? 6 : 1);
+  if (parsers_ == 0) parsers_ = dp.parser_threads > 0 ? dp.parser_threads : (encoded ? 6 : 1);   // as ParserThreads
   const int K = std::max(2, parsers_ + 1);
   slot_.resize(K);
   CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
   for (Slot& sl : slot_) {
-    CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&sl.buf.data), u8_bytes_));
+    CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&sl.buf.data), batch_bytes_));
     CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&sl.buf.label), sizeof(float) * N_));
     CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&sl.buf.record_id), sizeof(uint32_t) * N_));
     CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&sl.host_off), sizeof(int) * 3 * N_));
-    CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&sl.dev_u8), u8_bytes_));
+    CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&sl.dev_u8), batch_bytes_));
     CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&sl.dev_off), sizeof(int) * 3 * N_));
     CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&sl.dev_label), sizeof(float) * N_));
     CUDA_CHECK(cudaEventCreateWithFlags(&sl.copied, cudaEventDisableTiming));
@@ -94,7 +106,7 @@ void DataLayer::set_solver(int solver_count, int solver_rank) {
   solver_rank_ = solver_rank;
 }
 
-size_t DataLayer::h2d_bytes() const { return u8_bytes_ + sizeof(int) * 3 * (size_t)N_ + sizeof(float) * (size_t)N_; }
+size_t DataLayer::h2d_bytes() const { return batch_bytes_ + sizeof(int) * 3 * (size_t)N_ + sizeof(float) * (size_t)N_; }
 
 void DataLayer::EnsureStarted() {
   if (reader_) return;
@@ -109,7 +121,8 @@ void DataLayer::EnsureStarted() {
   p.host_crop = host_crop_ ? tp.crop_size : 0;
   p.train = layer_param_.phase != TEST;
   reader_.reset(new DataReader(p));
-  B2_CHECK(reader_->channels() == C_ && reader_->height() == Hd_ && reader_->width() == Wd_, "database changed shape between set-up and start");
+  B2_CHECK(reader_->channels() == C_ && reader_->height() == Hd_ && reader_->width() == Wd_ && reader_->float_data() == float_,
+           "database changed shape between set-up and start");
   // random_seed >= 0: "Use random_seed setting for deterministic transformations" (data_transformer.cpp:733-736); otherwise every
   // solver gets its own stream (the reference: Caffe::next_seed() of a solver seeded with seed + rank, parallel.cpp:179-187)
   const uint64_t s = tp.random_seed >= 0 ? (uint64_t)tp.random_seed : seed_ + 0x9E3779B9ull * (uint64_t)(solver_rank_ + 1);
@@ -140,7 +153,7 @@ void DataLayer::IssueCopy(int s) {
   } else {
     for (int i = 0; i < N_; ++i) draws_->Draw(Hd_, Wd_, sl.host_off + i, sl.host_off + N_ + i, mir + i);
   }
-  CUDA_CHECK(cudaMemcpyAsync(sl.dev_u8, sl.buf.data, u8_bytes_, cudaMemcpyHostToDevice, copy_stream_));
+  CUDA_CHECK(cudaMemcpyAsync(sl.dev_u8, sl.buf.data, batch_bytes_, cudaMemcpyHostToDevice, copy_stream_));
   CUDA_CHECK(cudaMemcpyAsync(sl.dev_off, sl.host_off, sizeof(int) * 3 * N_, cudaMemcpyHostToDevice, copy_stream_));
   CUDA_CHECK(cudaMemcpyAsync(sl.dev_label, sl.buf.label, sizeof(float) * N_, cudaMemcpyHostToDevice, copy_stream_));
   CUDA_CHECK(cudaEventRecord(sl.copied, copy_stream_));
@@ -152,9 +165,12 @@ void DataLayer::LoadBatch(const vector<Blob*>& top, cudaStream_t st) {
   Slot& sl = slot_[cur_];
   if (!sl.in_flight) IssueCopy(cur_);                    // the first batch: nothing was prefetched yet
   CUDA_CHECK(cudaStreamWaitEvent(st, sl.copied, 0));
-  B2C_CHECK(b2c_transform_u8(sl.dev_u8, N_, C_, Hd_, Wd_, crop_h_, crop_w_, sl.dev_off, sl.dev_off + N_,
-                             reinterpret_cast<const unsigned char*>(sl.dev_off + 2 * N_), dev_mean_values_, dev_mean_image_, layer_param_.transform_param.scale,
-                             top[0]->mutable_gpu_data(), st));
+  if (float_)                                            // float_data datums are the top's values already
+    CUDA_CHECK(cudaMemcpyAsync(top[0]->mutable_gpu_data(), sl.dev_u8, batch_bytes_, cudaMemcpyDeviceToDevice, st));
+  else
+    B2C_CHECK(b2c_transform_u8(sl.dev_u8, N_, C_, Hd_, Wd_, crop_h_, crop_w_, sl.dev_off, sl.dev_off + N_,
+                               reinterpret_cast<const unsigned char*>(sl.dev_off + 2 * N_), dev_mean_values_, dev_mean_image_, layer_param_.transform_param.scale,
+                               top[0]->mutable_gpu_data(), st));
   if (top.size() > 1)
     CUDA_CHECK(cudaMemcpyAsync(top[1]->mutable_gpu_data(), sl.dev_label, sizeof(float) * N_, cudaMemcpyDeviceToDevice, st));
   CUDA_CHECK(cudaEventRecord(sl.consumed, st));

@@ -10,6 +10,7 @@
 // GPU-first shape of the same pipeline:
 //   parser threads (DataReader)  --memcpy from the file mapping-->  pinned slot k  --cudaMemcpyAsync, copy stream-->  device slot k
 //   --b2c_transform_u8 on the compute stream, first thing of the step-->  top[0];   labels ride along and are copied into top[1].
+// float_data datums take the same path with 4 bytes per value and no transform (a transform_param is refused).
 // K = max(2, parser_threads + 1) slots circulate: while step i computes, batch i+1 is crossing PCIe and batches i+2.. are being
 // assembled by the parser threads.  A step moves 1 byte per pixel over PCIe (the reference's GPU transform moves Ftype-sized
 // elements, data_layer.cpp:235-237) and no host thread touches a pixel after the parser's one memcpy.
@@ -23,8 +24,11 @@ namespace caffe {
 class DataLayer : public LayerBase {
  public:
   // reads L.param's data_param and transform_param.  `seed` feeds the crop / mirror stream when transform_param.random_seed is unset
-  // (the reference draws Caffe::next_seed()); the TEST phase takes the centre crop window
-  DataLayer(const NetLayer& L, uint64_t seed);
+  // (the reference draws Caffe::next_seed()); the TEST phase takes the centre crop window.  parser_threads > 0 overrides
+  // ParserThreads(L) (a net whose Data layers must read in step gives them one count)
+  DataLayer(const NetLayer& L, uint64_t seed, int parser_threads = 0);
+  // the parser threads the layer runs: data_param.parser_threads, or the automatic count for its datums (see parsers_)
+  static int ParserThreads(const NetLayer& L);
   ~DataLayer() override;
   const char* type() const override { return "Data"; }
   void LayerSetUp(const vector<Blob*>& bottom, const vector<Blob*>& top) override;
@@ -47,7 +51,7 @@ class DataLayer : public LayerBase {
     BatchBuf buf;                 // pinned: data, label (and record ids)
     int* host_off = nullptr;      // pinned: h_off[N], w_off[N], mirror[N] (bytes)
     vector<unsigned> rand;        // host-crop mode: Fill3Randoms' draws of the batch this slot is assembling (3 per item)
-    unsigned char* dev_u8 = nullptr;
+    unsigned char* dev_u8 = nullptr;   // the batch on the device, as the slot's pinned `buf.data` holds it
     int* dev_off = nullptr;
     float* dev_label = nullptr;
     cudaEvent_t copied = nullptr, consumed = nullptr;
@@ -67,7 +71,9 @@ class DataLayer : public LayerBase {
   uint64_t seed_;
   int solver_count_ = 1, solver_rank_ = 0;
   int N_ = 0, C_ = 0, Hd_ = 0, Wd_ = 0, crop_h_ = 0, crop_w_ = 0;
-  size_t u8_bytes_ = 0;
+  // float_data datums (DIGITS' label databases): the slots carry floats, and LoadBatch copies the device slot into top[0] as it is
+  bool float_ = false;
+  size_t batch_bytes_ = 0;                 // one batch in a slot: N*C*Hd*Wd bytes, or floats for float_data datums
   std::unique_ptr<DataReader> reader_;
   std::unique_ptr<TransformDraws> draws_;
   vector<Slot> slot_;

@@ -24,18 +24,27 @@ void advance(db::LMDBCursor* cur, size_t n, size_t entries) {
 }  // namespace
 
 namespace {
-// What a datum contributes to a batch: its own bytes, or the decoded image of an encoded one (DecodeDatumToCVMat[Native] +
-// CVMatToDatum, io.cpp:167-230).  `img` is scratch that keeps the decoded pixels alive.
-void datum_pixels(const Datum& d, bool force_color, DecodedImage* img, const uint8_t** px, int* c, int* h, int* w) {
+// What a datum contributes to a batch: its own bytes, the decoded image of an encoded one (DecodeDatumToCVMat[Native] +
+// CVMatToDatum, io.cpp:167-230), or its float_data when it carries floats and no `data` (the label databases DIGITS writes for
+// DetectNet; DataTransformer::Copy moves them to the device as they are, data_transformer.cpp:92-110).  Returns whether the values are floats;
+// *px then points at c*h*w floats, else at c*h*w bytes.  `img` is scratch that keeps the decoded pixels alive.
+bool datum_values(const Datum& d, bool force_color, DecodedImage* img, const void** px, int* c, int* h, int* w) {
   if (d.encoded) {
     DecodeImage(d.data, d.data_size, force_color, img);        // JPEG or PNG, by the file's own signature (cv::imdecode does the same)
     *px = img->chw.data(); *c = img->channels; *h = img->height; *w = img->width;
-    return;
+    return false;
   }
-  B2_CHECK(d.data_size > 0 || d.float_data.empty(), "DataReader: float_data datums are not built (uint8 `data` only)");
   B2_CHECK(d.channels > 0 && d.height > 0 && d.width > 0, "DataReader: datum has no shape");
-  B2_CHECK(d.data_size == (size_t)d.channels * d.height * d.width, "DataReader: datum data size disagrees with channels*height*width");
-  *px = d.data; *c = d.channels; *h = d.height; *w = d.width;
+  const size_t n = (size_t)d.channels * d.height * d.width;
+  *c = d.channels; *h = d.height; *w = d.width;
+  if (d.data_size == 0 && !d.float_data.empty()) {
+    B2_CHECK(d.float_data.size() == n, "DataReader: datum float_data size disagrees with channels*height*width");
+    *px = d.float_data.data();
+    return true;
+  }
+  B2_CHECK(d.data_size == n, "DataReader: datum data size disagrees with channels*height*width");
+  *px = d.data;
+  return false;
 }
 }  // namespace
 
@@ -53,9 +62,10 @@ DataReader::DataReader(const DataReaderParam& p) : p_(p) {
     Datum d;
     B2_CHECK(ParseDatum(cur->data(), cur->size(), &d), "Database cursor failed to parse Datum record");
     DecodedImage img;
-    const uint8_t* px = nullptr;
-    datum_pixels(d, p_.force_encoded_color, &img, &px, &c_, &h_, &w_);
+    const void* px = nullptr;
+    float_ = datum_values(d, p_.force_encoded_color, &img, &px, &c_, &h_, &w_);
     if (p_.host_crop > 0) {
+      B2_CHECK(!float_, "DataReader: float_data datums are copied whole (no crop)");
       B2_CHECK(h_ >= p_.host_crop && w_ >= p_.host_crop, "crop_size larger than the datum");
       h_ = w_ = p_.host_crop;                            // the batch holds windows
     }
@@ -110,9 +120,11 @@ void DataReader::fill(db::LMDBCursor* cur, size_t rec_id, BatchBuf* b) {
   DecodedImage img;
   for (size_t j = 0; j < B; ++j) {
     B2_CHECK(ParseDatum(cur->data(), cur->size(), &d), "Database cursor failed to parse Datum record");
-    const uint8_t* px = nullptr;
+    const void* vals = nullptr;
     int c = 0, h = 0, w = 0;
-    datum_pixels(d, p_.force_encoded_color, &img, &px, &c, &h, &w);
+    B2_CHECK(datum_values(d, p_.force_encoded_color, &img, &vals, &c, &h, &w) == float_,
+             "DataReader: " + p_.source + " mixes float_data datums and uint8 datums");
+    const uint8_t* px = static_cast<const uint8_t*>(vals);
     B2_CHECK(c == c_, "Number of channels can't vary in the same batch");
     const size_t item = (rec_id + j) % B;                              // data_layer.cpp:256
     if (p_.host_crop > 0) {
@@ -188,7 +200,7 @@ bool UseDatabase(const std::string& source, int backend) {
   return true;
 }
 
-void PeekDatumShape(const std::string& source, int* c, int* h, int* w, bool force_encoded_color, bool* encoded) {
+void PeekDatumShape(const std::string& source, int* c, int* h, int* w, bool force_encoded_color, bool* encoded, bool* float_data) {
   db::LMDB env;
   env.Open(source, db::READ);
   std::unique_ptr<db::LMDBCursor> cur(env.NewCursor());
@@ -196,9 +208,10 @@ void PeekDatumShape(const std::string& source, int* c, int* h, int* w, bool forc
   Datum d;
   B2_CHECK(ParseDatum(cur->data(), cur->size(), &d), "Database cursor failed to parse Datum record");
   DecodedImage img;
-  const uint8_t* px = nullptr;
-  datum_pixels(d, force_encoded_color, &img, &px, c, h, w);
+  const void* px = nullptr;
+  const bool f = datum_values(d, force_encoded_color, &img, &px, c, h, w);
   if (encoded) *encoded = d.encoded;
+  if (float_data) *float_data = f;
 }
 
 // ------------------------------------------------------------------------------------------------ TransformDraws

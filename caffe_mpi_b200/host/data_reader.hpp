@@ -52,8 +52,8 @@ struct DataReaderParam {
   bool train = true;                            // TRAIN: random window; TEST: the centre window (data_transformer.cpp:219-229)
 };
 
-// One batch under assembly / assembled.  `data` is [batch][C][H][W] uint8 in datum layout, `label` one float per item (the
-// reference's label blob is Ftype), `record_id` the reader's numbering of the records it holds.
+// One batch under assembly / assembled.  `data` is [batch][C][H][W] uint8 in datum layout (float for float_data datums), `label`
+// one float per item (the reference's label blob is Ftype), `record_id` the reader's numbering of the records it holds.
 struct BatchBuf {
   uint8_t* data = nullptr;
   float* label = nullptr;
@@ -75,7 +75,9 @@ class DataReader {
   int channels() const { return c_; }
   int height() const { return h_; }
   int width() const { return w_; }
-  size_t datum_bytes() const { return (size_t)c_ * h_ * w_; }
+  // float_data datums (a datum with float_data and no `data`): the batch holds c*h*w floats per item instead of bytes
+  bool float_data() const { return float_; }
+  size_t datum_bytes() const { return (size_t)c_ * h_ * w_ * (float_ ? sizeof(float) : 1); }
   size_t entries() const { return db_->entries(); }
   size_t full_cycle() const { return full_cycle_; }
   // Hand an empty buffer to the reader: the n-th buffer pushed receives batch n (filled by parser thread n % P).  The buffer must
@@ -97,6 +99,7 @@ class DataReader {
   DataReaderParam p_;
   std::unique_ptr<db::LMDB> db_;
   int c_ = 0, h_ = 0, w_ = 0;
+  bool float_ = false;              // the first datum's kind; every datum of the database must be of it
   size_t full_cycle_ = 0;
   std::vector<std::unique_ptr<Queue>> free_, full_;
   std::vector<std::thread> threads_;
@@ -110,8 +113,16 @@ class DataReader {
 // reference's behaviour, db_lmdb.cpp:19); unset / "auto": the database when <source>/data.mdb exists, else the synthetic source
 // (bench.py and the tests run the reference's prototxts on machines that do not hold ImageNet).
 bool UseDatabase(const std::string& source, int backend);
-// channels / height / width of the first datum (DataReader::sample()); an encoded first datum is decoded to learn them
-void PeekDatumShape(const std::string& source, int* c, int* h, int* w, bool force_encoded_color = false, bool* encoded = nullptr);
+// A Data layer over float_data datums takes no transform_param: its values reach the top as they are stored
+inline bool FloatDatumsTakeNoTransform(float scale, bool mirror, int crop_size, bool has_mean) {
+  return scale == 1.f && !mirror && crop_size == 0 && !has_mean;
+}
+constexpr const char* kFloatDatumTransformMsg =
+    "its datums carry float_data, which are copied as they are: transform_param (crop_size, mirror, mean_file, mean_value, scale) is not built for them";
+// channels / height / width of the first datum (DataReader::sample()); an encoded first datum is decoded to learn them.
+// *float_data: the datum carries float_data and no `data`
+void PeekDatumShape(const std::string& source, int* c, int* h, int* w, bool force_encoded_color = false, bool* encoded = nullptr,
+                    bool* float_data = nullptr);
 
 // DataTransformer's random draws (src/caffe/data_transformer.cpp:127-137 Fill3Randoms, :187,219-226 their use, :729-749
 // InitRand / Rand): per datum  rand0 = Rand() + 1 if mirror;  rand1 = Rand() + 1, rand2 = Rand() + 1 if TRAIN and crop_size;

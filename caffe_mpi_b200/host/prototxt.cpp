@@ -423,7 +423,11 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
       if (type == "Data") {
         // DataLayerSetUp reads one datum to size the top blob (data_layer.cpp:176-183); so does this, when the database is there
         L.use_database = UseDatabase(dp.source, dp.backend);
-        if (L.use_database) PeekDatumShape(dp.source, &dc, &dh, &dw, dp.force_encoded_color);
+        bool float_data = false;
+        if (L.use_database) PeekDatumShape(dp.source, &dc, &dh, &dw, dp.force_encoded_color, nullptr, &float_data);
+        const TransformationParameter& tp = P.transform_param;
+        B2_CHECK(!float_data || FloatDatumsTakeNoTransform(tp.scale, tp.mirror, tp.crop_size, !tp.mean_value.empty() || !tp.mean_file.empty()),
+                 "Data layer '" + P.name + "': " + kFloatDatumTransformMsg);
       }
       if (crop > 0) {
         if (L.use_database) B2_CHECK(dh >= crop && dw >= crop, "crop_size larger than the datums of " + dp.source);
@@ -570,12 +574,12 @@ Net::Net(const PMessage& np, Phase phase, int batch_override, int default_channe
     } else if (type == "Softmax") {
       P.softmax_param.axis = canonical_axis(P.softmax_param.axis, bottom_shape(0));                 // softmax_layer.cpp:12-13
       tops.push_back(bottom_shape(0));
-    } else if (type == "SoftmaxWithLoss" || type == "EuclideanLoss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy") {
-      if (type == "EuclideanLoss" || type == "SigmoidCrossEntropyLoss") {
+    } else if (type == "SoftmaxWithLoss" || type == "EuclideanLoss" || type == "L1Loss" || type == "SigmoidCrossEntropyLoss" || type == "Accuracy") {
+      if (type == "EuclideanLoss" || type == "L1Loss" || type == "SigmoidCrossEntropyLoss") {
         const std::vector<int>& a = bottom_shape(0);
         const std::vector<int>& b = bottom_shape(1);
         B2_CHECK(!a.empty() && !b.empty() && a[0] == b[0], "The data and label should have the same number.");   // loss_layer.cpp:19-20
-        if (type == "EuclideanLoss") B2_CHECK(prod(a, 1) == prod(b, 1), "Inputs must have the same dimension.");
+        if (type != "SigmoidCrossEntropyLoss") B2_CHECK(prod(a, 1) == prod(b, 1), "Inputs must have the same dimension.");  // l1_loss_layer.cpp:14-15 too
         else B2_CHECK(prod(a) == prod(b), "SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.");
       }
       for (size_t i = 0; i < P.top.size(); ++i) tops.push_back({});

@@ -478,7 +478,7 @@ void FlattenLayer::Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, 
   CUDA_CHECK(cudaMemcpyAsync(b[0]->mutable_gpu_diff(), t[0]->gpu_diff(), sizeof(float) * t[0]->count(), cudaMemcpyDeviceToDevice, S()));
 }
 
-// ================================================================================================ EuclideanLoss / SigmoidCrossEntropyLoss
+// ================================================================================================ EuclideanLoss / L1Loss / SigmoidCrossEntropyLoss
 void EuclideanLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
   B2C_CHECK(b2c_euclidean_loss_forward(b[0]->shape(0), b[0]->count(), b[0]->gpu_data(), b[1]->gpu_data(), diff_.mutable_gpu_data(),
                                        t[0]->mutable_gpu_data(), S()));
@@ -488,6 +488,17 @@ void EuclideanLossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& 
     if (!pd[i]) continue;
     const float alpha = (i == 0 ? 1.f : -1.f) * loss_weight() / (float)b[i]->shape(0);
     B2C_CHECK(b2c_euclidean_loss_backward(b[i]->count(), diff_.gpu_data(), alpha, b[i]->mutable_gpu_diff(), S()));
+  }
+}
+void L1LossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
+  B2C_CHECK(b2c_l1_loss_forward(b[0]->shape(0), b[0]->count(), b[0]->gpu_data(), b[1]->gpu_data(), diff_.mutable_gpu_data(),
+                                t[0]->mutable_gpu_data(), S()));
+}
+void L1LossLayer::Backward_gpu(const vector<Blob*>&, const vector<bool>& pd, const vector<Blob*>& b) {
+  for (int i = 0; i < 2; ++i) {                    // l1_loss_layer.cu:31-41: alpha = sign * loss_weight / num, times sign(diff)
+    if (!pd[i]) continue;
+    const float alpha = (i == 0 ? 1.f : -1.f) * loss_weight() / (float)b[i]->shape(0);
+    B2C_CHECK(b2c_l1_loss_backward(b[i]->count(), diff_.gpu_data(), alpha, b[i]->mutable_gpu_diff(), S()));
   }
 }
 void SigmoidCrossEntropyLossLayer::Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) {
@@ -666,6 +677,7 @@ static shared_ptr<LayerBase> CreateLayer(const LayerParameter& p, const vector<v
   if (t == "Sigmoid") return std::make_shared<SigmoidLayer>(p);
   if (t == "Flatten") return std::make_shared<FlattenLayer>(p, top_shapes[0]);
   if (t == "EuclideanLoss") return std::make_shared<EuclideanLossLayer>(p);
+  if (t == "L1Loss") return std::make_shared<L1LossLayer>(p);
   if (t == "SigmoidCrossEntropyLoss") return std::make_shared<SigmoidCrossEntropyLossLayer>(p);
   if (t == "LRN") return std::make_shared<LRNLayer>(p);
   if (t == "Dropout") return std::make_shared<DropoutLayer>(p, dropout_seed);
@@ -712,6 +724,29 @@ TrainNet::TrainNet(const Net& net, const SolverParameter& sp, int num_classes, u
 }
 vector<ParamSpec> TrainNet::BuildNodes(const Net& net, int num_classes, uint64_t seed, int math) {
   vector<ParamSpec> specs;
+  // Data layers that each read an LMDB (DetectNet's images and labels): batch n of every one must hold the same record positions.
+  // DataReader's partition gives that when they share the batch size and, with several solvers, the parser thread count, so they
+  // all run the largest count any of them asks for or resolves to.  A net reads either its databases or one synthetic source: a
+  // synthetic layer next to a database one (an Input, or a Data layer whose source does not open) would never be reloaded, and the
+  // net would train on its placeholder values without a word
+  int db_layers = 0, db_parsers = 0, db_batch = 0;
+  string synthetic;
+  for (const NetLayer& L : net.layers()) {
+    const string& t = L.param.type;
+    if (!(t == "Data" && L.use_database)) {
+      if (synthetic.empty() && (t == "Data" || t == "Input" || t == "DummyData" || t == "ImageData")) synthetic = L.param.name;
+      continue;
+    }
+    B2_CHECK(db_layers == 0 || L.param.data_param.batch_size == db_batch,
+             "TrainNet: Data layers that read databases must have one batch_size, so that their batches hold the same records");
+    db_batch = L.param.data_param.batch_size;
+    db_parsers = std::max(db_parsers, DataLayer::ParserThreads(L));
+    ++db_layers;
+  }
+  B2_CHECK(db_layers == 0 || synthetic.empty(),
+           "TrainNet: layer '" + synthetic + "' feeds synthetic data next to Data layers that read databases (an Input / DummyData layer, "
+           "or a Data layer whose source does not open): one data source per net");
+  int db_index = 0;
   for (size_t li = 0; li < net.layers().size(); ++li) {
     const NetLayer& L = net.layers()[li];
     const string& type = L.param.type;
@@ -731,11 +766,12 @@ vector<ParamSpec> TrainNet::BuildNodes(const Net& net, int num_classes, uint64_t
     shared_ptr<LayerBase> layer;
     if (type == "Data" && L.use_database) {
       // data_param.source opened: the layer reads it (parser threads -> pinned batch -> device transform), data_layer.hpp
-      B2_CHECK(db_data_ == nullptr && data_ == nullptr, "TrainNet: one data source per net");
-      auto* d = new DataLayer(L, seed);
+      // Several such layers (DetectNet's images and labels) each read their own LMDB; every one loads a batch per step, so with equal
+      // batch sizes batch i of each holds the same record positions
+      // each layer its own crop / mirror stream (the first keeps `seed`), as the reference's layers each draw Caffe::next_seed()
+      auto* d = new DataLayer(L, seed + 0x9E3779B97F4A7C15ull * (uint64_t)db_index++, db_layers > 1 ? db_parsers : 0);
       layer.reset(d);
-      db_data_ = d;
-      db_data_node_ = (int)layers_.size();
+      db_data_.push_back({d, (int)layers_.size()});
     } else if (type == "Data" || type == "Input" || type == "DummyData" || type == "ImageData") {
       auto* d = new SyntheticDataLayer(L.param, shapes, num_classes, seed);
       layer.reset(d);
@@ -919,7 +955,7 @@ TrainNet::~TrainNet() {
 
 void TrainNet::AttachSync(P2PSync* sync) {
   sync_ = sync;
-  if (db_data_) db_data_->set_solver(sync->nranks(), sync->rank());     // each solver reads its own stripe of the database
+  for (auto& d : db_data_) d.first->set_solver(sync->nranks(), sync->rank());     // each solver reads its own stripe of the database
   sync_->on_start(solver_->arena());
   filters_dirty_ = true;
   sched_.reset(new ReduceScheduler(solver_.get(), sync_));
@@ -953,8 +989,9 @@ void TrainNet::PrepareFilters() {
 }
 void TrainNet::Forward(bool copy_input) {
   if (filters_dirty_) PrepareFilters();
-  if (db_data_) {                                                        // database source: a new batch per e2e step; the first one always
-    if (copy_input || !db_data_->loaded()) db_data_->LoadBatch(nodes_[db_data_node_].top, S());
+  if (!db_data_.empty()) {                                               // database sources: a new batch per e2e step; the first one always
+    for (auto& d : db_data_)
+      if (copy_input || !d.first->loaded()) d.first->LoadBatch(nodes_[d.second].top, S());
   } else if (copy_input && data_) data_->LoadBatch(nodes_[0].top[0], S());     // H2D of the batch (+ the device transform of uint8 datums)
   EventProfiler* prof = Caffe::profiler();
   for (size_t i = 0; i < layers_.size(); ++i) {
@@ -1146,12 +1183,13 @@ void TrainNet::ShareTrainedLayersWith(TrainNet& train) {
     if (!taken[sh.layer]) AliasShare(sh);
   // a multi-GPU trainer: rank r scores its stripe of the validation database (Net::Init's TEST DataReader gets (solver_count, rank))
   test_sync_ = train.sync_;
-  if (test_sync_ && db_data_) db_data_->set_solver(test_sync_->nranks(), test_sync_->rank());
+  if (test_sync_)
+    for (auto& d : db_data_) d.first->set_solver(test_sync_->nranks(), test_sync_->rank());
   filters_dirty_ = true;
 }
 void TrainNet::ForwardTest() {
   B2_CHECK(test_, "ForwardTest: the net was built for the TRAIN phase");
-  if (db_data_) db_data_->LoadBatch(nodes_[db_data_node_].top, S());   // every TEST forward reads the next batch
+  for (auto& d : db_data_) d.first->LoadBatch(nodes_[d.second].top, S());   // every TEST forward reads the next batch
   Forward(false);
 }
 float TrainNet::Test(int iterations, vector<float>* per_batch, vector<float>* mean) {

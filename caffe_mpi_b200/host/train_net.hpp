@@ -274,6 +274,17 @@ class EuclideanLossLayer : public LayerBase {  // loss = sum (a - b)^2 / N / 2; 
   Blob diff_;
 };
 
+class L1LossLayer : public LayerBase {         // loss = sum |a - b| / N; gradient +-loss_weight / N * sign(a - b) to each propagating bottom
+ public:
+  using LayerBase::LayerBase;
+  const char* type() const override { return "L1Loss"; }
+  void Reshape(const vector<Blob*>& b, const vector<Blob*>& t) override { diff_.ReshapeLike(*b[0]); t[0]->Reshape({1}); }
+ protected:
+  void Forward_gpu(const vector<Blob*>& b, const vector<Blob*>& t) override;
+  void Backward_gpu(const vector<Blob*>& t, const vector<bool>& pd, const vector<Blob*>& b) override;
+  Blob diff_;                                   // a - b; the backward takes its sign (the reference keeps a separate sign_ blob)
+};
+
 class SigmoidCrossEntropyLossLayer : public LayerBase {   // no sigmoid tensor: backward recomputes sigmoid(x)
  public:
   using LayerBase::LayerBase;
@@ -408,8 +419,13 @@ class TrainNet {
   const vector<shared_ptr<Blob>>& learnable_params() const { return learnable_; }
   const vector<int>& trainable_ids() const { return trainable_ids_; }               // ids the layers differentiate
   size_t activation_floats() const;
-  size_t input_bytes() const { return db_data_ ? db_data_->h2d_bytes() : data_ ? data_->h2d_bytes() : 0; }   // host -> device bytes of one e2e step's batch
-  DataLayer* database_layer() { return db_data_; }   // non-null when the net's Data layer reads its LMDB (data_layer.hpp)
+  size_t input_bytes() const {                     // host -> device bytes of one e2e step's batch
+    size_t n = data_ ? data_->h2d_bytes() : 0;
+    for (auto& d : db_data_) n += d.first->h2d_bytes();
+    return n;
+  }
+  // the first Data layer that reads its LMDB (data_layer.hpp), or null
+  DataLayer* database_layer() { return db_data_.empty() ? nullptr : db_data_[0].first; }
   // Solver::Snapshot (solver.cpp:447-520): <prefix>_iter_<N>.caffemodel (every layer's blobs, NVCaffe raw BlobProto) and
   // <prefix>_iter_<N>.solverstate (iter, learned_net, one history blob per learnable parameter, current_step).
   // Returns the .solverstate path.
@@ -501,8 +517,7 @@ class TrainNet {
   P2PSync* sync_ = nullptr;
   Blob* loss_blob_ = nullptr;
   SyntheticDataLayer* data_ = nullptr;
-  DataLayer* db_data_ = nullptr;                   // the LMDB-backed source, when data_param.source opened
-  int db_data_node_ = 0;
+  vector<std::pair<DataLayer*, int>> db_data_;     // the LMDB-backed sources (data_param.source opened) and their nodes
 };
 
 }  // namespace caffe

@@ -441,6 +441,11 @@ int b2c_sigmoid_ce_loss_backward(size_t count, const float* x, const float* targ
  * with alpha = +-loss_weight / N.  dx may be diff.                                                                             */
 int b2c_euclidean_loss_forward(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream);
 int b2c_euclidean_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream);
+/* L1LossLayer (NVCaffe's l1_loss_layer.cu:11-43): diff = a - b (kept for backward), *loss = float(sum |diff|) / N (device scalar,
+ * the same deterministic reduction as b2c_euclidean_loss_forward: the same bits on every call).  Backward, once per bottom that
+ * propagates: dx = alpha * sign(diff) with alpha = +-loss_weight / N and sign(0) = sign(NaN) = 0 (written as +0).  dx may be diff. */
+int b2c_l1_loss_forward(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream);
+int b2c_l1_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream);
 /* ContrastiveLossLayer (src/caffe/layers/contrastive_loss_layer.cpp), N pairs of C-channel features a, b [N, C] and labels y [N]
  * read as (int)y (0.7 is dissimilar, -1 similar).  Forward, one launch: diff = a - b [N, C] (kept for backward), dist_sq [N], and
  * *loss (device scalar) = sum_n (y_n ? d2_n : max(margin - sqrt(d2_n), 0)^2) / N / 2; legacy != 0 takes max(margin - d2_n, 0) as

@@ -63,8 +63,9 @@ void* b2h_data_reader_create(const char* source, int batch_size, int solver_coun
 void b2h_data_reader_destroy(void* reader);
 int b2h_data_reader_info(void* reader, int* chw, long long* entries, long long* full_cycle);   /* DataReader::sample() shape */
 long long b2h_data_reader_first_record(void* reader, long long batch);                           /* CursorManager::rewind / next */
-/* DataLayer::load_batch's view of one batch (src/caffe/layers/data_layer.cpp:232-296): uint8 datums [B][C][H][W] at
- * item_id = record_id % B, labels as floats, Datum::record_id per item */
+/* DataLayer::load_batch's view of one batch (src/caffe/layers/data_layer.cpp:232-296): uint8 datums [B][C][H][W] (floats when the
+ * database's datums carry float_data and no `data`, as DIGITS' label databases do) at item_id = record_id % B, labels as floats,
+ * Datum::record_id per item */
 int b2h_data_reader_next(void* reader, unsigned char* data, float* label, unsigned* record_id, long long* batch_id);
 
 /* ---- DataTransformer::Fill3Randoms + the crop / mirror rules of Transform (src/caffe/data_transformer.cpp:127-137,187,219-228) ------
