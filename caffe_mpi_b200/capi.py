@@ -72,6 +72,35 @@ class ConvParams(C.Structure):
         return 2 * self.N * self.O * self.Kd * self.Ho * self.Wo
 
 
+class DetectNetAug(C.Structure):
+    """b2c_detectnet_aug: one image's augmentation (the reference's AugmentSelection)."""
+    _fields_ = [("hue_rotation", C.c_float), ("saturation", C.c_float), ("flip", C.c_int), ("scale_w", C.c_int), ("scale_h", C.c_int),
+                ("rotation", C.c_float), ("crop_x", C.c_int), ("crop_y", C.c_int)]
+
+
+DETECTNET_MAX_CLASSES = 32
+DETECTNET_BAD_BOX_LENGTH, DETECTNET_TOO_MANY_BOXES = 1, 2
+GRIDBOX_TYPES = ("GRIDBOX_MAX", "GRIDBOX_MIN")
+
+
+class DetectNetGT(C.Structure):
+    """b2c_detectnet_gt: DetectNetGroundTruthParameter with RECTANGULAR coverage."""
+    _fields_ = [(n, C.c_int) for n in ("image_size_x", "image_size_y", "stride", "gridbox_type", "max_cvg_len", "min_cvg_len",
+                                      "obj_norm", "crop_bboxes")] + \
+               [("scale_cvg", C.c_float), ("n_classes", C.c_int), ("class_src", C.c_int * DETECTNET_MAX_CLASSES),
+                ("class_dst", C.c_int * DETECTNET_MAX_CLASSES)]
+
+    @classmethod
+    def make(cls, image_size_x=1248, image_size_y=384, stride=4, gridbox_type="GRIDBOX_MAX", max_cvg_len=50, min_cvg_len=50,
+             obj_norm=False, crop_bboxes=True, scale_cvg=0.5, object_class=()):
+        """caffe.proto's defaults; object_class a sequence of (src, dst) (empty: the reference's {1 -> 0})."""
+        g = cls(image_size_x, image_size_y, stride, GRIDBOX_TYPES.index(gridbox_type) if isinstance(gridbox_type, str) else gridbox_type,
+                max_cvg_len, min_cvg_len, int(bool(obj_norm)), int(bool(crop_bboxes)), scale_cvg, len(object_class))
+        for m, (src, dst) in enumerate(object_class):
+            g.class_src[m], g.class_dst[m] = src, dst
+        return g
+
+
 def declared_symbols():
     """Every function name include/b2c.h declares."""
     txt = open(HEADER).read()
@@ -180,6 +209,11 @@ def lib():
         "b2c_euclidean_loss_backward": (i, [sz, vp, f, vp, vp]),
         "b2c_l1_loss_forward": (i, [i, sz, vp, vp, vp, vp, vp]),
         "b2c_l1_loss_backward": (i, [sz, vp, f, vp, vp]),
+        "b2c_detectnet_image_workspace_bytes": (sz, [i, i, i]),
+        "b2c_detectnet_image": (i, [i, i, i, i, i, vp, vp, i, vp, C.POINTER(f), vp, sz, vp, vp]),
+        "b2c_detectnet_label_shape": (i, [C.POINTER(DetectNetGT), C.POINTER(i), C.POINTER(i), C.POINTER(i)]),
+        "b2c_detectnet_labels": (i, [i, i, i, i, vp, vp, C.POINTER(DetectNetGT), vp, vp, vp]),
+        "b2c_debug_detectnet_plan": (i, [i, i, i, i, i, i, i, C.POINTER(DetectNetGT), C.POINTER(i), i]),
         "b2c_contrastive_loss_forward": (i, [i, i, vp, vp, vp, f, i, vp, vp, vp, vp]),
         "b2c_contrastive_loss_backward": (i, [i, i, vp, vp, vp, f, i, f, vp, vp, vp]),
         "b2c_bias_forward": (i, [i, i, i, vp, vp, vp]),
@@ -546,6 +580,69 @@ def neuron_backward(kind, x, y, dy, dx, p=(0.0, 0.0, 0.0), stream=None):
     """b2c_neuron_backward; x / y may be None where the kind's rule does not read them."""
     p = tuple(p) + (0.0,) * (3 - len(p))
     check(lib().b2c_neuron_backward(NEURON_KINDS.index(kind), dy.numel(), _p(x), _p(y), _p(dy), _p(dx), *p, _stream(stream)))
+
+
+def detectnet_augs(augs):
+    """A CUDA uint8 tensor holding b2c_detectnet_aug[N] for `augs`: DetectNetAug structs or dicts of their fields."""
+    import torch
+    arr = (DetectNetAug * len(augs))(*[a if isinstance(a, DetectNetAug) else DetectNetAug(**a) for a in augs])
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).cuda()
+
+
+def detectnet_image_workspace_bytes(N, H, W):
+    return int(lib().b2c_detectnet_image_workspace_bytes(N, H, W))
+
+
+def detectnet_image(bottom, augs, top, mean_value=None, mean_image=None, workspace=None, stream=None):
+    """b2c_detectnet_image: bottom [N, 3, H, W] -> top [N, 3, OH, OW] (torch CUDA float32); augs a tensor from detectnet_augs;
+    mean_value 1 or 3 floats, or mean_image [3, H, W]; workspace allocated when None."""
+    import torch
+    N, _, H, W = bottom.shape
+    OH, OW = top.shape[2], top.shape[3]
+    ws_bytes = detectnet_image_workspace_bytes(N, H, W)
+    if workspace is None:
+        workspace = torch.empty(ws_bytes // 4, dtype=torch.float32, device=bottom.device)
+    kind, mv = 0, None
+    if mean_image is not None:
+        kind = 2
+    elif mean_value is not None:
+        vals = list(mean_value) * 3 if len(mean_value) == 1 else list(mean_value)
+        kind, mv = 1, (C.c_float * 3)(*vals)
+    check(lib().b2c_detectnet_image(N, H, W, OH, OW, _p(bottom), _p(augs), kind, _p(mean_image), mv, _p(workspace),
+                                    workspace.numel() * 4, _p(top), _stream(stream)))
+
+
+def detectnet_label_shape(gt):
+    """(channels, GH, GW) of the label top for a DetectNetGT."""
+    c, h, w = C.c_int(), C.c_int(), C.c_int()
+    check(lib().b2c_detectnet_label_shape(C.byref(gt), C.byref(c), C.byref(h), C.byref(w)))
+    return c.value, h.value, w.value
+
+
+def detectnet_labels(labels, H, W, augs, gt, top, status, stream=None):
+    """b2c_detectnet_labels: labels [N, 1, rows, 16] of H x W images -> top [N, C, GH, GW]; status a CUDA int32 tensor of one
+    element the kernel ORs its header errors into (see detectnet_check_status)."""
+    N, _, rows, _ = labels.shape
+    check(lib().b2c_detectnet_labels(N, rows, H, W, _p(labels), _p(augs), C.byref(gt), _p(top), _p(status), _stream(stream)))
+
+
+def detectnet_check_status(status):
+    """Raise the reference's CHECK message for the error bits a label call left in `status` (an int)."""
+    if status & DETECTNET_BAD_BOX_LENGTH:
+        raise B2CError("DetectNetTransformation label: Check failed: bboxLen == 16 (a label header's box length is not 16)")
+    if status & DETECTNET_TOO_MANY_BOXES:
+        raise B2CError("DetectNetTransformation label: Check failed: numOfBbox <= height (a label header lists more boxes "
+                       "than the blob has rows)")
+
+
+def detectnet_plan(op, N, H, W, OH=0, OW=0, rows=0, gt=None):
+    """b2c_debug_detectnet_plan: op "image" or "labels"."""
+    out = (C.c_int * 6)()
+    check(lib().b2c_debug_detectnet_plan(("image", "labels").index(op), N, H, W, OH, OW, rows, C.byref(gt) if gt is not None else None,
+                                         out, 6))
+    if op == "image":
+        return dict(launches=out[0], colour_ctas=out[1], sample_ctas=out[2], threads=out[3], workspace=(out[4] << 20) + out[5])
+    return dict(ctas=out[0], threads=out[1], smem=out[2], channels=out[3], grid_h=out[4], grid_w=out[5])
 
 
 def prelu_forward(N, Cc, dim, shared, x, slope, y, x_keep=None, stream=None):

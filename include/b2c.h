@@ -446,6 +446,59 @@ int b2c_euclidean_loss_backward(size_t count, const float* diff, float alpha, fl
  * propagates: dx = alpha * sign(diff) with alpha = +-loss_weight / N and sign(0) = sign(NaN) = 0 (written as +0).  dx may be diff. */
 int b2c_l1_loss_forward(int N, size_t count, const float* a, const float* b, float* diff, float* loss, void* stream);
 int b2c_l1_loss_backward(size_t count, const float* diff, float alpha, float* dx, void* stream);
+/* ---- DetectNetTransformationLayer (NVCaffe's src/caffe/layers/detectnet_transform_layer.{cpp,cu} and
+ * src/caffe/util/detectnet_coverage_rectangular.cpp); GPU parity: tests/test_detectnet_transform_gpu.py.
+ * One image's augmentation, the reference's AugmentSelection (include/caffe/layers/detectnet_transform_layer.hpp:29-45):
+ * hue_rotation in degrees (applied when |h| > FLT_EPSILON), saturation factor (applied when < 1 - 1/255), flip, the scaled size
+ * (scale_w x scale_h; scaling applies where it differs from the bottom's W x H), rotation in degrees (applied when
+ * |r| > FLT_EPSILON) and the crop offset.  The entry points read an array of N of them in DEVICE memory and draw nothing. */
+typedef struct {
+  float hue_rotation, saturation;
+  int flip, scale_w, scale_h;
+  float rotation;
+  int crop_x, crop_y;
+} b2c_detectnet_aug;
+/* DetectNetGroundTruthParameter (caffe.proto), RECTANGULAR coverage.  gridbox_type 0 GRIDBOX_MAX, 1 GRIDBOX_MIN.  class_src[m] ->
+ * class_dst[m] for m < n_classes is the object_class map (a later entry with the same src wins); n_classes 0 is the reference's
+ * default {1 -> 0}. */
+#define B2C_DETECTNET_MAX_CLASSES 32
+typedef struct {
+  int image_size_x, image_size_y, stride, gridbox_type, max_cvg_len, min_cvg_len, obj_norm, crop_bboxes;
+  float scale_cvg;
+  int n_classes;
+  int class_src[B2C_DETECTNET_MAX_CLASSES], class_dst[B2C_DETECTNET_MAX_CLASSES];
+} b2c_detectnet_gt;
+/* Image path (detectnet_transform_layer.cu:121-346, replacing its three kernels and their cudaStreamSynchronize): bottom
+ * [N, 3, H, W] of 0-255 values -> top [N, 3, OH, OW].  Per pixel: RGB -> HSV -> RGB with the hue rotation and desaturation, then
+ * the mean (mean_kind 0 none, 1 mean_value[3]: the transform_param values as written, host floats, of which the kernel subtracts
+ * float(float(m / 255) * 255) as the reference's GPU path does; 2 mean_image [3, H, W] device, subtracted as given), into `workspace`
+ * (b2c_detectnet_image_workspace_bytes); then per output pixel: crop offset, rotation, scale and flip in the reference's order and
+ * its bicubic (1-pixel replicated border, 0 beyond).  Float coordinates and HSV, the cubic in double, no FMA contraction: without
+ * rotation the result is bit-exact against a float32 / double restatement.  One departure: hue is wrapped into [-60, 360) by whole
+ * turns, for any hue_rotation, before the HSV sector is chosen (the reference never wraps it; DESIGN §4).  Two launches.  Refuses (B2C_ERR_INVALID) non-positive
+ * sizes, null pointers and a small workspace. */
+size_t b2c_detectnet_image_workspace_bytes(int N, int H, int W);
+int b2c_detectnet_image(int N, int H, int W, int OH, int OW, const float* bottom, const b2c_detectnet_aug* aug, int mean_kind,
+                        const float* mean_image, const float* mean_value, float* workspace, size_t workspace_bytes, float* top,
+                        void* stream);
+/* Label path (transform_label_cpu, detectnet_transform_layer.cpp:450-615, and CoverageGenerator::generate,
+ * detectnet_coverage_rectangular.cpp:292-360, which the reference runs on the host): labels [N, 1, rows, 16], the DIGITS layout
+ * (row 0 [num_boxes, 16, ...], then one BboxLabel_ per row), of images H x W -> top [N, C, GH, GW] (b2c_detectnet_label_shape):
+ * foreground, the box corners relative to the cell, 1 / width, 1 / height, obj_norm, then one coverage channel per class.  One CTA
+ * per image, the boxes in shared memory; each cell takes the last box in list order that covers it, which is what the reference's
+ * in-order overwrite leaves (no atomics, the same bits on every call).  A malformed header is never read as boxes: the image's
+ * labels are zeroed and *status (device int, zeroed by the caller; sticky) gains B2C_DETECTNET_BAD_BOX_LENGTH (the reference's
+ * CHECK bboxLen == 16) or B2C_DETECTNET_TOO_MANY_BOXES (CHECK numOfBbox <= height; boxes are the rows after the header, so
+ * num_boxes == rows is refused too).  rows - 1 <= 768.  Refuses (B2C_ERR_INVALID) bad shapes and parameters. */
+#define B2C_DETECTNET_BAD_BOX_LENGTH 1
+#define B2C_DETECTNET_TOO_MANY_BOXES 2
+int b2c_detectnet_label_shape(const b2c_detectnet_gt* gt, int* channels, int* grid_h, int* grid_w);
+int b2c_detectnet_labels(int N, int rows, int H, int W, const float* labels, const b2c_detectnet_aug* aug, const b2c_detectnet_gt* gt,
+                         float* top, int* status, void* stream);
+/* The launches of a DetectNet call.  op 0 (image; gt and rows unused): out[0] launches (2), [1] colour CTAs, [2] sampling CTAs,
+ * [3] threads per CTA, [4] workspace MiB, [5] workspace bytes beyond them.  op 1 (labels; OH, OW unused): [0] CTAs (N), [1] threads,
+ * [2] shared-memory bytes, [3] channels, [4] GH, [5] GW.  Needs n >= 6.  Pure host computation. */
+int b2c_debug_detectnet_plan(int op, int N, int H, int W, int OH, int OW, int rows, const b2c_detectnet_gt* gt, int* out, int n);
 /* ContrastiveLossLayer (src/caffe/layers/contrastive_loss_layer.cpp), N pairs of C-channel features a, b [N, C] and labels y [N]
  * read as (int)y (0.7 is dissimilar, -1 similar).  Forward, one launch: diff = a - b [N, C] (kept for backward), dist_sq [N], and
  * *loss (device scalar) = sum_n (y_n ? d2_n : max(margin - sqrt(d2_n), 0)^2) / N / 2; legacy != 0 takes max(margin - d2_n, 0) as
